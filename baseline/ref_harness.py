@@ -1,7 +1,7 @@
 """Run the UNMODIFIED reference (AaronZ345/StyleSinger) on the synthetic workload of bench.py.
 
 Reference arms only: `bench.py --impl reference`, `tools/baseline_arms.py` (CPU figures of BASELINE.md §3 and the
-GPU-PyTorch denominator of the >= 10x target) and `tests/test_gpu_reference_dropin.py`.  Nothing here is on the product
+GPU-PyTorch denominator of the >= 10x target).  Nothing here is on the product
 path, and nothing of this repo's engine is on the path timed here: the objects built below are the reference's own
 `inference.StyleSinger.StyleSingerInfer` (its `StyleSinger` model + its registered `HifiGAN_NSF` vocoder), constructed
 by the reference's own constructor from checkpoint directories written in the reference's on-disk format.

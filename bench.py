@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — StyleSinger ph -> mel -> wav hot path on B200 (driver contract; see the task statement).
+"""bench.py — StyleSinger ph -> mel -> wav hot path on one or more H100s.
 
     python bench.py --gpus 1 --steps K --warmup W [--workload utt10s|batch64] [--T 100]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
-    python bench.py --impl reference ...      # CPU arm: the UNMODIFIED reference (staged under baseline/_ref by
-                                              # build(); the oracle port only if that copy is absent), host cores
+    python bench.py --impl reference ...      # CPU arm: the UNMODIFIED reference (tools/ref_import.py finds it;
+                                              # the oracle port when there is none), host cores
     python bench.py --workload sweep          # BASELINE.json configs[4]: T sweep, persistent vs per-launch mel sampler
+    python bench.py ... --dump-outputs DIR    # also write what the last timed step computed as DIR/<name>.npy
 
 A "step" is one pass of the whole hot path (encoder, style adaptor + RVQ, two F0/UV diffusions, FFT
 decoder, T-step mel diffusion, HiFi-GAN-NSF) over one batch of seeded synthetic utterances
@@ -48,7 +49,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1400.0, "src": "fallback"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "src": "H100 SXM data sheet (dense, 700 W)"}
 
 
 class ClockSampler:
@@ -220,7 +221,7 @@ def run_b200(args, rank, world, local_rank):
     pb_host = pack_batch(utts, use_mel2ph=True, pin=True)
     pb_dev = pb_host.to(dev)
     frames = pb_host.total_frames
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -251,7 +252,14 @@ def run_b200(args, rank, world, local_rank):
     clocks = ClockSampler(local_rank)
     clocks.start()
     l0 = lib.ssb_launch_count()
-    ms = timed(lambda s: eng.run_device(pb_dev, seed=100 + s), args.steps)
+    last = {}
+
+    def value_step(s):
+        last["out"] = eng.run_device(pb_dev, seed=100 + s)
+
+    ms = timed(value_step, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])
     launches = int(lib.ssb_launch_count() - l0)
     clk = clocks.stop()
 
@@ -308,27 +316,20 @@ def run_b200(args, rank, world, local_rank):
     ms_mel = timed(lambda s: eng.model.mel_diffusion(cond, coarse, pb_dev.frame_offsets, seed=3 + s), max(1, min(args.steps, 3)))
     n_mel = int(lib.ssb_launch_count() - l1) // max(1, min(args.steps, 3))
     pk = peaks()
-    traffic = None  # dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed
-    tpath = os.path.join(REPO, "profiles", "traffic.json")  # ncu --set full capture of this workload (profiles/*.md)
-    if os.path.exists(tpath) and args.workload == "batch64" and T == 100:
-        try:
-            traffic = json.load(open(tpath))
-        except Exception:
-            traffic = None
+    traffic = None  # no DRAM-traffic capture of the dominant kernel is stored for this GPU
     flops = frames * T * MEL_STEP_FLOPS  # algorithmic (reference) FLOPs; executed: see executed_tflops below
     achieved = flops / (ms_mel / 1000.0) / 1e12
     executed = frames * (T * MEL_STEP_FLOPS_EXECUTED + MEL_HOIST_FLOPS) / (ms_mel / 1000.0) / 1e12
     gemm_launches = T * (2 * hp["residual_layers"] + 3) + 1
     roof = {"bound": "tensor", "achieved": achieved, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
             "frac": achieved / pk["bf16_tflops"], "traffic": (traffic or {}).get("bytes_per_launch"),
-            "traffic_detail": traffic, "peak_source": pk["src"] + " (cuBLAS bf16, sustained)",
-            "kernel": "conv_gemm_tc2r_kernel<128, GATE> (tcgen05 cta_group::2, tap reuse; 90.6 %% tensor pipe active under ncu) + "
-                      "conv_gemm_tc2_kernel<128, RES_SKIP>; mel denoiser stage: %d launches per sampler call, of which %d residual-layer GEMMs"
-                      % (n_mel, 2 * T * hp["residual_layers"]),
+            "traffic_detail": traffic, "peak_source": pk["src"],
+            "kernel": "conv_gemm_wg_kernel (wgmma + TMA, CTA pairs with multicast weight tiles on large batches); mel denoiser "
+                      "stage: %d launches per sampler call, of which %d residual-layer GEMMs" % (n_mel, 2 * T * hp["residual_layers"]),
             "avg_launch_us": 1000.0 * ms_mel / max(n_mel, 1), "stage_ms": ms_mel,
             "note": "useful FLOPs (26.43 MFLOP per frame-step, SURVEY 8d) over the CUDA-event time of the mel-diffusion stage; "
                     "the step-invariant conditioner projection is hoisted out of the T loop (executed_tflops counts what the tensor "
-                    "cores really do: 21.18 MFLOP per frame-step + 5.24 MFLOP per frame once); the GEMMs run as 3 tcgen05 fp16 MMAs "
+                    "cores really do: 21.18 MFLOP per frame-step + 5.24 MFLOP per frame once); the GEMMs run as 3 wgmma fp16 MMAs "
                     "per product (hi/lo split) for fp32-class accuracy, so the issued-MMA rate is 3x executed_tflops and the "
                     "effective ceiling of this precision scheme is peak/3",
             "executed_tflops": executed, "issued_mma_tflops": 3.0 * executed,
@@ -399,13 +400,13 @@ def run_b200(args, rank, world, local_rank):
             if "value" in gpu_ref and lat is not None:
                 line["target_10x"] = {"utt10s_b200_e2e_over_reference_gpu": lat["frames_per_s"] / gpu_ref["value"],
                                       "batch_b200_e2e_over_reference_gpu_b1": line["e2e"]["value"] / gpu_ref["value"],
-                                      "note": "reference = its own B=1 inference path on the same GPU; see profiles/ for the "
-                                              "padded-batch and allow_tf32=False variants (tools/baseline_arms.py)"}
+                                      "note": "reference = its own B=1 inference path on the same GPU; tools/baseline_arms.py "
+                                              "times the padded-batch and allow_tf32=False variants"}
         print(json.dumps(line), flush=True)
 
 
 def run_sweep(args, rank, world, local_rank):
-    """BASELINE.json configs[4]: T in {25, 50, 100, 200, 500} at batch 64 on one B200, mel sampler only (the F0 loops stay at
+    """BASELINE.json configs[4]: T in {25, 50, 100, 200, 500} at batch 64 on one GPU, mel sampler only (the F0 loops stay at
     100 steps and are not part of the timed stage): one launch per GEMM vs the persistent single-launch kernel run over
     groups of <= 48 row tiles (ssb_model_set_persistent_groups)."""
     from stylesinger_b200 import synth
@@ -466,6 +467,31 @@ def run_sweep(args, rank, world, local_rank):
     print(json.dumps(line), flush=True)
 
 
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, outs):
+    """Write what the timed path returned in its last step (StyleSingerInfer.run_device: mel [frames, 80], f0 [frames],
+    waveform [samples], and frame_offsets [B + 1], the waveform's per-utterance offsets counted in mel FRAMES, not
+    samples: utterance b's samples are wav[frame_offsets[b] * hop : frame_offsets[b + 1] * hop]) as <name>.npy: float arrays as float32, integer ones as
+    float64.  Together they stay under 64 MB: an array too large for its share is replaced by a fixed, seeded sample of
+    its elements (flattened order), and the sampled flat indices go beside it as <name>_index.npy.  Under
+    torch.distributed only rank 0 writes, so a multi-GPU dump holds rank 0's shard of the batch, not the whole batch."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for name, a in zip(["mel", "f0", "wav", "frame_offsets"], outs):
+        a = a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+        arrays[name] = a.astype(np.float64 if np.issubdtype(a.dtype, np.integer) else np.float32)
+    share = DUMP_MAX_BYTES // len(arrays)
+    for name, a in arrays.items():
+        if a.nbytes > share:
+            n = share // 16  # float32 values + float64 indices
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -480,6 +506,9 @@ def main():
     ap.add_argument("--sweep-T", default="25,50,100,200,500")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-latency", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed as DIR/<name>.npy (float32 / float64, <= 64 MB in all; "
+                         "with several GPUs: rank 0's shard only)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,4 +1,4 @@
-/* stylesinger_b200 — C ABI of the B200-native StyleSinger hot path (libstylesinger_b200.so).
+/* stylesinger_b200 — C ABI of the H100-native StyleSinger hot path (libstylesinger_b200.so).
  *
  * The reference (AaronZ345/StyleSinger) is pure Python/PyTorch and has NO FFI of its own
  * (SURVEY.md §8b); its extension points are Python classes and registries.  This header is the
@@ -214,7 +214,7 @@ int ssb_hifigan_generate(const ssb_vocoder_t* v, const float* mel, const float* 
                          int32_t B, const float* rand_ini, const float* src_noise, uint64_t seed, float* wav_out,
                          void* workspace, size_t workspace_bytes, void* stream);
 
-/* Select the GEMM path of the denoiser layers: 1 = tcgen05 tensor cores on fp16 hi/lo split operands
+/* Select the GEMM path of the denoiser layers: 1 = wgmma tensor cores on fp16 hi/lo split operands
  * (3 MMAs per product, fp32 accumulate; default when available), 0 = fp32 FFMA.  Returns the mode in effect. */
 int ssb_model_set_tensor_cores(ssb_model_t* m, int32_t enable);
 
@@ -229,16 +229,16 @@ int ssb_model_set_persistent(ssb_model_t* m, int32_t enable);
  * (shallow_diffusion_tts.py:303-304) as ONE persistent launch (production RNG mode only; each group draws from its own
  * Philox stream).  This is the "persistent-kernel" arm of BASELINE.json configs[4] at batch 64. */
 int ssb_model_set_persistent_groups(ssb_model_t* m, int32_t enable);
-/* 1 (default): the per-launch tcgen05 samplers compute the step-invariant conditioner_projection of all residual layers
+/* 1 (default): the per-launch tensor-core samplers compute the step-invariant conditioner_projection of all residual layers
  * (modules/diff/net.py:59,71 - Conv1d(256, 2C, 1) applied to the same cond in every one of the T steps) ONCE per sampler call
  * and add it in the gate epilogue; 0: contract it inside every layer GEMM of every step (round-1 behaviour). */
 int ssb_model_set_cond_hoist(ssb_model_t* m, int32_t enable);
 /* Decoder FFT blocks (modules/commons/transformer.py TransformerFFNLayer, conv k=9 -> gelu -> linear): run the FFN GEMMs
- * on the tcgen05 kernel for batches of >= 1024 frames (default on; 0 keeps them on the fp32 FFMA kernel). Returns the
+ * on the tensor-core kernel for batches of >= 1024 frames (default on; 0 keeps them on the fp32 FFMA kernel). Returns the
  * new setting. */
 int ssb_model_set_fft_tensor_cores(ssb_model_t* m, int32_t enable);
 
-/* Unit-test granularity: ssb_op_conv1d through the tcgen05 path (Cin % 64 == 0, N % 128 == 0, no activation). */
+/* Unit-test granularity: ssb_op_conv1d through the tensor-core path (Cin % 64 == 0, N % 128 == 0, no activation). */
 int ssb_op_conv1d_tc(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
                      const float* b_host, int32_t N, int32_t k, int32_t dilation, float* out, void* stream);
 
@@ -304,15 +304,7 @@ int64_t ssb_variant_launch_count(const char* variant);
 int32_t ssb_variant_names(char* buf, int32_t cap);
 void ssb_tensor_map_cache_stats(int64_t* encodes, int64_t* hits);
 
-/* Process-wide switch (default 0) of the interleaved residual-layer schedule of the large-batch samplers: the gate conv of
- * one group of utterances (or of one F0 net) and the 1x1 residual/skip conv of the other group share one launch and
- * alternate tile by tile inside every SM (kernel variant "tc2d<HB,GATE+RES_SKIP>"; reference loop net.py:66-78 inside
- * shallow_diffusion_tts.py:303-304 / gaussian_multinomial_diffusion.py:928-939).  Results agree with one launch per GEMM to
- * fp32 rounding (tests/test_gpu_scale.py); measured 3 % slower than it on B200, hence opt-in (DESIGN.md section 6).
- * Returns the new state. */
-int32_t ssb_set_interleaved_layers(int32_t enable);
-
-/* Process-wide switch of the tcgen05 / TMA attention kernel (csrc/attention_tc.cu) for the long-batch paths of the FFT blocks
+/* Process-wide switch of the wgmma / TMA attention kernel (csrc/attention_tc.cu) for the long-batch paths of the FFT blocks
  * (common_layers.py:277-286) and of the style aligner's cross-attention (lse.py:41); short batches always use the fp32
  * kernel.  Returns the new state. */
 int32_t ssb_set_attention_tensor_cores(int32_t enable);
@@ -324,7 +316,7 @@ int ssb_op_conv1d(const float* x, const int32_t* offsets, int32_t B, int32_t Cin
 /* Unit-test granularity: multi-head attention, 2 heads x 128; q [sumL,256], k/v [sumS,256]. */
 int ssb_op_attention(const float* q, const float* k, const float* v, const int32_t* q_offsets,
                      const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream);
-/* Same contract on the tcgen05 / TMA attention kernel (csrc/attention_tc.cu; 3-pass fp16 hi/lo split MMAs for QK^T and PV,
+/* Same contract on the wgmma / TMA attention kernel (csrc/attention_tc.cu; 3-pass fp16 hi/lo split MMAs for QK^T and PV,
  * TMA-staged K / V^T tiles), the path long batches take inside the FFT blocks (common_layers.py:277-286) and the style
  * aligner (lse.py:41). */
 int ssb_op_attention_tc(const float* q, const float* k, const float* v, const int32_t* q_offsets,

@@ -1,4 +1,4 @@
-"""stylesinger_b200 — B200-native (sm_100a) engine for StyleSinger's ph -> mel -> wav hot path.
+"""stylesinger_b200 — H100-native (sm_90a) engine for StyleSinger's ph -> mel -> wav hot path.
 
 Host side (this package): tensor plumbing, checkpoint packing, the drop-in mirrors of the
 reference's Python interfaces.  All arithmetic of the hot path runs in hand-written CUDA kernels

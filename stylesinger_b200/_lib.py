@@ -59,7 +59,7 @@ EXPORTS = [
     "ssb_vocoder_set_tensor_cores", "ssb_variant_launch_count", "ssb_variant_names", "ssb_tensor_map_cache_stats",
     "ssb_model_set_persistent_groups", "ssb_model_set_cond_hoist", "ssb_mel_diffusion_plms_workspace_bytes",
     "ssb_mel_diffusion_sample_plms", "ssb_fft_workspace_bytes", "ssb_fft_encoder", "ssb_fft_decoder",
-    "ssb_get_style_workspace_bytes", "ssb_get_style", "ssb_set_interleaved_layers", "ssb_op_attention_tc", "ssb_set_attention_tensor_cores",
+    "ssb_get_style_workspace_bytes", "ssb_get_style", "ssb_op_attention_tc", "ssb_set_attention_tensor_cores",
     "ssb_melspec_create", "ssb_melspec_free", "ssb_melspec_num_frames", "ssb_melspec_workspace_bytes", "ssb_melspec_forward",
     "ssb_melspec_create_ex", "ssb_lstm_encoder_create", "ssb_lstm_encoder_free", "ssb_lstm_encoder_workspace_bytes", "ssb_lstm_encoder_forward",
 ]
@@ -68,7 +68,7 @@ EXPORTS = [
 def _load():
     if not os.path.exists(LIB_PATH):
         raise SsbError(f"{LIB_PATH} not found: build it with `python -m stylesinger_b200.build` "
-                       f"(nvcc, sm_100a). There is no CPU / PyTorch fallback.")
+                       f"(nvcc, sm_90a). There is no CPU / PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     vp, i32, u64, sz = C.c_void_p, C.c_int32, C.c_uint64, C.c_size_t
     P = C.POINTER
@@ -113,7 +113,6 @@ def _load():
         "ssb_variant_launch_count": (C.c_int64, [C.c_char_p]),
         "ssb_variant_names": (i32, [C.c_char_p, i32]),
         "ssb_tensor_map_cache_stats": (None, [P(C.c_int64), P(C.c_int64)]),
-        "ssb_set_interleaved_layers": (i32, [i32]),
         "ssb_set_attention_tensor_cores": (i32, [i32]),
         "ssb_melspec_create": (C.c_int, [P(vp), i32, i32, i32, i32, i32, C.c_float, C.c_float, C.c_float]),
         "ssb_melspec_create_ex": (C.c_int, [P(vp), i32, i32, i32, i32, i32, C.c_float, C.c_float, C.c_float, i32, i32, i32]),
@@ -136,7 +135,7 @@ lib = _load()
 
 
 def variant_launches():
-    """{kernel variant name: launches so far} of the tcgen05 GEMM dispatcher (ssb_variant_names / _launch_count)."""
+    """{kernel variant name: launches so far} of the tensor-core GEMM dispatcher (ssb_variant_names / _launch_count)."""
     buf = C.create_string_buffer(4096)
     lib.ssb_variant_names(buf, 4096)
     names = [n for n in buf.value.decode().split(";") if n]

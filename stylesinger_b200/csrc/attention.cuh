@@ -19,7 +19,7 @@ struct AttnArgs {
 
 int attention(Ctx& ctx, const AttnArgs& a);
 
-// tcgen05 / TMA attention for long batches (attention_tc.cu).  Operands are fp16 hi/lo planes:
+// wgmma / TMA attention for long batches (attention_tc.cu).  Operands are fp16 hi/lo planes:
 //   Q  [rows_q, ldq], head h at columns qcol0 + 128 h;   K [rows_k, ldk], head h at columns kcol0 + 128 h;
 //   V^T [heads * 128, ldvt]: row = head * 128 + d, column = key row of the K/V layout (transpose_planes below).
 // Output: fp32 [rows_q, ldo] and / or fp16 hi/lo planes [rows_q, ldh] (head h at columns 128 h).

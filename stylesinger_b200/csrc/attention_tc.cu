@@ -1,17 +1,17 @@
-// Multi-head attention (2 heads x 128) on tcgen05 tensor cores with TMA-staged tiles.  sm_100a only.
+// Multi-head attention (2 heads x 128) on Hopper tensor cores (wgmma) with TMA-staged tiles.  sm_90a only.
 // Rows a3 / a12 of SURVEY.md section 8: self-attention of the FFT blocks (reference modules/commons/common_layers.py:277-286
 // -> F.multi_head_attention_forward: q * hd^-0.5, bmm, key-padding -> -inf, fp32 softmax, bmm) and the style aligner's
 // cross-attention (modules/StyleSinger/lse.py:41).  Used for long batches; short ones keep the fp32 kernel (attention.cu).
 //
 // One CTA = 128 queries of one (utterance, head); keys / values stream through a 4-slot shared-memory ring in tiles of 64.
-// Both contractions are 3-pass fp16 hi/lo split MMAs like every other tcgen05 GEMM of this library (fp32-class accuracy):
-//   S   = Q K^T      M128 x N64  x K128 (head dim),  A = Q planes, B = K planes              -> TMEM, double buffered
-//   O  += P V        M128 x N128 x K64  (keys),      A = P (written by the softmax warps),  B = V^T planes -> TMEM
+// Both contractions are 3-pass fp16 hi/lo split MMAs like every other tensor-core GEMM of this library (fp32-class accuracy):
+//   S   = Q K^T      M128 x N64  x K128 (head dim),  A = Q planes, B = K planes             -> registers
+//   O  += P V        M128 x N128 x K64  (keys),      A = P planes from registers,           B = V^T planes -> registers
 // No running rescale of O: pass 1 streams S once for the exact row maximum m, pass 2 recomputes S, forms
 // p = exp(scale * (s - m)) (masked keys -> 0), accumulates l = sum p in registers and O += P V on the tensor cores; the
 // epilogue divides by l.  P is carried as fp16 hi/lo planes of 256 * p so that weights down to 2^-33 survive the split.
 // The [L, S] score matrix is never materialised (63 MB / utterance / layer in the reference at F = 2812).
-//   warp 0: TMA producer   warp 1: MMA issuer   warp 2: TMEM allocator   warps 4-7: softmax / epilogue (thread = query row)
+//   warp 0: TMA producer   warps 4-11: two consumer warpgroups of 64 query rows each (MMAs, softmax, epilogue)
 #include <stdlib.h>
 
 #include <atomic>
@@ -33,11 +33,9 @@ constexpr int Q_BYTES = 4 * QT;            // hi_h0, hi_h1, lo_h0, lo_h1
 constexpr int KT = AK * 64 * 2;            // one [64 keys x 64 d] fp16 tile: 8 KB
 constexpr int SLOT = 4 * KT;               // K: hi_h0, hi_h1, lo_h0, lo_h1 ; V^T: hi [128 d x 64 keys], lo
 constexpr int NSLOT = 4;
-constexpr int PT = AQ * AK * 2;            // one P plane: 16 KB
-constexpr int ATT_SMEM = Q_BYTES + NSLOT * SLOT + 2 * PT + 1024 + 256;
-constexpr uint32_t ATT_TMEM = 256;         // S: 2 x 64 columns, O: 128 columns
-
-__device__ __forceinline__ void proxy_fence_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+constexpr int ATT_THREADS = 384;
+constexpr int ATT_SMEM = Q_BYTES + NSLOT * SLOT + 1024 + 256;
+static_assert(ATT_SMEM <= 227 * 1024, "exceeds the 227 KB of shared memory a Hopper block can have");
 
 struct AttnTCParams {
   const int4* utt_q;
@@ -49,47 +47,35 @@ struct AttnTCParams {
   __half* oh; __half* ol; int ldh;
 };
 
-__global__ void __launch_bounds__(256, 1)
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_constant__ CUtensorMap tmQ_lo,
                     const __grid_constant__ CUtensorMap tmK_hi, const __grid_constant__ CUtensorMap tmK_lo,
                     const __grid_constant__ CUtensorMap tmV_hi, const __grid_constant__ CUtensorMap tmV_lo, const AttnTCParams p) {
   const int b = blockIdx.z, head = blockIdx.y;
   const int4 uq = p.utt_q[b], uk = p.utt_k[b];
   const int q0 = blockIdx.x * AQ;
-  if (q0 >= uq.y) return;  // whole CTA, before any barrier / TMEM state exists
+  if (q0 >= uq.y) return;  // whole CTA, before any barrier state exists
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Q_BYTES + NSLOT * SLOT + 2 * PT);
-  // bars: qfull, kvfull[4], kvempty[4], sfull[2], sempty[2], pready, pfree, ofull ; then the TMEM base address
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-  const uint32_t qbase = smem_u32(smem), ring = qbase + Q_BYTES, pbase = ring + NSLOT * SLOT;
-  const uint32_t qfull = smem_u32(bars), kvfull0 = qfull + 8, kvempty0 = kvfull0 + 8 * NSLOT, sfull0 = kvempty0 + 8 * NSLOT;
-  const uint32_t sempty0 = sfull0 + 16, pready = sempty0 + 16, pfree = pready + 8, ofull = pfree + 8;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Q_BYTES + NSLOT * SLOT);  // qfull, kvfull[4], kvempty[4]
+  const uint32_t qbase = smem_u32(smem), ring = qbase + Q_BYTES;
+  const uint32_t qfull = smem_u32(bars), kvfull0 = qfull + 8, kvempty0 = kvfull0 + 8 * NSLOT;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     mbar_init(qfull, 1);
     for (int s = 0; s < NSLOT; ++s) {
       mbar_init(kvfull0 + 8 * s, 1);
-      mbar_init(kvempty0 + 8 * s, 1);
+      mbar_init(kvempty0 + 8 * s, 8);  // one arrival per consumer warp
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(sfull0 + 8 * a, 1);
-      mbar_init(sempty0 + 8 * a, 4);
-    }
-    mbar_init(pready, 4);
-    mbar_init(pfree, 1);
-    mbar_init(ofull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(ATT_TMEM) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
 
   // Key tiles sit on a grid aligned to 8 rows of the K/V layout: the V^T planes are read with the key index as the INNER
   // TMA coordinate, whose byte offset must be a multiple of 16.  The (up to 7) rows in front of the utterance are masked.
@@ -128,182 +114,159 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_con
         if (++slot == NSLOT) { slot = 0; ph ^= 1; }
       };
       for (int j = 0; j < n; ++j) load_k(j);  // pass 1: row maxima
-      load_k(0);                              // pass 2, in the order the MMA warp consumes: K0, K1, V0, K2, V1, ...
-      for (int j = 0; j < n; ++j) {
-        if (j + 1 < n) load_k(j + 1);
+      for (int j = 0; j < n; ++j) {           // pass 2, in the order the consumers use them: K0, V0, K1, V1, ...
+        load_k(j);
         load_v(j);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = (1u << 4) | ((uint32_t)(AK >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-      const uint32_t idesc_o = (1u << 4) | ((uint32_t)(HD >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-      int slot = 0, g = 0;
-      uint32_t ph = 0;
-      mbar_wait(qfull, 0);
-      tc_fence_after();
-      auto issue_s = [&]() {
-        const int a = g & 1;
-        mbar_wait(sempty0 + 8 * a, ((g >> 1) & 1) ^ 1);
-        mbar_wait(kvfull0 + 8 * slot, ph);
-        tc_fence_after();
-        const uint32_t sa = ring + slot * SLOT;
-        const uint32_t d = tmem_base + (uint32_t)(a * AK);
+  } else if (warp >= 4) {
+    // consumer warpgroup cw: query rows [64 cw, 64 cw + 64) of the tile; this thread holds rows rw and rw + 8 of them
+    const int cw = (warp - 4) >> 2, wq = warp & 3;
+    const int rw = 16 * wq + (lane >> 2);
+    const uint32_t qoff = (uint32_t)cw * 8192u;
+    int slot = 0;
+    uint32_t ph = 0;
+    auto release = [&]() {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(kvempty0 + 8 * slot);
+      if (++slot == NSLOT) { slot = 0; ph ^= 1; }
+    };
+    // S = Q K^T for the key tile in the current slot (3-pass split), then the slot goes back to the producer
+    float s[32];
+    auto scores = [&]() {
+      mbar_wait(kvfull0 + 8 * slot, ph);
+      const uint32_t sa = ring + slot * SLOT;
+      wg_fence();
+      fence_acc(s);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t off = (uint64_t)((ks * 32) >> 4);
-            const uint64_t qh = make_sdesc(qbase + h * QT) + off, ql = make_sdesc(qbase + 2 * QT + h * QT) + off;
-            const uint64_t kh = make_sdesc(sa + h * KT) + off, kl = make_sdesc(sa + 2 * KT + h * KT) + off;
-            tc_mma(d, qh, kh, idesc_s, (h | ks) != 0 ? 1u : 0u);
-            tc_mma(d, qh, kl, idesc_s, 1u);
-            tc_mma(d, ql, kh, idesc_s, 1u);
-          }
-        }
-        tc_commit(kvempty0 + 8 * slot);
-        tc_commit(sfull0 + 8 * a);
-        if (++slot == NSLOT) { slot = 0; ph ^= 1; }
-        ++g;
-      };
-      for (int j = 0; j < n; ++j) issue_s();
-      issue_s();
-      const uint32_t dO = tmem_base + 128u;
-      for (int j = 0; j < n; ++j) {
-        if (j + 1 < n) issue_s();
-        mbar_wait(pready, (uint32_t)(j & 1));
-        mbar_wait(kvfull0 + 8 * slot, ph);
-        tc_fence_after();
-        const uint32_t sv = ring + slot * SLOT;
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {
           const uint64_t off = (uint64_t)((ks * 32) >> 4);
-          const uint64_t ph_ = make_sdesc(pbase) + off, pl_ = make_sdesc(pbase + PT) + off;
-          const uint64_t vh = make_sdesc(sv) + off, vl = make_sdesc(sv + 2 * KT) + off;
-          tc_mma(dO, ph_, vh, idesc_o, (j | ks) != 0 ? 1u : 0u);
-          tc_mma(dO, ph_, vl, idesc_o, 1u);
-          tc_mma(dO, pl_, vh, idesc_o, 1u);
+          const uint64_t qh = make_sdesc(qbase + h * QT + qoff) + off, ql = make_sdesc(qbase + 2 * QT + h * QT + qoff) + off;
+          const uint64_t kh = make_sdesc(sa + h * KT) + off, kl = make_sdesc(sa + 2 * KT + h * KT) + off;
+          wgmma_n64(s, qh, kh, (h | ks) != 0 ? 1u : 0u);
+          wgmma_n64(s, qh, kl, 1u);
+          wgmma_n64(s, ql, kh, 1u);
         }
-        tc_commit(kvempty0 + 8 * slot);
-        tc_commit(pfree);
-        if (++slot == NSLOT) { slot = 0; ph ^= 1; }
       }
-      tc_commit(ofull);
-    }
-  } else if (warp >= 4) {
-    const int ew = warp & 3;
-    const int row = ew * 32 + lane;  // query row of this thread (= TMEM lane)
-    const uint32_t tlane = tmem_base + ((uint32_t)(ew * 32) << 16);
-    int g = 0;
-    float m = -INFINITY;
-    auto key_masks = [&](int j, uint32_t& m0, uint32_t& m1) {
-      const int k0 = j * AK + lane - kshift, k1 = k0 + 32;  // key index inside the utterance
-      bool v0 = k0 >= 0 && k0 < klen, v1 = k1 >= 0 && k1 < klen;
-      if (p.keymask) {
-        if (v0) v0 = __ldg(p.keymask + uk.x + k0) != 0.f;
-        if (v1) v1 = __ldg(p.keymask + uk.x + k1) != 0.f;
-      }
-      m0 = __ballot_sync(0xffffffffu, v0);
-      m1 = __ballot_sync(0xffffffffu, v1);
+      wg_commit();
+      fence_acc(s);
+      wg_wait<0>();
+      fence_acc(s);
+      release();
     };
-    // pass 1: exact row maximum of the raw scores over the valid keys
-    for (int j = 0; j < n; ++j, ++g) {
-      const int a = g & 1;
-      uint32_t m0, m1;
-      key_masks(j, m0, m1);
-      mbar_wait(sfull0 + 8 * a, (g >> 1) & 1);
-      tc_fence_after();
-      uint32_t v0[32], v1[32];
-      tmem_ld32(tlane + (uint32_t)(a * AK), v0);
-      tmem_ld32(tlane + (uint32_t)(a * AK + 32), v1);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(sempty0 + 8 * a);
+    // valid keys among this thread's 16 columns of key tile j: bit j of the mask <-> accumulator element j / j + 2
+    auto key_mask = [&](int j) {
+      uint32_t m = 0;
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        if ((m0 >> c) & 1u) m = fmaxf(m, __uint_as_float(v0[c]));
-        if ((m1 >> c) & 1u) m = fmaxf(m, __uint_as_float(v1[c]));
+      for (int e = 0; e < 16; ++e) {
+        const int c = frag_col(lane, (e >> 1) * 4 + (e & 1));
+        const int k = j * AK + c - kshift;  // key index inside the utterance
+        bool v = k >= 0 && k < klen;
+        if (v && p.keymask) v = __ldg(p.keymask + uk.x + k) != 0.f;
+        m |= (v ? 1u : 0u) << e;
+      }
+      return m;
+    };
+    mbar_wait(qfull, 0);
+    // pass 1: exact row maximum of the raw scores over the valid keys
+    float m0 = -INFINITY, m1 = -INFINITY;
+    for (int j = 0; j < n; ++j) {
+      const uint32_t km = key_mask(j);
+      scores();
+#pragma unroll
+      for (int e = 0; e < 16; ++e) {
+        if ((km >> e) & 1u) {
+          const int jj = (e >> 1) * 4 + (e & 1);
+          m0 = fmaxf(m0, s[jj]);
+          m1 = fmaxf(m1, s[jj + 2]);
+        }
       }
     }
-    const float mu = m == -INFINITY ? 0.f : m;
+#pragma unroll
+    for (int x = 1; x <= 2; x <<= 1) {
+      m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, x));
+      m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, x));
+    }
+    const float mu0 = m0 == -INFINITY ? 0.f : m0, mu1 = m1 == -INFINITY ? 0.f : m1;
     const float c2 = p.c2;
-    float l = 0.f;
-    const uint32_t prow = pbase + (uint32_t)row * 128u;
-    const int sw = row & 7;
-    // pass 2: p = exp(scale * (s - m)); O += P V
-    for (int j = 0; j < n; ++j, ++g) {
-      const int a = g & 1;
-      uint32_t m0, m1;
-      key_masks(j, m0, m1);
-      mbar_wait(sfull0 + 8 * a, (g >> 1) & 1);
-      tc_fence_after();
-      uint32_t v0[32], v1[32];
-      tmem_ld32(tlane + (uint32_t)(a * AK), v0);
-      tmem_ld32(tlane + (uint32_t)(a * AK + 32), v1);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(sempty0 + 8 * a);
-      float pv[64];
+    float l0 = 0.f, l1 = 0.f;
+    float o[64];
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        pv[c] = ((m0 >> c) & 1u) ? exp2f((__uint_as_float(v0[c]) - mu) * c2) : 0.f;
-        pv[32 + c] = ((m1 >> c) & 1u) ? exp2f((__uint_as_float(v1[c]) - mu) * c2) : 0.f;
+    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    // pass 2: p = exp(scale * (s - m)); O += P V with P as the register A operand (fp16 hi/lo planes of 256 p, so that
+    // weights down to 2^-33 survive the split)
+    for (int j = 0; j < n; ++j) {
+      const uint32_t km = key_mask(j);
+      scores();
+      float pv[32];
+#pragma unroll
+      for (int e = 0; e < 16; ++e) {
+        const int jj = (e >> 1) * 4 + (e & 1);
+        const bool v = (km >> e) & 1u;
+        pv[jj] = v ? exp2f((s[jj] - mu0) * c2) : 0.f;
+        pv[jj + 2] = v ? exp2f((s[jj + 2] - mu1) * c2) : 0.f;
+        l0 += pv[jj];
+        l1 += pv[jj + 2];
       }
+      uint32_t ah[4][4], al[4][4];
 #pragma unroll
-      for (int c = 0; c < 64; ++c) l += pv[c];
-      if (j > 0) mbar_wait(pfree, (uint32_t)((j - 1) & 1));  // the MMAs of P_{j-1} V_{j-1} have read the P buffer
-#pragma unroll
-      for (int ch = 0; ch < 8; ++ch) {
-        uint32_t hw[4], lw[4];
+      for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const float x0 = pv[ch * 8 + 2 * q] * 256.0f, x1 = pv[ch * 8 + 2 * q + 1] * 256.0f;
+          const float x0 = pv[8 * kk + 2 * q] * 256.0f, x1 = pv[8 * kk + 2 * q + 1] * 256.0f;
           const __half2 hh = __floats2half2_rn(x0, x1);
           const float2 hf = __half22float2(hh);
-          const __half2 ll = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-          hw[q] = *reinterpret_cast<const uint32_t*>(&hh);
-          lw[q] = *reinterpret_cast<const uint32_t*>(&ll);
+          ah[kk][q] = *reinterpret_cast<const uint32_t*>(&hh);
+          al[kk][q] = pack_half2(x0 - hf.x, x1 - hf.y);
         }
-        const uint32_t dst = prow + (uint32_t)((ch ^ sw) << 4);  // 128B swizzle: 16-byte chunk index XOR (row mod 8)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(hw[0]), "r"(hw[1]), "r"(hw[2]), "r"(hw[3]) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst + PT), "r"(lw[0]), "r"(lw[1]), "r"(lw[2]), "r"(lw[3]) : "memory");
       }
-      proxy_fence_smem();  // generic-proxy stores -> visible to the tensor core's async-proxy reads
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pready);
+      mbar_wait(kvfull0 + 8 * slot, ph);
+      const uint32_t sv = ring + slot * SLOT;
+      wg_fence();
+      fence_acc(o);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t off = (uint64_t)((kk * 32) >> 4);
+        const uint64_t vh = make_sdesc(sv) + off, vl = make_sdesc(sv + 2 * KT) + off;
+        wgmma_rs_n128(o, ah[kk], vh, 1u);
+        wgmma_rs_n128(o, ah[kk], vl, 1u);
+        wgmma_rs_n128(o, al[kk], vh, 1u);
+      }
+      wg_commit();
+      fence_acc(o);
+      wg_wait<0>();
+      fence_acc(o);
+      release();
+    }
+#pragma unroll
+    for (int x = 1; x <= 2; x <<= 1) {
+      l0 += __shfl_xor_sync(0xffffffffu, l0, x);
+      l1 += __shfl_xor_sync(0xffffffffu, l1, x);
     }
     // epilogue: O / (256 l)
-    mbar_wait(ofull, 0);
-    tc_fence_after();
-    const float inv = l > 0.f ? 1.0f / (256.0f * l) : 0.f;
-    const bool valid = q0 + row < uq.y;
-    const int64_t grow = (int64_t)qrow0 + row;
-#pragma unroll 1
-    for (int ch = 0; ch < 4; ++ch) {
-      uint32_t v[32];
-      tmem_ld32(tlane + 128u + (uint32_t)(ch * 32), v);
-      if (valid) {
-        float o[32];
+    const float inv0 = l0 > 0.f ? 1.0f / (256.0f * l0) : 0.f, inv1 = l1 > 0.f ? 1.0f / (256.0f * l1) : 0.f;
 #pragma unroll
-        for (int c = 0; c < 32; ++c) o[c] = __uint_as_float(v[c]) * inv;
-        if (p.out) {
-          float4* dst = reinterpret_cast<float4*>(p.out + grow * p.ldo + head * HD + ch * 32);
+    for (int hh = 0; hh < 2; ++hh) {
+      const int qr = 64 * cw + rw + 8 * hh;  // query row inside the tile
+      if (q0 + qr >= uq.y) continue;
+      const int64_t grow = (int64_t)qrow0 + qr;
+      const float inv = hh ? inv1 : inv0;
 #pragma unroll
-          for (int q = 0; q < 8; ++q) dst[q] = make_float4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]);
-        }
+      for (int nb = 0; nb < 16; ++nb) {
+        const int jj = 4 * nb + 2 * hh;
+        const int col = head * HD + frag_col(lane, jj);
+        const float a = o[jj] * inv, bb = o[jj + 1] * inv;
+        if (p.out) *reinterpret_cast<float2*>(p.out + grow * p.ldo + col) = make_float2(a, bb);
         if (p.oh) {
-          split_store16(p.oh + grow * p.ldh + head * HD + ch * 32, p.ol + grow * p.ldh + head * HD + ch * 32, o);
-          split_store16(p.oh + grow * p.ldh + head * HD + ch * 32 + 16, p.ol + grow * p.ldh + head * HD + ch * 32 + 16, o + 16);
+          const __half2 h2 = __floats2half2_rn(a, bb);
+          const float2 hf = __half22float2(h2);
+          *reinterpret_cast<__half2*>(p.oh + grow * p.ldh + col) = h2;
+          *reinterpret_cast<__half2*>(p.ol + grow * p.ldh + col) = __floats2half2_rn(a - hf.x, bb - hf.y);
         }
       }
     }
-    tc_fence_before();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ATT_TMEM) : "memory");
   }
 }
 
@@ -336,7 +299,7 @@ bool attention_tc_enabled() {
   int v = g_attn_tc.load(std::memory_order_relaxed);
   if (v < 0) {
     const char* e = getenv("SSB_ATTN_TC");
-    v = e ? (atoi(e) != 0 ? 1 : 0) : 1;  // default on (validated on B200: tests/test_gpu_tc.py, profiles/r02_*attention*)
+    v = e ? (atoi(e) != 0 ? 1 : 0) : 1;  // default on (checked against the fp32 kernel by tests/test_gpu_tc.py)
     g_attn_tc.store(v, std::memory_order_relaxed);
   }
   return v != 0 && tc_available();
@@ -383,7 +346,7 @@ int attention_tc(Ctx& ctx, const AttnTCArgs& a) {
   p.c2 = a.scale * 1.4426950408889634f;
   p.out = a.out; p.ldo = a.ldo; p.oh = a.oh; p.ol = a.ol; p.ldh = a.ldh;
   dim3 grid((a.max_q + AQ - 1) / AQ, a.heads, a.B);
-  attention_tc_kernel<<<grid, 256, ATT_SMEM, ctx.stream>>>(mq_h, mq_l, mk_h, mk_l, mv_h, mv_l, p);
+  attention_tc_kernel<<<grid, ATT_THREADS, ATT_SMEM, ctx.stream>>>(mq_h, mq_l, mk_h, mk_l, mv_h, mv_l, p);
   SSB_CUDA(cudaGetLastError());
   ++g_launches;
   return 0;

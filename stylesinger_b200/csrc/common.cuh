@@ -1,4 +1,4 @@
-// Common definitions for the stylesinger_b200 CUDA library (sm_100a only).
+// Common definitions for the stylesinger_b200 CUDA library (sm_90a only).
 //
 // Data layout used by every kernel in this library ("guard-banded ragged rows"):
 //   * activations are channels-last fp32 matrices [rows, C];

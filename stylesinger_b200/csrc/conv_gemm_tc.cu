@@ -1,14 +1,12 @@
-// tcgen05 + TMA + TMEM implicit-GEMM conv1d (see conv_gemm_tc.cuh).  sm_100a only.
+// wgmma + TMA implicit-GEMM conv1d for Hopper (see conv_gemm_tc.cuh).  sm_90a only.
 //
 // CTA = 384 threads, persistent over (M-tile, N-tile) pairs:
 //   warp 0 (1 lane)  TMA producer: per K block loads A_hi, A_lo [128x64] and W_hi, W_lo [BNx64] (128B swizzle)
-//   warp 1 (1 lane)  MMA issuer:   4 K-steps x 3 products of tcgen05.mma.kind::f16 (M128 N=BN K16), fp32 in TMEM
-//   warp 2           TMEM allocator (2 x BN columns = 2 accumulator buffers)
-//   warp 3           L2 prefetch of the next tile's epilogue operands (residual / skip rows)
-//   warps 4-11       epilogue: tcgen05.ld 32 lanes x 32 columns -> registers -> fused epilogue -> global,
-//                    with the epilogue's own global operands (residual / skip) prefetched one chunk ahead
-// smem ring: BN=128: 3 stages x 64 KB, BN=64: 4 stages x 48 KB; mbarriers: full/empty per stage,
-// tmem_full/tmem_empty per accumulator buffer.  BN=64 is picked for small problems (more CTAs in flight).
+//   warps 4-11       two consumer warpgroups: each issues the 3-product wgmma chain (M64 N=BN K16, fp32 accumulators in
+//                    registers) for its 64 rows, then runs the fused epilogue through shared-memory transpose buffers
+// smem ring: BN=128: 3 stages x 64 KB, BN=64: 4 stages x 48 KB; mbarriers full/empty per stage.  BN=64 is picked for
+// small problems (more CTAs in flight).  The CTA-pair variant (cluster of 2) gives each CTA its own row tile and one half
+// of a shared weight tile, which TMA multicasts into both CTAs.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -26,33 +24,39 @@ namespace {
 
 constexpr int BM = 128, BK = 64;
 constexpr int A_TILE = BM * BK * 2;  // 16 KB
-constexpr int EPI_WARPS = 8;                       // two warps per TMEM lane quarter, alternating 32-column chunks
+constexpr int EPI_WARPS = 8;                       // two consumer warpgroups
 constexpr int NTHREADS = 128 + 32 * EPI_WARPS;
 constexpr int XPOSE_BYTES = EPI_WARPS * 32 * 32 * 4;  // epilogue transpose buffers: one [32 x 32] fp32 per warp
 
-template <int BN>
+constexpr int HALO = 8;                     // largest dilation served by the tap-reuse variant (DiffNet: 1, 2, 4, 8)
+constexpr int A3_ROWS = BM + 2 * HALO;      // 144
+constexpr int A3_TILE = A3_ROWS * BK * 2;   // 18 KB per plane (a multiple of 1024: swizzle pattern alignment)
+constexpr int ASLOTS = 2;                   // tap-reuse activation ring
+
+template <int BN, bool REUSE>
 struct Cfg {
   static constexpr int B_TILE = BN * BK * 2;
-  static constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;
-  static constexpr int STAGES = BN == 256 ? 2 : (BN == 128 ? 3 : 4);
-  static constexpr int SMEM = STAGES * STAGE + XPOSE_BYTES + 1024 + 256;
-  static constexpr uint32_t TMEM_COLS = 2 * BN;  // BN = 256: the whole 512-column TMEM
+  static constexpr int STAGE = REUSE ? 2 * B_TILE : 2 * A_TILE + 2 * B_TILE;  // REUSE: weights only
+  static constexpr int STAGES = BN == 128 ? 3 : 4;
+  static constexpr int ARING = REUSE ? ASLOTS * 2 * A3_TILE : 0;
+  static constexpr int SMEM = ARING + STAGES * STAGE + XPOSE_BYTES + 1024 + 256;
+  static_assert(SMEM <= 227 * 1024, "exceeds the 227 KB of shared memory a Hopper block can have");
 };
 
 struct TCParams {
   const int2* tiles;
   int ntiles, NT, taps, kchunks, kchunks2, dil, center, N;
-  int dbg;  // SSB_TC_DEBUG probe bits (tools/gemm_probe.py): 1 = epilogue drains TMEM only, 2 = no MMAs, 4 = no TMA loads
+  int dbg;  // SSB_TC_DEBUG probe bits (tools/gemm_probe.py): 1 = no epilogue, 2 = no MMAs
   EpiTC e;
 };
 
 using namespace tc;
 
 // ---- epilogue ------------------------------------------------------------------------------------------------
-// tcgen05.ld hands every lane one ROW of the accumulator (32 consecutive columns).  Writing rows straight from that
-// mapping makes each warp store touch 32 different 128-byte lines (16 B each); measured with tools/gemm_probe.py the
-// epilogue alone then costs as much as the MMAs.  So each epilogue warp transposes its 32 x 32 chunk through a 4 KB
-// shared-memory buffer (float4 chunks XOR-swizzled by row: conflict-free both ways) and works in a COALESCED mapping:
+// The wgmma accumulator fragment scatters a row over four lanes in pairs of columns.  Storing from that mapping makes
+// every warp store touch many 128-byte lines with 8-byte pieces.  So each pair of consumer warps writes its 32 rows, 64
+// columns at a time, into two 4 KB shared-memory buffers (float4 chunks XOR-swizzled by row) and each warp then works on
+// one [32 x 32] chunk in a COALESCED mapping:
 // step i of 8 handles rows 4i + lane/8, columns 4*(lane%8) .. +3, i.e. every warp access covers 4 full 128-byte lines.
 
 struct Pre {
@@ -127,63 +131,7 @@ __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& uh, uint
   uh = *reinterpret_cast<const uint32_t*>(&h0);
   ul = *reinterpret_cast<const uint32_t*>(&l0);
 }
-__device__ __forceinline__ void split_store4(__half* hi, __half* lo, float a, float b, float c, float d) {
-  const __half2 h0 = __floats2half2_rn(a, b), h1 = __floats2half2_rn(c, d);
-  const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-  const __half2 l0 = __floats2half2_rn(a - f0.x, b - f0.y), l1 = __floats2half2_rn(c - f1.x, d - f1.y);
-  uint2 uh, ul;
-  uh.x = *reinterpret_cast<const uint32_t*>(&h0); uh.y = *reinterpret_cast<const uint32_t*>(&h1);
-  ul.x = *reinterpret_cast<const uint32_t*>(&l0); ul.y = *reinterpret_cast<const uint32_t*>(&l1);
-  *reinterpret_cast<uint2*>(hi) = uh;
-  *reinterpret_cast<uint2*>(lo) = ul;
-}
-__device__ __forceinline__ void split_store2(__half* hi, __half* lo, float a, float b) {
-  const __half2 h0 = __floats2half2_rn(a, b);
-  const float2 f0 = __half22float2(h0);
-  const __half2 l0 = __floats2half2_rn(a - f0.x, b - f0.y);
-  *reinterpret_cast<__half2*>(hi) = h0;
-  *reinterpret_cast<__half2*>(lo) = l0;
-}
-
-// Warp 3 pulls the NEXT tile's epilogue operands (residual / skip / accumulate rows) from HBM into L2 while the current
-// tile is being finished: the epilogue warps can keep only one chunk of loads in flight each, so with DRAM latency the
-// residual-layer kernels ran at 22 % tensor activity / 43 % of the DRAM bandwidth (profiles/r01_ncu_full_pair_v2_*).
-template <int MODE>
-__device__ __forceinline__ void prefetch_tile_l2(const EpiTC& e, int2 t, int n0, int bn, int lane, int mt) {
-  if (!e.l2_prefetch || (e.n_valid > 0 && n0 >= e.n_valid)) return;
-  const char* s1 = nullptr;
-  const char* s2 = nullptr;
-  int64_t st1 = 0, st2 = 0;       // row strides in bytes
-  uint32_t b1 = 0, b2 = 0;        // bytes per row (multiples of 16)
-  if constexpr (MODE == EPI_GENERIC) {
-    if (e.res) { s1 = reinterpret_cast<const char*>(e.res + n0); st1 = 4 * (int64_t)e.ld_res; b1 = (uint32_t)bn * 4u; }
-    if (e.accum && e.out) { s2 = reinterpret_cast<const char*>(e.out + n0); st2 = 4 * (int64_t)e.ldo; b2 = (uint32_t)bn * 4u; }
-  } else if constexpr (MODE == EPI_RES_SKIP) {
-    if (n0 < e.C) {
-      if (e.rh) {
-        s1 = reinterpret_cast<const char*>(e.rh + n0); s2 = reinterpret_cast<const char*>(e.rl + n0);
-        st1 = st2 = 2 * (int64_t)e.ld_rh; b1 = b2 = (uint32_t)bn * 2u;
-      } else {
-        s1 = reinterpret_cast<const char*>(e.res + n0); st1 = 4 * (int64_t)e.ld_res; b1 = (uint32_t)bn * 4u;
-      }
-    } else if (!e.skip_init) {
-      if (e.skip_tiled) {  // the tile's accumulator is one contiguous 128 x C block: walk it in C-float pieces
-        s1 = reinterpret_cast<const char*>(e.skip + ((int64_t)(e.tile_base + mt) * TILE_M - t.x) * e.C); st1 = 4 * (int64_t)e.C; b1 = (uint32_t)e.C * 4u;
-      } else {
-        s1 = reinterpret_cast<const char*>(e.skip + (n0 - e.C)); st1 = 4 * (int64_t)e.ld_skip; b1 = (uint32_t)bn * 4u;
-      }
-    }
-  } else {  // EPI_GATE
-    if (e.add) { s1 = reinterpret_cast<const char*>(e.add + n0); st1 = 4 * (int64_t)e.ld_add; b1 = (uint32_t)bn * 4u; }
-  }
-  if (!s1 && !s2) return;
-  for (int rr = lane; rr < t.y; rr += 32) {
-    if (s1) bulk_prefetch_l2(s1 + (int64_t)(t.x + rr) * st1, b1);
-    if (s2) bulk_prefetch_l2(s2 + (int64_t)(t.x + rr) * st2, b2);
-  }
-}
-
-// One 32 x 32 accumulator chunk (columns [n, n+32)) of this warp: transpose, then the fused epilogue.
+// One 32 x 32 accumulator chunk (columns [n, n+32)) of this warp, already in its transpose buffer: the fused epilogue.
 // MODE is a template parameter (and the chunk loop is not unrolled) to keep the epilogue's code small: the first
 // version carried all three modes x 4-8 unrolled chunks = 13k SASS instructions and ran out of the instruction cache.
 // Everything that does not depend on the step (pointers, flags, slopes) is hoisted into registers: the epilogue warps
@@ -192,14 +140,9 @@ __device__ __forceinline__ float act_slope_of(int act, float slope) {  // act(v)
   return act == ACT_RELU ? 0.0f : (act == ACT_LRELU ? slope : 1.0f);
 }
 template <int MODE>
-__device__ __forceinline__ void epilogue_chunk(const EpiTC& e, float4* xb, int64_t r0, int nrows, int n, int lane,
-                                               const uint32_t (&raw)[32], const Pre& pre, int tq) {
+__device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb, int64_t r0, int nrows, int n, int lane,
+                                               const Pre& pre, int tq) {
   if (e.n_valid > 0 && n >= e.n_valid) return;  // warp-uniform
-#pragma unroll
-  for (int c = 0; c < 8; ++c)
-    xb[lane * 8 + (c ^ (lane & 7))] = make_float4(__uint_as_float(raw[4 * c]), __uint_as_float(raw[4 * c + 1]),
-                                                  __uint_as_float(raw[4 * c + 2]), __uint_as_float(raw[4 * c + 3]));
-  __syncwarp();
   const int q = lane & 7, rq = lane >> 3;  // step i: row rq + 4i, columns n4 .. n4 + 3
   const int n4 = n + 4 * q;
   const int64_t rb = r0 + rq;
@@ -371,1015 +314,226 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, float4* xb, int64
       po += sto; ph += sth; pl += sth;
     }
   }
-  __syncwarp();  // the next chunk reuses the transpose buffer
 }
 
-template <int BN, int MODE>
+// REUSE (3-tap convs, centre tap 1, dilation <= HALO, no second operand): per K block ONE halo-extended activation tile of
+// BM + 2 HALO rows is loaded into its own ring, and the three taps read it through wgmma descriptors whose start address
+// is moved by whole 128-byte rows (the 128B swizzle phase follows the shared-memory address, and the tile starts on a
+// 1024-byte boundary).  Per tap only the weight tile is loaded: a third of the activation bytes of the plain variant.
+template <int BN, int CL, int MODE, bool REUSE>
 __global__ void __launch_bounds__(NTHREADS, 1)
-conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                     const __grid_constant__ CUtensorMap tmA2_hi, const __grid_constant__ CUtensorMap tmA2_lo,
                     const __grid_constant__ CUtensorMap tmB2_hi, const __grid_constant__ CUtensorMap tmB2_lo,
                     const TCParams p) {
-  using K = Cfg<BN>;
+  using K = Cfg<BN, REUSE>;
   constexpr int STAGES = K::STAGES;
+  constexpr int HB = BN / CL;  // weight rows this CTA loads per K block (CL == 2: and multicasts to its peer)
+  constexpr int NCH = BN / 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float4* xpose = reinterpret_cast<float4*>(smem + STAGES * K::STAGE);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * K::STAGE + XPOSE_BYTES);
-  // bars: full[STAGES], empty[STAGES], tfull[2], tempty[2]; then the TMEM base address
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * STAGES, tfull0 = empty0 + 8 * STAGES, tempty0 = tfull0 + 16;
+  // [activation ring (REUSE)][stage ring][transpose buffers][barriers]
+  float* xpose = reinterpret_cast<float*>(smem + K::ARING + STAGES * K::STAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + K::ARING + STAGES * K::STAGE + XPOSE_BYTES);
+  const uint32_t abase = smem_u32(smem), sbase = abase + K::ARING;
+  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * STAGES, afull0 = empty0 + 8 * STAGES, aempty0 = afull0 + 8 * ASLOTS;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t rank = CL > 1 ? cluster_rank() : 0u;
+  const int cid = (int)blockIdx.x / CL, ncl = (int)gridDim.x / CL;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, CL * EPI_WARPS);  // every consumer warp of every CTA that receives this stage's weights
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, EPI_WARPS + 1);  // + the L2 prefetch warp
+    for (int s = 0; s < ASLOTS; ++s) {
+      mbar_init(afull0 + 8 * s, 1);
+      mbar_init(aempty0 + 8 * s, EPI_WARPS);      // activation tiles are this CTA's own
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(K::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
+  if (CL > 1) cluster_sync_all();  // both CTAs' barriers initialised before any multicast or remote arrive
+  else __syncthreads();
 
-  const int total = p.ntiles * p.NT;
+  const int total = (CL > 1 ? (p.ntiles + 1) / 2 : p.ntiles) * p.NT;
   const int nk1 = p.taps * p.kchunks;
   const int nk = nk1 + p.kchunks2;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-        const int mt = tile / p.NT, nt = tile - mt * p.NT;
+  if (warp < 4) {  // warpgroup 0 only runs the TMA producer: its registers go to the consumer warpgroups
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (warp == 0 && lane == 0) {
+      int stage = 0, as = 0;
+      uint32_t phase = 0, aph = 0;
+      // weight tile (or this CTA's half of it, multicast to the pair) of one K block into stage `stage`
+      auto load_b = [&](const CUtensorMap* mb_h, const CUtensorMap* mb_l, int c0, int brow, uint32_t extra_bytes) {
+        mbar_wait(empty0 + 8 * stage, phase ^ 1);
+        const uint32_t fb = full0 + 8 * stage;
+        mbar_expect_tx(fb, 2 * K::B_TILE + extra_bytes);
+        const uint32_t sb = sbase + stage * K::STAGE + (REUSE ? 0u : (uint32_t)(2 * A_TILE));
+        if (CL > 1) {
+          const uint32_t boff = rank * (uint32_t)(HB * BK * 2);
+          tma_load_2d_mc(sb + boff, mb_h, fb, c0, brow + (int)rank * HB, (uint16_t)3);
+          tma_load_2d_mc(sb + K::B_TILE + boff, mb_l, fb, c0, brow + (int)rank * HB, (uint16_t)3);
+        } else {
+          tma_load_2d(sb, mb_h, fb, c0, brow);
+          tma_load_2d(sb + K::B_TILE, mb_l, fb, c0, brow);
+        }
+        return fb;
+      };
+      for (int tile = cid; tile < total; tile += ncl) {
+        const int mq = tile / p.NT, nt = tile - mq * p.NT;
+        int mt = CL * mq + (int)rank;
+        if (mt >= p.ntiles) mt = CL * mq;  // odd tile count: the peer re-loads the leader's rows and writes nothing
         const int row0 = p.tiles[mt].x;
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(empty0 + 8 * stage, phase ^ 1);
-          const uint32_t fb = full0 + 8 * stage;
-          if (p.dbg & 4) {
-            mbar_arrive(fb);
+        if constexpr (REUSE) {
+          for (int kc = 0; kc < p.kchunks; ++kc) {
+            mbar_wait(aempty0 + 8 * as, aph ^ 1);
+            const uint32_t ab = afull0 + 8 * as, sa = abase + as * (2 * A3_TILE);
+            mbar_expect_tx(ab, 2 * A3_TILE);
+            tma_load_2d(sa, &tmA_hi, ab, kc * BK, row0 - HALO);
+            tma_load_2d(sa + A3_TILE, &tmA_lo, ab, kc * BK, row0 - HALO);
+            if (++as == ASLOTS) { as = 0; aph ^= 1; }
+            for (int tap = 0; tap < 3; ++tap) {
+              load_b(&tmB_hi, &tmB_lo, kc * BK, tap * p.N + nt * BN, 0u);
+              if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+          }
+        } else {
+          for (int kb = 0; kb < nk; ++kb) {
+            const bool second = kb >= nk1;
+            const int tap = second ? 0 : kb / p.kchunks;
+            const int c0 = second ? (kb - nk1) * BK : (kb - tap * p.kchunks) * BK;
+            const int arow = second ? row0 : row0 + (tap - p.center) * p.dil;
+            // the expect_tx of load_b also covers this CTA's two activation boxes of the same stage
+            const uint32_t fb = load_b(second ? &tmB2_hi : &tmB_hi, second ? &tmB2_lo : &tmB_lo, c0,
+                                       second ? nt * BN : tap * p.N + nt * BN, (uint32_t)(2 * A_TILE));
+            const uint32_t sa = sbase + stage * K::STAGE;
+            tma_load_2d(sa, second ? &tmA2_hi : &tmA_hi, fb, c0, arow);
+            tma_load_2d(sa + A_TILE, second ? &tmA2_lo : &tmA_lo, fb, c0, arow);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            continue;
           }
-          mbar_expect_tx(fb, K::STAGE);
-          const uint32_t sa = sbase + stage * K::STAGE;
-          if (kb < nk1) {
-            const int tap = kb / p.kchunks;
-            const int c0 = (kb - tap * p.kchunks) * BK;
-            const int arow = row0 + (tap - p.center) * p.dil;
-            const int brow = tap * p.N + nt * BN;
-            tma_load_2d(sa, &tmA_hi, fb, c0, arow);
-            tma_load_2d(sa + A_TILE, &tmA_lo, fb, c0, arow);
-            tma_load_2d(sa + 2 * A_TILE, &tmB_hi, fb, c0, brow);
-            tma_load_2d(sa + 2 * A_TILE + K::B_TILE, &tmB_lo, fb, c0, brow);
-          } else {
-            const int c0 = (kb - nk1) * BK;
-            tma_load_2d(sa, &tmA2_hi, fb, c0, row0);
-            tma_load_2d(sa + A_TILE, &tmA2_lo, fb, c0, row0);
-            tma_load_2d(sa + 2 * A_TILE, &tmB2_hi, fb, c0, nt * BN);
-            tma_load_2d(sa + 2 * A_TILE + K::B_TILE, &tmB2_lo, fb, c0, nt * BN);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // instruction descriptor: D=F32, A=B=F16, both K-major, N=BN, M=128
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++it) {
-        const int a = it & 1;
-        const uint32_t aph = (it >> 1) & 1;
-        mbar_wait(tempty0 + 8 * a, aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(a * BN);
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(full0 + 8 * stage, phase);
-          tc_fence_after();
-          const uint32_t sa = sbase + stage * K::STAGE;
-          const uint64_t dah = make_sdesc(sa), dal = make_sdesc(sa + A_TILE);
-          const uint64_t dbh = make_sdesc(sa + 2 * A_TILE), dbl = make_sdesc(sa + 2 * A_TILE + K::B_TILE);
-#pragma unroll
-          for (int ks = 0; ks < BK / 16; ++ks) {
-            const uint64_t off = (uint64_t)((ks * 32) >> 4);  // 16 fp16 = 32 bytes along K inside the swizzle atom
-            if (p.dbg & 2) continue;
-            tc_mma(d_tmem, dah + off, dbh + off, idesc, (kb | ks) != 0 ? 1u : 0u);
-            tc_mma(d_tmem, dah + off, dbl + off, idesc, 1u);
-            tc_mma(d_tmem, dal + off, dbh + off, idesc, 1u);
-          }
-          tc_commit(empty0 + 8 * stage);  // smem stage reusable once these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit(tfull0 + 8 * a);        // accumulator complete -> epilogue
-      }
-    }
-  } else if (warp == 3) {
-    if ((int)blockIdx.x < total) {
-      const int mt = (int)blockIdx.x / p.NT, nt = (int)blockIdx.x - mt * p.NT;
-      prefetch_tile_l2<MODE>(p.e, p.tiles[mt], nt * BN, BN, lane, mt);
-    }
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++it) {
-      const int a = it & 1;
-      if (lane == 0) mbar_wait(tfull0 + 8 * a, (it >> 1) & 1);  // pace: one tile ahead of the epilogue
+    __syncwarp();
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+    // Two consumer warpgroups; warpgroup cw owns accumulator rows [64 cw, 64 cw + 64).  For the epilogue the warps pair up:
+    // pair ew (warps 4 + 2 ew, 5 + 2 ew) holds rows [32 ew, 32 ew + 32) and stages them, 64 columns at a time, into two
+    // [32 x 32] transpose buffers; warp parity eg then runs the fused epilogue on chunk 2 cp + eg of that pair of chunks.
+    const int cw = (warp - 4) >> 2;
+    const int ew = (warp - 4) >> 1;
+    const int eg = warp & 1;
+    float* xb_pair = xpose + ew * 2048;
+    const uint32_t pair_bar = 1u + (uint32_t)ew;
+    const uint32_t peer_empty0 = CL > 1 ? mapa_u32(empty0, rank ^ 1u) : 0u;
+    int stage = 0, as = 0;
+    uint32_t phase = 0, aph = 0;
+    float acc[BN / 2];
+    auto release_b = [&](int st) {  // this warp has finished reading stage st (in both CTAs' counts when CL == 2)
       __syncwarp();
-      {
-        const int nx = tile + gridDim.x;
-        if (nx < total) {
-          const int mt = nx / p.NT, nt = nx - mt * p.NT;
-          prefetch_tile_l2<MODE>(p.e, p.tiles[mt], nt * BN, BN, lane, mt);
+      if (lane == 0) {
+        mbar_arrive(empty0 + 8 * st);
+        if (CL > 1) mbar_arrive_cluster(peer_empty0 + 8 * st);
+      }
+    };
+    auto mma_block = [&](uint64_t dah, uint64_t dal, uint64_t dbh, uint64_t dbl) {
+      if (p.dbg & 2) return;
+      wg_fence();
+      fence_acc(acc);
+#pragma unroll
+      for (int ks = 0; ks < BK / 16; ++ks) {
+        const uint64_t off = (uint64_t)((ks * 32) >> 4);  // 16 fp16 = 32 bytes along K inside the swizzle atom
+        if constexpr (BN == 128) {
+          wgmma_n128(acc, dah + off, dbh + off, 1u);
+          wgmma_n128(acc, dah + off, dbl + off, 1u);
+          wgmma_n128(acc, dal + off, dbh + off, 1u);
+        } else {
+          wgmma_n64(acc, dah + off, dbh + off, 1u);
+          wgmma_n64(acc, dah + off, dbl + off, 1u);
+          wgmma_n64(acc, dal + off, dbh + off, 1u);
         }
       }
-      if (lane == 0) mbar_arrive_relaxed(tempty0 + 8 * a);
-    }
-  } else if (warp >= 4) {
-    const int ew = warp & 3;          // TMEM lanes [32*ew, 32*ew + 32)
-    const int eg = (warp - 4) >> 2;   // chunk parity handled by this warp
-    constexpr int NCH = BN / 32;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++it) {
-      const int a = it & 1;
-      const uint32_t aph = (it >> 1) & 1;
-      const int mt = tile / p.NT, nt = tile - mt * p.NT;
-      const int2 t = p.tiles[mt];
+      wg_commit();
+      fence_acc(acc);
+      wg_wait<1>();  // the MMAs of the previous K block are done: its stage can be refilled
+      fence_acc(acc);
+    };
+    for (int tile = cid; tile < total; tile += ncl) {
+      const int mq = tile / p.NT, nt = tile - mq * p.NT;
+      const int mt = CL * mq + (int)rank;
+      const int2 t = mt < p.ntiles ? p.tiles[mt] : make_int2(0, 0);
       const int64_t r0 = (int64_t)t.x + ew * 32;
       const int nrows = min(32, max(0, t.y - ew * 32));
-      float4* xb = xpose + (warp - 4) * 256;
+      const int tq = (p.e.tile_base + mt) * 4 + ew;
+      const int n0 = nt * BN;
       Pre cur, nxt;
-      prefetch_chunk<MODE>(p.e, r0, nrows, nt * BN + eg * 32, lane, cur, (p.e.tile_base + mt) * 4 + ew);  // issued before the accumulator is ready: overlaps the MMAs
-      mbar_wait(tfull0 + 8 * a, aph);
-      tc_fence_after();
-#pragma unroll 1
-      for (int ch = eg; ch < NCH; ch += 2) {
-        if (ch + 2 < NCH) prefetch_chunk<MODE>(p.e, r0, nrows, nt * BN + (ch + 2) * 32, lane, nxt, (p.e.tile_base + mt) * 4 + ew);
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(a * BN + ch * 32), v);
-        if (nrows > 0 && !(p.dbg & 1)) epilogue_chunk<MODE>(p.e, xb, r0, nrows, nt * BN + ch * 32, lane, v, cur, (p.e.tile_base + mt) * 4 + ew);
-        cur = nxt;
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_relaxed(tempty0 + 8 * a);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(K::TMEM_COLS) : "memory");
-  }
-}
-
-// tile (= cid + it * ncl) -> (row-tile pair, N tile).  With NT == 2 and an even cluster count the plain mapping
-// (mp = tile / 2, nt = tile % 2) hands every cluster tiles of ONE nt only; in the residual GEMM nt = 0 is the residual half
-// (planes in, planes out: the expensive epilogue) and nt = 1 the skip half, so half of the clusters did all the expensive
-// tiles and set the kernel's time (154 us measured whatever was optimised inside the epilogue).  Here the two tiles of a row
-// pair still go to neighbouring clusters, but which one gets which alternates with the iteration.
-__device__ __forceinline__ void pair_tile_decode(int tile, int cid, int ncl, int NT, int& mp, int& nt) {
-  if (NT == 2) {
-    const int it = (tile - cid) / ncl;
-    mp = tile >> 1;
-    nt = (ncl & 1) ? (tile & 1) : ((it + cid) & 1);
-  } else {
-    mp = tile / NT;
-    nt = tile - mp * NT;
-  }
-}
-
-// ---- epilogue warp loop of the CTA-pair kernels ------------------------------------------------------------------
-// Measured (tools/probe_layer.sh, profiles/r02_probe_layer_v5.md): with the epilogue reduced to draining TMEM the 1x1
-// residual GEMM still took 134 us of its 159 us - it was bound by the DEPENDENT global loads of its own epilogue operands
-// (one 32 x 32 chunk in flight per warp, issued one chunk ahead, and handed over with a register copy `cur = nxt` that
-// stalls on the load it copies).  Now the operands are fetched TWO CHUNKS ahead (across tile boundaries) into two ping-pong register sets.  The epilogue threads get the
-// registers for that with setmaxnreg (producer / MMA / allocator / L2-prefetch warps shrink to 40, the 8 epilogue warps grow to 232).
-struct EpiTile {
-  int64_t r0;   // first row of this warp's 32-row slice
-  int nrows;    // valid rows in the slice
-  int n0;       // first output column of the tile
-  int prob;     // dual kernel: 0 = gate problem, 1 = residual problem
-  int tq;       // tile-quarter index (row tile * 4 + warp quarter): address of the chunk-tiled skip accumulator
-  int ok;       // 0: past the last tile
-};
-template <int CPW, int MODE0, int MODE1, typename TileFn>
-__device__ __forceinline__ void pair_epilogue_loop(const EpiTC& e0, const EpiTC& e1, TileFn tile_at, float4* xb, uint32_t tmem_lanes,
-                                                   uint32_t acc_stride, uint32_t tfull0, uint32_t ltempty0, int eg, int lane, int dbg) {
-  auto fetch = [&](const EpiTile& t, int k, Pre& dst) {
-    const int n = t.n0 + (eg + 2 * k) * 32;
-    if constexpr (MODE0 == MODE1) prefetch_chunk<MODE0>(e0, t.r0, t.nrows, n, lane, dst, t.tq);
-    else if (t.prob == 0) prefetch_chunk<MODE0>(e0, t.r0, t.nrows, n, lane, dst, t.tq);
-    else prefetch_chunk<MODE1>(e1, t.r0, t.nrows, n, lane, dst, t.tq);
-  };
-  // DEPTH register sets, each owned by fixed chunk positions (no moves of registers with loads in flight - a rotating ring
-  // stalled every chunk on the scoreboard of the load issued one chunk earlier).  Even CPW: two sets in ping-pong, the chunk
-  // loop runs in pairs (lookahead = 2 chunks, crossing into the next tile); odd CPW: one set per chunk, fully unrolled.
-  constexpr int DEPTH = (CPW % 2 == 0) ? 2 : CPW;
-  EpiTile cur = tile_at(0);
-  Pre pr[DEPTH];
-  if (cur.ok) {
+      if (nrows > 0) prefetch_chunk<MODE>(p.e, r0, nrows, n0 + eg * 32, lane, cur, tq);  // overlaps the MMAs
 #pragma unroll
-    for (int k = 0; k < DEPTH; ++k) fetch(cur, k, pr[k]);
-  }
-  for (int it = 0; cur.ok; ++it) {
-    const int a = it & 1;
-    const EpiTile nx = tile_at(it + 1);
-    mbar_wait(tfull0 + 8 * a, (uint32_t)((it >> 1) & 1));
-    tc_fence_after();
-    // the accumulator chunks are pipelined as well: the tcgen05.ld of chunk k + 1 is in flight while chunk k is processed
-    // (ncu: the epilogue warps of the residual GEMM spent 9 % of their samples waiting on LDTM)
-    const uint32_t tacc = tmem_lanes + (uint32_t)a * acc_stride + (uint32_t)(eg * 32);
-    uint32_t vv[2][32];
-    tmem_ld32_issue(tacc, vv[0]);
-#pragma unroll 1
-    for (int k0 = 0; k0 < CPW; k0 += DEPTH) {
-#pragma unroll
-      for (int j = 0; j < DEPTH; ++j) {
-        uint32_t (&v)[32] = vv[j & 1];  // DEPTH is 1, 2 or 3: chunk k lives in buffer k & 1 for every k0 (k0 even or DEPTH == CPW)
-        const int k = k0 + j;
-        const int ch = eg + 2 * k;
-        tmem_ld_wait32(v);
-        if (k + 1 < CPW) tmem_ld32_issue(tacc + (uint32_t)((k + 1) * 64), vv[(j + 1) & 1]);
-        if (cur.nrows > 0 && !(dbg & 1)) {
-          if constexpr (MODE0 == MODE1) epilogue_chunk<MODE0>(e0, xb, cur.r0, cur.nrows, cur.n0 + ch * 32, lane, v, pr[j], cur.tq);
-          else if (cur.prob == 0) epilogue_chunk<MODE0>(e0, xb, cur.r0, cur.nrows, cur.n0 + ch * 32, lane, v, pr[j], cur.tq);
-          else epilogue_chunk<MODE1>(e1, xb, cur.r0, cur.nrows, cur.n0 + ch * 32, lane, v, pr[j], cur.tq);
-        }
-        // the register set just consumed takes the chunk DEPTH positions later: of this tile, or of the next one
-        if (k + DEPTH < CPW) fetch(cur, k + DEPTH, pr[j]);
-        else if (nx.ok) fetch(nx, k + DEPTH - CPW, pr[j]);
-      }
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive_cluster_relaxed(ltempty0 + 8 * a);
-    cur = nx;
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// CTA-pair kernel (cta_group::2): a cluster of two CTAs on one TPC computes a 256 x (2*HB) tile.  Each CTA stages its own
-// 128 rows of A (its own row tile of the ragged layout: the two row tiles of a pair need not be adjacent) and HB of
-// the 2*HB weight rows; the leader issues M=256 MMAs that read both CTAs' shared memory and write both CTAs' TMEM.
-// Per FLOP this halves the bytes each SM pulls through L2 (the limiter of the single-CTA kernel, profiles/r01_ncu_*).
-//   full[s]    leader only: 1 arrival (leader's expect_tx of 2 x STAGE bytes) + both CTAs' TMA transaction bytes
-//   empty[s]   per CTA: signalled by the leader's tcgen05.commit multicast to both CTAs
-//   tfull[a]   per CTA: same multicast commit;  tempty[a] leader only: 18 arrivals ((8 epilogue warps + the L2 prefetch warp) x 2 CTAs)
-template <int HB>
-struct Cfg2 {
-  static constexpr int BN = 2 * HB;
-  static constexpr int B_TILE = HB * BK * 2;
-  static constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;
-  static constexpr int STAGES = HB >= 96 ? 3 : 4;
-  static constexpr int SMEM = STAGES * STAGE + XPOSE_BYTES + 1024 + 256;
-  static constexpr uint32_t ACC_STRIDE = BN <= 64 ? 64 : (BN <= 128 ? 128 : 256);
-  static constexpr uint32_t TMEM_COLS = 2 * ACC_STRIDE;
-};
-
-template <int HB, int MODE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-conv_gemm_tc2_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-                     const __grid_constant__ CUtensorMap tmA2_hi, const __grid_constant__ CUtensorMap tmA2_lo,
-                     const __grid_constant__ CUtensorMap tmB2_hi, const __grid_constant__ CUtensorMap tmB2_lo,
-                     const TCParams p) {
-  using K = Cfg2<HB>;
-  constexpr int STAGES = K::STAGES;
-  constexpr int BN = K::BN;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float4* xpose = reinterpret_cast<float4*>(smem + STAGES * K::STAGE);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * K::STAGE + XPOSE_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * STAGES, tfull0 = empty0 + 8 * STAGES, tempty0 = tfull0 + 16;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();
-  const int cid = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 2 * EPI_WARPS + 2);  // + the two L2 prefetch warps
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(K::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();  // both CTAs' barriers initialised and TMEM allocated before any cross-CTA signal
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-
-  const int npairs = (p.ntiles + 1) >> 1;
-  const int total = npairs * p.NT;
-  const int nk1 = p.taps * p.kchunks;
-  const int nk = nk1 + p.kchunks2;
-
-  if (warp < 4) {  // warpgroup 0 (producer, MMA issuer, TMEM allocator, L2 prefetch) needs few registers
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t lfull0 = mapa_u32(full0, 0);  // the leader's full barriers (cluster address)
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = cid; tile < total; tile += ncl) {
-        int mp, nt;
-      pair_tile_decode(tile, cid, ncl, p.NT, mp, nt);
-        int mt = 2 * mp + (int)rank;
-        if (mt >= p.ntiles) mt = 2 * mp;  // odd tile count: the peer duplicates the leader's rows, writes nothing
-        const int row0 = p.tiles[mt].x;
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(empty0 + 8 * stage, phase ^ 1);
-          if (p.dbg & 4) {
-            if (rank == 0) mbar_arrive(full0 + 8 * stage);
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      if constexpr (REUSE) {
+        for (int kc = 0; kc < p.kchunks; ++kc) {
+          mbar_wait(afull0 + 8 * as, aph);
+          const uint32_t sa = abase + as * (2 * A3_TILE) + cw * 8192;
+          for (int tap = 0; tap < 3; ++tap) {
+            mbar_wait(full0 + 8 * stage, phase);
+            const uint32_t sb = sbase + stage * K::STAGE;
+            const uint32_t sh = (uint32_t)(HALO + (tap - 1) * p.dil) * 128u;  // whole rows
+            mma_block(make_sdesc(sa + sh), make_sdesc(sa + A3_TILE + sh), make_sdesc(sb), make_sdesc(sb + K::B_TILE));
+            if (prev >= 0) release_b(prev);
+            prev = stage;
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            continue;
           }
-          if (rank == 0) mbar_expect_tx(full0 + 8 * stage, 2 * K::STAGE);
-          const uint32_t fb = lfull0 + 8 * stage;
-          const uint32_t sa = sbase + stage * K::STAGE;
-          if (kb < nk1) {
-            const int tap = kb / p.kchunks;
-            const int c0 = (kb - tap * p.kchunks) * BK;
-            const int arow = row0 + (tap - p.center) * p.dil;
-            const int brow = tap * p.N + nt * BN + (int)rank * HB;
-            tma_load_2d_pair(sa, &tmA_hi, fb, c0, arow);
-            tma_load_2d_pair(sa + A_TILE, &tmA_lo, fb, c0, arow);
-            tma_load_2d_pair(sa + 2 * A_TILE, &tmB_hi, fb, c0, brow);
-            tma_load_2d_pair(sa + 2 * A_TILE + K::B_TILE, &tmB_lo, fb, c0, brow);
-          } else {
-            const int c0 = (kb - nk1) * BK;
-            const int brow = nt * BN + (int)rank * HB;
-            tma_load_2d_pair(sa, &tmA2_hi, fb, c0, row0);
-            tma_load_2d_pair(sa + A_TILE, &tmA2_lo, fb, c0, row0);
-            tma_load_2d_pair(sa + 2 * A_TILE, &tmB2_hi, fb, c0, brow);
-            tma_load_2d_pair(sa + 2 * A_TILE + K::B_TILE, &tmB2_lo, fb, c0, brow);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          wg_wait<0>();  // all three taps have read the activation tile
+          fence_acc(acc);
+          release_b(prev);
+          prev = -1;
+          __syncwarp();
+          if (lane == 0) mbar_arrive(aempty0 + 8 * as);
+          if (++as == ASLOTS) { as = 0; aph ^= 1; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      // instruction descriptor: D=F32, A=B=F16, both K-major, N = 2*HB, M = 256 (two CTAs x 128 rows)
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = cid; tile < total; tile += ncl, ++it) {
-        const int a = it & 1;
-        const uint32_t aph = (it >> 1) & 1;
-        mbar_wait(tempty0 + 8 * a, aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)a * K::ACC_STRIDE;
+      } else {
         for (int kb = 0; kb < nk; ++kb) {
           mbar_wait(full0 + 8 * stage, phase);
-          tc_fence_after();
           const uint32_t sa = sbase + stage * K::STAGE;
-          const uint64_t dah = make_sdesc(sa), dal = make_sdesc(sa + A_TILE);
-          const uint64_t dbh = make_sdesc(sa + 2 * A_TILE), dbl = make_sdesc(sa + 2 * A_TILE + K::B_TILE);
-#pragma unroll
-          for (int ks = 0; ks < BK / 16; ++ks) {
-            const uint64_t off = (uint64_t)((ks * 32) >> 4);
-            if (p.dbg & 2) continue;
-            tc_mma_pair(d_tmem, dah + off, dbh + off, idesc, (kb | ks) != 0 ? 1u : 0u);
-            tc_mma_pair(d_tmem, dah + off, dbl + off, idesc, 1u);
-            tc_mma_pair(d_tmem, dal + off, dbh + off, idesc, 1u);
-          }
-          tc_commit_pair(empty0 + 8 * stage);
+          mma_block(make_sdesc(sa + cw * 8192), make_sdesc(sa + A_TILE + cw * 8192), make_sdesc(sa + 2 * A_TILE),
+                    make_sdesc(sa + 2 * A_TILE + K::B_TILE));
+          if (prev >= 0) release_b(prev);
+          prev = stage;
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        tc_commit_pair(tfull0 + 8 * a);
+        wg_wait<0>();
+        fence_acc(acc);
+        if (prev >= 0) release_b(prev);
       }
-    }
-  } else if (warp == 3) {
-    const uint32_t ltempty0 = mapa_u32(tempty0, 0);
-    auto pf = [&](int tile) {
-      int mp, nt;
-      pair_tile_decode(tile, cid, ncl, p.NT, mp, nt);
-      const int mt = 2 * mp + (int)rank;
-      if (mt < p.ntiles) prefetch_tile_l2<MODE>(p.e, p.tiles[mt], nt * BN, BN, lane, mt);
-    };
-    if (cid < total) pf(cid);
-    int it = 0;
-    for (int tile = cid; tile < total; tile += ncl, ++it) {
-      const int a = it & 1;
-      if (lane == 0) mbar_wait(tfull0 + 8 * a, (it >> 1) & 1);
-      __syncwarp();
-      if (tile + ncl < total) pf(tile + ncl);
-      if (lane == 0) mbar_arrive_cluster_relaxed(ltempty0 + 8 * a);
-    }
-  }
-  } else {  // warps 4-11: the epilogue warpgroups take the registers the others released
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
-    const int ew = warp & 3;
-    const int eg = (warp - 4) >> 2;
-    auto tile_at = [&](int it) {
-      EpiTile t;
-      const int tile = cid + it * ncl;
-      t.ok = tile < total;
-      t.prob = 0;
-      if (!t.ok) { t.r0 = 0; t.nrows = 0; t.n0 = 0; t.tq = 0; return t; }
-      int mp, nt;
-      pair_tile_decode(tile, cid, ncl, p.NT, mp, nt);
-      const int mt = 2 * mp + (int)rank;
-      const int2 tl = mt < p.ntiles ? p.tiles[mt] : make_int2(0, 0);
-      t.r0 = (int64_t)tl.x + ew * 32;
-      t.tq = (p.e.tile_base + mt) * 4 + ew;
-      t.nrows = min(32, max(0, tl.y - ew * 32));
-      t.n0 = nt * BN;
-      return t;
-    };
-    pair_epilogue_loop<BN / 64, MODE, MODE>(p.e, p.e, tile_at, xpose + (warp - 4) * 256, tmem_base + ((uint32_t)(ew * 32) << 16),
-                                            K::ACC_STRIDE, tfull0, mapa_u32(tempty0, 0), eg, lane, p.dbg);
-  }
-  tc_fence_before();
-  cluster_sync_all();  // neither CTA may exit (or free TMEM) while its pair still reads / signals it
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(K::TMEM_COLS) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Tap-reuse variant of the CTA-pair kernel for 3-tap (dilated) convs without a second K segment: the DiffNet / DDiffNet
-// gate GEMM once the conditioner is hoisted.  The round-2 ncu captures show that GEMM moving ~1.4 GB of operands from L2
-// to shared memory per launch at ~8-10 TB/s - the chip-wide L2 -> SM throughput cap (B300_MICROARCH.md "LTS throughput
-// cap") - i.e. it is bound by operand traffic, not by the tensor pipe.  Half of that traffic is the SAME activation
-// rows loaded three times, once per tap, shifted by the dilation.  Here each K block's activation tile is loaded ONCE with
-// a halo (rows [row0 - 8, row0 + 136), one TMA box of 144 rows) and the three taps address it through UMMA descriptors
-// whose start address is advanced by whole 128-byte rows: in the K-major SWIZZLE_128B layout row m of the operand sits at
-// start + 128*m and the 16-byte-chunk XOR is a function of the absolute shared-memory address bits [7:9], so a descriptor
-// that starts s rows later reads exactly the rows TMA wrote for box rows s .. s+127.  Activation bytes per tile drop from
-// 3 x 32 KB to 36 KB per K block (-31 % of all operand traffic of the GEMM).
-// Rings: A (2 slots of 36 KB, one per K block, freed after its third tap), B (3-4 slots, one per (K block, tap)).
-constexpr int HALO = 8;                     // largest dilation served (DiffNet: 1, 2, 4, 8)
-constexpr int A3_ROWS = BM + 2 * HALO;      // 144
-constexpr int A3_TILE = A3_ROWS * BK * 2;   // 18 KB per plane (a multiple of 1024: swizzle pattern alignment)
-
-template <int HB>
-struct Cfg3 {
-  static constexpr int BN = 2 * HB;
-  static constexpr int B_TILE = HB * BK * 2;
-  static constexpr int ASLOT = 2 * A3_TILE, BSLOT = 2 * B_TILE;
-  static constexpr int ASLOTS = 2, BSLOTS = HB >= 128 ? 3 : 4;
-  static constexpr int RING = ASLOTS * ASLOT + BSLOTS * BSLOT;
-  static constexpr int SMEM = RING + XPOSE_BYTES + 1024 + 256;
-  static constexpr uint32_t ACC_STRIDE = BN <= 64 ? 64 : (BN <= 128 ? 128 : 256);
-  static constexpr uint32_t TMEM_COLS = 2 * ACC_STRIDE;
-};
-
-template <int HB, int MODE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-conv_gemm_tc2r_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                      const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, const TCParams p) {
-  using K = Cfg3<HB>;
-  constexpr int BN = K::BN, AS = K::ASLOTS, BS = K::BSLOTS;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float4* xpose = reinterpret_cast<float4*>(smem + K::RING);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + K::RING + XPOSE_BYTES);
-  // bars: afull[AS], aempty[AS], bfull[BS], bempty[BS], tfull[2], tempty[2]; then the TMEM base address
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * AS + 2 * BS + 4);
-  const uint32_t abase = smem_u32(smem), bbase = abase + AS * K::ASLOT;
-  const uint32_t afull0 = smem_u32(bars), aempty0 = afull0 + 8 * AS, bfull0 = aempty0 + 8 * AS, bempty0 = bfull0 + 8 * BS;
-  const uint32_t tfull0 = bempty0 + 8 * BS, tempty0 = tfull0 + 16;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();
-  const int cid = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < 2 * AS + 2 * BS; ++s) mbar_init(afull0 + 8 * s, 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 2 * EPI_WARPS + 2);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(K::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-
-  const int npairs = (p.ntiles + 1) >> 1;
-  const int total = npairs * p.NT;
-  const int nkc = p.kchunks;
-
-  if (warp < 4) {  // warpgroup 0 (producer, MMA issuer, TMEM allocator, L2 prefetch) needs few registers
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t lafull0 = mapa_u32(afull0, 0), lbfull0 = mapa_u32(bfull0, 0);
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0;
-      for (int tile = cid; tile < total; tile += ncl) {
-        int mp, nt;
-      pair_tile_decode(tile, cid, ncl, p.NT, mp, nt);
-        int mt = 2 * mp + (int)rank;
-        if (mt >= p.ntiles) mt = 2 * mp;
-        const int row0 = p.tiles[mt].x;
-        for (int kc = 0; kc < nkc; ++kc) {
-          mbar_wait(aempty0 + 8 * as, aph ^ 1);
-          if (rank == 0) mbar_expect_tx(afull0 + 8 * as, 2 * K::ASLOT);
-          const uint32_t sa = abase + as * K::ASLOT;
-          tma_load_2d_pair(sa, &tmA_hi, lafull0 + 8 * as, kc * BK, row0 - HALO);
-          tma_load_2d_pair(sa + A3_TILE, &tmA_lo, lafull0 + 8 * as, kc * BK, row0 - HALO);
-          if (++as == AS) { as = 0; aph ^= 1; }
-          for (int tap = 0; tap < 3; ++tap) {
-            mbar_wait(bempty0 + 8 * bs, bph ^ 1);
-            if (rank == 0) mbar_expect_tx(bfull0 + 8 * bs, 2 * K::BSLOT);
-            const uint32_t sb = bbase + bs * K::BSLOT;
-            const int brow = tap * p.N + nt * BN + (int)rank * HB;
-            tma_load_2d_pair(sb, &tmB_hi, lbfull0 + 8 * bs, kc * BK, brow);
-            tma_load_2d_pair(sb + K::B_TILE, &tmB_lo, lbfull0 + 8 * bs, kc * BK, brow);
-            if (++bs == BS) { bs = 0; bph ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      int as = 0, bs = 0, it = 0;
-      uint32_t aph = 0, bph = 0;
-      for (int tile = cid; tile < total; tile += ncl, ++it) {
-        const int a = it & 1;
-        mbar_wait(tempty0 + 8 * a, ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)a * K::ACC_STRIDE;
-        for (int kc = 0; kc < nkc; ++kc) {
-          mbar_wait(afull0 + 8 * as, aph);
-          tc_fence_after();
-          const uint32_t sa = abase + as * K::ASLOT;
-          for (int tap = 0; tap < 3; ++tap) {
-            mbar_wait(bfull0 + 8 * bs, bph);
-            tc_fence_after();
-            const uint32_t sh = (uint32_t)(HALO + (tap - 1) * p.dil) * 128u;  // whole rows: the swizzle phase follows the address
-            const uint32_t sb = bbase + bs * K::BSLOT;
-            const uint64_t dah = make_sdesc(sa + sh), dal = make_sdesc(sa + A3_TILE + sh);
-            const uint64_t dbh = make_sdesc(sb), dbl = make_sdesc(sb + K::B_TILE);
+      const int rbase = 16 * (warp & 1) + (lane >> 2);
 #pragma unroll
-            for (int ks = 0; ks < BK / 16; ++ks) {
-              const uint64_t off = (uint64_t)((ks * 32) >> 4);
-              tc_mma_pair(d_tmem, dah + off, dbh + off, idesc, (kc | tap | ks) != 0 ? 1u : 0u);
-              tc_mma_pair(d_tmem, dah + off, dbl + off, idesc, 1u);
-              tc_mma_pair(d_tmem, dal + off, dbh + off, idesc, 1u);
-            }
-            tc_commit_pair(bempty0 + 8 * bs);
-            if (++bs == BS) { bs = 0; bph ^= 1; }
-          }
-          tc_commit_pair(aempty0 + 8 * as);  // the halo tile is free once its third tap has been consumed
-          if (++as == AS) { as = 0; aph ^= 1; }
-        }
-        tc_commit_pair(tfull0 + 8 * a);
-      }
-    }
-  } else if (warp == 3) {
-    const uint32_t ltempty0 = mapa_u32(tempty0, 0);
-    auto pf = [&](int tile) {
-      int mp, nt;
-      pair_tile_decode(tile, cid, ncl, p.NT, mp, nt);
-      const int mt = 2 * mp + (int)rank;
-      if (mt < p.ntiles) prefetch_tile_l2<MODE>(p.e, p.tiles[mt], nt * BN, BN, lane, mt);
-    };
-    if (cid < total) pf(cid);
-    int it = 0;
-    for (int tile = cid; tile < total; tile += ncl, ++it) {
-      const int a = it & 1;
-      if (lane == 0) mbar_wait(tfull0 + 8 * a, (it >> 1) & 1);
-      __syncwarp();
-      if (tile + ncl < total) pf(tile + ncl);
-      if (lane == 0) mbar_arrive_cluster_relaxed(ltempty0 + 8 * a);
-    }
-  }
-  } else {  // warps 4-11: the epilogue warpgroups take the registers the others released
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
-    const int ew = warp & 3;
-    const int eg = (warp - 4) >> 2;
-    auto tile_at = [&](int it) {
-      EpiTile t;
-      const int tile = cid + it * ncl;
-      t.ok = tile < total;
-      t.prob = 0;
-      if (!t.ok) { t.r0 = 0; t.nrows = 0; t.n0 = 0; t.tq = 0; return t; }
-      int mp, nt;
-      pair_tile_decode(tile, cid, ncl, p.NT, mp, nt);
-      const int mt = 2 * mp + (int)rank;
-      const int2 tl = mt < p.ntiles ? p.tiles[mt] : make_int2(0, 0);
-      t.r0 = (int64_t)tl.x + ew * 32;
-      t.tq = (p.e.tile_base + mt) * 4 + ew;
-      t.nrows = min(32, max(0, tl.y - ew * 32));
-      t.n0 = nt * BN;
-      return t;
-    };
-    pair_epilogue_loop<BN / 64, MODE, MODE>(p.e, p.e, tile_at, xpose + (warp - 4) * 256, tmem_base + ((uint32_t)(ew * 32) << 16),
-                                            K::ACC_STRIDE, tfull0, mapa_u32(tempty0, 0), eg, lane, 0);
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(K::TMEM_COLS) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Interleaved two-problem CTA-pair kernel ("dual"): ONE launch works through the tiles of two independent GEMMs,
-//   problem 0 = a gate conv  (3 taps x C -> 2C, EPI_GATE:     tensor-pipe bound, ~15 us of MMAs per 256 x 256 tile),
-//   problem 1 = a 1x1 conv   (C -> 2C,         EPI_RES_SKIP:  bound by its epilogue's HBM streams, ~5 us of MMAs),
-// and every cluster ALTERNATES between them.  With the double-buffered TMEM accumulators the MMA warp runs one tile
-// ahead of the epilogue warps, so the long MMA phase of a gate tile hides the long epilogue of the 1x1 tile before it
-// and vice versa: the two kernels that ran back to back at 78 % / 22 % tensor-pipe activity (profiles/r01_ncu_full_pair_v2)
-// overlap inside every SM instead.  The two problems must be independent: the sampler drivers (stages.cu) pair the gate
-// conv of one half of the utterances (or of one F0 net) with the residual conv of the other half (other net).
-// Tile s of the interleaved sequence belongs to cluster s % ncl in its iteration s / ncl; while both problems have tiles
-// left, (s, s ^ 1) are the same tile index of the two problems and the problem alternates per cluster and iteration.
-struct TCProb {
-  const int2* tiles;
-  int ntiles, NT, taps, kchunks, dil, center, N;
-  EpiTC e;
-};
-struct TCDual {
-  TCProb q[2];
-  int n0, n1;  // tiles (row-tile pairs x NT) of problem 0 / 1
-};
-__device__ __forceinline__ bool dual_decode(int i, int cid, int ncl, int n0, int n1, int& p, int& t) {
-  const int s = i * ncl + cid;
-  if (s >= n0 + n1) return false;
-  const int m = n0 < n1 ? n0 : n1;
-  if (s < 2 * m) {
-    p = (ncl & 1) ? (s & 1) : ((i + cid) & 1);
-    t = s >> 1;
-  } else {
-    p = n0 > n1 ? 0 : 1;
-    t = m + (s - 2 * m);
-  }
-  return true;
-}
-#define DQ(field) (p ? P.q[1].field : P.q[0].field)
-
-template <int HB>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-conv_gemm_tc2d_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_constant__ CUtensorMap tmA0_lo,
-                      const __grid_constant__ CUtensorMap tmB0_hi, const __grid_constant__ CUtensorMap tmB0_lo,
-                      const __grid_constant__ CUtensorMap tmA1_hi, const __grid_constant__ CUtensorMap tmA1_lo,
-                      const __grid_constant__ CUtensorMap tmB1_hi, const __grid_constant__ CUtensorMap tmB1_lo,
-                      const __grid_constant__ TCDual P) {
-  using K = Cfg2<HB>;
-  constexpr int STAGES = K::STAGES;
-  constexpr int BN = K::BN;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float4* xpose = reinterpret_cast<float4*>(smem + STAGES * K::STAGE);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * K::STAGE + XPOSE_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * STAGES, tfull0 = empty0 + 8 * STAGES, tempty0 = tfull0 + 16;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();
-  const int cid = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-  const int n0 = P.n0, n1 = P.n1;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 2 * EPI_WARPS + 2);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(K::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-
-  if (warp < 4) {  // warpgroup 0 (producer, MMA issuer, TMEM allocator, L2 prefetch) needs few registers
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t lfull0 = mapa_u32(full0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int p, t;
-      for (int i = 0; dual_decode(i, cid, ncl, n0, n1, p, t); ++i) {
-        const int NT = DQ(NT), ntl = DQ(ntiles), kch = DQ(kchunks), taps = DQ(taps), dil = DQ(dil), center = DQ(center), N = DQ(N);
-        const int2* tiles = DQ(tiles);
-        const CUtensorMap* mAh = p ? &tmA1_hi : &tmA0_hi;
-        const CUtensorMap* mAl = p ? &tmA1_lo : &tmA0_lo;
-        const CUtensorMap* mBh = p ? &tmB1_hi : &tmB0_hi;
-        const CUtensorMap* mBl = p ? &tmB1_lo : &tmB0_lo;
-        const int mp = t / NT, nt = t - mp * NT;
-        int mt = 2 * mp + (int)rank;
-        if (mt >= ntl) mt = 2 * mp;
-        const int row0 = tiles[mt].x;
-        const int nk = taps * kch;
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(empty0 + 8 * stage, phase ^ 1);
-          if (rank == 0) mbar_expect_tx(full0 + 8 * stage, 2 * K::STAGE);
-          const uint32_t fb = lfull0 + 8 * stage;
-          const uint32_t sa = sbase + stage * K::STAGE;
-          const int tap = kb / kch;
-          const int c0 = (kb - tap * kch) * BK;
-          const int arow = row0 + (tap - center) * dil;
-          const int brow = tap * N + nt * BN + (int)rank * HB;
-          tma_load_2d_pair(sa, mAh, fb, c0, arow);
-          tma_load_2d_pair(sa + A_TILE, mAl, fb, c0, arow);
-          tma_load_2d_pair(sa + 2 * A_TILE, mBh, fb, c0, brow);
-          tma_load_2d_pair(sa + 2 * A_TILE + K::B_TILE, mBl, fb, c0, brow);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int p, t;
-      for (int it = 0; dual_decode(it, cid, ncl, n0, n1, p, t); ++it) {
-        const int a = it & 1;
-        const uint32_t aph = (it >> 1) & 1;
-        const int nk = DQ(taps) * DQ(kchunks);
-        mbar_wait(tempty0 + 8 * a, aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)a * K::ACC_STRIDE;
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(full0 + 8 * stage, phase);
-          tc_fence_after();
-          const uint32_t sa = sbase + stage * K::STAGE;
-          const uint64_t dah = make_sdesc(sa), dal = make_sdesc(sa + A_TILE);
-          const uint64_t dbh = make_sdesc(sa + 2 * A_TILE), dbl = make_sdesc(sa + 2 * A_TILE + K::B_TILE);
+      for (int cp = 0; cp < BN / 64; ++cp) {
 #pragma unroll
-          for (int ks = 0; ks < BK / 16; ++ks) {
-            const uint64_t off = (uint64_t)((ks * 32) >> 4);
-            tc_mma_pair(d_tmem, dah + off, dbh + off, idesc, (kb | ks) != 0 ? 1u : 0u);
-            tc_mma_pair(d_tmem, dah + off, dbl + off, idesc, 1u);
-            tc_mma_pair(d_tmem, dal + off, dbh + off, idesc, 1u);
-          }
-          tc_commit_pair(empty0 + 8 * stage);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit_pair(tfull0 + 8 * a);
-      }
-    }
-  } else if (warp == 3) {
-    const uint32_t ltempty0 = mapa_u32(tempty0, 0);
-    auto pf = [&](int i) {
-      int p, t;
-      if (!dual_decode(i, cid, ncl, n0, n1, p, t)) return;
-      const int NT = DQ(NT);
-      const int mp = t / NT, nt = t - mp * NT;
-      const int mt = 2 * mp + (int)rank;
-      if (mt >= DQ(ntiles)) return;
-      if (p == 0) prefetch_tile_l2<EPI_GATE>(P.q[0].e, P.q[0].tiles[mt], nt * BN, BN, lane, mt);
-      else prefetch_tile_l2<EPI_RES_SKIP>(P.q[1].e, P.q[1].tiles[mt], nt * BN, BN, lane, mt);
-    };
-    pf(0);
-    int p, t;
-    for (int it = 0; dual_decode(it, cid, ncl, n0, n1, p, t); ++it) {
-      const int a = it & 1;
-      if (lane == 0) mbar_wait(tfull0 + 8 * a, (it >> 1) & 1);
-      __syncwarp();
-      pf(it + 1);
-      if (lane == 0) mbar_arrive_cluster_relaxed(ltempty0 + 8 * a);
-    }
-  }
-  } else {  // warps 4-11: the epilogue warpgroups take the registers the others released
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
-    const int ew = warp & 3;
-    const int eg = (warp - 4) >> 2;
-    auto tile_at = [&](int it) {
-      EpiTile e;
-      int p, t;
-      e.ok = dual_decode(it, cid, ncl, n0, n1, p, t);
-      if (!e.ok) { e.r0 = 0; e.nrows = 0; e.n0 = 0; e.prob = 0; e.tq = 0; return e; }
-      e.prob = p;
-      const int NT = DQ(NT);
-      const int mp = t / NT, nt = t - mp * NT;
-      const int mt = 2 * mp + (int)rank;
-      const int2 tl = mt < DQ(ntiles) ? DQ(tiles)[mt] : make_int2(0, 0);
-      e.r0 = (int64_t)tl.x + ew * 32;
-      e.tq = (DQ(e.tile_base) + mt) * 4 + ew;
-      e.nrows = min(32, max(0, tl.y - ew * 32));
-      e.n0 = nt * BN;
-      return e;
-    };
-    pair_epilogue_loop<BN / 64, EPI_GATE, EPI_RES_SKIP>(P.q[0].e, P.q[1].e, tile_at, xpose + (warp - 4) * 256,
-                                                        tmem_base + ((uint32_t)(ew * 32) << 16), K::ACC_STRIDE, tfull0,
-                                                        mapa_u32(tempty0, 0), eg, lane, 0);
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(K::TMEM_COLS) : "memory");
-  }
-}
-
-// Dual kernel on the tap-reuse rings (Cfg3): the gate tiles load one halo-extended activation tile per K block and address
-// the three taps through row-shifted descriptors (-31 % operand bytes of the gate GEMM, which is bound by L2->SM operand
-// traffic: profiles/r02_probe_layer_v5.md); the 1x1 tiles use the same rings with a single tap (their 144-row box carries
-// 16 unused halo rows).
-template <int HB>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-conv_gemm_tc2dr_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_constant__ CUtensorMap tmA0_lo,
-                       const __grid_constant__ CUtensorMap tmB0_hi, const __grid_constant__ CUtensorMap tmB0_lo,
-                       const __grid_constant__ CUtensorMap tmA1_hi, const __grid_constant__ CUtensorMap tmA1_lo,
-                       const __grid_constant__ CUtensorMap tmB1_hi, const __grid_constant__ CUtensorMap tmB1_lo,
-                       const __grid_constant__ TCDual P) {
-  using K = Cfg3<HB>;
-  constexpr int BN = K::BN, AS = K::ASLOTS, BS = K::BSLOTS;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float4* xpose = reinterpret_cast<float4*>(smem + K::RING);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + K::RING + XPOSE_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * AS + 2 * BS + 4);
-  const uint32_t abase = smem_u32(smem), bbase = abase + AS * K::ASLOT;
-  const uint32_t afull0 = smem_u32(bars), aempty0 = afull0 + 8 * AS, bfull0 = aempty0 + 8 * AS, bempty0 = bfull0 + 8 * BS;
-  const uint32_t tfull0 = bempty0 + 8 * BS, tempty0 = tfull0 + 16;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();
-  const int cid = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-  const int n0 = P.n0, n1 = P.n1;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < 2 * AS + 2 * BS; ++s) mbar_init(afull0 + 8 * s, 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 2 * EPI_WARPS + 2);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(K::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-
-  if (warp < 4) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t lafull0 = mapa_u32(afull0, 0), lbfull0 = mapa_u32(bfull0, 0);
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0;
-      int p, t;
-      for (int i = 0; dual_decode(i, cid, ncl, n0, n1, p, t); ++i) {
-        const int NT = DQ(NT), ntl = DQ(ntiles), kch = DQ(kchunks), taps = DQ(taps), N = DQ(N);
-        const int2* tiles = DQ(tiles);
-        const CUtensorMap* mAh = p ? &tmA1_hi : &tmA0_hi;
-        const CUtensorMap* mAl = p ? &tmA1_lo : &tmA0_lo;
-        const CUtensorMap* mBh = p ? &tmB1_hi : &tmB0_hi;
-        const CUtensorMap* mBl = p ? &tmB1_lo : &tmB0_lo;
-        const int mp = t / NT, nt = t - mp * NT;
-        int mt = 2 * mp + (int)rank;
-        if (mt >= ntl) mt = 2 * mp;
-        const int row0 = tiles[mt].x;
-        for (int kc = 0; kc < kch; ++kc) {
-          mbar_wait(aempty0 + 8 * as, aph ^ 1);
-          if (rank == 0) mbar_expect_tx(afull0 + 8 * as, 2 * K::ASLOT);
-          const uint32_t sa = abase + as * K::ASLOT;
-          tma_load_2d_pair(sa, mAh, lafull0 + 8 * as, kc * BK, row0 - HALO);
-          tma_load_2d_pair(sa + A3_TILE, mAl, lafull0 + 8 * as, kc * BK, row0 - HALO);
-          if (++as == AS) { as = 0; aph ^= 1; }
-          for (int tap = 0; tap < taps; ++tap) {
-            mbar_wait(bempty0 + 8 * bs, bph ^ 1);
-            if (rank == 0) mbar_expect_tx(bfull0 + 8 * bs, 2 * K::BSLOT);
-            const uint32_t sb = bbase + bs * K::BSLOT;
-            const int brow = tap * N + nt * BN + (int)rank * HB;
-            tma_load_2d_pair(sb, mBh, lbfull0 + 8 * bs, kc * BK, brow);
-            tma_load_2d_pair(sb + K::B_TILE, mBl, lbfull0 + 8 * bs, kc * BK, brow);
-            if (++bs == BS) { bs = 0; bph ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0;
-      int p, t;
-      for (int it = 0; dual_decode(it, cid, ncl, n0, n1, p, t); ++it) {
-        const int a = it & 1;
-        const int kch = DQ(kchunks), taps = DQ(taps), dil = DQ(dil), center = DQ(center);
-        mbar_wait(tempty0 + 8 * a, ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)a * K::ACC_STRIDE;
-        for (int kc = 0; kc < kch; ++kc) {
-          mbar_wait(afull0 + 8 * as, aph);
-          tc_fence_after();
-          const uint32_t sa = abase + as * K::ASLOT;
-          for (int tap = 0; tap < taps; ++tap) {
-            mbar_wait(bfull0 + 8 * bs, bph);
-            tc_fence_after();
-            const uint32_t sh = (uint32_t)(HALO + (tap - center) * dil) * 128u;
-            const uint32_t sb = bbase + bs * K::BSLOT;
-            const uint64_t dah = make_sdesc(sa + sh), dal = make_sdesc(sa + A3_TILE + sh);
-            const uint64_t dbh = make_sdesc(sb), dbl = make_sdesc(sb + K::B_TILE);
+        for (int nb = 0; nb < 8; ++nb) {
+          float* xb = xb_pair + (nb >> 2) * 1024;
+          const int cc = 8 * (nb & 3) + 2 * (lane & 3);  // column inside the 32-wide chunk
 #pragma unroll
-            for (int ks = 0; ks < BK / 16; ++ks) {
-              const uint64_t off = (uint64_t)((ks * 32) >> 4);
-              tc_mma_pair(d_tmem, dah + off, dbh + off, idesc, (kc | tap | ks) != 0 ? 1u : 0u);
-              tc_mma_pair(d_tmem, dah + off, dbl + off, idesc, 1u);
-              tc_mma_pair(d_tmem, dal + off, dbh + off, idesc, 1u);
-            }
-            tc_commit_pair(bempty0 + 8 * bs);
-            if (++bs == BS) { bs = 0; bph ^= 1; }
+          for (int h = 0; h < 2; ++h) {
+            const int rr = rbase + 8 * h;
+            const int j = 4 * (8 * cp + nb) + 2 * h;
+            *reinterpret_cast<float2*>(xb + (rr * 8 + ((cc >> 2) ^ (rr & 7))) * 4 + (cc & 3)) = make_float2(acc[j], acc[j + 1]);
           }
-          tc_commit_pair(aempty0 + 8 * as);
-          if (++as == AS) { as = 0; aph ^= 1; }
         }
-        tc_commit_pair(tfull0 + 8 * a);
+        named_sync(pair_bar, 64);
+        const int ch = 2 * cp + eg;
+        if (ch + 2 < NCH && nrows > 0) prefetch_chunk<MODE>(p.e, r0, nrows, n0 + (ch + 2) * 32, lane, nxt, tq);
+        if (nrows > 0 && !(p.dbg & 1))
+          epilogue_chunk<MODE>(p.e, reinterpret_cast<float4*>(xb_pair + eg * 1024), r0, nrows, n0 + ch * 32, lane, cur, tq);
+        cur = nxt;
+        named_sync(pair_bar, 64);  // both chunks consumed before the buffers are refilled
       }
     }
-  } else if (warp == 3) {
-    const uint32_t ltempty0 = mapa_u32(tempty0, 0);
-    auto pf = [&](int i) {
-      int p, t;
-      if (!dual_decode(i, cid, ncl, n0, n1, p, t)) return;
-      const int NT = DQ(NT);
-      const int mp = t / NT, nt = t - mp * NT;
-      const int mt = 2 * mp + (int)rank;
-      if (mt >= DQ(ntiles)) return;
-      if (p == 0) prefetch_tile_l2<EPI_GATE>(P.q[0].e, P.q[0].tiles[mt], nt * BN, BN, lane, mt);
-      else prefetch_tile_l2<EPI_RES_SKIP>(P.q[1].e, P.q[1].tiles[mt], nt * BN, BN, lane, mt);
-    };
-    pf(0);
-    int p, t;
-    for (int it = 0; dual_decode(it, cid, ncl, n0, n1, p, t); ++it) {
-      const int a = it & 1;
-      if (lane == 0) mbar_wait(tfull0 + 8 * a, (it >> 1) & 1);
-      __syncwarp();
-      pf(it + 1);
-      if (lane == 0) mbar_arrive_cluster_relaxed(ltempty0 + 8 * a);
-    }
   }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
-    const int ew = warp & 3;
-    const int eg = (warp - 4) >> 2;
-    auto tile_at = [&](int it) {
-      EpiTile e;
-      int p, t;
-      e.ok = dual_decode(it, cid, ncl, n0, n1, p, t);
-      if (!e.ok) { e.r0 = 0; e.nrows = 0; e.n0 = 0; e.prob = 0; e.tq = 0; return e; }
-      e.prob = p;
-      const int NT = DQ(NT);
-      const int mp = t / NT, nt = t - mp * NT;
-      const int mt = 2 * mp + (int)rank;
-      const int2 tl = mt < DQ(ntiles) ? DQ(tiles)[mt] : make_int2(0, 0);
-      e.r0 = (int64_t)tl.x + ew * 32;
-      e.tq = (DQ(e.tile_base) + mt) * 4 + ew;
-      e.nrows = min(32, max(0, tl.y - ew * 32));
-      e.n0 = nt * BN;
-      return e;
-    };
-    pair_epilogue_loop<BN / 64, EPI_GATE, EPI_RES_SKIP>(P.q[0].e, P.q[1].e, tile_at, xpose + (warp - 4) * 256,
-                                                        tmem_base + ((uint32_t)(ew * 32) << 16), K::ACC_STRIDE, tfull0,
-                                                        mapa_u32(tempty0, 0), eg, lane, 0);
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(K::TMEM_COLS) : "memory");
-  }
+  if (CL > 1) cluster_sync_all();  // neither CTA may exit while its peer still multicasts into it or arrives on its barriers
 }
-#undef DQ
 
 __global__ void k_split_planes(const float* x, int ld, int64_t rows, int C, float scale, __half* hi, __half* lo) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1475,7 +629,7 @@ int device_sms() {
   int n = sms[dev].load(std::memory_order_relaxed);
   if (n == 0) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
     sms[dev].store(n, std::memory_order_relaxed);
   }
   return n;
@@ -1513,59 +667,14 @@ bool stream_hints_enabled() {
   static const bool off = getenv("SSB_TC_NO_STREAM_HINTS") != nullptr;
   return !off;
 }
-bool l2_prefetch_enabled() {
-  static const bool off = getenv("SSB_TC_NO_L2_PREFETCH") != nullptr;
-  return !off;
-}
-
-template <int BN, int MODE>
-int launch_m(Ctx& ctx, const GemmTC& p, const TCParams& tp, int num_sms) {
-  using KCfg = Cfg<BN>;
-  static std::atomic<bool> configured[MAX_DEV];
-  if (configure_once(conv_gemm_tc_kernel<BN, MODE>, configured, KCfg::SMEM)) return -2;
-  static std::atomic<long long>* const counter = [] {
-    static char name[48];
-    snprintf(name, sizeof(name), "tc<%d,%s>", BN, mode_name(MODE));
-    return variant_counter(name);
-  }();
-  const ConvTC& w = *p.w;
-  const ConvTC& w2 = p.w2 ? *p.w2 : *p.w;
-  const int bi = BN == 128 ? 0 : (BN == 64 ? 1 : 2);
-  CUtensorMap ta_hi, ta_lo, ta2_hi, ta2_lo;
-  if (cached_act_map(&ta_hi, p.A_hi, (uint64_t)p.rows_total, (uint64_t)w.Cin, BM)) return -1;
-  if (cached_act_map(&ta_lo, p.A_lo, (uint64_t)p.rows_total, (uint64_t)w.Cin, BM)) return -1;
-  if (p.w2) {
-    if (cached_act_map(&ta2_hi, p.A2_hi, (uint64_t)p.rows_total, (uint64_t)w2.Cin, BM)) return -1;
-    if (cached_act_map(&ta2_lo, p.A2_lo, (uint64_t)p.rows_total, (uint64_t)w2.Cin, BM)) return -1;
-  } else {
-    ta2_hi = ta_hi;
-    ta2_lo = ta_lo;
-  }
-  const int total = tp.ntiles * tp.NT;
-  const int grid = total < num_sms ? total : num_sms;
-  conv_gemm_tc_kernel<BN, MODE><<<grid, NTHREADS, KCfg::SMEM, ctx.stream>>>(ta_hi, ta_lo, w.tm_hi[bi], w.tm_lo[bi], ta2_hi, ta2_lo,
-                                                                       w2.tm_hi[bi], w2.tm_lo[bi], tp);
-  SSB_CUDA(cudaGetLastError());
-  ++g_launches;
-  counter->fetch_add(1, std::memory_order_relaxed);
-  return 0;
-}
-template <int BN>
-int launch(Ctx& ctx, const GemmTC& p, const TCParams& tp, int num_sms) {
-  switch (tp.e.mode) {
-    case EPI_GATE: return launch_m<BN, EPI_GATE>(ctx, p, tp, num_sms);
-    case EPI_RES_SKIP: return launch_m<BN, EPI_RES_SKIP>(ctx, p, tp, num_sms);
-    default: return launch_m<BN, EPI_GENERIC>(ctx, p, tp, num_sms);
-  }
-}
-
-// Two CTA-pair (cluster, cta_group::2) kernels in flight from DIFFERENT streams hung the B200 in round 1 (DESIGN.md
-// section 4; tools/repro_two_stream_hang.py).  Until that is root-caused the safe behaviour is the default: a pair
-// kernel never overlaps a pair kernel of another stream - each launch on a new stream first waits (on the device,
-// cudaStreamWaitEvent) for the last pair kernel launched on any other stream.  Same-stream launches are already
-// ordered and pay nothing.  SSB_TC_PAIR_CONCURRENT=1 switches the guard off (reproducer / diagnosis only).
-// Process-wide and thread-safe: the event and the "last stream" are guarded by a mutex held across wait + launch +
-// record, so two host threads cannot interleave between the wait and the record.
+// index into ConvTC::tm_hi / tm_lo of the weight descriptor whose box has `rows` rows
+constexpr int map_index(int rows) { return rows == 128 ? 0 : (rows == 64 ? 1 : 2); }
+// Cluster (CTA-pair) kernels from DIFFERENT streams are ordered against each other on the device: two such kernels in
+// flight from two streams hung an earlier build of this library, and the cause was never isolated.  Each pair launch on a
+// new stream first waits (cudaStreamWaitEvent) for the last pair launch of any other stream; same-stream launches are
+// already ordered and pay nothing, and at the sizes where pair kernels are chosen each one fills the GPU on its own.
+// SSB_TC_PAIR_CONCURRENT=1 switches the ordering off.  Process-wide and thread-safe: the mutex is held across wait +
+// launch + record.
 std::mutex g_pair_mu;
 cudaEvent_t g_pair_evt[MAX_DEV];
 cudaStream_t g_pair_last_stream[MAX_DEV];
@@ -1587,21 +696,24 @@ void pair_guard_end(int dev, cudaStream_t st) {  // g_pair_mu held
   g_pair_last_stream[dev] = st;
 }
 
-template <int HB, int MODE>
-int launch_pair_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
-  using KCfg = Cfg2<HB>;
-  const ConvTC& w = *p.w;
-  const ConvTC& w2 = p.w2 ? *p.w2 : *p.w;
+template <int BN, int CL, int MODE, bool REUSE>
+int launch_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
+  using KCfg = Cfg<BN, REUSE>;
   static std::atomic<bool> configured[MAX_DEV];
-  if (configure_once(conv_gemm_tc2_kernel<HB, MODE>, configured, KCfg::SMEM)) return -2;
+  if (configure_once(conv_gemm_wg_kernel<BN, CL, MODE, REUSE>, configured, KCfg::SMEM)) return -2;
   static std::atomic<long long>* const counter = [] {
     static char name[48];
-    snprintf(name, sizeof(name), "tc2<%d,%s>", HB, mode_name(MODE));
+    if (CL > 1) snprintf(name, sizeof(name), "tc2%s<%d,%s>", REUSE ? "r" : "", BN / 2, mode_name(MODE));
+    else snprintf(name, sizeof(name), "tc%s<%d,%s>", REUSE ? "r" : "", BN, mode_name(MODE));
     return variant_counter(name);
   }();
+  const ConvTC& w = *p.w;
+  const ConvTC& w2 = p.w2 ? *p.w2 : *p.w;
+  const int bi = map_index(BN / CL);
+  const uint32_t a_rows = REUSE ? A3_ROWS : BM;  // REUSE: halo-extended activation boxes
   CUtensorMap ta_hi, ta_lo, ta2_hi, ta2_lo;
-  if (cached_act_map(&ta_hi, p.A_hi, (uint64_t)p.rows_total, (uint64_t)w.Cin, BM)) return -1;
-  if (cached_act_map(&ta_lo, p.A_lo, (uint64_t)p.rows_total, (uint64_t)w.Cin, BM)) return -1;
+  if (cached_act_map(&ta_hi, p.A_hi, (uint64_t)p.rows_total, (uint64_t)w.Cin, a_rows)) return -1;
+  if (cached_act_map(&ta_lo, p.A_lo, (uint64_t)p.rows_total, (uint64_t)w.Cin, a_rows)) return -1;
   if (p.w2) {
     if (cached_act_map(&ta2_hi, p.A2_hi, (uint64_t)p.rows_total, (uint64_t)w2.Cin, BM)) return -1;
     if (cached_act_map(&ta2_lo, p.A2_lo, (uint64_t)p.rows_total, (uint64_t)w2.Cin, BM)) return -1;
@@ -1609,20 +721,30 @@ int launch_pair_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
     ta2_hi = ta_hi;
     ta2_lo = ta_lo;
   }
-  tp.NT = w.N / (2 * HB);
-  const int total = ((tp.ntiles + 1) / 2) * tp.NT;
-  const int ncl = total < num_sms / 2 ? total : num_sms / 2;
+  tp.NT = w.N / BN;
+  const int total = (CL > 1 ? (tp.ntiles + 1) / 2 : tp.ntiles) * tp.NT;
+  const int slots = num_sms / CL;
+  const int ncl = total < slots ? total : slots;
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3((unsigned)(CL * ncl));
+  cfg.blockDim = dim3(NTHREADS);
+  cfg.dynamicSmemBytes = KCfg::SMEM;
+  cfg.stream = ctx.stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;  // CL == 2: the two CTAs of a pair share a cluster (multicast, mapa)
+  at[0].val.clusterDim.x = (unsigned)CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
   {
-    const bool guard = pair_guard_enabled();
+    const bool guard = CL > 1 && pair_guard_enabled();
     const int dev = guard ? current_device() : 0;
     std::unique_lock<std::mutex> lk(g_pair_mu, std::defer_lock);
     if (guard) {
       lk.lock();
       pair_guard_begin(dev, ctx.stream);
     }
-    conv_gemm_tc2_kernel<HB, MODE><<<2 * ncl, NTHREADS, KCfg::SMEM, ctx.stream>>>(ta_hi, ta_lo, w.tm2_hi, w.tm2_lo, ta2_hi, ta2_lo,
-                                                                             w2.tm2_hi, w2.tm2_lo, tp);
-    const cudaError_t le = cudaGetLastError();
+    const cudaError_t le = cudaLaunchKernelEx(&cfg, conv_gemm_wg_kernel<BN, CL, MODE, REUSE>, ta_hi, ta_lo, w.tm_hi[bi],
+                                              w.tm_lo[bi], ta2_hi, ta2_lo, w2.tm_hi[bi], w2.tm_lo[bi], tp);
     if (guard) pair_guard_end(dev, ctx.stream);
     SSB_CUDA(le);
   }
@@ -1630,55 +752,20 @@ int launch_pair_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
   counter->fetch_add(1, std::memory_order_relaxed);
   return 0;
 }
-template <int HB, int MODE>
-int launch_pair_reuse_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
-  using KCfg = Cfg3<HB>;
-  const ConvTC& w = *p.w;
-  static std::atomic<bool> configured[MAX_DEV];
-  if (configure_once(conv_gemm_tc2r_kernel<HB, MODE>, configured, KCfg::SMEM)) return -2;
-  static std::atomic<long long>* const counter = [] {
-    static char name[48];
-    snprintf(name, sizeof(name), "tc2r<%d,%s>", HB, mode_name(MODE));
-    return variant_counter(name);
-  }();
-  CUtensorMap ta_hi, ta_lo;  // activation boxes of BM + 2 * HALO rows
-  if (cached_act_map(&ta_hi, p.A_hi, (uint64_t)p.rows_total, (uint64_t)w.Cin, A3_ROWS)) return -1;
-  if (cached_act_map(&ta_lo, p.A_lo, (uint64_t)p.rows_total, (uint64_t)w.Cin, A3_ROWS)) return -1;
-  tp.NT = w.N / (2 * HB);
-  const int total = ((tp.ntiles + 1) / 2) * tp.NT;
-  const int ncl = total < num_sms / 2 ? total : num_sms / 2;
-  {
-    const bool guard = pair_guard_enabled();
-    const int dev = guard ? current_device() : 0;
-    std::unique_lock<std::mutex> lk(g_pair_mu, std::defer_lock);
-    if (guard) {
-      lk.lock();
-      pair_guard_begin(dev, ctx.stream);
-    }
-    conv_gemm_tc2r_kernel<HB, MODE><<<2 * ncl, NTHREADS, KCfg::SMEM, ctx.stream>>>(ta_hi, ta_lo, w.tm2_hi, w.tm2_lo, tp);
-    const cudaError_t le = cudaGetLastError();
-    if (guard) pair_guard_end(dev, ctx.stream);
-    SSB_CUDA(le);
+template <int BN, int CL>
+int launch(Ctx& ctx, const GemmTC& p, const TCParams& tp, int num_sms) {
+  switch (tp.e.mode) {
+    case EPI_GATE: return launch_m<BN, CL, EPI_GATE, false>(ctx, p, tp, num_sms);
+    case EPI_RES_SKIP: return launch_m<BN, CL, EPI_RES_SKIP, false>(ctx, p, tp, num_sms);
+    default: return launch_m<BN, CL, EPI_GENERIC, false>(ctx, p, tp, num_sms);
   }
-  ++g_launches;
-  counter->fetch_add(1, std::memory_order_relaxed);
-  return 0;
 }
-// the tap-reuse kernel serves 3-tap convs with wide N: the gate GEMMs of the two denoisers (hb 128 / 96), the vocoder's
-// transposed convs (3-tap, N = u * C) and its k = 3 ResBlock convs; everything else keeps the general kernel
+// the tap-reuse variant serves the CTA-pair sizes of 3-tap convs: the gate GEMMs of both denoisers (with the hoisted
+// conditioner, i.e. without a second operand), the vocoder's transposed convs (3-tap, N = u * C) and its k = 3 ResBlock convs
 bool tap_reuse_eligible(const GemmTC& p, const ConvTC& w) {
   static const bool off = getenv("SSB_TC_NO_TAP_REUSE") != nullptr;
   return !off && !p.w2 && w.taps == 3 && w.center == 1 && w.dil >= 1 && w.dil <= HALO &&
-         (p.e.mode == EPI_GATE || p.e.mode == EPI_GENERIC) && (w.hb == 128 || w.hb == 96);
-}
-
-template <int HB>
-int launch_pair(Ctx& ctx, const GemmTC& p, const TCParams& tp, int num_sms) {
-  switch (tp.e.mode) {
-    case EPI_GATE: return launch_pair_m<HB, EPI_GATE>(ctx, p, tp, num_sms);
-    case EPI_RES_SKIP: return launch_pair_m<HB, EPI_RES_SKIP>(ctx, p, tp, num_sms);
-    default: return launch_pair_m<HB, EPI_GENERIC>(ctx, p, tp, num_sms);
-  }
+         (p.e.mode == EPI_GATE || p.e.mode == EPI_GENERIC);
 }
 
 }  // namespace
@@ -1720,22 +807,10 @@ int make_weight_maps(ConvTC* w) {
   }
   if (make_map(&w->tm_hi[1], w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 64)) return -1;
   if (make_map(&w->tm_lo[1], w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 64)) return -1;
-  if (w->N % 256 == 0) {
-    if (make_map(&w->tm_hi[2], w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 256)) return -1;
-    if (make_map(&w->tm_lo[2], w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 256)) return -1;
-  }
-  // CTA-pair kernel: the widest half-tile hb in {128, 96, 64, 32} with N % (2*hb) == 0
-  w->hb = 0;
-  for (int hb : {128, 96, 64, 32}) {
-    if (w->N % (2 * hb) == 0) {
-      w->hb = hb;
-      break;
-    }
-  }
-  if (w->hb) {
-    if (make_map(&w->tm2_hi, w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, (uint32_t)w->hb)) return -1;
-    if (make_map(&w->tm2_lo, w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, (uint32_t)w->hb)) return -1;
-  }
+  if (make_map(&w->tm_hi[2], w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 32)) return -1;
+  if (make_map(&w->tm_lo[2], w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 32)) return -1;
+  // CTA-pair kernel: each CTA of the pair loads hb weight rows of a 2*hb-wide N tile
+  w->hb = w->N % 128 == 0 ? 64 : 32;
   w->ok = true;
   return 0;
 }
@@ -1759,137 +834,21 @@ int conv_gemm_tc(Ctx& ctx, const GemmTC& p) {
     tp.dbg = d ? atoi(d) : 0;
   }
   if (!tp.e.bias) tp.e.bias = w.bias;
-  tp.e.l2_prefetch = l2_prefetch_enabled() ? 1 : 0;
   tp.e.stream_hints = stream_hints_enabled() ? 1 : 0;
-  // large problems: CTA pairs (256 x 2*hb tiles) halve the operand bytes each SM pulls through L2
+  // large problems: CTA pairs (two row tiles x one 2*hb-wide N tile per cluster, the weight tile multicast to both) halve
+  // the weight bytes each SM pulls through L2
   const bool pair_off = getenv("SSB_TC_NO_PAIR") != nullptr;
-  if (!pair_off && w.hb > 0 && (!p.w2 || p.w2->hb == w.hb) &&
-      (int64_t)((p.ntiles + 1) / 2) * (w.N / (2 * w.hb)) >= (int64_t)num_sms) {
+  if (!pair_off && (!p.w2 || p.w2->hb == w.hb) && (int64_t)((p.ntiles + 1) / 2) * (w.N / (2 * w.hb)) >= (int64_t)num_sms) {
     if (tap_reuse_eligible(p, w)) {
-      if (p.e.mode == EPI_GATE)
-        return w.hb == 128 ? launch_pair_reuse_m<128, EPI_GATE>(ctx, p, tp, num_sms) : launch_pair_reuse_m<96, EPI_GATE>(ctx, p, tp, num_sms);
-      return w.hb == 128 ? launch_pair_reuse_m<128, EPI_GENERIC>(ctx, p, tp, num_sms) : launch_pair_reuse_m<96, EPI_GENERIC>(ctx, p, tp, num_sms);
+      if (p.e.mode == EPI_GATE) return w.hb == 64 ? launch_m<128, 2, EPI_GATE, true>(ctx, p, tp, num_sms) : launch_m<64, 2, EPI_GATE, true>(ctx, p, tp, num_sms);
+      return w.hb == 64 ? launch_m<128, 2, EPI_GENERIC, true>(ctx, p, tp, num_sms) : launch_m<64, 2, EPI_GENERIC, true>(ctx, p, tp, num_sms);
     }
-    switch (w.hb) {
-      case 128: return launch_pair<128>(ctx, p, tp, num_sms);
-      case 96: return launch_pair<96>(ctx, p, tp, num_sms);
-      case 64: return launch_pair<64>(ctx, p, tp, num_sms);
-      default: return launch_pair<32>(ctx, p, tp, num_sms);
-    }
+    return w.hb == 64 ? launch<128, 2>(ctx, p, tp, num_sms) : launch<64, 2>(ctx, p, tp, num_sms);
   }
   // small problems: 64-wide N tiles keep more SMs busy and shorten each tile's dependent chain
-  const bool small = (w.N % 128 != 0) || (int64_t)p.ntiles * (w.N / 128) < (int64_t)num_sms * 2;
-  if (small) {
-    tp.NT = w.N / 64;
-    return launch<64>(ctx, p, tp, num_sms);
-  }
-  // 256-wide tiles halve the A-operand bytes per FLOP (the kernel is bound by L2->SM operand traffic,
-  // profiles/r01_ncu_*) but leave room for only a 2-stage ring (2 x 96 KB) and use the whole TMEM.  Measured on the
-  // batch64 mel stage: 1587 ms vs 1441 ms with 128-wide tiles / 3 stages, so it is opt-in (SSB_TC_BN256=1) only.
-  static const bool wide_ok = getenv("SSB_TC_BN256") != nullptr;
-  if (wide_ok && w.N % 256 == 0 && (!p.w2 || p.w2->N % 256 == 0) && (int64_t)p.ntiles * (w.N / 256) >= (int64_t)num_sms * 2) {
-    tp.NT = w.N / 256;
-    return launch<256>(ctx, p, tp, num_sms);
-  }
-  tp.NT = w.N / 128;
-  return launch<128>(ctx, p, tp, num_sms);
-}
-
-namespace {
-template <int HB, bool REUSE>
-int launch_dual(Ctx& ctx, const GemmTC& g, const GemmTC& r, int num_sms) {
-  constexpr int SMEM_BYTES = REUSE ? Cfg3<HB>::SMEM : Cfg2<HB>::SMEM;
-  static std::atomic<bool> configured[MAX_DEV];
-  if (REUSE ? configure_once(conv_gemm_tc2dr_kernel<HB>, configured, SMEM_BYTES) : configure_once(conv_gemm_tc2d_kernel<HB>, configured, SMEM_BYTES))
-    return -2;
-  static std::atomic<long long>* const counter = [] {
-    static char name[48];
-    snprintf(name, sizeof(name), "tc2d<%d,GATE+RES_SKIP>", HB);  // same name with or without tap reuse (SSB_TC_NO_TAP_REUSE)
-    return variant_counter(name);
-  }();
-  const GemmTC* gs[2] = {&g, &r};
-  CUtensorMap ta[2][2];
-  TCDual P;
-  for (int i = 0; i < 2; ++i) {
-    const GemmTC& q = *gs[i];
-    const ConvTC& w = *q.w;
-    if (cached_act_map(&ta[i][0], q.A_hi, (uint64_t)q.rows_total, (uint64_t)w.Cin, REUSE ? A3_ROWS : BM)) return -1;
-    if (cached_act_map(&ta[i][1], q.A_lo, (uint64_t)q.rows_total, (uint64_t)w.Cin, REUSE ? A3_ROWS : BM)) return -1;
-    TCProb& t = P.q[i];
-    t.tiles = q.tiles; t.ntiles = q.ntiles; t.NT = w.N / (2 * HB); t.taps = w.taps; t.kchunks = w.Cin / BK;
-    t.dil = w.dil; t.center = w.center; t.N = w.N; t.e = q.e;
-    if (!t.e.bias) t.e.bias = w.bias;
-    t.e.l2_prefetch = l2_prefetch_enabled() ? 1 : 0;
-    t.e.stream_hints = stream_hints_enabled() ? 1 : 0;
-  }
-  P.n0 = ((g.ntiles + 1) / 2) * P.q[0].NT;
-  P.n1 = ((r.ntiles + 1) / 2) * P.q[1].NT;
-  const int total = P.n0 + P.n1;
-  const int ncl = total < num_sms / 2 ? total : num_sms / 2;
-  {
-    const bool guard = pair_guard_enabled();
-    const int dev = guard ? current_device() : 0;
-    std::unique_lock<std::mutex> lk(g_pair_mu, std::defer_lock);
-    if (guard) {
-      lk.lock();
-      pair_guard_begin(dev, ctx.stream);
-    }
-    if (REUSE)
-      conv_gemm_tc2dr_kernel<HB><<<2 * ncl, NTHREADS, SMEM_BYTES, ctx.stream>>>(ta[0][0], ta[0][1], g.w->tm2_hi, g.w->tm2_lo, ta[1][0], ta[1][1],
-                                                                            r.w->tm2_hi, r.w->tm2_lo, P);
-    else
-      conv_gemm_tc2d_kernel<HB><<<2 * ncl, NTHREADS, SMEM_BYTES, ctx.stream>>>(ta[0][0], ta[0][1], g.w->tm2_hi, g.w->tm2_lo, ta[1][0], ta[1][1],
-                                                                           r.w->tm2_hi, r.w->tm2_lo, P);
-    const cudaError_t le = cudaGetLastError();
-    if (guard) pair_guard_end(dev, ctx.stream);
-    SSB_CUDA(le);
-  }
-  ++g_launches;
-  counter->fetch_add(1, std::memory_order_relaxed);
-  return 0;
-}
-}  // namespace
-
-static std::atomic<int> g_dual_on{-1};  // -1: not decided yet (environment), 0 / 1: off / on
-bool dual_enabled() {
-  int v = g_dual_on.load(std::memory_order_relaxed);
-  if (v < 0) {
-    // Off by default: once the residual GEMM's tile assignment was balanced (pair_tile_decode) one launch per GEMM measured
-    // 3 % faster than the interleaved schedule on the same box (profiles/r02_stage_times_batch64_v13_*.json): the 8 epilogue
-    // warps are the shared resource of both tile kinds, so the overlap the schedule was built for does not materialise.
-    const char* e = getenv("SSB_TC_DUAL");
-    v = e && atoi(e) != 0 && !getenv("SSB_TC_NO_DUAL") ? 1 : 0;
-    g_dual_on.store(v, std::memory_order_relaxed);
-  }
-  return v != 0;
-}
-int set_dual_enabled(int on) {
-  g_dual_on.store(on ? 1 : 0, std::memory_order_relaxed);
-  return on ? 1 : 0;
-}
-
-// gate conv (EPI_GATE, no second K segment) of one independent sub-problem + 1x1 residual conv (EPI_RES_SKIP) of another,
-// interleaved tile by tile in one launch (conv_gemm_tc2d_kernel).  Falls back to two launches when the shapes do not qualify.
-int conv_gemm_tc_dual(Ctx& ctx, const GemmTC& g, const GemmTC& r) {
-  if (ctx.dry) return 0;
-  if (g.ntiles == 0) return conv_gemm_tc(ctx, r);
-  if (r.ntiles == 0) return conv_gemm_tc(ctx, g);
-  const ConvTC& wg = *g.w;
-  const ConvTC& wr = *r.w;
-  const int num_sms = device_sms();
-  const bool pair_off = getenv("SSB_TC_NO_PAIR") != nullptr;
-  const bool ok = dual_enabled() && !pair_off && wg.ok && wr.ok && !g.w2 && !r.w2 && g.e.mode == EPI_GATE && r.e.mode == EPI_RES_SKIP &&
-                  wg.hb == wr.hb && (wg.hb == 128 || wg.hb == 96) && wg.taps == 3 && wr.taps == 1 &&
-                  (r.e.res || (r.e.rh && r.e.rl)) &&
-                  (int64_t)((g.ntiles + 1) / 2) * (wg.N / (2 * wg.hb)) + (int64_t)((r.ntiles + 1) / 2) * (wr.N / (2 * wr.hb)) >= (int64_t)num_sms;
-  if (!ok) {
-    if (int rc = conv_gemm_tc(ctx, g)) return rc;
-    return conv_gemm_tc(ctx, r);
-  }
-  static const bool no_reuse = getenv("SSB_TC_NO_TAP_REUSE") != nullptr;
-  if (!no_reuse && wg.center == 1 && wg.dil >= 1 && wg.dil <= HALO && wr.center == 0)
-    return wg.hb == 128 ? launch_dual<128, true>(ctx, g, r, num_sms) : launch_dual<96, true>(ctx, g, r, num_sms);
-  return wg.hb == 128 ? launch_dual<128, false>(ctx, g, r, num_sms) : launch_dual<96, false>(ctx, g, r, num_sms);
+  const bool small = (w.N % 128 != 0) || (p.w2 && p.w2->N % 128 != 0) || (int64_t)p.ntiles * (w.N / 128) < (int64_t)num_sms * 2;
+  if (small) return launch<64, 1>(ctx, p, tp, num_sms);
+  return launch<128, 1>(ctx, p, tp, num_sms);
 }
 
 int split_planes(Ctx& ctx, const float* x, int ld, int64_t rows, int C, float scale, __half* hi, __half* lo) {

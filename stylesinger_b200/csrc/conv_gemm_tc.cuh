@@ -1,23 +1,23 @@
-// tcgen05 / TMA implicit-GEMM conv1d for the dense contractions of the denoisers (SURVEY.md §8 a13/a18).
+// wgmma / TMA implicit-GEMM conv1d for the dense contractions of the denoisers (SURVEY.md §8 a13/a18).
 //
 // Precision: every fp32 operand is carried as TWO fp16 planes (hi = fp16(x), lo = fp16(x - hi));
-// each K step issues three tcgen05.mma (hi*hi + hi*lo + lo*hi) into one fp32 TMEM accumulator, so the
+// each K step issues three wgmma (hi*hi + hi*lo + lo*hi) into one fp32 register accumulator, so the
 // contraction keeps ~22 mantissa bits (SURVEY.md §7: single-pass bf16/fp16/TF32 cannot meet the
 // mel L-inf < 1e-3 bar at T=100; a 3-pass split can).  Effective tensor peak = 1/3 of the fp16 peak.
 //
 // Layout: A = activation planes [rows, C] fp16 row-major (guard-banded rows, see common.cuh), loaded by
 // TMA as [128 rows x 64 ch] boxes with 128B swizzle at row offset (tap - center) * dilation;
 // B = weights [taps*N, Cin] fp16 (K-major), boxes [BN n x 64 ch] (single-CTA kernel) or [hb x 64] (CTA-pair kernel:
-// each CTA of a 2-CTA cluster stages half of a 2*hb-wide N tile and its own 128 rows of A; the leader issues
-// cta_group::2 MMAs with M = 256).  D = fp32 in TMEM, double buffered so the epilogue of tile i overlaps the MMAs
-// of tile i+1 (persistent CTAs).  The pair kernel is used when there are >= num_SMs pair tiles, the 64-wide
-// single-CTA kernel otherwise (conv_gemm_tc()).
+// each CTA of a 2-CTA cluster loads its own 128 rows of A and half of a 2*hb-wide weight tile, multicast to both CTAs).
+// CTAs are persistent over the tiles.  The pair kernel is used when there are >= num_SMs pair tiles, the 64-wide
+// single-CTA kernel for small problems, the 128-wide one otherwise (conv_gemm_tc()).
 // An optional SECOND operand pair (A2, W2: 1 tap, no shift) extends the K loop: the DiffNet layer
 // GEMM contracts [3 taps x C of y | 256 of cond] in one accumulator, so the conditioner projection
 // needs neither a hoisted [rows, L*2C] fp32 buffer nor an epilogue read.
-// Env switches (diagnostics): SSB_TC_NO_PAIR=1 disables the pair kernel, SSB_TC_PAIR_CONCURRENT=1 lifts the cross-stream
-// serialisation of pair kernels (conv_gemm_tc.cu), SSB_TC_BN256=1 enables 256-wide single-CTA
-// tiles, SSB_TC_DEBUG=<bits> switches parts of the kernel off for tools/gemm_probe.py (results are then garbage).
+// 3-tap convs at pair sizes take the tap-reuse variant: one halo-extended activation tile per K block serves all three taps.
+// Env switches (diagnostics): SSB_TC_NO_PAIR=1 disables the pair kernel, SSB_TC_NO_TAP_REUSE=1 the tap-reuse variant,
+// SSB_TC_PAIR_CONCURRENT=1 lifts the cross-stream ordering of pair kernels,
+// SSB_TC_DEBUG=<bits> switches parts of the kernel off for tools/gemm_probe.py (results are then garbage).
 #pragma once
 #include <cuda.h>
 
@@ -29,9 +29,8 @@ namespace ssb {
 struct ConvTC {            // packed weights for the tensor-core path
   __half* W_hi = nullptr;  // [taps][N][Cin]
   __half* W_lo = nullptr;
-  CUtensorMap tm_hi[3], tm_lo[3];  // [0]: box 128 rows (BN=128), [1]: box 64 rows (BN=64), [2]: box 256 rows (BN=256)
-  CUtensorMap tm2_hi, tm2_lo;       // CTA-pair kernel: box hb rows (each CTA of a pair stages half of a 2*hb-wide N tile)
-  int hb = 0;                       // 0: no pair packing
+  CUtensorMap tm_hi[3], tm_lo[3];  // weight boxes of [0]: 128 rows, [1]: 64 rows, [2]: 32 rows
+  int hb = 0;                       // CTA-pair kernel: weight rows each CTA of a pair loads (half of a 2*hb-wide N tile)
   int taps = 1, Cin = 0, N = 0, dil = 1, center = 0;
   const float* bias = nullptr;  // [N] (packed column order)
   bool ok = false;
@@ -76,7 +75,6 @@ struct EpiTC {
   int64_t out_bs = 0;            //   [rows, out_nb] matrix at out + j * out_bs (the hoisted conditioner: one matrix per layer)
   int stream_hints = 1;          // skip accumulator and conditioner addends are touched once per launch: ld/st.global.cs (evict-first)
                                  //   so that they do not push the y / z planes (re-read by the next launch) out of L2; SSB_TC_NO_STREAM_HINTS=1: off
-  int l2_prefetch = 1;           // warp 3 pulls the next tile's epilogue operands into L2 (SSB_TC_NO_L2_PREFETCH=1: off)
   __half* sh = nullptr;          // RES_SKIP (last layer): the finished skip sum also as fp16 planes [rows, C]
   __half* sl = nullptr;
 };
@@ -99,12 +97,7 @@ int make_weight_maps(ConvTC* w);
 // TMA descriptor of an activation plane [rows, cols] fp16 (box 128 rows x 64 cols, 128B swizzle)
 int make_act_map(CUtensorMap* m, const void* ptr, int64_t rows, int cols, int box_rows = 128);
 int conv_gemm_tc(Ctx& ctx, const GemmTC& p);
-// One launch for two INDEPENDENT problems, interleaved tile by tile: g = a 3-tap gate conv (EPI_GATE), r = a 1x1 residual conv
-// (EPI_RES_SKIP).  Falls back to two launches when the shapes do not qualify.  Opt-in: ssb_set_interleaved_layers(1) / SSB_TC_DUAL=1.
-int conv_gemm_tc_dual(Ctx& ctx, const GemmTC& g, const GemmTC& r);
-bool dual_enabled();
-int set_dual_enabled(int on);  // process-wide switch (default off; SSB_TC_DUAL=1 starts with it on)
-// diagnostics: launches of one kernel variant ("tc2<128,GATE>", "tc<64,GENERIC>", ...), the variants seen so far,
+// diagnostics: launches of one kernel variant ("tc2<64,GATE>", "tc<64,GENERIC>", ...), the variants seen so far,
 // and the activation-descriptor cache counters
 long long variant_launch_count(const char* name);
 int variant_names(char* buf, int cap);

@@ -52,7 +52,7 @@ struct TensorMap {
 struct FFTLayer {
   float *ln1_g, *ln1_b, *ln2_g, *ln2_b;
   Conv qkv, out, ffn1, ffn2;
-  ConvTC ffn1_tc, ffn2_tc;  // the FFN (92 % of the block's FLOPs) on the tcgen05 path, used for long sequences
+  ConvTC ffn1_tc, ffn2_tc;  // the FFN (92 % of the block's FLOPs) on the tensor-core path, used for long sequences
   ConvTC qkv_tc, out_tc;    // self-attention in/out projections on the same path
 };
 struct FFT {
@@ -78,7 +78,7 @@ struct Denoiser {
   Conv mlp0, mlp2;
   std::vector<DenoiserLayer> layers;
   Conv cond_all;                // 256 -> L*2C, gate-interleaved per layer
-  ConvTC cond_all_tc;           // the same stacked projection for the tcgen05 kernel (hoisted out of the T loop; no bias)
+  ConvTC cond_all_tc;           // the same stacked projection for the tensor-core kernel (hoisted out of the T loop; no bias)
   Conv skip_proj, out_proj;
   // schedule-dependent (set by ssb_model_set_schedule)
   int T = 0;
@@ -86,7 +86,7 @@ struct Denoiser {
   float* gtab = nullptr;        // [T][8]
   float* mtab = nullptr;        // [T][8] (ddiff only)
   std::vector<float> gtab_h;
-  // persistent-sampler extras (mel net): every GEMM of a diffusion step on the tcgen05 path
+  // persistent-sampler extras (mel net): every GEMM of a diffusion step on the tensor-core path
   ConvTC in_tc;    // input_projection, K padded 80 -> 128
   ConvTC skip_tc;  // skip_projection with the 1/sqrt(L) skip scale folded into the weights
   ConvTC out_tc;   // output_projection, N padded 80 -> 256 (4 N-tiles of 64: one cluster)
@@ -96,7 +96,7 @@ struct Denoiser {
 
 struct AlignLayer {
   Conv q, kv, out, lin1, lin2;
-  ConvTC q_tc, kv_tc, out_tc, lin1_tc, lin2_tc;  // tcgen05 packing of the same projections (long batches)
+  ConvTC q_tc, kv_tc, out_tc, lin1_tc, lin2_tc;  // tensor-core packing of the same projections (long batches)
   float *n1_g, *n1_b, *n2_g, *n2_b;
 };
 
@@ -129,11 +129,11 @@ struct Model {
   cudaStream_t aux_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   bool persistent = true;  // single-launch persistent sampler for small batches (ssb_model_set_persistent)
-  bool cond_hoist = true;   // tcgen05 per-launch path: conditioner projection computed once per call ([rows, L*2C] fp32) and
+  bool cond_hoist = true;   // tensor-core per-launch path: conditioner projection computed once per call ([rows, L*2C] fp32) and
                             // added in the GATE epilogue, instead of being contracted inside every layer GEMM of every step
   bool persistent_groups = false;  // large batches: groups of <= 48 row tiles, one persistent launch each (mel sampler)
-  bool use_tc = true;  // tcgen05 path for the denoiser layer GEMMs (ssb_model_set_tensor_cores)
-  bool fft_tc = true;  // tcgen05 path for the decoder FFT blocks' FFN on long batches (ssb_model_set_fft_tensor_cores)
+  bool use_tc = true;  // tensor-core path for the denoiser layer GEMMs (ssb_model_set_tensor_cores)
+  bool fft_tc = true;  // tensor-core path for the decoder FFT blocks' FFN on long batches (ssb_model_set_fft_tensor_cores)
 };
 
 struct VocStage {

@@ -470,7 +470,7 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m) {
     PK(pack_linear(pool, tm.get(q + "multihead_attn.out_proj.weight"), tm.get(q + "multihead_attn.out_proj.bias"), &a.out));
     PK(pack_linear(pool, tm.get(q + "linear1.weight"), tm.get(q + "linear1.bias"), &a.lin1));
     PK(pack_linear(pool, tm.get(q + "linear2.weight"), tm.get(q + "linear2.bias"), &a.lin2));
-    {  // the same five projections for the tcgen05 kernel (biases: the packed fp32 vectors above)
+    {  // the same five projections for the tensor-core kernel (biases: the packed fp32 vectors above)
       auto lin_tc = [&](const float* data, int64_t n, int64_t k, const float* bias, ConvTC* out) {
         HostTensor ht;
         ht.data = data;

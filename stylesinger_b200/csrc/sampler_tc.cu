@@ -4,13 +4,13 @@
 // diffusion loop fused into a persistent kernel that keeps the mel state resident and launches once per
 // utterance"; configs[4] compares it with the per-step-launch path (ssb_model_set_persistent).
 //
-// Structure: the body of conv_gemm_tc_kernel<64> (TMA -> 4-stage smem ring -> tcgen05.mma 3-pass fp16 split ->
-// double-buffered TMEM -> epilogue warps) wrapped in a loop over a PHASE TABLE in device memory:
+// Structure: a 64-wide conv GEMM (TMA -> 4-stage smem ring -> 3-pass fp16 split wgmma into register accumulators ->
+// shared-memory staging -> per-row fused epilogue) wrapped in a loop over a PHASE TABLE in device memory:
 //   per step t:  in_proj | 20 x (dilated conv + conditioner -> gate ; 1x1 -> residual/skip) | skip_proj |
 //                out_proj + DDPM posterior update (q_posterior + noise) writing x_{t-1} and its fp16 planes
 // = 43 GEMM phases per step, separated by a grid-wide barrier (every phase reads what all CTAs wrote in
 // the previous one through +-dilation halos).  Tensor maps (activations + every layer's weights) live in a
-// device array; mbarrier phases, the smem ring and the TMEM allocation persist across all 43*T phases.
+// device array; mbarrier phases and the smem ring persist across all 43*T phases.
 #include <cuda_fp16.h>
 #include <string.h>
 
@@ -31,27 +31,14 @@ constexpr int A_TILE = BM * BK * 2;     // 16 KB
 constexpr int B_TILE = BN * BK * 2;     // 8 KB
 constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;  // 48 KB
 constexpr int STAGES = 4;
-constexpr int SMEM = STAGES * STAGE + 1024 + 512 + 1024;
-constexpr uint32_t TMEM_COLS = 2 * BN;
+constexpr int ACC_BYTES = BM * BN * 4;     // accumulator staging [128 rows x 64] fp32, float4 chunks XOR-swizzled by row
+constexpr int SMEM = STAGES * STAGE + ACC_BYTES + 1024 + 512 + 1024;
+static_assert(SMEM <= 227 * 1024, "exceeds the 227 KB of shared memory a Hopper block can have");
 static_assert(sizeof(SPhase) <= 1024, "the phase descriptor is staged in a 1 KB shared-memory slot");
 
 __device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ uint32_t cluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
 __device__ __forceinline__ uint32_t ncluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load whose box is written into the same smem offset of every CTA in `mask` (and signals each one's mbarrier)
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
 
 __device__ __forceinline__ void grid_barrier(unsigned* ctr, unsigned& gen, unsigned nblocks) {
   __threadfence();
@@ -267,36 +254,27 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
   // cs = cluster size along N: the cs CTAs of a cluster work on the same M-tile (consecutive N-tiles); each loads
   // 1/cs of the A tile and TMA-multicasts it to all of them, so the activation planes cross L2->SM once per
   // cluster instead of once per CTA.  Stage recycling therefore needs every CTA of the cluster to have consumed
-  // the stage: the MMA commit is multicast to all cs empty barriers (count cs).
+  // the stage: each consumer warp arrives on the empty barrier of all cs CTAs (count 4 cs).
+  // warp 0: TMA producer; warps 4-7: one consumer warpgroup (wgmma for rows 0-63 and 64-127, then the epilogue, thread =
+  // row); warps 1-3 only take part in the phase-descriptor staging and the barriers.
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  SPhase* sph = reinterpret_cast<SPhase*>(smem + STAGES * STAGE + 512);
+  float4* accs = reinterpret_cast<float4*>(smem + STAGES * STAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE + ACC_BYTES);
+  SPhase* sph = reinterpret_cast<SPhase*>(smem + STAGES * STAGE + ACC_BYTES + 512);
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * STAGES, tfull0 = empty0 + 8 * STAGES, tempty0 = tfull0 + 16;
+  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, (uint32_t)cs);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 4);
+      mbar_init(empty0 + 8 * s, (uint32_t)(4 * cs));
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-  const int cr = cs > 1 ? (int)cluster_ctarank() : 0;
+  const int cr = cs > 1 ? (int)cluster_rank() : 0;
   const int cid = cs > 1 ? (int)cluster_id_x() : (int)blockIdx.x;
   const int ncl = cs > 1 ? (int)ncluster_id_x() : (int)gridDim.x;
   const uint16_t cmask = (uint16_t)((1u << cs) - 1u);
@@ -307,9 +285,7 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
   // pipeline state, persistent across phases (each role keeps its own copy)
   int stage = 0;
   uint32_t phase_bit = 0;
-  int it = 0;
   unsigned gen = 0;
-  const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
 
   for (int ph = 0; ph < nphases; ++ph) {
     // stage the phase descriptor in shared memory
@@ -371,39 +347,21 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
           }
         }
       }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        for (int g = g_first; g < groups; g += ncl, ++it) {
-          const int a = it & 1;
-          const uint32_t aph = (it >> 1) & 1;
-          mbar_wait(tempty0 + 8 * a, aph ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)(a * BN);
-          for (int kb = 0; kb < nk; ++kb) {
-            mbar_wait(full0 + 8 * stage, phase_bit);
-            tc_fence_after();
-            const uint32_t sa = sbase + stage * STAGE;
-            const uint64_t dah = make_sdesc(sa), dal = make_sdesc(sa + A_TILE);
-            const uint64_t dbh = make_sdesc(sa + 2 * A_TILE), dbl = make_sdesc(sa + 2 * A_TILE + B_TILE);
-#pragma unroll
-            for (int ks = 0; ks < BK / 16; ++ks) {
-              const uint64_t off = (uint64_t)((ks * 32) >> 4);
-              tc_mma(d_tmem, dah + off, dbh + off, idesc, (kb | ks) != 0 ? 1u : 0u);
-              tc_mma(d_tmem, dah + off, dbl + off, idesc, 1u);
-              tc_mma(d_tmem, dal + off, dbh + off, idesc, 1u);
-            }
-            if (cs > 1) tc_commit_mc(empty0 + 8 * stage, cmask);
-            else tc_commit(empty0 + 8 * stage);
-            if (++stage == STAGES) { stage = 0; phase_bit ^= 1; }
-          }
-          tc_commit(tfull0 + 8 * a);
-        }
-      }
+      __syncwarp();
     } else if (warp >= 4) {
       const int ew = warp - 4;
-      for (int g = g_first; g < groups; g += ncl, ++it) {
-        const int a = it & 1;
-        const uint32_t aph = (it >> 1) & 1;
+      auto release = [&](int st) {  // this warp is done reading stage st: tell every CTA that multicasts into it
+        __syncwarp();
+        if (lane == 0) {
+          const uint32_t bar = empty0 + 8 * st;
+          if (cs > 1) {
+            for (int r = 0; r < cs; ++r) mbar_arrive_cluster(mapa_u32(bar, (uint32_t)r));
+          } else {
+            mbar_arrive(bar);
+          }
+        }
+      };
+      for (int g = g_first; g < groups; g += ncl) {
         const int mt = g / gpm, nt = (g - mt * gpm) * cs + cr;
         const int2 t = tiles[mt];
         const int rl = ew * 32 + lane;
@@ -412,33 +370,75 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
         const int64_t ti = (int64_t)tile_tight[mt] + rl;
         Pre cur, nxt;
         prefetch32(P, r, nt * BN, valid, cur);
-        mbar_wait(tfull0 + 8 * a, aph);
-        tc_fence_after();
+        float acc0[BN / 2], acc1[BN / 2];  // rows [0, 64) and [64, 128) of the tile
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < nk; ++kb) {
+          mbar_wait(full0 + 8 * stage, phase_bit);
+          const uint32_t sa = sbase + stage * STAGE;
+          const uint64_t dah = make_sdesc(sa), dal = make_sdesc(sa + A_TILE);
+          const uint64_t dbh = make_sdesc(sa + 2 * A_TILE), dbl = make_sdesc(sa + 2 * A_TILE + B_TILE);
+          wg_fence();
+          fence_acc(acc0);
+          fence_acc(acc1);
+#pragma unroll
+          for (int ks = 0; ks < BK / 16; ++ks) {
+            const uint64_t off = (uint64_t)((ks * 32) >> 4);
+            wgmma_n64(acc0, dah + off, dbh + off, 1u);
+            wgmma_n64(acc0, dah + off, dbl + off, 1u);
+            wgmma_n64(acc0, dal + off, dbh + off, 1u);
+            wgmma_n64(acc1, dah + 512 + off, dbh + off, 1u);  // +8192 bytes: rows 64-127
+            wgmma_n64(acc1, dah + 512 + off, dbl + off, 1u);
+            wgmma_n64(acc1, dal + 512 + off, dbh + off, 1u);
+          }
+          wg_commit();
+          fence_acc(acc0);
+          fence_acc(acc1);
+          wg_wait<1>();
+          fence_acc(acc0);
+          fence_acc(acc1);
+          if (prev >= 0) release(prev);
+          prev = stage;
+          if (++stage == STAGES) { stage = 0; phase_bit ^= 1; }
+        }
+        wg_wait<0>();
+        fence_acc(acc0);
+        fence_acc(acc1);
+        if (prev >= 0) release(prev);
+        // fragments -> [128 x 64] staging (row rr, float4 chunk c at rr * 16 + (c ^ (rr & 15))) -> one row per thread
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+          const int rr = frag_row(ew, lane, j), cc = frag_col(lane, j);
+          float* b0 = reinterpret_cast<float*>(accs + rr * 16 + ((cc >> 2) ^ (rr & 15))) + (cc & 3);
+          float* b1 = reinterpret_cast<float*>(accs + (rr + 64) * 16 + ((cc >> 2) ^ ((rr + 64) & 15))) + (cc & 3);
+          *reinterpret_cast<float2*>(b0) = make_float2(acc0[j], acc0[j + 1]);
+          *reinterpret_cast<float2*>(b1) = make_float2(acc1[j], acc1[j + 1]);
+        }
+        named_sync(1, 128);
 #pragma unroll 1
         for (int ch = 0; ch < BN / 32; ++ch) {
           if (ch + 1 < BN / 32) prefetch32(P, r, nt * BN + (ch + 1) * 32, valid, nxt);
           uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(a * BN + ch * 32), v);
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            const float4 x = accs[rl * 16 + ((ch * 8 + c) ^ (rl & 15))];
+            v[4 * c] = __float_as_uint(x.x); v[4 * c + 1] = __float_as_uint(x.y);
+            v[4 * c + 2] = __float_as_uint(x.z); v[4 * c + 3] = __float_as_uint(x.w);
+          }
           if (valid) epilogue32(P, r, ti, nt * BN + ch * 32, v, cur);
           cur = nxt;
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty0 + 8 * a);
+        named_sync(1, 128);  // staging buffer read by every thread before the next tile overwrites it
       }
     }
-    // the producer / MMA roles keep separate copies of (stage, phase_bit) and the MMA / epilogue roles of `it`:
-    // every role advances them by exactly the same amounts per phase, so no exchange is needed.
+    // the producer and the consumers keep separate copies of (stage, phase_bit): both advance them by exactly the same
+    // amounts per phase, so no exchange is needed.
     if (P.sync_after) grid_barrier(barrier_ctr, gen, gridDim.x);
     else __syncthreads();  // the next entry is independent of this one: only the descriptor slot is recycled
   }
-  tc_fence_before();
   __syncthreads();
   if (cs > 1) cluster_sync_all();  // nobody exits while a peer may still multicast into / arrive on its smem
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
 }
 
 // x [rows, 80] fp32 -> planes [rows, 128] (columns 80..127 zero), all rows

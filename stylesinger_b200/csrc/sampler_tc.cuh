@@ -1,4 +1,4 @@
-// Persistent tcgen05 sampler kernel: phase table + launch (see sampler_tc.cu).
+// Persistent wgmma sampler kernel: phase table + launch (see sampler_tc.cu).
 #pragma once
 #include <cuda.h>
 

@@ -78,7 +78,7 @@ int fft_blocks(Ctx& c, const FFT& f, const SeqDev& s, float* x, const float* kee
   float* att = alloc_rows(c, s, H);
   float* ff = tc ? nullptr : alloc_rows(c, s, 4 * H);
   __half *hh = nullptr, *hl = nullptr, *fh = nullptr, *fl = nullptr;  // fp16 hi/lo planes of h and of gelu(ffn_1)
-  // tcgen05 attention (attention_tc.cu): q/k/v only as fp16 hi/lo planes [rows, 768] + V^T planes [256, ldvt]
+  // wgmma attention (attention_tc.cu): q/k/v only as fp16 hi/lo planes [rows, 768] + V^T planes [256, ldvt]
   const bool atc = tc && attention_tc_enabled();
   const int64_t ldvt = (s.rows + 7) & ~int64_t(7);
   __half *qh = nullptr, *ql = nullptr, *vth = nullptr, *vtl = nullptr;
@@ -137,7 +137,7 @@ int fft_blocks(Ctx& c, const FFT& f, const SeqDev& s, float* x, const float* kee
       RUN(conv_gemm(c, g));
     }
     RUN(layernorm_rows(c, s, x, H, h, H, H, L.ln2_g, L.ln2_b, 1e-5f, nullptr));
-    if (tc) {  // TransformerFFNLayer (transformer.py): ffn_2(gelu(ffn_1(x) * k^-0.5)) on the tcgen05 kernel
+    if (tc) {  // TransformerFFNLayer (transformer.py): ffn_2(gelu(ffn_1(x) * k^-0.5)) on the tensor-core kernel
       RUN(split_planes(c, h, H, s.rows, H, 1.0f, hh, hl));
       GemmTC g1;
       g1.A_hi = hh; g1.A_lo = hl; g1.rows_total = s.rows; g1.w = &L.ffn1_tc; g1.tiles = s.tiles; g1.ntiles = s.ntiles;
@@ -268,7 +268,7 @@ int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const 
   float* q = alloc_rows(c, sf, H);
   float* att = alloc_rows(c, sf, H);
   float* tmp = alloc_rows(c, sf, H);
-  // long batches: the aligner's five projections per layer on the tcgen05 kernel (the 256 -> 2048 -> 256 feed-forward is
+  // long batches: the aligner's five projections per layer on the tensor-core kernel (the 256 -> 2048 -> 256 feed-forward is
   // 90 % of its FLOPs; its hidden activation then only exists as fp16 hi/lo planes); attention itself stays fp32
   bool tc = m.use_tc && m.fft_tc && tc_available() && sf.ntiles >= 8;
   for (int i = 0; i < 2; ++i)
@@ -387,7 +387,7 @@ int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const 
         RUN(conv_gemm(c, g));
       }
     }
-    if (atc) {  // cross-attention on the tcgen05 kernel: q planes [F rows, 256], k | v planes [R rows, 512]
+    if (atc) {  // cross-attention on the tensor-core kernel: q planes [F rows, 256], k | v planes [R rows, 512]
       RUN(transpose_planes(c, akh, akl, 2 * H, H, sr.rows, H, avth, avtl, ldvt));
       AttnTCArgs a;
       a.utt_q = sf.utt; a.utt_k = sr.utt; a.B = sf.B; a.max_q = sf.maxlen; a.heads = 2;
@@ -444,8 +444,8 @@ int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const 
 // ------------------------------------------------------------------------------------------------
 // a13/a18: the denoiser residual stack for one diffusion step.
 // On entry b.x holds the residual stream and (b.y | b.yh,b.yl) holds x + d[t][0]; both are overwritten.
-// SIMT path: fp32 conv_gemm.  Tensor-core path (b.tc): tcgen05 GEMMs on fp16 hi/lo planes.
-// The two tcgen05 GEMMs of residual layer l over the row tiles [tiles, tiles + ntiles) (net.py:66-78)
+// SIMT path: fp32 conv_gemm.  Tensor-core path (b.tc): wgmma GEMMs on fp16 hi/lo planes.
+// The two tensor-core GEMMs of residual layer l over the row tiles [tiles, tiles + ntiles) (net.py:66-78)
 static GemmTC layer_gate_gemm(const Denoiser& d, const DenoiserBufs& b, int64_t rows, const int2* tiles, int ntiles, int l) {
   const int C = d.C;
   GemmTC g;
@@ -473,40 +473,6 @@ static GemmTC layer_res_gemm(const Denoiser& d, const DenoiserBufs& b, int64_t r
   g.e.skip_tiled = b.skip_tiled ? 1 : 0; g.e.tile_base = tile0;
   if (b.tc_heads && l == L - 1) { g.e.sh = b.skh; g.e.sl = b.skl; }
   return g;
-}
-
-// One independent sub-problem of a sampler step: a denoiser, its buffers and the row tiles it covers.
-struct Lane {
-  const Denoiser* d;
-  const DenoiserBufs* b;
-  int64_t rows;
-  const int2* tiles;
-  int ntiles;
-  int t;
-  int tile0;  // index of tiles[0] in the layout's tile table
-};
-// Residual layers of TWO independent lanes, software-pipelined by half a layer: every launch but the first and the last is
-// the interleaved dual kernel (conv_gemm_tc_dual) working on the gate conv of one lane and the 1x1 residual conv of the
-// other, so the MMA-bound and the HBM-bound half of a layer overlap inside every SM.  2L + 1 launches instead of 2 x 2L.
-static int denoiser_layers_dual(Ctx& c, const Lane& A, const Lane& B) {
-  const int L = A.d->L;
-  const float* dtA = A.d->dtab + (size_t)A.t * L * A.d->C;
-  const float* dtB = B.d->dtab + (size_t)B.t * L * B.d->C;
-  RUN(conv_gemm_tc(c, layer_gate_gemm(*A.d, *A.b, A.rows, A.tiles, A.ntiles, 0)));
-  for (int l = 0; l < L; ++l) {
-    RUN(conv_gemm_tc_dual(c, layer_gate_gemm(*B.d, *B.b, B.rows, B.tiles, B.ntiles, l),
-                          layer_res_gemm(*A.d, *A.b, A.rows, A.tiles, A.ntiles, l, dtA, A.tile0)));
-    if (l + 1 < L)
-      RUN(conv_gemm_tc_dual(c, layer_gate_gemm(*A.d, *A.b, A.rows, A.tiles, A.ntiles, l + 1),
-                            layer_res_gemm(*B.d, *B.b, B.rows, B.tiles, B.ntiles, l, dtB, B.tile0)));
-    else
-      RUN(conv_gemm_tc(c, layer_res_gemm(*B.d, *B.b, B.rows, B.tiles, B.ntiles, l, dtB, B.tile0)));
-  }
-  return 0;
-}
-static bool dual_lane_ok(const Denoiser& d, const DenoiserBufs& b) {
-  return b.tc && b.condpre != nullptr && dual_enabled() && d.layers[0].dil_tc.hb == d.layers[0].outp_tc.hb &&
-         (d.layers[0].dil_tc.hb == 128 || d.layers[0].dil_tc.hb == 96);
 }
 
 // skip_projection + output_projection of the denoiser (net.py:126-130 / :262-266)
@@ -543,17 +509,10 @@ static int denoiser_heads(Ctx& c, const Denoiser& d, const SeqDev& s, DenoiserBu
   return 0;
 }
 
-// `split` (0 = off): row tiles [0, split) and [split, ntiles) belong to two disjoint sets of utterances; the residual layers
-// then run as two software-pipelined lanes on the interleaved dual kernel (denoiser_layers_dual).
-int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBufs& b, int split) {
+int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBufs& b) {
   const int C = d.C, L = d.L;
   SSB_CHECK(d.dtab != nullptr && t >= 0 && t < d.T, "denoiser: schedule not set (ssb_model_set_schedule) or bad t");
   const float* dt = d.dtab + (size_t)t * L * C;
-  if (split > 0 && split < s.ntiles && dual_lane_ok(d, b) && !c.dry) {
-    const Lane A{&d, &b, s.rows, s.tiles, split, t, 0}, B{&d, &b, s.rows, s.tiles + split, s.ntiles - split, t, split};
-    RUN(denoiser_layers_dual(c, A, B));
-    return denoiser_heads(c, d, s, b);
-  }
   for (int l = 0; l < L; ++l) {
     if (b.tc) {
       RUN(conv_gemm_tc(c, layer_gate_gemm(d, b, s.rows, s.tiles, s.ntiles, l)));
@@ -655,19 +614,7 @@ int prepare_cond(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g
 }
 
 // a18 entry for one evaluation (mel): x80 [rows,80] guarded -> head
-int lane_split_tile(const Seq* q) {
-  if (!q || q->B < 2) return 0;
-  const int total = q->ntiles(1);
-  int acc = 0, best = 0;
-  for (int b = 0; b + 1 < q->B; ++b) {
-    acc += (q->len[b] + TILE_M - 1) / TILE_M;
-    if (best == 0 || abs(2 * acc - total) < abs(2 * best - total)) best = acc;
-  }
-  // a lopsided split leaves most tiles without a partner of the other kind: not worth the extra launch
-  return (best * 4 >= total && best * 4 <= 3 * total) ? best : 0;
-}
-
-int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const float* x80, DenoiserBufs& b, int split) {
+int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const float* x80, DenoiserBufs& b) {
   if (b.x80h) {  // tensor-core input projection: K padded 80 -> 128
     RUN(x80_planes(c, x80, s.rows, b.x80h, b.x80l));
     GemmTC g;
@@ -675,7 +622,7 @@ int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const f
     g.e.mode = EPI_GENERIC; g.e.bias = d.in_proj.bias; g.e.act = ACT_RELU;  // planes of y = relu(in_proj) + step bias only
     g.e.oh = b.yh; g.e.ol = b.yl; g.e.ldh = d.C; g.e.vec2 = d.dtab + (size_t)t * d.L * d.C;
     RUN(conv_gemm_tc(c, g));
-    return denoiser_stack(c, d, s, t, b, split);
+    return denoiser_stack(c, d, s, t, b);
   }
   ConvGemm g = make_gemm(d.in_proj, s, x80, 80);
   g.e.act = ACT_RELU; g.e.out = b.x; g.e.ldo = d.C;
@@ -683,10 +630,10 @@ int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const f
   if (b.tc) { g.e.out2_h = b.yh; g.e.out2_l = b.yl; g.e.ldh = d.C; }
   else { g.e.out2 = b.y; g.e.ldo2 = d.C; }
   RUN(conv_gemm(c, g));
-  return denoiser_stack(c, d, s, t, b, split);
+  return denoiser_stack(c, d, s, t, b);
 }
 
-// a18+a19, single launch: all T reverse steps in the persistent tcgen05 kernel (sampler_tc.cu).
+// a18+a19, single launch: all T reverse steps in the persistent wgmma kernel (sampler_tc.cu).
 static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                                         const float* noise, uint64_t seed, float* mel_tight) {
   const Denoiser& d = m.melnet;
@@ -852,10 +799,8 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
   const size_t per = (size_t)s.total * 80;
   const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 6];
   RUN(mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, 1000));
-  // two utterance groups -> the residual layers run as two lanes on the interleaved dual kernel
-  const int split = s.ntiles >= 148 ? lane_split_tile(host_seq) : 0;
   for (int t = T - 1; t >= 0; --t) {
-    RUN(mel_denoiser_eval(c, d, s, t, xm, b, split));
+    RUN(mel_denoiser_eval(c, d, s, t, xm, b));
     const float* nz = noise ? noise + per * (size_t)(T - t) : nullptr;
     RUN(mel_p_sample(c, s, xm, 80, b.head, b.ld_head, nz, d.gtab + (size_t)t * 8, seed, 1001 + (uint64_t)t));
   }
@@ -1117,62 +1062,9 @@ int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const f
   return 0;
 }
 
-// a13+a14 for BOTH F0 nets of a large batch in lock step (the agnostic and the specific sampler are independent,
-// stylesinger.py:223-225): per reverse step the residual layers of the two nets run as the two lanes of the interleaved
-// dual kernel, everything else (DDiffNet input, heads, Gaussian + multinomial update) per net as in run_f0_diffusion.
-bool f0_dual_ok(const Model& m, const SeqDev& s) {
-  if (!m.use_tc || !m.cond_hoist || !dual_enabled() || s.ntiles < 74) return false;
-  for (int n = 0; n < 2; ++n) {
-    const Denoiser& d = m.f0net[n];
-    if (!denoiser_tc_ok(m, d) || !d.cond_all_tc.ok || d.T <= 0) return false;
-    const int hb = d.layers[0].dil_tc.hb;
-    if (hb != d.layers[0].outp_tc.hb || (hb != 128 && hb != 96)) return false;
-  }
-  return m.f0net[0].C == m.f0net[1].C && m.f0net[0].L == m.f0net[1].L && m.f0net[0].T == m.f0net[1].T &&
-         m.f0net[0].layers[0].dil_tc.hb == m.f0net[1].layers[0].dil_tc.hb;
-}
-int run_f0_diffusion_dual(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1, const float* lo,
-                          const float* hi, const float* const gnoise[2], const float* const unoise[2], uint64_t seed,
-                          float* const z[2], int32_t* const uv[2]) {
-  const size_t mk = c.mark();
-  DenoiserBufs b[2];
-  const int T = m.f0net[0].T;
-  const size_t per = (size_t)s.total;
-  for (int n = 0; n < 2; ++n) {
-    const Denoiser& d = m.f0net[n];
-    RUN(alloc_denoiser(c, d, s, true, &b[n], true));
-    RUN(prepare_cond(c, d, s, n == 0 ? cond0 : cond1, b[n]));
-    RUN(f0_init(c, s, z[n], uv[n], gnoise[n], seed, 2000 + (uint64_t)n * 100000));
-  }
-  SSB_CHECK(c.dry || (b[0].condpre && b[1].condpre), "f0 dual sampler needs the hoisted conditioner");
-  for (int t = T - 1; t >= 0; --t) {
-    for (int n = 0; n < 2; ++n) {
-      const Denoiser& d = m.f0net[n];
-      RUN(ddiff_input(c, s, z[n], uv[n], d.in_w, d.in_b, d.uv_emb, d.dtab + (size_t)t * d.L * d.C, nullptr, b[n].y, d.C, b[n].yh, b[n].yl));
-    }
-    if (!c.dry) {
-      const Lane A{&m.f0net[0], &b[0], s.rows, s.tiles, s.ntiles, t, 0}, B{&m.f0net[1], &b[1], s.rows, s.tiles, s.ntiles, t, 0};
-      RUN(denoiser_layers_dual(c, A, B));
-    }
-    for (int n = 0; n < 2; ++n) {
-      const Denoiser& d = m.f0net[n];
-      RUN(denoiser_heads(c, d, s, b[n]));
-      F0StepArgs a;
-      a.z = z[n]; a.uv = uv[n]; a.out3 = b[n].head; a.ld3 = b[n].ld_head; a.lo = lo; a.hi = hi;
-      a.gnoise = gnoise[n] ? gnoise[n] + per * (size_t)(T - t) : nullptr;
-      a.unoise = unoise[n] ? unoise[n] + per * 2 * (size_t)(T - 1 - t) : nullptr;
-      a.gtab = d.gtab + (size_t)t * 8; a.mtab = d.mtab + (size_t)t * 8; a.t = t; a.log_eps = m.log_eps;
-      a.seed = seed; a.stream_id = 2000 + (uint64_t)n * 100000 + 10 + 2 * (uint64_t)t;
-      RUN(f0_p_sample(c, s, a));
-    }
-  }
-  c.release(mk);
-  return 0;
-}
-
 // ------------------------------------------------------------------------------------------------
 // a20/a21: HifiGanGenerator.forward (hifigan_nsf.py:144-169)
-// Stages whose channel counts are multiples of 64 run on the tcgen05 kernel: every conv input is carried as
+// Stages whose channel counts are multiples of 64 run on the tensor-core kernel: every conv input is carried as
 // fp16 hi/lo planes of leaky_relu(x) written by the producing epilogue (the reference applies leaky_relu before
 // every conv), residuals / MRF accumulators stay fp32.  The narrow stage (C = 32) runs its ResBlocks through a
 // time-paired [rows/2, 64] view of the same memory with repacked weights (pack.cu, pack_conv_paired_tc).

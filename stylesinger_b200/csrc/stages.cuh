@@ -26,16 +26,8 @@ struct DenoiserBufs {
 bool denoiser_tc_ok(const Model& m, const Denoiser& d);
 int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, DenoiserBufs* b, bool hoist = false);
 int prepare_cond(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, DenoiserBufs& b);
-// split (0 = off): first row tile of the second utterance group; the residual layers then run as two software-pipelined lanes
-// on the interleaved gate / 1x1 kernel (conv_gemm_tc_dual)
-int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const float* x80, DenoiserBufs& b, int split = 0);
-int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBufs& b, int split = 0);
-int lane_split_tile(const Seq* host_seq);  // utterance boundary closest to half of the row tiles (0: no split possible)
-// both F0/UV samplers in lock step, their residual layers interleaved on the dual kernel (large batches)
-bool f0_dual_ok(const Model& m, const SeqDev& s);
-int run_f0_diffusion_dual(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1, const float* lo,
-                          const float* hi, const float* const gnoise[2], const float* const unoise[2], uint64_t seed,
-                          float* const z[2], int32_t* const uv[2]);
+int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const float* x80, DenoiserBufs& b);
+int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBufs& b);
 // host_seq (optional): the host-side layout of `s`; enables the experimental utterance grouping (SSB_MEL_GROUP_FRAMES)
 int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                       const float* noise, uint64_t seed, float* mel_tight, const Seq* host_seq = nullptr);

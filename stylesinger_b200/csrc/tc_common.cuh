@@ -1,5 +1,5 @@
-// Shared device-side helpers of the tcgen05 kernels: mbarrier / TMA / tcgen05 PTX wrappers, the UMMA
-// shared-memory descriptor for K-major 128B-swizzled tiles, TMEM loads and the fp16 hi/lo plane split.
+// Shared device-side helpers of the Hopper tensor-core kernels: mbarrier / TMA / cluster PTX wrappers, the wgmma
+// shared-memory descriptor for K-major 128B-swizzled tiles, the wgmma instructions themselves and the fp16 hi/lo plane split.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -41,23 +41,13 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// asynchronous HBM -> L2 prefetch of a contiguous range (16-byte aligned, size a multiple of 16)
-__device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// TMA load whose box is written into the same smem offset of every CTA in `mask` (and signals each one's mbarrier at `bar`)
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, uint16_t mask) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
-// ---- CTA-pair (cta_group::2) variants: one MMA spans two SMs (M = 256), each CTA stages its own 128 rows of A and
-// HALF of the weight tile; the leader CTA (cluster rank 0) issues the MMAs and owns the full / tmem_empty barriers.
 __device__ __forceinline__ uint32_t cluster_rank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -71,64 +61,68 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
   return r;
 }
-// TMA load into THIS CTA's smem, transaction bytes reported to a (possibly remote) barrier of the CTA pair
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, uint32_t bar_cluster, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
+// arrive on an mbarrier of any CTA of the cluster (address from mapa_u32); release: this thread's prior reads of the
+// stage it guards are ordered before the arrival
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
 }
-// "Accumulator drained" signal of the epilogue warps: RELAXED.  By the time it is sent the warp's tcgen05.ld have completed
-// (tcgen05.wait::ld), which is all the MMA issuer needs; the default release semantics made every epilogue warp wait, once
-// per tile, until ALL its global stores of that tile had drained (ncu: 0.92 membar stalls per issued instruction in the
-// residual GEMM, profiles/r02_ncu_nodual_v11.md) although nobody synchronises on those stores inside the kernel.
-__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint32_t bar_cluster) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_relaxed(uint32_t bar) {
-  asm volatile("mbarrier.arrive.relaxed.cta.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// MMA completion -> the barrier at this smem offset in BOTH CTAs of the pair
-__device__ __forceinline__ void tc_commit_pair(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tc_mma_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-// K-major, 128B-swizzled tile (rows of 128 bytes, 8-row atoms of 1024 bytes): shared-memory matrix descriptor
+
+// ---- wgmma ------------------------------------------------------------------------------------------
+// K-major, 128B-swizzled tile (rows of 128 bytes, 8-row atoms of 1024 bytes): shared-memory matrix descriptor.
+// One k16 step inside the 64-wide K block is +32 bytes (+2 in the address field); 64 rows further is +8192 bytes.
 __device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);   // start address
+  d |= (uint64_t)1 << 16;                     // leading byte offset (unused for swizzled K-major tiles)
   d |= (uint64_t)(1024u >> 4) << 32;          // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                     // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                     // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                     // SWIZZLE_128B
   return d;
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across a wgmma wait / issue
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both K-major fp16 in shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accum) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accum));
+}
+
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both K-major fp16 in shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accum) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accum));
+}
+
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, A from registers (accumulator fragment layout), B K-major in shared memory
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t accum) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accum));
 }
 
 // WaveNet gate sigmoid(g) * tanh(f) = (e^{2f} - 1) / ((e^{2f} + 1) (1 + e^{-g})): two ex2.approx (2 ulp), one fast division,
 // branch-free.  The libm forms (expf + IEEE division, tanhf with its range branches) cost ~100 dependent instructions per
-// gate and made the epilogue warps - not the tensor pipe - the limiter of the gate GEMM (profiles/r02_ncu_dual_v3.md:
-// 0.17 IPC per epilogue warp).  Absolute error <= ~3e-7, the size of the fp32 rounding already in the accumulators.
+// gate.  Absolute error <= ~3e-7, the size of the fp32 rounding already in the accumulators.
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -140,30 +134,6 @@ __device__ __forceinline__ float gate_act(float g, float f) {
   const float e2f = ex2_approx(f * 2.8853900817779268f);
   const float eg = ex2_approx(g * -1.4426950408889634f);
   return __fdividef(e2f - 1.0f, (e2f + 1.0f) * (1.0f + eg));
-}
-
-// Split form of tmem_ld32 for software pipelining: issue the load of the NEXT chunk, work on the current one, then wait.
-// The wait names the destination registers as in/out operands so that the compiler cannot move a use above it.
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait32(uint32_t (&v)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]),
-                 "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]), "+r"(v[16]),
-                 "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]), "+r"(v[24]),
-                 "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-               :
-               : "memory");
 }
 
 __device__ __forceinline__ void split_store16(__half* hi, __half* lo, const float* z) {
@@ -180,6 +150,10 @@ __device__ __forceinline__ void split_store16(__half* hi, __half* lo, const floa
   *reinterpret_cast<uint4*>(lo + 8) = *reinterpret_cast<const uint4*>(&l[8]);
 }
 
+// wgmma accumulator fragment of an m64nN tile: element j of thread t (lane l of warp w of the warpgroup) sits at
+//   row 16 w + l / 4 + 8 ((j / 2) % 2),  column 8 (j / 4) + 2 (l % 4) + j % 2
+__device__ __forceinline__ int frag_row(int w, int lane, int j) { return 16 * w + (lane >> 2) + 8 * ((j >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int lane, int j) { return 8 * (j >> 2) + 2 * (lane & 3) + (j & 1); }
 
 }  // namespace tc
 }  // namespace ssb

@@ -19,7 +19,7 @@ from .schedules import multinomial_table, sampler_table
 
 def _require_cuda():
     if not torch.cuda.is_available():
-        raise _lib.SsbError("stylesinger_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise _lib.SsbError("stylesinger_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -168,7 +168,7 @@ class AcousticModel:
             self._h = None
 
     def set_tensor_cores(self, enable=True):
-        """tcgen05 (fp16 hi/lo split, 3 MMAs) vs fp32 FFMA for the denoiser layer GEMMs. Returns the mode in effect."""
+        """wgmma (fp16 hi/lo split, 3 MMAs) vs fp32 FFMA for the denoiser layer GEMMs. Returns the mode in effect."""
         return bool(lib.ssb_model_set_tensor_cores(self._h, 1 if enable else 0))
 
     def set_persistent(self, enable=True):
@@ -184,7 +184,7 @@ class AcousticModel:
         return bool(lib.ssb_model_set_persistent_groups(self._h, 1 if enable else 0))
 
     def set_fft_tensor_cores(self, enable: bool) -> bool:
-        """Decoder FFT-block FFN GEMMs on the tcgen05 kernel for batches of >= 1024 frames (default on)."""
+        """Decoder FFT-block FFN GEMMs on the tensor-core kernel for batches of >= 1024 frames (default on)."""
         return bool(lib.ssb_model_set_fft_tensor_cores(self._h, 1 if enable else 0))
 
     # -- schedules -------------------------------------------------------------------------------
@@ -619,7 +619,7 @@ def op_conv1d_tc(x, offsets, w, b, dilation=1):
 
 
 def op_attention(q, k, v, q_offsets, k_offsets, scale, tc=False):
-    """tc=True: the tcgen05 / TMA kernel (ssb_op_attention_tc) instead of the fp32 one."""
+    """tc=True: the wgmma / TMA kernel (ssb_op_attention_tc) instead of the fp32 one."""
     _require_cuda()
     qo = np.ascontiguousarray(q_offsets, np.int32)
     ko = np.ascontiguousarray(k_offsets, np.int32)

@@ -88,7 +88,7 @@ def set_hparams(user=None, **overrides):
 
 
 def _check_supported(hp):
-    """The B200 path implements exactly the configuration egs/stylesinger.yaml selects.
+    """The CUDA path implements exactly the configuration egs/stylesinger.yaml selects.
     Anything else fails loudly instead of silently computing something different."""
     req = {"encoder_type": "fft", "decoder_type": "fft", "ffn_act": "gelu", "ffn_padding": "SAME",
            "dur_loss": "mse", "pitch_type": "frame", "f0_gen": "gmdiff", "decoder": "diffsinger",

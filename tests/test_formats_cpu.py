@@ -1,11 +1,8 @@
-"""stylesinger_b200/formats.py against the reference's own writers / loaders (imported by file path from /root/reference
-when it is present - it is in the build container, where the CPU suite runs - and hand-written files otherwise)."""
-import importlib.util
+"""stylesinger_b200/formats.py against the reference's own writers / loaders: what they produced on the seeded inputs below
+is stored under tests/golden (ref_formats.npz, ref_indexed_dataset.*; tools/make_golden_formats.py), plus hand-written files."""
 import json
 import os
 import pickle
-import sys
-import types
 
 import numpy as np
 import pytest
@@ -13,29 +10,11 @@ import torch
 
 from stylesinger_b200 import formats as F
 
-REF = "/root/reference"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-def _ref_module(rel, name, stubs=()):
-    path = os.path.join(REF, rel)
-    if not os.path.exists(path):
-        pytest.skip("reference sources not present")
-    added = []
-    for s in stubs:
-        if s not in sys.modules:
-            sys.modules[s] = types.ModuleType(s)
-            added.append(s)
-    prev = sys.dont_write_bytecode
-    sys.dont_write_bytecode = True  # never write into /root/reference
-    try:
-        spec = importlib.util.spec_from_file_location(name, path)
-        mod = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(mod)
-    finally:
-        sys.dont_write_bytecode = prev
-        for s in added:
-            del sys.modules[s]
-    return mod
+def _golden():
+    return np.load(os.path.join(GOLDEN, "ref_formats.npz"))
 
 
 def _tiny_sd(seed):
@@ -66,25 +45,28 @@ def test_checkpoint_selection_and_key_layouts(tmp_path):
         F.load_state_dict(str(tmp_path / "empty_dir_that_does_not_exist"))
 
 
-def test_checkpoint_loader_agrees_with_the_reference_load_ckpt(tmp_path):
-    ck = _ref_module("utils/commons/ckpt_utils.py", "ref_ckpt_utils")
+class Tiny(torch.nn.Module):
+    def __init__(self):
+        super().__init__()
+        self.encoder = torch.nn.Linear(4, 3)
+        self.proj = torch.nn.Conv1d(3, 2, 3)
 
-    class Tiny(torch.nn.Module):
-        def __init__(self):
-            super().__init__()
-            self.encoder = torch.nn.Linear(4, 3)
-            self.proj = torch.nn.Conv1d(3, 2, 3)
 
+def write_tiny_checkpoints(d):
     torch.manual_seed(0)
     src = Tiny()
-    d = str(tmp_path)
     torch.save({"state_dict": {"model": src.state_dict()}, "global_step": 7}, os.path.join(d, "model_ckpt_steps_7.ckpt"))
     torch.save({"state_dict": {"model": Tiny().state_dict()}}, os.path.join(d, "model_ckpt_steps_3.ckpt"))
-    dst = Tiny()
-    ck.load_ckpt(dst, d, "model", strict=True)  # the reference picks the newest step
+
+
+def test_checkpoint_loader_agrees_with_the_reference_load_ckpt(tmp_path):
+    d = str(tmp_path)
+    write_tiny_checkpoints(d)
+    g = _golden()
+    ref = {k[len("ckpt/"):]: torch.from_numpy(g[k]) for k in g.files if k.startswith("ckpt/")}  # the reference's load_ckpt
     mine, _ = F.load_state_dict(d, "model")
-    assert sorted(mine) == sorted(dst.state_dict())
-    assert all(torch.equal(mine[k], v) for k, v in dst.state_dict().items())
+    assert sorted(mine) == sorted(ref) == sorted(Tiny().state_dict())
+    assert all(torch.equal(mine[k], v) for k, v in ref.items())
 
 
 def test_vocoder_checkpoint_layouts(tmp_path):
@@ -122,23 +104,16 @@ def _items(n=5):
     return out
 
 
-def test_indexed_dataset_written_by_the_reference_builder(tmp_path):
-    ids = _ref_module("utils/commons/indexed_datasets.py", "ref_indexed_datasets")
+def test_indexed_dataset_written_by_the_reference_builder():
     items = _items()
-    prefix = str(tmp_path / "test")
-    b = ids.IndexedDatasetBuilder(prefix)
-    for it in items:
-        b.add_item(it)
-    b.finalize()
-    with F.IndexedDatasetReader(prefix) as ds:
+    with F.IndexedDatasetReader(os.path.join(GOLDEN, "ref_indexed_dataset")) as ds:  # written by the reference's builder
         assert len(ds) == len(items)
         for i in (3, 0, 4, 1, 2):
             got = ds[i]
             assert got["item_name"] == items[i]["item_name"] and np.array_equal(got["mel"], items[i]["mel"])
+        assert np.array_equal(ds[2]["f0"], items[2]["f0"])
         with pytest.raises(IndexError):
             ds[len(items)]
-    ref_ds = ids.IndexedDataset(prefix)
-    assert len(ref_ds) == len(items) and np.array_equal(ref_ds[2]["f0"], items[2]["f0"])
 
 
 def test_indexed_dataset_hand_written_files(tmp_path):
@@ -154,16 +129,23 @@ def test_indexed_dataset_hand_written_files(tmp_path):
     ds.close()
 
 
-def test_norm_interp_f0_matches_the_reference():
-    pu = _ref_module("utils/pitch_utils.py", "ref_pitch_utils", stubs=("librosa",))
+def f0_cases():
     rng = np.random.default_rng(1)
-    hp = {"pitch_norm": "log", "use_uv": True}
+    out = []
     for n, p0 in ((50, 0.3), (17, 0.0), (9, 1.0), (64, 0.9)):
         f0 = rng.uniform(100, 600, n).astype(np.float32)
         f0[rng.random(n) < p0] = 0.0
-        rf, ru = pu.norm_interp_f0(f0.copy(), hp)
+        out.append(f0)
+    return out
+
+
+def test_norm_interp_f0_matches_the_reference():
+    g = _golden()
+    for i, f0 in enumerate(f0_cases()):
+        assert np.array_equal(f0, g[f"f0/{i}/in"])
+        rf, ru = g[f"f0/{i}/f0"], g[f"f0/{i}/uv"]  # the reference's norm_interp_f0 (log, use_uv)
         mf, mu = F.norm_interp_f0(f0.copy(), "log", True)
-        assert np.array_equal(mu, ru.numpy()) and np.allclose(mf, rf.numpy(), rtol=0, atol=1e-6)
+        assert np.array_equal(mu, ru) and np.allclose(mf, rf, rtol=0, atol=1e-6)
 
 
 def test_item_to_utterance_feeds_pack_batch():

@@ -2,8 +2,8 @@
 
 Bars: LSTM outputs against the UNMODIFIED reference's EmotionEncoder (tests/golden/ref_emotion_encoder.npz, tools/make_golden.py)
 and against the float64 restatement in oracle/frontend_oracle.py: |d hidden| < 1e-6 (fp32 FFMA, 480 dependent steps; torch's
-own fp32 CPU LSTM sits 2e-8 from the float64 oracle; measured on B200: <= 1.2e-7).  Power mel against the numpy restatement of
-librosa: |d| < 2e-5 of the loudest band (one fp32 GEMM with K = 640 per frame, errors relative to the frame's energy; measured 1.1e-6).
+own fp32 CPU LSTM sits 2e-8 from the float64 oracle).  Power mel against the numpy restatement of
+librosa: |d| < 2e-5 of the loudest band (one fp32 GEMM with K = 640 per frame, errors relative to the frame's energy).
 """
 import os
 

@@ -1,5 +1,5 @@
 """Parity at the sizes bench.py runs (VERDICT r1, "next round" item 2): BASELINE.json configs[1] end to end, the CTA-pair
-tcgen05 kernels through chained T=100 samplers on a >= 20 k-frame ragged batch, the pair-kernel variants by name, the
+wgmma kernels through chained T=100 samplers on a >= 20 k-frame ragged batch, the pair-kernel variants by name, the
 mel post-process glue, RVQ at configs[2] scale, and the reference-named module facades on the real engine.
 
 Tolerances: mel L-inf < 1e-3 (north_star); waveform from the ORACLE's mel < 1e-3; RVQ codes bit-exact.
@@ -101,7 +101,7 @@ def test_config1_utt10s_T100_forward_model_vs_oracle():
 
 
 # ---------------------------------------------------------------------------------------------------
-# (b) chained T=100 samplers on a 20 k-frame ragged batch: CTA-pair tcgen05 kernels vs the fp32 FFMA path and the oracle
+# (b) chained T=100 samplers on a 20 k-frame ragged batch: CTA-pair wgmma kernels vs the fp32 FFMA path and the oracle
 def _batch_inputs(seed):
     gen = torch.Generator().manual_seed(seed)
     offs = np.concatenate([[0], np.cumsum(BATCH_LENS)]).astype(np.int32)
@@ -111,14 +111,9 @@ def _batch_inputs(seed):
     return offs, n, cond, coarse
 
 
-def _interleaved(on):
-    from stylesinger_b200._lib import lib
-    return lib.ssb_set_interleaved_layers(1 if on else 0)
-
-
 def test_mel_sampler_T100_pair_kernels_vs_simt_philox_20k_frames():
-    """Three runs of the same T=100 Philox sampler: interleaved dual kernel (opt-in: the gate conv of one utterance group and
-    the 1x1 residual conv of the other share a launch), one launch per GEMM (default), and the fp32 FFMA path."""
+    """Two runs of the same T=100 Philox sampler: one launch per GEMM on the CTA-pair tensor-core kernels, and the fp32 FFMA
+    path."""
     T = 100
     m = acoustic_engine(T, 4)
     offs, n, cond, coarse = _batch_inputs(31)
@@ -126,28 +121,19 @@ def test_mel_sampler_T100_pair_kernels_vs_simt_philox_20k_frames():
     out, ran = {}, {}
     try:
         m.set_persistent(False)
-        for mode in ("dual", "tc", "simt"):
+        for mode in ("tc", "simt"):
             m.set_tensor_cores(mode != "simt")
-            _interleaved(mode == "dual")
             before = _variants()
             out[mode] = m.mel_diffusion(cond, coarse, offs, None, seed=17).clone()
             ran[mode] = _delta(before, _variants())
     finally:
         m.set_tensor_cores(True)
         m.set_persistent(True)
-        _interleaved(False)  # library default
     err = _maxabs(out["tc"], out["simt"])
-    err_d = _maxabs(out["dual"], out["tc"])
-    print(f"mel sampler T=100, {n} frames, philox: pair-tc vs simt L-inf {err:.3e}, interleaved vs per-GEMM {err_d:.3e}; "
-          f"kernels {ran['dual']} | {ran['tc']}")
-    assert ran["tc"].get("tc2r<128,GATE>", 0) == T * 20 and ran["tc"].get("tc2<128,RES_SKIP>", 0) == T * 20
-    # two lanes, software-pipelined by half a layer: first gate and last 1x1 alone, 2L - 1 interleaved launches in between
-    assert ran["dual"].get("tc2d<128,GATE+RES_SKIP>", 0) == T * 39, ran["dual"]
-    # (the lone first gate / last 1x1 of a step cover half the batch: here small enough for the single-CTA kernel)
-    assert sum(v for k, v in ran["dual"].items() if k.endswith(",GATE>")) == T, ran["dual"]
-    assert sum(v for k, v in ran["dual"].items() if k.endswith(",RES_SKIP>")) == T, ran["dual"]
-    assert not ran["simt"], ran["simt"]  # the fp32 FFMA path launches no tcgen05 kernel
-    assert torch.isfinite(out["dual"]).all() and err < 1e-3 and err_d < 1e-4
+    print(f"mel sampler T=100, {n} frames, philox: pair-tc vs simt L-inf {err:.3e}; kernels {ran['tc']}")
+    assert ran["tc"].get("tc2r<64,GATE>", 0) == T * 20 and ran["tc"].get("tc2<64,RES_SKIP>", 0) == T * 20
+    assert not ran["simt"], ran["simt"]  # the fp32 FFMA path launches no tensor-core kernel
+    assert torch.isfinite(out["tc"]).all() and err < 1e-3
 
 
 def test_mel_sampler_T100_pair_kernels_vs_oracle_two_utterances_of_the_batch():
@@ -164,7 +150,7 @@ def test_mel_sampler_T100_pair_kernels_vs_oracle_two_utterances_of_the_batch():
         ran = _delta(before, _variants())
     finally:
         m.set_persistent(True)
-    assert ran.get("tc2r<128,GATE>", 0) == T * 20 and ran.get("tc2<128,RES_SKIP>", 0) == T * 20, ran  # default: one launch per GEMM
+    assert ran.get("tc2r<64,GATE>", 0) == T * 20 and ran.get("tc2<64,RES_SKIP>", 0) == T * 20, ran  # default: one launch per GEMM
     worst = 0.0
     for b in (3, 9):  # 800 and 1111 frames
         a, e = int(offs[b]), int(offs[b + 1])
@@ -192,7 +178,7 @@ def test_f0_sampler_T100_pair_kernels_vs_oracle_two_utterances_of_the_batch():
     before = _variants()
     z, uv = m.f0_diffusion(1, cond.to(DEV), lo.reshape(n).to(DEV), hi.reshape(n).to(DEV), offs, g.to(DEV), u.to(DEV))
     ran = _delta(before, _variants())
-    assert ran.get("tc2r<96,GATE>", 0) == T * 10 and ran.get("tc2<96,RES_SKIP>", 0) == T * 10, ran
+    assert ran.get("tc2r<64,GATE>", 0) == T * 10 and ran.get("tc2<64,RES_SKIP>", 0) == T * 10, ran
     agree, total = 0, 0
     for b in (3, 9):
         a, e = int(offs[b]), int(offs[b + 1])
@@ -211,41 +197,11 @@ def test_f0_sampler_T100_pair_kernels_vs_oracle_two_utterances_of_the_batch():
     assert agree >= 0.99 * total
 
 
-def test_forward_f0_nets_interleaved_vs_per_gemm_batch():
-    """Full forward on a 20 k-frame batch (mel diffusion skipped): the two F0/UV samplers run in lock step with their residual
-    layers interleaved on the dual kernel (tc2d<96,...>); same Philox streams as the per-GEMM schedule, so pitch must agree
-    except where a Gumbel-argmax UV decision sits within rounding distance of a tie."""
-    from stylesinger_b200 import synth
-    from stylesinger_b200.engine import pack_batch
-    T = 25
-    m = acoustic_engine(4, T)
-    utts = [synth.make_utterance(L / 187.5, utt_idx=40 + i, frames=L) for i, L in enumerate(BATCH_LENS)]
-    pb = pack_batch(utts).to(DEV)
-    out, ran = {}, {}
-    try:
-        for on in (True, False):
-            _interleaved(on)
-            before = _variants()
-            r = m.forward(pb, seed=5, skip_mel_diffusion=True, want=("pitch_pred", "f0_denorm"))
-            out[on] = {k: v.clone() for k, v in r.items()}
-            ran[on] = _delta(before, _variants())
-    finally:
-        _interleaved(False)  # library default
-    assert ran[True].get("tc2d<96,GATE+RES_SKIP>", 0) == T * 19, ran[True]  # L = 10: 2L - 1 interleaved launches per step
-    assert "tc2d<96,GATE+RES_SKIP>" not in ran[False]
-    pp_a, pp_b = out[True]["pitch_pred"].cpu().numpy(), out[False]["pitch_pred"].cpu().numpy()
-    same_uv = (pp_a[:, 1] > 0) == (pp_b[:, 1] > 0)
-    close = np.abs(pp_a[:, 0] - pp_b[:, 0]) < 1e-3
-    frac = float((same_uv & close).mean())
-    print(f"forward, {pb.total_frames} frames, T_f0={T}: interleaved vs per-GEMM F0 nets agree on {frac * 100:.3f} % of the frames; {ran[True]}")
-    assert frac >= 0.995
-
-
 # ---------------------------------------------------------------------------------------------------
-# (c) every CTA-pair variant by name, incl. tc2<64,GENERIC> (295 launches / 4.2 % of the batch64 step, untested in round 1)
-@pytest.mark.parametrize("cin,n_out,k,dil,reps,variant", [(256, 512, 3, 4, 1, "tc2r<128,GENERIC>"), (256, 384, 3, 2, 1, "tc2r<96,GENERIC>"),
-                                                         (256, 512, 3, 8, 1, "tc2r<128,GENERIC>"), (256, 512, 3, 1, 1, "tc2r<128,GENERIC>"),
-                                                         (256, 512, 1, 1, 1, "tc2<128,GENERIC>"), (192, 384, 5, 1, 1, "tc2<96,GENERIC>"),
+# (c) every kernel variant by name: CTA pairs (hb = 64 / 32 by N; tap reuse for 3-tap convs) and the single-CTA 64-wide tiles
+@pytest.mark.parametrize("cin,n_out,k,dil,reps,variant", [(256, 512, 3, 4, 1, "tc2r<64,GENERIC>"), (256, 384, 3, 2, 1, "tc2r<64,GENERIC>"),
+                                                         (256, 512, 3, 8, 1, "tc2r<64,GENERIC>"), (256, 512, 3, 1, 1, "tc2r<64,GENERIC>"),
+                                                         (256, 512, 1, 1, 1, "tc2<64,GENERIC>"), (192, 384, 5, 1, 1, "tc2<64,GENERIC>"),
                                                          (128, 128, 7, 1, 2, "tc2<64,GENERIC>"), (64, 64, 11, 1, 2, "tc2<32,GENERIC>"),
                                                          (128, 128, 3, 1, 1, "tc<64,GENERIC>")])
 def test_conv1d_tc_variant_by_name(cin, n_out, k, dil, reps, variant):

@@ -1,4 +1,4 @@
-"""tcgen05 path (fp16 hi/lo split operands, 3 MMAs per product, fp32 TMEM accumulators) against torch fp32
+"""wgmma path (fp16 hi/lo split operands, 3 MMAs per product, fp32 register accumulators) against torch fp32
 and against the reference-generated goldens; and SIMT-vs-tensor-core agreement of the samplers."""
 import numpy as np
 import pytest
@@ -42,8 +42,8 @@ def test_conv1d_tc_matches_torch(cin, n, k, dil):
                                                        (192, 384, 1, 1, 1, 77), (128, 128, 7, 1, 1, 0), (64, 64, 11, 1, 2, 5),
                                                        (64, 2048, 3, 1, 1, 0)])
 def test_conv1d_tc_large_problem_uses_cta_pairs(cin, n_out, k, dil, reps, extra):
-    """Enough row tiles for the CTA-pair kernel (cta_group::2, 256 x 2*hb tiles; hb = 128 / 96 / 64 / 32 by N):
-    persistent tile loop, TMEM double buffering, odd tile counts (the peer CTA of the last pair idles)."""
+    """Enough row tiles for the CTA-pair kernel (2-CTA clusters, two row tiles x one 2*hb-wide N tile, the weight tile
+    multicast to both; hb = 64 / 32 by N): persistent tile loop, odd tile counts (the peer CTA of the last pair idles)."""
     from stylesinger_b200.engine import op_conv1d_tc
     g = torch.Generator().manual_seed(11 + n_out + k)
     lens = [2800, 1500, 2999, 700, 2100, 1900, 2500, 3000, 1234, 2222] * reps + ([extra] if extra else [])
@@ -109,8 +109,8 @@ def test_denoisers_match_reference_golden(tc):
 
 @pytest.mark.parametrize("mode", ["persistent", "per_launch_tc", "simt"])
 def test_mel_diffusion_T100_vs_oracle(mode):
-    """T=100 reverse steps with injected noise: single-launch persistent tcgen05 kernel, one launch per GEMM
-    (tcgen05), and the fp32 FFMA path all stay far below the mel L-inf < 1e-3 bar."""
+    """T=100 reverse steps with injected noise: single-launch persistent wgmma kernel, one launch per GEMM
+    (wgmma), and the fp32 FFMA path all stay far below the mel L-inf < 1e-3 bar."""
     T, Fr = 100, 200
     hp = hp_for(T)
     gen = torch.Generator().manual_seed(77)
@@ -186,7 +186,7 @@ def test_f0_pair_persistent_matches_oracle_and_per_launch():
 
 def test_decoder_fft_ffn_tensor_cores_match_ffma():
     """A 12 s utterance (2250 frames) puts the decoder's GEMMs (QKV / out projections, FFN conv k=9 -> gelu -> linear) and
-    the style aligner's five projections per layer on the tcgen05 kernel; the same pass with that switch off keeps them on
+    the style aligner's five projections per layer on the wgmma kernel; the same pass with that switch off keeps them on
     the fp32 FFMA kernel.  Same Philox streams, so style / decoder_inp / coarse_mel must agree to fp32 rounding."""
     from stylesinger_b200 import synth
     from stylesinger_b200.engine import pack_batch
@@ -206,21 +206,21 @@ def test_decoder_fft_ffn_tensor_cores_match_ffma():
             out[on] = {k: v.clone() for k, v in o.items()}
     finally:
         m.set_fft_tensor_cores(True)
-    # 2 aligner layers x 5 projections + 4 decoder layers x (qkv, out, ffn1, ffn2) GENERIC tcgen05 GEMMs more than with the switch off
+    # 2 aligner layers x 5 projections + 4 decoder layers x (qkv, out, ffn1, ffn2) GENERIC wgmma GEMMs more than with the switch off
     assert sum(ran[True].values()) - sum(ran[False].values()) == 2 * 5 + 4 * 4, ran
     for k in ("style", "decoder_inp"):
         e = _maxabs(out[True][k], out[False][k])
         sc = float(out[False][k].abs().max())
-        print(f"{k}: tcgen05 vs FFMA max |diff| {e:.3e} (max |value| {sc:.2f})")
+        print(f"{k}: wgmma vs FFMA max |diff| {e:.3e} (max |value| {sc:.2f})")
         assert e < 1e-4 * max(1.0, sc), k
     err = _maxabs(out[True]["coarse_mel"], out[False]["coarse_mel"])
     scale = float(out[False]["coarse_mel"].abs().max())
-    print(f"decoder FFN tcgen05 vs FFMA: coarse_mel max |diff| {err:.3e} (max |value| {scale:.2f})")
+    print(f"decoder FFN wgmma vs FFMA: coarse_mel max |diff| {err:.3e} (max |value| {scale:.2f})")
     assert err < 1e-4 * max(1.0, scale)
 
 
 # ---------------------------------------------------------------------------------------------------
-# tcgen05 / TMA attention kernel (csrc/attention_tc.cu) against torch fp32 (float64 accumulation as the arbiter)
+# wgmma / TMA attention kernel (csrc/attention_tc.cu) against torch fp32 (float64 accumulation as the arbiter)
 @pytest.mark.parametrize("ql,kl", [([70, 1, 200], [33, 150, 64]),            # ragged, single-tile keys, 1-row query
                                    ([2812, 300, 129], [2812, 300, 129]),    # self-attention at the longest bench utterance
                                    ([1500, 2200], [1125, 1125])])           # the style aligner's cross-attention shape
@@ -243,7 +243,7 @@ def test_attention_tc_op_matches_torch(ql, kl):
             worst = max(worst, float((out[qo[i]:qo[i + 1], h * 128:(h + 1) * 128].double() - ref).abs().max()))
     print(f"attention_tc {ql} x {kl}: L-inf vs float64 {worst:.3e}; fp32 kernel vs tc {float((out - simt).abs().max()):.3e}")
     # 3-pass fp16-split MMAs with the tensor core's fp32 accumulation over up to 44 key tiles: same error class as the other
-    # tcgen05 GEMMs (3e-5 at T=100); the fp32 kernel itself sits ~1e-5 from the float64 result at these lengths
+    # wgmma GEMMs (3e-5 at T=100); the fp32 kernel itself sits ~1e-5 from the float64 result at these lengths
     assert torch.isfinite(out).all() and worst < 5e-5
 
 
@@ -251,8 +251,8 @@ ATTN_TC_DEFAULT = 1  # library default of the switch (csrc/attention_tc.cu atten
 
 
 def test_forward_attention_tensor_cores_match_fp32_kernel():
-    """Same 12 s forward with the decoder's self-attention and the aligner's cross-attention on the tcgen05 kernel vs the
-    fp32 kernel (all projections on tcgen05 both times): style / decoder_inp / coarse_mel agree to fp32 rounding."""
+    """Same 12 s forward with the decoder's self-attention and the aligner's cross-attention on the wgmma kernel vs the
+    fp32 kernel (all projections on wgmma both times): style / decoder_inp / coarse_mel agree to fp32 rounding."""
     from stylesinger_b200 import synth
     from stylesinger_b200._lib import lib
     from stylesinger_b200.engine import pack_batch
@@ -272,16 +272,13 @@ def test_forward_attention_tensor_cores_match_fp32_kernel():
     for k in ("style", "decoder_inp", "coarse_mel"):
         e = _maxabs(out[True][k], out[False][k])
         sc = float(out[False][k].abs().max())
-        print(f"{k}: attention tcgen05 vs fp32 kernel max |diff| {e:.3e} (max |value| {sc:.2f})")
+        print(f"{k}: attention wgmma vs fp32 kernel max |diff| {e:.3e} (max |value| {sc:.2f})")
         assert torch.isfinite(out[True][k]).all() and e < 1e-4 * max(1.0, sc), k
 
 
 def test_two_model_handles_on_two_streams_match_sequential():
-    """Two model handles driving CTA-pair (cluster) GEMMs from two torch streams at once (the configuration that hung the GPU
-    in round 1; the library orders pair-kernel launches of different streams on the device, conv_gemm_tc.cu pair guard):
-    both streams must drain and reproduce the sequential results bit for bit.  (With the guard lifted,
-    SSB_TC_PAIR_CONCURRENT=1, tools/repro_two_stream_hang.py ran 100 iterations x 2 streams without a hang on the round-2
-    kernels; the guard stays on because it costs nothing at sizes where pair kernels are used.)"""
+    """Two model handles driving CTA-pair (cluster) GEMMs from two torch streams at once: both streams must drain and
+    reproduce the sequential results bit for bit."""
     from stylesinger_b200.engine import AcousticModel
     from stylesinger_b200._lib import variant_launches
     T = 6

@@ -1,6 +1,6 @@
-"""Timing probe for the tcgen05 conv GEMM kernels: one DiffNet-layer-shaped GEMM (K = 3 x 256, N = 512) on ~110k rows,
+"""Timing probe for the tensor-core conv GEMM kernels: one DiffNet-layer-shaped GEMM (K = 3 x 256, N = 512) on ~110k rows,
 single-CTA vs CTA-pair kernel, with parts of the kernel disabled (SSB_TC_DEBUG bits) to see which of TMA / MMA /
-epilogue bounds the tile loop.  Run under `ncu --metrics gpu__time_duration.sum -k regex:conv_gemm_tc` for per-kernel
+epilogue bounds the tile loop.  Run under `ncu --metrics gpu__time_duration.sum -k regex:conv_gemm_wg` for per-kernel
 times; the CUDA-event times printed here include the plane split / unpack kernels of the op wrapper."""
 import json
 import os

@@ -1,5 +1,5 @@
 """Batch test path over the reference's on-disk formats (SURVEY.md section 8f, f4): reads a released acoustic checkpoint
-directory, a HiFi-GAN vocoder directory and a binarised IndexedDataset, runs ph -> mel -> wav on the B200 engine in
+directory, a HiFi-GAN vocoder directory and a binarised IndexedDataset, runs ph -> mel -> wav on the CUDA engine in
 ragged batches and writes one wav per item.  Equivalent of `python tasks/run.py --config ... --infer` of the reference
 (tasks/StyleSinger/stylesinger.py:168-275, which asserts B=1).
 

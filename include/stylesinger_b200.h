@@ -80,6 +80,18 @@ const char* ssb_last_error(void);
 int ssb_model_create(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp);
 void ssb_model_free(ssb_model_t* m);
 
+/* hparams['decoder'] (modules/StyleSinger/stylesinger.py:98-117,176-184): which mel decoder the model was built with. */
+#define SSB_MEL_DECODER_DIFFSINGER 0 /* FFT decoder -> mel_out -> ln_proj -> DDPM over postdiff.denoise_fn (the default) */
+#define SSB_MEL_DECODER_PRODIFF 1    /* ProDiff teacher (modules/diff/prodiff.py:59-232): decoder_inp is the condition of an
+                                      * x0-predicting sampler over diff_decoder.denoise_fn; no FFT decoder / mel_out / ln_proj */
+/* ssb_model_create with the mel decoder chosen: ssb_model_create(...) == ssb_model_create_ex(..., SSB_MEL_DECODER_DIFFSINGER).
+ * PRODIFF loads the mel DiffNet from "diff_decoder.denoise_fn.*" and needs no "postdiff.*" / "ln_proj.*" ("decoder.*" is
+ * still packed for ssb_fft_decoder; "mel_out.*" and the "diff_decoder.*" buffers are accepted and ignored).  The schedule
+ * (ssb_model_set_schedule, which = 0) is then the ProDiff table: slots {0, -1, post_coef1, post_coef2, sigma, -, -,
+ * alphas_cumprod} of the vpsde schedule (prodiff.py:11-13,69-117).  An unknown mel_decoder fails before any CUDA call. */
+int ssb_model_create_ex(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
+                        int32_t mel_decoder);
+
 /* Diffusion schedules (GaussianDiffusion.__init__ modules/diff/shallow_diffusion_tts.py:68-122;
  * GaussianMultinomialDiffusion.__init__ modules/diff/gaussian_multinomial_diffusion.py:208-284).
  * which: 0 = mel denoiser, 1 = both F0 denoisers.  Host arrays:
@@ -141,13 +153,15 @@ size_t ssb_durations_workspace_bytes(const ssb_model_t* m, const ssb_acoustic_in
 int ssb_predict_durations(const ssb_model_t* m, const ssb_acoustic_inputs* in, int32_t* dur_out, float* logdur_out,
                           void* workspace, size_t workspace_bytes, void* stream);
 
-/* StyleSinger.forward(infer=True, global_steps > diff_start): rows a1-a19 of SURVEY.md §8. */
+/* StyleSinger.forward(infer=True, global_steps > diff_start): rows a1-a19 of SURVEY.md §8.
+ * On a PRODIFF model (stylesinger.py:174-177): decoder_inp goes straight to the ProDiff sampler (no FFT decoder, mel_out or
+ * ln_proj); pndm_speedup is ignored like the reference ignores it; asking for coarse_mel or diff_cond is an error. */
 size_t ssb_acoustic_workspace_bytes(const ssb_model_t* m, const ssb_acoustic_inputs* in);
 int ssb_acoustic_forward(const ssb_model_t* m, const ssb_acoustic_inputs* in, const ssb_acoustic_outputs* out,
                          void* workspace, size_t workspace_bytes, void* stream);
 
 /* DiffusionDecoder.forward(infer=True) alone (modules/diff/shallow_diffusion_tts.py:284-307):
- * cond [sumF,256], coarse [sumF,80] -> mel [sumF,80]. */
+ * cond [sumF,256], coarse [sumF,80] -> mel [sumF,80].  DiffSinger models only (the PLMS entry point too). */
 size_t ssb_mel_diffusion_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B);
 int ssb_mel_diffusion_sample(const ssb_model_t* m, const float* cond, const float* coarse_mel,
                              const int32_t* frame_offsets, int32_t B, const float* noise, uint64_t seed,
@@ -160,6 +174,15 @@ size_t ssb_mel_diffusion_plms_workspace_bytes(const ssb_model_t* m, const int32_
 int ssb_mel_diffusion_sample_plms(const ssb_model_t* m, const float* cond, const float* coarse_mel,
                                   const int32_t* frame_offsets, int32_t B, const float* q_noise, uint64_t seed,
                                   int32_t interval, float* mel_out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ProDiffusion.forward(cond, infer=True) alone (modules/diff/prodiff.py:204-222, p_sample :143-148, q_posterior_sample
+ * :135-141), PRODIFF models only: x_T = randn; per step x0 = denoise_fn(x_t, t, cond) (no eps -> x0 conversion, no clip),
+ * x_{t-1} = posterior mean + [t > 0] exp(0.5 logvar) noise; mel = x_0 (denorm_spec is the identity, no mask).
+ * cond [sumF,256] (decoder_inp); noise [(T+1),sumF,80] = the x_T draw then one per step t = T-1..0, or NULL (Philox). */
+size_t ssb_mel_prodiff_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B);
+int ssb_mel_prodiff_sample(const ssb_model_t* m, const float* cond, const int32_t* frame_offsets, int32_t B,
+                           const float* noise, uint64_t seed, float* mel_out, void* workspace, size_t workspace_bytes,
+                           void* stream);
 
 /* One denoiser evaluation, DiffNet.forward / DDiffNet.forward (modules/diff/net.py:107-130,242-266).
  * which: 0 mel (x [sumF,80] -> eps [sumF,80]); 1 / 2 F0 agnostic / specific (x = f0 [sumF], uv int32 [sumF]

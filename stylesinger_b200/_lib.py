@@ -62,6 +62,7 @@ EXPORTS = [
     "ssb_get_style_workspace_bytes", "ssb_get_style", "ssb_op_attention_tc", "ssb_set_attention_tensor_cores",
     "ssb_melspec_create", "ssb_melspec_free", "ssb_melspec_num_frames", "ssb_melspec_workspace_bytes", "ssb_melspec_forward",
     "ssb_melspec_create_ex", "ssb_lstm_encoder_create", "ssb_lstm_encoder_free", "ssb_lstm_encoder_workspace_bytes", "ssb_lstm_encoder_forward",
+    "ssb_model_create_ex", "ssb_mel_prodiff_workspace_bytes", "ssb_mel_prodiff_sample",
 ]
 
 
@@ -76,6 +77,7 @@ def _load():
         "ssb_version": (C.c_int, []),
         "ssb_last_error": (C.c_char_p, []),
         "ssb_model_create": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams)]),
+        "ssb_model_create_ex": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32]),
         "ssb_model_free": (None, [vp]),
         "ssb_model_set_schedule": (C.c_int, [vp, i32, i32, vp, vp, vp, vp]),
         "ssb_durations_workspace_bytes": (sz, [vp, P(AcousticInputs)]),
@@ -84,6 +86,8 @@ def _load():
         "ssb_acoustic_forward": (C.c_int, [vp, P(AcousticInputs), P(AcousticOutputs), vp, sz, vp]),
         "ssb_mel_diffusion_workspace_bytes": (sz, [vp, vp, i32]),
         "ssb_mel_diffusion_sample": (C.c_int, [vp, vp, vp, vp, i32, vp, u64, vp, vp, sz, vp]),
+        "ssb_mel_prodiff_workspace_bytes": (sz, [vp, vp, i32]),
+        "ssb_mel_prodiff_sample": (C.c_int, [vp, vp, vp, i32, vp, u64, vp, vp, sz, vp]),
         "ssb_mel_diffusion_plms_workspace_bytes": (sz, [vp, vp, i32]),
         "ssb_mel_diffusion_sample_plms": (C.c_int, [vp, vp, vp, vp, i32, vp, u64, i32, vp, vp, sz, vp]),
         "ssb_denoiser_eval": (C.c_int, [vp, i32, vp, vp, i32, vp, vp, i32, vp, vp, sz, vp]),

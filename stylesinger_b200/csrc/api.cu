@@ -49,6 +49,8 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   SSB_CHECK(B >= 1 && in.ph_offsets && in.ref_offsets, "acoustic: bad batch description");
   SSB_CHECK(durations_only || in.frame_offsets, "acoustic: frame_offsets required");
   SSB_CHECK(durations_only || in.mel2ph || in.dur, "acoustic: need mel2ph or dur");
+  SSB_CHECK(m.mel_decoder != SSB_MEL_DECODER_PRODIFF || (!out.coarse_mel && !out.diff_cond),
+            "acoustic: a ProDiff model has no coarse_mel / diff_cond (decoder_inp is the sampler's condition)");
   Seq qp, qr, qf;
   qp.build(in.ph_offsets, B);
   qr.build(in.ref_offsets, B);
@@ -217,6 +219,16 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   }
   if (out.decoder_inp) RUN(unpack_rows(c, sf, dec, H, out.decoder_inp, H, H));
 
+  if (m.mel_decoder == SSB_MEL_DECODER_PRODIFF) {
+    // ProDiff (stylesinger.py:176-177): ret = diff_decoder(decoder_inp, ...) - no FFT decoder, mel_out, ln_proj or coarse
+    // mel, and no pndm_speedup (ProDiffusion.forward never reads it)
+    if (!in.skip_mel_diffusion) {
+      SSB_CHECK(out.mel_out != nullptr, "acoustic: mel_out required");
+      RUN(run_mel_diffusion(c, m, sf, dec, nullptr, in.mel_noise, in.seed, out.mel_out, &qf));
+    }
+    return 0;
+  }
+
   // ---- FFT decoder + mel_out (fs2.py:233-237, tts_modules.py:281-306)
   float* coarse = alloc_rows(c, sf, 80);
   float* cond = alloc_rows(c, sf, H);
@@ -311,11 +323,18 @@ int ssb_version(void) { return 100; }
 const char* ssb_last_error(void) { return ssb::last_error(); }
 
 int ssb_model_create(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp) {
+  return ssb_model_create_ex(out, tensors, n, hp, SSB_MEL_DECODER_DIFFSINGER);
+}
+int ssb_model_create_ex(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
+                        int32_t mel_decoder) {
+  SSB_CHECK(mel_decoder == SSB_MEL_DECODER_DIFFSINGER || mel_decoder == SSB_MEL_DECODER_PRODIFF,
+            "ssb_model_create_ex: unknown mel_decoder " + std::to_string(mel_decoder) +
+                " (SSB_MEL_DECODER_DIFFSINGER = 0, SSB_MEL_DECODER_PRODIFF = 1)");
   SSB_CHECK(out && tensors && hp, "ssb_model_create: null argument");
   TensorMap tm;
   if (to_map(tensors, n, &tm)) return -1;
   ssb_model* m = new ssb_model();
-  if (build_model(tm, *hp, &m->m) != 0) {
+  if (build_model(tm, *hp, &m->m, mel_decoder) != 0) {
     delete m;
     return -1;
   }
@@ -371,6 +390,8 @@ int ssb_acoustic_forward(const ssb_model_t* m, const ssb_acoustic_inputs* in, co
 
 static int mel_diff_impl(Ctx& c, const Model& m, const float* cond, const float* coarse, const int32_t* offs, int B,
                          const float* noise, uint64_t seed, float* mel_out) {
+  SSB_CHECK(m.mel_decoder == SSB_MEL_DECODER_DIFFSINGER,
+            "ssb_mel_diffusion_sample: the DDPM sampler needs a DiffSinger model; use ssb_mel_prodiff_sample on a ProDiff model");
   Seq q;
   q.build(offs, B);
   SeqDev s;
@@ -394,6 +415,31 @@ static int mel_plms_impl(Ctx& c, const Model& m, const float* cond, const float*
   RUN(pack_rows(c, s, cond, 256, cg, 256, 256));
   RUN(pack_rows(c, s, coarse, 80, co, 80, 80));
   return run_mel_diffusion_plms(c, m, s, cg, co, q_noise, seed, interval, mel_out);
+}
+static int mel_prodiff_impl(Ctx& c, const Model& m, const float* cond, const int32_t* offs, int B, const float* noise,
+                            uint64_t seed, float* mel_out) {
+  SSB_CHECK(m.mel_decoder == SSB_MEL_DECODER_PRODIFF,
+            "ssb_mel_prodiff_sample: the ProDiff sampler needs a model created with SSB_MEL_DECODER_PRODIFF");
+  Seq q;
+  q.build(offs, B);
+  SeqDev s;
+  RUN(upload_layout(c, q, 1, &s));
+  float* cg = alloc_rows(c, s, 256);
+  WS_OK(c);
+  RUN(pack_rows(c, s, cond, 256, cg, 256, 256));
+  return run_mel_diffusion(c, m, s, cg, nullptr, noise, seed, mel_out, &q);
+}
+size_t ssb_mel_prodiff_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B) {
+  Ctx c = make_ctx(nullptr, 0, nullptr, true);
+  if (mel_prodiff_impl(c, m->m, nullptr, frame_offsets, B, nullptr, 0, nullptr) != 0) return 0;
+  return c.high + 4096;
+}
+int ssb_mel_prodiff_sample(const ssb_model_t* m, const float* cond, const int32_t* frame_offsets, int32_t B,
+                           const float* noise, uint64_t seed, float* mel_out, void* workspace, size_t workspace_bytes,
+                           void* stream) {
+  SSB_CHECK(m && cond && frame_offsets && mel_out && workspace, "null argument");
+  Ctx c = make_ctx(workspace, workspace_bytes, stream);
+  return mel_prodiff_impl(c, m->m, cond, frame_offsets, B, noise, seed, mel_out);
 }
 size_t ssb_mel_diffusion_plms_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B) {
   Ctx c = make_ctx(nullptr, 0, nullptr, true);

@@ -122,7 +122,10 @@ struct Model {
   AlignLayer align[2];
   Denoiser f0net[2];
   Denoiser melnet;
-  Conv mel_out, ln_proj;
+  Conv mel_out, ln_proj;  // DiffSinger mode only
+  // SSB_MEL_DECODER_DIFFSINGER: hparams['decoder'] == 'diffsinger' (FFT decoder + mel_out + ln_proj + DDPM over postdiff.*);
+  // SSB_MEL_DECODER_PRODIFF: 'prodiff' (decoder_inp straight into the x0-predicting sampler over diff_decoder.*)
+  int mel_decoder = SSB_MEL_DECODER_DIFFSINGER;
   float log_eps = 0.f;
   // auxiliary stream + fork/join events: lets the two independent F0 samplers overlap (created in build_model).
   // Calls on one model are therefore serialised with respect to these events (one in-flight forward per model).
@@ -163,7 +166,7 @@ int pack_conv(DevicePool& pool, const HostTensor* w, const HostTensor* b, int di
 int pack_conv_tc(DevicePool& pool, const HostTensor* w, int dil, PackMode mode, const float* packed_bias, ConvTC* out);
 int pack_linear(DevicePool& pool, const HostTensor* w, const HostTensor* b, Conv* out, int row0 = 0, int nrows = -1);
 int pack_conv_transpose(DevicePool& pool, const HostTensor* v, const HostTensor* g, const HostTensor* b, int u, Conv* out);
-int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m);
+int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder = SSB_MEL_DECODER_DIFFSINGER);
 int build_vocoder(TensorMap& tm, const ssb_vocoder_config& cfg, Vocoder* v);
 int set_schedule(Model* m, int which, int T, const float* step_emb, const float* gtab, const float* mtab,
                  cudaStream_t stream);

@@ -285,18 +285,24 @@ __global__ void k_mel_q_sample(const int4* utt, const float* coarse, int ldc, co
                                const float* smax, float sa, float s1a, float* x, int ldx, uint64_t seed, uint64_t sid) {
   ROW_SETUP();
   for (int c = threadIdx.x; c < 80; c += 32) {
+    if (!coarse) {  // ProDiff: x_T = randn, no coarse mel and no normalisation (prodiff.py:214-216)
+      x[r * ldx + c] = noise_n(noise, ti * 80 + c, seed, sid);
+      continue;
+    }
     const float x0 = (coarse[r * ldc + c] - smin[c]) / (smax[c] - smin[c]) * 2.0f - 1.0f;
     x[r * ldx + c] = sa * x0 + s1a * noise_n(noise, ti * 80 + c, seed, sid);
   }
 }
+// DDPM (shallow_diffusion_tts.py:145-162): eps -> clipped x0.  ProDiff (prodiff.py:135-148): the table holds (0, -1) in
+// slots 0-1 so x0 = eps exactly, and clip = 0.
 __global__ void k_mel_p_sample(const int4* utt, float* x, int ldx, const float* eps, int lde, const float* noise,
-                               const float* tab, uint64_t seed, uint64_t sid) {
+                               const float* tab, uint64_t seed, uint64_t sid, int clip) {
   ROW_SETUP();
   const float a = tab[0], bq = tab[1], c1 = tab[2], c2 = tab[3], sig = tab[4];
   for (int c = threadIdx.x; c < 80; c += 32) {
     const float xt = x[r * ldx + c];
     float x0 = a * xt - bq * eps[r * lde + c];
-    x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
+    if (clip) x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
     const float mean = c1 * x0 + c2 * xt;
     // reference: mean + nonzero_mask * exp(0.5*logvar) * noise ; sig already folds the mask
     x[r * ldx + c] = mean + sig * noise_n(noise, ti * 80 + c, seed, sid);
@@ -813,8 +819,8 @@ int mel_q_sample(Ctx& ctx, const SeqDev& s, const float* coarse, int ldc, const 
   return 0;
 }
 int mel_p_sample(Ctx& ctx, const SeqDev& s, float* x, int ldx, const float* eps, int lde, const float* noise,
-                 const float* tab, uint64_t seed, uint64_t sid) {
-  LAUNCH_ROWS(k_mel_p_sample, s, x, ldx, eps, lde, noise, tab, seed, sid);
+                 const float* tab, uint64_t seed, uint64_t sid, bool clip) {
+  LAUNCH_ROWS(k_mel_p_sample, s, x, ldx, eps, lde, noise, tab, seed, sid, clip ? 1 : 0);
   return 0;
 }
 int plms_update(Ctx& ctx, const SeqDev& s, const PlmsArgs& a) {

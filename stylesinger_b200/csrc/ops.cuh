@@ -78,7 +78,7 @@ int rvq_lookup(Ctx&, const SeqDev&, const float* x, int ldx, const float* codebo
 int codebook_norms(Ctx&, const float* codebooks, int n, float* out);  // ||c||^2 for n rows of 256
 
 // ---- samplers (a14, a19) ------------------------------------------------------------------------------
-// x = sqrt_ac * norm_spec(coarse) + sqrt_1m_ac * noise
+// x = sqrt_ac * norm_spec(coarse) + sqrt_1m_ac * noise ; coarse == null (ProDiff): x = noise
 int mel_q_sample(Ctx&, const SeqDev&, const float* coarse, int ldc, const float* noise /*tight [total,80] or null*/,
                  const float* spec_min, const float* spec_max, float sa, float s1a, float* x, int ldx,
                  uint64_t seed, uint64_t stream_id);
@@ -95,7 +95,8 @@ struct PlmsArgs {  // one PLMS update over [rows, 80] guarded buffers (see k_plm
 };
 int plms_update(Ctx&, const SeqDev&, const PlmsArgs&);
 int mel_p_sample(Ctx&, const SeqDev&, float* x, int ldx, const float* eps, int lde, const float* noise,
-                 const float* tab /*dev ptr to 8 floats for this t*/, uint64_t seed, uint64_t stream_id);
+                 const float* tab /*dev ptr to 8 floats for this t*/, uint64_t seed, uint64_t stream_id,
+                 bool clip = true /*false: ProDiff, x0 unclipped*/);
 int mel_denorm(Ctx&, const SeqDev&, const float* x, int ldx, const float* spec_min, const float* spec_max,
                const float* rowmask, float* mel_tight, int ld);
 

@@ -391,9 +391,11 @@ static int build_denoiser(TensorMap& tm, DevicePool& pool, const std::string& p,
   return 0;
 }
 
-int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m) {
+int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder) {
   DevicePool& pool = m->pool;
   m->hp = hp;
+  m->mel_decoder = mel_decoder;
+  const bool prodiff = mel_decoder == SSB_MEL_DECODER_PRODIFF;
   const int H = hp.hidden_size;
   SSB_CHECK(H == 256, "hidden_size must be 256");
   SSB_CHECK(hp.dur_layers <= 4 && hp.rq_depth <= 8, "unsupported dur_layers / rq_depth");
@@ -414,8 +416,10 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m) {
   m->dur_w = upload_tensor(pool, tm.get("note_encoder.dur_ln.weight", {H, 1}));
   m->dur_b = upload_tensor(pool, tm.get("note_encoder.dur_ln.bias", {H}));
   m->pitch_emb = upload_tensor(pool, tm.get("pitch_embed.weight", {300, H}));
-  m->spec_min = upload_tensor(pool, tm.get("postdiff.spec_min"));
-  m->spec_max = upload_tensor(pool, tm.get("postdiff.spec_max"));
+  if (!prodiff) {  // ProDiffusion.norm_spec / denorm_spec are the identity (prodiff.py:225-229): its spec_min/max go unread
+    m->spec_min = upload_tensor(pool, tm.get("postdiff.spec_min"));
+    m->spec_max = upload_tensor(pool, tm.get("postdiff.spec_max"));
+  }
   PK(pack_linear(pool, tm.get("spk_embed_proj.weight"), tm.get("spk_embed_proj.bias"), &m->spk_proj));
   PK(pack_linear(pool, tm.get("emo_embed_proj.weight"), tm.get("emo_embed_proj.bias"), &m->emo_proj));
   PK(build_fft(tm, pool, "encoder.", hp.enc_layers, hp.enc_ffn_kernel, false, &m->enc));
@@ -494,9 +498,15 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m) {
   }
   PK(build_denoiser(tm, pool, "gm_diffnet.", hp.f0_channels, hp.f0_layers, hp.f0_cycle, 1, 3, true, &m->f0net[0]));
   PK(build_denoiser(tm, pool, "gm_diffnet_inpainte.", hp.f0_channels, hp.f0_layers, hp.f0_cycle, 1, 3, true, &m->f0net[1]));
-  PK(build_denoiser(tm, pool, "postdiff.denoise_fn.", hp.mel_channels, hp.mel_layers, hp.mel_cycle, hp.mel_bins, hp.mel_bins, false, &m->melnet));
-  PK(pack_linear(pool, tm.get("mel_out.weight"), tm.get("mel_out.bias"), &m->mel_out));
-  PK(pack_linear(pool, tm.get("ln_proj.weight"), tm.get("ln_proj.bias"), &m->ln_proj));
+  if (prodiff) {
+    // StyleSinger.__init__ with decoder 'prodiff' (stylesinger.py:111-117): the mel DiffNet is diff_decoder.denoise_fn; there
+    // is no postdiff / ln_proj, and mel_out (built by FastSpeech2.__init__) is not used at inference (:176-177)
+    PK(build_denoiser(tm, pool, "diff_decoder.denoise_fn.", hp.mel_channels, hp.mel_layers, hp.mel_cycle, hp.mel_bins, hp.mel_bins, false, &m->melnet));
+  } else {
+    PK(build_denoiser(tm, pool, "postdiff.denoise_fn.", hp.mel_channels, hp.mel_layers, hp.mel_cycle, hp.mel_bins, hp.mel_bins, false, &m->melnet));
+    PK(pack_linear(pool, tm.get("mel_out.weight"), tm.get("mel_out.bias"), &m->mel_out));
+    PK(pack_linear(pool, tm.get("ln_proj.weight"), tm.get("ln_proj.bias"), &m->ln_proj));
+  }
   m->log_eps = logf(1e-30f);
   if (cudaStreamCreateWithFlags(&m->aux_stream, cudaStreamNonBlocking) != cudaSuccess) m->aux_stream = nullptr;
   if (m->aux_stream && (cudaEventCreateWithFlags(&m->ev_fork, cudaEventDisableTiming) != cudaSuccess ||

@@ -217,9 +217,12 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
     return;
   }
   if (e.mode == SP_MEL_SAMPLE) {
-    // p_sample (shallow_diffusion_tts.py:155-162): v = eps for columns n..n+31 (valid below n_valid)
+    // p_sample (shallow_diffusion_tts.py:155-162): v = eps for columns n..n+31 (valid below n_valid).  ProDiff
+    // (prodiff.py:143-148): v = x0 itself; its table holds (0, -1) in slots 0-1 and no_clip is set.
     if (n >= e.n_valid) return;
     const float a = __ldg(e.tab + 0), bq = __ldg(e.tab + 1), c1 = __ldg(e.tab + 2), c2 = __ldg(e.tab + 3), sig = __ldg(e.tab + 4);
+    // clip bound 1 (DDPM) or +inf (ProDiff: no clip).  A bound rather than a branch keeps the kernel at its register count.
+    const float lim = e.no_clip ? __int_as_float(0x7f800000) : 1.0f;
     float xn[32];
 #pragma unroll
     for (int q = 0; q < 8; ++q) {
@@ -233,7 +236,7 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
         const int c = n + 4 * q + k;
         const float xt = xs[k];
         float x0 = a * xt - bq * v[4 * q + k];
-        x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
+        x0 = fminf(fmaxf(x0, -lim), lim);
         const float mean = c1 * x0 + c2 * xt;
         const float nz = e.noise ? __ldg(e.noise + ti * 80 + c) : philox_normal(e.seed, e.stream_id, (uint64_t)(ti * 80 + c));
         xn[4 * q + k] = mean + sig * nz;

@@ -36,6 +36,7 @@ struct SPhase {
   int n_valid;         // MEL_SAMPLE / SKIPPROJ: valid output columns
   int sync_after;      // 1: grid barrier after this entry; 0: the next entry is independent (e.g. the other F0 net)
   int goff;            // tile-group rotation: group g is processed by cluster (g + goff) % nclusters
+  int no_clip;         // MEL_SAMPLE: 1 = use x0 as predicted, no clamp to [-1, 1] (ProDiff p_sample, prodiff.py:143-148)
   // F0_SAMPLE (GaussianMultinomialDiffusion step, gaussian_multinomial_diffusion.py:325-333,398-413) + next DDiffNet input
   int tstep, has_next;
   float log_eps;

@@ -633,6 +633,24 @@ int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const f
   return denoiser_stack(c, d, s, t, b);
 }
 
+// x_T of the mel sampler.  DiffSinger: q_sample(norm_spec(coarse), T-1) (shallow_diffusion_tts.py:298-302); ProDiff:
+// randn (prodiff.py:214-216), no coarse mel.  Both draw block 0 of the injected noise, or Philox stream 1000.
+static int mel_init(Ctx& c, const Model& m, const SeqDev& s, const float* coarse_g, const float* noise, uint64_t seed,
+                    float* xm) {
+  const Denoiser& d = m.melnet;
+  const int T = d.T;
+  if (m.mel_decoder == SSB_MEL_DECODER_PRODIFF)
+    return mel_q_sample(c, s, nullptr, 80, noise, nullptr, nullptr, 0.f, 0.f, xm, 80, seed, 1000);
+  const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 6];
+  return mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, 1000);
+}
+// x_0 -> mel_out.  DiffSinger: denorm_spec (shallow_diffusion_tts.py:305,274-275); ProDiff: denorm_spec is the identity
+// and mel_out is not masked (prodiff.py:221-222,228-229).
+static int mel_finish(Ctx& c, const Model& m, const SeqDev& s, const float* xm, float* mel_tight) {
+  if (m.mel_decoder == SSB_MEL_DECODER_PRODIFF) return unpack_rows(c, s, xm, 80, mel_tight, 80, 80);
+  return mel_denorm(c, s, xm, 80, m.spec_min, m.spec_max, nullptr, mel_tight, 80);
+}
+
 // a18+a19, single launch: all T reverse steps in the persistent wgmma kernel (sampler_tc.cu).
 static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                                         const float* noise, uint64_t seed, float* mel_tight) {
@@ -656,8 +674,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
   unsigned* ctr = c.alloc<unsigned>(4);
   WS_OK(c);
   const size_t per = (size_t)s.total * 80;
-  const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 6];
-  RUN(mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, 1000));
+  RUN(mel_init(c, m, s, coarse_g, noise, seed, xm));
   RUN(x80_planes(c, xm, s.rows, pl[0], pl[1]));
   RUN(split_planes(c, cond_g, 256, s.rows, 256, 1.0f, pl[6], pl[7]));
   // step-invariant conditioner projection of all L layers, once per call (one per-launch GEMM): the gate phases then
@@ -727,6 +744,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
         q.a1 = 10; q.w1 = W_OUT; q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE; q.bias = d.out_bias_pad;
         q.out = xm; q.ldo = 80; q.oh = pl[0]; q.ol = pl[1]; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
         q.noise = noise ? noise + per * (size_t)(T - t) : nullptr; q.seed = seed; q.stream_id = 1001 + (uint64_t)t; q.n_valid = 80;
+        q.no_clip = m.mel_decoder == SSB_MEL_DECODER_PRODIFF;
         ph[k++] = q;
       }
     }
@@ -734,12 +752,13 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
     SSB_CUDA(cudaMemcpyAsync(ph_dev, ph.data(), sizeof(SPhase) * nph, cudaMemcpyHostToDevice, c.stream));
     RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s.tiles, s.tile_tight, s.ntiles, 2 * C / 64, ctr, CS));
   }
-  RUN(mel_denorm(c, s, xm, 80, m.spec_min, m.spec_max, nullptr, mel_tight, 80));
+  RUN(mel_finish(c, m, s, xm, mel_tight));
   c.release(mk);
   return 0;
 }
 
-// a18+a19: DiffusionDecoder.forward(infer=True) (shallow_diffusion_tts.py:284-307)
+// a18+a19: DiffusionDecoder.forward(infer=True) (shallow_diffusion_tts.py:284-307), or on a ProDiff model
+// ProDiffusion.forward(infer=True) (prodiff.py:204-222; coarse_g unused, pass null)
 int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                       const float* noise /*tight [(T+1), total, 80] or null*/, uint64_t seed, float* mel_tight,
                       const Seq* host_seq) {
@@ -776,7 +795,7 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
         SeqDev sg;
         RUN(upload_layout(c, q, 1, &sg));
         const int64_t row_off = (int64_t)host_seq->rs[b0] - GUARD;  // the sub-layout's row 0 inside the big buffers
-        RUN(run_mel_diffusion(c, m, sg, cond_g + row_off * 256, coarse_g + row_off * 80, nullptr,
+        RUN(run_mel_diffusion(c, m, sg, cond_g + row_off * 256, coarse_g ? coarse_g + row_off * 80 : nullptr, nullptr,
                               seed + 0x9E3779B97F4A7C15ull * (uint64_t)gi, mel_tight + tight0 * 80, nullptr));
         c.release(mkg);
         tight0 += fr;
@@ -797,14 +816,14 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
   RUN(prepare_cond(c, d, s, cond_g, b));
   const int T = d.T;
   const size_t per = (size_t)s.total * 80;
-  const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 6];
-  RUN(mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, 1000));
+  const bool clip = m.mel_decoder != SSB_MEL_DECODER_PRODIFF;
+  RUN(mel_init(c, m, s, coarse_g, noise, seed, xm));
   for (int t = T - 1; t >= 0; --t) {
     RUN(mel_denoiser_eval(c, d, s, t, xm, b));
     const float* nz = noise ? noise + per * (size_t)(T - t) : nullptr;
-    RUN(mel_p_sample(c, s, xm, 80, b.head, b.ld_head, nz, d.gtab + (size_t)t * 8, seed, 1001 + (uint64_t)t));
+    RUN(mel_p_sample(c, s, xm, 80, b.head, b.ld_head, nz, d.gtab + (size_t)t * 8, seed, 1001 + (uint64_t)t, clip));
   }
-  RUN(mel_denorm(c, s, xm, 80, m.spec_min, m.spec_max, nullptr, mel_tight, 80));
+  RUN(mel_finish(c, m, s, xm, mel_tight));
   c.release(mk);
   return 0;
 }
@@ -814,6 +833,8 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
 int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                            const float* q_noise /*tight [total, 80] or null*/, uint64_t seed, int interval, float* mel_tight) {
   const Denoiser& d = m.melnet;
+  SSB_CHECK(m.mel_decoder == SSB_MEL_DECODER_DIFFSINGER,
+            "plms: the PLMS sampler needs a DiffSinger model (the ProDiff sampler predicts x0, not eps)");
   SSB_CHECK(d.T > 0, "mel schedule not set: call ssb_model_set_schedule(which=0)");
   SSB_CHECK(interval >= 1 && interval < d.T, "plms: interval (pndm_speedup) must be in [1, T)");
   const size_t mk = c.mark();

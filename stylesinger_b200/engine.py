@@ -14,7 +14,9 @@ import torch
 from . import _lib
 from ._lib import AcousticInputs, AcousticOutputs, HParams, TensorDesc, VocoderConfig, check, lib
 from .hparams import DEFAULT_VOCODER_CONFIG, resolve
-from .schedules import multinomial_table, sampler_table
+from .schedules import multinomial_table, prodiff_table, sampler_table
+
+MEL_DECODERS = {"diffsinger": 0, "prodiff": 1}  # SSB_MEL_DECODER_* of include/stylesinger_b200.h
 
 
 def _require_cuda():
@@ -134,7 +136,8 @@ class _Workspace:
 
 
 class AcousticModel:
-    """Packed StyleSinger acoustic model on one GPU (ssb_model_t)."""
+    """Packed StyleSinger acoustic model on one GPU (ssb_model_t).  hparams['decoder'] selects the mel decoder:
+    'diffsinger' (FFT decoder + DDPM refinement, the default) or 'prodiff' (the ProDiff teacher, decoder_inp -> mel)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], hparams=None, device=None, max_positions=4096):
         _require_cuda()
@@ -153,9 +156,11 @@ class AcousticModel:
                     hp["residual_channels"], hp["residual_layers"], hp["dilation_cycle_length"],
                     hp["f0_residual_channels"], hp["f0_residual_layers"], hp["f0_dilation_cycle_length"],
                     hp["audio_num_mel_bins"])
+        self.mel_decoder = hp["decoder"]
         arr, keep = _descs(sd)
         handle = C.c_void_p()
-        check(lib.ssb_model_create(C.byref(handle), arr, len(sd), C.byref(h)), "ssb_model_create")
+        check(lib.ssb_model_create_ex(C.byref(handle), arr, len(sd), C.byref(h), MEL_DECODERS[self.mel_decoder]),
+              "ssb_model_create_ex")
         self._h = handle
         self._ws = _Workspace(self.device)
         self.T = self.f0_T = None
@@ -192,7 +197,10 @@ class AcousticModel:
         stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
         if T is not None and T != self.T:
             emb = step_embedding(T, self.hp["residual_channels"])
-            g = np.ascontiguousarray(sampler_table(T, self.hp["max_beta"]))
+            if self.mel_decoder == "prodiff":
+                g = np.ascontiguousarray(prodiff_table(T, self.hp["schedule_type"]))
+            else:
+                g = np.ascontiguousarray(sampler_table(T, self.hp["max_beta"]))
             check(lib.ssb_model_set_schedule(self._h, 0, T, C.c_void_p(emb.data_ptr()), g.ctypes.data_as(C.c_void_p),
                                              None, stream), "ssb_model_set_schedule(mel)")
             self.T = T
@@ -242,7 +250,8 @@ class AcousticModel:
                 a.mel_noise = noise["mel"].data_ptr()
         a.seed = int(seed)
         a.skip_mel_diffusion = 1 if skip_mel else 0
-        a.pndm_speedup = int(self.hp.get("pndm_speedup") or 0)  # reference hparam: 0 / absent = DDPM (the StyleSinger default)
+        # reference hparam: 0 / absent = DDPM (the StyleSinger default); the ProDiff sampler ignores it, as the reference does
+        a.pndm_speedup = 0 if self.mel_decoder == "prodiff" else int(self.hp.get("pndm_speedup") or 0)
         return a
 
     # -- entry points ------------------------------------------------------------------------------
@@ -300,6 +309,20 @@ class AcousticModel:
         mel = torch.empty((int(fo[-1]), 80), dtype=torch.float32, device=self.device)
         check(lib.ssb_mel_diffusion_sample(self._h, _ptr(cond), _ptr(coarse), fo.ctypes.data, B, _ptr(noise), int(seed),
                                            _ptr(mel), _ptr(ws), ws.numel(), self._stream()), "ssb_mel_diffusion_sample")
+        return mel
+
+    def mel_prodiff(self, cond, frame_offsets, noise=None, seed=0):
+        """ProDiffusion.forward(cond, infer=True) on a 'prodiff' model: cond = decoder_inp [sumF,256] (device, tight) ->
+        mel [sumF,80].  noise: [(T+1), sumF, 80] (the x_T draw, then one per step), or None for the in-kernel Philox."""
+        fo = np.ascontiguousarray(frame_offsets, np.int32)
+        B = len(fo) - 1
+        n = lib.ssb_mel_prodiff_workspace_bytes(self._h, fo.ctypes.data, B)
+        if n == 0:
+            check(-1, "ssb_mel_prodiff_workspace_bytes")
+        ws = self._ws.get(n)
+        mel = torch.empty((int(fo[-1]), 80), dtype=torch.float32, device=self.device)
+        check(lib.ssb_mel_prodiff_sample(self._h, _ptr(cond), fo.ctypes.data, B, _ptr(noise), int(seed), _ptr(mel), _ptr(ws),
+                                         ws.numel(), self._stream()), "ssb_mel_prodiff_sample")
         return mel
 
     def mel_diffusion_plms(self, cond, coarse, frame_offsets, interval, q_noise=None, seed=0):

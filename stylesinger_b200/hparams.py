@@ -90,9 +90,11 @@ def set_hparams(user=None, **overrides):
 def _check_supported(hp):
     """The CUDA path implements exactly the configuration egs/stylesinger.yaml selects.
     Anything else fails loudly instead of silently computing something different."""
+    prodiff = hp.get("decoder") == "prodiff"  # the ProDiff teacher of the commented block egs/stylesinger.yaml:145-155
     req = {"encoder_type": "fft", "decoder_type": "fft", "ffn_act": "gelu", "ffn_padding": "SAME",
-           "dur_loss": "mse", "pitch_type": "frame", "f0_gen": "gmdiff", "decoder": "diffsinger",
-           "diff_decoder_type": "wavenet", "schedule_type": "linear", "pitch_norm": "log",
+           "dur_loss": "mse", "pitch_type": "frame", "f0_gen": "gmdiff",
+           "decoder": "prodiff" if prodiff else "diffsinger",
+           "diff_decoder_type": "wavenet", "schedule_type": "vpsde" if prodiff else "linear", "pitch_norm": "log",
            "use_uv": True, "emo": True, "style": True, "umln": True, "use_spk_embed": True,
            "use_spk_id": False, "use_pitch_embed": True, "use_energy_embed": False,
            "use_pos_embed": True, "use_txt_cond": True, "num_heads": 2, "hidden_size": 256}
@@ -101,11 +103,13 @@ def _check_supported(hp):
             raise NotImplementedError(
                 f"stylesinger_b200 implements the egs/stylesinger.yaml configuration only: "
                 f"hparams[{k!r}]={hp.get(k)!r}, required {v!r}")
+    if hp.get("rel_pos"):
+        raise NotImplementedError("rel_pos is not selected by egs/stylesinger.yaml")
+    if prodiff:  # ProDiffusion.forward(infer=True) never reads K_step or pndm_speedup (prodiff.py:204-222)
+        return
     if hp.get("pndm_speedup"):  # PLMS sampler over the mel denoiser (SURVEY.md §8 f2, ssb_mel_diffusion_sample_plms)
         k = int(hp["pndm_speedup"])
         if not (1 <= k < int(hp["timesteps"])):
             raise ValueError(f"pndm_speedup must be in [1, timesteps), got {k}")
-    if hp.get("rel_pos"):
-        raise NotImplementedError("rel_pos is not selected by egs/stylesinger.yaml")
     if hp["K_step"] != hp["timesteps"]:
         raise NotImplementedError("K_step must equal timesteps (as in egs/stylesinger.yaml)")

@@ -5,9 +5,11 @@
 tasks/StyleSinger/stylesinger.py:122-123,190-195).  ``HifiGAN`` mirrors the registered vocoder class
 (tasks/tts/vocoder_infer/hifigan_nsf.py:46-75: ``spec2wav(mel np[T,80], f0=np[T]) -> np[T*hop]``).
 
+Both mel decoders of ``hparams['decoder']`` are implemented: 'diffsinger' (the default) and 'prodiff', the ProDiff
+teacher (stylesinger.py:111-117,176-177), whose sampler always runs, whatever ``global_steps`` is.
 Only what the ph -> mel -> wav inference path uses is implemented; everything else raises instead of silently
 doing something different (training mode, teacher-forced f0/uv, the `forcing` aligner branch of early training
-steps, ProDiff / fft decoders).
+steps, the fft decoder).
 """
 from typing import Dict, List, Optional
 
@@ -132,8 +134,10 @@ class StyleSinger:
             lens = [int(d[po[i]:po[i + 1]].sum()) for i in range(pb.B)]
             pb.frame_offsets = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
             ret["dur"] = packed_to_padded(dur, po)
-        # the reference runs the shallow-diffusion refinement only once training passed diff_start (stylesinger.py:181)
-        run_diff = (not skip_decoder) and global_steps > hp.get("diff_start", 0)
+        # the reference runs the shallow-diffusion refinement only once training passed diff_start (stylesinger.py:181);
+        # the ProDiff branch has no such gate and no coarse mel (:176-177)
+        prodiff = hp["decoder"] == "prodiff"
+        run_diff = (not skip_decoder) and (prodiff or global_steps > hp.get("diff_start", 0))
         want = ["f0_denorm", "mel2ph", "decoder_inp", "style", "pitch_pred", "spk_proj", "emo_proj"]
         if not skip_decoder:
             want.append("mel_out" if run_diff else "coarse_mel")

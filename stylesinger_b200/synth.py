@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from .hparams import DEFAULT_VOCODER_CONFIG, resolve
-from .schedules import gaussian_schedule, multinomial_schedule
+from .schedules import gaussian_schedule, multinomial_schedule, prodiff_schedule
 
 N_TOKENS = 61  # 58 phones + <pad>,<EOS>,<UNK> (reference ZH_checkpoint_phone_set.json)
 
@@ -135,6 +135,12 @@ def acoustic_param_shapes(hp):
         out += [(f"{gen}.{b}", (Tf,)) for b in _GAUSS_BUFS]
         out += _diffnet(gen + "._denoise_fn.", Cf, Lf, 1, 3, H, True)
     T = hp["timesteps"]
+    if hp["decoder"] == "prodiff":  # ProDiffusion (stylesinger.py:111-117, prodiff.py:59-117): buffers of length T+1
+        out += [("embed_positions._float_tensor", (1,)), ("diff_decoder.timesteps", ()), ("diff_decoder.timescale", ())]
+        out += [(f"diff_decoder.{b}", (T + 1,)) for b in _GAUSS_BUFS]
+        out += [("diff_decoder.spec_min", (1, 1, 80)), ("diff_decoder.spec_max", (1, 1, 80))]
+        out += _diffnet("diff_decoder.denoise_fn.", hp["residual_channels"], hp["residual_layers"], 80, 80, H, False)
+        return out
     out += [("embed_positions._float_tensor", (1,)), ("ln_proj.weight", (H, 80 + 4 * H)), ("ln_proj.bias", (H,))]
     out += [(f"postdiff.{b}", (T,)) for b in _GAUSS_BUFS]
     out += [("postdiff.spec_min", (1, 1, 80)), ("postdiff.spec_max", (1, 1, 80))]
@@ -201,14 +207,20 @@ def acoustic_state_dict(hp=None, seed=0):
     sched = {"f0": (gaussian_schedule(hp["f0_timesteps"], hp["f0_max_beta"]),
                     multinomial_schedule(hp["f0_timesteps"], hp["f0_max_beta"])),
              "mel": (gaussian_schedule(hp["timesteps"], hp["max_beta"]), None)}
+    if hp["decoder"] == "prodiff":
+        sched["mel"] = (prodiff_schedule(hp["timesteps"], hp["schedule_type"]), None)
     for name, shape in shapes:
         base = name.split(".")[-1]
         if name.endswith("_float_tensor"):
             t = torch.zeros(1)
         elif name.endswith("pos_embed_alpha"):
             t = torch.ones(1)
-        elif name.split(".")[0] in ("f0_gen", "f0_gen_inpainte", "postdiff") and base in _GAUSS_BUFS:
-            s = sched["mel" if name.startswith("postdiff") else "f0"][0]
+        elif name == "diff_decoder.timesteps":
+            t = torch.tensor(float(hp["timesteps"]))
+        elif name == "diff_decoder.timescale":
+            t = torch.tensor(float(hp.get("timescale", 1)))
+        elif name.split(".")[0] in ("f0_gen", "f0_gen_inpainte", "postdiff", "diff_decoder") and base in _GAUSS_BUFS:
+            s = sched["f0" if name.startswith("f0_gen") else "mel"][0]
             t = torch.from_numpy(s[base].copy())
         elif base in _MULTI_BUFS:
             t = torch.from_numpy(sched["f0"][1][base].copy())

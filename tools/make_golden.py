@@ -187,6 +187,46 @@ def case_plms(name, T=100, interval=10, frames=48, seed=61):
     print("wrote", name, mel.shape, float(mel.abs().max()))
 
 
+PRODIFF_OVERRIDES = {"decoder": "prodiff", "schedule_type": "vpsde", "timescale": 1}  # egs/stylesinger.yaml:145-155
+
+
+def case_prodiff(name, T=8, f0_T=4, frames=32, phones=4, ref_frames=32, seed=81, utt_idx=103, sampler_frames=48):
+    """The ProDiff teacher mel decoder (hparams['decoder'] == 'prodiff', stylesinger.py:111-117,176-177,
+    modules/diff/prodiff.py:59-232) with the vpsde schedule: a full B=1 forward, a sampler-only run of
+    ProDiffusion.forward(cond, infer=True) on seeded cond, the registered schedule buffers and the state dict's key list."""
+    import ref_import
+    hp = ref_import.install(T=T, f0_T=f0_T, overrides=PRODIFF_OVERRIDES)
+    import modules.diff.prodiff as pdm
+    import modules.diff.gaussian_multinomial_diffusion as gmd
+    pdm.tqdm = lambda it, **k: it
+    gmd.tqdm = lambda it, **k: it
+    from modules.StyleSinger.stylesinger import StyleSinger
+    model = StyleSinger(_Dict()).eval()
+    sd = synth.acoustic_state_dict(dict(hp), seed=0)
+    model.load_state_dict(sd, strict=True)
+    u = synth.make_utterance(frames / 187.5, utt_idx=utt_idx, ref_frames=ref_frames, frames=frames, phones=phones)
+    out, log = run_model(model, u, seed)
+    g = torch.Generator().manual_seed(seed + 2)
+    cond = torch.randn(1, sampler_frames, 256, generator=g)
+    ns = NoiseSource(seed + 3)
+    with torch.no_grad(), patched_rng(ns):
+        smp = model.diff_decoder(cond, infer=True)["mel_out"]
+    gk = ["betas", "alphas_cumprod", "alphas_cumprod_prev", "sqrt_alphas_cumprod", "sqrt_one_minus_alphas_cumprod",
+          "log_one_minus_alphas_cumprod", "sqrt_recip_alphas_cumprod", "sqrt_recipm1_alphas_cumprod", "posterior_variance",
+          "posterior_log_variance_clipped", "posterior_mean_coef1", "posterior_mean_coef2"]
+    keys = [[k, list(v.shape)] for k, v in model.state_dict().items()]
+    d = {"meta": json.dumps({"T": T, "f0_T": f0_T, "frames": frames, "phones": phones, "ref_frames": ref_frames,
+                             "seed": seed, "utt_idx": utt_idx, "noise_log": log, "sampler_frames": sampler_frames,
+                             "sampler_seed": seed + 3, "sampler_noise_log": ns.log, "overrides": PRODIFF_OVERRIDES,
+                             "state_dict": keys}),
+         "mel_out": np32(out["mel_out"][0]), "f0_denorm": np32(out["f0_denorm"][0]),
+         "decoder_inp": np32(out["decoder_inp"][0]), "sampler_cond": np32(cond[0]), "sampler_mel": np32(smp[0])}
+    for k in gk:
+        d["sched_" + k] = np32(getattr(model.diff_decoder, k))
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()})
+
+
 def case_schedules(name, Ts=(4, 25, 50, 100, 200, 500)):
     """Registered schedule buffers of the reference's DiffusionDecoder / GaussianMultinomialDiffusion at several T
     (shallow_diffusion_tts.py:86-119, gaussian_multinomial_diffusion.py:237-283): pins the oracle's and the product's
@@ -249,7 +289,7 @@ def case_emotion_encoder(name, partials=5, seed=71):
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
-    which = sys.argv[1:] or ["small", "t25", "t100", "plms", "sched", "voc", "emo"]
+    which = sys.argv[1:] or ["small", "t25", "t100", "plms", "prodiff", "sched", "voc", "emo"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
@@ -258,6 +298,8 @@ if __name__ == "__main__":
         case_model("ref_f32_T100", T=100, frames=32, phones=4, ref_frames=32, seed=41, utt_idx=102, with_dur_case=False)
     if "plms" in which:
         case_plms("ref_plms_T100_i10")
+    if "prodiff" in which:
+        case_prodiff("ref_prodiff_T8")
     if "sched" in which:
         case_schedules("ref_schedules")
     if "voc" in which:

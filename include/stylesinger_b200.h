@@ -252,10 +252,6 @@ int ssb_model_set_persistent(ssb_model_t* m, int32_t enable);
  * (shallow_diffusion_tts.py:303-304) as ONE persistent launch (production RNG mode only; each group draws from its own
  * Philox stream).  This is the "persistent-kernel" arm of BASELINE.json configs[4] at batch 64. */
 int ssb_model_set_persistent_groups(ssb_model_t* m, int32_t enable);
-/* 1 (default): the per-launch tensor-core samplers compute the step-invariant conditioner_projection of all residual layers
- * (modules/diff/net.py:59,71 - Conv1d(256, 2C, 1) applied to the same cond in every one of the T steps) ONCE per sampler call
- * and add it in the gate epilogue; 0: contract it inside every layer GEMM of every step (round-1 behaviour). */
-int ssb_model_set_cond_hoist(ssb_model_t* m, int32_t enable);
 /* Decoder FFT blocks (modules/commons/transformer.py TransformerFFNLayer, conv k=9 -> gelu -> linear): run the FFN GEMMs
  * on the tensor-core kernel for batches of >= 1024 frames (default on; 0 keeps them on the fp32 FFMA kernel). Returns the
  * new setting. */

@@ -57,7 +57,7 @@ EXPORTS = [
     "ssb_op_conv1d", "ssb_op_attention", "ssb_mel_postprocess", "ssb_launch_count",
     "ssb_model_set_tensor_cores", "ssb_op_conv1d_tc", "ssb_model_set_persistent", "ssb_model_set_fft_tensor_cores",
     "ssb_vocoder_set_tensor_cores", "ssb_variant_launch_count", "ssb_variant_names", "ssb_tensor_map_cache_stats",
-    "ssb_model_set_persistent_groups", "ssb_model_set_cond_hoist", "ssb_mel_diffusion_plms_workspace_bytes",
+    "ssb_model_set_persistent_groups", "ssb_mel_diffusion_plms_workspace_bytes",
     "ssb_mel_diffusion_sample_plms", "ssb_fft_workspace_bytes", "ssb_fft_encoder", "ssb_fft_decoder",
     "ssb_get_style_workspace_bytes", "ssb_get_style", "ssb_op_attention_tc", "ssb_set_attention_tensor_cores",
     "ssb_melspec_create", "ssb_melspec_free", "ssb_melspec_num_frames", "ssb_melspec_workspace_bytes", "ssb_melspec_forward",
@@ -105,7 +105,6 @@ def _load():
         "ssb_model_set_tensor_cores": (C.c_int, [vp, i32]),
         "ssb_model_set_persistent": (C.c_int, [vp, i32]),
         "ssb_model_set_persistent_groups": (C.c_int, [vp, i32]),
-        "ssb_model_set_cond_hoist": (C.c_int, [vp, i32]),
         "ssb_model_set_fft_tensor_cores": (C.c_int, [vp, i32]),
         "ssb_vocoder_set_tensor_cores": (C.c_int, [vp, i32]),
         "ssb_op_conv1d_tc": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, vp]),

@@ -172,20 +172,18 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
       // Two streams only for small batches (latency-bound chains).  From ~8k frames on every GEMM fills the GPU on its
       // own, and the CTA-pair (cluster) kernels used there must not run concurrently with each other from two streams:
       // that combination hung the GPU in an earlier version of these kernels (root cause not isolated).
-      // SSB_F0_FORK_ALWAYS=1 (diagnosis only): fork at any size, i.e. the round-1 configuration that hung with CTA-pair kernels
-      static const bool fork_always = getenv("SSB_F0_FORK_ALWAYS") != nullptr;
-      const bool fork = !c.dry && m.aux_stream != nullptr && (sf.ntiles <= 64 || fork_always);
+      const bool fork = !c.dry && m.aux_stream != nullptr && sf.ntiles <= 64;
       if (fork) {
         SSB_CUDA(cudaEventRecord(m.ev_fork, c.stream));
         SSB_CUDA(cudaStreamWaitEvent(m.aux_stream, m.ev_fork, 0));
       }
       const size_t off0 = c.off;
-      RUN(run_f0_diffusion(c, m, 0, sf, cond, lo, hi, in.f0_gauss_noise[0], in.f0_unif_noise[0], in.seed, za, uva, &qf));
+      RUN(run_f0_diffusion(c, m, 0, sf, cond, lo, hi, in.f0_gauss_noise[0], in.f0_unif_noise[0], in.seed, za, uva));
       c.off = c.high;  // keep sampler 0's buffers alive: sampler 1 allocates above them
       {
         Ctx c2 = c;
         if (fork) c2.stream = m.aux_stream;
-        RUN(run_f0_diffusion(c2, m, 1, sf, cond2, lo, hi, in.f0_gauss_noise[1], in.f0_unif_noise[1], in.seed, zs, uvs, &qf));
+        RUN(run_f0_diffusion(c2, m, 1, sf, cond2, lo, hi, in.f0_gauss_noise[1], in.f0_unif_noise[1], in.seed, zs, uvs));
         if (c2.high > c.high) c.high = c2.high;
         c.failed = c.failed || c2.failed;
       }
@@ -274,7 +272,7 @@ int denoiser_eval_api(Ctx& c, const Model& m, int which, const SeqDev& s, const 
   SSB_CHECK(d.T > 0, "denoiser_eval: schedule not set");
   float* cond = alloc_rows(c, s, 256);
   DenoiserBufs b;
-  RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b, false));  // a single evaluation: nothing to amortise a hoist over
+  RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
   RUN(pack_rows(c, s, cond_tight, 256, cond, 256, 256));
   RUN(prepare_cond(c, d, s, cond, b));
   if (which == 0) {
@@ -498,7 +496,7 @@ int ssb_f0_diffusion_sample(const ssb_model_t* m, int32_t which, const float* co
   RUN(pack_rows(c, s, cond, 256, cg, 256, 256));
   RUN(pack_rows(c, s, clip_lo, 1, lo, 1, 1));
   RUN(pack_rows(c, s, clip_hi, 1, hi, 1, 1));
-  RUN(run_f0_diffusion(c, m->m, which, s, cg, lo, hi, gauss_noise, unif_noise, seed, z, uv, &q));
+  RUN(run_f0_diffusion(c, m->m, which, s, cg, lo, hi, gauss_noise, unif_noise, seed, z, uv));
   RUN(unpack_rows(c, s, z, 1, f0_norm_out, 1, 1));
   RUN(unpack_rows_i32(c, s, uv, uv_out));
   return 0;
@@ -660,12 +658,6 @@ int ssb_model_set_persistent(ssb_model_t* m, int32_t enable) {
   SSB_CHECK(m, "null model");
   m->m.persistent = enable != 0;
   return m->m.persistent ? 1 : 0;
-}
-
-int ssb_model_set_cond_hoist(ssb_model_t* m, int32_t enable) {
-  SSB_CHECK(m, "null model");
-  m->m.cond_hoist = enable != 0;
-  return m->m.cond_hoist ? 1 : 0;
 }
 
 int ssb_model_set_persistent_groups(ssb_model_t* m, int32_t enable) {

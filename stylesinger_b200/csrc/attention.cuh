@@ -36,7 +36,7 @@ struct AttnTCArgs {
   __half* oh = nullptr; __half* ol = nullptr; int ldh = 0;
 };
 int attention_tc(Ctx& ctx, const AttnTCArgs& a);
-bool attention_tc_enabled();           // process-wide switch for the long-batch paths (SSB_ATTN_TC=0/1 sets the start value)
+bool attention_tc_enabled();           // process-wide switch for the long-batch paths (ssb_set_attention_tensor_cores; default on)
 int set_attention_tc_enabled(int on);
 // planes [rows, ld] (columns col0 .. col0 + C) -> transposed planes [C, ldt]; columns rows .. ldt are zero-filled
 int transpose_planes(Ctx& ctx, const __half* xh, const __half* xl, int ld, int col0, int64_t rows, int C, __half* th, __half* tl,

@@ -294,16 +294,8 @@ __global__ void k_transpose_planes(const __half* __restrict__ xh, const __half* 
 
 }  // namespace
 
-static std::atomic<int> g_attn_tc{-1};
-bool attention_tc_enabled() {
-  int v = g_attn_tc.load(std::memory_order_relaxed);
-  if (v < 0) {
-    const char* e = getenv("SSB_ATTN_TC");
-    v = e ? (atoi(e) != 0 ? 1 : 0) : 1;  // default on (checked against the fp32 kernel by tests/test_gpu_tc.py)
-    g_attn_tc.store(v, std::memory_order_relaxed);
-  }
-  return v != 0 && tc_available();
-}
+static std::atomic<int> g_attn_tc{1};  // default on (checked against the fp32 kernel by tests/test_gpu_tc.py)
+bool attention_tc_enabled() { return g_attn_tc.load(std::memory_order_relaxed) != 0 && tc_available(); }
 int set_attention_tc_enabled(int on) {
   g_attn_tc.store(on ? 1 : 0, std::memory_order_relaxed);
   return on ? 1 : 0;

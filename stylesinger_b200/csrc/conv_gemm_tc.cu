@@ -45,8 +45,7 @@ struct Cfg {
 
 struct TCParams {
   const int2* tiles;
-  int ntiles, NT, taps, kchunks, kchunks2, dil, center, N;
-  int dbg;  // SSB_TC_DEBUG probe bits (tools/gemm_probe.py): 1 = no epilogue, 2 = no MMAs
+  int ntiles, NT, taps, kchunks, dil, center, N;
   EpiTC e;
 };
 
@@ -99,12 +98,12 @@ __device__ __forceinline__ void prefetch_chunk(const EpiTC& e, int64_t r0, int n
       } else {
         src = e.skip + (r0 + rq) * e.ld_skip + (n - e.C) + q4; st = 4 * (int64_t)e.ld_skip;
       }
-      once = e.stream_hints != 0;
+      once = true;
     } else return;
   } else {  // EPI_GATE: the hoisted conditioner projection of this layer
     if (!e.add) return;
     src = e.add + (r0 + rq) * e.ld_add + n + q4; st = 4 * (int64_t)e.ld_add;
-    once = e.stream_hints != 0;
+    once = true;
   }
   if (once) {
 #pragma unroll
@@ -234,10 +233,7 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb,
           v0 += o.x; v1 += o.y; v2 += o.z; v3 += o.w;
         }
         const bool ok = i < nsteps;
-        if (ok) {
-          if (e.stream_hints) __stcs(reinterpret_cast<float4*>(ps), make_float4(v0, v1, v2, v3));
-          else *reinterpret_cast<float4*>(ps) = make_float4(v0, v1, v2, v3);
-        }
+        if (ok) __stcs(reinterpret_cast<float4*>(ps), make_float4(v0, v1, v2, v3));
         if (planes) {  // last layer only
           uint2 kh, kl;
           split_pack4(v0, v1, v2, v3, kh, kl);
@@ -316,7 +312,7 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb,
   }
 }
 
-// REUSE (3-tap convs, centre tap 1, dilation <= HALO, no second operand): per K block ONE halo-extended activation tile of
+// REUSE (3-tap convs, centre tap 1, dilation <= HALO): per K block ONE halo-extended activation tile of
 // BM + 2 HALO rows is loaded into its own ring, and the three taps read it through wgmma descriptors whose start address
 // is moved by whole 128-byte rows (the 128B swizzle phase follows the shared-memory address, and the tile starts on a
 // 1024-byte boundary).  Per tap only the weight tile is loaded: a third of the activation bytes of the plain variant.
@@ -324,8 +320,6 @@ template <int BN, int CL, int MODE, bool REUSE>
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-                    const __grid_constant__ CUtensorMap tmA2_hi, const __grid_constant__ CUtensorMap tmA2_lo,
-                    const __grid_constant__ CUtensorMap tmB2_hi, const __grid_constant__ CUtensorMap tmB2_lo,
                     const TCParams p) {
   using K = Cfg<BN, REUSE>;
   constexpr int STAGES = K::STAGES;
@@ -357,8 +351,7 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   else __syncthreads();
 
   const int total = (CL > 1 ? (p.ntiles + 1) / 2 : p.ntiles) * p.NT;
-  const int nk1 = p.taps * p.kchunks;
-  const int nk = nk1 + p.kchunks2;
+  const int nk = p.taps * p.kchunks;
 
   if (warp < 4) {  // warpgroup 0 only runs the TMA producer: its registers go to the consumer warpgroups
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
@@ -401,16 +394,14 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
           }
         } else {
           for (int kb = 0; kb < nk; ++kb) {
-            const bool second = kb >= nk1;
-            const int tap = second ? 0 : kb / p.kchunks;
-            const int c0 = second ? (kb - nk1) * BK : (kb - tap * p.kchunks) * BK;
-            const int arow = second ? row0 : row0 + (tap - p.center) * p.dil;
+            const int tap = kb / p.kchunks;
+            const int c0 = (kb - tap * p.kchunks) * BK;
+            const int arow = row0 + (tap - p.center) * p.dil;
             // the expect_tx of load_b also covers this CTA's two activation boxes of the same stage
-            const uint32_t fb = load_b(second ? &tmB2_hi : &tmB_hi, second ? &tmB2_lo : &tmB_lo, c0,
-                                       second ? nt * BN : tap * p.N + nt * BN, (uint32_t)(2 * A_TILE));
+            const uint32_t fb = load_b(&tmB_hi, &tmB_lo, c0, tap * p.N + nt * BN, (uint32_t)(2 * A_TILE));
             const uint32_t sa = sbase + stage * K::STAGE;
-            tma_load_2d(sa, second ? &tmA2_hi : &tmA_hi, fb, c0, arow);
-            tma_load_2d(sa + A_TILE, second ? &tmA2_lo : &tmA_lo, fb, c0, arow);
+            tma_load_2d(sa, &tmA_hi, fb, c0, arow);
+            tma_load_2d(sa + A_TILE, &tmA_lo, fb, c0, arow);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
@@ -439,7 +430,6 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       }
     };
     auto mma_block = [&](uint64_t dah, uint64_t dal, uint64_t dbh, uint64_t dbl) {
-      if (p.dbg & 2) return;
       wg_fence();
       fence_acc(acc);
 #pragma unroll
@@ -525,7 +515,7 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         named_sync(pair_bar, 64);
         const int ch = 2 * cp + eg;
         if (ch + 2 < NCH && nrows > 0) prefetch_chunk<MODE>(p.e, r0, nrows, n0 + (ch + 2) * 32, lane, nxt, tq);
-        if (nrows > 0 && !(p.dbg & 1))
+        if (nrows > 0)
           epilogue_chunk<MODE>(p.e, reinterpret_cast<float4*>(xb_pair + eg * 1024), r0, nrows, n0 + ch * 32, lane, cur, tq);
         cur = nxt;
         named_sync(pair_bar, 64);  // both chunks consumed before the buffers are refilled
@@ -663,26 +653,17 @@ std::atomic<long long>* variant_counter(const char* name) {
 }
 const char* mode_name(int mode) { return mode == EPI_GATE ? "GATE" : (mode == EPI_RES_SKIP ? "RES_SKIP" : "GENERIC"); }
 
-bool stream_hints_enabled() {
-  static const bool off = getenv("SSB_TC_NO_STREAM_HINTS") != nullptr;
-  return !off;
-}
 // index into ConvTC::tm_hi / tm_lo of the weight descriptor whose box has `rows` rows
 constexpr int map_index(int rows) { return rows == 128 ? 0 : (rows == 64 ? 1 : 2); }
 // Cluster (CTA-pair) kernels from DIFFERENT streams are ordered against each other on the device: two such kernels in
 // flight from two streams hung an earlier build of this library, and the cause was never isolated.  Each pair launch on a
 // new stream first waits (cudaStreamWaitEvent) for the last pair launch of any other stream; same-stream launches are
 // already ordered and pay nothing, and at the sizes where pair kernels are chosen each one fills the GPU on its own.
-// SSB_TC_PAIR_CONCURRENT=1 switches the ordering off.  Process-wide and thread-safe: the mutex is held across wait +
-// launch + record.
+// Process-wide and thread-safe: the mutex is held across wait + launch + record.
 std::mutex g_pair_mu;
 cudaEvent_t g_pair_evt[MAX_DEV];
 cudaStream_t g_pair_last_stream[MAX_DEV];
 bool g_pair_evt_valid[MAX_DEV];
-bool pair_guard_enabled() {
-  static const bool off = getenv("SSB_TC_PAIR_CONCURRENT") != nullptr;
-  return !off;
-}
 void pair_guard_begin(int dev, cudaStream_t st) {  // g_pair_mu held
   if (!g_pair_evt[dev] && cudaEventCreateWithFlags(&g_pair_evt[dev], cudaEventDisableTiming) != cudaSuccess) {
     g_pair_evt[dev] = nullptr;
@@ -708,19 +689,11 @@ int launch_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
     return variant_counter(name);
   }();
   const ConvTC& w = *p.w;
-  const ConvTC& w2 = p.w2 ? *p.w2 : *p.w;
   const int bi = map_index(BN / CL);
   const uint32_t a_rows = REUSE ? A3_ROWS : BM;  // REUSE: halo-extended activation boxes
-  CUtensorMap ta_hi, ta_lo, ta2_hi, ta2_lo;
+  CUtensorMap ta_hi, ta_lo;
   if (cached_act_map(&ta_hi, p.A_hi, (uint64_t)p.rows_total, (uint64_t)w.Cin, a_rows)) return -1;
   if (cached_act_map(&ta_lo, p.A_lo, (uint64_t)p.rows_total, (uint64_t)w.Cin, a_rows)) return -1;
-  if (p.w2) {
-    if (cached_act_map(&ta2_hi, p.A2_hi, (uint64_t)p.rows_total, (uint64_t)w2.Cin, BM)) return -1;
-    if (cached_act_map(&ta2_lo, p.A2_lo, (uint64_t)p.rows_total, (uint64_t)w2.Cin, BM)) return -1;
-  } else {
-    ta2_hi = ta_hi;
-    ta2_lo = ta_lo;
-  }
   tp.NT = w.N / BN;
   const int total = (CL > 1 ? (tp.ntiles + 1) / 2 : tp.ntiles) * tp.NT;
   const int slots = num_sms / CL;
@@ -736,15 +709,15 @@ int launch_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
   at[0].val.clusterDim.x = (unsigned)CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
   {
-    const bool guard = CL > 1 && pair_guard_enabled();
+    const bool guard = CL > 1;
     const int dev = guard ? current_device() : 0;
     std::unique_lock<std::mutex> lk(g_pair_mu, std::defer_lock);
     if (guard) {
       lk.lock();
       pair_guard_begin(dev, ctx.stream);
     }
-    const cudaError_t le = cudaLaunchKernelEx(&cfg, conv_gemm_wg_kernel<BN, CL, MODE, REUSE>, ta_hi, ta_lo, w.tm_hi[bi],
-                                              w.tm_lo[bi], ta2_hi, ta2_lo, w2.tm_hi[bi], w2.tm_lo[bi], tp);
+    const cudaError_t le =
+        cudaLaunchKernelEx(&cfg, conv_gemm_wg_kernel<BN, CL, MODE, REUSE>, ta_hi, ta_lo, w.tm_hi[bi], w.tm_lo[bi], tp);
     if (guard) pair_guard_end(dev, ctx.stream);
     SSB_CUDA(le);
   }
@@ -760,12 +733,10 @@ int launch(Ctx& ctx, const GemmTC& p, const TCParams& tp, int num_sms) {
     default: return launch_m<BN, CL, EPI_GENERIC, false>(ctx, p, tp, num_sms);
   }
 }
-// the tap-reuse variant serves the CTA-pair sizes of 3-tap convs: the gate GEMMs of both denoisers (with the hoisted
-// conditioner, i.e. without a second operand), the vocoder's transposed convs (3-tap, N = u * C) and its k = 3 ResBlock convs
+// the tap-reuse variant serves the CTA-pair sizes of 3-tap convs: the gate GEMMs of both denoisers, the vocoder's transposed
+// convs (3-tap, N = u * C) and its k = 3 ResBlock convs
 bool tap_reuse_eligible(const GemmTC& p, const ConvTC& w) {
-  static const bool off = getenv("SSB_TC_NO_TAP_REUSE") != nullptr;
-  return !off && !p.w2 && w.taps == 3 && w.center == 1 && w.dil >= 1 && w.dil <= HALO &&
-         (p.e.mode == EPI_GATE || p.e.mode == EPI_GENERIC);
+  return w.taps == 3 && w.center == 1 && w.dil >= 1 && w.dil <= HALO && (p.e.mode == EPI_GATE || p.e.mode == EPI_GENERIC);
 }
 
 }  // namespace
@@ -818,7 +789,7 @@ int make_weight_maps(ConvTC* w) {
 int conv_gemm_tc(Ctx& ctx, const GemmTC& p) {
   if (ctx.dry || p.ntiles == 0) return 0;
   const ConvTC& w = *p.w;
-  SSB_CHECK(w.ok && (!p.w2 || (p.w2->ok && p.w2->N == w.N && p.w2->taps == 1)), "conv_gemm_tc: weights not packed for the tensor-core path");
+  SSB_CHECK(w.ok, "conv_gemm_tc: weights not packed for the tensor-core path");
   SSB_CHECK(p.e.act == ACT_NONE || p.e.act == ACT_RELU || p.e.act == ACT_LRELU || p.e.act == ACT_GELU,
             "conv_gemm_tc: unsupported epilogue activation");
   SSB_CHECK(p.e.plane_act == ACT_NONE || p.e.plane_act == ACT_LRELU, "conv_gemm_tc: unsupported plane activation");
@@ -827,18 +798,11 @@ int conv_gemm_tc(Ctx& ctx, const GemmTC& p) {
   const int num_sms = device_sms();
   TCParams tp;
   tp.tiles = p.tiles; tp.ntiles = p.ntiles; tp.taps = w.taps; tp.kchunks = w.Cin / BK;
-  tp.kchunks2 = p.w2 ? p.w2->Cin / BK : 0;
   tp.dil = w.dil; tp.center = w.center; tp.N = w.N; tp.e = p.e;
-  {
-    const char* d = getenv("SSB_TC_DEBUG");
-    tp.dbg = d ? atoi(d) : 0;
-  }
   if (!tp.e.bias) tp.e.bias = w.bias;
-  tp.e.stream_hints = stream_hints_enabled() ? 1 : 0;
   // large problems: CTA pairs (two row tiles x one 2*hb-wide N tile per cluster, the weight tile multicast to both) halve
   // the weight bytes each SM pulls through L2
-  const bool pair_off = getenv("SSB_TC_NO_PAIR") != nullptr;
-  if (!pair_off && (!p.w2 || p.w2->hb == w.hb) && (int64_t)((p.ntiles + 1) / 2) * (w.N / (2 * w.hb)) >= (int64_t)num_sms) {
+  if ((int64_t)((p.ntiles + 1) / 2) * (w.N / (2 * w.hb)) >= (int64_t)num_sms) {
     if (tap_reuse_eligible(p, w)) {
       if (p.e.mode == EPI_GATE) return w.hb == 64 ? launch_m<128, 2, EPI_GATE, true>(ctx, p, tp, num_sms) : launch_m<64, 2, EPI_GATE, true>(ctx, p, tp, num_sms);
       return w.hb == 64 ? launch_m<128, 2, EPI_GENERIC, true>(ctx, p, tp, num_sms) : launch_m<64, 2, EPI_GENERIC, true>(ctx, p, tp, num_sms);
@@ -846,7 +810,7 @@ int conv_gemm_tc(Ctx& ctx, const GemmTC& p) {
     return w.hb == 64 ? launch<128, 2>(ctx, p, tp, num_sms) : launch<64, 2>(ctx, p, tp, num_sms);
   }
   // small problems: 64-wide N tiles keep more SMs busy and shorten each tile's dependent chain
-  const bool small = (w.N % 128 != 0) || (p.w2 && p.w2->N % 128 != 0) || (int64_t)p.ntiles * (w.N / 128) < (int64_t)num_sms * 2;
+  const bool small = (w.N % 128 != 0) || (int64_t)p.ntiles * (w.N / 128) < (int64_t)num_sms * 2;
   if (small) return launch<64, 1>(ctx, p, tp, num_sms);
   return launch<128, 1>(ctx, p, tp, num_sms);
 }

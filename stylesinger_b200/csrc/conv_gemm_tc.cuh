@@ -11,13 +11,8 @@
 // each CTA of a 2-CTA cluster loads its own 128 rows of A and half of a 2*hb-wide weight tile, multicast to both CTAs).
 // CTAs are persistent over the tiles.  The pair kernel is used when there are >= num_SMs pair tiles, the 64-wide
 // single-CTA kernel for small problems, the 128-wide one otherwise (conv_gemm_tc()).
-// An optional SECOND operand pair (A2, W2: 1 tap, no shift) extends the K loop: the DiffNet layer
-// GEMM contracts [3 taps x C of y | 256 of cond] in one accumulator, so the conditioner projection
-// needs neither a hoisted [rows, L*2C] fp32 buffer nor an epilogue read.
 // 3-tap convs at pair sizes take the tap-reuse variant: one halo-extended activation tile per K block serves all three taps.
-// Env switches (diagnostics): SSB_TC_NO_PAIR=1 disables the pair kernel, SSB_TC_NO_TAP_REUSE=1 the tap-reuse variant,
-// SSB_TC_PAIR_CONCURRENT=1 lifts the cross-stream ordering of pair kernels,
-// SSB_TC_DEBUG=<bits> switches parts of the kernel off for tools/gemm_probe.py (results are then garbage).
+// Pair launches from different streams are ordered against each other on the device (conv_gemm_tc.cu).
 #pragma once
 #include <cuda.h>
 
@@ -36,6 +31,8 @@ struct ConvTC {            // packed weights for the tensor-core path
   bool ok = false;
 };
 
+// The skip accumulator (RES_SKIP) and the conditioner addend (GATE) are touched once per launch: they are read and written
+// with ld/st.global.cs (evict-first), so that they do not push the y / z planes (re-read by the next launch) out of L2.
 struct EpiTC {
   int mode = EPI_GENERIC;        // EPI_GENERIC: out = acc + bias ; EPI_GATE ; EPI_RES_SKIP
   const float* bias = nullptr;
@@ -73,8 +70,6 @@ struct EpiTC {
   int tile_base = 0;             //   index of tiles[0] in the full tile table (a GEMM over a sub-range of the row tiles)
   int out_nb = 0;                // GENERIC, > 0: `out` is column-block-major: block j = columns [j*out_nb, (j+1)*out_nb) is its own
   int64_t out_bs = 0;            //   [rows, out_nb] matrix at out + j * out_bs (the hoisted conditioner: one matrix per layer)
-  int stream_hints = 1;          // skip accumulator and conditioner addends are touched once per launch: ld/st.global.cs (evict-first)
-                                 //   so that they do not push the y / z planes (re-read by the next launch) out of L2; SSB_TC_NO_STREAM_HINTS=1: off
   __half* sh = nullptr;          // RES_SKIP (last layer): the finished skip sum also as fp16 planes [rows, C]
   __half* sl = nullptr;
 };
@@ -84,9 +79,6 @@ struct GemmTC {
   const __half* A_lo = nullptr;
   int64_t rows_total = 0;
   const ConvTC* w = nullptr;
-  const __half* A2_hi = nullptr; // optional second operand [rows_total, w2->Cin], contracted with w2 (1 tap)
-  const __half* A2_lo = nullptr;
-  const ConvTC* w2 = nullptr;
   const int2* tiles = nullptr;
   int ntiles = 0;
   EpiTC e;

@@ -8,8 +8,9 @@
 //   * the recurrence runs on one 8-CTA thread-block CLUSTER per group of up to 8 partials: CTA r keeps the W_hh rows of
 //     hidden units 32 r .. 32 r + 31 (all four gates, 128 x 256 fp32 = 128 KB) resident in its REGISTER FILE for the whole
 //     sequence (128 registers per thread), computes those gates for every partial of the group, applies the cell update and
-//     writes its 32 new h values into the (double-buffered) h vector of all 8 CTAs through distributed shared memory; one
-//     cluster barrier per frame.  W_hh is read from HBM once per layer instead of once per frame.
+//     writes its 32 new h values into the (double-buffered) h vector of all 8 CTAs through distributed shared memory
+//     (mbarrier-signalled `st.async`, no cluster-wide barrier per frame).  W_hh is read from HBM once per layer instead
+//     of once per frame.
 #include <cooperative_groups.h>
 #include <math.h>
 #include <stdlib.h>
@@ -135,18 +136,18 @@ __device__ __forceinline__ void hbar_wait(uint32_t bar, uint32_t parity) {
 // shared memory: per frame the SM issues 8 x 128 x 256 FFMAs and only 16 KB of shared-memory reads.
 // Cell role: warp `up` = partial, lane `uj` = hidden unit 32 r + uj (c in a register for the whole sequence): sums the two K
 // halves and the input projection (fetched one frame ahead), applies the gates, stores h_t into every CTA of the cluster.
-// Exchange of h_t, ASYNC = true: `st.async` stores that report their bytes to an mbarrier of the receiving CTA (one per h
-// buffer, 8 KB expected per frame); a CTA starts frame t + 1 as soon as ITS copy of h_t is complete - no cluster-wide
-// barrier.  Double buffering is enough: h_{t+1} values can only be sent by a CTA that has received all of h_t, i.e. after
-// every CTA has finished the mat-vec of frame t - 1 that read the buffer being overwritten.  ASYNC = false: plain remote
-// stores + one barrier.cluster per frame (kept as the A/B reference, SSB_LSTM_CLUSTER_BARRIER=1).
+// Exchange of h_t: `st.async` stores that report their bytes to an mbarrier of the receiving CTA (one per h buffer, 8 KB
+// expected per frame); a CTA starts frame t + 1 as soon as ITS copy of h_t is complete - no cluster-wide barrier.  Double
+// buffering is enough: h_{t+1} values can only be sent by a CTA that has received all of h_t, i.e. after every CTA has
+// finished the mat-vec of frame t - 1 that read the buffer being overwritten.
 // KQ = K splits of the mat-vec: RPC * KQ threads, each with H / KQ weights in registers.
-template <bool ASYNC, int KQ>
-__global__ void __cluster_dims__(NCTA, 1, 1) __launch_bounds__(RPC * KQ, 1)
+constexpr int KQ = 2;
+constexpr int LSTM_THREADS = RPC * KQ;
+__global__ void __cluster_dims__(NCTA, 1, 1) __launch_bounds__(LSTM_THREADS, 1)
     k_lstm_layer(const float* __restrict__ xproj, const float* __restrict__ whh_p, int P, int T, float* __restrict__ hseq,
                  float* __restrict__ hlast) {
   __shared__ __align__(16) float hsm[2 * H * PB];   // [2][H][PB]
-  constexpr int LSTM_THREADS = RPC * KQ, KH = H / KQ;
+  constexpr int KH = H / KQ;
   __shared__ float gsm[KQ * PB * RPC];              // [kh][partial][row]
   __shared__ __align__(8) unsigned long long hbar[2];
   cg::cluster_group cl = cg::this_cluster();
@@ -163,7 +164,7 @@ __global__ void __cluster_dims__(NCTA, 1, 1) __launch_bounds__(RPC * KQ, 1)
     for (int k = 0; k < KH; ++k) w[k] = src[(size_t)k * RPC];
   }
   for (int i = tid; i < 2 * H * PB; i += LSTM_THREADS) hsm[i] = 0.f;
-  if (ASYNC && tid == 0) {
+  if (tid == 0) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_addr(&hbar[0])) : "memory");
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_addr(&hbar[1])) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -179,9 +180,6 @@ __global__ void __cluster_dims__(NCTA, 1, 1) __launch_bounds__(RPC * KQ, 1)
 #pragma unroll
     for (int q = 0; q < 4; ++q) nx[q] = xg[q * UPC];
   }
-  float* remote[NCTA];
-#pragma unroll
-  for (int d = 0; d < NCTA; ++d) remote[d] = cl.map_shared_rank(hsm, d);
   const uint32_t hsm_a = smem_addr(hsm), bar_a = smem_addr(&hbar[0]);
   cl.sync();  // every CTA of the cluster is resident and has zeroed its h buffers before any remote write
 
@@ -194,7 +192,7 @@ __global__ void __cluster_dims__(NCTA, 1, 1) __launch_bounds__(RPC * KQ, 1)
 #pragma unroll
       for (int q = 0; q < 4; ++q) nx[q] = xg[(size_t)(t + 1) * G4 + q * UPC];
     }
-    if (ASYNC && t > 0) hbar_wait(bar_a + 8u * (uint32_t)(t & 1), (uint32_t)(((t - 1) >> 1) & 1));  // h_{t-1} has arrived here
+    if (t > 0) hbar_wait(bar_a + 8u * (uint32_t)(t & 1), (uint32_t)(((t - 1) >> 1) & 1));  // h_{t-1} has arrived here
     float acc[PB];
 #pragma unroll
     for (int j = 0; j < PB; ++j) acc[j] = 0.f;
@@ -228,30 +226,24 @@ __global__ void __cluster_dims__(NCTA, 1, 1) __launch_bounds__(RPC * KQ, 1)
       c_state = sigmoidf_(gf) * c_state + sigmoidf_(gi) * tanhf(gg);
       const float h = sigmoidf_(go) * tanhf(c_state);
       const int off = (cur ^ 1) * H * PB + (r * UPC + uj) * PB + up;
-      if (ASYNC) {
-        if (t + 1 < T) {
-          const uint32_t nb = 8u * (uint32_t)((t + 1) & 1);
-          // arm the barrier frame t + 1 waits on: everybody's 32 units x 8 partials x 4 bytes.  Its previous phase (frame
-          // t - 1) has completed (this thread waited on it); bytes that arrive before the arming are simply counted first
-          if (tid == 0)
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a + nb), "r"((uint32_t)(H * PB * 4)) : "memory");
+      if (t + 1 < T) {
+        const uint32_t nb = 8u * (uint32_t)((t + 1) & 1);
+        // arm the barrier frame t + 1 waits on: everybody's 32 units x 8 partials x 4 bytes.  Its previous phase (frame
+        // t - 1) has completed (this thread waited on it); bytes that arrive before the arming are simply counted first
+        if (tid == 0)
+          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a + nb), "r"((uint32_t)(H * PB * 4)) : "memory");
 #pragma unroll
-          for (int d = 0; d < NCTA; ++d)
-            st_async_f32(map_rank(hsm_a + 4u * (uint32_t)off, (uint32_t)d), h, map_rank(bar_a + nb, (uint32_t)d));
-        }
-      } else {
-#pragma unroll
-        for (int d = 0; d < NCTA; ++d) remote[d][off] = h;
+        for (int d = 0; d < NCTA; ++d)
+          st_async_f32(map_rank(hsm_a + 4u * (uint32_t)off, (uint32_t)d), h, map_rank(bar_a + nb, (uint32_t)d));
       }
       if (cell_valid) {
         if (hseq) hseq[((size_t)(p0 + up) * T + t) * H + r * UPC + uj] = h;
         if (hlast && t == T - 1) hlast[(size_t)(p0 + up) * H + r * UPC + uj] = h;
       }
     }
-    if (!ASYNC) cl.sync();  // h_t complete in every CTA; gsm and the old h buffer are free again
     cur ^= 1;
   }
-  if (ASYNC) cl.sync();  // nobody leaves while a neighbour could still be storing into its shared memory
+  cl.sync();  // nobody leaves while a neighbour could still be storing into its shared memory
 }
 
 // relu(linear(h)) L2-normalised per partial (model.py:51-57); one block of 256 threads per partial
@@ -312,10 +304,6 @@ int run_lstm(Ctx& c, const ssb_lstm_encoder& m, const float* frames, int P, int 
   const float* x = frames;
   int K = m.n_in;
   const unsigned groups = (unsigned)((P + PB - 1) / PB);
-  const char* cb = getenv("SSB_LSTM_CLUSTER_BARRIER");  // A/B: 1 = one barrier.cluster per frame instead of mbarrier-signalled stores
-  const bool cluster_barrier = cb && cb[0] == '1';
-  const char* k4 = getenv("SSB_LSTM_KSPLIT4");  // A/B: 512 threads, four K quarters per gate row
-  const bool ksplit4 = k4 && k4[0] == '1';
   for (int l = 0; l < m.layers; ++l) {
     k_gemm_bias<<<dim3(G4 / 64, (unsigned)((rows + 63) / 64)), 256, 0, c.stream>>>(x, m.wih_t[(size_t)l], m.bias[(size_t)l], xproj,
                                                                                    (int64_t)rows, G4, K);
@@ -325,12 +313,7 @@ int run_lstm(Ctx& c, const ssb_lstm_encoder& m, const float* frames, int P, int 
     float* out_seq = last ? nullptr : ((l & 1) ? seq_b : seq_a);
     float* hl = last ? hid : nullptr;
     const float* wp = m.whh_p[(size_t)l];
-    if (cluster_barrier)
-      k_lstm_layer<false, 2><<<groups * NCTA, RPC * 2, 0, c.stream>>>(xproj, wp, P, T, out_seq, hl);
-    else if (ksplit4)
-      k_lstm_layer<true, 4><<<groups * NCTA, RPC * 4, 0, c.stream>>>(xproj, wp, P, T, out_seq, hl);
-    else
-      k_lstm_layer<true, 2><<<groups * NCTA, RPC * 2, 0, c.stream>>>(xproj, wp, P, T, out_seq, hl);
+    k_lstm_layer<<<groups * NCTA, LSTM_THREADS, 0, c.stream>>>(xproj, wp, P, T, out_seq, hl);
     SSB_CUDA(cudaGetLastError());
     ++g_launches;
     x = out_seq;

@@ -67,8 +67,7 @@ struct DenoiserLayer {
   Conv outp;   // 1x1, N = 2C ([res | skip])
   Conv dproj;  // diffusion_projection C -> C (used only to build the step-bias table)
   ConvTC dil_tc, outp_tc;  // tensor-core packing of dil / outp (ok == false when not eligible)
-  ConvTC cond_tc;          // conditioner_projection (256 -> 2C, gate-interleaved) as the 2nd K segment of dil_tc
-  float* bias_gate_tc = nullptr;  // dil bias + conditioner bias (packed column order)
+  float* bias_gate_tc = nullptr;  // dil bias + conditioner bias (packed column order): the GATE GEMM's bias (cond_all_tc has none)
 };
 struct Denoiser {
   int C = 0, L = 0, in_dims = 0, out_dims = 0, cycle = 4;
@@ -132,8 +131,6 @@ struct Model {
   cudaStream_t aux_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   bool persistent = true;  // single-launch persistent sampler for small batches (ssb_model_set_persistent)
-  bool cond_hoist = true;   // tensor-core per-launch path: conditioner projection computed once per call ([rows, L*2C] fp32) and
-                            // added in the GATE epilogue, instead of being contracted inside every layer GEMM of every step
   bool persistent_groups = false;  // large batches: groups of <= 48 row tiles, one persistent launch each (mel sampler)
   bool use_tc = true;  // tensor-core path for the denoiser layer GEMMs (ssb_model_set_tensor_cores)
   bool fft_tc = true;  // tensor-core path for the decoder FFT blocks' FFN on long batches (ssb_model_set_fft_tensor_cores)

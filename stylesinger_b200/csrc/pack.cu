@@ -326,13 +326,12 @@ static int build_denoiser(TensorMap& tm, DevicePool& pool, const std::string& p,
       for (int c = 0; c < H; ++c) Wc[(size_t)c * L * N2 + pn] = cw->data[(size_t)n * H + c];
       Bc[pn] = cb->data[n];
     }
-    {  // tensor-core path: conditioner projection folded into the layer GEMM as a second K segment
+    {  // tensor-core path: the gate GEMM's bias (the hoisted conditioner projection below carries none)
       const HostTensor* db = tm.get(q + "dilated_conv.bias");
       if (!db) return -1;
       std::vector<float> bs((size_t)N2);
       for (int n = 0; n < N2; ++n) bs[perm_col(n, N2, PACK_GATE_SIG_TANH)] = db->data[n] + cb->data[n];
       d->layers[i].bias_gate_tc = pool.upload(bs);
-      if (pack_conv_tc(pool, cw, 1, PACK_GATE_SIG_TANH, d->layers[i].bias_gate_tc, &d->layers[i].cond_tc)) return -1;
     }
   }
   {  // tensor-core packing of the SAME stacked projection (no bias: bias_gate_tc already carries dil + conditioner bias):

@@ -79,11 +79,9 @@ __device__ __forceinline__ void prefetch32(const SPhase& e, int64_t r, int n, bo
       for (int q = 0; q < 8; ++q) p.a[q] = __ldcg(sp + q);
     }
   } else if (e.mode == SP_GATE) {
-    if (e.add) {
-      const float4* ap = reinterpret_cast<const float4*>(e.add + r * e.ld_add + n);
+    const float4* ap = reinterpret_cast<const float4*>(e.add + r * e.ld_add + n);
 #pragma unroll
-      for (int q = 0; q < 8; ++q) p.a[q] = __ldg(ap + q);
-    }
+    for (int q = 0; q < 8; ++q) p.a[q] = __ldg(ap + q);
   } else if (e.mode == SP_MEL_SAMPLE) {
     const float4* xp = reinterpret_cast<const float4*>(e.out + r * e.ldo + n);
 #pragma unroll
@@ -98,11 +96,9 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
 #pragma unroll
   for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]) + __ldg(e.bias + n + j);
   if (e.mode == SP_GATE) {
-    if (e.add) {
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        v[4 * q] += pre.a[q].x; v[4 * q + 1] += pre.a[q].y; v[4 * q + 2] += pre.a[q].z; v[4 * q + 3] += pre.a[q].w;
-      }
+    for (int q = 0; q < 8; ++q) {
+      v[4 * q] += pre.a[q].x; v[4 * q + 1] += pre.a[q].y; v[4 * q + 2] += pre.a[q].z; v[4 * q + 3] += pre.a[q].w;
     }
     float z[16];
 #pragma unroll
@@ -302,16 +298,13 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
     const int gpm = P.NT / cs;           // tile groups (clusters' worth of N-tiles) per M-tile
     const int groups = ntiles * gpm;
     const int g_first = ((cid - P.goff) % ncl + ncl) % ncl;  // group g runs on cluster (g + goff) % ncl
-    const int nk1 = P.taps * P.kchunks;
-    const int nk = nk1 + P.kchunks2;
+    const int nk = P.taps * P.kchunks;
 
     if (warp == 0) {
       if (lane == 0) {
         proxy_fence();
         const CUtensorMap* mA = maps + P.a1;
         const CUtensorMap* mW = maps + P.w1;
-        const CUtensorMap* mA2 = maps + (P.a2 >= 0 ? P.a2 : P.a1);
-        const CUtensorMap* mW2 = maps + (P.a2 >= 0 ? P.w2 : P.w1);
         for (int g = g_first; g < groups; g += ncl) {
           const int mt = g / gpm, nt = (g - mt * gpm) * cs + cr;
           const int row0 = tiles[mt].x;
@@ -320,32 +313,19 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
             const uint32_t fb = full0 + 8 * stage;
             mbar_expect_tx(fb, STAGE);
             const uint32_t sa = sbase + stage * STAGE;
-            if (kb < nk1) {
-              const int tap = kb / P.kchunks;
-              const int c0 = (kb - tap * P.kchunks) * BK;
-              const int arow = row0 + (tap - P.center) * P.dil;
-              const int brow = tap * P.N + nt * BN;
-              if (cs > 1) {
-                tma_load_2d_mc(sa + cr * slice_bytes, mA, fb, c0, arow + cr * slice_rows, cmask);
-                tma_load_2d_mc(sa + A_TILE + cr * slice_bytes, mA + 1, fb, c0, arow + cr * slice_rows, cmask);
-              } else {
-                tma_load_2d(sa, mA, fb, c0, arow);
-                tma_load_2d(sa + A_TILE, mA + 1, fb, c0, arow);
-              }
-              tma_load_2d(sa + 2 * A_TILE, mW, fb, c0, brow);
-              tma_load_2d(sa + 2 * A_TILE + B_TILE, mW + 1, fb, c0, brow);
+            const int tap = kb / P.kchunks;
+            const int c0 = (kb - tap * P.kchunks) * BK;
+            const int arow = row0 + (tap - P.center) * P.dil;
+            const int brow = tap * P.N + nt * BN;
+            if (cs > 1) {
+              tma_load_2d_mc(sa + cr * slice_bytes, mA, fb, c0, arow + cr * slice_rows, cmask);
+              tma_load_2d_mc(sa + A_TILE + cr * slice_bytes, mA + 1, fb, c0, arow + cr * slice_rows, cmask);
             } else {
-              const int c0 = (kb - nk1) * BK;
-              if (cs > 1) {
-                tma_load_2d_mc(sa + cr * slice_bytes, mA2, fb, c0, row0 + cr * slice_rows, cmask);
-                tma_load_2d_mc(sa + A_TILE + cr * slice_bytes, mA2 + 1, fb, c0, row0 + cr * slice_rows, cmask);
-              } else {
-                tma_load_2d(sa, mA2, fb, c0, row0);
-                tma_load_2d(sa + A_TILE, mA2 + 1, fb, c0, row0);
-              }
-              tma_load_2d(sa + 2 * A_TILE, mW2, fb, c0, nt * BN);
-              tma_load_2d(sa + 2 * A_TILE + B_TILE, mW2 + 1, fb, c0, nt * BN);
+              tma_load_2d(sa, mA, fb, c0, arow);
+              tma_load_2d(sa + A_TILE, mA + 1, fb, c0, arow);
             }
+            tma_load_2d(sa + 2 * A_TILE, mW, fb, c0, brow);
+            tma_load_2d(sa + 2 * A_TILE + B_TILE, mW + 1, fb, c0, brow);
             if (++stage == STAGES) { stage = 0; phase_bit ^= 1; }
           }
         }

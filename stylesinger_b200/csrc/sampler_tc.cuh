@@ -8,11 +8,11 @@ namespace ssb {
 
 enum SPhaseMode { SP_GATE = 0, SP_RES_SKIP = 1, SP_INPROJ = 2, SP_SKIPPROJ = 3, SP_MEL_SAMPLE = 4, SP_F0_SAMPLE = 5 };
 
-// One GEMM phase of the persistent sampler: D[128 x 64 tiles] = A1 (*) W1 (+ A2 * W2), then a fused epilogue.
+// One GEMM phase of the persistent sampler: D[128 x 64 tiles] = A1 (*) W1, then a fused epilogue.
 struct SPhase {
-  int a1, a2;          // tensor-map index of the A operand's hi plane (lo = +1); a2 < 0: no second operand
-  int w1, w2;          // tensor-map index of the weights' hi plane (lo = +1), box [64 x 64]
-  int taps, kchunks, kchunks2, dil, center, N, NT;
+  int a1;              // tensor-map index of the A operand's hi plane (lo = +1)
+  int w1;              // tensor-map index of the weights' hi plane (lo = +1), box [64 x 64]
+  int taps, kchunks, dil, center, N, NT;
   int mode;
   const float* bias;   // [N]
   float* out;          // fp32 output (x, or the sampler state x_t [rows,80])
@@ -24,7 +24,7 @@ struct SPhase {
   int ld_res;
   float beta;
   const float* vec2;   // step bias added before the planes are written
-  const float* add;    // GATE: hoisted conditioner projection of this layer [rows, ld_add] (packed gate column order), or null
+  const float* add;    // GATE: hoisted conditioner projection of this layer [rows, ld_add] (packed gate column order)
   int ld_add;
   float* skip;         // RES_SKIP: skip accumulator
   int ld_skip, C, skip_init;

@@ -450,11 +450,8 @@ static GemmTC layer_gate_gemm(const Denoiser& d, const DenoiserBufs& b, int64_t 
   const int C = d.C;
   GemmTC g;
   g.A_hi = b.yh; g.A_lo = b.yl; g.rows_total = rows; g.w = &d.layers[l].dil_tc; g.tiles = tiles; g.ntiles = ntiles;
-  if (b.condpre) {  // conditioner hoisted: K = 3*C only, the projection arrives as an epilogue addend (one [rows, 2C] matrix per layer)
-    g.e.add = b.condpre + (size_t)l * (size_t)rows * 2 * C; g.e.ld_add = 2 * C;
-  } else {
-    g.A2_hi = b.ch; g.A2_lo = b.cl; g.w2 = &d.layers[l].cond_tc;  // K = 3*C (taps of y) + 256 (cond)
-  }
+  // K = 3*C (taps of y); the hoisted conditioner projection arrives as an epilogue addend (one [rows, 2C] matrix per layer)
+  g.e.add = b.condpre + (size_t)l * (size_t)rows * 2 * C; g.e.ld_add = 2 * C;
   g.e.mode = EPI_GATE; g.e.bias = d.layers[l].bias_gate_tc;
   g.e.oh = b.zh; g.e.ol = b.zl; g.e.ldh = C;
   return g;
@@ -542,12 +539,12 @@ static __half* alloc_half_rows(Ctx& c, const SeqDev& s, int C) {
   return p;
 }
 bool denoiser_tc_ok(const Model& m, const Denoiser& d) {
-  if (!m.use_tc) return false;
+  if (!m.use_tc || !d.cond_all_tc.ok) return false;
   for (auto& l : d.layers)
-    if (!l.dil_tc.ok || !l.outp_tc.ok || !l.cond_tc.ok) return false;
+    if (!l.dil_tc.ok || !l.outp_tc.ok) return false;
   return true;
 }
-int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, DenoiserBufs* b, bool hoist) {
+int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, DenoiserBufs* b) {
   b->tc = tc;
   b->condpre = nullptr;
   b->x = alloc_rows(c, s, d.C);
@@ -574,7 +571,7 @@ int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, Denoiser
     b->ch = alloc_half_rows(c, s, 256);
     b->cl = alloc_half_rows(c, s, 256);
     // only valid rows are ever written or read (epilogues are row-bounded): no 4.6 GB memset for batch64
-    if (hoist && d.cond_all_tc.ok) b->condpre = alloc_rows(c, s, d.L * 2 * d.C, false);
+    b->condpre = alloc_rows(c, s, d.L * 2 * d.C, false);
   } else {
     b->y = alloc_rows(c, s, d.C);
     b->zg = alloc_rows(c, s, d.C);
@@ -582,8 +579,7 @@ int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, Denoiser
   }
   // tensor-core heads: the fp32 skip accumulator is private to the RES_SKIP epilogue (the heads read the planes the last
   // layer writes), so it is kept chunk-tiled (every 32 x 32 epilogue chunk one contiguous 4 KB block; conv_gemm_tc.cuh)
-  static const bool skip_rowmajor = getenv("SSB_SKIP_ROWMAJOR") != nullptr;  // A/B switch for the layout experiment
-  b->skip_tiled = b->tc_heads && !skip_rowmajor;
+  b->skip_tiled = b->tc_heads;
   if (b->skip_tiled) {
     const size_t n = (size_t)s.ntiles * TILE_M * d.C;
     b->skip = c.alloc<float>(n);  // fully written by layer 0 (skip_init) before it is read: no memset
@@ -596,18 +592,22 @@ int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, Denoiser
   WS_OK(c);
   return 0;
 }
-// Conditioner: tensor-core path -> fp16 hi/lo planes of cond (contracted inside every layer GEMM);
-// SIMT path -> the step-invariant projection of all L layers hoisted into one [rows, L*2C] buffer.
+// Tensor-core path: cond -> fp16 hi/lo planes (ch, cl) -> the step-invariant conditioner projection of all L layers at
+// once, [rows, 256] x [256, L*2C], once per sampler call.  condpre is layer-major (row pitch 2C floats instead of L * 2C):
+// matrix l is the GATE epilogue addend of layer l.
+static int hoist_cond_tc(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, __half* ch, __half* cl,
+                         float* condpre) {
+  RUN(split_planes(c, cond_g, 256, s.rows, 256, 1.0f, ch, cl));
+  GemmTC g;
+  g.A_hi = ch; g.A_lo = cl; g.rows_total = s.rows; g.w = &d.cond_all_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
+  g.e.mode = EPI_GENERIC; g.e.out = condpre; g.e.ldo = d.L * 2 * d.C;
+  g.e.out_nb = 2 * d.C; g.e.out_bs = (int64_t)s.rows * 2 * d.C;
+  return conv_gemm_tc(c, g);
+}
+// Conditioner: the step-invariant projection of all L layers hoisted into one [rows, L*2C] buffer (tensor-core path:
+// hoist_cond_tc; SIMT path: row-major, the layers side by side).
 int prepare_cond(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, DenoiserBufs& b) {
-  if (b.tc) {
-    RUN(split_planes(c, cond_g, 256, s.rows, 256, 1.0f, b.ch, b.cl));
-    if (!b.condpre) return 0;
-    GemmTC g;  // all L conditioner projections at once: [rows, 256] x [256, L*2C], once per sampler call
-    g.A_hi = b.ch; g.A_lo = b.cl; g.rows_total = s.rows; g.w = &d.cond_all_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-    g.e.mode = EPI_GENERIC; g.e.out = b.condpre; g.e.ldo = d.L * 2 * d.C;
-    g.e.out_nb = 2 * d.C; g.e.out_bs = (int64_t)s.rows * 2 * d.C;  // layer-major: row pitch 2C floats instead of L * 2C
-    return conv_gemm_tc(c, g);
-  }
+  if (b.tc) return hoist_cond_tc(c, d, s, cond_g, b.ch, b.cl, b.condpre);
   ConvGemm g = make_gemm(d.cond_all, s, cond_g, 256);
   g.e.out = b.condall; g.e.ldo = d.L * 2 * d.C;
   return conv_gemm(c, g);
@@ -661,13 +661,16 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
   float* xm = alloc_rows(c, s, 80);
   float* x = alloc_rows(c, s, C);
   float* skip = alloc_rows(c, s, C);
-  __half* pl[12];
-  const int pcols[6] = {128, C, C, 256, C, C};  // x80, y, z, cond, skip, s
-  for (int i = 0; i < 6; ++i) {
+  __half* pl[10];
+  const int pcols[5] = {128, C, C, C, C};  // x80, y, z, skip, s
+  for (int i = 0; i < 5; ++i) {
     pl[2 * i] = alloc_half_rows(c, s, pcols[i]);
     pl[2 * i + 1] = alloc_half_rows(c, s, pcols[i]);
   }
-  const int nmaps = 12 + 2 + 6 * L + 4;
+  __half* ch = alloc_half_rows(c, s, 256);
+  __half* cl = alloc_half_rows(c, s, 256);
+  float* condpre = alloc_rows(c, s, L * 2 * C, false);
+  const int nmaps = 10 + 2 + 4 * L + 4;
   const int nph = T * (2 * L + 3);
   CUtensorMap* maps_dev = c.alloc<CUtensorMap>((size_t)nmaps);
   SPhase* ph_dev = c.alloc<SPhase>((size_t)nph);
@@ -676,32 +679,20 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
   const size_t per = (size_t)s.total * 80;
   RUN(mel_init(c, m, s, coarse_g, noise, seed, xm));
   RUN(x80_planes(c, xm, s.rows, pl[0], pl[1]));
-  RUN(split_planes(c, cond_g, 256, s.rows, 256, 1.0f, pl[6], pl[7]));
-  // step-invariant conditioner projection of all L layers, once per call (one per-launch GEMM): the gate phases then
-  // contract K = 3C instead of 3C + 256 and add it in the epilogue
-  float* condpre = nullptr;
-  if (m.cond_hoist && d.cond_all_tc.ok) {
-    condpre = alloc_rows(c, s, L * 2 * C, false);
-    WS_OK(c);
-    GemmTC g;
-    g.A_hi = pl[6]; g.A_lo = pl[7]; g.rows_total = s.rows; g.w = &d.cond_all_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-    g.e.mode = EPI_GENERIC; g.e.out = condpre; g.e.ldo = L * 2 * C;
-    g.e.out_nb = 2 * C; g.e.out_bs = (int64_t)s.rows * 2 * C;
-    RUN(conv_gemm_tc(c, g));
-  }
+  // one per-launch GEMM: the gate phases contract K = 3C and add the conditioner projection in the epilogue
+  RUN(hoist_cond_tc(c, d, s, cond_g, ch, cl, condpre));
   if (!c.dry) {
     std::vector<CUtensorMap> maps((size_t)nmaps);
-    for (int i = 0; i < 6; ++i) {
+    for (int i = 0; i < 5; ++i) {
       if (make_act_map(&maps[2 * i], pl[2 * i], s.rows, pcols[i], 128 / CS)) return -1;
       if (make_act_map(&maps[2 * i + 1], pl[2 * i + 1], s.rows, pcols[i], 128 / CS)) return -1;
     }
     auto put = [&](int idx, const ConvTC& w) { maps[idx] = w.tm_hi[1]; maps[idx + 1] = w.tm_lo[1]; };
-    const int W_IN = 12, W_L0 = 14, W_SKIP = 14 + 6 * L, W_OUT = W_SKIP + 2;
+    const int W_IN = 10, W_L0 = 12, W_SKIP = W_L0 + 4 * L, W_OUT = W_SKIP + 2;
     put(W_IN, d.in_tc);
     for (int l = 0; l < L; ++l) {
-      put(W_L0 + 6 * l, d.layers[l].dil_tc);
-      put(W_L0 + 6 * l + 2, d.layers[l].cond_tc);
-      put(W_L0 + 6 * l + 4, d.layers[l].outp_tc);
+      put(W_L0 + 4 * l, d.layers[l].dil_tc);
+      put(W_L0 + 4 * l + 2, d.layers[l].outp_tc);
     }
     put(W_SKIP, d.skip_tc);
     put(W_OUT, d.out_tc);
@@ -711,7 +702,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
       const float* dt = d.dtab + (size_t)t * L * C;
       SPhase z;
       memset(&z, 0, sizeof(z));
-      z.a2 = -1; z.taps = 1; z.dil = 1; z.beta = 1.0f; z.sync_after = 1;
+      z.taps = 1; z.dil = 1; z.beta = 1.0f; z.sync_after = 1;
       {  // input_projection + ReLU ; y = x + step bias of layer 0
         SPhase q = z;
         q.a1 = 0; q.w1 = W_IN; q.kchunks = 2; q.N = C; q.NT = C / 64; q.mode = SP_INPROJ; q.bias = d.in_proj.bias;
@@ -719,29 +710,29 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
         ph[k++] = q;
       }
       for (int l = 0; l < L; ++l) {
-        SPhase a = z;  // dilated conv (3 taps of y) + conditioner (cond) -> gate -> z planes
-        a.a1 = 2; a.a2 = 6; a.w1 = W_L0 + 6 * l; a.w2 = W_L0 + 6 * l + 2; a.taps = 3; a.kchunks = C / 64; a.kchunks2 = 4;
+        SPhase a = z;  // dilated conv (3 taps of y) + hoisted conditioner projection -> gate -> z planes
+        a.a1 = 2; a.w1 = W_L0 + 4 * l; a.taps = 3; a.kchunks = C / 64;
         a.dil = d.layers[l].dil_tc.dil; a.center = 1; a.N = 2 * C; a.NT = 2 * C / 64; a.mode = SP_GATE;
         a.bias = d.layers[l].bias_gate_tc; a.oh = pl[4]; a.ol = pl[5]; a.ldh = C;
-        if (condpre) { a.a2 = -1; a.kchunks2 = 0; a.add = condpre + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C; }
+        a.add = condpre + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C;
         ph[k++] = a;
         SPhase b = z;  // 1x1 output projection -> residual stream, next layer's input planes, skip sum
-        b.a1 = 4; b.w1 = W_L0 + 6 * l + 4; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
+        b.a1 = 4; b.w1 = W_L0 + 4 * l + 2; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
         b.bias = d.layers[l].outp.bias; b.res = x; b.ld_res = C; b.out = x; b.ldo = C; b.beta = 0.70710678118654752440f;
         if (l + 1 < L) { b.oh = pl[2]; b.ol = pl[3]; b.ldh = C; b.vec2 = dt + (size_t)(l + 1) * C; }
         b.skip = skip; b.ld_skip = C; b.C = C; b.skip_init = (l == 0);
-        if (l == L - 1) { b.sh = pl[8]; b.sl = pl[9]; }
+        if (l == L - 1) { b.sh = pl[6]; b.sl = pl[7]; }
         ph[k++] = b;
       }
       {  // skip_projection (1/sqrt(L) folded into the weights) + ReLU -> s planes
         SPhase q = z;
-        q.a1 = 8; q.w1 = W_SKIP; q.kchunks = C / 64; q.N = C; q.NT = C / 64; q.mode = SP_SKIPPROJ; q.bias = d.skip_proj.bias;
-        q.oh = pl[10]; q.ol = pl[11]; q.ldh = C;
+        q.a1 = 6; q.w1 = W_SKIP; q.kchunks = C / 64; q.N = C; q.NT = C / 64; q.mode = SP_SKIPPROJ; q.bias = d.skip_proj.bias;
+        q.oh = pl[8]; q.ol = pl[9]; q.ldh = C;
         ph[k++] = q;
       }
       {  // output_projection -> eps ; fused DDPM posterior step on x_t
         SPhase q = z;
-        q.a1 = 10; q.w1 = W_OUT; q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE; q.bias = d.out_bias_pad;
+        q.a1 = 8; q.w1 = W_OUT; q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE; q.bias = d.out_bias_pad;
         q.out = xm; q.ldo = 80; q.oh = pl[0]; q.ol = pl[1]; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
         q.noise = noise ? noise + per * (size_t)(T - t) : nullptr; q.seed = seed; q.stream_id = 1001 + (uint64_t)t; q.n_valid = 80;
         q.no_clip = m.mel_decoder == SSB_MEL_DECODER_PRODIFF;
@@ -764,53 +755,46 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
                       const Seq* host_seq) {
   const Denoiser& d = m.melnet;
   SSB_CHECK(d.T > 0, "mel schedule not set: call ssb_model_set_schedule(which=0)");
-  // Utterances are independent, so the T x L loop can run per GROUP of consecutive utterances (a contiguous slice of the
-  // guard-banded layout: the sub-batch simply aliases the big buffers).  Two users, production (Philox) mode only - the
-  // injected-noise tensors are strided by the whole batch; each group gets its own seed:
-  //  * SSB_MEL_GROUP_FRAMES=<n> (experiment, DESIGN.md): groups of ~n frames whose working set stays L2-resident;
-  //  * ssb_model_set_persistent_groups(1): groups of <= 48 row tiles, each run by the single-launch persistent kernel
-  //    (BASELINE.json configs[4]: persistent-kernel vs per-step-launch at batch 64).
-  if (host_seq && !noise && !c.dry) {
-    const char* ge = getenv("SSB_MEL_GROUP_FRAMES");
-    const long gf = ge ? atol(ge) : 0;
-    const bool by_tiles = m.persistent_groups && m.persistent && s.ntiles > 48;
-    if (by_tiles || (gf > 0 && host_seq->total > gf + gf / 2)) {
-      int b0 = 0;
-      int64_t tight0 = 0;
-      int gi = 0;
-      auto tiles_of = [&](int b) { return (host_seq->len[b] + TILE_M - 1) / TILE_M; };
-      while (b0 < host_seq->B) {
-        int b1 = b0;
-        int64_t fr = 0, nt = 0;
-        while (b1 < host_seq->B &&
-               (b1 == b0 || (by_tiles ? nt + tiles_of(b1) <= 48 : fr + host_seq->len[b1] <= gf))) {
-          nt += tiles_of(b1);
-          fr += host_seq->len[b1++];
-        }
-        std::vector<int32_t> offs((size_t)(b1 - b0) + 1, 0);
-        for (int b = b0; b < b1; ++b) offs[(size_t)(b - b0) + 1] = offs[(size_t)(b - b0)] + host_seq->len[b];
-        Seq q;
-        q.build(offs.data(), b1 - b0);
-        const size_t mkg = c.mark();
-        SeqDev sg;
-        RUN(upload_layout(c, q, 1, &sg));
-        const int64_t row_off = (int64_t)host_seq->rs[b0] - GUARD;  // the sub-layout's row 0 inside the big buffers
-        RUN(run_mel_diffusion(c, m, sg, cond_g + row_off * 256, coarse_g ? coarse_g + row_off * 80 : nullptr, nullptr,
-                              seed + 0x9E3779B97F4A7C15ull * (uint64_t)gi, mel_tight + tight0 * 80, nullptr));
-        c.release(mkg);
-        tight0 += fr;
-        b0 = b1;
-        ++gi;
+  // ssb_model_set_persistent_groups(1): utterances are independent, so the T x L loop runs per GROUP of consecutive
+  // utterances of <= 48 row tiles (a contiguous slice of the guard-banded layout: the sub-batch simply aliases the big
+  // buffers), each by the single-launch persistent kernel (BASELINE.json configs[4]: persistent-kernel vs per-step-launch
+  // at batch 64).  Production (Philox) mode only - the injected-noise tensors are strided by the whole batch; each group
+  // gets its own seed.
+  if (host_seq && !noise && !c.dry && m.persistent_groups && m.persistent && s.ntiles > 48) {
+    int b0 = 0;
+    int64_t tight0 = 0;
+    int gi = 0;
+    auto tiles_of = [&](int b) { return (host_seq->len[b] + TILE_M - 1) / TILE_M; };
+    while (b0 < host_seq->B) {
+      int b1 = b0;
+      int64_t fr = 0, nt = 0;
+      while (b1 < host_seq->B && (b1 == b0 || nt + tiles_of(b1) <= 48)) {
+        nt += tiles_of(b1);
+        fr += host_seq->len[b1++];
       }
-      return 0;
+      std::vector<int32_t> offs((size_t)(b1 - b0) + 1, 0);
+      for (int b = b0; b < b1; ++b) offs[(size_t)(b - b0) + 1] = offs[(size_t)(b - b0)] + host_seq->len[b];
+      Seq q;
+      q.build(offs.data(), b1 - b0);
+      const size_t mkg = c.mark();
+      SeqDev sg;
+      RUN(upload_layout(c, q, 1, &sg));
+      const int64_t row_off = (int64_t)host_seq->rs[b0] - GUARD;  // the sub-layout's row 0 inside the big buffers
+      RUN(run_mel_diffusion(c, m, sg, cond_g + row_off * 256, coarse_g ? coarse_g + row_off * 80 : nullptr, nullptr,
+                            seed + 0x9E3779B97F4A7C15ull * (uint64_t)gi, mel_tight + tight0 * 80, nullptr));
+      c.release(mkg);
+      tight0 += fr;
+      b0 = b1;
+      ++gi;
     }
+    return 0;
   }
   if (m.persistent && denoiser_tc_ok(m, d) && d.in_tc.ok && d.skip_tc.ok && d.out_tc.ok && s.ntiles <= 48 &&
       sampler_tc_max_ctas() > 0)
     return run_mel_diffusion_persistent(c, m, s, cond_g, coarse_g, noise, seed, mel_tight);
   const size_t mk = c.mark();
   DenoiserBufs b;
-  RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b, m.cond_hoist));
+  RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
   float* xm = alloc_rows(c, s, 80);
   WS_OK(c);
   RUN(prepare_cond(c, d, s, cond_g, b));
@@ -839,7 +823,7 @@ int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float*
   SSB_CHECK(interval >= 1 && interval < d.T, "plms: interval (pndm_speedup) must be in [1, T)");
   const size_t mk = c.mark();
   DenoiserBufs b;
-  RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b, m.cond_hoist));
+  RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
   float* xm = alloc_rows(c, s, 80);
   float* xp = alloc_rows(c, s, 80);
   float* hist[3] = {alloc_rows(c, s, 80), alloc_rows(c, s, 80), alloc_rows(c, s, 80)};
@@ -897,20 +881,19 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
   const int C = d0.C, L = d0.L, T = d0.T;
   const int CS = 2;
   const size_t mk = c.mark();
-  const int NA = 10;           // activation maps per net: y, z, cond, skip, s (hi/lo)
-  const int NW = 6 * L + 4;    // weight maps per net
+  const int NA = 8;            // activation maps per net: y, z, skip, s (hi/lo)
+  const int NW = 4 * L + 4;    // weight maps per net: dil, outp per layer, skip, out (hi/lo)
   const int nmaps = 2 * (NA + NW);
   const int per_step = 2 * L + 2;
   const int nph = 2 * T * per_step;
-  float* x[2]; float* skip[2]; __half* pl[2][10];
-  const int pcols[5] = {C, C, 256, C, C};
+  float* x[2]; float* skip[2]; float* condpre[2]; __half* pl[2][8]; __half* cpl[2][2];
   for (int n = 0; n < 2; ++n) {
     x[n] = alloc_rows(c, s, C);
     skip[n] = alloc_rows(c, s, C);
-    for (int i = 0; i < 5; ++i) {
-      pl[n][2 * i] = alloc_half_rows(c, s, pcols[i]);
-      pl[n][2 * i + 1] = alloc_half_rows(c, s, pcols[i]);
-    }
+    for (int i = 0; i < 8; ++i) pl[n][i] = alloc_half_rows(c, s, C);
+    cpl[n][0] = alloc_half_rows(c, s, 256);
+    cpl[n][1] = alloc_half_rows(c, s, 256);
+    condpre[n] = alloc_rows(c, s, L * 2 * C, false);
   }
   CUtensorMap* maps_dev = c.alloc<CUtensorMap>((size_t)nmaps);
   SPhase* ph_dev = c.alloc<SPhase>((size_t)nph);
@@ -922,19 +905,7 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
     const uint64_t sbase = 2000 + (uint64_t)n * 100000;
     RUN(f0_init(c, s, z[n], uv[n], gnoise[n], seed, sbase));
     RUN(ddiff_input(c, s, z[n], uv[n], d.in_w, d.in_b, d.uv_emb, d.dtab + (size_t)(T - 1) * L * C, x[n], nullptr, C, pl[n][0], pl[n][1]));
-    RUN(split_planes(c, n == 0 ? cond0 : cond1, 256, s.rows, 256, 1.0f, pl[n][4], pl[n][5]));
-  }
-  float* condpre[2] = {nullptr, nullptr};  // hoisted conditioner projections (see run_mel_diffusion_persistent)
-  if (m.cond_hoist && m.f0net[0].cond_all_tc.ok && m.f0net[1].cond_all_tc.ok) {
-    for (int n = 0; n < 2; ++n) {
-      condpre[n] = alloc_rows(c, s, L * 2 * C, false);
-      WS_OK(c);
-      GemmTC g;
-      g.A_hi = pl[n][4]; g.A_lo = pl[n][5]; g.rows_total = s.rows; g.w = &m.f0net[n].cond_all_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-      g.e.mode = EPI_GENERIC; g.e.out = condpre[n]; g.e.ldo = L * 2 * C;
-      g.e.out_nb = 2 * C; g.e.out_bs = (int64_t)s.rows * 2 * C;
-      RUN(conv_gemm_tc(c, g));
-    }
+    RUN(hoist_cond_tc(c, d, s, n == 0 ? cond0 : cond1, cpl[n][0], cpl[n][1], condpre[n]));
   }
   if (!c.dry) {
     std::vector<CUtensorMap> maps((size_t)nmaps);
@@ -949,16 +920,13 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
     for (int n = 0; n < 2; ++n) {
       const Denoiser& d = m.f0net[n];
       const int MB = n * (NA + NW);
-      for (int i = 0; i < 5; ++i) {
-        if (make_act_map(&maps[MB + 2 * i], pl[n][2 * i], s.rows, pcols[i], 128 / CS)) return -1;
-        if (make_act_map(&maps[MB + 2 * i + 1], pl[n][2 * i + 1], s.rows, pcols[i], 128 / CS)) return -1;
-      }
+      for (int i = 0; i < NA; ++i)
+        if (make_act_map(&maps[MB + i], pl[n][i], s.rows, C, 128 / CS)) return -1;
       auto put = [&](int idx, const ConvTC& w) { maps[idx] = w.tm_hi[1]; maps[idx + 1] = w.tm_lo[1]; };
-      const int W_L0 = MB + NA, W_SKIP = W_L0 + 6 * L, W_OUT = W_SKIP + 2;
+      const int W_L0 = MB + NA, W_SKIP = W_L0 + 4 * L, W_OUT = W_SKIP + 2;
       for (int l = 0; l < L; ++l) {
-        put(W_L0 + 6 * l, d.layers[l].dil_tc);
-        put(W_L0 + 6 * l + 2, d.layers[l].cond_tc);
-        put(W_L0 + 6 * l + 4, d.layers[l].outp_tc);
+        put(W_L0 + 4 * l, d.layers[l].dil_tc);
+        put(W_L0 + 4 * l + 2, d.layers[l].outp_tc);
       }
       put(W_SKIP, d.skip_tc);
       put(W_OUT, d.out_tc);
@@ -968,34 +936,34 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
         const float* dt = d.dtab + (size_t)t * L * C;
         SPhase zp;
         memset(&zp, 0, sizeof(zp));
-        zp.a2 = -1; zp.taps = 1; zp.dil = 1; zp.beta = 1.0f; zp.sync_after = (n == 1);
+        zp.taps = 1; zp.dil = 1; zp.beta = 1.0f; zp.sync_after = (n == 1);
         // entry k of step ti for net n sits at ((ti * per_step + k) * 2 + n)
         size_t k = 0;
         auto slot = [&](size_t kk) -> SPhase& { return ph[((size_t)ti * per_step + kk) * 2 + n]; };
         for (int l = 0; l < L; ++l) {
           SPhase a = zp;
-          a.a1 = MB + 0; a.a2 = MB + 4; a.w1 = W_L0 + 6 * l; a.w2 = W_L0 + 6 * l + 2; a.taps = 3; a.kchunks = C / 64; a.kchunks2 = 4;
+          a.a1 = MB + 0; a.w1 = W_L0 + 4 * l; a.taps = 3; a.kchunks = C / 64;
           a.dil = d.layers[l].dil_tc.dil; a.center = 1; a.N = 2 * C; a.NT = 2 * C / 64; a.mode = SP_GATE;
           a.bias = d.layers[l].bias_gate_tc; a.oh = pl[n][2]; a.ol = pl[n][3]; a.ldh = C;
-          if (condpre[n]) { a.a2 = -1; a.kchunks2 = 0; a.add = condpre[n] + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C; }
+          a.add = condpre[n] + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C;
           slot(k++) = a;
           SPhase b = zp;
-          b.a1 = MB + 2; b.w1 = W_L0 + 6 * l + 4; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
+          b.a1 = MB + 2; b.w1 = W_L0 + 4 * l + 2; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
           b.bias = d.layers[l].outp.bias; b.res = x[n]; b.ld_res = C; b.out = x[n]; b.ldo = C; b.beta = 0.70710678118654752440f;
           if (l + 1 < L) { b.oh = pl[n][0]; b.ol = pl[n][1]; b.ldh = C; b.vec2 = dt + (size_t)(l + 1) * C; }
           b.skip = skip[n]; b.ld_skip = C; b.C = C; b.skip_init = (l == 0);
-          if (l == L - 1) { b.sh = pl[n][6]; b.sl = pl[n][7]; }
+          if (l == L - 1) { b.sh = pl[n][4]; b.sl = pl[n][5]; }
           slot(k++) = b;
         }
         {
           SPhase q = zp;
-          q.a1 = MB + 6; q.w1 = W_SKIP; q.kchunks = C / 64; q.N = d.skip_tc.N; q.NT = d.skip_tc.N / 64; q.mode = SP_SKIPPROJ;
-          q.bias = d.skip_bias_pad; q.oh = pl[n][8]; q.ol = pl[n][9]; q.ldh = C; q.n_valid = C;
+          q.a1 = MB + 4; q.w1 = W_SKIP; q.kchunks = C / 64; q.N = d.skip_tc.N; q.NT = d.skip_tc.N / 64; q.mode = SP_SKIPPROJ;
+          q.bias = d.skip_bias_pad; q.oh = pl[n][6]; q.ol = pl[n][7]; q.ldh = C; q.n_valid = C;
           slot(k++) = q;
         }
         {
           SPhase q = zp;
-          q.a1 = MB + 8; q.w1 = W_OUT; q.kchunks = C / 64; q.N = d.out_tc.N; q.NT = d.out_tc.N / 64; q.mode = SP_F0_SAMPLE;
+          q.a1 = MB + 6; q.w1 = W_OUT; q.kchunks = C / 64; q.N = d.out_tc.N; q.NT = d.out_tc.N / 64; q.mode = SP_F0_SAMPLE;
           q.bias = d.out_bias_pad; q.out = z[n]; q.uv = uv[n]; q.clip_lo = lo; q.clip_hi = hi;
           q.tab = d.gtab + (size_t)t * 8; q.tab2 = d.mtab + (size_t)t * 8; q.tstep = t; q.log_eps = m.log_eps;
           q.noise = gnoise[n] ? gnoise[n] + per * (size_t)(T - t) : nullptr;
@@ -1028,40 +996,12 @@ bool f0_pair_persistent_ok(const Model& m, const SeqDev& s) {
 
 // a13+a14: GaussianMultinomialDiffusion.sample (gaussian_multinomial_diffusion.py:921-942)
 int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const float* cond_g, const float* lo,
-                     const float* hi, const float* gnoise, const float* unoise, uint64_t seed, float* z, int32_t* uv,
-                     const Seq* host_seq) {
+                     const float* hi, const float* gnoise, const float* unoise, uint64_t seed, float* z, int32_t* uv) {
   const Denoiser& d = m.f0net[which];
   SSB_CHECK(d.T > 0, "f0 schedule not set: call ssb_model_set_schedule(which=1)");
-  // EXPERIMENTAL utterance grouping, off unless SSB_F0_GROUP_FRAMES=<n> is set: see run_mel_diffusion.
-  if (host_seq && !gnoise && !unoise && !c.dry) {
-    const char* ge = getenv("SSB_F0_GROUP_FRAMES");
-    const long gf = ge ? atol(ge) : 0;
-    if (gf > 0 && host_seq->total > gf + gf / 2) {
-      int b0 = 0, gi = 0;
-      while (b0 < host_seq->B) {
-        int b1 = b0;
-        int64_t fr = 0;
-        while (b1 < host_seq->B && (b1 == b0 || fr + host_seq->len[b1] <= gf)) fr += host_seq->len[b1++];
-        std::vector<int32_t> offs((size_t)(b1 - b0) + 1, 0);
-        for (int b = b0; b < b1; ++b) offs[(size_t)(b - b0) + 1] = offs[(size_t)(b - b0)] + host_seq->len[b];
-        Seq q;
-        q.build(offs.data(), b1 - b0);
-        const size_t mkg = c.mark();
-        SeqDev sg;
-        RUN(upload_layout(c, q, 1, &sg));
-        const int64_t ro = (int64_t)host_seq->rs[b0] - GUARD;  // all operands here are guard-banded [rows, ld] buffers
-        RUN(run_f0_diffusion(c, m, which, sg, cond_g + ro * 256, lo + ro, hi + ro, nullptr, nullptr,
-                             seed + 0x9E3779B97F4A7C15ull * (uint64_t)gi, z + ro, uv + ro, nullptr));
-        c.release(mkg);
-        b0 = b1;
-        ++gi;
-      }
-      return 0;
-    }
-  }
   const size_t mk = c.mark();
   DenoiserBufs b;
-  RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b, m.cond_hoist));
+  RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
   RUN(prepare_cond(c, d, s, cond_g, b));
   const int T = d.T;
   const size_t per = (size_t)s.total;

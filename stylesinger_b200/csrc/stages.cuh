@@ -13,9 +13,9 @@ int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const 
               const float* reff0_g, float* style, int32_t* codes, float* rq_in_out);
 struct DenoiserBufs {
   float *x, *y, *zg, *skip, *sbuf, *head, *condall;
-  float* condpre;             // tensor-core path with the hoisted conditioner: [rows, L*2C] fp32 pre-activation addends
+  float* condpre;             // tensor-core path: hoisted conditioner projection, [rows, 2C] fp32 pre-activation addends per layer
   __half *yh, *yl, *zh, *zl;  // tensor-core path: fp16 hi/lo planes of y = x + step bias and of the gate output
-  __half *ch, *cl;            // tensor-core path: fp16 hi/lo planes of the conditioner [rows,256]
+  __half *ch, *cl;            // tensor-core path: fp16 hi/lo planes of the conditioner [rows,256] (A of the hoisted projection)
   __half *skh, *skl, *sh, *sl;  // tensor-core heads: planes of the skip sum and of relu(skip_proj)
   __half *x80h, *x80l;          // mel net, tensor-core in_proj: planes of x_t padded to 128 columns
   bool tc_heads;
@@ -24,18 +24,17 @@ struct DenoiserBufs {
   bool tc;
 };
 bool denoiser_tc_ok(const Model& m, const Denoiser& d);
-int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, DenoiserBufs* b, bool hoist = false);
+int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, DenoiserBufs* b);
 int prepare_cond(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, DenoiserBufs& b);
 int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const float* x80, DenoiserBufs& b);
 int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBufs& b);
-// host_seq (optional): the host-side layout of `s`; enables the experimental utterance grouping (SSB_MEL_GROUP_FRAMES)
+// host_seq (optional): the host-side layout of `s`; needed for the utterance grouping of ssb_model_set_persistent_groups
 int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                       const float* noise, uint64_t seed, float* mel_tight, const Seq* host_seq = nullptr);
 int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                            const float* q_noise, uint64_t seed, int interval, float* mel_tight);
 int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const float* cond_g, const float* lo,
-                     const float* hi, const float* gnoise, const float* unoise, uint64_t seed, float* z, int32_t* uv,
-                     const Seq* host_seq = nullptr);  // host_seq: see run_mel_diffusion (SSB_F0_GROUP_FRAMES)
+                     const float* hi, const float* gnoise, const float* unoise, uint64_t seed, float* z, int32_t* uv);
 int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1,
                                      const float* lo, const float* hi, const float* const gnoise[2],
                                      const float* const unoise[2], uint64_t seed, float* const z[2], int32_t* const uv[2]);

@@ -180,10 +180,6 @@ class AcousticModel:
         """Single-launch persistent sampler kernel for small batches (True) vs one launch per GEMM (False)."""
         return bool(lib.ssb_model_set_persistent(self._h, 1 if enable else 0))
 
-    def set_cond_hoist(self, enable=True):
-        """Conditioner projection hoisted out of the T loop (default) vs contracted inside every layer GEMM."""
-        return bool(lib.ssb_model_set_cond_hoist(self._h, 1 if enable else 0))
-
     def set_persistent_groups(self, enable=True):
         """Large batches: run the mel sampler as one persistent launch per group of <= 48 row tiles (default off)."""
         return bool(lib.ssb_model_set_persistent_groups(self._h, 1 if enable else 0))

@@ -52,6 +52,15 @@ def test_product_never_imports_oracle():
                 assert "import oracle" not in txt and "from oracle" not in txt, f
 
 
+def test_library_reads_no_environment():
+    """Every execution choice of the library is derived from the input or the platform, or set through the C ABI (where
+    tests can reach it): no environment variable selects a code path."""
+    csrc = os.path.join(REPO, "stylesinger_b200", "csrc")
+    for f in sorted(os.listdir(csrc)):
+        txt = open(os.path.join(csrc, f)).read()
+        assert not re.search(r"\bgetenv\s*\(", txt), f"{f} calls getenv"
+
+
 def test_front_end_argument_checks_need_no_gpu():
     """Geometry / argument validation of the f3 entry points happens before any CUDA call: same error behaviour on any host."""
     import numpy as np

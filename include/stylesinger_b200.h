@@ -11,13 +11,16 @@
  *  - all DEVICE tensors are fp32 (or int32) row-major and "tight packed": a batch of B utterances
  *    of lengths L_b is one [sum L_b, C] matrix; `*_offsets` are HOST int32 arrays of B+1 prefix
  *    sums.  Every utterance is processed with true-length (the reference's B=1) semantics —
- *    results do not depend on batch composition.
+ *    with injected noise, results do not depend on batch composition.
  *  - the caller owns every device buffer including the workspace (`*_workspace_bytes`); entry
  *    points enqueue on `stream`, never allocate device memory and never synchronise — except
  *    ssb_model_create / ssb_vocoder_create / ssb_model_set_schedule, which own the packed weights.
  *  - return 0 on success, negative on error with a message in ssb_last_error() (thread-local).
  *  - noise: NULL noise pointers select the in-kernel counter-based generator (Philox, `seed`);
  *    non-NULL pointers inject the noise explicitly (parity mode; SURVEY.md A.10 draw order).
+ *    Philox draws are indexed by the tight row of the call (and the persistent mel groups re-seed
+ *    each group), so in that mode an utterance's noise depends on the batch it is in.  The stream
+ *    plan is documented in csrc/philox.cuh.
  */
 #ifndef STYLESINGER_B200_H
 #define STYLESINGER_B200_H

@@ -360,7 +360,7 @@ __global__ void k_f0_p_sample(const int4* utt, F0StepArgs a) {
   float x0 = a.gtab[0] * zt - a.gtab[1] * o[0];
   x0 = fmaxf(fminf(x0, a.hi[r]), a.lo[r]);
   const float mean = a.gtab[2] * x0 + a.gtab[3] * zt;
-  a.z[r] = mean + a.gtab[4] * noise_n(a.gnoise, ti, a.seed, a.stream_id);
+  a.z[r] = mean + a.gtab[4] * noise_n(a.gnoise, ti, a.seed, a.gauss_stream);
   // multinomial half (p_pred / q_posterior, :374-413)
   const float l0a = o[1], l0b = o[2];
   const float mx = fmaxf(l0a, l0b);
@@ -379,8 +379,8 @@ __global__ void k_f0_p_sample(const int4* utt, F0StepArgs a) {
   const float m2 = fmaxf(u0, u1);
   const float lse2 = m2 + logf(expf(u0 - m2) + expf(u1 - m2));  // torch.logsumexp
   const float p0 = u0 - lse2, p1 = u1 - lse2;
-  const float r0 = noise_u(a.unoise, ti * 2 + 0, a.seed, a.stream_id + 1);
-  const float r1 = noise_u(a.unoise, ti * 2 + 1, a.seed, a.stream_id + 1);
+  const float r0 = noise_u(a.unoise, ti * 2 + 0, a.seed, a.unif_stream);
+  const float r1 = noise_u(a.unoise, ti * 2 + 1, a.seed, a.unif_stream);
   const float g0 = -logf(-logf(r0 + 1e-30f) + 1e-30f);
   const float g1 = -logf(-logf(r1 + 1e-30f) + 1e-30f);
   a.uv[r] = (g1 + p1) > (g0 + p0) ? 1 : 0;  // argmax, ties -> 0
@@ -484,7 +484,7 @@ __global__ void k_nsf_phase(const int4* utt1, const int4* utt256, const float* f
   __shared__ double sh[16];
   const int N = u2.y;
   float ini = 0.f;
-  if (h > 0) ini = rand_ini ? rand_ini[b * 9 + h] : philox_uniform(seed, 0x5151ull + b, (uint64_t)h);
+  if (h > 0) ini = rand_ini ? rand_ini[b * 9 + h] : philox_uniform(seed, stream_voc_ini(b), (uint64_t)h);
   double carry1 = 0.0, carry2 = 0.0;
   float prev_over = 0.f;  // tmp_over_one of the previous sample
   for (int n0 = 0; n0 < N; n0 += 256) {
@@ -533,7 +533,7 @@ __global__ void k_nsf_merge(const int4* utt1, const int4* utt256, const float* f
 #pragma unroll
   for (int h = 0; h < 9; ++h) {
     const float s = sines[ti * 9 + h] * 0.1f;
-    const float nz = namp * (noise ? noise[ti * 9 + h] : philox_normal(seed, 0x7171ull, (uint64_t)(ti * 9 + h)));
+    const float nz = namp * (noise ? noise[ti * 9 + h] : philox_normal(seed, stream_voc_src(), (uint64_t)(ti * 9 + h)));
     acc = fmaf(s * uv + nz, lw[h], acc);
   }
   har[(int64_t)u2.x + n] = tanhf(acc);

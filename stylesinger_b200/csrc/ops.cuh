@@ -113,7 +113,7 @@ struct F0StepArgs {
   const float* mtab = nullptr;   // device, 8 floats for this t
   int t = 0;
   float log_eps = 0.f;           // fp32 log(1e-30)
-  uint64_t seed = 0, stream_id = 0;
+  uint64_t seed = 0, gauss_stream = 0, unif_stream = 0;  // Philox streams of this step (philox.cuh)
 };
 int f0_p_sample(Ctx&, const SeqDev&, const F0StepArgs&);
 int f0_init(Ctx&, const SeqDev&, float* z, int32_t* uv, const float* gnoise, uint64_t seed, uint64_t stream_id);

@@ -170,8 +170,8 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
     const float m2 = fmaxf(u0, u1);
     const float lse2 = m2 + logf(expf(u0 - m2) + expf(u1 - m2));
     const float p0 = u0 - lse2, p1 = u1 - lse2;
-    const float r0 = e.noise2 ? __ldg(e.noise2 + ti * 2) : philox_uniform(e.seed, e.stream_id + 1, (uint64_t)(ti * 2));
-    const float r1 = e.noise2 ? __ldg(e.noise2 + ti * 2 + 1) : philox_uniform(e.seed, e.stream_id + 1, (uint64_t)(ti * 2 + 1));
+    const float r0 = e.noise2 ? __ldg(e.noise2 + ti * 2) : philox_uniform(e.seed, e.stream2, (uint64_t)(ti * 2));
+    const float r1 = e.noise2 ? __ldg(e.noise2 + ti * 2 + 1) : philox_uniform(e.seed, e.stream2, (uint64_t)(ti * 2 + 1));
     const float g0 = -logf(-logf(r0 + 1e-30f) + 1e-30f);
     const float g1 = -logf(-logf(r1 + 1e-30f) + 1e-30f);
     const int cls = (g1 + p1) > (g0 + p0) ? 1 : 0;

@@ -32,7 +32,8 @@ struct SPhase {
   __half* sl;
   const float* tab;    // MEL_SAMPLE: 8 schedule scalars of this step
   const float* noise;  // MEL_SAMPLE: tight [total, 80] noise of this step, or null (Philox)
-  unsigned long long seed, stream_id;
+  unsigned long long seed, stream_id;  // Philox stream of the Gaussian draws (philox.cuh)
+  unsigned long long stream2;          // F0_SAMPLE: Philox stream of the uniform draws
   int n_valid;         // MEL_SAMPLE / SKIPPROJ: valid output columns
   int sync_after;      // 1: grid barrier after this entry; 0: the next entry is independent (e.g. the other F0 net)
   int goff;            // tile-group rotation: group g is processed by cluster (g + goff) % nclusters

@@ -1,6 +1,7 @@
 // Stage drivers: compose the kernels into the reference's modules (one function per SURVEY.md §8a group).
 #include <string.h>
 
+#include "philox.cuh"
 #include "sampler_tc.cuh"
 #include "stages.cuh"
 
@@ -634,15 +635,15 @@ int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const f
 }
 
 // x_T of the mel sampler.  DiffSinger: q_sample(norm_spec(coarse), T-1) (shallow_diffusion_tts.py:298-302); ProDiff:
-// randn (prodiff.py:214-216), no coarse mel.  Both draw block 0 of the injected noise, or Philox stream 1000.
+// randn (prodiff.py:214-216), no coarse mel.  Both draw block 0 of the injected noise, or Philox stream_mel_xt().
 static int mel_init(Ctx& c, const Model& m, const SeqDev& s, const float* coarse_g, const float* noise, uint64_t seed,
                     float* xm) {
   const Denoiser& d = m.melnet;
   const int T = d.T;
   if (m.mel_decoder == SSB_MEL_DECODER_PRODIFF)
-    return mel_q_sample(c, s, nullptr, 80, noise, nullptr, nullptr, 0.f, 0.f, xm, 80, seed, 1000);
+    return mel_q_sample(c, s, nullptr, 80, noise, nullptr, nullptr, 0.f, 0.f, xm, 80, seed, stream_mel_xt());
   const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 6];
-  return mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, 1000);
+  return mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, stream_mel_xt());
 }
 // x_0 -> mel_out.  DiffSinger: denorm_spec (shallow_diffusion_tts.py:305,274-275); ProDiff: denorm_spec is the identity
 // and mel_out is not masked (prodiff.py:221-222,228-229).
@@ -734,7 +735,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
         SPhase q = z;
         q.a1 = 8; q.w1 = W_OUT; q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE; q.bias = d.out_bias_pad;
         q.out = xm; q.ldo = 80; q.oh = pl[0]; q.ol = pl[1]; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
-        q.noise = noise ? noise + per * (size_t)(T - t) : nullptr; q.seed = seed; q.stream_id = 1001 + (uint64_t)t; q.n_valid = 80;
+        q.noise = noise ? noise + per * (size_t)(T - t) : nullptr; q.seed = seed; q.stream_id = stream_mel_step(t); q.n_valid = 80;
         q.no_clip = m.mel_decoder == SSB_MEL_DECODER_PRODIFF;
         ph[k++] = q;
       }
@@ -805,7 +806,7 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
   for (int t = T - 1; t >= 0; --t) {
     RUN(mel_denoiser_eval(c, d, s, t, xm, b));
     const float* nz = noise ? noise + per * (size_t)(T - t) : nullptr;
-    RUN(mel_p_sample(c, s, xm, 80, b.head, b.ld_head, nz, d.gtab + (size_t)t * 8, seed, 1001 + (uint64_t)t, clip));
+    RUN(mel_p_sample(c, s, xm, 80, b.head, b.ld_head, nz, d.gtab + (size_t)t * 8, seed, stream_mel_step(t), clip));
   }
   RUN(mel_finish(c, m, s, xm, mel_tight));
   c.release(mk);
@@ -832,7 +833,7 @@ int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float*
   const int T = d.T;
   auto acp = [&](int t) { return c.dry ? 0.5f : d.gtab_h[(size_t)t * 8 + 7]; };
   const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 6];
-  RUN(mel_q_sample(c, s, coarse_g, 80, q_noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, 1000));
+  RUN(mel_q_sample(c, s, coarse_g, 80, q_noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, stream_mel_xt()));
   int nh = 0;  // predictions in the history; hist[(head + k) % 3] is the k-th newest
   int head = 0;
   int t0 = 0;
@@ -902,8 +903,7 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
   const size_t per = (size_t)s.total;
   for (int n = 0; n < 2; ++n) {
     const Denoiser& d = m.f0net[n];
-    const uint64_t sbase = 2000 + (uint64_t)n * 100000;
-    RUN(f0_init(c, s, z[n], uv[n], gnoise[n], seed, sbase));
+    RUN(f0_init(c, s, z[n], uv[n], gnoise[n], seed, stream_f0_xt(n)));
     RUN(ddiff_input(c, s, z[n], uv[n], d.in_w, d.in_b, d.uv_emb, d.dtab + (size_t)(T - 1) * L * C, x[n], nullptr, C, pl[n][0], pl[n][1]));
     RUN(hoist_cond_tc(c, d, s, n == 0 ? cond0 : cond1, cpl[n][0], cpl[n][1], condpre[n]));
   }
@@ -930,7 +930,6 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
       }
       put(W_SKIP, d.skip_tc);
       put(W_OUT, d.out_tc);
-      const uint64_t sbase = 2000 + (uint64_t)n * 100000;
       for (int ti = 0; ti < T; ++ti) {
         const int t = T - 1 - ti;
         const float* dt = d.dtab + (size_t)t * L * C;
@@ -968,7 +967,7 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
           q.tab = d.gtab + (size_t)t * 8; q.tab2 = d.mtab + (size_t)t * 8; q.tstep = t; q.log_eps = m.log_eps;
           q.noise = gnoise[n] ? gnoise[n] + per * (size_t)(T - t) : nullptr;
           q.noise2 = unoise[n] ? unoise[n] + per * 2 * (size_t)(T - 1 - t) : nullptr;
-          q.seed = seed; q.stream_id = sbase + 10 + 2 * (uint64_t)t;
+          q.seed = seed; q.stream_id = stream_f0_gauss(n, t); q.stream2 = stream_f0_unif(n, t);
           q.has_next = t > 0; q.C = C; q.in_w = d.in_w; q.in_b = d.in_b; q.uv_emb = d.uv_emb; q.x_next = x[n];
           q.oh = pl[n][0]; q.ol = pl[n][1]; q.ldh = C;
           q.vec2 = t > 0 ? d.dtab + (size_t)(t - 1) * L * C : nullptr;
@@ -1005,8 +1004,7 @@ int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const f
   RUN(prepare_cond(c, d, s, cond_g, b));
   const int T = d.T;
   const size_t per = (size_t)s.total;
-  const uint64_t sbase = 2000 + (uint64_t)which * 100000;
-  RUN(f0_init(c, s, z, uv, gnoise, seed, sbase));
+  RUN(f0_init(c, s, z, uv, gnoise, seed, stream_f0_xt(which)));
   for (int t = T - 1; t >= 0; --t) {
     const float* dt = d.dtab + (size_t)t * d.L * d.C;
     RUN(ddiff_input(c, s, z, uv, d.in_w, d.in_b, d.uv_emb, dt, b.tc ? nullptr : b.x, b.y, d.C, b.yh, b.yl));
@@ -1016,7 +1014,7 @@ int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const f
     a.gnoise = gnoise ? gnoise + per * (size_t)(T - t) : nullptr;
     a.unoise = unoise ? unoise + per * 2 * (size_t)(T - 1 - t) : nullptr;
     a.gtab = d.gtab + (size_t)t * 8; a.mtab = d.mtab + (size_t)t * 8; a.t = t; a.log_eps = m.log_eps;
-    a.seed = seed; a.stream_id = sbase + 10 + 2 * (uint64_t)t;
+    a.seed = seed; a.gauss_stream = stream_f0_gauss(which, t); a.unif_stream = stream_f0_unif(which, t);
     RUN(f0_p_sample(c, s, a));
   }
   c.release(mk);

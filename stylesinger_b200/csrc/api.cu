@@ -162,37 +162,9 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
         a.rowmask = tgt; a.out = cond2; a.ldo = H; a.C = H;
         RUN(combine_rows(c, sf, a));
       }
-      // The two F0/UV samplers are independent (stylesinger.py:223-225): run the second one on the model's
-      // auxiliary stream so that their latency-bound dependent chains overlap.  Disjoint workspace regions.
-      if (f0_pair_persistent_ok(m, sf)) {
-        float* zz[2] = {za, zs};
-        int32_t* uu[2] = {uva, uvs};
-        RUN(run_f0_diffusion_pair_persistent(c, m, sf, cond, cond2, lo, hi, in.f0_gauss_noise, in.f0_unif_noise, in.seed, zz, uu));
-      } else {
-      // Two streams only for small batches (latency-bound chains).  From ~8k frames on every GEMM fills the GPU on its
-      // own, and the CTA-pair (cluster) kernels used there must not run concurrently with each other from two streams:
-      // that combination hung the GPU in an earlier version of these kernels (root cause not isolated).
-      const bool fork = !c.dry && m.aux_stream != nullptr && sf.ntiles <= 64;
-      if (fork) {
-        SSB_CUDA(cudaEventRecord(m.ev_fork, c.stream));
-        SSB_CUDA(cudaStreamWaitEvent(m.aux_stream, m.ev_fork, 0));
-      }
-      const size_t off0 = c.off;
-      RUN(run_f0_diffusion(c, m, 0, sf, cond, lo, hi, in.f0_gauss_noise[0], in.f0_unif_noise[0], in.seed, za, uva));
-      c.off = c.high;  // keep sampler 0's buffers alive: sampler 1 allocates above them
-      {
-        Ctx c2 = c;
-        if (fork) c2.stream = m.aux_stream;
-        RUN(run_f0_diffusion(c2, m, 1, sf, cond2, lo, hi, in.f0_gauss_noise[1], in.f0_unif_noise[1], in.seed, zs, uvs));
-        if (c2.high > c.high) c.high = c2.high;
-        c.failed = c.failed || c2.failed;
-      }
-      if (fork) {
-        SSB_CUDA(cudaEventRecord(m.ev_join, m.aux_stream));
-        SSB_CUDA(cudaStreamWaitEvent(c.stream, m.ev_join, 0));
-      }
-      c.off = off0;
-      }
+      float* zz[2] = {za, zs};
+      int32_t* uu[2] = {uva, uvs};
+      RUN(run_f0_samplers(c, m, sf, cond, cond2, lo, hi, in.f0_gauss_noise, in.f0_unif_noise, in.seed, zz, uu));
     }
     PitchGlueArgs pg;
     pg.za = za; pg.uva = uva; pg.zs = zs; pg.uvs = uvs; pg.midi = midi; pg.mel2ph = mel2ph;

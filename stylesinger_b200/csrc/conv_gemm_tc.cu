@@ -456,7 +456,7 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       const int2 t = mt < p.ntiles ? p.tiles[mt] : make_int2(0, 0);
       const int64_t r0 = (int64_t)t.x + ew * 32;
       const int nrows = min(32, max(0, t.y - ew * 32));
-      const int tq = (p.e.tile_base + mt) * 4 + ew;
+      const int tq = mt * 4 + ew;
       const int n0 = nt * BN;
       Pre cur, nxt;
       if (nrows > 0) prefetch_chunk<MODE>(p.e, r0, nrows, n0 + eg * 32, lane, cur, tq);  // overlaps the MMAs

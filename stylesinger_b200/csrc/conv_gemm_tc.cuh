@@ -67,7 +67,6 @@ struct EpiTC {
   int n_valid = 0;               // > 0: output columns >= n_valid are padding (weights padded to a tile multiple): skipped
   int skip_tiled = 0;            // RES_SKIP: skip accumulator stored chunk-tiled - [row tile][32-row quarter][32-col chunk][32 rows][32 cols]
                                  //   fp32, so that every 32 x 32 epilogue chunk is one contiguous 4 KB block (private to this epilogue)
-  int tile_base = 0;             //   index of tiles[0] in the full tile table (a GEMM over a sub-range of the row tiles)
   int out_nb = 0;                // GENERIC, > 0: `out` is column-block-major: block j = columns [j*out_nb, (j+1)*out_nb) is its own
   int64_t out_bs = 0;            //   [rows, out_nb] matrix at out + j * out_bs (the hoisted conditioner: one matrix per layer)
   __half* sh = nullptr;          // RES_SKIP (last layer): the finished skip sum also as fp16 planes [rows, C]

@@ -446,32 +446,6 @@ int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const 
 // a13/a18: the denoiser residual stack for one diffusion step.
 // On entry b.x holds the residual stream and (b.y | b.yh,b.yl) holds x + d[t][0]; both are overwritten.
 // SIMT path: fp32 conv_gemm.  Tensor-core path (b.tc): wgmma GEMMs on fp16 hi/lo planes.
-// The two tensor-core GEMMs of residual layer l over the row tiles [tiles, tiles + ntiles) (net.py:66-78)
-static GemmTC layer_gate_gemm(const Denoiser& d, const DenoiserBufs& b, int64_t rows, const int2* tiles, int ntiles, int l) {
-  const int C = d.C;
-  GemmTC g;
-  g.A_hi = b.yh; g.A_lo = b.yl; g.rows_total = rows; g.w = &d.layers[l].dil_tc; g.tiles = tiles; g.ntiles = ntiles;
-  // K = 3*C (taps of y); the hoisted conditioner projection arrives as an epilogue addend (one [rows, 2C] matrix per layer)
-  g.e.add = b.condpre + (size_t)l * (size_t)rows * 2 * C; g.e.ld_add = 2 * C;
-  g.e.mode = EPI_GATE; g.e.bias = d.layers[l].bias_gate_tc;
-  g.e.oh = b.zh; g.e.ol = b.zl; g.e.ldh = C;
-  return g;
-}
-static GemmTC layer_res_gemm(const Denoiser& d, const DenoiserBufs& b, int64_t rows, const int2* tiles, int ntiles, int l,
-                             const float* dt, int tile0 = 0 /* index of tiles[0] in the layout's tile table */) {
-  const int C = d.C, L = d.L;
-  GemmTC g;
-  g.A_hi = b.zh; g.A_lo = b.zl; g.rows_total = rows; g.w = &d.layers[l].outp_tc; g.tiles = tiles; g.ntiles = ntiles;
-  // residual stream carried ONLY as the fp16 hi/lo planes of y = x + step bias (in place: this epilogue reads
-  // y_l[row] and writes y_{l+1}[row] for the same rows/columns): no fp32 x is read or written in the T x L loop
-  g.e.mode = EPI_RES_SKIP; g.e.C = C; g.e.beta = 0.70710678118654752440f;
-  g.e.rh = b.yh; g.e.rl = b.yl; g.e.ld_rh = C; g.e.vec1 = dt + (size_t)l * C;
-  if (l + 1 < L) { g.e.oh = b.yh; g.e.ol = b.yl; g.e.ldh = C; g.e.vec2 = dt + (size_t)(l + 1) * C; }
-  g.e.skip = b.skip; g.e.ld_skip = C; g.e.skip_init = (l == 0);
-  g.e.skip_tiled = b.skip_tiled ? 1 : 0; g.e.tile_base = tile0;
-  if (b.tc_heads && l == L - 1) { g.e.sh = b.skh; g.e.sl = b.skl; }
-  return g;
-}
 
 // skip_projection + output_projection of the denoiser (net.py:126-130 / :262-266)
 static int denoiser_heads(Ctx& c, const Denoiser& d, const SeqDev& s, DenoiserBufs& b) {
@@ -511,10 +485,28 @@ int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBu
   const int C = d.C, L = d.L;
   SSB_CHECK(d.dtab != nullptr && t >= 0 && t < d.T, "denoiser: schedule not set (ssb_model_set_schedule) or bad t");
   const float* dt = d.dtab + (size_t)t * L * C;
-  for (int l = 0; l < L; ++l) {
+  for (int l = 0; l < L; ++l) {  // residual layer l (net.py:66-78)
     if (b.tc) {
-      RUN(conv_gemm_tc(c, layer_gate_gemm(d, b, s.rows, s.tiles, s.ntiles, l)));
-      RUN(conv_gemm_tc(c, layer_res_gemm(d, b, s.rows, s.tiles, s.ntiles, l, dt)));
+      {
+        GemmTC g;
+        g.A_hi = b.yh; g.A_lo = b.yl; g.rows_total = s.rows; g.w = &d.layers[l].dil_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
+        // K = 3*C (taps of y); the hoisted conditioner projection arrives as an epilogue addend (one [rows, 2C] matrix per layer)
+        g.e.add = b.condpre + (size_t)l * (size_t)s.rows * 2 * C; g.e.ld_add = 2 * C;
+        g.e.mode = EPI_GATE; g.e.bias = d.layers[l].bias_gate_tc;
+        g.e.oh = b.zh; g.e.ol = b.zl; g.e.ldh = C;
+        RUN(conv_gemm_tc(c, g));
+      }
+      GemmTC g;
+      g.A_hi = b.zh; g.A_lo = b.zl; g.rows_total = s.rows; g.w = &d.layers[l].outp_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
+      // residual stream carried ONLY as the fp16 hi/lo planes of y = x + step bias (in place: this epilogue reads
+      // y_l[row] and writes y_{l+1}[row] for the same rows/columns): no fp32 x is read or written in the T x L loop
+      g.e.mode = EPI_RES_SKIP; g.e.C = C; g.e.beta = 0.70710678118654752440f;
+      g.e.rh = b.yh; g.e.rl = b.yl; g.e.ld_rh = C; g.e.vec1 = dt + (size_t)l * C;
+      if (l + 1 < L) { g.e.oh = b.yh; g.e.ol = b.yl; g.e.ldh = C; g.e.vec2 = dt + (size_t)(l + 1) * C; }
+      g.e.skip = b.skip; g.e.ld_skip = C; g.e.skip_init = (l == 0);
+      g.e.skip_tiled = b.tc_heads ? 1 : 0;
+      if (b.tc_heads && l == L - 1) { g.e.sh = b.skh; g.e.sl = b.skl; }
+      RUN(conv_gemm_tc(c, g));
       continue;
     }
     {
@@ -580,8 +572,7 @@ int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, Denoiser
   }
   // tensor-core heads: the fp32 skip accumulator is private to the RES_SKIP epilogue (the heads read the planes the last
   // layer writes), so it is kept chunk-tiled (every 32 x 32 epilogue chunk one contiguous 4 KB block; conv_gemm_tc.cuh)
-  b->skip_tiled = b->tc_heads;
-  if (b->skip_tiled) {
+  if (b->tc_heads) {
     const size_t n = (size_t)s.ntiles * TILE_M * d.C;
     b->skip = c.alloc<float>(n);  // fully written by layer 0 (skip_init) before it is read: no memset
   } else {
@@ -652,26 +643,106 @@ static int mel_finish(Ctx& c, const Model& m, const SeqDev& s, const float* xm, 
   return mel_denorm(c, s, xm, 80, m.spec_min, m.spec_max, nullptr, mel_tight, 80);
 }
 
-// a18+a19, single launch: all T reverse steps in the persistent wgmma kernel (sampler_tc.cu).
+// ------------------------------------------------------------------------------------------------
+// Persistent samplers (sampler_tc.cu): all T reverse steps of a denoiser in one cooperative launch, driven by a table
+// of GEMM phases (SPhase) over a table of tensor maps.  PersistentNet is one DiffNet's part of such a launch; the
+// samplers add their own input and sampling phases around it.
+struct PersistentNet {
+  // fp16 hi/lo plane pairs: pl[i] (hi) and pl[i + 1] (lo), tensor maps mb + i and mb + i + 1
+  enum { Y = 0, Z = 2, SKIP = 4, S = 6, NPL = 8 };  // y = x + step bias, gate output, finished skip sum, relu(skip_proj)
+  const Denoiser* d = nullptr;
+  float* x = nullptr;        // fp32 residual stream [rows, C]
+  float* skip = nullptr;     // skip accumulator [rows, C]
+  __half* pl[NPL] = {};      // [rows, C] each
+  float* condpre = nullptr;  // hoisted conditioner projection (hoist_cond_tc)
+  int mb = 0;                // index of the net's first tensor map
+  // the net's maps from mb: its NPL activation planes, then (hi, lo) weights of dil_tc and outp_tc per layer, skip, out
+  static int nmaps(int L) { return NPL + 4 * L + 4; }
+  int w_layer(int l) const { return mb + NPL + 4 * l; }  // dil_tc; outp_tc at + 2
+  int w_skip() const { return mb + NPL + 4 * d->L; }
+  int w_out() const { return w_skip() + 2; }
+};
+
+// Allocates the net's buffers and hoists its conditioner projection, so that its gate phases contract K = 3C and add
+// that projection in the epilogue.
+static int persistent_net_setup(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, int mb, PersistentNet* p) {
+  p->d = &d;
+  p->mb = mb;
+  p->x = alloc_rows(c, s, d.C);
+  p->skip = alloc_rows(c, s, d.C);
+  for (int i = 0; i < PersistentNet::NPL; ++i) p->pl[i] = alloc_half_rows(c, s, d.C);
+  __half* ch = alloc_half_rows(c, s, 256);
+  __half* cl = alloc_half_rows(c, s, 256);
+  p->condpre = alloc_rows(c, s, d.L * 2 * d.C, false);
+  WS_OK(c);
+  return hoist_cond_tc(c, d, s, cond_g, ch, cl, p->condpre);
+}
+
+// Writes the net's tensor maps into maps[p.mb, p.mb + nmaps(L)); activation boxes of 128 / cs rows, one cs-th of an
+// M-tile per CTA of a cluster.
+static int persistent_net_maps(const PersistentNet& p, const SeqDev& s, int cs, CUtensorMap* maps) {
+  const Denoiser& d = *p.d;
+  for (int i = 0; i < PersistentNet::NPL; ++i)
+    if (make_act_map(&maps[p.mb + i], p.pl[i], s.rows, d.C, 128 / cs)) return -1;
+  auto put = [&](int idx, const ConvTC& w) { maps[idx] = w.tm_hi[1]; maps[idx + 1] = w.tm_lo[1]; };
+  for (int l = 0; l < d.L; ++l) {
+    put(p.w_layer(l), d.layers[l].dil_tc);
+    put(p.w_layer(l) + 2, d.layers[l].outp_tc);
+  }
+  put(p.w_skip(), d.skip_tc);
+  put(p.w_out(), d.out_tc);
+  return 0;
+}
+
+static SPhase sphase(int sync_after) {
+  SPhase z;
+  memset(&z, 0, sizeof(z));
+  z.taps = 1; z.dil = 1; z.beta = 1.0f; z.sync_after = sync_after;
+  return z;
+}
+
+// Appends the net's phases of reverse step t, from its input planes y (written by the caller's previous phase) to the
+// s planes: L (gate, residual + skip) pairs, then skip_projection.  Every entry gets sync_after.
+static void persistent_net_step(const PersistentNet& p, const SeqDev& s, int t, int sync_after, std::vector<SPhase>& ph) {
+  using P = PersistentNet;
+  const Denoiser& d = *p.d;
+  const int C = d.C, L = d.L;
+  const float* dt = d.dtab + (size_t)t * L * C;
+  for (int l = 0; l < L; ++l) {
+    SPhase a = sphase(sync_after);  // dilated conv (3 taps of y) + hoisted conditioner projection -> gate -> z planes
+    a.a1 = p.mb + P::Y; a.w1 = p.w_layer(l); a.taps = 3; a.kchunks = C / 64;
+    a.dil = d.layers[l].dil_tc.dil; a.center = 1; a.N = 2 * C; a.NT = 2 * C / 64; a.mode = SP_GATE;
+    a.bias = d.layers[l].bias_gate_tc; a.oh = p.pl[P::Z]; a.ol = p.pl[P::Z + 1]; a.ldh = C;
+    a.add = p.condpre + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C;
+    ph.push_back(a);
+    SPhase b = sphase(sync_after);  // 1x1 output projection -> residual stream, next layer's input planes, skip sum
+    b.a1 = p.mb + P::Z; b.w1 = p.w_layer(l) + 2; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
+    b.bias = d.layers[l].outp.bias; b.res = p.x; b.ld_res = C; b.out = p.x; b.ldo = C; b.beta = 0.70710678118654752440f;
+    if (l + 1 < L) { b.oh = p.pl[P::Y]; b.ol = p.pl[P::Y + 1]; b.ldh = C; b.vec2 = dt + (size_t)(l + 1) * C; }
+    b.skip = p.skip; b.ld_skip = C; b.C = C; b.skip_init = (l == 0);
+    if (l == L - 1) { b.sh = p.pl[P::SKIP]; b.sl = p.pl[P::SKIP + 1]; }
+    ph.push_back(b);
+  }
+  SPhase q = sphase(sync_after);  // skip_projection (1/sqrt(L) folded into the weights, N padded) + ReLU -> s planes
+  q.a1 = p.mb + P::SKIP; q.w1 = p.w_skip(); q.kchunks = C / 64; q.N = d.skip_tc.N; q.NT = d.skip_tc.N / 64;
+  q.mode = SP_SKIPPROJ; q.bias = d.skip_bias_pad; q.oh = p.pl[P::S]; q.ol = p.pl[P::S + 1]; q.ldh = C; q.n_valid = C;
+  ph.push_back(q);
+}
+
+// a18+a19, single launch: all T reverse steps of the mel DiffNet.
 static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                                         const float* noise, uint64_t seed, float* mel_tight) {
+  using P = PersistentNet;
   const Denoiser& d = m.melnet;
   const int C = d.C, L = d.L, T = d.T;
   const int CS = 4;  // cluster size along N: A tiles are TMA-multicast to the 4 CTAs that share an M-tile
   const size_t mk = c.mark();
   float* xm = alloc_rows(c, s, 80);
-  float* x = alloc_rows(c, s, C);
-  float* skip = alloc_rows(c, s, C);
-  __half* pl[10];
-  const int pcols[5] = {128, C, C, C, C};  // x80, y, z, skip, s
-  for (int i = 0; i < 5; ++i) {
-    pl[2 * i] = alloc_half_rows(c, s, pcols[i]);
-    pl[2 * i + 1] = alloc_half_rows(c, s, pcols[i]);
-  }
-  __half* ch = alloc_half_rows(c, s, 256);
-  __half* cl = alloc_half_rows(c, s, 256);
-  float* condpre = alloc_rows(c, s, L * 2 * C, false);
-  const int nmaps = 10 + 2 + 4 * L + 4;
+  P net;
+  RUN(persistent_net_setup(c, d, s, cond_g, 0, &net));
+  __half* x80h = alloc_half_rows(c, s, 128);  // planes of x_t, K padded 80 -> 128
+  __half* x80l = alloc_half_rows(c, s, 128);
+  const int M_X80 = P::nmaps(L), W_IN = M_X80 + 2, nmaps = W_IN + 2;
   const int nph = T * (2 * L + 3);
   CUtensorMap* maps_dev = c.alloc<CUtensorMap>((size_t)nmaps);
   SPhase* ph_dev = c.alloc<SPhase>((size_t)nph);
@@ -679,66 +750,27 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
   WS_OK(c);
   const size_t per = (size_t)s.total * 80;
   RUN(mel_init(c, m, s, coarse_g, noise, seed, xm));
-  RUN(x80_planes(c, xm, s.rows, pl[0], pl[1]));
-  // one per-launch GEMM: the gate phases contract K = 3C and add the conditioner projection in the epilogue
-  RUN(hoist_cond_tc(c, d, s, cond_g, ch, cl, condpre));
+  RUN(x80_planes(c, xm, s.rows, x80h, x80l));
   if (!c.dry) {
     std::vector<CUtensorMap> maps((size_t)nmaps);
-    for (int i = 0; i < 5; ++i) {
-      if (make_act_map(&maps[2 * i], pl[2 * i], s.rows, pcols[i], 128 / CS)) return -1;
-      if (make_act_map(&maps[2 * i + 1], pl[2 * i + 1], s.rows, pcols[i], 128 / CS)) return -1;
-    }
-    auto put = [&](int idx, const ConvTC& w) { maps[idx] = w.tm_hi[1]; maps[idx + 1] = w.tm_lo[1]; };
-    const int W_IN = 10, W_L0 = 12, W_SKIP = W_L0 + 4 * L, W_OUT = W_SKIP + 2;
-    put(W_IN, d.in_tc);
-    for (int l = 0; l < L; ++l) {
-      put(W_L0 + 4 * l, d.layers[l].dil_tc);
-      put(W_L0 + 4 * l + 2, d.layers[l].outp_tc);
-    }
-    put(W_SKIP, d.skip_tc);
-    put(W_OUT, d.out_tc);
-    std::vector<SPhase> ph((size_t)nph);
-    size_t k = 0;
+    if (persistent_net_maps(net, s, CS, maps.data())) return -1;
+    if (make_act_map(&maps[M_X80], x80h, s.rows, 128, 128 / CS)) return -1;
+    if (make_act_map(&maps[M_X80 + 1], x80l, s.rows, 128, 128 / CS)) return -1;
+    maps[W_IN] = d.in_tc.tm_hi[1]; maps[W_IN + 1] = d.in_tc.tm_lo[1];
+    std::vector<SPhase> ph;
+    ph.reserve((size_t)nph);
     for (int t = T - 1; t >= 0; --t) {
-      const float* dt = d.dtab + (size_t)t * L * C;
-      SPhase z;
-      memset(&z, 0, sizeof(z));
-      z.taps = 1; z.dil = 1; z.beta = 1.0f; z.sync_after = 1;
-      {  // input_projection + ReLU ; y = x + step bias of layer 0
-        SPhase q = z;
-        q.a1 = 0; q.w1 = W_IN; q.kchunks = 2; q.N = C; q.NT = C / 64; q.mode = SP_INPROJ; q.bias = d.in_proj.bias;
-        q.out = x; q.ldo = C; q.oh = pl[2]; q.ol = pl[3]; q.ldh = C; q.vec2 = dt;
-        ph[k++] = q;
-      }
-      for (int l = 0; l < L; ++l) {
-        SPhase a = z;  // dilated conv (3 taps of y) + hoisted conditioner projection -> gate -> z planes
-        a.a1 = 2; a.w1 = W_L0 + 4 * l; a.taps = 3; a.kchunks = C / 64;
-        a.dil = d.layers[l].dil_tc.dil; a.center = 1; a.N = 2 * C; a.NT = 2 * C / 64; a.mode = SP_GATE;
-        a.bias = d.layers[l].bias_gate_tc; a.oh = pl[4]; a.ol = pl[5]; a.ldh = C;
-        a.add = condpre + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C;
-        ph[k++] = a;
-        SPhase b = z;  // 1x1 output projection -> residual stream, next layer's input planes, skip sum
-        b.a1 = 4; b.w1 = W_L0 + 4 * l + 2; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
-        b.bias = d.layers[l].outp.bias; b.res = x; b.ld_res = C; b.out = x; b.ldo = C; b.beta = 0.70710678118654752440f;
-        if (l + 1 < L) { b.oh = pl[2]; b.ol = pl[3]; b.ldh = C; b.vec2 = dt + (size_t)(l + 1) * C; }
-        b.skip = skip; b.ld_skip = C; b.C = C; b.skip_init = (l == 0);
-        if (l == L - 1) { b.sh = pl[6]; b.sl = pl[7]; }
-        ph[k++] = b;
-      }
-      {  // skip_projection (1/sqrt(L) folded into the weights) + ReLU -> s planes
-        SPhase q = z;
-        q.a1 = 6; q.w1 = W_SKIP; q.kchunks = C / 64; q.N = C; q.NT = C / 64; q.mode = SP_SKIPPROJ; q.bias = d.skip_proj.bias;
-        q.oh = pl[8]; q.ol = pl[9]; q.ldh = C;
-        ph[k++] = q;
-      }
-      {  // output_projection -> eps ; fused DDPM posterior step on x_t
-        SPhase q = z;
-        q.a1 = 8; q.w1 = W_OUT; q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE; q.bias = d.out_bias_pad;
-        q.out = xm; q.ldo = 80; q.oh = pl[0]; q.ol = pl[1]; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
-        q.noise = noise ? noise + per * (size_t)(T - t) : nullptr; q.seed = seed; q.stream_id = stream_mel_step(t); q.n_valid = 80;
-        q.no_clip = m.mel_decoder == SSB_MEL_DECODER_PRODIFF;
-        ph[k++] = q;
-      }
+      SPhase q = sphase(1);  // input_projection + ReLU ; y = x + step bias of layer 0
+      q.a1 = M_X80; q.w1 = W_IN; q.kchunks = 2; q.N = C; q.NT = C / 64; q.mode = SP_INPROJ; q.bias = d.in_proj.bias;
+      q.out = net.x; q.ldo = C; q.oh = net.pl[P::Y]; q.ol = net.pl[P::Y + 1]; q.ldh = C; q.vec2 = d.dtab + (size_t)t * L * C;
+      ph.push_back(q);
+      persistent_net_step(net, s, t, 1, ph);
+      q = sphase(1);  // output_projection -> eps ; fused DDPM posterior step on x_t
+      q.a1 = net.mb + P::S; q.w1 = net.w_out(); q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE;
+      q.bias = d.out_bias_pad; q.out = xm; q.ldo = 80; q.oh = x80h; q.ol = x80l; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
+      q.noise = noise ? noise + per * (size_t)(T - t) : nullptr; q.seed = seed; q.stream_id = stream_mel_step(t); q.n_valid = 80;
+      q.no_clip = m.mel_decoder == SSB_MEL_DECODER_PRODIFF;
+      ph.push_back(q);
     }
     SSB_CUDA(cudaMemcpyAsync(maps_dev, maps.data(), sizeof(CUtensorMap) * nmaps, cudaMemcpyHostToDevice, c.stream));
     SSB_CUDA(cudaMemcpyAsync(ph_dev, ph.data(), sizeof(SPhase) * nph, cudaMemcpyHostToDevice, c.stream));
@@ -875,27 +907,18 @@ int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float*
 
 // a13+a14 for BOTH F0 nets in one persistent launch: the agnostic and the specific sampler are independent
 // (stylesinger.py:223-225), so each phase of the table carries two entries (one per net, no barrier between them).
-int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1,
-                                     const float* lo, const float* hi, const float* const gnoise[2],
-                                     const float* const unoise[2], uint64_t seed, float* const z[2], int32_t* const uv[2]) {
-  const Denoiser& d0 = m.f0net[0];
-  const int C = d0.C, L = d0.L, T = d0.T;
+static int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1,
+                                            const float* lo, const float* hi, const float* const gnoise[2],
+                                            const float* const unoise[2], uint64_t seed, float* const z[2],
+                                            int32_t* const uv[2]) {
+  using P = PersistentNet;
+  const int C = m.f0net[0].C, L = m.f0net[0].L, T = m.f0net[0].T;
   const int CS = 2;
   const size_t mk = c.mark();
-  const int NA = 8;            // activation maps per net: y, z, skip, s (hi/lo)
-  const int NW = 4 * L + 4;    // weight maps per net: dil, outp per layer, skip, out (hi/lo)
-  const int nmaps = 2 * (NA + NW);
-  const int per_step = 2 * L + 2;
-  const int nph = 2 * T * per_step;
-  float* x[2]; float* skip[2]; float* condpre[2]; __half* pl[2][8]; __half* cpl[2][2];
-  for (int n = 0; n < 2; ++n) {
-    x[n] = alloc_rows(c, s, C);
-    skip[n] = alloc_rows(c, s, C);
-    for (int i = 0; i < 8; ++i) pl[n][i] = alloc_half_rows(c, s, C);
-    cpl[n][0] = alloc_half_rows(c, s, 256);
-    cpl[n][1] = alloc_half_rows(c, s, 256);
-    condpre[n] = alloc_rows(c, s, L * 2 * C, false);
-  }
+  P net[2];
+  for (int n = 0; n < 2; ++n) RUN(persistent_net_setup(c, m.f0net[n], s, n == 0 ? cond0 : cond1, n * P::nmaps(L), &net[n]));
+  const int nmaps = 2 * P::nmaps(L);
+  const int nph = 2 * T * (2 * L + 2);
   CUtensorMap* maps_dev = c.alloc<CUtensorMap>((size_t)nmaps);
   SPhase* ph_dev = c.alloc<SPhase>((size_t)nph);
   unsigned* ctr = c.alloc<unsigned>(4);
@@ -904,12 +927,30 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
   for (int n = 0; n < 2; ++n) {
     const Denoiser& d = m.f0net[n];
     RUN(f0_init(c, s, z[n], uv[n], gnoise[n], seed, stream_f0_xt(n)));
-    RUN(ddiff_input(c, s, z[n], uv[n], d.in_w, d.in_b, d.uv_emb, d.dtab + (size_t)(T - 1) * L * C, x[n], nullptr, C, pl[n][0], pl[n][1]));
-    RUN(hoist_cond_tc(c, d, s, n == 0 ? cond0 : cond1, cpl[n][0], cpl[n][1], condpre[n]));
+    RUN(ddiff_input(c, s, z[n], uv[n], d.in_w, d.in_b, d.uv_emb, d.dtab + (size_t)(T - 1) * L * C, net[n].x, nullptr, C,
+                    net[n].pl[P::Y], net[n].pl[P::Y + 1]));
   }
   if (!c.dry) {
     std::vector<CUtensorMap> maps((size_t)nmaps);
-    std::vector<SPhase> ph((size_t)nph);
+    std::vector<SPhase> seq[2];  // each net's phases in order; sync_after on net 1's only
+    for (int n = 0; n < 2; ++n) {
+      const Denoiser& d = m.f0net[n];
+      if (persistent_net_maps(net[n], s, CS, maps.data())) return -1;
+      for (int t = T - 1; t >= 0; --t) {
+        persistent_net_step(net[n], s, t, n == 1, seq[n]);
+        SPhase q = sphase(n == 1);  // output_projection -> (eps, logits) ; F0/UV step ; DDiffNet input of step t-1
+        q.a1 = net[n].mb + P::S; q.w1 = net[n].w_out(); q.kchunks = C / 64; q.N = d.out_tc.N; q.NT = d.out_tc.N / 64;
+        q.mode = SP_F0_SAMPLE; q.bias = d.out_bias_pad; q.out = z[n]; q.uv = uv[n]; q.clip_lo = lo; q.clip_hi = hi;
+        q.tab = d.gtab + (size_t)t * 8; q.tab2 = d.mtab + (size_t)t * 8; q.tstep = t; q.log_eps = m.log_eps;
+        q.noise = gnoise[n] ? gnoise[n] + per * (size_t)(T - t) : nullptr;
+        q.noise2 = unoise[n] ? unoise[n] + per * 2 * (size_t)(T - 1 - t) : nullptr;
+        q.seed = seed; q.stream_id = stream_f0_gauss(n, t); q.stream2 = stream_f0_unif(n, t);
+        q.has_next = t > 0; q.C = C; q.in_w = d.in_w; q.in_b = d.in_b; q.uv_emb = d.uv_emb; q.x_next = net[n].x;
+        q.oh = net[n].pl[P::Y]; q.ol = net[n].pl[P::Y + 1]; q.ldh = C;
+        q.vec2 = t > 0 ? d.dtab + (size_t)(t - 1) * L * C : nullptr;
+        seq[n].push_back(q);
+      }
+    }
     // number of clusters the launcher will use: needed for the tile-group rotation of the second net
     int ncl = s.ntiles * (2 * (2 * C / 64) / CS);
     {
@@ -917,66 +958,15 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
       if (ncl > cap) ncl = cap;
       if (ncl < 1) ncl = 1;
     }
-    for (int n = 0; n < 2; ++n) {
-      const Denoiser& d = m.f0net[n];
-      const int MB = n * (NA + NW);
-      for (int i = 0; i < NA; ++i)
-        if (make_act_map(&maps[MB + i], pl[n][i], s.rows, C, 128 / CS)) return -1;
-      auto put = [&](int idx, const ConvTC& w) { maps[idx] = w.tm_hi[1]; maps[idx + 1] = w.tm_lo[1]; };
-      const int W_L0 = MB + NA, W_SKIP = W_L0 + 4 * L, W_OUT = W_SKIP + 2;
-      for (int l = 0; l < L; ++l) {
-        put(W_L0 + 4 * l, d.layers[l].dil_tc);
-        put(W_L0 + 4 * l + 2, d.layers[l].outp_tc);
-      }
-      put(W_SKIP, d.skip_tc);
-      put(W_OUT, d.out_tc);
-      for (int ti = 0; ti < T; ++ti) {
-        const int t = T - 1 - ti;
-        const float* dt = d.dtab + (size_t)t * L * C;
-        SPhase zp;
-        memset(&zp, 0, sizeof(zp));
-        zp.taps = 1; zp.dil = 1; zp.beta = 1.0f; zp.sync_after = (n == 1);
-        // entry k of step ti for net n sits at ((ti * per_step + k) * 2 + n)
-        size_t k = 0;
-        auto slot = [&](size_t kk) -> SPhase& { return ph[((size_t)ti * per_step + kk) * 2 + n]; };
-        for (int l = 0; l < L; ++l) {
-          SPhase a = zp;
-          a.a1 = MB + 0; a.w1 = W_L0 + 4 * l; a.taps = 3; a.kchunks = C / 64;
-          a.dil = d.layers[l].dil_tc.dil; a.center = 1; a.N = 2 * C; a.NT = 2 * C / 64; a.mode = SP_GATE;
-          a.bias = d.layers[l].bias_gate_tc; a.oh = pl[n][2]; a.ol = pl[n][3]; a.ldh = C;
-          a.add = condpre[n] + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C;
-          slot(k++) = a;
-          SPhase b = zp;
-          b.a1 = MB + 2; b.w1 = W_L0 + 4 * l + 2; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
-          b.bias = d.layers[l].outp.bias; b.res = x[n]; b.ld_res = C; b.out = x[n]; b.ldo = C; b.beta = 0.70710678118654752440f;
-          if (l + 1 < L) { b.oh = pl[n][0]; b.ol = pl[n][1]; b.ldh = C; b.vec2 = dt + (size_t)(l + 1) * C; }
-          b.skip = skip[n]; b.ld_skip = C; b.C = C; b.skip_init = (l == 0);
-          if (l == L - 1) { b.sh = pl[n][4]; b.sl = pl[n][5]; }
-          slot(k++) = b;
-        }
-        {
-          SPhase q = zp;
-          q.a1 = MB + 4; q.w1 = W_SKIP; q.kchunks = C / 64; q.N = d.skip_tc.N; q.NT = d.skip_tc.N / 64; q.mode = SP_SKIPPROJ;
-          q.bias = d.skip_bias_pad; q.oh = pl[n][6]; q.ol = pl[n][7]; q.ldh = C; q.n_valid = C;
-          slot(k++) = q;
-        }
-        {
-          SPhase q = zp;
-          q.a1 = MB + 6; q.w1 = W_OUT; q.kchunks = C / 64; q.N = d.out_tc.N; q.NT = d.out_tc.N / 64; q.mode = SP_F0_SAMPLE;
-          q.bias = d.out_bias_pad; q.out = z[n]; q.uv = uv[n]; q.clip_lo = lo; q.clip_hi = hi;
-          q.tab = d.gtab + (size_t)t * 8; q.tab2 = d.mtab + (size_t)t * 8; q.tstep = t; q.log_eps = m.log_eps;
-          q.noise = gnoise[n] ? gnoise[n] + per * (size_t)(T - t) : nullptr;
-          q.noise2 = unoise[n] ? unoise[n] + per * 2 * (size_t)(T - 1 - t) : nullptr;
-          q.seed = seed; q.stream_id = stream_f0_gauss(n, t); q.stream2 = stream_f0_unif(n, t);
-          q.has_next = t > 0; q.C = C; q.in_w = d.in_w; q.in_b = d.in_b; q.uv_emb = d.uv_emb; q.x_next = x[n];
-          q.oh = pl[n][0]; q.ol = pl[n][1]; q.ldh = C;
-          q.vec2 = t > 0 ? d.dtab + (size_t)(t - 1) * L * C : nullptr;
-          slot(k++) = q;
-        }
-      }
+    // the nets' entries alternate, so each phase holds one of each; net 1's tile groups start where net 0's end, so
+    // one phase pair spreads over all clusters
+    std::vector<SPhase> ph;
+    ph.reserve((size_t)nph);
+    for (size_t i = 0; i < seq[0].size(); ++i) {
+      ph.push_back(seq[0][i]);
+      ph.push_back(seq[1][i]);
+      ph.back().goff = (s.ntiles * (seq[0][i].NT / CS)) % ncl;
     }
-    // net 1's tile groups start where net 0's end, so one phase pair spreads over all clusters
-    for (size_t i = 1; i < ph.size(); i += 2) ph[i].goff = (s.ntiles * (ph[i - 1].NT / CS)) % ncl;
     SSB_CUDA(cudaMemcpyAsync(maps_dev, maps.data(), sizeof(CUtensorMap) * nmaps, cudaMemcpyHostToDevice, c.stream));
     SSB_CUDA(cudaMemcpyAsync(ph_dev, ph.data(), sizeof(SPhase) * nph, cudaMemcpyHostToDevice, c.stream));
     RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s.tiles, s.tile_tight, s.ntiles, 2 * (2 * C / 64), ctr, CS));
@@ -984,7 +974,7 @@ int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, co
   c.release(mk);
   return 0;
 }
-bool f0_pair_persistent_ok(const Model& m, const SeqDev& s) {
+static bool f0_pair_persistent_ok(const Model& m, const SeqDev& s) {
   if (!m.persistent || !m.use_tc || s.ntiles > 48 || sampler_tc_max_ctas() <= 0) return false;
   for (int n = 0; n < 2; ++n) {
     const Denoiser& d = m.f0net[n];
@@ -1018,6 +1008,38 @@ int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const f
     RUN(f0_p_sample(c, s, a));
   }
   c.release(mk);
+  return 0;
+}
+
+int run_f0_samplers(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1, const float* lo,
+                    const float* hi, const float* const gnoise[2], const float* const unoise[2], uint64_t seed,
+                    float* const z[2], int32_t* const uv[2]) {
+  if (f0_pair_persistent_ok(m, s)) return run_f0_diffusion_pair_persistent(c, m, s, cond0, cond1, lo, hi, gnoise, unoise, seed, z, uv);
+  // The two samplers are independent (stylesinger.py:223-225): run the second one on the model's auxiliary stream so
+  // that their latency-bound dependent chains overlap.  Disjoint workspace regions.
+  // Two streams only for small batches (latency-bound chains).  From ~8k frames on every GEMM fills the GPU on its
+  // own, and the CTA-pair (cluster) kernels used there must not run concurrently with each other from two streams:
+  // that combination hung the GPU in an earlier version of these kernels (root cause not isolated).
+  const bool fork = !c.dry && m.aux_stream != nullptr && s.ntiles <= 64;
+  if (fork) {
+    SSB_CUDA(cudaEventRecord(m.ev_fork, c.stream));
+    SSB_CUDA(cudaStreamWaitEvent(m.aux_stream, m.ev_fork, 0));
+  }
+  const size_t off0 = c.off;
+  RUN(run_f0_diffusion(c, m, 0, s, cond0, lo, hi, gnoise[0], unoise[0], seed, z[0], uv[0]));
+  c.off = c.high;  // keep sampler 0's buffers alive: sampler 1 allocates above them
+  {
+    Ctx c2 = c;
+    if (fork) c2.stream = m.aux_stream;
+    RUN(run_f0_diffusion(c2, m, 1, s, cond1, lo, hi, gnoise[1], unoise[1], seed, z[1], uv[1]));
+    if (c2.high > c.high) c.high = c2.high;
+    c.failed = c.failed || c2.failed;
+  }
+  if (fork) {
+    SSB_CUDA(cudaEventRecord(m.ev_join, m.aux_stream));
+    SSB_CUDA(cudaStreamWaitEvent(c.stream, m.ev_join, 0));
+  }
+  c.off = off0;
   return 0;
 }
 

@@ -18,8 +18,7 @@ struct DenoiserBufs {
   __half *ch, *cl;            // tensor-core path: fp16 hi/lo planes of the conditioner [rows,256] (A of the hoisted projection)
   __half *skh, *skl, *sh, *sl;  // tensor-core heads: planes of the skip sum and of relu(skip_proj)
   __half *x80h, *x80l;          // mel net, tensor-core in_proj: planes of x_t padded to 128 columns
-  bool tc_heads;
-  bool skip_tiled;              // skip accumulator in the chunk-tiled layout (EpiTC::skip_tiled)
+  bool tc_heads;                // also: the skip accumulator is in the chunk-tiled layout (EpiTC::skip_tiled)
   int ld_head;
   bool tc;
 };
@@ -35,10 +34,10 @@ int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float*
                            const float* q_noise, uint64_t seed, int interval, float* mel_tight);
 int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const float* cond_g, const float* lo,
                      const float* hi, const float* gnoise, const float* unoise, uint64_t seed, float* z, int32_t* uv);
-int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1,
-                                     const float* lo, const float* hi, const float* const gnoise[2],
-                                     const float* const unoise[2], uint64_t seed, float* const z[2], int32_t* const uv[2]);
-bool f0_pair_persistent_ok(const Model& m, const SeqDev& s);
+// both F0 samplers (agnostic: cond0, gnoise[0], ... ; specific: cond1, gnoise[1], ...)
+int run_f0_samplers(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1, const float* lo,
+                    const float* hi, const float* const gnoise[2], const float* const unoise[2], uint64_t seed,
+                    float* const z[2], int32_t* const uv[2]);
 int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight, const float* f0_tight,
                 const float* rand_ini, const float* src_noise, uint64_t seed, float* wav_tight);
 int denoiser_eval_api(Ctx& c, const Model& m, int which, const SeqDev& s, const float* x_tight, const int32_t* uv_tight,

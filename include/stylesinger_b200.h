@@ -343,6 +343,13 @@ int ssb_op_attention(const float* q, const float* k, const float* v, const int32
  * aligner (lse.py:41). */
 int ssb_op_attention_tc(const float* q, const float* k, const float* v, const int32_t* q_offsets,
                         const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream);
+/* Either kernel (tc = 0: fp32, tc = 1: wgmma) with a key-padding mask: keymask is a device array [sumS] in the tight
+ * layout of k, 0 = masked (the -inf of key_padding_mask), anything else = attend.  Both kernels write NaN for every query
+ * of an utterance whose keys are all masked (or that has no keys), as torch's softmax over all -inf does; the other
+ * utterances of the batch are unaffected. */
+int ssb_op_attention_masked(const float* q, const float* k, const float* v, const int32_t* q_offsets,
+                            const int32_t* k_offsets, int32_t B, float scale, const float* keymask, int32_t tc, float* out,
+                            void* stream);
 
 #ifdef __cplusplus
 }

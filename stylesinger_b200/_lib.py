@@ -63,6 +63,7 @@ EXPORTS = [
     "ssb_melspec_create", "ssb_melspec_free", "ssb_melspec_num_frames", "ssb_melspec_workspace_bytes", "ssb_melspec_forward",
     "ssb_melspec_create_ex", "ssb_lstm_encoder_create", "ssb_lstm_encoder_free", "ssb_lstm_encoder_workspace_bytes", "ssb_lstm_encoder_forward",
     "ssb_model_create_ex", "ssb_mel_prodiff_workspace_bytes", "ssb_mel_prodiff_sample",
+    "ssb_op_attention_masked",
 ]
 
 
@@ -100,6 +101,7 @@ def _load():
         "ssb_op_conv1d": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, i32, i32, i32, vp, vp]),
         "ssb_op_attention": (C.c_int, [vp, vp, vp, vp, vp, i32, C.c_float, vp, vp]),
         "ssb_op_attention_tc": (C.c_int, [vp, vp, vp, vp, vp, i32, C.c_float, vp, vp]),
+        "ssb_op_attention_masked": (C.c_int, [vp, vp, vp, vp, vp, i32, C.c_float, vp, i32, vp, vp]),
         "ssb_mel_postprocess": (C.c_int, [vp, C.c_int64, C.c_float, C.c_float, vp, vp]),
         "ssb_launch_count": (C.c_int64, []),
         "ssb_model_set_tensor_cores": (C.c_int, [vp, i32]),

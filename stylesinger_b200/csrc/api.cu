@@ -732,47 +732,27 @@ int ssb_op_conv1d(const float* x, const int32_t* offsets, int32_t B, int32_t Cin
 
 int ssb_op_attention(const float* q, const float* k, const float* v, const int32_t* q_offsets,
                      const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream) {
-  SSB_CHECK(q && k && v && q_offsets && k_offsets && out, "null argument");
-  Seq sq, sk;
-  sq.build(q_offsets, B);
-  sk.build(k_offsets, B);
-  const size_t bytes = ((size_t)sq.rows() * 512 + (size_t)sk.rows() * 512 + 4096) * sizeof(float) + (1 << 16);
-  void* ws = nullptr;
-  SSB_CUDA(cudaMalloc(&ws, bytes));
-  Ctx c = make_ctx(ws, bytes, stream);
-  SeqDev dq, dk;
-  int rc = upload_layout(c, sq, 1, &dq);
-  if (rc == 0) rc = upload_layout(c, sk, 1, &dk);
-  float* qg = alloc_rows(c, dq, 256);
-  float* og = alloc_rows(c, dq, 256);
-  float* kg = alloc_rows(c, dk, 256);
-  float* vg = alloc_rows(c, dk, 256);
-  if (rc == 0 && c.failed) rc = -1;
-  if (rc == 0) rc = pack_rows(c, dq, q, 256, qg, 256, 256);
-  if (rc == 0) rc = pack_rows(c, dk, k, 256, kg, 256, 256);
-  if (rc == 0) rc = pack_rows(c, dk, v, 256, vg, 256, 256);
-  if (rc == 0) {
-    AttnArgs a;
-    a.utt_q = dq.utt; a.utt_k = dk.utt; a.B = B; a.max_q = dq.maxlen; a.heads = 2;
-    a.Q = qg; a.ldq = 256; a.K = kg; a.ldk = 256; a.V = vg; a.ldv = 256; a.scale = scale; a.out = og; a.ldo = 256;
-    rc = attention(c, a);
-  }
-  if (rc == 0) rc = unpack_rows(c, dq, og, 256, out, 256, 256);
-  cudaStreamSynchronize((cudaStream_t)stream);
-  cudaFree(ws);
-  return rc;
+  return ssb_op_attention_masked(q, k, v, q_offsets, k_offsets, B, scale, nullptr, 0, out, stream);
 }
 
 /* wgmma attention kernel at unit-test granularity: same contract as ssb_op_attention (fp32 in / out, tight rows) */
 int ssb_op_attention_tc(const float* q, const float* k, const float* v, const int32_t* q_offsets,
                         const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream) {
+  return ssb_op_attention_masked(q, k, v, q_offsets, k_offsets, B, scale, nullptr, 1, out, stream);
+}
+
+/* Either attention kernel with a key-padding mask (tight [sumS], 0 = masked), packed into the guarded layout the
+ * FFT blocks and the style aligner hand the kernels. */
+int ssb_op_attention_masked(const float* q, const float* k, const float* v, const int32_t* q_offsets,
+                            const int32_t* k_offsets, int32_t B, float scale, const float* keymask, int32_t tc, float* out,
+                            void* stream) {
   SSB_CHECK(q && k && v && q_offsets && k_offsets && out, "null argument");
-  SSB_CHECK(tc_available(), "tensor-core path unavailable (cuTensorMapEncodeTiled)");
+  SSB_CHECK(!tc || tc_available(), "tensor-core path unavailable (cuTensorMapEncodeTiled)");
   Seq sq, sk;
   sq.build(q_offsets, B);
   sk.build(k_offsets, B);
   const int64_t ldvt = (sk.rows() + 7) & ~int64_t(7);
-  const size_t bytes = ((size_t)sq.rows() * 768 + (size_t)sk.rows() * 1024 + (size_t)ldvt * 256 + 4096) * sizeof(float) + (1 << 16);
+  const size_t bytes = ((size_t)sq.rows() * 768 + (size_t)sk.rows() * 1025 + (size_t)ldvt * 256 + 4096) * sizeof(float) + (1 << 16);
   void* ws = nullptr;
   SSB_CUDA(cudaMalloc(&ws, bytes));
   Ctx c = make_ctx(ws, bytes, stream);
@@ -783,26 +763,38 @@ int ssb_op_attention_tc(const float* q, const float* k, const float* v, const in
   float* og = alloc_rows(c, dq, 256);
   float* kg = alloc_rows(c, dk, 256);
   float* vg = alloc_rows(c, dk, 256);
-  __half* pl[6];  // q, k, v planes (hi, lo)
-  for (int i = 0; i < 6; ++i) pl[i] = c.alloc<__half>((size_t)(i < 2 ? dq.rows : dk.rows) * 256);
-  __half* vth = c.alloc<__half>((size_t)ldvt * 256);
-  __half* vtl = c.alloc<__half>((size_t)ldvt * 256);
+  float* mg = keymask ? alloc_rows(c, dk, 1) : nullptr;
   if (rc == 0 && c.failed) rc = -1;
   if (rc == 0) rc = pack_rows(c, dq, q, 256, qg, 256, 256);
   if (rc == 0) rc = pack_rows(c, dk, k, 256, kg, 256, 256);
   if (rc == 0) rc = pack_rows(c, dk, v, 256, vg, 256, 256);
-  if (rc == 0) rc = split_planes(c, qg, 256, dq.rows, 256, 1.0f, pl[0], pl[1]);
-  if (rc == 0) rc = split_planes(c, kg, 256, dk.rows, 256, 1.0f, pl[2], pl[3]);
-  if (rc == 0) rc = split_planes(c, vg, 256, dk.rows, 256, 1.0f, pl[4], pl[5]);
-  if (rc == 0) rc = transpose_planes(c, pl[4], pl[5], 256, 0, dk.rows, 256, vth, vtl, ldvt);
-  if (rc == 0) {
-    AttnTCArgs a;
+  if (rc == 0 && mg) rc = pack_rows(c, dk, keymask, 1, mg, 1, 1);
+  if (rc == 0 && !tc) {
+    AttnArgs a;
     a.utt_q = dq.utt; a.utt_k = dk.utt; a.B = B; a.max_q = dq.maxlen; a.heads = 2;
-    a.Qh = pl[0]; a.Ql = pl[1]; a.rows_q = dq.rows; a.ldq = 256;
-    a.Kh = pl[2]; a.Kl = pl[3]; a.rows_k = dk.rows; a.ldk = 256;
-    a.Vth = vth; a.Vtl = vtl; a.ldvt = ldvt;
-    a.scale = scale; a.out = og; a.ldo = 256;
-    rc = attention_tc(c, a);
+    a.Q = qg; a.ldq = 256; a.K = kg; a.ldk = 256; a.V = vg; a.ldv = 256; a.keymask = mg; a.scale = scale;
+    a.out = og; a.ldo = 256;
+    rc = attention(c, a);
+  }
+  if (rc == 0 && tc) {
+    __half* pl[6];  // q, k, v planes (hi, lo)
+    for (int i = 0; i < 6; ++i) pl[i] = c.alloc<__half>((size_t)(i < 2 ? dq.rows : dk.rows) * 256);
+    __half* vth = c.alloc<__half>((size_t)ldvt * 256);
+    __half* vtl = c.alloc<__half>((size_t)ldvt * 256);
+    if (c.failed) rc = -1;
+    if (rc == 0) rc = split_planes(c, qg, 256, dq.rows, 256, 1.0f, pl[0], pl[1]);
+    if (rc == 0) rc = split_planes(c, kg, 256, dk.rows, 256, 1.0f, pl[2], pl[3]);
+    if (rc == 0) rc = split_planes(c, vg, 256, dk.rows, 256, 1.0f, pl[4], pl[5]);
+    if (rc == 0) rc = transpose_planes(c, pl[4], pl[5], 256, 0, dk.rows, 256, vth, vtl, ldvt);
+    if (rc == 0) {
+      AttnTCArgs a;
+      a.utt_q = dq.utt; a.utt_k = dk.utt; a.B = B; a.max_q = dq.maxlen; a.heads = 2;
+      a.Qh = pl[0]; a.Ql = pl[1]; a.rows_q = dq.rows; a.ldq = 256;
+      a.Kh = pl[2]; a.Kl = pl[3]; a.rows_k = dk.rows; a.ldk = 256;
+      a.Vth = vth; a.Vtl = vtl; a.ldvt = ldvt;
+      a.keymask = mg; a.scale = scale; a.out = og; a.ldo = 256;
+      rc = attention_tc(c, a);
+    }
   }
   if (rc == 0) rc = unpack_rows(c, dq, og, 256, out, 256, 256);
   cudaStreamSynchronize((cudaStream_t)stream);

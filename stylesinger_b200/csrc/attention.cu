@@ -147,7 +147,7 @@ __global__ void __launch_bounds__(256, 1) attention_kernel(AttnArgs a) {
   for (int i = 0; i < 4; ++i) {
     const int row = ty * 4 + i;
     if (row >= nq) continue;
-    const float inv = 1.0f / l_run[i];
+    const float inv = 1.0f / l_run[i];  // no valid key: l = 0 and o = 0, so the row is NaN (attention_tc.cu does the same)
     float* dst = a.out + ((int64_t)uq.x + q0 + row) * a.ldo + hoff;
     *reinterpret_cast<float4*>(dst + tx * 4) = make_float4(o[i][0] * inv, o[i][1] * inv, o[i][2] * inv, o[i][3] * inv);
     *reinterpret_cast<float4*>(dst + 64 + tx * 4) = make_float4(o[i][4] * inv, o[i][5] * inv, o[i][6] * inv, o[i][7] * inv);

@@ -245,8 +245,9 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_con
       l0 += __shfl_xor_sync(0xffffffffu, l0, x);
       l1 += __shfl_xor_sync(0xffffffffu, l1, x);
     }
-    // epilogue: O / (256 l)
-    const float inv0 = l0 > 0.f ? 1.0f / (256.0f * l0) : 0.f, inv1 = l1 > 0.f ? 1.0f / (256.0f * l1) : 0.f;
+    // epilogue: O / (256 l).  l >= 1 when any key is valid (the maximum contributes exp2(0)); a row without one has l = 0 and
+    // O = 0 and writes 0 * inf = NaN, like the fp32 kernel and torch's softmax over all -inf
+    const float inv0 = 1.0f / (256.0f * l0), inv1 = 1.0f / (256.0f * l1);
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int qr = 64 * cw + rw + 8 * hh;  // query row inside the tile

@@ -637,13 +637,22 @@ def op_conv1d_tc(x, offsets, w, b, dilation=1):
     return out
 
 
-def op_attention(q, k, v, q_offsets, k_offsets, scale, tc=False):
-    """tc=True: the wgmma / TMA kernel (ssb_op_attention_tc) instead of the fp32 one."""
+def op_attention(q, k, v, q_offsets, k_offsets, scale, tc=False, keymask=None):
+    """tc=True: the wgmma / TMA kernel (ssb_op_attention_tc) instead of the fp32 one.  keymask: optional [sumS] tensor on
+    q's device, 0 = masked key (ssb_op_attention_masked); an utterance whose keys are all masked gets NaN rows."""
     _require_cuda()
     qo = np.ascontiguousarray(q_offsets, np.int32)
     ko = np.ascontiguousarray(k_offsets, np.int32)
     out = torch.empty_like(q)
     stream = C.c_void_p(torch.cuda.current_stream(q.device).cuda_stream)
+    if keymask is not None:
+        km = keymask.to(device=q.device, dtype=torch.float32).contiguous()
+        if km.shape != (k.shape[0],):
+            raise ValueError(f"keymask must have shape ({k.shape[0]},), got {tuple(km.shape)}")
+        check(lib.ssb_op_attention_masked(_ptr(q), _ptr(k), _ptr(v), qo.ctypes.data, ko.ctypes.data, len(qo) - 1,
+                                          float(scale), _ptr(km), 1 if tc else 0, _ptr(out), stream),
+              "ssb_op_attention_masked")
+        return out
     fn = lib.ssb_op_attention_tc if tc else lib.ssb_op_attention
     check(fn(_ptr(q), _ptr(k), _ptr(v), qo.ctypes.data, ko.ctypes.data, len(qo) - 1, float(scale),
              _ptr(out), stream), "ssb_op_attention_tc" if tc else "ssb_op_attention")

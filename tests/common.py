@@ -39,6 +39,11 @@ def utt_from_meta(meta):
                                 frames=meta["frames"], phones=meta["phones"])
 
 
+def utt_from_fixture(g):
+    """The inputs a fixture stores as in_* arrays (padded inputs that synth.make_utterance cannot rebuild)."""
+    return {k[3:]: torch.from_numpy(np.array(g[k])) for k in g.files if k.startswith("in_")}
+
+
 def oracle_forward(u, hp, seed, use_mel2ph=True, **kw):
     ns = O.NoiseSource(seed)
     with torch.no_grad():

@@ -135,6 +135,52 @@ def case_model(name, T, frames, phones, ref_frames, seed, utt_idx, with_dur_case
     print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()})
 
 
+def padded_utterance(frames, phones, ref_frames, utt_idx, pad_phones=3, gap=(52, 60), tail_frames=10,
+                     ref_tail=8, ref_col0_row=17):
+    """A synthetic utterance with every kind of padding the model masks: `pad_phones` trailing padding phones (token,
+    note, note_type and note_dur 0), an interior run `gap` and a trailing run of padding frames (mel2ph 0), `ref_tail`
+    all-zero reference-mel rows at the end (ref_f0 0 there) and one interior reference row whose column 0 alone is 0
+    (column-0 masks drop it, whole-row masks keep it)."""
+    u = synth.make_utterance(frames / 187.5, utt_idx=utt_idx, ref_frames=ref_frames, frames=frames, phones=phones)
+    for k in ("txt_tokens", "note", "note_type", "note_dur"):
+        u[k] = torch.cat([u[k], torch.zeros(pad_phones, dtype=u[k].dtype)])
+    u["mel2ph"][gap[0]:gap[1]] = 0
+    u["mel2ph"][frames - tail_frames:] = 0
+    u["ref_mels"][ref_frames - ref_tail:] = 0
+    u["ref_f0"][ref_frames - ref_tail:] = 0
+    u["ref_mels"][ref_col0_row, 0] = 0
+    return u
+
+
+UTT_KEYS = ("txt_tokens", "note", "note_dur", "note_type", "mel2ph", "spk_embed", "emo_embed", "ref_mels", "ref_f0")
+
+
+def case_padded(name, T=4, frames=120, phones=12, ref_frames=48, seed=91, utt_idx=104):
+    """Padding phones, padding frames (interior and trailing) and a padded reference mel through the full forward, with
+    mel2ph given and through the duration path.  The inputs are stored in the fixture (in_*): they are not what
+    synth.make_utterance returns."""
+    model, hp, sd = build_reference_model(T)
+    u = padded_utterance(frames, phones, ref_frames, utt_idx)
+    out, log = run_model(model, u, seed)
+    coarse, _ = run_model(model, u, seed, global_steps=50000)
+    o2, log2 = run_model(model, u, seed + 1, mel2ph=False)
+    d = {
+        "meta": json.dumps({"T": T, "frames": frames, "phones": phones, "ref_frames": ref_frames, "seed": seed,
+                            "utt_idx": utt_idx, "noise_log": log, "dur_noise_log": log2}),
+        "style": np32(out["style"][0]), "rq_codes": out["rq_codes"][0].numpy().astype(np.int64),
+        "rq_in": np32(out["rq_in"][0]),
+        "pitch_pred": np32(out["pitch_pred"][0]), "f0_denorm": np32(out["f0_denorm"][0]),
+        "decoder_inp": np32(out["decoder_inp"][0]), "coarse_mel": np32(coarse["mel_out"][0]),
+        "mel_out": np32(out["mel_out"][0]),
+        "dur_mel2ph": o2["mel2ph"][0].numpy().astype(np.int64), "dur_logdur": np32(o2["dur"][0]),
+        "dur_mel_out": np32(o2["mel_out"][0]), "dur_f0_denorm": np32(o2["f0_denorm"][0]),
+    }
+    for k in UTT_KEYS:
+        d["in_" + k] = u[k].numpy()
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()})
+
+
 def case_vocoder(name, frames, seed):
     import ref_import
     ref_import.install(T=4)
@@ -289,13 +335,15 @@ def case_emotion_encoder(name, partials=5, seed=71):
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
-    which = sys.argv[1:] or ["small", "t25", "t100", "plms", "prodiff", "sched", "voc", "emo"]
+    which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "sched", "voc", "emo"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
         case_model("ref_f64_T25", T=25, frames=64, phones=8, ref_frames=48, seed=21, utt_idx=101, with_dur_case=False)
     if "t100" in which:  # the bench's step count (T=100 mel + 2 x 100 F0 steps) on a tiny utterance
         case_model("ref_f32_T100", T=100, frames=32, phones=4, ref_frames=32, seed=41, utt_idx=102, with_dur_case=False)
+    if "padded" in which:
+        case_padded("ref_padded_T4")
     if "plms" in which:
         case_plms("ref_plms_T100_i10")
     if "prodiff" in which:

@@ -661,40 +661,44 @@ def source_module(f0_up, sd, noise):
     return har
 
 
-def hifigan_generator(mel, f0, sd, h, noise):
+def hifigan_generator(mel, f0, sd, h, noise, dtype=torch.float32):
     """HifiGanGenerator.forward after remove_weight_norm (hifigan_nsf.py:144-178).
-    mel [B,80,F], f0 [B,F] or None -> wav [B,1,256F]."""
+    mel [B,80,F], f0 [B,F] or None -> wav [B,1,256F] in `dtype`.
+    dtype=torch.float64 runs the conv stack, the leaky ReLUs and the tanh in double precision: an arbiter for the CUDA
+    path.  The NSF source stays fp32 whatever `dtype` is: the reference accumulates the phase with an fp32 cumsum and the
+    CUDA kernel reproduces that rounding; a float64 phase drifts from both by ~1e-2 over 10 s."""
     rates, ks = h["upsample_rates"], h["upsample_kernel_sizes"]
     nk = len(h["resblock_kernel_sizes"])
-    W = lambda n: fold_weight_norm(sd[n + ".weight_g"], sd[n + ".weight_v"])
+    W = lambda n: fold_weight_norm(sd[n + ".weight_g"], sd[n + ".weight_v"]).to(dtype)
+    P = lambda n: sd[n].to(dtype)
     har = None
     if f0 is not None:
         up = f0[:, None].repeat_interleave(int(np.prod(rates)), dim=2).transpose(1, 2)
-        har = source_module(up, sd, noise).transpose(1, 2)
-    x = F.conv1d(mel, W("conv_pre"), sd["conv_pre.bias"], padding=3)
+        har = source_module(up, sd, noise).transpose(1, 2).to(dtype)
+    x = F.conv1d(mel.to(dtype), W("conv_pre"), P("conv_pre.bias"), padding=3)
     for i, (u, k) in enumerate(zip(rates, ks)):
         x = F.leaky_relu(x, 0.1)
-        x = F.conv_transpose1d(x, W(f"ups.{i}"), sd[f"ups.{i}.bias"], stride=u, padding=(k - u) // 2)
+        x = F.conv_transpose1d(x, W(f"ups.{i}"), P(f"ups.{i}.bias"), stride=u, padding=(k - u) // 2)
         if har is not None:
             if i + 1 < len(rates):
                 s = int(np.prod(rates[i + 1:]))
-                x = x + F.conv1d(har, sd[f"noise_convs.{i}.weight"], sd[f"noise_convs.{i}.bias"], stride=s, padding=s // 2)
+                x = x + F.conv1d(har, P(f"noise_convs.{i}.weight"), P(f"noise_convs.{i}.bias"), stride=s, padding=s // 2)
             else:
-                x = x + F.conv1d(har, sd[f"noise_convs.{i}.weight"], sd[f"noise_convs.{i}.bias"])
+                x = x + F.conv1d(har, P(f"noise_convs.{i}.weight"), P(f"noise_convs.{i}.bias"))
         xs = None
         for j, (rk, rd) in enumerate(zip(h["resblock_kernel_sizes"], h["resblock_dilation_sizes"])):
             r = x
             q = f"resblocks.{i * nk + j}."
             for m_, d in enumerate(rd):
                 xt = F.leaky_relu(r, 0.1)
-                xt = F.conv1d(xt, W(f"{q}convs1.{m_}"), sd[f"{q}convs1.{m_}.bias"], padding=(rk * d - d) // 2, dilation=d)
+                xt = F.conv1d(xt, W(f"{q}convs1.{m_}"), P(f"{q}convs1.{m_}.bias"), padding=(rk * d - d) // 2, dilation=d)
                 xt = F.leaky_relu(xt, 0.1)
-                xt = F.conv1d(xt, W(f"{q}convs2.{m_}"), sd[f"{q}convs2.{m_}.bias"], padding=(rk - 1) // 2)
+                xt = F.conv1d(xt, W(f"{q}convs2.{m_}"), P(f"{q}convs2.{m_}.bias"), padding=(rk - 1) // 2)
                 r = xt + r
             xs = r if xs is None else xs + r
         x = xs / nk
     x = F.leaky_relu(x)  # default slope 0.01 (hifigan_nsf.py:165)
-    x = F.conv1d(x, W("conv_post"), sd["conv_post.bias"], padding=3)
+    x = F.conv1d(x, W("conv_post"), P("conv_post.bias"), padding=3)
     return torch.tanh(x)
 
 
@@ -709,8 +713,9 @@ def postprocess_mel(mel_out, f0_denorm, hp):
     return mel, f0[mask]
 
 
-def spec2wav(mel, f0, vsd, h, noise):
-    """HifiGAN.spec2wav (tasks/tts/vocoder_infer/hifigan_nsf.py:62-75). mel np [F,80], f0 np [F] -> wav np."""
+def spec2wav(mel, f0, vsd, h, noise, dtype=torch.float32):
+    """HifiGAN.spec2wav (tasks/tts/vocoder_infer/hifigan_nsf.py:62-75). mel np [F,80], f0 np [F] -> wav np in `dtype`
+    (see hifigan_generator)."""
     c = torch.from_numpy(np.ascontiguousarray(mel)).float().unsqueeze(0).transpose(2, 1)
     f = None if f0 is None else torch.from_numpy(np.ascontiguousarray(f0)).float()[None, :]
-    return hifigan_generator(c, f, vsd, h, noise).view(-1).numpy()
+    return hifigan_generator(c, f, vsd, h, noise, dtype).view(-1).numpy()

@@ -208,6 +208,47 @@ def case_vocoder(name, frames, seed):
     print("wrote", name, y.shape, float(y.abs().max()), float(y.std()))
 
 
+VOCODER_EDGE_LENGTHS = (1, 2, 3, 5, 17)
+
+
+def case_vocoder_edges(name, lengths=VOCODER_EDGE_LENGTHS, seed=37):
+    """The reference HifiGanGenerator (B = 1) on utterances shorter than conv_pre's reach of 3 frames and just past a
+    16-frame tile, with and without f0.  f0 alternates voiced / unvoiced every frame; the 5- and 17-frame utterances
+    carry one frame at ~1100 Hz (9 harmonics up to ~9.9 kHz) and the 3-frame one is entirely unvoiced.  Every mel holds
+    values at both clip bounds (-6 and 1.5).  The inputs are stored (mel_<L>, f0_<L>); the noise of length L is drawn from
+    NoiseSource(seed + L), logged in meta."""
+    import ref_import
+    ref_import.install(T=4)
+    from modules.hifigan.hifigan_nsf import HifiGanGenerator
+    h = dict(DEFAULT_VOCODER_CONFIG)
+    gen = HifiGanGenerator(h)
+    gen.load_state_dict(synth.vocoder_state_dict(h, seed=0), strict=True)
+    gen.remove_weight_norm()
+    gen.eval()
+    g = torch.Generator().manual_seed(seed)
+    d, logs = {}, {}
+    for L in lengths:
+        mel = (-3.0 + 2.0 * torch.randn(L, 80, generator=g)).clamp(-6, 1.5)
+        mel[:, 0], mel[:, 79] = -6.0, 1.5
+        f0 = 150 + 350 * torch.rand(L, generator=g)
+        f0[1::2] = 0
+        if L == 3:
+            f0[:] = 0
+        if L in (5, 17):
+            f0[2] = 1100.0
+        ns = NoiseSource(seed + L)
+        with torch.no_grad(), patched_rng(ns):
+            c = mel.t()[None].contiguous()
+            y = gen(c, f0[None].clone()).view(-1)
+        with torch.no_grad():
+            y_nof0 = gen(c).view(-1)
+        logs[L] = ns.log
+        d.update({f"mel_{L}": np32(mel), f"f0_{L}": np32(f0), f"wav_{L}": np32(y), f"wav_nof0_{L}": np32(y_nof0)})
+    d["meta"] = json.dumps({"lengths": list(lengths), "seed": seed, "noise_log": {str(k): v for k, v in logs.items()}})
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, {k: v.shape for k, v in d.items() if k != "meta"})
+
+
 def case_plms(name, T=100, interval=10, frames=48, seed=61):
     """f2: the reference's PLMS sampler (GaussianDiffusion.p_sample_plms, shallow_diffusion_tts.py:164-197) driven exactly
     as GaussianDiffusion.forward does under hparams['pndm_speedup'] (:254-260), on the StyleSinger mel denoiser (the
@@ -335,7 +376,7 @@ def case_emotion_encoder(name, partials=5, seed=71):
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
-    which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "sched", "voc", "emo"]
+    which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "sched", "voc", "vocoder_edges", "emo"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
@@ -352,5 +393,7 @@ if __name__ == "__main__":
         case_schedules("ref_schedules")
     if "voc" in which:
         case_vocoder("ref_vocoder_f24", frames=24, seed=31)
+    if "vocoder_edges" in which:
+        case_vocoder_edges("ref_vocoder_edges")
     if "emo" in which:
         case_emotion_encoder("ref_emotion_encoder")

@@ -95,6 +95,19 @@ void ssb_model_free(ssb_model_t* m);
 int ssb_model_create_ex(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
                         int32_t mel_decoder);
 
+/* hparams['f0_gen'] (modules/StyleSinger/stylesinger.py:66-82,223-228): which F0 generator the model was built with. */
+#define SSB_F0_GEN_GMDIFF 0 /* two 100-step Gaussian-multinomial diffusion samplers over gm_diffnet(_inpainte) (the default) */
+#define SSB_F0_GEN_CONV 1   /* two FastSpeech-2 PitchPredictors (modules/fastspeech/tts_modules.py:191-234): deterministic */
+/* ssb_model_create_ex with the F0 generator chosen as well: ssb_model_create_ex(..., d) ==
+ * ssb_model_create_ex2(..., d, SSB_F0_GEN_GMDIFF).  CONV loads "pitch_predictor.*" (domain agnostic) and
+ * "pitch_inpainter_predictor.*" (domain specific): per predictor conv.{0..4}.1.weight [256,256,k] (k odd, (k-1)/2 <= 16) /
+ * .bias, conv.{i}.3.weight / .bias (LayerNorm), linear.weight [2,256] / .bias and pos_embed_alpha [1]; "gm_diffnet*" and
+ * "f0_gen*" are neither required nor packed.  On a CONV model the F0 schedule (ssb_model_set_schedule, which = 1),
+ * ssb_f0_diffusion_sample, ssb_denoiser_eval(which = 1 / 2) and F0 noise pointers in ssb_acoustic_inputs are errors; on a
+ * GMDIFF model ssb_pitch_predictor is.  An unknown mel_decoder or f0_gen fails before any CUDA call. */
+int ssb_model_create_ex2(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
+                         int32_t mel_decoder, int32_t f0_gen);
+
 /* Diffusion schedules (GaussianDiffusion.__init__ modules/diff/shallow_diffusion_tts.py:68-122;
  * GaussianMultinomialDiffusion.__init__ modules/diff/gaussian_multinomial_diffusion.py:208-284).
  * which: 0 = mel denoiser, 1 = both F0 denoisers.  Host arrays:
@@ -158,7 +171,11 @@ int ssb_predict_durations(const ssb_model_t* m, const ssb_acoustic_inputs* in, i
 
 /* StyleSinger.forward(infer=True, global_steps > diff_start): rows a1-a19 of SURVEY.md §8.
  * On a PRODIFF model (stylesinger.py:174-177): decoder_inp goes straight to the ProDiff sampler (no FFT decoder, mel_out or
- * ln_proj); pndm_speedup is ignored like the reference ignores it; asking for coarse_mel or diff_cond is an error. */
+ * ln_proj); pndm_speedup is ignored like the reference ignores it; asking for coarse_mel or diff_cond is an error.
+ * On a CONV F0 model (inpaint_pitch, stylesinger.py:216-247): pitch_pred = specific/2 + agnostic/2 of the two
+ * PitchPredictors (always run, also with teacher-forced f0); f0 = pitch_pred[..., 0] in log2 Hz with no MIDI band or
+ * de-normalisation, uv = pitch_pred[..., 1] > 0, rests not forced unvoiced; no F0 noise is drawn (mel_noise is then the
+ * forward's only noise), and non-NULL f0_gauss_noise / f0_unif_noise are an error. */
 size_t ssb_acoustic_workspace_bytes(const ssb_model_t* m, const ssb_acoustic_inputs* in);
 int ssb_acoustic_forward(const ssb_model_t* m, const ssb_acoustic_inputs* in, const ssb_acoustic_outputs* out,
                          void* workspace, size_t workspace_bytes, void* stream);
@@ -201,6 +218,16 @@ int ssb_f0_diffusion_sample(const ssb_model_t* m, int32_t which, const float* co
                             const float* clip_hi, const int32_t* frame_offsets, int32_t B, const float* gauss_noise,
                             const float* unif_noise, uint64_t seed, float* f0_norm_out, int32_t* uv_out,
                             void* workspace, size_t workspace_bytes, void* stream);
+
+/* PitchPredictor.forward(xs) alone (modules/fastspeech/tts_modules.py:191-234), CONV F0 models only.  which: 0
+ * pitch_predictor (run on decoder_inp * tgt_nonpadding), 1 pitch_inpainter_predictor (run on (decoder_inp + spk + emo +
+ * style) * tgt_nonpadding), stylesinger.py:155-163,223-225.  x [sumF,256] -> out [sumF,2] (log2-Hz f0, uv logit).  Per
+ * utterance: x += pos_embed_alpha * sinusoid[make_positions(x[:, 0])] (a row whose channel 0 is exactly 0 gets position 0
+ * and does not advance the count), then 5 x (zero SAME pad, Conv1d 256 -> 256 + bias, ReLU, LayerNorm over channels eps
+ * 1e-5), then Linear 256 -> 2; no mask anywhere (the reference applies none). */
+size_t ssb_pitch_predictor_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B);
+int ssb_pitch_predictor(const ssb_model_t* m, int32_t which, const float* x, const int32_t* frame_offsets, int32_t B,
+                        float* out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Per-registry drop-ins (SURVEY.md section 8b).  The reference dispatches through FS_ENCODERS / FS_DECODERS
  * (modules/fastspeech/fs2.py:9-18,30-31) and calls StyleSinger.get_style (modules/StyleSinger/stylesinger.py:189-214):

@@ -64,6 +64,7 @@ EXPORTS = [
     "ssb_melspec_create_ex", "ssb_lstm_encoder_create", "ssb_lstm_encoder_free", "ssb_lstm_encoder_workspace_bytes", "ssb_lstm_encoder_forward",
     "ssb_model_create_ex", "ssb_mel_prodiff_workspace_bytes", "ssb_mel_prodiff_sample",
     "ssb_op_attention_masked",
+    "ssb_model_create_ex2", "ssb_pitch_predictor_workspace_bytes", "ssb_pitch_predictor",
 ]
 
 
@@ -79,6 +80,9 @@ def _load():
         "ssb_last_error": (C.c_char_p, []),
         "ssb_model_create": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams)]),
         "ssb_model_create_ex": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32]),
+        "ssb_model_create_ex2": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32, i32]),
+        "ssb_pitch_predictor_workspace_bytes": (sz, [vp, vp, i32]),
+        "ssb_pitch_predictor": (C.c_int, [vp, i32, vp, vp, i32, vp, vp, sz, vp]),
         "ssb_model_free": (None, [vp]),
         "ssb_model_set_schedule": (C.c_int, [vp, i32, i32, vp, vp, vp, vp]),
         "ssb_durations_workspace_bytes": (sz, [vp, P(AcousticInputs)]),

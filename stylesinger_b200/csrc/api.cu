@@ -51,6 +51,9 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   SSB_CHECK(durations_only || in.mel2ph || in.dur, "acoustic: need mel2ph or dur");
   SSB_CHECK(m.mel_decoder != SSB_MEL_DECODER_PRODIFF || (!out.coarse_mel && !out.diff_cond),
             "acoustic: a ProDiff model has no coarse_mel / diff_cond (decoder_inp is the sampler's condition)");
+  SSB_CHECK(m.f0_gen != SSB_F0_GEN_CONV || (!in.f0_gauss_noise[0] && !in.f0_gauss_noise[1] && !in.f0_unif_noise[0] &&
+                                            !in.f0_unif_noise[1]),
+            "acoustic: a model with the conv F0 generator draws no F0 noise (f0_gauss_noise / f0_unif_noise must be NULL)");
   Seq qp, qr, qf;
   qp.build(in.ph_offsets, B);
   qr.build(in.ref_offsets, B);
@@ -130,7 +133,44 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   float* f0_in = nullptr;
   float* uv_in = nullptr;
   WS_OK(c);
-  {
+  if (m.f0_gen == SSB_F0_GEN_CONV) {
+    // f0_gen 'conv' (:223-236): both PitchPredictors always run (teacher-forced f0 only replaces f0 / uv); no MIDI band,
+    // no noise
+    const size_t mk = c.mark();
+    float* cond = alloc_rows(c, sf, H);
+    float* cond2 = alloc_rows(c, sf, H);
+    float* pa = alloc_rows(c, sf, 2);
+    float* ps = alloc_rows(c, sf, 2);
+    WS_OK(c);
+    if (in.f0) {
+      f0_in = alloc_rows(c, sf, 1);
+      uv_in = alloc_rows(c, sf, 1);
+      WS_OK(c);
+      RUN(pack_rows(c, sf, in.f0, 1, f0_in, 1, 1));
+      if (in.uv) RUN(pack_rows(c, sf, in.uv, 1, uv_in, 1, 1));
+    }
+    {
+      CombineArgs a;  // pitch_inp_domain_agnostic = decoder_inp * tgt_nonpadding (:156)
+      a.m[0] = dec0; a.ldm[0] = H; a.rowmask = tgt; a.out = cond; a.ldo = H; a.C = H;
+      RUN(combine_rows(c, sf, a));
+    }
+    {
+      CombineArgs a;  // (decoder_inp + spk + emo + style) * tgt_nonpadding (:157-162)
+      a.m[0] = dec0; a.ldm[0] = H; a.m[1] = style; a.ldm[1] = H; a.v[0] = spk; a.v[1] = emo;
+      a.rowmask = tgt; a.out = cond2; a.ldo = H; a.C = H;
+      RUN(combine_rows(c, sf, a));
+    }
+    // the FFT decoder's rule for its FFN GEMMs: long batches on the tensor-core kernel
+    const bool tc = m.use_tc && m.fft_tc && tc_available() && sf.ntiles >= 8;
+    RUN(run_pitch_predictor(c, m, 0, sf, cond, pa, tc));
+    RUN(run_pitch_predictor(c, m, 1, sf, cond2, ps, tc));
+    PitchGlueConvArgs pg;
+    pg.pa = pa; pg.ps = ps; pg.mel2ph = mel2ph;
+    pg.f0_in = f0_in; pg.uv_in = in.uv ? uv_in : nullptr;
+    pg.pitch_pred = pitch_pred; pg.f0_denorm = f0_denorm; pg.pitch = pitch;
+    RUN(pitch_glue_conv(c, sf, pg));
+    c.release(mk);
+  } else {
     const size_t mk = c.mark();
     float* za = alloc_rows(c, sf, 1);
     float* zs = alloc_rows(c, sf, 1);
@@ -297,14 +337,21 @@ int ssb_model_create(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t 
 }
 int ssb_model_create_ex(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
                         int32_t mel_decoder) {
+  return ssb_model_create_ex2(out, tensors, n, hp, mel_decoder, SSB_F0_GEN_GMDIFF);
+}
+int ssb_model_create_ex2(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
+                         int32_t mel_decoder, int32_t f0_gen) {
   SSB_CHECK(mel_decoder == SSB_MEL_DECODER_DIFFSINGER || mel_decoder == SSB_MEL_DECODER_PRODIFF,
             "ssb_model_create_ex: unknown mel_decoder " + std::to_string(mel_decoder) +
                 " (SSB_MEL_DECODER_DIFFSINGER = 0, SSB_MEL_DECODER_PRODIFF = 1)");
+  SSB_CHECK(f0_gen == SSB_F0_GEN_GMDIFF || f0_gen == SSB_F0_GEN_CONV,
+            "ssb_model_create_ex2: unknown f0_gen " + std::to_string(f0_gen) +
+                " (SSB_F0_GEN_GMDIFF = 0, SSB_F0_GEN_CONV = 1)");
   SSB_CHECK(out && tensors && hp, "ssb_model_create: null argument");
   TensorMap tm;
   if (to_map(tensors, n, &tm)) return -1;
   ssb_model* m = new ssb_model();
-  if (build_model(tm, *hp, &m->m, mel_decoder) != 0) {
+  if (build_model(tm, *hp, &m->m, mel_decoder, f0_gen) != 0) {
     delete m;
     return -1;
   }
@@ -440,6 +487,8 @@ int ssb_denoiser_eval(const ssb_model_t* m, int32_t which, const float* x, const
                       const float* cond, const int32_t* frame_offsets, int32_t B, float* out, void* workspace,
                       size_t workspace_bytes, void* stream) {
   SSB_CHECK(m && x && cond && frame_offsets && out && workspace && which >= 0 && which <= 2, "bad argument");
+  SSB_CHECK(which == 0 || m->m.f0_gen == SSB_F0_GEN_GMDIFF,
+            "ssb_denoiser_eval: a model with the conv F0 generator (SSB_F0_GEN_CONV) has no F0 denoisers (which = 1 / 2)");
   Ctx c = make_ctx(workspace, workspace_bytes, stream);
   Seq q;
   q.build(frame_offsets, B);
@@ -454,6 +503,9 @@ int ssb_f0_diffusion_sample(const ssb_model_t* m, int32_t which, const float* co
                             void* workspace, size_t workspace_bytes, void* stream) {
   SSB_CHECK(m && cond && clip_lo && clip_hi && frame_offsets && f0_norm_out && uv_out && workspace, "null argument");
   SSB_CHECK(which == 0 || which == 1, "which must be 0 or 1");
+  SSB_CHECK(m->m.f0_gen == SSB_F0_GEN_GMDIFF,
+            "ssb_f0_diffusion_sample: a model with the conv F0 generator (SSB_F0_GEN_CONV) has no F0 sampler; use "
+            "ssb_pitch_predictor");
   Ctx c = make_ctx(workspace, workspace_bytes, stream);
   Seq q;
   q.build(frame_offsets, B);
@@ -472,6 +524,33 @@ int ssb_f0_diffusion_sample(const ssb_model_t* m, int32_t which, const float* co
   RUN(unpack_rows(c, s, z, 1, f0_norm_out, 1, 1));
   RUN(unpack_rows_i32(c, s, uv, uv_out));
   return 0;
+}
+
+static int pitch_predictor_impl(Ctx& c, const Model& m, int which, const float* x, const int32_t* offs, int B, float* out) {
+  SSB_CHECK(m.f0_gen == SSB_F0_GEN_CONV,
+            "ssb_pitch_predictor: the PitchPredictors need a model created with SSB_F0_GEN_CONV (a gmdiff model samples F0)");
+  Seq q;
+  q.build(offs, B);
+  SSB_CHECK(q.maxlen + 2 <= m.pos_rows, "frame sequence longer than __pos_table");
+  SeqDev s;
+  RUN(upload_layout(c, q, 1, &s));
+  float* xg = alloc_rows(c, s, 256);
+  float* og = alloc_rows(c, s, 2);
+  WS_OK(c);
+  RUN(pack_rows(c, s, x, 256, xg, 256, 256));
+  RUN(run_pitch_predictor(c, m, which, s, xg, og, m.use_tc && m.fft_tc && tc_available() && s.ntiles >= 8));
+  return unpack_rows(c, s, og, 2, out, 2, 2);
+}
+size_t ssb_pitch_predictor_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B) {
+  Ctx c = make_ctx(nullptr, 0, nullptr, true);
+  if (pitch_predictor_impl(c, m->m, 0, nullptr, frame_offsets, B, nullptr) != 0) return 0;
+  return c.high + 4096;
+}
+int ssb_pitch_predictor(const ssb_model_t* m, int32_t which, const float* x, const int32_t* frame_offsets, int32_t B,
+                        float* out, void* workspace, size_t workspace_bytes, void* stream) {
+  SSB_CHECK(m && x && frame_offsets && out && workspace, "null argument");
+  Ctx c = make_ctx(workspace, workspace_bytes, stream);
+  return pitch_predictor_impl(c, m->m, which, x, frame_offsets, B, out);
 }
 
 // ---- per-registry drop-ins (FS_ENCODERS / FS_DECODERS 'fft', StyleSinger.get_style) ------------------------------------

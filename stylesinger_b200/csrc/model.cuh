@@ -93,6 +93,17 @@ struct Denoiser {
   float* skip_bias_pad = nullptr;
 };
 
+// FastSpeech-2 PitchPredictor (tts_modules.py:191-234): f0_gen 'conv' only
+struct PitchPredictor {
+  static constexpr int kLayers = 5;
+  Conv conv[kLayers];       // k-tap Conv1d 256 -> 256 + bias (fp32 path)
+  ConvTC conv_tc[kLayers];  // the same convs for the tensor-core kernel (long batches)
+  float* ln_g[kLayers] = {};
+  float* ln_b[kLayers] = {};
+  Conv linear;              // 256 -> 2
+  float* pos_alpha = nullptr;  // device scalar
+};
+
 struct AlignLayer {
   Conv q, kv, out, lin1, lin2;
   ConvTC q_tc, kv_tc, out_tc, lin1_tc, lin2_tc;  // tensor-core packing of the same projections (long batches)
@@ -119,7 +130,10 @@ struct Model {
   float* codebooks = nullptr; float* cb_norm2 = nullptr;  // [depth][n_embed][256], [depth][n_embed]
   Conv l1;
   AlignLayer align[2];
-  Denoiser f0net[2];
+  Denoiser f0net[2];        // GMDIFF only
+  PitchPredictor pp[2];     // CONV only: [0] pitch_predictor (domain agnostic), [1] pitch_inpainter_predictor (specific)
+  // SSB_F0_GEN_GMDIFF: hparams['f0_gen'] == 'gmdiff' (two F0 diffusion samplers); SSB_F0_GEN_CONV: 'conv' (pp above)
+  int f0_gen = SSB_F0_GEN_GMDIFF;
   Denoiser melnet;
   Conv mel_out, ln_proj;  // DiffSinger mode only
   // SSB_MEL_DECODER_DIFFSINGER: hparams['decoder'] == 'diffsinger' (FFT decoder + mel_out + ln_proj + DDPM over postdiff.*);
@@ -163,7 +177,8 @@ int pack_conv(DevicePool& pool, const HostTensor* w, const HostTensor* b, int di
 int pack_conv_tc(DevicePool& pool, const HostTensor* w, int dil, PackMode mode, const float* packed_bias, ConvTC* out);
 int pack_linear(DevicePool& pool, const HostTensor* w, const HostTensor* b, Conv* out, int row0 = 0, int nrows = -1);
 int pack_conv_transpose(DevicePool& pool, const HostTensor* v, const HostTensor* g, const HostTensor* b, int u, Conv* out);
-int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder = SSB_MEL_DECODER_DIFFSINGER);
+int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder = SSB_MEL_DECODER_DIFFSINGER,
+                int f0_gen = SSB_F0_GEN_GMDIFF);
 int build_vocoder(TensorMap& tm, const ssb_vocoder_config& cfg, Vocoder* v);
 int set_schedule(Model* m, int which, int T, const float* step_emb, const float* gtab, const float* mtab,
                  cudaStream_t stream);

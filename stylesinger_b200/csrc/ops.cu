@@ -419,6 +419,22 @@ __global__ void k_midi_band(const int4* utt, const int32_t* midi, float* lo, flo
   hi[r] = fminf(fmaxf(minmax_norm_(up), -1.f), 1.f);
   lo[r] = fminf(fmaxf(minmax_norm_(dn), -1.f), 1.f);
 }
+// The tail of inpaint_pitch shared by both F0 generators (stylesinger.py:237-243): f0 (log2 Hz) and uv of row r ->
+// f0_denorm (Hz) and the coarse pitch bin.
+__device__ __forceinline__ void f0_denorm_coarse(float f0, bool uv, int32_t mel2ph, float* f0_denorm, int32_t* pitch) {
+  float hz = exp2f(f0);  // denorm_f0, pitch_norm == 'log' (utils/pitch_utils.py:65-78)
+  if (uv) hz = 0.f;
+  if (mel2ph == 0) hz = 0.f;
+  *f0_denorm = hz;
+  // f0_to_coarse (utils/pitch_utils.py:22-31)
+  const float mel_min = 1127.0f * logf(1.0f + 50.0f / 700.0f);
+  const float mel_max = 1127.0f * logf(1.0f + 1100.0f / 700.0f);
+  float mel = 1127.0f * logf(1.0f + hz / 700.0f);
+  if (mel > 0.f) mel = (mel - mel_min) * 254.0f / (mel_max - mel_min) + 1.0f;
+  if (mel <= 1.f) mel = 1.f;
+  if (mel > 255.f) mel = 255.f;
+  *pitch = (int32_t)(mel + 0.5f);
+}
 __global__ void k_pitch_glue(const int4* utt, PitchGlueArgs a) {
   ROW_SETUP();
   if (threadIdx.x != 0) return;
@@ -432,18 +448,19 @@ __global__ void k_pitch_glue(const int4* utt, PitchGlueArgs a) {
   if (a.pitch_pred) { a.pitch_pred[r * 2] = pf; a.pitch_pred[r * 2 + 1] = pu; }
   float f0 = a.f0_in ? a.f0_in[r] : pf;
   const bool uv = a.f0_in ? (a.uv_in ? a.uv_in[r] > 0.f : false) : (pu > 0.f);
-  float hz = exp2f(f0);  // denorm_f0, pitch_norm == 'log' (utils/pitch_utils.py:65-78)
-  if (uv) hz = 0.f;
-  if (a.mel2ph[r] == 0) hz = 0.f;
-  a.f0_denorm[r] = hz;
-  // f0_to_coarse (utils/pitch_utils.py:22-31)
-  const float mel_min = 1127.0f * logf(1.0f + 50.0f / 700.0f);
-  const float mel_max = 1127.0f * logf(1.0f + 1100.0f / 700.0f);
-  float mel = 1127.0f * logf(1.0f + hz / 700.0f);
-  if (mel > 0.f) mel = (mel - mel_min) * 254.0f / (mel_max - mel_min) + 1.0f;
-  if (mel <= 1.f) mel = 1.f;
-  if (mel > 255.f) mel = 255.f;
-  a.pitch[r] = (int32_t)(mel + 0.5f);
+  f0_denorm_coarse(f0, uv, a.mel2ph[r], &a.f0_denorm[r], &a.pitch[r]);
+}
+// f0_gen 'conv' (stylesinger.py:223-236): the two PitchPredictor outputs are averaged as they are - no minmax_denorm, no
+// forced-unvoiced rests; uv thresholds the averaged logit.
+__global__ void k_pitch_glue_conv(const int4* utt, PitchGlueConvArgs a) {
+  ROW_SETUP();
+  if (threadIdx.x != 0) return;
+  const float pf = a.ps[r * 2] / 2.0f + a.pa[r * 2] / 2.0f;  // pitch_domain_specific/2 + pitch_domain_agnostic/2  (:230)
+  const float pu = a.ps[r * 2 + 1] / 2.0f + a.pa[r * 2 + 1] / 2.0f;
+  if (a.pitch_pred) { a.pitch_pred[r * 2] = pf; a.pitch_pred[r * 2 + 1] = pu; }
+  const float f0 = a.f0_in ? a.f0_in[r] : pf;
+  const bool uv = a.f0_in ? (a.uv_in ? a.uv_in[r] > 0.f : false) : (pu > 0.f);
+  f0_denorm_coarse(f0, uv, a.mel2ph[r], &a.f0_denorm[r], &a.pitch[r]);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -851,6 +868,10 @@ int midi_clip_band(Ctx& ctx, const SeqDev& s, const int32_t* midi, float* lo, fl
 }
 int pitch_glue(Ctx& ctx, const SeqDev& s, const PitchGlueArgs& a) {
   LAUNCH_ROWS(k_pitch_glue, s, a);
+  return 0;
+}
+int pitch_glue_conv(Ctx& ctx, const SeqDev& s, const PitchGlueConvArgs& a) {
+  LAUNCH_ROWS(k_pitch_glue_conv, s, a);
   return 0;
 }
 

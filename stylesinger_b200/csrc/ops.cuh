@@ -136,6 +136,18 @@ struct PitchGlueArgs {
   int32_t* pitch = nullptr;       // guarded [rows] coarse bin
 };
 int pitch_glue(Ctx&, const SeqDev&, const PitchGlueArgs&);
+// f0_gen 'conv': pred[r] = ps/2 + pa/2 of the two PitchPredictor outputs (log2 Hz, uv logit) ; f0_denorm ; coarse bin
+struct PitchGlueConvArgs {
+  const float* pa = nullptr;      // guarded [rows, 2]: pitch_predictor output (domain agnostic)
+  const float* ps = nullptr;      // guarded [rows, 2]: pitch_inpainter_predictor output (domain specific)
+  const int32_t* mel2ph = nullptr;
+  const float* f0_in = nullptr;   // optional teacher-forced f0 (log2 Hz) guarded [rows]
+  const float* uv_in = nullptr;   // optional teacher-forced uv
+  float* pitch_pred = nullptr;    // guarded [rows, 2]
+  float* f0_denorm = nullptr;     // guarded [rows]
+  int32_t* pitch = nullptr;       // guarded [rows] coarse bin
+};
+int pitch_glue_conv(Ctx&, const SeqDev&, const PitchGlueConvArgs&);
 
 // ---- vocoder helpers (a20, a21) ---------------------------------------------------------------------------
 // harmonic source: f0 frames [rows1] -> har [rows256] (guarded at rate 256)

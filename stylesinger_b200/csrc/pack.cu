@@ -390,10 +390,34 @@ static int build_denoiser(TensorMap& tm, DevicePool& pool, const std::string& p,
   return 0;
 }
 
-int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder) {
+// PitchPredictor(idim = n_chans = H, n_layers 5, odim 2, kernel_size = predictor_kernel) (stylesinger.py:73-82,
+// tts_modules.py:191-219): the convs in both the fp32 and the tensor-core layout, like the decoder's FFN convs
+static int build_pitch_predictor(TensorMap& tm, DevicePool& pool, const std::string& p, int H, PitchPredictor* pp) {
+  for (int i = 0; i < PitchPredictor::kLayers; ++i) {
+    const std::string q = p + "conv." + std::to_string(i) + ".";
+    const HostTensor* w = tm.get(q + "1.weight");
+    if (!w) return -1;
+    const int k = w->shape.size() == 3 ? (int)w->shape[2] : 0;
+    SSB_CHECK(w->shape.size() == 3 && w->shape[0] == H && w->shape[1] == H,
+              "ssb_model_create: " + q + "1.weight must be [" + std::to_string(H) + ", " + std::to_string(H) + ", k]");
+    SSB_CHECK(k % 2 == 1 && (k - 1) / 2 <= GUARD,
+              "ssb_model_create: " + q + "1.weight: kernel size " + std::to_string(k) + " must be odd with (k - 1) / 2 <= " +
+                  std::to_string(GUARD));
+    if (pack_conv(pool, w, tm.get(q + "1.bias", {H}), 1, PACK_PLAIN, &pp->conv[i])) return -1;
+    if (pack_conv_tc(pool, w, 1, PACK_PLAIN, pp->conv[i].bias, &pp->conv_tc[i])) return -1;
+    pp->ln_g[i] = upload_tensor(pool, tm.get(q + "3.weight", {H}));
+    pp->ln_b[i] = upload_tensor(pool, tm.get(q + "3.bias", {H}));
+  }
+  if (pack_linear(pool, tm.get(p + "linear.weight", {2, H}), tm.get(p + "linear.bias", {2}), &pp->linear)) return -1;
+  pp->pos_alpha = upload_tensor(pool, tm.get(p + "pos_embed_alpha", {1}));
+  return 0;
+}
+
+int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder, int f0_gen) {
   DevicePool& pool = m->pool;
   m->hp = hp;
   m->mel_decoder = mel_decoder;
+  m->f0_gen = f0_gen;
   const bool prodiff = mel_decoder == SSB_MEL_DECODER_PRODIFF;
   const int H = hp.hidden_size;
   SSB_CHECK(H == 256, "hidden_size must be 256");
@@ -495,8 +519,15 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder)
     a.n2_g = upload_tensor(pool, tm.get(q + "norm2.weight"));
     a.n2_b = upload_tensor(pool, tm.get(q + "norm2.bias"));
   }
-  PK(build_denoiser(tm, pool, "gm_diffnet.", hp.f0_channels, hp.f0_layers, hp.f0_cycle, 1, 3, true, &m->f0net[0]));
-  PK(build_denoiser(tm, pool, "gm_diffnet_inpainte.", hp.f0_channels, hp.f0_layers, hp.f0_cycle, 1, 3, true, &m->f0net[1]));
+  if (f0_gen == SSB_F0_GEN_CONV) {
+    // f0_gen 'conv' (stylesinger.py:73-82): FastSpeech2 built pitch_predictor (unused with gmdiff, not packed then) and
+    // StyleSinger rebuilds it with the same shapes; pitch_inpainter_predictor is the second one.  No F0 DiffNets.
+    PK(build_pitch_predictor(tm, pool, "pitch_predictor.", H, &m->pp[0]));
+    PK(build_pitch_predictor(tm, pool, "pitch_inpainter_predictor.", H, &m->pp[1]));
+  } else {
+    PK(build_denoiser(tm, pool, "gm_diffnet.", hp.f0_channels, hp.f0_layers, hp.f0_cycle, 1, 3, true, &m->f0net[0]));
+    PK(build_denoiser(tm, pool, "gm_diffnet_inpainte.", hp.f0_channels, hp.f0_layers, hp.f0_cycle, 1, 3, true, &m->f0net[1]));
+  }
   if (prodiff) {
     // StyleSinger.__init__ with decoder 'prodiff' (stylesinger.py:111-117): the mel DiffNet is diff_decoder.denoise_fn; there
     // is no postdiff / ln_proj, and mel_out (built by FastSpeech2.__init__) is not used at inference (:176-177)
@@ -683,6 +714,8 @@ int set_schedule(Model* m, int which, int T, const float* step_emb, const float*
     m->pool.release(old_d);
     m->pool.release(old_g);
   } else {
+    SSB_CHECK(m->f0_gen == SSB_F0_GEN_GMDIFF,
+              "set_schedule: a model with the conv F0 generator (SSB_F0_GEN_CONV) has no F0 diffusion schedule (which = 1)");
     SSB_CHECK(mtab != nullptr, "set_schedule: multinomial table required for the F0 nets");
     std::vector<float> mt(mtab, mtab + (size_t)T * 8);
     for (int i = 0; i < 2; ++i) {

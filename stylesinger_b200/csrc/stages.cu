@@ -245,6 +245,57 @@ int run_duration_predictor(Ctx& c, const Model& m, const SeqDev& sp, const float
   return 0;
 }
 
+// f0_gen 'conv': PitchPredictor.forward (tts_modules.py:221-234), eval mode.  x [rows,256] -> out [rows,2].  No mask
+// anywhere, as in the reference: every buffer's guard rows stay zero, which is the SAME padding of a B=1 call.
+int run_pitch_predictor(Ctx& c, const Model& m, int which, const SeqDev& s, const float* x_g, float* out_g, bool tc) {
+  const int H = 256;
+  SSB_CHECK(m.f0_gen == SSB_F0_GEN_CONV, "pitch predictor: the model was not created with SSB_F0_GEN_CONV");
+  SSB_CHECK(which == 0 || which == 1, "pitch predictor: which must be 0 (pitch_predictor) or 1 (pitch_inpainter_predictor)");
+  const PitchPredictor& p = m.pp[which];
+  for (int i = 0; i < PitchPredictor::kLayers; ++i) tc = tc && p.conv_tc[i].ok;
+  const size_t mk = c.mark();
+  float* xs = alloc_rows(c, s, H);
+  float* a = alloc_rows(c, s, H);
+  float* b = alloc_rows(c, s, H);
+  float* c0 = alloc_rows(c, s, 1);
+  int32_t* pos = alloc_rows_i32(c, s);
+  __half *hh = nullptr, *hl = nullptr;
+  if (tc) {
+    hh = alloc_half_rows(c, s, H);
+    hl = alloc_half_rows(c, s, H);
+  }
+  WS_OK(c);
+  // positions = pos_embed_alpha * embed_positions(xs[..., 0]); xs = xs + positions
+  if (!c.dry) SSB_CUDA(cudaMemcpyAsync(xs, x_g, (size_t)s.rows * H * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
+  RUN(col0_nonzero_mask(c, s, xs, H, c0));
+  RUN(positions_from_mask(c, s, c0, pos));
+  RUN(add_positional(c, s, xs, H, H, pos, m.pos_table, m.pos_rows, p.pos_alpha));
+  const float* cur = xs;
+  for (int i = 0; i < PitchPredictor::kLayers; ++i) {
+    // ConstantPad1d + Conv1d + ReLU (the guard rows are the zero pad), then LayerNorm(dim=1); Dropout is off
+    if (tc) {
+      RUN(split_planes(c, cur, H, s.rows, H, 1.0f, hh, hl));
+      GemmTC g;
+      g.A_hi = hh; g.A_lo = hl; g.rows_total = s.rows; g.w = &p.conv_tc[i]; g.tiles = s.tiles; g.ntiles = s.ntiles;
+      g.e.mode = EPI_GENERIC; g.e.act = ACT_RELU; g.e.out = a; g.e.ldo = H;
+      RUN(conv_gemm_tc(c, g));
+    } else {
+      ConvGemm g = make_gemm(p.conv[i], s, cur, H);
+      g.e.act = ACT_RELU; g.e.out = a; g.e.ldo = H;
+      RUN(conv_gemm(c, g));
+    }
+    RUN(layernorm_rows(c, s, a, H, b, H, H, p.ln_g[i], p.ln_b[i], 1e-5f, nullptr));
+    cur = b;  // the next conv reads b and writes a; the LN after it overwrites b only once that conv has finished
+  }
+  {
+    ConvGemm g = make_gemm(p.linear, s, cur, H);
+    g.e.out = out_g; g.e.ldo = 2;
+    RUN(conv_gemm(c, g));
+  }
+  c.release(mk);
+  return 0;
+}
+
 // a10-a12: get_style (stylesinger.py:189-214)
 int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const float* dec0, const float* ref_g /*[rows,80]*/,
               const float* reff0_g /*[rows]*/, float* style /*[rows_f,256]*/, int32_t* codes /*[rows_r,depth] guarded*/,

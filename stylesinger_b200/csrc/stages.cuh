@@ -9,6 +9,9 @@ int run_encoder(Ctx& c, const Model& m, const SeqDev& sp, const int32_t* tok_g, 
 int run_fft_decoder(Ctx& c, const Model& m, const SeqDev& sf, const float* dec_in, float* xd, bool tc);
 int run_duration_predictor(Ctx& c, const Model& m, const SeqDev& sp, const float* dur_inp, const float* srcmask,
                            float* logdur, int32_t* dur);
+// f0_gen 'conv': one PitchPredictor (which 0: pitch_predictor, 1: pitch_inpainter_predictor), x [rows,256] -> out
+// [rows,2]; tc: the five convs on the tensor-core kernel
+int run_pitch_predictor(Ctx& c, const Model& m, int which, const SeqDev& s, const float* x_g, float* out_g, bool tc);
 int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const float* dec0, const float* ref_g,
               const float* reff0_g, float* style, int32_t* codes, float* rq_in_out);
 struct DenoiserBufs {

@@ -17,6 +17,7 @@ from .hparams import DEFAULT_VOCODER_CONFIG, resolve
 from .schedules import multinomial_table, prodiff_table, sampler_table
 
 MEL_DECODERS = {"diffsinger": 0, "prodiff": 1}  # SSB_MEL_DECODER_* of include/stylesinger_b200.h
+F0_GENS = {"gmdiff": 0, "conv": 1}  # SSB_F0_GEN_*
 
 
 def _require_cuda():
@@ -137,7 +138,9 @@ class _Workspace:
 
 class AcousticModel:
     """Packed StyleSinger acoustic model on one GPU (ssb_model_t).  hparams['decoder'] selects the mel decoder:
-    'diffsinger' (FFT decoder + DDPM refinement, the default) or 'prodiff' (the ProDiff teacher, decoder_inp -> mel)."""
+    'diffsinger' (FFT decoder + DDPM refinement, the default) or 'prodiff' (the ProDiff teacher, decoder_inp -> mel).
+    hparams['f0_gen'] selects the F0 generator: 'gmdiff' (two F0 diffusion samplers, the default) or 'conv' (two
+    deterministic FastSpeech-2 PitchPredictors; no F0 schedule, no F0 noise)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], hparams=None, device=None, max_positions=4096):
         _require_cuda()
@@ -157,14 +160,15 @@ class AcousticModel:
                     hp["f0_residual_channels"], hp["f0_residual_layers"], hp["f0_dilation_cycle_length"],
                     hp["audio_num_mel_bins"])
         self.mel_decoder = hp["decoder"]
+        self.f0_gen = hp["f0_gen"]
         arr, keep = _descs(sd)
         handle = C.c_void_p()
-        check(lib.ssb_model_create_ex(C.byref(handle), arr, len(sd), C.byref(h), MEL_DECODERS[self.mel_decoder]),
-              "ssb_model_create_ex")
+        check(lib.ssb_model_create_ex2(C.byref(handle), arr, len(sd), C.byref(h), MEL_DECODERS[self.mel_decoder],
+                                       F0_GENS[self.f0_gen]), "ssb_model_create_ex2")
         self._h = handle
         self._ws = _Workspace(self.device)
         self.T = self.f0_T = None
-        self.set_timesteps(hp["timesteps"], hp["f0_timesteps"])
+        self.set_timesteps(hp["timesteps"], hp["f0_timesteps"] if self.f0_gen == "gmdiff" else None)
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -200,7 +204,7 @@ class AcousticModel:
             check(lib.ssb_model_set_schedule(self._h, 0, T, C.c_void_p(emb.data_ptr()), g.ctypes.data_as(C.c_void_p),
                                              None, stream), "ssb_model_set_schedule(mel)")
             self.T = T
-        if f0_T is not None and f0_T != self.f0_T:
+        if f0_T is not None and f0_T != self.f0_T:  # (the library refuses it on an f0_gen 'conv' model)
             emb = step_embedding(f0_T, self.hp["f0_residual_channels"])
             g = np.ascontiguousarray(sampler_table(f0_T, self.hp["f0_max_beta"]))
             m = np.ascontiguousarray(multinomial_table(f0_T, self.hp["f0_max_beta"]))
@@ -359,6 +363,21 @@ class AcousticModel:
                                           _ptr(gauss_noise), _ptr(unif_noise), int(seed), _ptr(z), _ptr(uv), _ptr(ws),
                                           ws.numel(), self._stream()), "ssb_f0_diffusion_sample")
         return z, uv
+
+    def pitch_predictor(self, which, x, frame_offsets):
+        """PitchPredictor.forward on an f0_gen 'conv' model: which 0 = pitch_predictor (domain agnostic input), 1 =
+        pitch_inpainter_predictor (domain specific input); x [sumF,256] (device, tight) -> [sumF,2] (log2-Hz f0, uv
+        logit)."""
+        fo = np.ascontiguousarray(frame_offsets, np.int32)
+        B = len(fo) - 1
+        n = lib.ssb_pitch_predictor_workspace_bytes(self._h, fo.ctypes.data, B)
+        if n == 0:
+            check(-1, "ssb_pitch_predictor_workspace_bytes")
+        ws = self._ws.get(n)
+        out = torch.empty((int(fo[-1]), 2), dtype=torch.float32, device=self.device)
+        check(lib.ssb_pitch_predictor(self._h, int(which), _ptr(x), fo.ctypes.data, B, _ptr(out), _ptr(ws), ws.numel(),
+                                      self._stream()), "ssb_pitch_predictor")
+        return out
 
     def fft_encoder(self, txt_tokens, ph_offsets):
         """FastspeechEncoder.forward: int32 tokens [sumP] (device) -> [sumP,256]."""

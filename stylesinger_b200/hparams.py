@@ -34,7 +34,7 @@ _SPEC_MAX = [0.03640973940491676, 0.039425432682037354, 0.29524752497673035, 0.4
 DEFAULT_HPARAMS = {
     "hidden_size": 256, "enc_layers": 4, "dec_layers": 4, "num_heads": 2,
     "enc_ffn_kernel_size": 9, "dec_ffn_kernel_size": 9, "ffn_act": "gelu", "ffn_padding": "SAME",
-    "dur_predictor_layers": 2, "dur_predictor_kernel": 3, "predictor_hidden": -1,
+    "dur_predictor_layers": 2, "dur_predictor_kernel": 3, "predictor_hidden": -1, "predictor_kernel": 5,
     "use_pos_embed": True, "encoder_type": "fft", "decoder_type": "fft", "dur_loss": "mse",
     "use_pitch_embed": True, "use_energy_embed": False, "pitch_type": "frame",
     "mel_vmin": -6, "mel_vmax": 1.5, "timesteps": 100, "K_step": 100, "f0_timesteps": 100,
@@ -91,8 +91,11 @@ def _check_supported(hp):
     """The CUDA path implements exactly the configuration egs/stylesinger.yaml selects.
     Anything else fails loudly instead of silently computing something different."""
     prodiff = hp.get("decoder") == "prodiff"  # the ProDiff teacher of the commented block egs/stylesinger.yaml:145-155
+    # f0_gen 'conv': two FastSpeech-2 PitchPredictors instead of the two F0 diffusion samplers (stylesinger.py:66-82);
+    # f0_timesteps / f0_max_beta are then unread
+    conv_f0 = hp.get("f0_gen") == "conv"
     req = {"encoder_type": "fft", "decoder_type": "fft", "ffn_act": "gelu", "ffn_padding": "SAME",
-           "dur_loss": "mse", "pitch_type": "frame", "f0_gen": "gmdiff",
+           "dur_loss": "mse", "pitch_type": "frame", "f0_gen": "conv" if conv_f0 else "gmdiff",
            "decoder": "prodiff" if prodiff else "diffsinger",
            "diff_decoder_type": "wavenet", "schedule_type": "vpsde" if prodiff else "linear", "pitch_norm": "log",
            "use_uv": True, "emo": True, "style": True, "umln": True, "use_spk_embed": True,

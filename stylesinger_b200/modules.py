@@ -6,7 +6,8 @@ tasks/StyleSinger/stylesinger.py:122-123,190-195).  ``HifiGAN`` mirrors the regi
 (tasks/tts/vocoder_infer/hifigan_nsf.py:46-75: ``spec2wav(mel np[T,80], f0=np[T]) -> np[T*hop]``).
 
 Both mel decoders of ``hparams['decoder']`` are implemented: 'diffsinger' (the default) and 'prodiff', the ProDiff
-teacher (stylesinger.py:111-117,176-177), whose sampler always runs, whatever ``global_steps`` is.
+teacher (stylesinger.py:111-117,176-177), whose sampler always runs, whatever ``global_steps`` is.  Both F0 generators
+of ``hparams['f0_gen']`` are implemented: 'gmdiff' (the default) and 'conv' (stylesinger.py:73-82; ``PitchPredictor``).
 Only what the ph -> mel -> wav inference path uses is implemented; everything else raises instead of silently
 doing something different (training mode, teacher-forced f0/uv, the `forcing` aligner branch of early training
 steps, the fft decoder).
@@ -245,6 +246,23 @@ class DDiffNet(_Registered):
         out = self.engine.denoiser_eval(self.which, x, u, t, c, offs)  # [B*F, 3]
         out = out.reshape(B, Fr, 3).transpose(1, 2).contiguous()
         return out if nonpadding is None else out * nonpadding[:, None, :].to(out.device)
+
+
+class PitchPredictor(_Registered):
+    """Drop-in for the two FastSpeech-2 PitchPredictors of an f0_gen 'conv' model (stylesinger.py:73-82,223-225;
+    tts_modules.py:191-234): ``forward(xs [B,T,256]) -> [B,T,2]`` (log2-Hz f0, uv logit).  which: 0 = pitch_predictor
+    (domain agnostic), 1 = pitch_inpainter_predictor (domain specific).  The reference applies no mask inside the
+    predictor, so every batch element runs over the full padded length T, exactly as the reference computes it."""
+
+    def __init__(self, engine: AcousticModel, which: int):
+        super().__init__(engine)
+        self.which = which
+
+    def forward(self, xs):
+        B, T, H = xs.shape
+        offs = (np.arange(B + 1) * T).astype(np.int32)
+        x = xs.reshape(B * T, H).to(self.engine.device, torch.float32).contiguous()
+        return self.engine.pitch_predictor(self.which, x, offs).reshape(B, T, 2)
 
 
 class HifiGAN:

@@ -88,7 +88,8 @@ def acoustic_param_shapes(hp):
             ("spk_embed_proj.weight", (H, 256)), ("spk_embed_proj.bias", (H,))]
     out += _predictor("dur_predictor.", H, hp["dur_predictor_layers"], hp["dur_predictor_kernel"], 1)
     out += [("pitch_embed.weight", (300, H)), ("pitch_predictor.pos_embed_alpha", (1,))]
-    out += _predictor("pitch_predictor.", H, 5, 5, 2)  # constructed by FastSpeech2, unused with gmdiff
+    # constructed by FastSpeech2 (unused with gmdiff); f0_gen 'conv' rebuilds it in place with the same shapes
+    out += _predictor("pitch_predictor.", H, 5, hp["predictor_kernel"], 2)
     out += [("pitch_predictor.embed_positions._float_tensor", (1,)),
             ("note_encoder.emb.weight", (100, H)), ("note_encoder.type_emb.weight", (5, H)),
             ("note_encoder.dur_ln.weight", (H, 1)), ("note_encoder.dur_ln.bias", (H,)),
@@ -128,7 +129,12 @@ def acoustic_param_shapes(hp):
                 (q + "linear2.weight", (H, 2048)), (q + "linear2.bias", (H,)),
                 (q + "norm2.weight", (H,)), (q + "norm2.bias", (H,))]
     Cf, Lf, Tf = hp["f0_residual_channels"], hp["f0_residual_layers"], hp["f0_timesteps"]
-    for net, gen in (("gm_diffnet", "f0_gen"), ("gm_diffnet_inpainte", "f0_gen_inpainte")):
+    if hp["f0_gen"] == "conv":  # StyleSinger.__init__ (stylesinger.py:73-82): a second PitchPredictor, no F0 diffusion
+        out += [("pitch_inpainter_predictor.pos_embed_alpha", (1,))]
+        out += _predictor("pitch_inpainter_predictor.", H, 5, hp["predictor_kernel"], 2)
+        out += [("pitch_inpainter_predictor.embed_positions._float_tensor", (1,))]
+    f0_nets = () if hp["f0_gen"] == "conv" else (("gm_diffnet", "f0_gen"), ("gm_diffnet_inpainte", "f0_gen_inpainte"))
+    for net, gen in f0_nets:
         out += _diffnet(net + ".", Cf, Lf, 1, 3, H, True)
         out += [(f"{gen}.{b}", (Tf,)) for b in _MULTI_BUFS]
         out += [(f"{gen}.Lt_history", (Tf,)), (f"{gen}.Lt_count", (Tf,))]
@@ -275,6 +281,14 @@ def acoustic_state_dict(hp=None, seed=0):
         for k in list(sd.keys()):
             if k.startswith(gen + "._denoise_fn."):
                 sd[k] = sd[net + "." + k[len(gen + "._denoise_fn."):]]
+    if hp["f0_gen"] == "conv":
+        # The generic init puts the predicted f0 (log2 Hz) around 0-3, i.e. below 8 Hz, where every frame falls into
+        # coarse bin 1.  Centre the f0 row on 8 (256 Hz) with a spread of about +-0.7 octave so that f0_to_coarse and
+        # pitch_embed see a realistic range; the uv row (about half the frames > 0) is left as generated.  No random
+        # numbers are drawn here.
+        for p in ("pitch_predictor.", "pitch_inpainter_predictor."):
+            sd[p + "linear.weight"][0] *= 0.35
+            sd[p + "linear.bias"][0] = 8.0
     return sd
 
 

@@ -314,6 +314,65 @@ def case_prodiff(name, T=8, f0_T=4, frames=32, phones=4, ref_frames=32, seed=81,
     print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()})
 
 
+CONVF0_OVERRIDES = {"f0_gen": "conv"}
+CONVF0_ZERO_ROWS = (0, 7, 150, 151, 299)  # rows of the predictor-only inputs whose channel 0 is exactly 0
+
+
+def case_convf0(name, T=4, frames=96, phones=12, ref_frames=64, seed=111, utt_idx=105, pred_frames=300,
+                prodiff_T=8, prodiff_frames=32, prodiff_phones=4, prodiff_seed=121, prodiff_utt_idx=106):
+    """The convolutional F0 generator (hparams['f0_gen'] == 'conv', stylesinger.py:73-82,223-225: two FastSpeech-2
+    PitchPredictors, tts_modules.py:191-234): a B=1 full forward with mel2ph given and with predicted durations
+    (DiffSinger decoder), each predictor alone on seeded inputs whose channel 0 is exactly 0 in a few rows (the
+    position skip of make_positions), a B=1 full forward with the ProDiff decoder, and both state dicts' key lists."""
+    import ref_import
+    hp = ref_import.install(T=T, overrides=CONVF0_OVERRIDES)
+    import modules.diff.shallow_diffusion_tts as sdt
+    sdt.tqdm = lambda it, **k: it
+    from modules.StyleSinger.stylesinger import StyleSinger
+    model = StyleSinger(_Dict()).eval()
+    model.load_state_dict(synth.acoustic_state_dict(dict(hp), seed=0), strict=True)
+    u = synth.make_utterance(frames / 187.5, utt_idx=utt_idx, ref_frames=ref_frames, frames=frames, phones=phones)
+    out, log = run_model(model, u, seed)
+    o2, log2 = run_model(model, u, seed + 1, mel2ph=False)
+    g = torch.Generator().manual_seed(seed + 2)
+    xs = torch.randn(2, 1, pred_frames, 256, generator=g)
+    xs[:, :, list(CONVF0_ZERO_ROWS), 0] = 0
+    with torch.no_grad():
+        pa = model.pitch_predictor(xs[0].clone())
+        ps = model.pitch_inpainter_predictor(xs[1].clone())
+    keys = [[k, list(v.shape)] for k, v in model.state_dict().items()]
+    d = {"pitch_pred": np32(out["pitch_pred"][0]), "f0_denorm": np32(out["f0_denorm"][0]),
+         "decoder_inp": np32(out["decoder_inp"][0]), "mel_out": np32(out["mel_out"][0]),
+         "dur_mel2ph": o2["mel2ph"][0].numpy().astype(np.int64), "dur_pitch_pred": np32(o2["pitch_pred"][0]),
+         "dur_f0_denorm": np32(o2["f0_denorm"][0]), "dur_decoder_inp": np32(o2["decoder_inp"][0]),
+         "dur_mel_out": np32(o2["mel_out"][0]),
+         # the predictor inputs are regenerated from pred_seed by the tests (tests/f0conv_oracle.predictor_inputs); their
+         # first rows are kept to check that
+         "pred_x_head": np32(xs[:, 0, :4]), "pred_out_agnostic": np32(pa[0]), "pred_out_specific": np32(ps[0])}
+    # (d) ProDiff decoder + conv F0 generator: the fast configuration
+    hp2 = ref_import.install(T=prodiff_T, overrides=dict(PRODIFF_OVERRIDES, **CONVF0_OVERRIDES))
+    import modules.diff.prodiff as pdm
+    pdm.tqdm = lambda it, **k: it
+    model2 = StyleSinger(_Dict()).eval()
+    model2.load_state_dict(synth.acoustic_state_dict(dict(hp2), seed=0), strict=True)
+    u2 = synth.make_utterance(prodiff_frames / 187.5, utt_idx=prodiff_utt_idx, ref_frames=prodiff_frames,
+                              frames=prodiff_frames, phones=prodiff_phones)
+    out2, log3 = run_model(model2, u2, prodiff_seed)
+    keys2 = [[k, list(v.shape)] for k, v in model2.state_dict().items()]
+    d.update({"pd_pitch_pred": np32(out2["pitch_pred"][0]), "pd_f0_denorm": np32(out2["f0_denorm"][0]),
+              "pd_decoder_inp": np32(out2["decoder_inp"][0]), "pd_mel_out": np32(out2["mel_out"][0])})
+    d["meta"] = json.dumps({"T": T, "frames": frames, "phones": phones, "ref_frames": ref_frames, "seed": seed,
+                            "utt_idx": utt_idx, "noise_log": log, "dur_noise_log": log2, "overrides": CONVF0_OVERRIDES,
+                            "pred_frames": pred_frames, "pred_seed": seed + 2, "pred_zero_rows": list(CONVF0_ZERO_ROWS),
+                            "state_dict": keys,
+                            "prodiff": {"T": prodiff_T, "frames": prodiff_frames, "phones": prodiff_phones,
+                                        "ref_frames": prodiff_frames, "seed": prodiff_seed, "utt_idx": prodiff_utt_idx,
+                                        "noise_log": log3, "overrides": dict(PRODIFF_OVERRIDES, **CONVF0_OVERRIDES),
+                                        "state_dict": keys2}})
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()})
+
+
 def case_schedules(name, Ts=(4, 25, 50, 100, 200, 500)):
     """Registered schedule buffers of the reference's DiffusionDecoder / GaussianMultinomialDiffusion at several T
     (shallow_diffusion_tts.py:86-119, gaussian_multinomial_diffusion.py:237-283): pins the oracle's and the product's
@@ -376,7 +435,8 @@ def case_emotion_encoder(name, partials=5, seed=71):
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
-    which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "sched", "voc", "vocoder_edges", "emo"]
+    which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "convf0", "sched", "voc",
+                             "vocoder_edges", "emo"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
@@ -389,6 +449,8 @@ if __name__ == "__main__":
         case_plms("ref_plms_T100_i10")
     if "prodiff" in which:
         case_prodiff("ref_prodiff_T8")
+    if "convf0" in which:
+        case_convf0("ref_convf0")
     if "sched" in which:
         case_schedules("ref_schedules")
     if "voc" in which:

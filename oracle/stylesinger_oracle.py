@@ -265,19 +265,25 @@ def conv_blocks(x, sd, p="style_extractor.encoder."):
     return x.transpose(1, 2)
 
 
-def rq_quantize(x, sd, depth=4, p="style_extractor.rqvae.codebooks."):
+def rq_quantize(x, sd, depth=4, p="style_extractor.rqvae.codebooks.", codes=None):
     """RQBottleneck.quantize/forward + VQEmbedding.compute_distances (RQ.py:226-270,29-55).
-    x [B,R,256] -> (quants_trunc [B,R,256], codes int64 [B,R,depth])."""
+    x [B,R,256] -> (quants_trunc [B,R,256], codes int64 [B,R,depth]).
+    codes: optional [B,R,depth] to use instead of the argmin (a float64 run then takes the codes an fp32 run chose: the
+    reference decides the argmin in fp32, and a near-tie that float64 resolves the other way is not an error)."""
     res = x.detach().clone()
     agg = torch.zeros_like(x)
+    given = codes
     codes = []
     for d in range(depth):
-        cb = sd[f"{p}{d}.weight"][:-1]
-        cbt = cb.t()
-        flat = res.reshape(-1, res.shape[-1])
-        dist = torch.addmm(flat.pow(2.0).sum(dim=1, keepdim=True) + cbt.pow(2.0).sum(dim=0, keepdim=True),
-                           flat, cbt, alpha=-2.0)
-        idx = dist.argmin(dim=-1).reshape(res.shape[:-1])
+        if given is not None:
+            idx = torch.as_tensor(given)[..., d].long().reshape(res.shape[:-1])
+        else:
+            cb = sd[f"{p}{d}.weight"][:-1]
+            cbt = cb.t()
+            flat = res.reshape(-1, res.shape[-1])
+            dist = torch.addmm(flat.pow(2.0).sum(dim=1, keepdim=True) + cbt.pow(2.0).sum(dim=0, keepdim=True),
+                               flat, cbt, alpha=-2.0)
+            idx = dist.argmin(dim=-1).reshape(res.shape[:-1])
         q = F.embedding(idx, sd[f"{p}{d}.weight"])
         res.sub_(q)
         agg.add_(q)
@@ -285,15 +291,15 @@ def rq_quantize(x, sd, depth=4, p="style_extractor.rqvae.codebooks."):
     return x + (agg - x), torch.cat(codes, dim=-1)
 
 
-def local_style_adaptor(ref_mels, ref_f0, sd, hp):
-    """LocalStyleAdaptor.forward (lse.py:103-129). ref_mels [B,R,80], ref_f0 [B,R] or [R]."""
+def local_style_adaptor(ref_mels, ref_f0, sd, hp, codes=None):
+    """LocalStyleAdaptor.forward (lse.py:103-129). ref_mels [B,R,80], ref_f0 [B,R] or [R]; codes: see rq_quantize."""
     pad = ref_mels[:, :, 0].eq(0)
     x = wn_forward(ref_mels.transpose(1, 2), (~pad).unsqueeze(1).repeat([1, 80, 1]).float(), sd).transpose(1, 2)
     if ref_f0 is not None:
         f = ref_f0.unsqueeze(ref_f0.dim()).repeat([1, 1, 80])
         x = x + f
     style = conv_blocks(x, sd)
-    return rq_quantize(style, sd, hp["rq_depth"])
+    return rq_quantize(style, sd, hp["rq_depth"], codes=codes)
 
 
 def cross_atten_layer(src, emo, key_pad, sd, p):
@@ -306,10 +312,10 @@ def cross_atten_layer(src, emo, key_pad, sd, p):
     return layer_norm(src + y, sd[p + "norm2.weight"], sd[p + "norm2.bias"])
 
 
-def get_style(decoder_inp, ref_mels, ref_f0, sd, hp):
+def get_style(decoder_inp, ref_mels, ref_f0, sd, hp, codes=None):
     """StyleSinger.get_style, infer / global_steps>=forcing (stylesinger.py:189-214).
-    Returns (style [B,F,H], codes)."""
-    z, codes = local_style_adaptor(ref_mels, ref_f0, sd, hp)
+    Returns (style [B,F,H], codes).  codes: see rq_quantize."""
+    z, codes = local_style_adaptor(ref_mels, ref_f0, sd, hp, codes)
     pos = sinusoid_positions(z[:, :, 0], hp["hidden_size"])
     z = F.linear(torch.cat([z, pos], dim=-1), sd["l1.weight"], sd["l1.bias"])
     key_pad = z[:, :, 0].eq(0)
@@ -593,9 +599,9 @@ def inpaint_pitch(agn, spec, mel2ph, midi, sd, hp, noise, f0=None, uv=None):
 # a17 + whole model
 # ----------------------------------------------------------------------------------------------
 def stylesinger_forward(sd, hp, txt_tokens, note, note_dur, note_type, spk_embed, emo_embed, ref_mels, ref_f0,
-                        noise, mel2ph=None, f0=None, uv=None, skip_diffusion=False):
+                        noise, mel2ph=None, f0=None, uv=None, skip_diffusion=False, codes=None):
     """StyleSinger.forward(infer=True, global_steps > diff_start) (stylesinger.py:119-187) for B=1.
-    All tensors carry a leading batch dim of 1 (ref_f0 may be [R])."""
+    All tensors carry a leading batch dim of 1 (ref_f0 may be [R]); codes: see rq_quantize."""
     ret = {}
     enc = fastspeech_encoder(txt_tokens, sd, hp) + note_encoder(note, note_dur, note_type, sd, hp["hidden_size"])
     src_np = (txt_tokens > 0).float()[:, :, None]
@@ -611,7 +617,7 @@ def stylesinger_forward(sd, hp, txt_tokens, note, note_dur, note_type, spk_embed
     tgt_np = (mel2ph > 0).float()[:, :, None]
     dec = expand_states(enc, mel2ph)  # UMLN = identity in eval (umln.py:49-50)
     ret["encoder_out"] = enc
-    style, codes = get_style(dec, ref_mels, ref_f0, sd, hp)
+    style, codes = get_style(dec, ref_mels, ref_f0, sd, hp, codes)
     ret["style"], ret["rq_codes"] = style, codes
     midi = expand_states(note[:, :, None], mel2ph).transpose(-1, -2)
     agn = dec * tgt_np

@@ -96,7 +96,7 @@ class StyleSinger:
         """modules/StyleSinger/stylesinger.py:189-214 with padded tensors (ret['ref_f0'] as there)."""
         dev = self.engine.device
         fl = _true_lengths(encoder_out)
-        rl = [max(int(v), 1) for v in (ref_mels.abs().sum(-1) > 0).sum(1).tolist()]
+        rl = _true_lengths(ref_mels)
         fo = np.concatenate([[0], np.cumsum(fl)]).astype(np.int32)
         ro = np.concatenate([[0], np.cumsum(rl)]).astype(np.int32)
         rf0 = ret["ref_f0"]
@@ -163,12 +163,18 @@ class StyleSinger:
         return ret
 
 
+def _lengths_from_mask(nz: torch.Tensor):
+    """Per batch element of a [B, L] non-padding mask, the index after its last True (at least 1).  Padding only ever
+    trails, so this is the true length; an interior padding row stays inside it, where the library masks it exactly as
+    the reference does (a count of the True entries would drop the last real row instead)."""
+    L = nz.shape[1]
+    idx = torch.arange(1, L + 1, device=nz.device)[None, :] * nz
+    return [max(int(v), 1) for v in idx.max(dim=1).values.tolist()]
+
+
 def _true_lengths(x: torch.Tensor):
     """Per batch element, the index after the last row that is not all zero (the reference's padding rows are zero)."""
-    nz = (x.abs().sum(-1) > 0)
-    L = x.shape[1]
-    idx = torch.arange(1, L + 1, device=x.device)[None, :] * nz
-    return [max(int(v), 1) for v in idx.max(dim=1).values.tolist()]
+    return _lengths_from_mask(x.abs().sum(-1) > 0)
 
 
 class _Registered(torch.nn.Module):
@@ -185,7 +191,7 @@ class FastspeechEncoder(_Registered):
 
     def forward(self, txt_tokens):
         dev = self.engine.device
-        lens = [max(int(v), 1) for v in (txt_tokens > 0).sum(1).tolist()]  # pad id 0 only ever trails (dictionary.pad())
+        lens = _lengths_from_mask(txt_tokens != 0)  # pad id 0 (dictionary.pad())
         offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
         tight = torch.cat([txt_tokens[i, :n] for i, n in enumerate(lens)]).to(dev, torch.int32).contiguous()
         out = self.engine.fft_encoder(tight, offs)

@@ -28,6 +28,49 @@ def acoustic_sd():
     return _CACHE["sd"]
 
 
+def acoustic_sd64():
+    """acoustic_sd() cast to float64: the oracle functions then run in double precision (the positional table stays fp32,
+    as the reference's is)."""
+    if "sd64" not in _CACHE:
+        _CACHE["sd64"] = {k: (v.double() if v.is_floating_point() else v) for k, v in acoustic_sd().items()}
+    return _CACHE["sd64"]
+
+
+def registry_inputs(seed=131):
+    """Inputs of the per-registry drop-in fixture ref_registry (tools/make_golden.py registry), rebuilt from the seed.
+
+    enc_tokens [3, 12]: true lengths 12, 7, 9, then trailing padding tokens (0); utterance 0 also has an interior 0 token
+    (position 3), which the encoder masks like padding.  dec_x [3, 24, 256]: true lengths 24, 13, 19, then all-zero rows;
+    utterance 0 has an interior all-zero row (11) and a row whose column 0 alone is 0 (5), utterance 2 another such row
+    (5).  The interior cases sit in the longest utterance because only an utterance without trailing padding is the same
+    in the reference's padded batch and in its own B = 1 call (a padding row after a LayerNorm holds the LN bias, and the
+    FFN conv reads it); the library computes B = 1 semantics for every utterance.  style_dec_<i> /
+    style_ref_<i> / style_f0_<i>: two B = 1 get_style inputs (decoder_inp [1, F, 256], ref_mels [1, R, 80], ref_f0 [R]);
+    reference mel 1 has an interior all-zero row (9)."""
+    g = torch.Generator().manual_seed(seed)
+    enc_lens, dec_lens = (12, 7, 9), (24, 13, 19)
+    tok = torch.zeros(3, max(enc_lens), dtype=torch.long)
+    for b, n in enumerate(enc_lens):
+        tok[b, :n] = torch.randint(3, synth.N_TOKENS, (n,), generator=g)
+    tok[0, 3] = 0
+    x = torch.zeros(3, max(dec_lens), 256)
+    for b, n in enumerate(dec_lens):
+        x[b, :n] = torch.randn(n, 256, generator=g)
+    x[0, 11] = 0
+    x[0, 5, 0] = 0
+    x[2, 5, 0] = 0
+    d = {"enc_tokens": tok, "dec_x": x}
+    for i, (F_, R, idx) in enumerate(((21, 17, 110), (30, 26, 111))):
+        u = synth.make_utterance(F_ / 187.5, utt_idx=idx, ref_frames=R, frames=F_, phones=6)
+        ref = u["ref_mels"].clone()
+        if i == 1:
+            ref[9] = 0
+        d[f"style_dec_{i}"] = torch.randn(1, F_, 256, generator=g)
+        d[f"style_ref_{i}"] = ref[None]
+        d[f"style_f0_{i}"] = u["ref_f0"]
+    return d
+
+
 def vocoder_sd():
     if "vsd" not in _CACHE:
         _CACHE["vsd"] = synth.vocoder_state_dict(DEFAULT_VOCODER_CONFIG, seed=0)

@@ -25,6 +25,7 @@ sys.path.insert(0, os.path.join(REPO, "tools"))
 from oracle.stylesinger_oracle import NoiseSource  # noqa: E402
 from stylesinger_b200 import synth  # noqa: E402
 from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG  # noqa: E402
+from tests.common import registry_inputs  # noqa: E402
 
 OUT = os.path.join(REPO, "tests", "golden")
 
@@ -373,6 +374,36 @@ def case_convf0(name, T=4, frames=96, phones=12, ref_frames=64, seed=111, utt_id
     print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()})
 
 
+def case_registry(name, T=4, seed=131):
+    """The reference's per-registry modules that the C ABI replaces one by one (FS_ENCODERS['fft'], FS_DECODERS['fft'],
+    StyleSinger.get_style): FastspeechEncoder.forward and FastspeechDecoder.forward on padded B = 3 batches and on each
+    utterance alone, and get_style at B = 1 (a padded get_style batch is not B = 1-equal in the reference: its padding rows
+    are quantised and attended to)."""
+    model, hp, sd = build_reference_model(T)
+    d_in = registry_inputs(seed)
+    with torch.no_grad():
+        enc = model.encoder(d_in["enc_tokens"])
+        dec = model.decoder(d_in["dec_x"])
+        d = {"enc_out": np32(enc), "dec_out": np32(dec)}
+        # each utterance alone (B = 1) on its rows up to the last non-padding one
+        tok, x = d_in["enc_tokens"], d_in["dec_x"]
+        for b in range(3):
+            n = int((tok[b] != 0).nonzero()[-1]) + 1
+            d[f"enc_b1_{b}"] = np32(model.encoder(tok[b:b + 1, :n])[0])
+            n = int((x[b].abs().sum(-1) > 0).nonzero()[-1]) + 1
+            d[f"dec_b1_{b}"] = np32(model.decoder(x[b:b + 1, :n])[0])
+        for i in range(2):
+            ret = {"ref_f0": d_in[f"style_f0_{i}"].clone()}
+            d[f"style_{i}"] = np32(model.get_style(d_in[f"style_dec_{i}"], d_in[f"style_ref_{i}"].clone(), ret, infer=True,
+                                                   global_steps=320000)[0])
+    # the tests regenerate the inputs from the seed; their first values are kept to check that
+    d["in_enc_tokens"] = d_in["enc_tokens"].numpy().astype(np.int64)
+    d["in_dec_x_head"] = np32(d_in["dec_x"][:, :2, :4])
+    d["meta"] = json.dumps({"T": T, "seed": seed})
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()})
+
+
 def case_schedules(name, Ts=(4, 25, 50, 100, 200, 500)):
     """Registered schedule buffers of the reference's DiffusionDecoder / GaussianMultinomialDiffusion at several T
     (shallow_diffusion_tts.py:86-119, gaussian_multinomial_diffusion.py:237-283): pins the oracle's and the product's
@@ -436,7 +467,7 @@ if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "convf0", "sched", "voc",
-                             "vocoder_edges", "emo"]
+                             "vocoder_edges", "emo", "registry"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
@@ -459,3 +490,5 @@ if __name__ == "__main__":
         case_vocoder_edges("ref_vocoder_edges")
     if "emo" in which:
         case_emotion_encoder("ref_emotion_encoder")
+    if "registry" in which:
+        case_registry("ref_registry")

@@ -36,6 +36,7 @@ typedef struct ssb_model ssb_model_t;     /* packed StyleSinger acoustic model (
 typedef struct ssb_vocoder ssb_vocoder_t; /* packed HiFi-GAN(-NSF) generator */
 typedef struct ssb_melspec ssb_melspec_t; /* STFT + mel filterbank of the reference-audio front-end */
 typedef struct ssb_lstm_encoder ssb_lstm_encoder_t; /* LSTM utterance encoder of the reference-audio front-end (emo_embed) */
+typedef struct ssb_wav_denoise ssb_wav_denoise_t; /* spectral-subtraction denoiser of the vocoder output (vocoder_denoise_c) */
 
 /* One named fp32 HOST tensor of a reference state_dict (names exactly as in the reference's
  * checkpoints: utils/commons/ckpt_utils.py:26-67 loads state_dict['model']). */
@@ -319,6 +320,28 @@ int32_t ssb_melspec_num_frames(const ssb_melspec_t* m, int64_t n_samples);
 size_t ssb_melspec_workspace_bytes(const ssb_melspec_t* m, const int32_t* sample_offsets, int32_t B);
 int ssb_melspec_forward(const ssb_melspec_t* m, const float* wav, const int32_t* sample_offsets, int32_t B, float* mel_out,
                         void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- vocoder output denoiser --------------------------------------------------------------------------------------------
+ * Replaces denoise(wav, v) of tasks/tts/vocoder_infer/hifigan_nsf.py:14-22, which HifiGAN.spec2wav (:73-74) applies to the
+ * generator's waveform when hparams['vocoder_denoise_c'] > 0 (same code: vocoders/vocoder_utils.py:7-15): librosa.stft
+ * (center=True, pad_mode="constant", periodic Hann window) -> S * max(0, 1 - v / |S|) (= max(|S| - v, 0) e^{i angle S}, 0
+ * where |S| = 0) -> librosa.istft (center=True: irfft, window, overlap-add, division by the window sum-square where it exceeds
+ * tiny(float32), n_fft / 2 trimmed from each end).  Every utterance is denoised on its own (the reference's B = 1).
+ * create: fft_size even, hop_size a multiple of 16, win_length <= fft_size, fft_size <= 32 hop_size (egs/stylesinger.yaml:
+ * 1024 / 256 / 1024).  Refused before any CUDA call: bad geometry (create leaves *out NULL), an utterance length that is not
+ * a positive multiple of hop_size (the only lengths the vocoder produces; workspace_bytes then returns 0), v < 0 or not
+ * finite.  v = 0 is the STFT round trip.  wav_in / wav_out: device fp32 [sum n_b], utterances concatenated, sample_offsets:
+ * host [B+1]; the output has the input's length and wav_out may alias wav_in.  Batches of >= 8 row tiles of 128 frames run
+ * both DFT GEMMs on the tensor-core kernel (fp16 hi/lo split, 3 MMAs), smaller ones on the fp32 FFMA kernel. */
+int ssb_wav_denoise_create(ssb_wav_denoise_t** out, int32_t fft_size, int32_t hop_size, int32_t win_length); /* hifigan_nsf.py:14-22 */
+void ssb_wav_denoise_free(ssb_wav_denoise_t* d); /* hifigan_nsf.py:14-22 */
+size_t ssb_wav_denoise_workspace_bytes(const ssb_wav_denoise_t* d, const int32_t* sample_offsets, int32_t B); /* hifigan_nsf.py:14-22 */
+int ssb_wav_denoise_forward(const ssb_wav_denoise_t* d, const float* wav_in, const int32_t* sample_offsets, int32_t B, float v,
+                            float* wav_out, void* workspace, size_t workspace_bytes, void* stream); /* hifigan_nsf.py:14-22 */
+/* Test / measurement switch of the GEMM path (hifigan_nsf.py:14-22): 1 = tensor cores on batches of >= 8 row tiles, FFMA
+ * below (the default when the tensor-core path is available), 0 = fp32 FFMA always, 2 = tensor cores at every size.
+ * Returns the mode in effect (0 when the tensor-core path is unavailable). */
+int ssb_wav_denoise_set_tensor_cores(ssb_wav_denoise_t* d, int32_t enable);
 
 /* ---- f3: LSTM utterance encoder of the reference audio (SURVEY.md section 8f) -------------------------------------------
  * Replaces data_gen/tts/emotion/model.py:10-77 (EmotionEncoder: batch-first torch.nn.LSTM 40 -> 256 x 3 layers from zero

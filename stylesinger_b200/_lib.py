@@ -65,6 +65,8 @@ EXPORTS = [
     "ssb_model_create_ex", "ssb_mel_prodiff_workspace_bytes", "ssb_mel_prodiff_sample",
     "ssb_op_attention_masked",
     "ssb_model_create_ex2", "ssb_pitch_predictor_workspace_bytes", "ssb_pitch_predictor",
+    "ssb_wav_denoise_create", "ssb_wav_denoise_free", "ssb_wav_denoise_workspace_bytes", "ssb_wav_denoise_forward",
+    "ssb_wav_denoise_set_tensor_cores",
 ]
 
 
@@ -133,6 +135,11 @@ def _load():
         "ssb_lstm_encoder_free": (None, [vp]),
         "ssb_lstm_encoder_workspace_bytes": (sz, [vp, i32, i32, i32]),
         "ssb_lstm_encoder_forward": (C.c_int, [vp, vp, i32, i32, vp, i32, vp, vp, vp, vp, sz, vp]),
+        "ssb_wav_denoise_create": (C.c_int, [P(vp), i32, i32, i32]),
+        "ssb_wav_denoise_free": (None, [vp]),
+        "ssb_wav_denoise_workspace_bytes": (sz, [vp, vp, i32]),
+        "ssb_wav_denoise_forward": (C.c_int, [vp, vp, vp, i32, C.c_float, vp, vp, sz, vp]),
+        "ssb_wav_denoise_set_tensor_cores": (C.c_int, [vp, i32]),
     }
     for name in EXPORTS:
         fn = getattr(lib, name)  # AttributeError if the .so does not export a declared symbol

@@ -11,7 +11,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libstylesinger_b200.so")
-SOURCES = ["conv_gemm.cu", "conv_gemm_tc.cu", "sampler_tc.cu", "ops.cu", "attention.cu", "attention_tc.cu", "pack.cu", "stages.cu", "frontend.cu", "lstm.cu", "api.cu"]
+SOURCES = ["conv_gemm.cu", "conv_gemm_tc.cu", "sampler_tc.cu", "ops.cu", "attention.cu", "attention_tc.cu", "pack.cu", "stages.cu", "frontend.cu", "wav_denoise.cu", "lstm.cu", "api.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 

@@ -41,8 +41,6 @@ ConvGemm make_gemm(const Conv& c, const SeqDev& s, const float* A, int lda);  //
   } while (0)
 #define WS_OK(c) SSB_CHECK((c).dry || !(c).failed, "workspace too small")
 
-namespace {
-
 // tight waveform [sum n_b] -> rows of `hop` samples in the guard-banded layout (zero fill behind the last sample)
 __global__ void k_wav_rows(const int4* utt, const int32_t* sample_offs, const float* wav, int hop, float* rows) {
   const int b = blockIdx.y;
@@ -52,6 +50,63 @@ __global__ void k_wav_rows(const int4* utt, const int32_t* sample_offs, const fl
   if (i >= (int64_t)u.y * hop) return;
   rows[(int64_t)u.x * hop + i] = i < n ? wav[(int64_t)sample_offs[b] + i] : 0.f;
 }
+
+int wav_rows(Ctx& c, const SeqDev& s, const int32_t* sample_offs_dev, const float* wav, int hop, float* rows) {
+  if (c.dry || s.B == 0) return 0;
+  const int64_t per = (int64_t)s.maxlen * hop;
+  k_wav_rows<<<dim3((unsigned)((per + 255) / 256), (unsigned)s.B), 256, 0, c.stream>>>(s.utt, sample_offs_dev, wav, hop, rows);
+  SSB_CUDA(cudaGetLastError());
+  ++g_launches;
+  return 0;
+}
+
+int frames_of(int64_t n, int hop) { return (int)(1 + n / hop); }  // librosa.stft, center=True
+
+int build_seq(const int32_t* sample_offsets, int B, int hop, Seq* q) {
+  std::vector<int32_t> fo((size_t)B + 1, 0);
+  for (int b = 0; b < B; ++b) {
+    const int64_t n = (int64_t)sample_offsets[b + 1] - sample_offsets[b];
+    SSB_CHECK(n >= 0, "sample offsets must be non-decreasing");
+    fo[(size_t)b + 1] = fo[(size_t)b] + frames_of(n, hop);
+  }
+  q->build(fo.data(), B);
+  return 0;
+}
+
+int stft_span(int n_fft, int hop) { return (n_fft + 2 * hop - 1) / (2 * hop) * (2 * hop); }
+
+std::vector<double> hann_window(int n_fft, int win) {
+  // scipy.signal.get_window("hann", win_length, fftbins=True), zero-padded on both sides to n_fft (librosa.util.pad_center)
+  const double PI = 3.14159265358979323846;
+  std::vector<double> w((size_t)n_fft, 0.0);
+  const int lpad = (n_fft - win) / 2;
+  for (int i = 0; i < win; ++i) w[(size_t)lpad + i] = 0.5 - 0.5 * cos(2.0 * PI * i / win);
+  return w;
+}
+
+std::vector<float> dft_basis(int n_fft, int hop, int win, int nbp, bool inverse) {
+  const double PI = 3.14159265358979323846;
+  const std::vector<double> w = hann_window(n_fft, win);
+  const int span = stft_span(n_fft, hop), lead = (span - n_fft) / 2, nbins = n_fft / 2 + 1, N2 = 2 * nbp;
+  std::vector<float> W((size_t)span * N2, 0.f);  // [tap][c][n]: row sample tap * hop + c = frame sample j + lead
+  for (int j = 0; j < n_fft; ++j)
+    for (int k = 0; k < nbins; ++k) {
+      const double ph = 2.0 * PI * (double)(((int64_t)j * k) % n_fft) / n_fft;
+      if (!inverse) {
+        W[(size_t)(j + lead) * N2 + k] = (float)(w[(size_t)j] * cos(ph));
+        W[(size_t)(j + lead) * N2 + nbp + k] = (float)(-w[(size_t)j] * sin(ph));
+      } else {
+        const bool edge = k == 0 || 2 * k == n_fft;  // numpy's irfft ignores the imaginary parts of the DC and Nyquist bins
+        const double ck = edge ? 1.0 : 2.0;
+        W[(size_t)(j + lead) * N2 + k] = (float)(ck * w[(size_t)j] * cos(ph));
+        W[(size_t)(j + lead) * N2 + nbp + k] = edge ? 0.f : (float)(-ck * w[(size_t)j] * sin(ph));
+      }
+    }
+  return W;
+}
+
+namespace {
+
 // np.pad(y, n_fft / 2, mode="reflect") of librosa.stft's default centring: sample -i is y[i], sample n - 1 + i is y[n - 1 - i].
 // Written into the guard rows in front of the utterance and behind its last sample (pad <= 8 rows each side; the 16 guard
 // rows between neighbours keep the two utterances' pads apart).  Like numpy, needs n > pad.
@@ -100,19 +155,6 @@ double mel_to_hz(double m) {
   return m >= min_log_mel ? min_log_hz * exp(logstep * (m - min_log_mel)) : f_sp * m;
 }
 
-int frames_of(int64_t n, int hop) { return (int)(1 + n / hop); }  // librosa.stft, center=True
-
-int build_seq(const int32_t* sample_offsets, int B, int hop, Seq* q) {
-  std::vector<int32_t> fo((size_t)B + 1, 0);
-  for (int b = 0; b < B; ++b) {
-    const int64_t n = (int64_t)sample_offsets[b + 1] - sample_offsets[b];
-    SSB_CHECK(n >= 0, "sample offsets must be non-decreasing");
-    fo[(size_t)b + 1] = fo[(size_t)b] + frames_of(n, hop);
-  }
-  q->build(fo.data(), B);
-  return 0;
-}
-
 int run_melspec(Ctx& c, const ssb_melspec& m, const Seq& q, const float* wav, const int32_t* sample_offsets_host, int B, float* mel_out) {
   SeqDev s;
   RUN(upload_layout(c, q, 1, &s));
@@ -124,12 +166,7 @@ int run_melspec(Ctx& c, const ssb_melspec& m, const Seq& q, const float* wav, co
   WS_OK(c);
   if (c.dry || B == 0) return 0;
   SSB_CUDA(cudaMemcpyAsync(offs_dev, sample_offsets_host, sizeof(int32_t) * ((size_t)B + 1), cudaMemcpyHostToDevice, c.stream));
-  {
-    const int64_t per = (int64_t)s.maxlen * m.hop;
-    k_wav_rows<<<dim3((unsigned)((per + 255) / 256), (unsigned)B), 256, 0, c.stream>>>(s.utt, offs_dev, wav, m.hop, rows);
-    SSB_CUDA(cudaGetLastError());
-    ++g_launches;
-  }
+  RUN(wav_rows(c, s, offs_dev, wav, m.hop, rows));
   if (m.reflect) {
     const int pad = m.n_fft / 2;
     for (int b = 0; b < B; ++b)
@@ -184,8 +221,7 @@ int ssb_melspec_create_ex(ssb_melspec_t** out, int32_t sample_rate, int32_t fft_
   SSB_CHECK(fft_size % 2 == 0 && hop_size % 16 == 0, "the implicit-GEMM STFT needs an even n_fft and hop_size a multiple of 16");
   // frame = `taps` whole rows of hop samples centred on sample t * hop: span = n_fft rounded up to a multiple of 2 hop, the
   // DFT weights of the `lead` samples in front of / behind the n_fft window are zero
-  const int span = (fft_size + 2 * hop_size - 1) / (2 * hop_size) * (2 * hop_size);
-  const int lead = (span - fft_size) / 2;
+  const int span = stft_span(fft_size, hop_size);
   // the frame reaches taps / 2 rows into the guard band on either side; with reflect centring both neighbours WRITE their
   // pads into the guard rows they share, so the two pads together must fit
   SSB_CHECK(span / hop_size / 2 <= (pad_reflect ? GUARD / 2 : GUARD), "n_fft / hop_size too large for the guard band");
@@ -199,20 +235,8 @@ int ssb_melspec_create_ex(ssb_melspec_t** out, int32_t sample_rate, int32_t fft_
   m->reflect = pad_reflect ? 1 : 0; m->power = power ? 1 : 0; m->log10 = take_log ? 1 : 0;
   if (fmin < 0) fmin = 0.f;                       // librosa_wav2spec: fmin == -1 -> 0, fmax == -1 -> sr / 2
   if (fmax < 0) fmax = 0.5f * (float)sample_rate;
-  const double PI = 3.14159265358979323846;
-  // window: scipy.signal.get_window("hann", win_length, fftbins=True), zero-padded on both sides to n_fft (librosa.util.pad_center)
-  std::vector<double> w((size_t)fft_size, 0.0);
-  const int lpad = (fft_size - win_length) / 2;
-  for (int i = 0; i < win_length; ++i) w[(size_t)lpad + i] = 0.5 - 0.5 * cos(2.0 * PI * i / win_length);
   const int N2 = 2 * m->nbp;
-  std::vector<float> W((size_t)span * N2, 0.f);  // [tap][c][n]: row sample tap * hop + c = frame sample j + lead
-  for (int j = 0; j < fft_size; ++j)
-    for (int k = 0; k < m->nbins; ++k) {
-      const double ph = 2.0 * PI * (double)(((int64_t)j * k) % fft_size) / fft_size;
-      W[(size_t)(j + lead) * N2 + k] = (float)(w[(size_t)j] * cos(ph));
-      W[(size_t)(j + lead) * N2 + m->nbp + k] = (float)(-w[(size_t)j] * sin(ph));
-    }
-  m->dft.W = m->pool.upload(W);
+  m->dft.W = m->pool.upload(dft_basis(fft_size, hop_size, win_length, m->nbp, false));
   m->dft.bias = nullptr;
   m->dft.taps = m->taps; m->dft.Cin = hop_size; m->dft.N = N2; m->dft.Npad = N2; m->dft.dil = 1; m->dft.center = m->taps / 2;
   // mel basis (librosa.filters.mel, Slaney)

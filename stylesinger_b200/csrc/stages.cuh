@@ -45,6 +45,23 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
                 const float* rand_ini, const float* src_noise, uint64_t seed, float* wav_tight);
 int denoiser_eval_api(Ctx& c, const Model& m, int which, const SeqDev& s, const float* x_tight, const int32_t* uv_tight,
                       int t, const float* cond_tight, float* out_tight);
+// ---- implicit-GEMM STFT pieces shared by the mel front-end and the vocoder output denoiser (frontend.cu) ----------------
+// A frame of n_fft samples centred on sample t * hop is `span / hop` consecutive rows of hop samples (rows t - taps/2 ..
+// t + taps/2 - 1), span = n_fft rounded up to a multiple of 2 hop, with (span - n_fft) / 2 zero-weight samples on each side.
+int stft_span(int n_fft, int hop);
+// librosa.stft, center=True: 1 + n / hop frames; the frame layout of a batch of waveforms (sample_offsets: host [B+1])
+int frames_of(int64_t n, int hop);
+int build_seq(const int32_t* sample_offsets, int B, int hop, Seq* q);
+// tight waveform -> rows of hop samples in the frame layout `s` (zero behind the last sample); sample_offs_dev: device [B+1]
+int wav_rows(Ctx& c, const SeqDev& s, const int32_t* sample_offs_dev, const float* wav, int hop, float* rows);
+// periodic Hann window of `win` samples zero-padded (centred) to n_fft, float64 (librosa's 'hann' window)
+std::vector<double> hann_window(int n_fft, int win);
+// windowed DFT basis of one frame, [span][2 nbp] = (re | im) columns of bins 0 .. n_fft/2 (padding columns zero); row i is
+// frame sample i - lead.  inverse = false: w[j] cos, -w[j] sin (rfft of the windowed frame, librosa.stft).  inverse = true:
+// c_k w[j] cos, -c_k w[j] sin with c_k = 1 for bins 0 and n_fft/2 (whose imaginary parts numpy's irfft ignores: zero) and
+// 2 otherwise, i.e. irfft times the window of librosa.istft WITHOUT its 1/n_fft (the caller scales the GEMM's output).
+std::vector<float> dft_basis(int n_fft, int hop, int win, int nbp, bool inverse);
+
 int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ssb_acoustic_outputs& out, bool durations_only,
                  int32_t* dur_out, float* logdur_out);
 

@@ -433,10 +433,16 @@ class AcousticModel:
 
 
 class Vocoder:
-    """Packed HiFi-GAN(-NSF) generator on one GPU (ssb_vocoder_t)."""
+    """Packed HiFi-GAN(-NSF) generator on one GPU (ssb_vocoder_t).  ``denoise_c`` > 0 runs the reference's output denoiser
+    (hparams['vocoder_denoise_c'], tasks/tts/vocoder_infer/hifigan_nsf.py:73-74) on every generated waveform, with the
+    fft_size / hop_size / win_size of ``denoise_hp`` (the reference reads its global hparams; default: ``config``, then the
+    WavDenoiser defaults).  Nothing is created for the denoiser unless a call asks for it."""
 
-    def __init__(self, state_dict, config=None, device=None):
+    def __init__(self, state_dict, config=None, device=None, denoise_c=0.0, denoise_hp=None):
         _require_cuda()
+        self.denoise_c = float(denoise_c)
+        self._denoise_hp = denoise_hp
+        self._denoiser = None
         self.cfg = dict(DEFAULT_VOCODER_CONFIG, **(config or {}))
         self.device = torch.device(device if device is not None else "cuda:0")
         torch.cuda.set_device(self.device)
@@ -474,11 +480,14 @@ class Vocoder:
 
     max_frames_per_call = 24000  # ~0.9 MB of stage buffers per frame: bounds the workspace to ~20 GB
 
-    def generate(self, mel, f0, frame_offsets, rand_ini=None, src_noise=None, seed=0):
+    def generate(self, mel, f0, frame_offsets, rand_ini=None, src_noise=None, seed=0, denoise_c=None):
         """mel [sumF,80], f0 [sumF] or None (device, tight) -> wav [sumF*hop] (device).
-        Large batches are processed in groups of utterances (results are per-utterance, so grouping is exact)."""
+        Large batches are processed in groups of utterances (results are per-utterance, so grouping is exact).
+        denoise_c: the denoiser strength for this call (None = the vocoder's own ``denoise_c``); > 0 denoises every group
+        in place right after it is generated."""
         fo = np.ascontiguousarray(frame_offsets, np.int32)
         B = len(fo) - 1
+        c = self.denoise_c if denoise_c is None else float(denoise_c)
         if B > 1 and int(fo[-1]) > self.max_frames_per_call:
             wav = torch.empty(int(fo[-1]) * self.hop, dtype=torch.float32, device=self.device)
             b0 = 0
@@ -490,7 +499,7 @@ class Vocoder:
                 a, e = int(fo[b0]), int(fo[b1])
                 w = self.generate(mel[a:e], None if f0 is None else f0[a:e], sub_fo,
                                   None if rand_ini is None else rand_ini[b0:b1].contiguous(),
-                                  None if src_noise is None else src_noise[a * self.hop:e * self.hop], seed + b0)
+                                  None if src_noise is None else src_noise[a * self.hop:e * self.hop], seed + b0, c)
                 wav[a * self.hop:e * self.hop] = w
                 b0 = b1
             return wav
@@ -502,7 +511,58 @@ class Vocoder:
         stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
         check(lib.ssb_hifigan_generate(self._h, _ptr(mel), _ptr(f0), fo.ctypes.data, B, _ptr(rand_ini), _ptr(src_noise),
                                        int(seed), _ptr(wav), _ptr(ws), ws.numel(), stream), "ssb_hifigan_generate")
+        if c > 0:  # hifigan_nsf.py:73-74: only a positive strength runs the denoiser
+            if self._denoiser is None:
+                self._denoiser = WavDenoiser(self._denoise_hp if self._denoise_hp is not None else self.cfg, self.device)
+            self._denoiser(wav, fo * self.hop, c, out=wav, workspace=self._ws)
         return wav
+
+
+class WavDenoiser:
+    """Spectral-subtraction denoiser of the vocoder output (ssb_wav_denoise_t): denoise(wav, v) of the reference
+    (tasks/tts/vocoder_infer/hifigan_nsf.py:14-22), every utterance on its own.  Geometry from hp's fft_size / hop_size /
+    win_size (defaults 1024 / 256 / 1024, as MelSpectrogram)."""
+
+    def __init__(self, hp=None, device=None):
+        _require_cuda()
+        h = dict(fft_size=1024, hop_size=256, win_size=1024)
+        h.update({k: v for k, v in (hp or {}).items() if k in h})
+        self.hp = h
+        self.device = torch.device(device if device is not None else "cuda:0")
+        torch.cuda.set_device(self.device)
+        handle = C.c_void_p()
+        check(lib.ssb_wav_denoise_create(C.byref(handle), h["fft_size"], h["hop_size"], h["win_size"]), "ssb_wav_denoise_create")
+        self._h = handle
+        self._ws = _Workspace(self.device)
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            lib.ssb_wav_denoise_free(h)
+            self._h = None
+
+    def set_tensor_cores(self, mode=1):
+        """GEMM path: 1 / True = tensor cores for batches of >= 8 row tiles, FFMA below (default); 0 / False = fp32 FFMA
+        always; 2 = tensor cores at every size (tests, measurement).  Returns the mode in effect."""
+        return int(lib.ssb_wav_denoise_set_tensor_cores(self._h, int(mode)))
+
+    def workspace_bytes(self, sample_offsets):
+        so = np.ascontiguousarray(sample_offsets, np.int32)
+        return int(lib.ssb_wav_denoise_workspace_bytes(self._h, so.ctypes.data, len(so) - 1))
+
+    def __call__(self, wav, sample_offsets, v, out=None, workspace=None):
+        """wav: device fp32 [sum n_b] (utterances concatenated, every n_b a positive multiple of hop_size), sample_offsets:
+        [B+1].  Returns the denoised waveform (``out``, which may be ``wav`` itself, or a new tensor)."""
+        so = np.ascontiguousarray(sample_offsets, np.int32)
+        n = lib.ssb_wav_denoise_workspace_bytes(self._h, so.ctypes.data, len(so) - 1)
+        if n == 0:
+            check(-1, "ssb_wav_denoise_workspace_bytes")
+        ws = (workspace or self._ws).get(n)
+        out = torch.empty_like(wav) if out is None else out
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        check(lib.ssb_wav_denoise_forward(self._h, _ptr(wav), so.ctypes.data, len(so) - 1, float(v), _ptr(out), _ptr(ws),
+                                          ws.numel(), stream), "ssb_wav_denoise_forward")
+        return out
 
 
 # unit-test granularity ops -------------------------------------------------------------------------

@@ -29,7 +29,9 @@ class StyleSingerInfer:
         if model_state_dict is None or vocoder_state_dict is None:
             raise ValueError("state dicts required (reference checkpoints or stylesinger_b200.synth.*_state_dict)")
         self.model = AcousticModel(model_state_dict, self.hparams, self.device)
-        self.vocoder = Vocoder(vocoder_state_dict, vocoder_config, self.device)
+        # HifiGAN.spec2wav (tasks/tts/vocoder_infer/hifigan_nsf.py:73-74): denoise the waveform when vocoder_denoise_c > 0
+        self.vocoder = Vocoder(vocoder_state_dict, vocoder_config, self.device,
+                               denoise_c=self.hparams.get("vocoder_denoise_c", 0.0), denoise_hp=self.hparams)
         self._cnt = torch.zeros(1, dtype=torch.int32, device=self.device)
         self._pinned = []  # [(pinned tensor, weakref to the numpy array handed out last)]: see _host_out
 

@@ -272,11 +272,14 @@ class PitchPredictor(_Registered):
 
 
 class HifiGAN:
-    """``spec2wav(mel, f0=...)`` with numpy in / numpy out (tasks/tts/vocoder_infer/hifigan_nsf.py:62-75)."""
+    """``spec2wav(mel, f0=...)`` with numpy in / numpy out (tasks/tts/vocoder_infer/hifigan_nsf.py:62-75).  ``denoise_c`` is
+    hparams['vocoder_denoise_c']: > 0 runs the reference's output denoiser (:14-22,73-74) on the waveform."""
 
-    def __init__(self, state_dict=None, config=None, device=None, use_nsf=True, engine: Optional[Vocoder] = None):
+    def __init__(self, state_dict=None, config=None, device=None, use_nsf=True, engine: Optional[Vocoder] = None,
+                 denoise_c=0.0):
         self.v = engine if engine is not None else Vocoder(state_dict, config, device)
         self.use_nsf = use_nsf
+        self.denoise_c = float(denoise_c)
 
     def spec2wav(self, mel, **kwargs):
         f0 = kwargs.get("f0")
@@ -286,5 +289,5 @@ class HifiGAN:
         if f0 is not None and self.use_nsf:
             f = torch.as_tensor(np.ascontiguousarray(f0), dtype=torch.float32).to(dev)
         offs = np.array([0, m.shape[0]], np.int32)
-        wav = self.v.generate(m, f, offs, seed=int(kwargs.get("seed", 0)))
+        wav = self.v.generate(m, f, offs, seed=int(kwargs.get("seed", 0)), denoise_c=self.denoise_c)
         return wav.cpu().numpy()

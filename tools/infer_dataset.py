@@ -4,7 +4,7 @@ ragged batches and writes one wav per item.  Equivalent of `python tasks/run.py 
 (tasks/StyleSinger/stylesinger.py:168-275, which asserts B=1).
 
     python tools/infer_dataset.py --ckpt checkpoints/StyleSinger --vocoder checkpoints/hifigan --data data/binary/x/test \
-        --out infer_out [--batch 64] [--T 100] [--limit N] [--use-gt-dur]
+        --out infer_out [--batch 64] [--T 100] [--limit N] [--use-gt-dur] [--vocoder-denoise-c 0.1]
 
 Like the reference's test_step (tasks/StyleSinger/stylesinger.py:177-180 with `use_gt_dur: false` in egs/stylesinger.yaml) the
 durations come from the duration predictor unless --use-gt-dur is given (then the items' ground-truth mel2ph is fed).
@@ -29,6 +29,8 @@ def main():
     ap.add_argument("--limit", type=int, default=0)
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--use-gt-dur", action="store_true", help="feed the items' ground-truth mel2ph (reference hparam use_gt_dur)")
+    ap.add_argument("--vocoder-denoise-c", type=float, default=0.0,
+                    help="reference hparam vocoder_denoise_c: > 0 denoises every waveform (hifigan_nsf.py:14-22,73-74)")
     args = ap.parse_args()
 
     from scipy.io import wavfile
@@ -36,7 +38,7 @@ def main():
     from stylesinger_b200.hparams import resolve
     from stylesinger_b200.infer import StyleSingerInfer
 
-    hp = resolve(timesteps=args.T, K_step=args.T, f0_timesteps=args.T)
+    hp = resolve(timesteps=args.T, K_step=args.T, f0_timesteps=args.T, vocoder_denoise_c=args.vocoder_denoise_c)
     sd, path = formats.load_state_dict(args.ckpt, "model")
     vsd, vcfg, vpath = formats.load_vocoder_checkpoint(args.vocoder)
     print(f"| acoustic checkpoint {path} ({len(sd)} tensors); vocoder {vpath}")

@@ -9,19 +9,6 @@ struct ssb_vocoder { ssb::Vocoder v; };
 
 namespace ssb {
 
-#define RUN(x)                 \
-  do {                         \
-    int rc_ = (x);             \
-    if (rc_ != 0) return rc_;  \
-  } while (0)
-#define WS_OK(c) SSB_CHECK((c).dry || !(c).failed, "workspace too small")
-
-static int32_t* alloc_rows_i32(Ctx& c, const SeqDev& s, int C = 1) {
-  int32_t* p = c.alloc<int32_t>((size_t)s.rows * C);
-  if (!c.dry && p && !c.failed) cudaMemsetAsync(p, 0, (size_t)s.rows * C * sizeof(int32_t), c.stream);
-  return p;
-}
-
 // project per-utterance vectors (spk_embed_proj / emo_embed_proj, stylesinger.py:130-132)
 static int project_vec(Ctx& c, const Conv& w, const float* in_tight, int B, float* out_tight) {
   Seq s1;
@@ -161,7 +148,7 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
       RUN(combine_rows(c, sf, a));
     }
     // the FFT decoder's rule for its FFN GEMMs: long batches on the tensor-core kernel
-    const bool tc = m.use_tc && m.fft_tc && tc_available() && sf.ntiles >= 8;
+    const bool tc = long_batch_tc(m, sf);
     RUN(run_pitch_predictor(c, m, 0, sf, cond, pa, tc));
     RUN(run_pitch_predictor(c, m, 1, sf, cond2, ps, tc));
     PitchGlueConvArgs pg;
@@ -249,7 +236,7 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
     WS_OK(c);
     // long batches: the decoder's FFN GEMMs on the tensor-core kernel (short ones stay on the fp32 FFMA path, which is
     // what the reference-golden parity tests pin)
-    RUN(run_fft_decoder(c, m, sf, dec, xd, m.use_tc && m.fft_tc && tc_available() && sf.ntiles >= 8));
+    RUN(run_fft_decoder(c, m, sf, dec, xd, long_batch_tc(m, sf)));
     {
       ConvGemm g = make_gemm(m.mel_out, sf, xd, H);
       g.e.rowmask = tgt; g.e.out = coarse; g.e.ldo = 80;
@@ -538,7 +525,7 @@ static int pitch_predictor_impl(Ctx& c, const Model& m, int which, const float* 
   float* og = alloc_rows(c, s, 2);
   WS_OK(c);
   RUN(pack_rows(c, s, x, 256, xg, 256, 256));
-  RUN(run_pitch_predictor(c, m, which, s, xg, og, m.use_tc && m.fft_tc && tc_available() && s.ntiles >= 8));
+  RUN(run_pitch_predictor(c, m, which, s, xg, og, long_batch_tc(m, s)));
   return unpack_rows(c, s, og, 2, out, 2, 2);
 }
 size_t ssb_pitch_predictor_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B) {
@@ -578,7 +565,7 @@ static int fft_decoder_impl(Ctx& c, const Model& m, const float* x, const int32_
   float* xd = alloc_rows(c, sf, 256);
   WS_OK(c);
   RUN(pack_rows(c, sf, x, 256, xin, 256, 256));
-  RUN(run_fft_decoder(c, m, sf, xin, xd, m.use_tc && m.fft_tc && tc_available() && sf.ntiles >= 8));
+  RUN(run_fft_decoder(c, m, sf, xin, xd, long_batch_tc(m, sf)));
   return unpack_rows(c, sf, xd, 256, out, 256, 256);
 }
 static int get_style_impl(Ctx& c, const Model& m, const float* dec_inp, const int32_t* foffs, const float* ref_mels,
@@ -746,9 +733,8 @@ int ssb_op_conv1d_tc(const float* x, const int32_t* offsets, int32_t B, int32_t 
   if (rc == 0) rc = pack_rows(c, s, x, Cin, xg, Cin, Cin);
   if (rc == 0) rc = split_planes(c, xg, Cin, s.rows, Cin, 1.0f, xh, xl);
   if (rc == 0) {
-    GemmTC g;
-    g.A_hi = xh; g.A_lo = xl; g.rows_total = s.rows; g.w = &ct; g.tiles = s.tiles; g.ntiles = s.ntiles;
-    g.e.mode = EPI_GENERIC; g.e.out = og; g.e.ldo = N;
+    GemmTC g = make_gemm_tc(ct, s, xh, xl);
+    g.e.out = og; g.e.ldo = N;
     rc = conv_gemm_tc(c, g);
   }
   if (rc == 0) rc = unpack_rows(c, s, og, N, out, N, N);

@@ -34,13 +34,6 @@ namespace ssb {
 
 ConvGemm make_gemm(const Conv& c, const SeqDev& s, const float* A, int lda);  // stages.cu
 
-#define RUN(x)                 \
-  do {                         \
-    int rc_ = (x);             \
-    if (rc_ != 0) return rc_;  \
-  } while (0)
-#define WS_OK(c) SSB_CHECK((c).dry || !(c).failed, "workspace too small")
-
 // tight waveform [sum n_b] -> rows of `hop` samples in the guard-banded layout (zero fill behind the last sample)
 __global__ void k_wav_rows(const int4* utt, const int32_t* sample_offs, const float* wav, int hop, float* rows) {
   const int b = blockIdx.y;

@@ -21,6 +21,13 @@ struct Conv {
   int taps = 1, Cin = 0, N = 0, Npad = 0, dil = 1, center = 0;
 };
 
+// A dense layer whose weights are packed for both GEMMs: fp32 FFMA (conv_gemm) and tensor cores (conv_gemm_tc; t.ok is
+// false when the shape is not eligible).  run_dense (stages.cuh) enqueues either.
+struct Dense {
+  Conv f;
+  ConvTC t;
+};
+
 enum PackMode { PACK_PLAIN = 0, PACK_GATE_SIG_TANH = 1 /* DiffNet: [sigmoid C | tanh C] */,
                 PACK_GATE_TANH_SIG = 2 /* WN: [tanh C | sigmoid C] */ };
 
@@ -51,22 +58,21 @@ struct TensorMap {
 
 struct FFTLayer {
   float *ln1_g, *ln1_b, *ln2_g, *ln2_b;
-  Conv qkv, out, ffn1, ffn2;
-  ConvTC ffn1_tc, ffn2_tc;  // the FFN (92 % of the block's FLOPs) on the tensor-core path, used for long sequences
-  ConvTC qkv_tc, out_tc;    // self-attention in/out projections on the same path
+  // the FFN is 92 % of the block's FLOPs; the tensor-core packing of all four is used for long sequences
+  Dense qkv, out, ffn1, ffn2;
 };
 struct FFT {
   std::vector<FFTLayer> layers;
+  bool tc_ok = true;  // every layer's four GEMMs are tensor-core eligible
   float *ln_g = nullptr, *ln_b = nullptr;
   float* pos_alpha = nullptr;  // device scalar, null for the encoder
   int kernel = 9;
 };
 
 struct DenoiserLayer {
-  Conv dil;    // k3 dilated, gate-interleaved columns, N = 2C
-  Conv outp;   // 1x1, N = 2C ([res | skip])
+  Dense dil;   // k3 dilated, gate-interleaved columns, N = 2C
+  Dense outp;  // 1x1, N = 2C ([res | skip])
   Conv dproj;  // diffusion_projection C -> C (used only to build the step-bias table)
-  ConvTC dil_tc, outp_tc;  // tensor-core packing of dil / outp (ok == false when not eligible)
   float* bias_gate_tc = nullptr;  // dil bias + conditioner bias (packed column order): the GATE GEMM's bias (cond_all_tc has none)
 };
 struct Denoiser {
@@ -78,6 +84,7 @@ struct Denoiser {
   std::vector<DenoiserLayer> layers;
   Conv cond_all;                // 256 -> L*2C, gate-interleaved per layer
   ConvTC cond_all_tc;           // the same stacked projection for the tensor-core kernel (hoisted out of the T loop; no bias)
+  bool tc_ok = false;           // cond_all_tc and every layer's dil / outp are tensor-core eligible
   Conv skip_proj, out_proj;
   // schedule-dependent (set by ssb_model_set_schedule)
   int T = 0;
@@ -96,8 +103,8 @@ struct Denoiser {
 // FastSpeech-2 PitchPredictor (tts_modules.py:191-234): f0_gen 'conv' only
 struct PitchPredictor {
   static constexpr int kLayers = 5;
-  Conv conv[kLayers];       // k-tap Conv1d 256 -> 256 + bias (fp32 path)
-  ConvTC conv_tc[kLayers];  // the same convs for the tensor-core kernel (long batches)
+  Dense conv[kLayers];      // k-tap Conv1d 256 -> 256 + bias; the tensor-core packing is used for long batches
+  bool tc_ok = true;        // all of them are tensor-core eligible
   float* ln_g[kLayers] = {};
   float* ln_b[kLayers] = {};
   Conv linear;              // 256 -> 2
@@ -105,8 +112,7 @@ struct PitchPredictor {
 };
 
 struct AlignLayer {
-  Conv q, kv, out, lin1, lin2;
-  ConvTC q_tc, kv_tc, out_tc, lin1_tc, lin2_tc;  // tensor-core packing of the same projections (long batches)
+  Dense q, kv, out, lin1, lin2;  // the tensor-core packing is used for long batches
   float *n1_g, *n1_b, *n2_g, *n2_b;
 };
 
@@ -130,6 +136,7 @@ struct Model {
   float* codebooks = nullptr; float* cb_norm2 = nullptr;  // [depth][n_embed][256], [depth][n_embed]
   Conv l1;
   AlignLayer align[2];
+  bool align_tc_ok = true;  // all ten projections are tensor-core eligible
   Denoiser f0net[2];        // GMDIFF only
   PitchPredictor pp[2];     // CONV only: [0] pitch_predictor (domain agnostic), [1] pitch_inpainter_predictor (specific)
   // SSB_F0_GEN_GMDIFF: hparams['f0_gen'] == 'gmdiff' (two F0 diffusion samplers); SSB_F0_GEN_CONV: 'conv' (pp above)
@@ -151,12 +158,11 @@ struct Model {
 };
 
 struct VocStage {
-  Conv up;          // transposed conv as 3-tap conv, N = u * Cout
+  Dense up;         // transposed conv as 3-tap conv, N = u * Cout
   int u = 1, Cout = 0;
   float *nc_w = nullptr, *nc_b = nullptr; int nc_s = 1;  // noise conv
   float* nc_wt = nullptr;                                 // the same weights as [K, C] (tiled kernel)
-  struct RB { Conv c1[3], c2[3]; ConvTC c1_tc[3], c2_tc[3]; } rb[4];
-  ConvTC up_tc;     // tensor-core packing of the transposed conv
+  struct RB { Dense c1[3], c2[3]; } rb[4];  // paired stage: the tensor-core halves hold the time-paired packing
   bool res_tc = false;  // all ResBlock convs of this stage are tensor-core eligible (C % 64 == 0)
   bool paired = false;  // C == 32: ResBlock convs packed as 64-channel convs over PAIRS of time steps (see pack.cu)
 };
@@ -175,7 +181,10 @@ struct Vocoder {
 int pack_conv(DevicePool& pool, const HostTensor* w, const HostTensor* b, int dil, PackMode mode, Conv* out,
               const HostTensor* g = nullptr /* weight-norm g: w is v */);
 int pack_conv_tc(DevicePool& pool, const HostTensor* w, int dil, PackMode mode, const float* packed_bias, ConvTC* out);
-int pack_linear(DevicePool& pool, const HostTensor* w, const HostTensor* b, Conv* out, int row0 = 0, int nrows = -1);
+int pack_linear(DevicePool& pool, const HostTensor* w, const HostTensor* b, Conv* out);
+// both packings of one layer from one tensor: w [N, Cin, k], or a Linear's [N, Cin] as a 1-tap conv, rows [row0, row0 + nrows)
+int pack_dense(DevicePool& pool, const HostTensor* w, const HostTensor* b, int dil, PackMode mode, Dense* out,
+               const HostTensor* g = nullptr /* weight-norm g: w is v */, int row0 = 0, int nrows = -1);
 int pack_conv_transpose(DevicePool& pool, const HostTensor* v, const HostTensor* g, const HostTensor* b, int u, Conv* out);
 int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder = SSB_MEL_DECODER_DIFFSINGER,
                 int f0_gen = SSB_F0_GEN_GMDIFF);
@@ -185,5 +194,6 @@ int set_schedule(Model* m, int which, int T, const float* step_emb, const float*
 
 // ---- op helpers (stages.cu) ------------------------------------------------------------------------
 ConvGemm make_gemm(const Conv& c, const SeqDev& s, const float* A, int lda);
+GemmTC make_gemm_tc(const ConvTC& w, const SeqDev& s, const __half* A_hi, const __half* A_lo);
 
 }  // namespace ssb

@@ -136,15 +136,24 @@ int pack_conv_tc(DevicePool& pool, const HostTensor* w, int dil, PackMode mode, 
   return make_weight_maps(out);
 }
 
-// weight-normed Conv1d -> tensor-core packing
-static int pack_conv_tc_wn(DevicePool& pool, const HostTensor* v, const HostTensor* g, int dil, const float* packed_bias, ConvTC* out) {
-  if (!v || !g) return -1;
-  std::vector<float> w;
-  fold_weight_norm(v, g, w);
-  HostTensor t;
-  t.data = w.data();
-  t.shape = v->shape;
-  return pack_conv_tc(pool, &t, dil, PACK_PLAIN, packed_bias, out);
+int pack_dense(DevicePool& pool, const HostTensor* w, const HostTensor* b, int dil, PackMode mode, Dense* out,
+               const HostTensor* g, int row0, int nrows) {
+  if (!w) return -1;
+  SSB_CHECK(w->shape.size() == 3 || w->shape.size() == 2, "pack_dense: weight must be [N,Cin,k] or [N,Cin]");
+  const int Cin = (int)w->shape[1], k = w->shape.size() == 3 ? (int)w->shape[2] : 1;
+  if (nrows < 0) nrows = (int)w->shape[0] - row0;
+  std::vector<float> folded;
+  const float* src = w->data;
+  if (g) {
+    fold_weight_norm(w, g, folded);
+    src = folded.data();
+  }
+  src += (size_t)row0 * Cin * k;
+  if (pack_from_host(pool, src, nrows, Cin, k, b ? b->data + row0 : nullptr, dil, mode, &out->f)) return -1;
+  HostTensor t;  // the tensor-core packer reads the torch conv layout [N, Cin, k]; its bias is the packed fp32 vector
+  t.data = src;
+  t.shape = {nrows, Cin, k};
+  return pack_conv_tc(pool, &t, dil, mode, out->f.bias, &out->t);
 }
 // Narrow convs (C = 32) on the 64-wide tensor-core K block: view [rows, 32] as [rows/2, 64] (two consecutive time
 // steps per "super row", super channel = phase*32 + c).  y[2q+phi, n] = sum_j sum_c W[n][c][j] x[2q + phi + s_j, c]
@@ -205,11 +214,9 @@ static int pack_conv_transpose_tc(DevicePool& pool, const HostTensor* v, const H
   return pack_conv_tc(pool, &ht, 1, PACK_PLAIN, packed_bias, out);
 }
 
-int pack_linear(DevicePool& pool, const HostTensor* w, const HostTensor* b, Conv* out, int row0, int nrows) {
+int pack_linear(DevicePool& pool, const HostTensor* w, const HostTensor* b, Conv* out) {
   if (!w) return -1;
-  const int Ntot = (int)w->shape[0], Cin = (int)w->shape[1];
-  if (nrows < 0) nrows = Ntot - row0;
-  return pack_from_host(pool, w->data + (size_t)row0 * Cin, nrows, Cin, 1, b ? b->data + row0 : nullptr, 1, PACK_PLAIN, out);
+  return pack_from_host(pool, w->data, (int)w->shape[0], (int)w->shape[1], 1, b ? b->data : nullptr, 1, PACK_PLAIN, out);
 }
 
 // ConvTranspose1d(Cin, Cout, k, stride u, padding (k-u)/2) as a 3-tap conv with N = u*Cout:
@@ -266,27 +273,12 @@ static int build_fft(TensorMap& tm, DevicePool& pool, const std::string& p, int 
     L.ln1_b = upload_tensor(pool, tm.get(q + "layer_norm1.bias"));
     L.ln2_g = upload_tensor(pool, tm.get(q + "layer_norm2.weight"));
     L.ln2_b = upload_tensor(pool, tm.get(q + "layer_norm2.bias"));
-    if (pack_linear(pool, tm.get(q + "self_attn.in_proj_weight"), nullptr, &L.qkv)) return -1;
-    if (pack_linear(pool, tm.get(q + "self_attn.out_proj.weight"), nullptr, &L.out)) return -1;
-    if (pack_conv(pool, tm.get(q + "ffn.ffn_1.weight"), tm.get(q + "ffn.ffn_1.bias"), 1, PACK_PLAIN, &L.ffn1)) return -1;
-    if (pack_linear(pool, tm.get(q + "ffn.ffn_2.weight"), tm.get(q + "ffn.ffn_2.bias"), &L.ffn2)) return -1;
-    if (pack_conv_tc(pool, tm.get(q + "ffn.ffn_1.weight"), 1, PACK_PLAIN, L.ffn1.bias, &L.ffn1_tc)) return -1;
-    for (int which = 0; which < 2; ++which) {  // in_proj [3H, H] / out_proj [H, H], bias-free (common_layers.py:200-205)
-      const HostTensor* w = tm.get(q + (which == 0 ? "self_attn.in_proj_weight" : "self_attn.out_proj.weight"));
-      if (!w) return -1;
-      HostTensor ht;
-      ht.data = w->data;
-      ht.shape = {w->shape[0], w->shape[1], 1};
-      if (pack_conv_tc(pool, &ht, 1, PACK_PLAIN, nullptr, which == 0 ? &L.qkv_tc : &L.out_tc)) return -1;
-    }
-    {
-      const HostTensor* w2 = tm.get(q + "ffn.ffn_2.weight");  // Linear [H, 4H] as a 1-tap conv
-      if (!w2) return -1;
-      HostTensor ht;
-      ht.data = w2->data;
-      ht.shape = {w2->shape[0], w2->shape[1], 1};
-      if (pack_conv_tc(pool, &ht, 1, PACK_PLAIN, L.ffn2.bias, &L.ffn2_tc)) return -1;
-    }
+    // in_proj [3H, H] / out_proj [H, H], bias-free (common_layers.py:200-205)
+    if (pack_dense(pool, tm.get(q + "self_attn.in_proj_weight"), nullptr, 1, PACK_PLAIN, &L.qkv)) return -1;
+    if (pack_dense(pool, tm.get(q + "self_attn.out_proj.weight"), nullptr, 1, PACK_PLAIN, &L.out)) return -1;
+    if (pack_dense(pool, tm.get(q + "ffn.ffn_1.weight"), tm.get(q + "ffn.ffn_1.bias"), 1, PACK_PLAIN, &L.ffn1)) return -1;
+    if (pack_dense(pool, tm.get(q + "ffn.ffn_2.weight"), tm.get(q + "ffn.ffn_2.bias"), 1, PACK_PLAIN, &L.ffn2)) return -1;
+    f->tc_ok = f->tc_ok && L.qkv.t.ok && L.out.t.ok && L.ffn1.t.ok && L.ffn2.t.ok;
   }
   f->ln_g = upload_tensor(pool, tm.get(p + "layer_norm.weight"));
   f->ln_b = upload_tensor(pool, tm.get(p + "layer_norm.bias"));
@@ -313,11 +305,9 @@ static int build_denoiser(TensorMap& tm, DevicePool& pool, const std::string& p,
   for (int i = 0; i < L; ++i) {
     const std::string q = p + "residual_layers." + std::to_string(i) + ".";
     const int dil = 1 << (i % cycle);
-    if (pack_conv(pool, tm.get(q + "dilated_conv.weight"), tm.get(q + "dilated_conv.bias"), dil, PACK_GATE_SIG_TANH, &d->layers[i].dil)) return -1;
-    if (pack_conv(pool, tm.get(q + "output_projection.weight"), tm.get(q + "output_projection.bias"), 1, PACK_PLAIN, &d->layers[i].outp)) return -1;
+    if (pack_dense(pool, tm.get(q + "dilated_conv.weight"), tm.get(q + "dilated_conv.bias"), dil, PACK_GATE_SIG_TANH, &d->layers[i].dil)) return -1;
+    if (pack_dense(pool, tm.get(q + "output_projection.weight"), tm.get(q + "output_projection.bias"), 1, PACK_PLAIN, &d->layers[i].outp)) return -1;
     if (pack_linear(pool, tm.get(q + "diffusion_projection.weight"), tm.get(q + "diffusion_projection.bias"), &d->layers[i].dproj)) return -1;
-    if (pack_conv_tc(pool, tm.get(q + "dilated_conv.weight"), dil, PACK_GATE_SIG_TANH, d->layers[i].dil.bias, &d->layers[i].dil_tc)) return -1;
-    if (pack_conv_tc(pool, tm.get(q + "output_projection.weight"), 1, PACK_PLAIN, d->layers[i].outp.bias, &d->layers[i].outp_tc)) return -1;
     const HostTensor* cw = tm.get(q + "conditioner_projection.weight");
     const HostTensor* cb = tm.get(q + "conditioner_projection.bias");
     if (!cw || !cb) return -1;
@@ -344,6 +334,8 @@ static int build_denoiser(TensorMap& tm, DevicePool& pool, const std::string& p,
     ht.shape = {L * N2, H, 1};
     if (pack_conv_tc(pool, &ht, 1, PACK_PLAIN, nullptr, &d->cond_all_tc)) return -1;
   }
+  d->tc_ok = d->cond_all_tc.ok;
+  for (auto& l : d->layers) d->tc_ok = d->tc_ok && l.dil.t.ok && l.outp.t.ok;
   d->cond_all.W = pool.upload(Wc);
   d->cond_all.bias = pool.upload(Bc);
   d->cond_all.taps = 1; d->cond_all.Cin = H; d->cond_all.N = L * N2; d->cond_all.Npad = L * N2; d->cond_all.dil = 1; d->cond_all.center = 0;
@@ -403,8 +395,8 @@ static int build_pitch_predictor(TensorMap& tm, DevicePool& pool, const std::str
     SSB_CHECK(k % 2 == 1 && (k - 1) / 2 <= GUARD,
               "ssb_model_create: " + q + "1.weight: kernel size " + std::to_string(k) + " must be odd with (k - 1) / 2 <= " +
                   std::to_string(GUARD));
-    if (pack_conv(pool, w, tm.get(q + "1.bias", {H}), 1, PACK_PLAIN, &pp->conv[i])) return -1;
-    if (pack_conv_tc(pool, w, 1, PACK_PLAIN, pp->conv[i].bias, &pp->conv_tc[i])) return -1;
+    if (pack_dense(pool, w, tm.get(q + "1.bias", {H}), 1, PACK_PLAIN, &pp->conv[i])) return -1;
+    pp->tc_ok = pp->tc_ok && pp->conv[i].t.ok;
     pp->ln_g[i] = upload_tensor(pool, tm.get(q + "3.weight", {H}));
     pp->ln_b[i] = upload_tensor(pool, tm.get(q + "3.bias", {H}));
   }
@@ -492,28 +484,12 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder,
     AlignLayer& a = m->align[i];
     const HostTensor* iw = tm.get(q + "multihead_attn.in_proj_weight", {3 * H, H});
     const HostTensor* ib = tm.get(q + "multihead_attn.in_proj_bias", {3 * H});
-    PK(pack_linear(pool, iw, ib, &a.q, 0, H));
-    PK(pack_linear(pool, iw, ib, &a.kv, H, 2 * H));
-    PK(pack_linear(pool, tm.get(q + "multihead_attn.out_proj.weight"), tm.get(q + "multihead_attn.out_proj.bias"), &a.out));
-    PK(pack_linear(pool, tm.get(q + "linear1.weight"), tm.get(q + "linear1.bias"), &a.lin1));
-    PK(pack_linear(pool, tm.get(q + "linear2.weight"), tm.get(q + "linear2.bias"), &a.lin2));
-    {  // the same five projections for the tensor-core kernel (biases: the packed fp32 vectors above)
-      auto lin_tc = [&](const float* data, int64_t n, int64_t k, const float* bias, ConvTC* out) {
-        HostTensor ht;
-        ht.data = data;
-        ht.shape = {n, k, 1};
-        return pack_conv_tc(pool, &ht, 1, PACK_PLAIN, bias, out);
-      };
-      const HostTensor* ow = tm.get(q + "multihead_attn.out_proj.weight");
-      const HostTensor* w1 = tm.get(q + "linear1.weight");
-      const HostTensor* w2 = tm.get(q + "linear2.weight");
-      if (!iw || !ow || !w1 || !w2) goto fail;
-      PK(lin_tc(iw->data, H, H, a.q.bias, &a.q_tc));
-      PK(lin_tc(iw->data + (size_t)H * H, 2 * H, H, a.kv.bias, &a.kv_tc));
-      PK(lin_tc(ow->data, ow->shape[0], ow->shape[1], a.out.bias, &a.out_tc));
-      PK(lin_tc(w1->data, w1->shape[0], w1->shape[1], a.lin1.bias, &a.lin1_tc));
-      PK(lin_tc(w2->data, w2->shape[0], w2->shape[1], a.lin2.bias, &a.lin2_tc));
-    }
+    PK(pack_dense(pool, iw, ib, 1, PACK_PLAIN, &a.q, nullptr, 0, H));
+    PK(pack_dense(pool, iw, ib, 1, PACK_PLAIN, &a.kv, nullptr, H, 2 * H));
+    PK(pack_dense(pool, tm.get(q + "multihead_attn.out_proj.weight"), tm.get(q + "multihead_attn.out_proj.bias"), 1, PACK_PLAIN, &a.out));
+    PK(pack_dense(pool, tm.get(q + "linear1.weight"), tm.get(q + "linear1.bias"), 1, PACK_PLAIN, &a.lin1));
+    PK(pack_dense(pool, tm.get(q + "linear2.weight"), tm.get(q + "linear2.bias"), 1, PACK_PLAIN, &a.lin2));
+    m->align_tc_ok = m->align_tc_ok && a.q.t.ok && a.kv.t.ok && a.out.t.ok && a.lin1.t.ok && a.lin2.t.ok;
     a.n1_g = upload_tensor(pool, tm.get(q + "norm1.weight"));
     a.n1_b = upload_tensor(pool, tm.get(q + "norm1.bias"));
     a.n2_g = upload_tensor(pool, tm.get(q + "norm2.weight"));
@@ -571,8 +547,8 @@ int build_vocoder(TensorMap& tm, const ssb_vocoder_config& cfg, Vocoder* v) {
       s.u = cfg.up_rates[i];
       s.Cout = c / 2;
       SSB_CHECK(cfg.up_kernels[i] == 2 * cfg.up_rates[i] || cfg.up_kernels[i] - cfg.up_rates[i] >= 0, "vocoder: bad upsample kernel");
-      PK(pack_conv_transpose(pool, tm.get(u + "weight_v"), tm.get(u + "weight_g"), tm.get(u + "bias"), s.u, &s.up));
-      PK(pack_conv_transpose_tc(pool, tm.get(u + "weight_v"), tm.get(u + "weight_g"), s.u, s.up.bias, &s.up_tc));
+      PK(pack_conv_transpose(pool, tm.get(u + "weight_v"), tm.get(u + "weight_g"), tm.get(u + "bias"), s.u, &s.up.f));
+      PK(pack_conv_transpose_tc(pool, tm.get(u + "weight_v"), tm.get(u + "weight_g"), s.u, s.up.f.bias, &s.up.t));
       s.res_tc = true;
       prod_after /= s.u;
       if (v->nsf) {
@@ -596,19 +572,17 @@ int build_vocoder(TensorMap& tm, const ssb_vocoder_config& cfg, Vocoder* v) {
         for (int mI = 0; mI < 3; ++mI) {
           const std::string q = "resblocks." + std::to_string(i * cfg.n_res + j) + ".";
           const std::string a = q + "convs1." + std::to_string(mI) + ".", b2 = q + "convs2." + std::to_string(mI) + ".";
-          PK(pack_conv(pool, tm.get(a + "weight_v"), tm.get(a + "bias"), cfg.res_dilations[j][mI], PACK_PLAIN, &s.rb[j].c1[mI], tm.get(a + "weight_g")));
-          PK(pack_conv(pool, tm.get(b2 + "weight_v"), tm.get(b2 + "bias"), 1, PACK_PLAIN, &s.rb[j].c2[mI], tm.get(b2 + "weight_g")));
-          PK(pack_conv_tc_wn(pool, tm.get(a + "weight_v"), tm.get(a + "weight_g"), cfg.res_dilations[j][mI], s.rb[j].c1[mI].bias, &s.rb[j].c1_tc[mI]));
-          PK(pack_conv_tc_wn(pool, tm.get(b2 + "weight_v"), tm.get(b2 + "weight_g"), 1, s.rb[j].c2[mI].bias, &s.rb[j].c2_tc[mI]));
-          if (!s.rb[j].c1_tc[mI].ok || !s.rb[j].c2_tc[mI].ok) s.res_tc = false;
+          PK(pack_dense(pool, tm.get(a + "weight_v"), tm.get(a + "bias"), cfg.res_dilations[j][mI], PACK_PLAIN, &s.rb[j].c1[mI], tm.get(a + "weight_g")));
+          PK(pack_dense(pool, tm.get(b2 + "weight_v"), tm.get(b2 + "bias"), 1, PACK_PLAIN, &s.rb[j].c2[mI], tm.get(b2 + "weight_g")));
+          if (!s.rb[j].c1[mI].t.ok || !s.rb[j].c2[mI].t.ok) s.res_tc = false;
           if (s.Cout == 32) {  // narrow stage: time-paired packing instead
             const HostTensor* b1 = tm.get(a + "bias");
             const HostTensor* b3 = tm.get(b2 + "bias");
             float* bp = nullptr;
-            PK(pack_conv_paired_tc(pool, tm.get(a + "weight_v"), tm.get(a + "weight_g"), cfg.res_dilations[j][mI], b1 ? b1->data : nullptr, &s.rb[j].c1_tc[mI], &bp));
-            PK(pack_conv_paired_tc(pool, tm.get(b2 + "weight_v"), tm.get(b2 + "weight_g"), 1, b3 ? b3->data : nullptr, &s.rb[j].c2_tc[mI], &bp));
+            PK(pack_conv_paired_tc(pool, tm.get(a + "weight_v"), tm.get(a + "weight_g"), cfg.res_dilations[j][mI], b1 ? b1->data : nullptr, &s.rb[j].c1[mI].t, &bp));
+            PK(pack_conv_paired_tc(pool, tm.get(b2 + "weight_v"), tm.get(b2 + "weight_g"), 1, b3 ? b3->data : nullptr, &s.rb[j].c2[mI].t, &bp));
             if (mI == 0 && j == 0) s.paired = true;
-            if (!s.rb[j].c1_tc[mI].ok || !s.rb[j].c2_tc[mI].ok) s.paired = false;
+            if (!s.rb[j].c1[mI].t.ok || !s.rb[j].c2[mI].t.ok) s.paired = false;
           }
         }
       }

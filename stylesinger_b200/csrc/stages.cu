@@ -14,6 +14,38 @@ ConvGemm make_gemm(const Conv& c, const SeqDev& s, const float* A, int lda) {
   g.e.bias = c.bias;
   return g;
 }
+GemmTC make_gemm_tc(const ConvTC& w, const SeqDev& s, const __half* A_hi, const __half* A_lo) {
+  GemmTC g;
+  g.A_hi = A_hi; g.A_lo = A_lo; g.rows_total = s.rows; g.w = &w; g.tiles = s.tiles; g.ntiles = s.ntiles;
+  g.e.mode = EPI_GENERIC;
+  return g;
+}
+
+int run_dense(Ctx& c, const Dense& d, bool tc, const SeqDev& s, const DenseIn& in, const Epi& e) {
+  SSB_CHECK(!e.bias, "run_dense: the bias is the layer's own");
+  if (!tc) {
+    SSB_CHECK(in.x != nullptr, "run_dense: the fp32 kernel needs the input as fp32 rows");
+    ConvGemm g = make_gemm(d.f, s, in.x, in.ld);
+    g.a_act = in.act; g.a_slope = in.slope;
+    g.e = e;
+    g.e.bias = d.f.bias;
+    return conv_gemm(c, g);
+  }
+  SSB_CHECK(d.t.ok && in.hi && in.lo, "run_dense: the tensor-core kernel needs eligible weights and the input as fp16 planes");
+  SSB_CHECK(e.mode == EPI_GENERIC && !e.add && e.beta == 1.0f && !e.out2,
+            "run_dense: the tensor-core kernel's generic epilogue has no gate / skip mode, addend, beta or second fp32 output");
+  GemmTC g = make_gemm_tc(d.t, s, in.hi, in.lo);
+  EpiTC& t = g.e;
+  t.out = e.out; t.ldo = e.ldo;
+  t.oh = e.out2_h; t.ol = e.out2_l; t.ldh = e.ldh; t.vec2 = e.vec2;
+  t.plane_act = e.plane_act; t.plane_slope = e.plane_slope;
+  t.res = e.res; t.ld_res = e.ld_res; t.rowmask = e.rowmask;
+  t.alpha = e.alpha; t.act = e.act; t.act_slope = e.act_slope;
+  t.accum = e.accum; t.gamma = e.gamma;
+  return conv_gemm_tc(c, g);
+}
+
+bool long_batch_tc(const Model& m, const SeqDev& s) { return m.use_tc && m.fft_tc && tc_available() && s.ntiles >= 8; }
 
 int upload_layout(Ctx& c, const Seq& s, int rate, SeqDev* out) {
   const int nt = s.ntiles(rate);
@@ -52,20 +84,16 @@ float* alloc_rows(Ctx& c, const SeqDev& s, int C, bool zero) {
   if (!c.dry && p && !c.failed && zero) cudaMemsetAsync(p, 0, (size_t)s.rows * C * sizeof(float), c.stream);
   return p;
 }
-static int32_t* alloc_rows_i32(Ctx& c, const SeqDev& s, int C = 1) {
+int32_t* alloc_rows_i32(Ctx& c, const SeqDev& s, int C) {
   int32_t* p = c.alloc<int32_t>((size_t)s.rows * C);
   if (!c.dry && p && !c.failed) cudaMemsetAsync(p, 0, (size_t)s.rows * C * sizeof(int32_t), c.stream);
   return p;
 }
-
-static __half* alloc_half_rows(Ctx& c, const SeqDev& s, int C);
-
-#define RUN(x)                 \
-  do {                         \
-    int rc_ = (x);             \
-    if (rc_ != 0) return rc_;  \
-  } while (0)
-#define WS_OK(c) SSB_CHECK((c).dry || !(c).failed, "workspace too small")
+__half* alloc_half_rows(Ctx& c, const SeqDev& s, int C) {
+  __half* p = c.alloc<__half>((size_t)s.rows * C);
+  if (!c.dry && p && !c.failed) cudaMemsetAsync(p, 0, (size_t)s.rows * C * sizeof(__half), c.stream);
+  return p;
+}
 
 // ------------------------------------------------------------------------------------------------
 // a2-a5: FFTBlocks body (tts_modules.py:293-305 + EncSALayer common_layers.py:649-673)
@@ -73,7 +101,7 @@ static __half* alloc_half_rows(Ctx& c, const SeqDev& s, int C);
 int fft_blocks(Ctx& c, const FFT& f, const SeqDev& s, float* x, const float* keep, bool tc) {
   const int H = 256;
   const size_t mk = c.mark();
-  for (auto& L : f.layers) tc = tc && L.ffn1_tc.ok && L.ffn2_tc.ok && L.qkv_tc.ok && L.out_tc.ok;
+  tc = tc && f.tc_ok;
   float* h = alloc_rows(c, s, H);
   float* qkv = alloc_rows(c, s, 3 * H);
   float* att = alloc_rows(c, s, H);
@@ -95,18 +123,12 @@ int fft_blocks(Ctx& c, const FFT& f, const SeqDev& s, float* x, const float* kee
   for (size_t i = 0; i < f.layers.size(); ++i) {
     const FFTLayer& L = f.layers[i];
     RUN(layernorm_rows(c, s, x, H, h, H, H, L.ln1_g, L.ln1_b, 1e-5f, nullptr));
-    if (tc) {
-      RUN(split_planes(c, h, H, s.rows, H, 1.0f, hh, hl));
-      GemmTC g;
-      g.A_hi = hh; g.A_lo = hl; g.rows_total = s.rows; g.w = &L.qkv_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-      g.e.mode = EPI_GENERIC;
-      if (atc) { g.e.oh = qh; g.e.ol = ql; g.e.ldh = 3 * H; }
-      else { g.e.out = qkv; g.e.ldo = 3 * H; }
-      RUN(conv_gemm_tc(c, g));
-    } else {
-      ConvGemm g = make_gemm(L.qkv, s, h, H);
-      g.e.out = qkv; g.e.ldo = 3 * H;
-      RUN(conv_gemm(c, g));
+    if (tc) RUN(split_planes(c, h, H, s.rows, H, 1.0f, hh, hl));
+    {
+      Epi e;
+      if (atc) { e.out2_h = qh; e.out2_l = ql; e.ldh = 3 * H; }
+      else { e.out = qkv; e.ldo = 3 * H; }
+      RUN(run_dense(c, L.qkv, tc, s, {h, H, hh, hl}, e));
     }
     if (atc) {
       RUN(transpose_planes(c, qh, ql, 3 * H, 2 * H, s.rows, H, vth, vtl, ldvt));
@@ -126,41 +148,20 @@ int fft_blocks(Ctx& c, const FFT& f, const SeqDev& s, float* x, const float* kee
       a.out = att; a.ldo = H;
       RUN(attention(c, a));
     }
-    if (tc) {
-      if (!atc) RUN(split_planes(c, att, H, s.rows, H, 1.0f, hh, hl));
-      GemmTC g;
-      g.A_hi = hh; g.A_lo = hl; g.rows_total = s.rows; g.w = &L.out_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-      g.e.mode = EPI_GENERIC; g.e.res = x; g.e.ld_res = H; g.e.rowmask = keep; g.e.out = x; g.e.ldo = H;
-      RUN(conv_gemm_tc(c, g));
-    } else {
-      ConvGemm g = make_gemm(L.out, s, att, H);
-      g.e.res = x; g.e.ld_res = H; g.e.rowmask = keep; g.e.out = x; g.e.ldo = H;
-      RUN(conv_gemm(c, g));
-    }
+    if (tc && !atc) RUN(split_planes(c, att, H, s.rows, H, 1.0f, hh, hl));
+    Epi eres;  // x = (x + layer output) * keep: the epilogue of the out-projection and of ffn_2
+    eres.res = x; eres.ld_res = H; eres.rowmask = keep; eres.out = x; eres.ldo = H;
+    RUN(run_dense(c, L.out, tc, s, {att, H, hh, hl}, eres));
     RUN(layernorm_rows(c, s, x, H, h, H, H, L.ln2_g, L.ln2_b, 1e-5f, nullptr));
-    if (tc) {  // TransformerFFNLayer (transformer.py): ffn_2(gelu(ffn_1(x) * k^-0.5)) on the tensor-core kernel
-      RUN(split_planes(c, h, H, s.rows, H, 1.0f, hh, hl));
-      GemmTC g1;
-      g1.A_hi = hh; g1.A_lo = hl; g1.rows_total = s.rows; g1.w = &L.ffn1_tc; g1.tiles = s.tiles; g1.ntiles = s.ntiles;
-      g1.e.mode = EPI_GENERIC; g1.e.alpha = 1.0f / sqrtf((float)f.kernel); g1.e.act = ACT_GELU;
-      g1.e.oh = fh; g1.e.ol = fl; g1.e.ldh = 4 * H;
-      RUN(conv_gemm_tc(c, g1));
-      GemmTC g2;
-      g2.A_hi = fh; g2.A_lo = fl; g2.rows_total = s.rows; g2.w = &L.ffn2_tc; g2.tiles = s.tiles; g2.ntiles = s.ntiles;
-      g2.e.mode = EPI_GENERIC; g2.e.res = x; g2.e.ld_res = H; g2.e.rowmask = keep; g2.e.out = x; g2.e.ldo = H;
-      RUN(conv_gemm_tc(c, g2));
-      continue;
+    if (tc) RUN(split_planes(c, h, H, s.rows, H, 1.0f, hh, hl));
+    {  // TransformerFFNLayer (transformer.py): ffn_2(gelu(ffn_1(x) * k^-0.5)); on tensor cores gelu(ffn_1) exists only as planes
+      Epi e;
+      e.alpha = 1.0f / sqrtf((float)f.kernel); e.act = ACT_GELU;
+      if (tc) { e.out2_h = fh; e.out2_l = fl; e.ldh = 4 * H; }
+      else { e.out = ff; e.ldo = 4 * H; }
+      RUN(run_dense(c, L.ffn1, tc, s, {h, H, hh, hl}, e));
     }
-    {
-      ConvGemm g = make_gemm(L.ffn1, s, h, H);
-      g.e.alpha = 1.0f / sqrtf((float)f.kernel); g.e.act = ACT_GELU; g.e.out = ff; g.e.ldo = 4 * H;
-      RUN(conv_gemm(c, g));
-    }
-    {
-      ConvGemm g = make_gemm(L.ffn2, s, ff, 4 * H);
-      g.e.res = x; g.e.ld_res = H; g.e.rowmask = keep; g.e.out = x; g.e.ldo = H;
-      RUN(conv_gemm(c, g));
-    }
+    RUN(run_dense(c, L.ffn2, tc, s, {ff, 4 * H, fh, fl}, eres));
   }
   // final LN * mask, in place via h
   RUN(layernorm_rows(c, s, x, H, h, H, H, f.ln_g, f.ln_b, 1e-5f, keep));
@@ -252,7 +253,7 @@ int run_pitch_predictor(Ctx& c, const Model& m, int which, const SeqDev& s, cons
   SSB_CHECK(m.f0_gen == SSB_F0_GEN_CONV, "pitch predictor: the model was not created with SSB_F0_GEN_CONV");
   SSB_CHECK(which == 0 || which == 1, "pitch predictor: which must be 0 (pitch_predictor) or 1 (pitch_inpainter_predictor)");
   const PitchPredictor& p = m.pp[which];
-  for (int i = 0; i < PitchPredictor::kLayers; ++i) tc = tc && p.conv_tc[i].ok;
+  tc = tc && p.tc_ok;
   const size_t mk = c.mark();
   float* xs = alloc_rows(c, s, H);
   float* a = alloc_rows(c, s, H);
@@ -273,17 +274,10 @@ int run_pitch_predictor(Ctx& c, const Model& m, int which, const SeqDev& s, cons
   const float* cur = xs;
   for (int i = 0; i < PitchPredictor::kLayers; ++i) {
     // ConstantPad1d + Conv1d + ReLU (the guard rows are the zero pad), then LayerNorm(dim=1); Dropout is off
-    if (tc) {
-      RUN(split_planes(c, cur, H, s.rows, H, 1.0f, hh, hl));
-      GemmTC g;
-      g.A_hi = hh; g.A_lo = hl; g.rows_total = s.rows; g.w = &p.conv_tc[i]; g.tiles = s.tiles; g.ntiles = s.ntiles;
-      g.e.mode = EPI_GENERIC; g.e.act = ACT_RELU; g.e.out = a; g.e.ldo = H;
-      RUN(conv_gemm_tc(c, g));
-    } else {
-      ConvGemm g = make_gemm(p.conv[i], s, cur, H);
-      g.e.act = ACT_RELU; g.e.out = a; g.e.ldo = H;
-      RUN(conv_gemm(c, g));
-    }
+    if (tc) RUN(split_planes(c, cur, H, s.rows, H, 1.0f, hh, hl));
+    Epi e;
+    e.act = ACT_RELU; e.out = a; e.ldo = H;
+    RUN(run_dense(c, p.conv[i], tc, s, {cur, H, hh, hl}, e));
     RUN(layernorm_rows(c, s, a, H, b, H, H, p.ln_g[i], p.ln_b[i], 1e-5f, nullptr));
     cur = b;  // the next conv reads b and writes a; the LN after it overwrites b only once that conv has finished
   }
@@ -322,9 +316,7 @@ int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const 
   float* tmp = alloc_rows(c, sf, H);
   // long batches: the aligner's five projections per layer on the tensor-core kernel (the 256 -> 2048 -> 256 feed-forward is
   // 90 % of its FLOPs; its hidden activation then only exists as fp16 hi/lo planes); attention itself stays fp32
-  bool tc = m.use_tc && m.fft_tc && tc_available() && sf.ntiles >= 8;
-  for (int i = 0; i < 2; ++i)
-    tc = tc && m.align[i].q_tc.ok && m.align[i].kv_tc.ok && m.align[i].out_tc.ok && m.align[i].lin1_tc.ok && m.align[i].lin2_tc.ok;
+  const bool tc = long_batch_tc(m, sf) && m.align_tc_ok;
   float* hid = tc ? nullptr : alloc_rows(c, sf, 2048);
   WS_OK(c);
   // LocalStyleAdaptor.forward (lse.py:103-129)
@@ -409,35 +401,20 @@ int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const 
     avth = c.alloc<__half>((size_t)ldvt * H); avtl = c.alloc<__half>((size_t)ldvt * H);
     WS_OK(c);
   }
-  auto tcg = [&](const SeqDev& sq, const __half* ah, const __half* al, const ConvTC& w) {
-    GemmTC g;
-    g.A_hi = ah; g.A_lo = al; g.rows_total = sq.rows; g.w = &w; g.tiles = sq.tiles; g.ntiles = sq.ntiles;
-    g.e.mode = EPI_GENERIC;
-    return g;
-  };
   for (int i = 0; i < 2; ++i) {
     const AlignLayer& L = m.align[i];
-    if (tc) {
-      RUN(split_planes(c, style, H, sf.rows, H, 1.0f, sth, stl));
-      GemmTC gq = tcg(sf, sth, stl, L.q_tc);
-      if (atc) { gq.e.oh = aqh; gq.e.ol = aql; gq.e.ldh = H; }
-      else { gq.e.out = q; gq.e.ldo = H; }
-      RUN(conv_gemm_tc(c, gq));
-      GemmTC gk = tcg(sr, zlh, zll, L.kv_tc);
-      if (atc) { gk.e.oh = akh; gk.e.ol = akl; gk.e.ldh = 2 * H; }
-      else { gk.e.out = kv; gk.e.ldo = 2 * H; }
-      RUN(conv_gemm_tc(c, gk));
-    } else {
-      {
-        ConvGemm g = make_gemm(L.q, sf, style, H);
-        g.e.out = q; g.e.ldo = H;
-        RUN(conv_gemm(c, g));
-      }
-      {
-        ConvGemm g = make_gemm(L.kv, sr, zl, H);
-        g.e.out = kv; g.e.ldo = 2 * H;
-        RUN(conv_gemm(c, g));
-      }
+    if (tc) RUN(split_planes(c, style, H, sf.rows, H, 1.0f, sth, stl));
+    {
+      Epi e;
+      if (atc) { e.out2_h = aqh; e.out2_l = aql; e.ldh = H; }
+      else { e.out = q; e.ldo = H; }
+      RUN(run_dense(c, L.q, tc, sf, {style, H, sth, stl}, e));
+    }
+    {
+      Epi e;
+      if (atc) { e.out2_h = akh; e.out2_l = akl; e.ldh = 2 * H; }
+      else { e.out = kv; e.ldo = 2 * H; }
+      RUN(run_dense(c, L.kv, tc, sr, {zl, H, zlh, zll}, e));
     }
     if (atc) {  // cross-attention on the tensor-core kernel: q planes [F rows, 256], k | v planes [R rows, 512]
       RUN(transpose_planes(c, akh, akl, 2 * H, H, sr.rows, H, avth, avtl, ldvt));
@@ -456,37 +433,20 @@ int run_style(Ctx& c, const Model& m, const SeqDev& sf, const SeqDev& sr, const 
       a.keymask = kmask; a.scale = 0.08838834764831845f; a.out = att; a.ldo = H;
       RUN(attention(c, a));
     }
-    if (tc) {
-      if (!atc) RUN(split_planes(c, att, H, sf.rows, H, 1.0f, sth, stl));
-      GemmTC g = tcg(sf, sth, stl, L.out_tc);
-      g.e.res = style; g.e.ld_res = H; g.e.out = tmp; g.e.ldo = H;
-      RUN(conv_gemm_tc(c, g));
-    } else {
-      ConvGemm g = make_gemm(L.out, sf, att, H);
-      g.e.res = style; g.e.ld_res = H; g.e.out = tmp; g.e.ldo = H;
-      RUN(conv_gemm(c, g));
-    }
+    if (tc && !atc) RUN(split_planes(c, att, H, sf.rows, H, 1.0f, sth, stl));
+    Epi eres;  // tmp = style + layer output: the epilogue of the out-projection and of linear2
+    eres.res = style; eres.ld_res = H; eres.out = tmp; eres.ldo = H;
+    RUN(run_dense(c, L.out, tc, sf, {att, H, sth, stl}, eres));
     RUN(layernorm_rows(c, sf, tmp, H, style, H, H, L.n1_g, L.n1_b, 1e-5f, nullptr));
-    if (tc) {
-      RUN(split_planes(c, style, H, sf.rows, H, 1.0f, sth, stl));
-      GemmTC g1 = tcg(sf, sth, stl, L.lin1_tc);
-      g1.e.act = ACT_RELU; g1.e.oh = hdh; g1.e.ol = hdl; g1.e.ldh = 2048;
-      RUN(conv_gemm_tc(c, g1));
-      GemmTC g2 = tcg(sf, hdh, hdl, L.lin2_tc);
-      g2.e.res = style; g2.e.ld_res = H; g2.e.out = tmp; g2.e.ldo = H;
-      RUN(conv_gemm_tc(c, g2));
-    } else {
-      {
-        ConvGemm g = make_gemm(L.lin1, sf, style, H);
-        g.e.act = ACT_RELU; g.e.out = hid; g.e.ldo = 2048;
-        RUN(conv_gemm(c, g));
-      }
-      {
-        ConvGemm g = make_gemm(L.lin2, sf, hid, 2048);
-        g.e.res = style; g.e.ld_res = H; g.e.out = tmp; g.e.ldo = H;
-        RUN(conv_gemm(c, g));
-      }
+    if (tc) RUN(split_planes(c, style, H, sf.rows, H, 1.0f, sth, stl));
+    {
+      Epi e;
+      e.act = ACT_RELU;
+      if (tc) { e.out2_h = hdh; e.out2_l = hdl; e.ldh = 2048; }
+      else { e.out = hid; e.ldo = 2048; }
+      RUN(run_dense(c, L.lin1, tc, sf, {style, H, sth, stl}, e));
     }
+    RUN(run_dense(c, L.lin2, tc, sf, {hid, 2048, hdh, hdl}, eres));
     RUN(layernorm_rows(c, sf, tmp, H, style, H, H, L.n2_g, L.n2_b, 1e-5f, nullptr));
   }
   c.release(mk);
@@ -503,16 +463,14 @@ static int denoiser_heads(Ctx& c, const Denoiser& d, const SeqDev& s, DenoiserBu
   const int C = d.C, L = d.L;
   if (b.tc_heads) {
     {  // skip_projection (1/sqrt(L) folded into the packed weights) + ReLU -> planes
-      GemmTC g;
-      g.A_hi = b.skh; g.A_lo = b.skl; g.rows_total = s.rows; g.w = &d.skip_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-      g.e.mode = EPI_GENERIC; g.e.bias = d.skip_bias_pad; g.e.act = ACT_RELU; g.e.oh = b.sh; g.e.ol = b.sl; g.e.ldh = C;
+      GemmTC g = make_gemm_tc(d.skip_tc, s, b.skh, b.skl);
+      g.e.bias = d.skip_bias_pad; g.e.act = ACT_RELU; g.e.oh = b.sh; g.e.ol = b.sl; g.e.ldh = C;
       g.e.n_valid = C;
       RUN(conv_gemm_tc(c, g));
     }
     {  // output_projection (N padded to a tile multiple; only the first out_dims columns are meaningful)
-      GemmTC g;
-      g.A_hi = b.sh; g.A_lo = b.sl; g.rows_total = s.rows; g.w = &d.out_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-      g.e.mode = EPI_GENERIC; g.e.bias = d.out_bias_pad; g.e.out = b.head; g.e.ldo = b.ld_head;
+      GemmTC g = make_gemm_tc(d.out_tc, s, b.sh, b.sl);
+      g.e.bias = d.out_bias_pad; g.e.out = b.head; g.e.ldo = b.ld_head;
       g.e.n_valid = (d.out_dims + 31) / 32 * 32;
       RUN(conv_gemm_tc(c, g));
     }
@@ -539,16 +497,14 @@ int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBu
   for (int l = 0; l < L; ++l) {  // residual layer l (net.py:66-78)
     if (b.tc) {
       {
-        GemmTC g;
-        g.A_hi = b.yh; g.A_lo = b.yl; g.rows_total = s.rows; g.w = &d.layers[l].dil_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
+        GemmTC g = make_gemm_tc(d.layers[l].dil.t, s, b.yh, b.yl);
         // K = 3*C (taps of y); the hoisted conditioner projection arrives as an epilogue addend (one [rows, 2C] matrix per layer)
         g.e.add = b.condpre + (size_t)l * (size_t)s.rows * 2 * C; g.e.ld_add = 2 * C;
         g.e.mode = EPI_GATE; g.e.bias = d.layers[l].bias_gate_tc;
         g.e.oh = b.zh; g.e.ol = b.zl; g.e.ldh = C;
         RUN(conv_gemm_tc(c, g));
       }
-      GemmTC g;
-      g.A_hi = b.zh; g.A_lo = b.zl; g.rows_total = s.rows; g.w = &d.layers[l].outp_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
+      GemmTC g = make_gemm_tc(d.layers[l].outp.t, s, b.zh, b.zl);
       // residual stream carried ONLY as the fp16 hi/lo planes of y = x + step bias (in place: this epilogue reads
       // y_l[row] and writes y_{l+1}[row] for the same rows/columns): no fp32 x is read or written in the T x L loop
       g.e.mode = EPI_RES_SKIP; g.e.C = C; g.e.beta = 0.70710678118654752440f;
@@ -561,12 +517,12 @@ int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBu
       continue;
     }
     {
-      ConvGemm g = make_gemm(d.layers[l].dil, s, b.y, C);
+      ConvGemm g = make_gemm(d.layers[l].dil.f, s, b.y, C);
       g.e.mode = EPI_GATE; g.e.add = b.condall + (size_t)l * 2 * C; g.e.ld_add = L * 2 * C; g.e.out = b.zg; g.e.ldo = C;
       RUN(conv_gemm(c, g));
     }
     {
-      ConvGemm g = make_gemm(d.layers[l].outp, s, b.zg, C);
+      ConvGemm g = make_gemm(d.layers[l].outp.f, s, b.zg, C);
       g.e.mode = EPI_RES_SKIP; g.e.C = C; g.e.res = b.x; g.e.ld_res = C; g.e.beta = 0.70710678118654752440f;
       g.e.out = b.x; g.e.ldo = C;
       if (l + 1 < L) { g.e.out2 = b.y; g.e.ldo2 = C; g.e.vec2 = dt + (size_t)(l + 1) * C; }
@@ -577,17 +533,7 @@ int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBu
   return denoiser_heads(c, d, s, b);
 }
 
-static __half* alloc_half_rows(Ctx& c, const SeqDev& s, int C) {
-  __half* p = c.alloc<__half>((size_t)s.rows * C);
-  if (!c.dry && p && !c.failed) cudaMemsetAsync(p, 0, (size_t)s.rows * C * sizeof(__half), c.stream);
-  return p;
-}
-bool denoiser_tc_ok(const Model& m, const Denoiser& d) {
-  if (!m.use_tc || !d.cond_all_tc.ok) return false;
-  for (auto& l : d.layers)
-    if (!l.dil_tc.ok || !l.outp_tc.ok) return false;
-  return true;
-}
+bool denoiser_tc_ok(const Model& m, const Denoiser& d) { return m.use_tc && d.tc_ok; }
 int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, DenoiserBufs* b) {
   b->tc = tc;
   b->condpre = nullptr;
@@ -641,9 +587,8 @@ int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, Denoiser
 static int hoist_cond_tc(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, __half* ch, __half* cl,
                          float* condpre) {
   RUN(split_planes(c, cond_g, 256, s.rows, 256, 1.0f, ch, cl));
-  GemmTC g;
-  g.A_hi = ch; g.A_lo = cl; g.rows_total = s.rows; g.w = &d.cond_all_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-  g.e.mode = EPI_GENERIC; g.e.out = condpre; g.e.ldo = d.L * 2 * d.C;
+  GemmTC g = make_gemm_tc(d.cond_all_tc, s, ch, cl);
+  g.e.out = condpre; g.e.ldo = d.L * 2 * d.C;
   g.e.out_nb = 2 * d.C; g.e.out_bs = (int64_t)s.rows * 2 * d.C;
   return conv_gemm_tc(c, g);
 }
@@ -660,9 +605,8 @@ int prepare_cond(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g
 int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const float* x80, DenoiserBufs& b) {
   if (b.x80h) {  // tensor-core input projection: K padded 80 -> 128
     RUN(x80_planes(c, x80, s.rows, b.x80h, b.x80l));
-    GemmTC g;
-    g.A_hi = b.x80h; g.A_lo = b.x80l; g.rows_total = s.rows; g.w = &d.in_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-    g.e.mode = EPI_GENERIC; g.e.bias = d.in_proj.bias; g.e.act = ACT_RELU;  // planes of y = relu(in_proj) + step bias only
+    GemmTC g = make_gemm_tc(d.in_tc, s, b.x80h, b.x80l);
+    g.e.bias = d.in_proj.bias; g.e.act = ACT_RELU;  // planes of y = relu(in_proj) + step bias only
     g.e.oh = b.yh; g.e.ol = b.yl; g.e.ldh = d.C; g.e.vec2 = d.dtab + (size_t)t * d.L * d.C;
     RUN(conv_gemm_tc(c, g));
     return denoiser_stack(c, d, s, t, b);
@@ -707,9 +651,9 @@ struct PersistentNet {
   __half* pl[NPL] = {};      // [rows, C] each
   float* condpre = nullptr;  // hoisted conditioner projection (hoist_cond_tc)
   int mb = 0;                // index of the net's first tensor map
-  // the net's maps from mb: its NPL activation planes, then (hi, lo) weights of dil_tc and outp_tc per layer, skip, out
+  // the net's maps from mb: its NPL activation planes, then (hi, lo) weights of dil.t and outp.t per layer, skip, out
   static int nmaps(int L) { return NPL + 4 * L + 4; }
-  int w_layer(int l) const { return mb + NPL + 4 * l; }  // dil_tc; outp_tc at + 2
+  int w_layer(int l) const { return mb + NPL + 4 * l; }  // dil.t; outp.t at + 2
   int w_skip() const { return mb + NPL + 4 * d->L; }
   int w_out() const { return w_skip() + 2; }
 };
@@ -737,8 +681,8 @@ static int persistent_net_maps(const PersistentNet& p, const SeqDev& s, int cs, 
     if (make_act_map(&maps[p.mb + i], p.pl[i], s.rows, d.C, 128 / cs)) return -1;
   auto put = [&](int idx, const ConvTC& w) { maps[idx] = w.tm_hi[1]; maps[idx + 1] = w.tm_lo[1]; };
   for (int l = 0; l < d.L; ++l) {
-    put(p.w_layer(l), d.layers[l].dil_tc);
-    put(p.w_layer(l) + 2, d.layers[l].outp_tc);
+    put(p.w_layer(l), d.layers[l].dil.t);
+    put(p.w_layer(l) + 2, d.layers[l].outp.t);
   }
   put(p.w_skip(), d.skip_tc);
   put(p.w_out(), d.out_tc);
@@ -762,13 +706,13 @@ static void persistent_net_step(const PersistentNet& p, const SeqDev& s, int t, 
   for (int l = 0; l < L; ++l) {
     SPhase a = sphase(sync_after);  // dilated conv (3 taps of y) + hoisted conditioner projection -> gate -> z planes
     a.a1 = p.mb + P::Y; a.w1 = p.w_layer(l); a.taps = 3; a.kchunks = C / 64;
-    a.dil = d.layers[l].dil_tc.dil; a.center = 1; a.N = 2 * C; a.NT = 2 * C / 64; a.mode = SP_GATE;
+    a.dil = d.layers[l].dil.t.dil; a.center = 1; a.N = 2 * C; a.NT = 2 * C / 64; a.mode = SP_GATE;
     a.bias = d.layers[l].bias_gate_tc; a.oh = p.pl[P::Z]; a.ol = p.pl[P::Z + 1]; a.ldh = C;
     a.add = p.condpre + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C;
     ph.push_back(a);
     SPhase b = sphase(sync_after);  // 1x1 output projection -> residual stream, next layer's input planes, skip sum
     b.a1 = p.mb + P::Z; b.w1 = p.w_layer(l) + 2; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
-    b.bias = d.layers[l].outp.bias; b.res = p.x; b.ld_res = C; b.out = p.x; b.ldo = C; b.beta = 0.70710678118654752440f;
+    b.bias = d.layers[l].outp.f.bias; b.res = p.x; b.ld_res = C; b.out = p.x; b.ldo = C; b.beta = 0.70710678118654752440f;
     if (l + 1 < L) { b.oh = p.pl[P::Y]; b.ol = p.pl[P::Y + 1]; b.ldh = C; b.vec2 = dt + (size_t)(l + 1) * C; }
     b.skip = p.skip; b.ld_skip = C; b.C = C; b.skip_init = (l == 0);
     if (l == L - 1) { b.sh = p.pl[P::SKIP]; b.sl = p.pl[P::SKIP + 1]; }
@@ -1127,7 +1071,7 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
   int C = v.cfg.initial_channel;
   float* x = alloc_rows(c, s1, C);
   __half *pin_h = nullptr, *pin_l = nullptr;  // planes of leaky_relu(stage input), when the next ups runs on tensor cores
-  const bool up0_tc = tc && !v.stages.empty() && v.stages[0].up_tc.ok;
+  const bool up0_tc = tc && !v.stages.empty() && v.stages[0].up.t.ok;
   if (up0_tc) {
     pin_h = alloc_half_rows(c, s1, C);
     pin_l = alloc_half_rows(c, s1, C);
@@ -1148,7 +1092,7 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
     const int rate_out = rate * st.u;
     SeqDev so;
     RUN(upload_layout(c, seq, rate_out, &so));
-    const bool up_tc = tc && st.up_tc.ok && pin_h != nullptr;
+    const bool up_tc = tc && st.up.t.ok && pin_h != nullptr;
     const bool paired = tc && st.paired && (rate_out % 2 == 0);
     const bool res_tc = tc && (st.res_tc || paired);
     // paired stage: [rows, 32] is processed as [rows/2, 64] (same memory) with the time-paired weight packing
@@ -1158,7 +1102,7 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
       RUN(upload_layout(c, seq, rate_out / 2, &sw));
       sw.rows = so.rows / 2;  // exactly the memory of the [so.rows, Co] buffers (TMA zero-fills beyond)
     }
-    const bool next_up_tc = tc && i + 1 < v.stages.size() && v.stages[i + 1].up_tc.ok;
+    const bool next_up_tc = tc && i + 1 < v.stages.size() && v.stages[i + 1].up.t.ok;
     float* xu = alloc_rows(c, so, Co);
     float* r = alloc_rows(c, so, Co);
     float* acc = alloc_rows(c, so, Co);
@@ -1174,19 +1118,15 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
     }
     if (next_up_tc) { pa_h = alloc_half_rows(c, so, Co); pa_l = alloc_half_rows(c, so, Co); }
     WS_OK(c);
-    // x = ups[i](leaky_relu(x, 0.1))
-    if (up_tc) {
-      GemmTC g;
-      g.A_hi = pin_h; g.A_lo = pin_l; g.rows_total = sin.rows; g.w = &st.up_tc; g.tiles = sin.tiles; g.ntiles = sin.ntiles;
-      g.e.mode = EPI_GENERIC; g.e.out = xu; g.e.ldo = st.u * Co;
-      if (res_tc && !nsf) { g.e.oh = px_h; g.e.ol = px_l; g.e.ldh = st.u * Co; g.e.plane_act = ACT_LRELU; g.e.plane_slope = 0.1f; }
-      RUN(conv_gemm_tc(c, g));
-    } else {
-      ConvGemm g = make_gemm(st.up, sin, xin, C);
-      g.a_act = ACT_LRELU; g.a_slope = 0.1f;
-      g.e.out = xu; g.e.ldo = st.u * Co;
-      if (res_tc && !nsf) { g.e.out2_h = px_h; g.e.out2_l = px_l; g.e.ldh = st.u * Co; g.e.plane_act = ACT_LRELU; g.e.plane_slope = 0.1f; }
-      RUN(conv_gemm(c, g));
+    // fp16 planes of leaky_relu(v, 0.1), the pre-activation of the conv that consumes them, beside an epilogue's output
+    auto lrelu_planes = [](Epi& e, __half* hi, __half* lo, int ld) {
+      e.out2_h = hi; e.out2_l = lo; e.ldh = ld; e.plane_act = ACT_LRELU; e.plane_slope = 0.1f;
+    };
+    {  // x = ups[i](leaky_relu(x, 0.1))
+      Epi e;
+      e.out = xu; e.ldo = st.u * Co;
+      if (res_tc && !nsf) lrelu_planes(e, px_h, px_l, st.u * Co);
+      RUN(run_dense(c, st.up, up_tc, sin, {xin, C, pin_h, pin_l, ACT_LRELU, 0.1f}, e));
     }
     if (nsf) RUN(noise_conv_add(c, so, s256, xu, Co, Co, har, st.nc_w, st.nc_b, st.nc_s, res_tc ? px_h : nullptr, px_l, 0.1f, st.nc_wt));
     for (int j = 0; j < v.nk; ++j) {  // MRF: mean of the resblocks
@@ -1195,45 +1135,23 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
       for (int mI = 0; mI < 3; ++mI) {
         const bool last = (mI == 2);
         const bool lastj = (j == v.nk - 1);
-        if (res_tc) {
-          {
-            GemmTC g;  // xt = c1(leaky_relu(r)) ; only leaky_relu(xt) is ever consumed -> planes only
-            g.A_hi = rin_h; g.A_lo = rin_l; g.rows_total = sw.rows; g.w = &st.rb[j].c1_tc[mI]; g.tiles = sw.tiles; g.ntiles = sw.ntiles;
-            g.e.mode = EPI_GENERIC; g.e.oh = pt_h; g.e.ol = pt_l; g.e.ldh = Cw; g.e.plane_act = ACT_LRELU; g.e.plane_slope = 0.1f;
-            RUN(conv_gemm_tc(c, g));
-          }
-          GemmTC g;  // r = c2(leaky_relu(xt)) + r
-          g.A_hi = pt_h; g.A_lo = pt_l; g.rows_total = sw.rows; g.w = &st.rb[j].c2_tc[mI]; g.tiles = sw.tiles; g.ntiles = sw.ntiles;
-          g.e.mode = EPI_GENERIC; g.e.res = rin; g.e.ld_res = Cw;
-          if (!last) {
-            g.e.out = r; g.e.ldo = Cw; g.e.oh = pr_h; g.e.ol = pr_l; g.e.ldh = Cw; g.e.plane_act = ACT_LRELU; g.e.plane_slope = 0.1f;
-          } else {
-            g.e.out = acc; g.e.ldo = Cw; g.e.accum = (j > 0); g.e.gamma = lastj ? 1.0f / (float)v.nk : 1.0f;
-            if (lastj && next_up_tc) { g.e.oh = pa_h; g.e.ol = pa_l; g.e.ldh = Cw; g.e.plane_act = ACT_LRELU; g.e.plane_slope = 0.1f; }
-          }
-          RUN(conv_gemm_tc(c, g));
-          rin = r; rin_h = pr_h; rin_l = pr_l;
-          continue;
+        {  // xt = c1(leaky_relu(r)) ; on tensor cores only leaky_relu(xt) is ever consumed -> planes only
+          Epi e;
+          if (res_tc) lrelu_planes(e, pt_h, pt_l, Cw);
+          else { e.out = xt; e.ldo = Cw; }
+          RUN(run_dense(c, st.rb[j].c1[mI], res_tc, sw, {rin, Cw, rin_h, rin_l, ACT_LRELU, 0.1f}, e));
         }
-        {
-          ConvGemm g = make_gemm(st.rb[j].c1[mI], so, rin, Co);
-          g.a_act = ACT_LRELU; g.a_slope = 0.1f;
-          g.e.out = xt; g.e.ldo = Co;
-          RUN(conv_gemm(c, g));
-        }
-        ConvGemm g = make_gemm(st.rb[j].c2[mI], so, xt, Co);
-        g.a_act = ACT_LRELU; g.a_slope = 0.1f;
-        g.e.res = rin; g.e.ld_res = Co;
+        Epi e;  // r = c2(leaky_relu(xt)) + r
+        e.res = rin; e.ld_res = Cw;
         if (!last) {
-          g.e.out = r; g.e.ldo = Co;
+          e.out = r; e.ldo = Cw;
+          if (res_tc) lrelu_planes(e, pr_h, pr_l, Cw);
         } else {
-          g.e.out = acc; g.e.ldo = Co;
-          g.e.accum = (j > 0);
-          g.e.gamma = lastj ? 1.0f / (float)v.nk : 1.0f;
-          if (lastj && next_up_tc) { g.e.out2_h = pa_h; g.e.out2_l = pa_l; g.e.ldh = Co; g.e.plane_act = ACT_LRELU; g.e.plane_slope = 0.1f; }
+          e.out = acc; e.ldo = Cw; e.accum = (j > 0); e.gamma = lastj ? 1.0f / (float)v.nk : 1.0f;
+          if (lastj && next_up_tc) lrelu_planes(e, pa_h, pa_l, Cw);
         }
-        RUN(conv_gemm(c, g));
-        rin = r;
+        RUN(run_dense(c, st.rb[j].c2[mI], res_tc, sw, {xt, Cw, pt_h, pt_l, ACT_LRELU, 0.1f}, e));
+        rin = r; rin_h = pr_h; rin_l = pr_l;
       }
     }
     xin = acc; sin = so; C = Co; rate = rate_out;

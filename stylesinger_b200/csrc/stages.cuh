@@ -3,6 +3,33 @@
 
 namespace ssb {
 
+#define RUN(x)                 \
+  do {                         \
+    int rc_ = (x);             \
+    if (rc_ != 0) return rc_;  \
+  } while (0)
+#define WS_OK(c) SSB_CHECK((c).dry || !(c).failed, "workspace too small")
+
+// zero-filled guard-banded rows of other element types (alloc_rows: common.cuh)
+int32_t* alloc_rows_i32(Ctx& c, const SeqDev& s, int C = 1);
+__half* alloc_half_rows(Ctx& c, const SeqDev& s, int C);
+
+// Long batches (>= 8 row tiles) run the FFT decoder, the aligner and the pitch predictors on the tensor-core kernel
+bool long_batch_tc(const Model& m, const SeqDev& s);
+
+// The input act(x) of a dense layer: fp32 rows x (the FFMA kernel applies act on load) and / or fp16 hi/lo planes that
+// already hold act(x) (written by the producing epilogue or by split_planes).  A path reads the form it needs.
+struct DenseIn {
+  const float* x = nullptr;
+  int ld = 0;
+  const __half *hi = nullptr, *lo = nullptr;
+  int act = ACT_NONE;  // ACT_NONE or ACT_LRELU
+  float slope = 0.1f;
+};
+// Enqueues the layer over the rows of `s` on the tensor-core (tc) or the fp32 FFMA kernel.  `e` describes the epilogue
+// for both (bias: the layer's own); a field the chosen kernel cannot honour is an error.
+int run_dense(Ctx& c, const Dense& d, bool tc, const SeqDev& s, const DenseIn& in, const Epi& e);
+
 int fft_blocks(Ctx& c, const FFT& f, const SeqDev& s, float* x, const float* keep, bool tc = false);
 int run_encoder(Ctx& c, const Model& m, const SeqDev& sp, const int32_t* tok_g, const int32_t* note_g,
                 const int32_t* type_g, const float* ndur_g, float* srcmask, float* enc_out);

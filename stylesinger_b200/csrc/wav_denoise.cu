@@ -37,13 +37,6 @@ struct ssb_wav_denoise {
 
 namespace ssb {
 
-#define RUN(x)                 \
-  do {                         \
-    int rc_ = (x);             \
-    if (rc_ != 0) return rc_;  \
-  } while (0)
-#define WS_OK(c) SSB_CHECK((c).dry || !(c).failed, "workspace too small")
-
 namespace {
 
 // S * max(0, 1 - v / |S|) for the bins < nbins of every frame row; the output's padding bins and guard rows stay zero
@@ -118,7 +111,7 @@ int run_denoise(Ctx& c, const ssb_wav_denoise& d, const Seq& q, const float* wav
   SeqDev s;
   RUN(upload_layout(c, q, 1, &s));
   const int N2 = 2 * d.nbp;
-  const bool tc = d.tc_mode == 2 || (d.tc_mode == 1 && s.ntiles >= 8);  // the FFT decoder's / pitch predictor's rule (stages.cu)
+  const bool tc = d.tc_mode == 2 || (d.tc_mode == 1 && s.ntiles >= 8);  // long_batch_tc's threshold (stages.cu)
   int32_t* offs_dev = c.alloc<int32_t>((size_t)B + 1);
   float* rows = alloc_rows(c, s, d.hop);  // zero-filled incl. guards = the constant centre padding
   float* spec = alloc_rows(c, s, N2, false);
@@ -143,9 +136,8 @@ int run_denoise(Ctx& c, const ssb_wav_denoise& d, const Seq& q, const float* wav
   RUN(wav_rows(c, s, offs_dev, wav, d.hop, rows));
   if (tc) {
     RUN(split_planes(c, rows, d.hop, s.rows, d.hop, 1.0f, wh, wl));
-    GemmTC g;
-    g.A_hi = wh; g.A_lo = wl; g.rows_total = s.rows; g.w = &d.fwd_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-    g.e.mode = EPI_GENERIC; g.e.out = spec; g.e.ldo = N2;
+    GemmTC g = make_gemm_tc(d.fwd_tc, s, wh, wl);
+    g.e.out = spec; g.e.ldo = N2;
     RUN(conv_gemm_tc(c, g));
   } else {
     ConvGemm g = make_gemm(d.fwd, s, rows, d.hop);
@@ -163,9 +155,8 @@ int run_denoise(Ctx& c, const ssb_wav_denoise& d, const Seq& q, const float* wav
   // epilogue's alpha
   const float inv_n = 1.0f / (float)d.n_fft;
   if (tc) {
-    GemmTC g;
-    g.A_hi = sh; g.A_lo = sl; g.rows_total = s.rows; g.w = &d.inv_tc; g.tiles = s.tiles; g.ntiles = s.ntiles;
-    g.e.mode = EPI_GENERIC; g.e.alpha = inv_n; g.e.out = y; g.e.ldo = d.hop;
+    GemmTC g = make_gemm_tc(d.inv_tc, s, sh, sl);
+    g.e.alpha = inv_n; g.e.out = y; g.e.ldo = d.hop;
     RUN(conv_gemm_tc(c, g));
   } else {
     ConvGemm g = make_gemm(d.inv, s, sub, N2);

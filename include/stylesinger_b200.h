@@ -119,6 +119,15 @@ int ssb_model_create_ex2(ssb_model_t** out, const ssb_tensor_desc* tensors, int3
 int ssb_model_set_schedule(ssb_model_t* m, int32_t which, int32_t T, const float* step_emb, const float* gauss_tab,
                            const float* multi_tab, void* stream);
 
+/* hparams['K_step'] of the DiffSinger mel sampler (shallow diffusion; GaussianDiffusion.__init__ and
+ * DiffusionDecoder.forward, modules/diff/shallow_diffusion_tts.py:92,297-304): x_K = q_sample(norm_spec(coarse), K-1) on
+ * the T-step schedule, then K reverse steps t = K-1 .. 0 (the PLMS sampler: t0 = the largest multiple of the interval
+ * below K).  K = 0 (the default) follows the schedule's T.  Every mel-sampler entry (ssb_acoustic_forward,
+ * ssb_mel_diffusion_sample, ssb_mel_diffusion_sample_plms and their *_workspace_bytes) then uses K_eff = K ? K : T and
+ * fails if K_eff > T.  K < 0, and any K on a PRODIFF model (ProDiffusion.forward never reads K_step), are errors.
+ * Philox mode: step t draws the same stream at every K. */
+int ssb_model_set_mel_k_step(ssb_model_t* m, int32_t K);
+
 /* Inputs of StyleSinger.forward(..., infer=True) (modules/StyleSinger/stylesinger.py:119-187). */
 typedef struct {
   int32_t B;
@@ -139,12 +148,13 @@ typedef struct {
   const float* uv;              /* dev [sumF] optional teacher-forced uv */
   const float* f0_gauss_noise[2]; /* dev [(T_f0+1), sumF]: z init then one per step t=T-1..0; NULL -> Philox */
   const float* f0_unif_noise[2];  /* dev [T_f0, sumF, 2] */
-  const float* mel_noise;         /* dev [(T+1), sumF, 80]: q_sample then one per step */
+  const float* mel_noise;         /* dev [(K+1), sumF, 80]: the q_sample draw, then one per step t = K-1 .. 0
+                                   * (K = ssb_model_set_mel_k_step's K_eff; T on a PRODIFF model) */
   uint64_t seed;
   int32_t skip_mel_diffusion;     /* 1: stop after the coarse mel / diff_cond */
-  int32_t pndm_speedup;           /* 0: DDPM ancestral sampling, T steps (the StyleSinger default, DiffusionDecoder.forward);
-                                   * k > 0: PLMS with iteration interval k (hparams['pndm_speedup'],
-                                   * modules/diff/shallow_diffusion_tts.py:164-197,254-260): T / k (+1) denoiser evaluations */
+  int32_t pndm_speedup;           /* 0: DDPM ancestral sampling, K steps (the StyleSinger default, DiffusionDecoder.forward);
+                                   * k in [1, K): PLMS with iteration interval k (hparams['pndm_speedup'],
+                                   * modules/diff/shallow_diffusion_tts.py:164-197,254-260): K / k (+1) denoiser evaluations */
 } ssb_acoustic_inputs;
 
 /* Outputs (all optional except mel_out/f0_denorm when diffusion runs); device, tight packed. */
@@ -182,7 +192,8 @@ int ssb_acoustic_forward(const ssb_model_t* m, const ssb_acoustic_inputs* in, co
                          void* workspace, size_t workspace_bytes, void* stream);
 
 /* DiffusionDecoder.forward(infer=True) alone (modules/diff/shallow_diffusion_tts.py:284-307):
- * cond [sumF,256], coarse [sumF,80] -> mel [sumF,80].  DiffSinger models only (the PLMS entry point too). */
+ * cond [sumF,256], coarse [sumF,80] -> mel [sumF,80].  DiffSinger models only (the PLMS entry point too).
+ * noise [(K+1),sumF,80] = the q_sample draw, then one per step t = K-1 .. 0 (K: ssb_model_set_mel_k_step), or NULL (Philox). */
 size_t ssb_mel_diffusion_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B);
 int ssb_mel_diffusion_sample(const ssb_model_t* m, const float* cond, const float* coarse_mel,
                              const int32_t* frame_offsets, int32_t B, const float* noise, uint64_t seed,
@@ -190,7 +201,8 @@ int ssb_mel_diffusion_sample(const ssb_model_t* m, const float* cond, const floa
 
 /* PLMS / PNDM sampler over the same DiffNet (SURVEY.md section 8f, f2): GaussianDiffusion.p_sample_plms driven by the
  * `pndm_speedup` loop of GaussianDiffusion.forward (modules/diff/shallow_diffusion_tts.py:164-197,254-260).
- * interval = hparams['pndm_speedup']; q_noise [sumF,80] (tight) is the single q_sample draw, NULL = in-kernel Philox. */
+ * interval = hparams['pndm_speedup'], in [1, K) (K: ssb_model_set_mel_k_step); q_noise [sumF,80] (tight) is the single
+ * q_sample draw (at K-1), NULL = in-kernel Philox. */
 size_t ssb_mel_diffusion_plms_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B);
 int ssb_mel_diffusion_sample_plms(const ssb_model_t* m, const float* cond, const float* coarse_mel,
                                   const int32_t* frame_offsets, int32_t B, const float* q_noise, uint64_t seed,

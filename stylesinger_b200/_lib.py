@@ -67,6 +67,7 @@ EXPORTS = [
     "ssb_model_create_ex2", "ssb_pitch_predictor_workspace_bytes", "ssb_pitch_predictor",
     "ssb_wav_denoise_create", "ssb_wav_denoise_free", "ssb_wav_denoise_workspace_bytes", "ssb_wav_denoise_forward",
     "ssb_wav_denoise_set_tensor_cores",
+    "ssb_model_set_mel_k_step",
 ]
 
 
@@ -87,6 +88,7 @@ def _load():
         "ssb_pitch_predictor": (C.c_int, [vp, i32, vp, vp, i32, vp, vp, sz, vp]),
         "ssb_model_free": (None, [vp]),
         "ssb_model_set_schedule": (C.c_int, [vp, i32, i32, vp, vp, vp, vp]),
+        "ssb_model_set_mel_k_step": (C.c_int, [vp, i32]),
         "ssb_durations_workspace_bytes": (sz, [vp, P(AcousticInputs)]),
         "ssb_predict_durations": (C.c_int, [vp, P(AcousticInputs), vp, vp, vp, sz, vp]),
         "ssb_acoustic_workspace_bytes": (sz, [vp, P(AcousticInputs)]),

@@ -362,6 +362,15 @@ int ssb_model_set_schedule(ssb_model_t* m, int32_t which, int32_t T, const float
   return set_schedule(&m->m, which, T, step_emb, gauss_tab, multi_tab, (cudaStream_t)stream);
 }
 
+int ssb_model_set_mel_k_step(ssb_model_t* m, int32_t K) {
+  SSB_CHECK(m, "null model");
+  SSB_CHECK(K >= 0, "ssb_model_set_mel_k_step: K must be >= 0 (0 follows the schedule's T), got " + std::to_string(K));
+  SSB_CHECK(m->m.mel_decoder == SSB_MEL_DECODER_DIFFSINGER,
+            "ssb_model_set_mel_k_step: a ProDiff model has no K_step (ProDiffusion.forward never reads it)");
+  m->m.mel_k_step = K;
+  return 0;
+}
+
 size_t ssb_durations_workspace_bytes(const ssb_model_t* m, const ssb_acoustic_inputs* in) {
   Ctx c = make_ctx(nullptr, 0, nullptr, true);
   ssb_acoustic_outputs o;

@@ -146,6 +146,9 @@ struct Model {
   // SSB_MEL_DECODER_DIFFSINGER: hparams['decoder'] == 'diffsinger' (FFT decoder + mel_out + ln_proj + DDPM over postdiff.*);
   // SSB_MEL_DECODER_PRODIFF: 'prodiff' (decoder_inp straight into the x0-predicting sampler over diff_decoder.*)
   int mel_decoder = SSB_MEL_DECODER_DIFFSINGER;
+  // hparams['K_step'] of the DiffSinger mel sampler (ssb_model_set_mel_k_step): q_sample at K-1, then K reverse steps on the
+  // T-step schedule.  0 follows the schedule's T.
+  int mel_k_step = 0;
   float log_eps = 0.f;
   // auxiliary stream + fork/join events: lets the two independent F0 samplers overlap (created in build_model).
   // Calls on one model are therefore serialised with respect to these events (one in-flight forward per model).

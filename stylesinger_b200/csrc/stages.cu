@@ -620,15 +620,26 @@ int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const f
   return denoiser_stack(c, d, s, t, b);
 }
 
-// x_T of the mel sampler.  DiffSinger: q_sample(norm_spec(coarse), T-1) (shallow_diffusion_tts.py:298-302); ProDiff:
-// randn (prodiff.py:214-216), no coarse mel.  Both draw block 0 of the injected noise, or Philox stream_mel_xt().
+// Reverse steps of the mel sampler: hparams['K_step'] (DiffusionDecoder.forward's t = self.K_step,
+// shallow_diffusion_tts.py:297-304), set by ssb_model_set_mel_k_step; 0 follows the schedule's T.  The reference would
+// index past its schedule buffers with K > T, so that is an error here.
+static int mel_k_step(const Model& m, int* K) {
+  const int T = m.melnet.T;
+  *K = m.mel_k_step > 0 ? m.mel_k_step : T;
+  SSB_CHECK(*K <= T, "mel sampler: K_step " + std::to_string(*K) + " (ssb_model_set_mel_k_step) exceeds the schedule's T " +
+                         std::to_string(T));
+  return 0;
+}
+
+// x_K of the mel sampler.  DiffSinger: q_sample(norm_spec(coarse), K-1) on the T-step schedule
+// (shallow_diffusion_tts.py:298-302); ProDiff: randn (prodiff.py:214-216), no coarse mel.  Both draw block 0 of the
+// injected noise, or Philox stream_mel_xt().
 static int mel_init(Ctx& c, const Model& m, const SeqDev& s, const float* coarse_g, const float* noise, uint64_t seed,
-                    float* xm) {
+                    int K, float* xm) {
   const Denoiser& d = m.melnet;
-  const int T = d.T;
   if (m.mel_decoder == SSB_MEL_DECODER_PRODIFF)
     return mel_q_sample(c, s, nullptr, 80, noise, nullptr, nullptr, 0.f, 0.f, xm, 80, seed, stream_mel_xt());
-  const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 6];
+  const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(K - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(K - 1) * 8 + 6];
   return mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, stream_mel_xt());
 }
 // x_0 -> mel_out.  DiffSinger: denorm_spec (shallow_diffusion_tts.py:305,274-275); ProDiff: denorm_spec is the identity
@@ -724,12 +735,12 @@ static void persistent_net_step(const PersistentNet& p, const SeqDev& s, int t, 
   ph.push_back(q);
 }
 
-// a18+a19, single launch: all T reverse steps of the mel DiffNet.
+// a18+a19, single launch: all K reverse steps (t = K-1 .. 0) of the mel DiffNet, K (2L + 3) phases.
 static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
-                                        const float* noise, uint64_t seed, float* mel_tight) {
+                                        const float* noise, uint64_t seed, int K, float* mel_tight) {
   using P = PersistentNet;
   const Denoiser& d = m.melnet;
-  const int C = d.C, L = d.L, T = d.T;
+  const int C = d.C, L = d.L;
   const int CS = 4;  // cluster size along N: A tiles are TMA-multicast to the 4 CTAs that share an M-tile
   const size_t mk = c.mark();
   float* xm = alloc_rows(c, s, 80);
@@ -738,13 +749,13 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
   __half* x80h = alloc_half_rows(c, s, 128);  // planes of x_t, K padded 80 -> 128
   __half* x80l = alloc_half_rows(c, s, 128);
   const int M_X80 = P::nmaps(L), W_IN = M_X80 + 2, nmaps = W_IN + 2;
-  const int nph = T * (2 * L + 3);
+  const int nph = K * (2 * L + 3);
   CUtensorMap* maps_dev = c.alloc<CUtensorMap>((size_t)nmaps);
   SPhase* ph_dev = c.alloc<SPhase>((size_t)nph);
   unsigned* ctr = c.alloc<unsigned>(4);
   WS_OK(c);
   const size_t per = (size_t)s.total * 80;
-  RUN(mel_init(c, m, s, coarse_g, noise, seed, xm));
+  RUN(mel_init(c, m, s, coarse_g, noise, seed, K, xm));
   RUN(x80_planes(c, xm, s.rows, x80h, x80l));
   if (!c.dry) {
     std::vector<CUtensorMap> maps((size_t)nmaps);
@@ -754,7 +765,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
     maps[W_IN] = d.in_tc.tm_hi[1]; maps[W_IN + 1] = d.in_tc.tm_lo[1];
     std::vector<SPhase> ph;
     ph.reserve((size_t)nph);
-    for (int t = T - 1; t >= 0; --t) {
+    for (int t = K - 1; t >= 0; --t) {
       SPhase q = sphase(1);  // input_projection + ReLU ; y = x + step bias of layer 0
       q.a1 = M_X80; q.w1 = W_IN; q.kchunks = 2; q.N = C; q.NT = C / 64; q.mode = SP_INPROJ; q.bias = d.in_proj.bias;
       q.out = net.x; q.ldo = C; q.oh = net.pl[P::Y]; q.ol = net.pl[P::Y + 1]; q.ldh = C; q.vec2 = d.dtab + (size_t)t * L * C;
@@ -763,7 +774,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
       q = sphase(1);  // output_projection -> eps ; fused DDPM posterior step on x_t
       q.a1 = net.mb + P::S; q.w1 = net.w_out(); q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE;
       q.bias = d.out_bias_pad; q.out = xm; q.ldo = 80; q.oh = x80h; q.ol = x80l; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
-      q.noise = noise ? noise + per * (size_t)(T - t) : nullptr; q.seed = seed; q.stream_id = stream_mel_step(t); q.n_valid = 80;
+      q.noise = noise ? noise + per * (size_t)(K - t) : nullptr; q.seed = seed; q.stream_id = stream_mel_step(t); q.n_valid = 80;
       q.no_clip = m.mel_decoder == SSB_MEL_DECODER_PRODIFF;
       ph.push_back(q);
     }
@@ -779,11 +790,13 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
 // a18+a19: DiffusionDecoder.forward(infer=True) (shallow_diffusion_tts.py:284-307), or on a ProDiff model
 // ProDiffusion.forward(infer=True) (prodiff.py:204-222; coarse_g unused, pass null)
 int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
-                      const float* noise /*tight [(T+1), total, 80] or null*/, uint64_t seed, float* mel_tight,
+                      const float* noise /*tight [(K+1), total, 80] or null*/, uint64_t seed, float* mel_tight,
                       const Seq* host_seq) {
   const Denoiser& d = m.melnet;
   SSB_CHECK(d.T > 0, "mel schedule not set: call ssb_model_set_schedule(which=0)");
-  // ssb_model_set_persistent_groups(1): utterances are independent, so the T x L loop runs per GROUP of consecutive
+  int K = 0;
+  RUN(mel_k_step(m, &K));
+  // ssb_model_set_persistent_groups(1): utterances are independent, so the K x L loop runs per GROUP of consecutive
   // utterances of <= 48 row tiles (a contiguous slice of the guard-banded layout: the sub-batch simply aliases the big
   // buffers), each by the single-launch persistent kernel (BASELINE.json configs[4]: persistent-kernel vs per-step-launch
   // at batch 64).  Production (Philox) mode only - the injected-noise tensors are strided by the whole batch; each group
@@ -819,20 +832,19 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
   }
   if (m.persistent && denoiser_tc_ok(m, d) && d.in_tc.ok && d.skip_tc.ok && d.out_tc.ok && s.ntiles <= 48 &&
       sampler_tc_max_ctas() > 0)
-    return run_mel_diffusion_persistent(c, m, s, cond_g, coarse_g, noise, seed, mel_tight);
+    return run_mel_diffusion_persistent(c, m, s, cond_g, coarse_g, noise, seed, K, mel_tight);
   const size_t mk = c.mark();
   DenoiserBufs b;
   RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
   float* xm = alloc_rows(c, s, 80);
   WS_OK(c);
   RUN(prepare_cond(c, d, s, cond_g, b));
-  const int T = d.T;
   const size_t per = (size_t)s.total * 80;
   const bool clip = m.mel_decoder != SSB_MEL_DECODER_PRODIFF;
-  RUN(mel_init(c, m, s, coarse_g, noise, seed, xm));
-  for (int t = T - 1; t >= 0; --t) {
+  RUN(mel_init(c, m, s, coarse_g, noise, seed, K, xm));
+  for (int t = K - 1; t >= 0; --t) {
     RUN(mel_denoiser_eval(c, d, s, t, xm, b));
-    const float* nz = noise ? noise + per * (size_t)(T - t) : nullptr;
+    const float* nz = noise ? noise + per * (size_t)(K - t) : nullptr;
     RUN(mel_p_sample(c, s, xm, 80, b.head, b.ld_head, nz, d.gtab + (size_t)t * 8, seed, stream_mel_step(t), clip));
   }
   RUN(mel_finish(c, m, s, xm, mel_tight));
@@ -841,14 +853,16 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
 }
 
 // f2 (SURVEY 8f): PLMS / PNDM sampler over the same denoiser (GaussianDiffusion.p_sample_plms + the pndm_speedup loop of
-// GaussianDiffusion.forward, shallow_diffusion_tts.py:164-197,254-260): T / interval evaluations (+1 for the first step).
+// GaussianDiffusion.forward, shallow_diffusion_tts.py:164-197,254-260): K / interval evaluations (+1 for the first step).
 int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
                            const float* q_noise /*tight [total, 80] or null*/, uint64_t seed, int interval, float* mel_tight) {
   const Denoiser& d = m.melnet;
   SSB_CHECK(m.mel_decoder == SSB_MEL_DECODER_DIFFSINGER,
             "plms: the PLMS sampler needs a DiffSinger model (the ProDiff sampler predicts x0, not eps)");
   SSB_CHECK(d.T > 0, "mel schedule not set: call ssb_model_set_schedule(which=0)");
-  SSB_CHECK(interval >= 1 && interval < d.T, "plms: interval (pndm_speedup) must be in [1, T)");
+  int K = 0;
+  RUN(mel_k_step(m, &K));
+  SSB_CHECK(interval >= 1 && interval < K, "plms: interval (pndm_speedup) must be in [1, K_step)");
   const size_t mk = c.mark();
   DenoiserBufs b;
   RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
@@ -857,14 +871,12 @@ int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float*
   float* hist[3] = {alloc_rows(c, s, 80), alloc_rows(c, s, 80), alloc_rows(c, s, 80)};
   WS_OK(c);
   RUN(prepare_cond(c, d, s, cond_g, b));
-  const int T = d.T;
   auto acp = [&](int t) { return c.dry ? 0.5f : d.gtab_h[(size_t)t * 8 + 7]; };
-  const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(T - 1) * 8 + 6];
-  RUN(mel_q_sample(c, s, coarse_g, 80, q_noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, stream_mel_xt()));
+  RUN(mel_init(c, m, s, coarse_g, q_noise, seed, K, xm));
   int nh = 0;  // predictions in the history; hist[(head + k) % 3] is the k-th newest
   int head = 0;
   int t0 = 0;
-  for (int t = 0; t < T; t += interval) t0 = t;  // reversed(range(0, T, interval)) starts at the largest multiple
+  for (int t = 0; t < K; t += interval) t0 = t;  // reversed(range(0, K, interval)) starts at the largest multiple below K
   for (int t = t0; t >= 0; t -= interval) {
     const int tp = t - interval > 0 ? t - interval : 0;
     RUN(mel_denoiser_eval(c, d, s, t, xm, b));

@@ -169,6 +169,9 @@ class AcousticModel:
         self._ws = _Workspace(self.device)
         self.T = self.f0_T = None
         self.set_timesteps(hp["timesteps"], hp["f0_timesteps"] if self.f0_gen == "gmdiff" else None)
+        self.K = None  # K_step of the mel sampler; None follows T
+        if self.mel_decoder == "diffsinger" and int(hp["K_step"]) != hp["timesteps"]:
+            self.set_mel_k_step(int(hp["K_step"]))
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -212,6 +215,14 @@ class AcousticModel:
                                              g.ctypes.data_as(C.c_void_p), m.ctypes.data_as(C.c_void_p), stream),
                   "ssb_model_set_schedule(f0)")
             self.f0_T = f0_T
+
+    def set_mel_k_step(self, K=None):
+        """hparams['K_step'] of the DiffSinger mel sampler (shallow diffusion): q_sample at K-1 of the T-step schedule, then
+        K reverse steps; injected mel noise is then [(K+1), sumF, 80].  None or 0 follows T.  A K above T fails at the
+        sampler call; any K on a 'prodiff' model fails here."""
+        K = int(K or 0)
+        check(lib.ssb_model_set_mel_k_step(self._h, K), "ssb_model_set_mel_k_step")
+        self.K = K or None
 
     # -- helpers ---------------------------------------------------------------------------------
     def _stream(self):
@@ -300,6 +311,8 @@ class AcousticModel:
         return out
 
     def mel_diffusion(self, cond, coarse, frame_offsets, noise=None, seed=0):
+        """DiffusionDecoder.forward(infer=True): cond [sumF,256], coarse [sumF,80] -> mel [sumF,80].  noise: [(K+1), sumF, 80]
+        (the q_sample draw, then one per step t = K-1 .. 0; K = K_step, else T), or None for the in-kernel Philox."""
         fo = np.ascontiguousarray(frame_offsets, np.int32)
         B = len(fo) - 1
         n = lib.ssb_mel_diffusion_workspace_bytes(self._h, fo.ctypes.data, B)
@@ -326,7 +339,7 @@ class AcousticModel:
         return mel
 
     def mel_diffusion_plms(self, cond, coarse, frame_offsets, interval, q_noise=None, seed=0):
-        """PLMS sampler (hparams['pndm_speedup'] = interval) over the mel denoiser: T / interval (+1) evaluations."""
+        """PLMS sampler (hparams['pndm_speedup'] = interval, in [1, K)) over the mel denoiser: K / interval (+1) evaluations."""
         fo = np.ascontiguousarray(frame_offsets, np.int32)
         B = len(fo) - 1
         n = lib.ssb_mel_diffusion_plms_workspace_bytes(self._h, fo.ctypes.data, B)

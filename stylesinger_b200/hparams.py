@@ -110,9 +110,12 @@ def _check_supported(hp):
         raise NotImplementedError("rel_pos is not selected by egs/stylesinger.yaml")
     if prodiff:  # ProDiffusion.forward(infer=True) never reads K_step or pndm_speedup (prodiff.py:204-222)
         return
+    # shallow diffusion (DiffusionDecoder.forward, shallow_diffusion_tts.py:297-304): q_sample at K_step - 1 of the
+    # timesteps-long schedule, then K_step reverse steps; beyond timesteps the reference indexes past its buffers
+    K = int(hp["K_step"])
+    if not (1 <= K <= int(hp["timesteps"])):
+        raise ValueError(f"K_step must be in [1, timesteps = {hp['timesteps']}], got {K}")
     if hp.get("pndm_speedup"):  # PLMS sampler over the mel denoiser (SURVEY.md §8 f2, ssb_mel_diffusion_sample_plms)
         k = int(hp["pndm_speedup"])
-        if not (1 <= k < int(hp["timesteps"])):
-            raise ValueError(f"pndm_speedup must be in [1, timesteps), got {k}")
-    if hp["K_step"] != hp["timesteps"]:
-        raise NotImplementedError("K_step must equal timesteps (as in egs/stylesinger.yaml)")
+        if not (1 <= k < K):
+            raise ValueError(f"pndm_speedup must be in [1, K_step = {K}), got {k}")

@@ -4,7 +4,7 @@ ragged batches and writes one wav per item.  Equivalent of `python tasks/run.py 
 (tasks/StyleSinger/stylesinger.py:168-275, which asserts B=1).
 
     python tools/infer_dataset.py --ckpt checkpoints/StyleSinger --vocoder checkpoints/hifigan --data data/binary/x/test \
-        --out infer_out [--batch 64] [--T 100] [--limit N] [--use-gt-dur] [--vocoder-denoise-c 0.1]
+        --out infer_out [--batch 64] [--T 100] [--k-step 50] [--limit N] [--use-gt-dur] [--vocoder-denoise-c 0.1]
 
 Like the reference's test_step (tasks/StyleSinger/stylesinger.py:177-180 with `use_gt_dur: false` in egs/stylesinger.yaml) the
 durations come from the duration predictor unless --use-gt-dur is given (then the items' ground-truth mel2ph is fed).
@@ -26,6 +26,8 @@ def main():
     ap.add_argument("--out", required=True)
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--T", type=int, default=100)
+    ap.add_argument("--k-step", type=int, default=None,
+                    help="reference hparam K_step (shallow diffusion): mel reverse steps from q_sample at K-1; default --T")
     ap.add_argument("--limit", type=int, default=0)
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--use-gt-dur", action="store_true", help="feed the items' ground-truth mel2ph (reference hparam use_gt_dur)")
@@ -38,7 +40,8 @@ def main():
     from stylesinger_b200.hparams import resolve
     from stylesinger_b200.infer import StyleSingerInfer
 
-    hp = resolve(timesteps=args.T, K_step=args.T, f0_timesteps=args.T, vocoder_denoise_c=args.vocoder_denoise_c)
+    hp = resolve(timesteps=args.T, K_step=args.T if args.k_step is None else args.k_step, f0_timesteps=args.T,
+                 vocoder_denoise_c=args.vocoder_denoise_c)
     sd, path = formats.load_state_dict(args.ckpt, "model")
     vsd, vcfg, vpath = formats.load_vocoder_checkpoint(args.vocoder)
     print(f"| acoustic checkpoint {path} ({len(sd)} tensors); vocoder {vpath}")

@@ -57,9 +57,11 @@ class _Dict:
         return synth.N_TOKENS
 
 
-def build_reference_model(T, f0_T=None):
+def build_reference_model(T, f0_T=None, K=None):
     import ref_import
     hp = ref_import.install(T=T, f0_T=f0_T)
+    if K is not None:  # StyleSinger.__init__ hands hparams['K_step'] to the DiffusionDecoder (stylesinger.py:103-110)
+        hp["K_step"] = K
     # fresh import state for every T: the schedule buffers are built in __init__
     import modules.diff.shallow_diffusion_tts as sdt
     import modules.diff.gaussian_multinomial_diffusion as gmd
@@ -67,7 +69,7 @@ def build_reference_model(T, f0_T=None):
     gmd.tqdm = lambda it, **k: it
     from modules.StyleSinger.stylesinger import StyleSinger
     model = StyleSinger(_Dict()).eval()
-    sd = synth.acoustic_state_dict(dict(hp), seed=0)
+    sd = synth.acoustic_state_dict(dict(hp, K_step=T), seed=0)  # the weights do not depend on K_step
     missing, unexpected = model.load_state_dict(sd, strict=True), None
     return model, hp, sd
 
@@ -275,6 +277,65 @@ def case_plms(name, T=100, interval=10, frames=48, seed=61):
     print("wrote", name, mel.shape, float(mel.abs().max()))
 
 
+def case_kstep(name, T_fwd=25, K_fwd=11, frames=64, phones=8, ref_frames=48, seed=141, utt_idx=106, T=100, K=51,
+               intervals=(10, 7), sampler_frames=48):
+    """Shallow diffusion, hparams['K_step'] < timesteps (GaussianDiffusion.__init__ :92, DiffusionDecoder.forward :297-304):
+    x_K = q_sample(norm_spec(coarse), K - 1) on the T-step schedule, then K reverse steps.
+    (a) fwd_*: a full B = 1 forward at T_fwd / K_fwd with mel2ph given, and its coarse mel;
+    (b) smp_*: DiffusionDecoder.forward(infer=True) alone at T / K on seeded cond and coarse;
+    (c) plms_i<k>_*: the PLMS loop driven as case_plms does but from t = K (t0 = the largest multiple of k below K);
+    (d) smp1_*: (b) at K = 1, one step at t = 0 (its noise is drawn and multiplied by 0).
+    Every noise log is in meta."""
+    from collections import deque
+    model, hp, sd = build_reference_model(T_fwd, K=K_fwd)
+    assert model.postdiff.K_step == K_fwd and model.postdiff.num_timesteps == T_fwd
+    u = synth.make_utterance(frames / 187.5, utt_idx=utt_idx, ref_frames=ref_frames, frames=frames, phones=phones)
+    out, log = run_model(model, u, seed)
+    coarse_fwd, _ = run_model(model, u, seed, global_steps=50000)  # forcing < global_steps < diff_start: coarse mel only
+    meta = {"T_fwd": T_fwd, "K_fwd": K_fwd, "frames": frames, "phones": phones, "ref_frames": ref_frames, "seed": seed,
+            "utt_idx": utt_idx, "noise_log": log, "T": T, "K": K, "intervals": list(intervals),
+            "sampler_frames": sampler_frames}
+    d = {"fwd_style": np32(out["style"][0]), "fwd_rq_codes": out["rq_codes"][0].numpy().astype(np.int64),
+         "fwd_pitch_pred": np32(out["pitch_pred"][0]), "fwd_f0_denorm": np32(out["f0_denorm"][0]),
+         "fwd_decoder_inp": np32(out["decoder_inp"][0]), "fwd_coarse_mel": np32(coarse_fwd["mel_out"][0]),
+         "fwd_mel_out": np32(out["mel_out"][0])}
+    g = torch.Generator().manual_seed(seed + 1)
+    cond = torch.randn(1, sampler_frames, 256, generator=g)
+    coarse = (-3 + 0.8 * torch.randn(1, sampler_frames, 80, generator=g)).clamp(-6, 0.5)
+    d.update({"smp_cond": np32(cond[0]), "smp_coarse": np32(coarse[0])})
+    for key, k_step in (("smp", K), ("smp1", 1)):
+        model, _, _ = build_reference_model(T, K=k_step)
+        pd = model.postdiff
+        assert pd.K_step == k_step and pd.num_timesteps == T
+        ns = NoiseSource(seed + 2)
+        ret = {}
+        with torch.no_grad(), patched_rng(ns):
+            pd(cond, None, coarse, ret, infer=True)
+        d[key + "_mel"] = np32(ret["mel_out"][0])
+        meta[key + "_noise_log"] = ns.log
+    model, _, _ = build_reference_model(T, K=K)
+    pd = model.postdiff
+    for k in intervals:
+        ns = NoiseSource(seed + 3)
+        with torch.no_grad(), patched_rng(ns):
+            c = cond.transpose(1, 2)
+            fs2 = pd.norm_spec(coarse).transpose(1, 2)[:, None, :, :]
+            t = pd.K_step
+            x = pd.q_sample(x_start=fs2, t=torch.tensor([t - 1]).long())
+            pd.noise_list = deque(maxlen=4)
+            steps = list(reversed(range(0, t, k)))
+            for i in steps:
+                x = pd.p_sample_plms(x, torch.full((1,), i, dtype=torch.long), k, c)
+            mel = pd.denorm_spec(x[:, 0].transpose(1, 2))
+        d[f"plms_i{k}_mel"] = np32(mel[0])
+        meta[f"plms_i{k}_noise_log"] = ns.log
+        meta[f"plms_i{k}_t0"] = steps[0]
+    d["meta"] = json.dumps(meta)
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()},
+          {k: v for k, v in meta.items() if k.endswith("_t0")})
+
+
 PRODIFF_OVERRIDES = {"decoder": "prodiff", "schedule_type": "vpsde", "timescale": 1}  # egs/stylesinger.yaml:145-155
 
 
@@ -467,7 +528,7 @@ if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "convf0", "sched", "voc",
-                             "vocoder_edges", "emo", "registry"]
+                             "vocoder_edges", "emo", "registry", "kstep"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
@@ -492,3 +553,5 @@ if __name__ == "__main__":
         case_emotion_encoder("ref_emotion_encoder")
     if "registry" in which:
         case_registry("ref_registry")
+    if "kstep" in which:
+        case_kstep("ref_kstep")

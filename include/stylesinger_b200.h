@@ -16,11 +16,20 @@
  *    points enqueue on `stream`, never allocate device memory and never synchronise — except
  *    ssb_model_create / ssb_vocoder_create / ssb_model_set_schedule, which own the packed weights.
  *  - return 0 on success, negative on error with a message in ssb_last_error() (thread-local).
- *  - noise: NULL noise pointers select the in-kernel counter-based generator (Philox, `seed`);
+ *  - noise: NULL noise pointers select the in-kernel counter-based generator (Philox);
  *    non-NULL pointers inject the noise explicitly (parity mode; SURVEY.md A.10 draw order).
- *    Philox draws are indexed by the tight row of the call (and the persistent mel groups re-seed
- *    each group), so in that mode an utterance's noise depends on the batch it is in.  The stream
- *    plan is documented in csrc/philox.cuh.
+ *    Philox has two modes, which draw the same streams (csrc/philox.cuh) under different keys and counters:
+ *     - one seed per call (`seed`, the default): every draw is keyed by `seed` and counted by the tight
+ *       row of the whole call (frame, or sample for the vocoder source), and the vocoder's initial
+ *       phases by the utterance index; the persistent mel groups (ssb_model_set_persistent_groups) key
+ *       group g by seed + 0x9E3779B97F4A7C15 g and count rows inside the group.  An utterance's noise
+ *       therefore depends on the batch it is in.
+ *     - one seed per utterance (ssb_acoustic_forward_keyed, ssb_hifigan_generate_keyed): utterance b's
+ *       draws are keyed by utt_seeds[b] and counted from its own first row, with initial-phase stream
+ *       index 0, and nothing is re-seeded per group.  Each draw is bit-for-bit the draw of a B = 1
+ *       call with seed = utt_seeds[b], whatever else the batch holds.
+ *    The standalone sampler entries (ssb_mel_diffusion_sample[_plms], ssb_mel_prodiff_sample,
+ *    ssb_f0_diffusion_sample) have only the per-call mode.
  */
 #ifndef STYLESINGER_B200_H
 #define STYLESINGER_B200_H
@@ -190,6 +199,12 @@ int ssb_predict_durations(const ssb_model_t* m, const ssb_acoustic_inputs* in, i
 size_t ssb_acoustic_workspace_bytes(const ssb_model_t* m, const ssb_acoustic_inputs* in);
 int ssb_acoustic_forward(const ssb_model_t* m, const ssb_acoustic_inputs* in, const ssb_acoustic_outputs* out,
                          void* workspace, size_t workspace_bytes, void* stream);
+/* ssb_acoustic_forward with one Philox seed per utterance: utt_seeds (HOST [B], required) keys utterance b's draws, so
+ * its outputs are those of a B = 1 ssb_acoustic_forward with seed = utt_seeds[b] (up to the GEMM path a batch of that size
+ * takes).  in->seed is ignored; injected noise (mel_noise, f0_gauss_noise, f0_unif_noise) is an error.  The workspace is
+ * ssb_acoustic_workspace_bytes(m, in). */
+int ssb_acoustic_forward_keyed(const ssb_model_t* m, const ssb_acoustic_inputs* in, const uint64_t* utt_seeds,
+                               const ssb_acoustic_outputs* out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* DiffusionDecoder.forward(infer=True) alone (modules/diff/shallow_diffusion_tts.py:284-307):
  * cond [sumF,256], coarse [sumF,80] -> mel [sumF,80].  DiffSinger models only (the PLMS entry point too).
@@ -279,6 +294,11 @@ size_t ssb_vocoder_workspace_bytes(const ssb_vocoder_t* v, const int32_t* frame_
 int ssb_hifigan_generate(const ssb_vocoder_t* v, const float* mel, const float* f0, const int32_t* frame_offsets,
                          int32_t B, const float* rand_ini, const float* src_noise, uint64_t seed, float* wav_out,
                          void* workspace, size_t workspace_bytes, void* stream);
+/* ssb_hifigan_generate with one Philox seed per utterance (utt_seeds: HOST [B], required) and no injected noise: utterance
+ * b's SineGen draws are those of a B = 1 call with seed = utt_seeds[b].  The workspace is ssb_vocoder_workspace_bytes. */
+int ssb_hifigan_generate_keyed(const ssb_vocoder_t* v, const float* mel, const float* f0, const int32_t* frame_offsets,
+                               int32_t B, const uint64_t* utt_seeds, float* wav_out, void* workspace,
+                               size_t workspace_bytes, void* stream);
 
 /* Select the GEMM path of the denoiser layers: 1 = wgmma tensor cores on fp16 hi/lo split operands
  * (3 MMAs per product, fp32 accumulate; default when available), 0 = fp32 FFMA.  Returns the mode in effect. */

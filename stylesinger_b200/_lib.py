@@ -68,6 +68,7 @@ EXPORTS = [
     "ssb_wav_denoise_create", "ssb_wav_denoise_free", "ssb_wav_denoise_workspace_bytes", "ssb_wav_denoise_forward",
     "ssb_wav_denoise_set_tensor_cores",
     "ssb_model_set_mel_k_step",
+    "ssb_acoustic_forward_keyed", "ssb_hifigan_generate_keyed",
 ]
 
 
@@ -93,6 +94,7 @@ def _load():
         "ssb_predict_durations": (C.c_int, [vp, P(AcousticInputs), vp, vp, vp, sz, vp]),
         "ssb_acoustic_workspace_bytes": (sz, [vp, P(AcousticInputs)]),
         "ssb_acoustic_forward": (C.c_int, [vp, P(AcousticInputs), P(AcousticOutputs), vp, sz, vp]),
+        "ssb_acoustic_forward_keyed": (C.c_int, [vp, P(AcousticInputs), vp, P(AcousticOutputs), vp, sz, vp]),
         "ssb_mel_diffusion_workspace_bytes": (sz, [vp, vp, i32]),
         "ssb_mel_diffusion_sample": (C.c_int, [vp, vp, vp, vp, i32, vp, u64, vp, vp, sz, vp]),
         "ssb_mel_prodiff_workspace_bytes": (sz, [vp, vp, i32]),
@@ -106,6 +108,7 @@ def _load():
         "ssb_vocoder_free": (None, [vp]),
         "ssb_vocoder_workspace_bytes": (sz, [vp, vp, i32]),
         "ssb_hifigan_generate": (C.c_int, [vp, vp, vp, vp, i32, vp, vp, u64, vp, vp, sz, vp]),
+        "ssb_hifigan_generate_keyed": (C.c_int, [vp, vp, vp, vp, i32, vp, vp, vp, sz, vp]),
         "ssb_op_conv1d": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, i32, i32, i32, vp, vp]),
         "ssb_op_attention": (C.c_int, [vp, vp, vp, vp, vp, i32, C.c_float, vp, vp]),
         "ssb_op_attention_tc": (C.c_int, [vp, vp, vp, vp, vp, i32, C.c_float, vp, vp]),

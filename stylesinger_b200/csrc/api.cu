@@ -31,7 +31,7 @@ static int project_vec(Ctx& c, const Conv& w, const float* in_tight, int B, floa
 
 // StyleSinger.forward(infer=True) (stylesinger.py:119-187); durations_only stops after add_dur.
 int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ssb_acoustic_outputs& out,
-                 bool durations_only, int32_t* dur_out, float* logdur_out) {
+                 bool durations_only, int32_t* dur_out, float* logdur_out, const uint64_t* utt_seeds) {
   const int H = 256, B = in.B;
   SSB_CHECK(B >= 1 && in.ph_offsets && in.ref_offsets, "acoustic: bad batch description");
   SSB_CHECK(durations_only || in.frame_offsets, "acoustic: frame_offsets required");
@@ -83,6 +83,8 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   }
 
   qf.build(in.frame_offsets, B);
+  qf.seed = in.seed;
+  qf.utt_seeds = utt_seeds;
   SSB_CHECK(qf.maxlen + 2 <= m.pos_rows, "frame sequence longer than __pos_table");
   RUN(upload_layout(c, qf, 1, &sf));
   int32_t* mel2ph = alloc_rows_i32(c, sf);
@@ -191,7 +193,7 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
       }
       float* zz[2] = {za, zs};
       int32_t* uu[2] = {uva, uvs};
-      RUN(run_f0_samplers(c, m, sf, cond, cond2, lo, hi, in.f0_gauss_noise, in.f0_unif_noise, in.seed, zz, uu));
+      RUN(run_f0_samplers(c, m, sf, cond, cond2, lo, hi, in.f0_gauss_noise, in.f0_unif_noise, zz, uu));
     }
     PitchGlueArgs pg;
     pg.za = za; pg.uva = uva; pg.zs = zs; pg.uvs = uvs; pg.midi = midi; pg.mel2ph = mel2ph;
@@ -221,7 +223,7 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
     // mel, and no pndm_speedup (ProDiffusion.forward never reads it)
     if (!in.skip_mel_diffusion) {
       SSB_CHECK(out.mel_out != nullptr, "acoustic: mel_out required");
-      RUN(run_mel_diffusion(c, m, sf, dec, nullptr, in.mel_noise, in.seed, out.mel_out, &qf));
+      RUN(run_mel_diffusion(c, m, sf, dec, nullptr, in.mel_noise, out.mel_out, &qf));
     }
     return 0;
   }
@@ -258,9 +260,9 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   if (!in.skip_mel_diffusion) {
     SSB_CHECK(out.mel_out != nullptr, "acoustic: mel_out required");
     if (in.pndm_speedup > 0)  // PLMS: mel_noise, when given, supplies only the q_sample draw (its first [sumF, 80] block)
-      RUN(run_mel_diffusion_plms(c, m, sf, cond, coarse, in.mel_noise, in.seed, in.pndm_speedup, out.mel_out));
+      RUN(run_mel_diffusion_plms(c, m, sf, cond, coarse, in.mel_noise, in.pndm_speedup, out.mel_out));
     else
-      RUN(run_mel_diffusion(c, m, sf, cond, coarse, in.mel_noise, in.seed, out.mel_out, &qf));
+      RUN(run_mel_diffusion(c, m, sf, cond, coarse, in.mel_noise, out.mel_out, &qf));
   }
   return 0;
 }
@@ -316,7 +318,7 @@ static Ctx make_ctx(void* ws, size_t bytes, void* stream, bool dry = false) {
 
 extern "C" {
 
-int ssb_version(void) { return 100; }
+int ssb_version(void) { return 101; }
 const char* ssb_last_error(void) { return ssb::last_error(); }
 
 int ssb_model_create(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp) {
@@ -400,6 +402,16 @@ int ssb_acoustic_forward(const ssb_model_t* m, const ssb_acoustic_inputs* in, co
   Ctx c = make_ctx(workspace, workspace_bytes, stream);
   return run_acoustic(c, m->m, *in, *out, false, nullptr, nullptr);
 }
+int ssb_acoustic_forward_keyed(const ssb_model_t* m, const ssb_acoustic_inputs* in, const uint64_t* utt_seeds,
+                               const ssb_acoustic_outputs* out, void* workspace, size_t workspace_bytes, void* stream) {
+  SSB_CHECK(m && in && out && workspace, "null argument");
+  SSB_CHECK(utt_seeds, "ssb_acoustic_forward_keyed: utt_seeds (one seed per utterance) is required");
+  SSB_CHECK(!in->mel_noise && !in->f0_gauss_noise[0] && !in->f0_gauss_noise[1] && !in->f0_unif_noise[0] &&
+                !in->f0_unif_noise[1],
+            "ssb_acoustic_forward_keyed: per-utterance seeds key the in-kernel noise; injected noise must be NULL");
+  Ctx c = make_ctx(workspace, workspace_bytes, stream);
+  return run_acoustic(c, m->m, *in, *out, false, nullptr, nullptr, utt_seeds);
+}
 
 static int mel_diff_impl(Ctx& c, const Model& m, const float* cond, const float* coarse, const int32_t* offs, int B,
                          const float* noise, uint64_t seed, float* mel_out) {
@@ -407,6 +419,7 @@ static int mel_diff_impl(Ctx& c, const Model& m, const float* cond, const float*
             "ssb_mel_diffusion_sample: the DDPM sampler needs a DiffSinger model; use ssb_mel_prodiff_sample on a ProDiff model");
   Seq q;
   q.build(offs, B);
+  q.seed = seed;
   SeqDev s;
   RUN(upload_layout(c, q, 1, &s));
   float* cg = alloc_rows(c, s, 256);
@@ -414,12 +427,13 @@ static int mel_diff_impl(Ctx& c, const Model& m, const float* cond, const float*
   WS_OK(c);
   RUN(pack_rows(c, s, cond, 256, cg, 256, 256));
   RUN(pack_rows(c, s, coarse, 80, co, 80, 80));
-  return run_mel_diffusion(c, m, s, cg, co, noise, seed, mel_out, &q);
+  return run_mel_diffusion(c, m, s, cg, co, noise, mel_out, &q);
 }
 static int mel_plms_impl(Ctx& c, const Model& m, const float* cond, const float* coarse, const int32_t* offs, int B,
                          const float* q_noise, uint64_t seed, int interval, float* mel_out) {
   Seq q;
   q.build(offs, B);
+  q.seed = seed;
   SeqDev s;
   RUN(upload_layout(c, q, 1, &s));
   float* cg = alloc_rows(c, s, 256);
@@ -427,7 +441,7 @@ static int mel_plms_impl(Ctx& c, const Model& m, const float* cond, const float*
   WS_OK(c);
   RUN(pack_rows(c, s, cond, 256, cg, 256, 256));
   RUN(pack_rows(c, s, coarse, 80, co, 80, 80));
-  return run_mel_diffusion_plms(c, m, s, cg, co, q_noise, seed, interval, mel_out);
+  return run_mel_diffusion_plms(c, m, s, cg, co, q_noise, interval, mel_out);
 }
 static int mel_prodiff_impl(Ctx& c, const Model& m, const float* cond, const int32_t* offs, int B, const float* noise,
                             uint64_t seed, float* mel_out) {
@@ -435,12 +449,13 @@ static int mel_prodiff_impl(Ctx& c, const Model& m, const float* cond, const int
             "ssb_mel_prodiff_sample: the ProDiff sampler needs a model created with SSB_MEL_DECODER_PRODIFF");
   Seq q;
   q.build(offs, B);
+  q.seed = seed;
   SeqDev s;
   RUN(upload_layout(c, q, 1, &s));
   float* cg = alloc_rows(c, s, 256);
   WS_OK(c);
   RUN(pack_rows(c, s, cond, 256, cg, 256, 256));
-  return run_mel_diffusion(c, m, s, cg, nullptr, noise, seed, mel_out, &q);
+  return run_mel_diffusion(c, m, s, cg, nullptr, noise, mel_out, &q);
 }
 size_t ssb_mel_prodiff_workspace_bytes(const ssb_model_t* m, const int32_t* frame_offsets, int32_t B) {
   Ctx c = make_ctx(nullptr, 0, nullptr, true);
@@ -505,6 +520,7 @@ int ssb_f0_diffusion_sample(const ssb_model_t* m, int32_t which, const float* co
   Ctx c = make_ctx(workspace, workspace_bytes, stream);
   Seq q;
   q.build(frame_offsets, B);
+  q.seed = seed;
   SeqDev s;
   RUN(upload_layout(c, q, 1, &s));
   float* cg = alloc_rows(c, s, 256);
@@ -516,7 +532,7 @@ int ssb_f0_diffusion_sample(const ssb_model_t* m, int32_t which, const float* co
   RUN(pack_rows(c, s, cond, 256, cg, 256, 256));
   RUN(pack_rows(c, s, clip_lo, 1, lo, 1, 1));
   RUN(pack_rows(c, s, clip_hi, 1, hi, 1, 1));
-  RUN(run_f0_diffusion(c, m->m, which, s, cg, lo, hi, gauss_noise, unif_noise, seed, z, uv));
+  RUN(run_f0_diffusion(c, m->m, which, s, cg, lo, hi, gauss_noise, unif_noise, z, uv));
   RUN(unpack_rows(c, s, z, 1, f0_norm_out, 1, 1));
   RUN(unpack_rows_i32(c, s, uv, uv_out));
   return 0;
@@ -670,7 +686,7 @@ size_t ssb_vocoder_workspace_bytes(const ssb_vocoder_t* v, const int32_t* frame_
   Ctx c = make_ctx(nullptr, 0, nullptr, true);
   Seq q;
   q.build(frame_offsets, B);
-  if (run_vocoder(c, v->v, q, nullptr, (const float*)(uintptr_t)256, nullptr, nullptr, 0, nullptr) != 0) return 0;
+  if (run_vocoder(c, v->v, q, nullptr, (const float*)(uintptr_t)256, nullptr, nullptr, nullptr) != 0) return 0;
   return c.high + 4096;
 }
 int ssb_hifigan_generate(const ssb_vocoder_t* v, const float* mel, const float* f0, const int32_t* frame_offsets,
@@ -680,7 +696,19 @@ int ssb_hifigan_generate(const ssb_vocoder_t* v, const float* mel, const float* 
   Ctx c = make_ctx(workspace, workspace_bytes, stream);
   Seq q;
   q.build(frame_offsets, B);
-  return run_vocoder(c, v->v, q, mel, f0, rand_ini, src_noise, seed, wav_out);
+  q.seed = seed;
+  return run_vocoder(c, v->v, q, mel, f0, rand_ini, src_noise, wav_out);
+}
+int ssb_hifigan_generate_keyed(const ssb_vocoder_t* v, const float* mel, const float* f0, const int32_t* frame_offsets,
+                               int32_t B, const uint64_t* utt_seeds, float* wav_out, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  SSB_CHECK(v && mel && frame_offsets && wav_out && workspace, "null argument");
+  SSB_CHECK(utt_seeds, "ssb_hifigan_generate_keyed: utt_seeds (one seed per utterance) is required");
+  Ctx c = make_ctx(workspace, workspace_bytes, stream);
+  Seq q;
+  q.build(frame_offsets, B);
+  q.utt_seeds = utt_seeds;
+  return run_vocoder(c, v->v, q, mel, f0, nullptr, nullptr, wav_out);
 }
 
 int ssb_model_set_tensor_cores(ssb_model_t* m, int32_t enable) {

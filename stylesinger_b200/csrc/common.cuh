@@ -58,6 +58,10 @@ struct Seq {
   int64_t rows1 = 0;      // (rs_{B-1} + L_{B-1} + G): rows at rate 1 excluding slack
   int64_t total = 0;      // sum L_b
   int maxlen = 0;
+  // Philox keys of the layout's draws (philox.cuh, "Batch composition"): utt_seeds (host [B]) keys utterance b by
+  // utt_seeds[b] and counts its rows from 0; NULL keys every utterance by `seed` and counts the tight rows of the layout.
+  uint64_t seed = 0;
+  const uint64_t* utt_seeds = nullptr;
 
   void build(const int32_t* offsets, int B_) {
     B = B_;
@@ -83,17 +87,26 @@ struct Seq {
   }
 };
 
+// Philox key and counter base of one utterance: its row t (at the layout's rate) draws with counter row row0 + t, and
+// its vocoder initial phase from stream_voc_ini(ini) (philox.cuh).
+struct UttRng {
+  uint64_t key;
+  int32_t row0;
+  int32_t ini;
+};
+
 // Device-side view of one layout at one rate.
 struct SeqDev {
   const int2* tiles = nullptr;  // (row0, nvalid) per 128-row tile
   int ntiles = 0;
   const int4* utt = nullptr;    // per utterance: (row_start, len, tight_offset, 0) at this rate
+  const UttRng* rng = nullptr;  // per utterance: Philox key and counter base at this rate
   int B = 0;
   int64_t rows = 0;             // allocated rows (incl. slack)
   int64_t total = 0;            // tight rows
   int maxlen = 0;
   int rate = 1;
-  const int* tile_tight = nullptr;  // per tile: tight (packed) index of its first row
+  const int4* tile_pos = nullptr;  // per tile: (tight index of its first row, utterance, first row inside it, 0)
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -274,30 +274,36 @@ __global__ void k_rvq(const int4* utt, const float* x, int ldx, const float* cb,
 
 // ------------------------------------------------------------------------------------------------
 // samplers
-__device__ __forceinline__ float noise_n(const float* noise, int64_t idx, uint64_t seed, uint64_t stream_id) {
-  return noise ? noise[idx] : philox_normal(seed, stream_id, (uint64_t)idx);
+// Injected noise is indexed by the tight row ti of the call; a Philox draw by the utterance's counter row g.row0 + t under
+// its key g.key (SeqDev::rng).  `per` draws per row, element j of the row.
+__device__ __forceinline__ float noise_n(const float* noise, int64_t ti, const UttRng& g, int t, int per, int j,
+                                         uint64_t stream_id) {
+  return noise ? noise[ti * per + j] : philox_normal(g.key, stream_id, (uint64_t)((int64_t)g.row0 + t) * per + j);
 }
-__device__ __forceinline__ float noise_u(const float* noise, int64_t idx, uint64_t seed, uint64_t stream_id) {
-  return noise ? noise[idx] : philox_uniform(seed, stream_id, (uint64_t)idx);
+__device__ __forceinline__ float noise_u(const float* noise, int64_t ti, const UttRng& g, int t, int per, int j,
+                                         uint64_t stream_id) {
+  return noise ? noise[ti * per + j] : philox_uniform(g.key, stream_id, (uint64_t)((int64_t)g.row0 + t) * per + j);
 }
 
-__global__ void k_mel_q_sample(const int4* utt, const float* coarse, int ldc, const float* noise, const float* smin,
-                               const float* smax, float sa, float s1a, float* x, int ldx, uint64_t seed, uint64_t sid) {
+__global__ void k_mel_q_sample(const int4* utt, const UttRng* rng, const float* coarse, int ldc, const float* noise,
+                               const float* smin, const float* smax, float sa, float s1a, float* x, int ldx, uint64_t sid) {
   ROW_SETUP();
+  const UttRng g = rng[b];
   for (int c = threadIdx.x; c < 80; c += 32) {
     if (!coarse) {  // ProDiff: x_T = randn, no coarse mel and no normalisation (prodiff.py:214-216)
-      x[r * ldx + c] = noise_n(noise, ti * 80 + c, seed, sid);
+      x[r * ldx + c] = noise_n(noise, ti, g, t, 80, c, sid);
       continue;
     }
     const float x0 = (coarse[r * ldc + c] - smin[c]) / (smax[c] - smin[c]) * 2.0f - 1.0f;
-    x[r * ldx + c] = sa * x0 + s1a * noise_n(noise, ti * 80 + c, seed, sid);
+    x[r * ldx + c] = sa * x0 + s1a * noise_n(noise, ti, g, t, 80, c, sid);
   }
 }
 // DDPM (shallow_diffusion_tts.py:145-162): eps -> clipped x0.  ProDiff (prodiff.py:135-148): the table holds (0, -1) in
 // slots 0-1 so x0 = eps exactly, and clip = 0.
-__global__ void k_mel_p_sample(const int4* utt, float* x, int ldx, const float* eps, int lde, const float* noise,
-                               const float* tab, uint64_t seed, uint64_t sid, int clip) {
+__global__ void k_mel_p_sample(const int4* utt, const UttRng* rng, float* x, int ldx, const float* eps, int lde,
+                               const float* noise, const float* tab, uint64_t sid, int clip) {
   ROW_SETUP();
+  const UttRng g = rng[b];
   const float a = tab[0], bq = tab[1], c1 = tab[2], c2 = tab[3], sig = tab[4];
   for (int c = threadIdx.x; c < 80; c += 32) {
     const float xt = x[r * ldx + c];
@@ -305,7 +311,7 @@ __global__ void k_mel_p_sample(const int4* utt, float* x, int ldx, const float* 
     if (clip) x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
     const float mean = c1 * x0 + c2 * xt;
     // reference: mean + nonzero_mask * exp(0.5*logvar) * noise ; sig already folds the mask
-    x[r * ldx + c] = mean + sig * noise_n(noise, ti * 80 + c, seed, sid);
+    x[r * ldx + c] = mean + sig * noise_n(noise, ti, g, t, 80, c, sid);
   }
 }
 // PLMS update (shallow_diffusion_tts.py:164-197).  prime = (w0*eps + w1*h1 + w2*h2 + w3*h3) / den; x_out = x + x_delta with
@@ -343,16 +349,17 @@ __device__ __forceinline__ float log_add_exp(float a, float b) {
   const float m = fmaxf(a, b);
   return m + logf(expf(a - m) + expf(b - m));
 }
-__global__ void k_f0_init(const int4* utt, float* z, int32_t* uv, const float* gnoise, uint64_t seed, uint64_t sid) {
+__global__ void k_f0_init(const int4* utt, const UttRng* rng, float* z, int32_t* uv, const float* gnoise, uint64_t sid) {
   ROW_SETUP();
   if (threadIdx.x == 0) {
-    z[r] = noise_n(gnoise, ti, seed, sid);
+    z[r] = noise_n(gnoise, ti, rng[b], t, 1, 0, sid);
     uv[r] = 0;  // log_sample_categorical over a size-1 class dim (gaussian_multinomial_diffusion.py:924-926)
   }
 }
 __global__ void k_f0_p_sample(const int4* utt, F0StepArgs a) {
   ROW_SETUP();
   if (threadIdx.x != 0) return;
+  const UttRng g = a.rng[b];
   const float ln2 = 0.69314718055994530942f;
   const float* o = a.out3 + r * a.ld3;
   // gaussian half (gaussian_p_sample, :325-333)
@@ -360,7 +367,7 @@ __global__ void k_f0_p_sample(const int4* utt, F0StepArgs a) {
   float x0 = a.gtab[0] * zt - a.gtab[1] * o[0];
   x0 = fmaxf(fminf(x0, a.hi[r]), a.lo[r]);
   const float mean = a.gtab[2] * x0 + a.gtab[3] * zt;
-  a.z[r] = mean + a.gtab[4] * noise_n(a.gnoise, ti, a.seed, a.gauss_stream);
+  a.z[r] = mean + a.gtab[4] * noise_n(a.gnoise, ti, g, t, 1, 0, a.gauss_stream);
   // multinomial half (p_pred / q_posterior, :374-413)
   const float l0a = o[1], l0b = o[2];
   const float mx = fmaxf(l0a, l0b);
@@ -379,8 +386,8 @@ __global__ void k_f0_p_sample(const int4* utt, F0StepArgs a) {
   const float m2 = fmaxf(u0, u1);
   const float lse2 = m2 + logf(expf(u0 - m2) + expf(u1 - m2));  // torch.logsumexp
   const float p0 = u0 - lse2, p1 = u1 - lse2;
-  const float r0 = noise_u(a.unoise, ti * 2 + 0, a.seed, a.unif_stream);
-  const float r1 = noise_u(a.unoise, ti * 2 + 1, a.seed, a.unif_stream);
+  const float r0 = noise_u(a.unoise, ti, g, t, 2, 0, a.unif_stream);
+  const float r1 = noise_u(a.unoise, ti, g, t, 2, 1, a.unif_stream);
   const float g0 = -logf(-logf(r0 + 1e-30f) + 1e-30f);
   const float g1 = -logf(-logf(r1 + 1e-30f) + 1e-30f);
   a.uv[r] = (g1 + p1) > (g0 + p0) ? 1 : 0;  // argmax, ties -> 0
@@ -493,15 +500,15 @@ __device__ double block_scan_incl(double v, double* sh, double& total) {
   return v + base;
 }
 
-__global__ void k_nsf_phase(const int4* utt1, const int4* utt256, const float* f0, const float* rand_ini, float* sines,
-                            uint64_t seed, int upp, float sr) {
+__global__ void k_nsf_phase(const int4* utt1, const int4* utt256, const UttRng* rng1, const float* f0, const float* rand_ini,
+                            float* sines, int upp, float sr) {
   // sines: tight [total256, 9] -> sin(2*pi*phase) (amplitude / uv / noise applied in k_nsf_merge)
   const int b = blockIdx.y, h = blockIdx.x;  // harmonic h in 0..8
   const int4 u1 = utt1[b], u2 = utt256[b];
   __shared__ double sh[16];
   const int N = u2.y;
   float ini = 0.f;
-  if (h > 0) ini = rand_ini ? rand_ini[b * 9 + h] : philox_uniform(seed, stream_voc_ini(b), (uint64_t)h);
+  if (h > 0) ini = rand_ini ? rand_ini[b * 9 + h] : philox_uniform(rng1[b].key, stream_voc_ini(rng1[b].ini), (uint64_t)h);
   double carry1 = 0.0, carry2 = 0.0;
   float prev_over = 0.f;  // tmp_over_one of the previous sample
   for (int n0 = 0; n0 < N; n0 += 256) {
@@ -536,12 +543,13 @@ __global__ void k_nsf_phase(const int4* utt1, const int4* utt256, const float* f
     prev_over = last;
   }
 }
-__global__ void k_nsf_merge(const int4* utt1, const int4* utt256, const float* f0, const float* sines, const float* noise,
-                            const float* lw, const float* lb, float* har, uint64_t seed, int upp) {
+__global__ void k_nsf_merge(const int4* utt1, const int4* utt256, const UttRng* rng256, const float* f0, const float* sines,
+                            const float* noise, const float* lw, const float* lb, float* har, int upp) {
   const int b = blockIdx.y;
   const int4 u1 = utt1[b], u2 = utt256[b];
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= u2.y) return;
+  const UttRng g = rng256[b];
   const float f = f0[(int64_t)u1.x + n / upp];
   const float uv = f > 0.f ? 1.f : 0.f;
   const float namp = uv * 0.003f + (1.0f - uv) * 0.1f / 3.0f;
@@ -550,7 +558,7 @@ __global__ void k_nsf_merge(const int4* utt1, const int4* utt256, const float* f
 #pragma unroll
   for (int h = 0; h < 9; ++h) {
     const float s = sines[ti * 9 + h] * 0.1f;
-    const float nz = namp * (noise ? noise[ti * 9 + h] : philox_normal(seed, stream_voc_src(), (uint64_t)(ti * 9 + h)));
+    const float nz = namp * noise_n(noise, ti, g, n, 9, h, stream_voc_src());
     acc = fmaf(s * uv + nz, lw[h], acc);
   }
   har[(int64_t)u2.x + n] = tanhf(acc);
@@ -831,13 +839,13 @@ int rvq_lookup(Ctx& ctx, const SeqDev& s, const float* x, int ldx, const float* 
   return 0;
 }
 int mel_q_sample(Ctx& ctx, const SeqDev& s, const float* coarse, int ldc, const float* noise, const float* smin,
-                 const float* smax, float sa, float s1a, float* x, int ldx, uint64_t seed, uint64_t sid) {
-  LAUNCH_ROWS(k_mel_q_sample, s, coarse, ldc, noise, smin, smax, sa, s1a, x, ldx, seed, sid);
+                 const float* smax, float sa, float s1a, float* x, int ldx, const UttRng* rng, uint64_t sid) {
+  LAUNCH_ROWS(k_mel_q_sample, s, rng, coarse, ldc, noise, smin, smax, sa, s1a, x, ldx, sid);
   return 0;
 }
 int mel_p_sample(Ctx& ctx, const SeqDev& s, float* x, int ldx, const float* eps, int lde, const float* noise,
-                 const float* tab, uint64_t seed, uint64_t sid, bool clip) {
-  LAUNCH_ROWS(k_mel_p_sample, s, x, ldx, eps, lde, noise, tab, seed, sid, clip ? 1 : 0);
+                 const float* tab, const UttRng* rng, uint64_t sid, bool clip) {
+  LAUNCH_ROWS(k_mel_p_sample, s, rng, x, ldx, eps, lde, noise, tab, sid, clip ? 1 : 0);
   return 0;
 }
 int plms_update(Ctx& ctx, const SeqDev& s, const PlmsArgs& a) {
@@ -853,8 +861,8 @@ int f0_p_sample(Ctx& ctx, const SeqDev& s, const F0StepArgs& a) {
   LAUNCH_ROWS(k_f0_p_sample, s, a);
   return 0;
 }
-int f0_init(Ctx& ctx, const SeqDev& s, float* z, int32_t* uv, const float* gnoise, uint64_t seed, uint64_t sid) {
-  LAUNCH_ROWS(k_f0_init, s, z, uv, gnoise, seed, sid);
+int f0_init(Ctx& ctx, const SeqDev& s, float* z, int32_t* uv, const float* gnoise, const UttRng* rng, uint64_t sid) {
+  LAUNCH_ROWS(k_f0_init, s, rng, z, uv, gnoise, sid);
   return 0;
 }
 int ddiff_input(Ctx& ctx, const SeqDev& s, const float* z, const int32_t* uv, const float* w, const float* b,
@@ -878,13 +886,13 @@ int pitch_glue_conv(Ctx& ctx, const SeqDev& s, const PitchGlueConvArgs& a) {
 size_t nsf_scratch_doubles(const SeqDev& s256) { return (size_t)(s256.total * 9 * sizeof(float) + 7) / 8 + 8; }
 
 int nsf_source(Ctx& ctx, const SeqDev& s1, const SeqDev& s256, const float* f0, const float* lw, const float* lb,
-               const float* rand_ini, const float* noise, float* har, double* scratch, uint64_t seed, int upp, float sr) {
+               const float* rand_ini, const float* noise, float* har, double* scratch, int upp, float sr) {
   if (ctx.dry || s1.B == 0) return 0;
   float* sines = reinterpret_cast<float*>(scratch);
-  k_nsf_phase<<<dim3(9, s1.B), 256, 0, ctx.stream>>>(s1.utt, s256.utt, f0, rand_ini, sines, seed, upp, sr);
+  k_nsf_phase<<<dim3(9, s1.B), 256, 0, ctx.stream>>>(s1.utt, s256.utt, s1.rng, f0, rand_ini, sines, upp, sr);
   SSB_CUDA(cudaGetLastError());
-  k_nsf_merge<<<dim3((s256.maxlen + 255) / 256, s1.B), 256, 0, ctx.stream>>>(s1.utt, s256.utt, f0, sines, noise, lw, lb,
-                                                                            har, seed, upp);
+  k_nsf_merge<<<dim3((s256.maxlen + 255) / 256, s1.B), 256, 0, ctx.stream>>>(s1.utt, s256.utt, s256.rng, f0, sines, noise,
+                                                                            lw, lb, har, upp);
   SSB_CUDA(cudaGetLastError());
   g_launches += 2;
   return 0;

@@ -78,10 +78,12 @@ int rvq_lookup(Ctx&, const SeqDev&, const float* x, int ldx, const float* codebo
 int codebook_norms(Ctx&, const float* codebooks, int n, float* out);  // ||c||^2 for n rows of 256
 
 // ---- samplers (a14, a19) ------------------------------------------------------------------------------
-// x = sqrt_ac * norm_spec(coarse) + sqrt_1m_ac * noise ; coarse == null (ProDiff): x = noise
+// x = sqrt_ac * norm_spec(coarse) + sqrt_1m_ac * noise ; coarse == null (ProDiff): x = noise.  Null noise draws Philox
+// stream_id with the key and counter base of each utterance's entry of `rng` (the layout's SeqDev::rng); so do the
+// other samplers.
 int mel_q_sample(Ctx&, const SeqDev&, const float* coarse, int ldc, const float* noise /*tight [total,80] or null*/,
-                 const float* spec_min, const float* spec_max, float sa, float s1a, float* x, int ldx,
-                 uint64_t seed, uint64_t stream_id);
+                 const float* spec_min, const float* spec_max, float sa, float s1a, float* x, int ldx, const UttRng* rng,
+                 uint64_t stream_id);
 // one reverse step: x <- c1*clamp(a*x - b*eps) + c2*x + sigma*noise
 struct PlmsArgs {  // one PLMS update over [rows, 80] guarded buffers (see k_plms_update)
   const float* x = nullptr;      // x_t
@@ -95,7 +97,7 @@ struct PlmsArgs {  // one PLMS update over [rows, 80] guarded buffers (see k_plm
 };
 int plms_update(Ctx&, const SeqDev&, const PlmsArgs&);
 int mel_p_sample(Ctx&, const SeqDev&, float* x, int ldx, const float* eps, int lde, const float* noise,
-                 const float* tab /*dev ptr to 8 floats for this t*/, uint64_t seed, uint64_t stream_id,
+                 const float* tab /*dev ptr to 8 floats for this t*/, const UttRng* rng, uint64_t stream_id,
                  bool clip = true /*false: ProDiff, x0 unclipped*/);
 int mel_denorm(Ctx&, const SeqDev&, const float* x, int ldx, const float* spec_min, const float* spec_max,
                const float* rowmask, float* mel_tight, int ld);
@@ -113,10 +115,11 @@ struct F0StepArgs {
   const float* mtab = nullptr;   // device, 8 floats for this t
   int t = 0;
   float log_eps = 0.f;           // fp32 log(1e-30)
-  uint64_t seed = 0, gauss_stream = 0, unif_stream = 0;  // Philox streams of this step (philox.cuh)
+  const UttRng* rng = nullptr;                  // Philox keys of the layout (SeqDev::rng)
+  uint64_t gauss_stream = 0, unif_stream = 0;  // Philox streams of this step (philox.cuh)
 };
 int f0_p_sample(Ctx&, const SeqDev&, const F0StepArgs&);
-int f0_init(Ctx&, const SeqDev&, float* z, int32_t* uv, const float* gnoise, uint64_t seed, uint64_t stream_id);
+int f0_init(Ctx&, const SeqDev&, float* z, int32_t* uv, const float* gnoise, const UttRng* rng, uint64_t stream_id);
 // DDiffNet input: x[r, c<C/2] = f0*w+b ; x[r, c>=C/2] = E_uv[uv]; y = x + d0
 int ddiff_input(Ctx&, const SeqDev&, const float* z, const int32_t* uv, const float* w, const float* b, const float* Euv,
                 const float* d0, float* x, float* y, int C, __half* yh = nullptr, __half* yl = nullptr);
@@ -150,10 +153,11 @@ struct PitchGlueConvArgs {
 int pitch_glue_conv(Ctx&, const SeqDev&, const PitchGlueConvArgs&);
 
 // ---- vocoder helpers (a20, a21) ---------------------------------------------------------------------------
-// harmonic source: f0 frames [rows1] -> har [rows256] (guarded at rate 256)
+// harmonic source: f0 frames [rows1] -> har [rows256] (guarded at rate 256); Philox keys: s1.rng (initial phase),
+// s256.rng (source noise)
 int nsf_source(Ctx&, const SeqDev& s1, const SeqDev& s256, const float* f0, const float* lin_w, const float* lin_b,
                const float* rand_ini /*[B,9] or null*/, const float* noise /*tight [total*256, 9] or null*/,
-               float* har, double* scratch, uint64_t seed, int upp, float sr);
+               float* har, double* scratch, int upp, float sr);
 size_t nsf_scratch_doubles(const SeqDev& s256);
 // x[r, n] += b[n] + sum_j w[n][j] * har[r*s - s/2 + j]   (noise_convs[i], kernel 2s stride s; s==1: kernel 1)
 int noise_conv_add(Ctx&, const SeqDev& sx, const SeqDev& s256, float* x, int ld, int C, const float* har, const float* w,

@@ -14,13 +14,17 @@
 //   vocoder NSF initial phase, utterance b < 8224  0x5151 + b          (else tag 8) counter h (harmonic 1..8)
 //   vocoder NSF source noise                   0x7171                                counter ti*9 + h
 // i.e. [1000, 2000), [2000, 10010), [20817, 29041), 29041, [102000, 110010), and every tagged id is >= 2^32, so no two
-// kinds share a stream whatever T, the batch size or the utterance index.  ti is the tight row (frame, or sample for
-// the vocoder source) of the whole call.
+// kinds share a stream whatever T, the batch size or the utterance index.  ti is the counter row: row0 + the row (frame,
+// or sample for the vocoder source) inside the utterance, and b the initial-phase stream index, both from the
+// utterance's entry of the layout's key table (UttRng, common.cuh), whose key is the Philox key of its draws.
 //
-// Batch composition.  With injected noise every utterance's result is independent of the batch it is in.  Philox draws
-// are indexed by the tight row of the call, so an utterance draws different noise in a different batch; the persistent
-// mel groups (ssb_model_set_persistent_groups) re-seed each group (seed + 0x9E3779B97F4A7C15 * group) and index rows
-// inside the group.
+// Batch composition.  With injected noise every utterance's result is independent of the batch it is in.  The key
+// table has two fillings (upload_layout), and the streams above are the same in both:
+//   one seed per call (Seq::seed): key = seed, row0 = the utterance's tight offset in the call, stream index b = the
+//     utterance's index, so an utterance draws different noise in a different batch.  The persistent mel groups
+//     (ssb_model_set_persistent_groups) key group g by seed + 0x9E3779B97F4A7C15 g and count rows inside the group;
+//   one seed per utterance (Seq::utt_seeds, the ssb_*_keyed entries): key = utt_seeds[b], row0 = 0, stream index 0,
+//     i.e. exactly the draws of a B = 1 call with seed utt_seeds[b] (which is group 0 of itself), whatever the batch.
 #pragma once
 #include <stdint.h>
 

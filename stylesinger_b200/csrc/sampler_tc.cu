@@ -90,8 +90,10 @@ __device__ __forceinline__ void prefetch32(const SPhase& e, int64_t r, int n, bo
   }
 }
 
-__device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t ti, int n, const uint32_t (&raw)[32],
-                                           const Pre& pre) {
+// ti: the row's tight index in the call (injected noise); g, lr: its utterance's Philox entry and its row inside the
+// utterance (Philox counter row g->row0 + lr)
+__device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t ti, const UttRng* g, int lr, int n,
+                                           const uint32_t (&raw)[32], const Pre& pre) {
   float v[32];
 #pragma unroll
   for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]) + __ldg(e.bias + n + j);
@@ -149,7 +151,7 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
     float x0 = __ldg(e.tab + 0) * zt - __ldg(e.tab + 1) * v[0];
     x0 = fmaxf(fminf(x0, __ldg(e.clip_hi + r)), __ldg(e.clip_lo + r));
     const float mean = __ldg(e.tab + 2) * x0 + __ldg(e.tab + 3) * zt;
-    const float gz = e.noise ? __ldg(e.noise + ti) : philox_normal(e.seed, e.stream_id, (uint64_t)ti);
+    const float gz = e.noise ? __ldg(e.noise + ti) : philox_normal(g->key, e.stream_id, (uint64_t)((int64_t)g->row0 + lr));
     const float zn = mean + __ldg(e.tab + 4) * gz;
     e.out[r] = zn;
     const float l0a = v[1], l0b = v[2];
@@ -170,8 +172,9 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
     const float m2 = fmaxf(u0, u1);
     const float lse2 = m2 + logf(expf(u0 - m2) + expf(u1 - m2));
     const float p0 = u0 - lse2, p1 = u1 - lse2;
-    const float r0 = e.noise2 ? __ldg(e.noise2 + ti * 2) : philox_uniform(e.seed, e.stream2, (uint64_t)(ti * 2));
-    const float r1 = e.noise2 ? __ldg(e.noise2 + ti * 2 + 1) : philox_uniform(e.seed, e.stream2, (uint64_t)(ti * 2 + 1));
+    const uint64_t gc = (uint64_t)((int64_t)g->row0 + lr) * 2;
+    const float r0 = e.noise2 ? __ldg(e.noise2 + ti * 2) : philox_uniform(g->key, e.stream2, gc);
+    const float r1 = e.noise2 ? __ldg(e.noise2 + ti * 2 + 1) : philox_uniform(g->key, e.stream2, gc + 1);
     const float g0 = -logf(-logf(r0 + 1e-30f) + 1e-30f);
     const float g1 = -logf(-logf(r1 + 1e-30f) + 1e-30f);
     const int cls = (g1 + p1) > (g0 + p0) ? 1 : 0;
@@ -234,7 +237,8 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
         float x0 = a * xt - bq * v[4 * q + k];
         x0 = fminf(fmaxf(x0, -lim), lim);
         const float mean = c1 * x0 + c2 * xt;
-        const float nz = e.noise ? __ldg(e.noise + ti * 80 + c) : philox_normal(e.seed, e.stream_id, (uint64_t)(ti * 80 + c));
+        const float nz = e.noise ? __ldg(e.noise + ti * 80 + c)
+                                 : philox_normal(g->key, e.stream_id, (uint64_t)((int64_t)g->row0 + lr) * 80 + c);
         xn[4 * q + k] = mean + sig * nz;
       }
       *reinterpret_cast<float4*>(e.out + r * e.ldo + n + 4 * q) = make_float4(xn[4 * q], xn[4 * q + 1], xn[4 * q + 2], xn[4 * q + 3]);
@@ -248,8 +252,8 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
 
 __global__ void __launch_bounds__(256, 1)
 sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict__ phases, int nphases,
-                  const int2* __restrict__ tiles, const int* __restrict__ tile_tight, int ntiles, unsigned* barrier_ctr,
-                  int cs) {
+                  const int2* __restrict__ tiles, const int4* __restrict__ tile_pos, const UttRng* __restrict__ rng,
+                  int ntiles, unsigned* barrier_ctr, int cs) {
   // cs = cluster size along N: the cs CTAs of a cluster work on the same M-tile (consecutive N-tiles); each loads
   // 1/cs of the A tile and TMA-multicasts it to all of them, so the activation planes cross L2->SM once per
   // cluster instead of once per CTA.  Stage recycling therefore needs every CTA of the cluster to have consumed
@@ -350,7 +354,10 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
         const int rl = ew * 32 + lane;
         const bool valid = rl < t.y;
         const int64_t r = (int64_t)t.x + rl;
-        const int64_t ti = (int64_t)tile_tight[mt] + rl;
+        const int4 tp = tile_pos[mt];  // tiles never straddle utterances
+        const int64_t ti = (int64_t)tp.x + rl;
+        const UttRng* ug = rng + tp.y;
+        const int lr = tp.z + rl;
         Pre cur, nxt;
         prefetch32(P, r, nt * BN, valid, cur);
         float acc0[BN / 2], acc1[BN / 2];  // rows [0, 64) and [64, 128) of the tile
@@ -409,7 +416,7 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
             v[4 * c] = __float_as_uint(x.x); v[4 * c + 1] = __float_as_uint(x.y);
             v[4 * c + 2] = __float_as_uint(x.z); v[4 * c + 3] = __float_as_uint(x.w);
           }
-          if (valid) epilogue32(P, r, ti, nt * BN + ch * 32, v, cur);
+          if (valid) epilogue32(P, r, ti, ug, lr, nt * BN + ch * 32, v, cur);
           cur = nxt;
         }
         named_sync(1, 128);  // staging buffer read by every thread before the next tile overwrites it
@@ -481,8 +488,9 @@ int sampler_tc_max_clusters(int cs) {
 
 int sampler_tc_max_ctas() { return sampler_tc_max_clusters(1); }
 
-int launch_sampler_tc(Ctx& ctx, const CUtensorMap* maps_dev, const SPhase* phases_dev, int nphases, const int2* tiles,
-                      const int* tile_tight, int ntiles, int max_nt, unsigned* barrier_ctr, int cs) {
+int launch_sampler_tc(Ctx& ctx, const CUtensorMap* maps_dev, const SPhase* phases_dev, int nphases, const SeqDev& s,
+                      int max_nt, unsigned* barrier_ctr, int cs) {
+  const int ntiles = s.ntiles;
   if (ctx.dry) return 0;
   const int cap = sampler_tc_max_clusters(cs);
   SSB_CHECK(cap > 0, "persistent sampler kernel cannot be resident on this device");
@@ -501,7 +509,8 @@ int launch_sampler_tc(Ctx& ctx, const CUtensorMap* maps_dev, const SPhase* phase
   at[1].id = cudaLaunchAttributeClusterDimension;
   at[1].val.clusterDim.x = (unsigned)cs; at[1].val.clusterDim.y = 1; at[1].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 2;
-  SSB_CUDA(cudaLaunchKernelEx(&cfg, sampler_tc_kernel, maps_dev, phases_dev, nphases, tiles, tile_tight, ntiles, barrier_ctr, cs));
+  SSB_CUDA(cudaLaunchKernelEx(&cfg, sampler_tc_kernel, maps_dev, phases_dev, nphases, s.tiles, s.tile_pos, s.rng, ntiles,
+                              barrier_ctr, cs));
   ++g_launches;
   return 0;
 }

@@ -32,7 +32,7 @@ struct SPhase {
   __half* sl;
   const float* tab;    // MEL_SAMPLE: 8 schedule scalars of this step
   const float* noise;  // MEL_SAMPLE: tight [total, 80] noise of this step, or null (Philox)
-  unsigned long long seed, stream_id;  // Philox stream of the Gaussian draws (philox.cuh)
+  unsigned long long stream_id;        // Philox stream of the Gaussian draws, keyed per utterance (SeqDev::rng)
   unsigned long long stream2;          // F0_SAMPLE: Philox stream of the uniform draws
   int n_valid;         // MEL_SAMPLE / SKIPPROJ: valid output columns
   int sync_after;      // 1: grid barrier after this entry; 0: the next entry is independent (e.g. the other F0 net)
@@ -54,8 +54,9 @@ struct SPhase {
 
 int sampler_tc_max_ctas();
 int sampler_tc_max_clusters(int cs);  // co-resident clusters of size cs (cooperative launch limit)
-int launch_sampler_tc(Ctx& ctx, const CUtensorMap* maps_dev, const SPhase* phases_dev, int nphases, const int2* tiles,
-                      const int* tile_tight, int ntiles, int max_nt, unsigned* barrier_ctr, int cs);
+// runs the phases over the row tiles of `s`; the sampling phases draw with s.rng
+int launch_sampler_tc(Ctx& ctx, const CUtensorMap* maps_dev, const SPhase* phases_dev, int nphases, const SeqDev& s,
+                      int max_nt, unsigned* barrier_ctr, int cs);
 int x80_planes(Ctx& ctx, const float* x, int64_t rows, __half* hi, __half* lo);
 
 }  // namespace ssb

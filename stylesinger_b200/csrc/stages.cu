@@ -51,30 +51,34 @@ int upload_layout(Ctx& c, const Seq& s, int rate, SeqDev* out) {
   const int nt = s.ntiles(rate);
   int2* tiles = c.alloc<int2>((size_t)nt + 1);
   int4* utt = c.alloc<int4>((size_t)s.B + 1);
-  int* ttight = c.alloc<int>((size_t)nt + 1);
-  out->tile_tight = ttight;
-  out->tiles = tiles; out->ntiles = nt; out->utt = utt; out->B = s.B; out->rows = s.rows(rate);
+  UttRng* rng = c.alloc<UttRng>((size_t)s.B + 1);
+  int4* tpos = c.alloc<int4>((size_t)nt + 1);
+  out->tile_pos = tpos;
+  out->tiles = tiles; out->ntiles = nt; out->utt = utt; out->rng = rng; out->B = s.B; out->rows = s.rows(rate);
   out->total = s.total * rate; out->maxlen = s.maxlen * rate; out->rate = rate;
   if (c.dry) return 0;
-  SSB_CHECK(!c.failed && tiles && utt, "workspace too small (layout tables)");
+  SSB_CHECK(!c.failed && tiles && utt && rng && tpos, "workspace too small (layout tables)");
   std::vector<int2> ht((size_t)nt + 1);
   std::vector<int4> hu((size_t)s.B + 1);
-  std::vector<int> htt((size_t)nt + 1);
+  std::vector<UttRng> hr((size_t)s.B + 1);
+  std::vector<int4> htp((size_t)nt + 1);
   int k = 0;
   int64_t tight = 0;
   for (int b = 0; b < s.B; ++b) {
     const int len = s.len[b] * rate;
     const int rs = s.rs[b] * rate;
     hu[b] = make_int4(rs, len, (int)tight, 0);
-    tight += len;
+    hr[b] = s.utt_seeds ? UttRng{s.utt_seeds[b], 0, 0} : UttRng{s.seed, (int32_t)tight, b};
     for (int t0 = 0; t0 < len; t0 += TILE_M) {
-      htt[k] = (int)(tight - len) + t0;
+      htp[k] = make_int4((int)tight + t0, b, t0, 0);
       ht[k++] = make_int2(rs + t0, (len - t0) < TILE_M ? (len - t0) : TILE_M);
     }
+    tight += len;
   }
-  SSB_CUDA(cudaMemcpyAsync(ttight, htt.data(), sizeof(int) * nt, cudaMemcpyHostToDevice, c.stream));
+  SSB_CUDA(cudaMemcpyAsync(tpos, htp.data(), sizeof(int4) * nt, cudaMemcpyHostToDevice, c.stream));
   SSB_CUDA(cudaMemcpyAsync(tiles, ht.data(), sizeof(int2) * nt, cudaMemcpyHostToDevice, c.stream));
   SSB_CUDA(cudaMemcpyAsync(utt, hu.data(), sizeof(int4) * s.B, cudaMemcpyHostToDevice, c.stream));
+  SSB_CUDA(cudaMemcpyAsync(rng, hr.data(), sizeof(UttRng) * s.B, cudaMemcpyHostToDevice, c.stream));
   // pageable-source async copies are staged before returning, so the host vectors may die here
   return 0;
 }
@@ -634,13 +638,12 @@ static int mel_k_step(const Model& m, int* K) {
 // x_K of the mel sampler.  DiffSinger: q_sample(norm_spec(coarse), K-1) on the T-step schedule
 // (shallow_diffusion_tts.py:298-302); ProDiff: randn (prodiff.py:214-216), no coarse mel.  Both draw block 0 of the
 // injected noise, or Philox stream_mel_xt().
-static int mel_init(Ctx& c, const Model& m, const SeqDev& s, const float* coarse_g, const float* noise, uint64_t seed,
-                    int K, float* xm) {
+static int mel_init(Ctx& c, const Model& m, const SeqDev& s, const float* coarse_g, const float* noise, int K, float* xm) {
   const Denoiser& d = m.melnet;
   if (m.mel_decoder == SSB_MEL_DECODER_PRODIFF)
-    return mel_q_sample(c, s, nullptr, 80, noise, nullptr, nullptr, 0.f, 0.f, xm, 80, seed, stream_mel_xt());
+    return mel_q_sample(c, s, nullptr, 80, noise, nullptr, nullptr, 0.f, 0.f, xm, 80, s.rng, stream_mel_xt());
   const float sa = c.dry ? 0.f : d.gtab_h[(size_t)(K - 1) * 8 + 5], s1a = c.dry ? 0.f : d.gtab_h[(size_t)(K - 1) * 8 + 6];
-  return mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, seed, stream_mel_xt());
+  return mel_q_sample(c, s, coarse_g, 80, noise, m.spec_min, m.spec_max, sa, s1a, xm, 80, s.rng, stream_mel_xt());
 }
 // x_0 -> mel_out.  DiffSinger: denorm_spec (shallow_diffusion_tts.py:305,274-275); ProDiff: denorm_spec is the identity
 // and mel_out is not masked (prodiff.py:221-222,228-229).
@@ -737,7 +740,7 @@ static void persistent_net_step(const PersistentNet& p, const SeqDev& s, int t, 
 
 // a18+a19, single launch: all K reverse steps (t = K-1 .. 0) of the mel DiffNet, K (2L + 3) phases.
 static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
-                                        const float* noise, uint64_t seed, int K, float* mel_tight) {
+                                        const float* noise, int K, float* mel_tight) {
   using P = PersistentNet;
   const Denoiser& d = m.melnet;
   const int C = d.C, L = d.L;
@@ -755,7 +758,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
   unsigned* ctr = c.alloc<unsigned>(4);
   WS_OK(c);
   const size_t per = (size_t)s.total * 80;
-  RUN(mel_init(c, m, s, coarse_g, noise, seed, K, xm));
+  RUN(mel_init(c, m, s, coarse_g, noise, K, xm));
   RUN(x80_planes(c, xm, s.rows, x80h, x80l));
   if (!c.dry) {
     std::vector<CUtensorMap> maps((size_t)nmaps);
@@ -774,13 +777,13 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
       q = sphase(1);  // output_projection -> eps ; fused DDPM posterior step on x_t
       q.a1 = net.mb + P::S; q.w1 = net.w_out(); q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE;
       q.bias = d.out_bias_pad; q.out = xm; q.ldo = 80; q.oh = x80h; q.ol = x80l; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
-      q.noise = noise ? noise + per * (size_t)(K - t) : nullptr; q.seed = seed; q.stream_id = stream_mel_step(t); q.n_valid = 80;
+      q.noise = noise ? noise + per * (size_t)(K - t) : nullptr; q.stream_id = stream_mel_step(t); q.n_valid = 80;
       q.no_clip = m.mel_decoder == SSB_MEL_DECODER_PRODIFF;
       ph.push_back(q);
     }
     SSB_CUDA(cudaMemcpyAsync(maps_dev, maps.data(), sizeof(CUtensorMap) * nmaps, cudaMemcpyHostToDevice, c.stream));
     SSB_CUDA(cudaMemcpyAsync(ph_dev, ph.data(), sizeof(SPhase) * nph, cudaMemcpyHostToDevice, c.stream));
-    RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s.tiles, s.tile_tight, s.ntiles, 2 * C / 64, ctr, CS));
+    RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s, 2 * C / 64, ctr, CS));
   }
   RUN(mel_finish(c, m, s, xm, mel_tight));
   c.release(mk);
@@ -790,8 +793,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
 // a18+a19: DiffusionDecoder.forward(infer=True) (shallow_diffusion_tts.py:284-307), or on a ProDiff model
 // ProDiffusion.forward(infer=True) (prodiff.py:204-222; coarse_g unused, pass null)
 int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
-                      const float* noise /*tight [(K+1), total, 80] or null*/, uint64_t seed, float* mel_tight,
-                      const Seq* host_seq) {
+                      const float* noise /*tight [(K+1), total, 80] or null*/, float* mel_tight, const Seq* host_seq) {
   const Denoiser& d = m.melnet;
   SSB_CHECK(d.T > 0, "mel schedule not set: call ssb_model_set_schedule(which=0)");
   int K = 0;
@@ -799,8 +801,9 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
   // ssb_model_set_persistent_groups(1): utterances are independent, so the K x L loop runs per GROUP of consecutive
   // utterances of <= 48 row tiles (a contiguous slice of the guard-banded layout: the sub-batch simply aliases the big
   // buffers), each by the single-launch persistent kernel (BASELINE.json configs[4]: persistent-kernel vs per-step-launch
-  // at batch 64).  Production (Philox) mode only - the injected-noise tensors are strided by the whole batch; each group
-  // gets its own seed.
+  // at batch 64).  Production (Philox) mode only - the injected-noise tensors are strided by the whole batch.  With one
+  // seed for the call each group g is keyed seed + 0x9E3779B97F4A7C15 g and counts its own rows; per-utterance seeds
+  // carry over as they are (philox.cuh, "Batch composition").
   if (host_seq && !noise && !c.dry && m.persistent_groups && m.persistent && s.ntiles > 48) {
     int b0 = 0;
     int64_t tight0 = 0;
@@ -817,12 +820,14 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
       for (int b = b0; b < b1; ++b) offs[(size_t)(b - b0) + 1] = offs[(size_t)(b - b0)] + host_seq->len[b];
       Seq q;
       q.build(offs.data(), b1 - b0);
+      q.seed = host_seq->seed + 0x9E3779B97F4A7C15ull * (uint64_t)gi;
+      q.utt_seeds = host_seq->utt_seeds ? host_seq->utt_seeds + b0 : nullptr;
       const size_t mkg = c.mark();
       SeqDev sg;
       RUN(upload_layout(c, q, 1, &sg));
       const int64_t row_off = (int64_t)host_seq->rs[b0] - GUARD;  // the sub-layout's row 0 inside the big buffers
       RUN(run_mel_diffusion(c, m, sg, cond_g + row_off * 256, coarse_g ? coarse_g + row_off * 80 : nullptr, nullptr,
-                            seed + 0x9E3779B97F4A7C15ull * (uint64_t)gi, mel_tight + tight0 * 80, nullptr));
+                            mel_tight + tight0 * 80, nullptr));
       c.release(mkg);
       tight0 += fr;
       b0 = b1;
@@ -832,7 +837,7 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
   }
   if (m.persistent && denoiser_tc_ok(m, d) && d.in_tc.ok && d.skip_tc.ok && d.out_tc.ok && s.ntiles <= 48 &&
       sampler_tc_max_ctas() > 0)
-    return run_mel_diffusion_persistent(c, m, s, cond_g, coarse_g, noise, seed, K, mel_tight);
+    return run_mel_diffusion_persistent(c, m, s, cond_g, coarse_g, noise, K, mel_tight);
   const size_t mk = c.mark();
   DenoiserBufs b;
   RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
@@ -841,11 +846,11 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
   RUN(prepare_cond(c, d, s, cond_g, b));
   const size_t per = (size_t)s.total * 80;
   const bool clip = m.mel_decoder != SSB_MEL_DECODER_PRODIFF;
-  RUN(mel_init(c, m, s, coarse_g, noise, seed, K, xm));
+  RUN(mel_init(c, m, s, coarse_g, noise, K, xm));
   for (int t = K - 1; t >= 0; --t) {
     RUN(mel_denoiser_eval(c, d, s, t, xm, b));
     const float* nz = noise ? noise + per * (size_t)(K - t) : nullptr;
-    RUN(mel_p_sample(c, s, xm, 80, b.head, b.ld_head, nz, d.gtab + (size_t)t * 8, seed, stream_mel_step(t), clip));
+    RUN(mel_p_sample(c, s, xm, 80, b.head, b.ld_head, nz, d.gtab + (size_t)t * 8, s.rng, stream_mel_step(t), clip));
   }
   RUN(mel_finish(c, m, s, xm, mel_tight));
   c.release(mk);
@@ -855,7 +860,7 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
 // f2 (SURVEY 8f): PLMS / PNDM sampler over the same denoiser (GaussianDiffusion.p_sample_plms + the pndm_speedup loop of
 // GaussianDiffusion.forward, shallow_diffusion_tts.py:164-197,254-260): K / interval evaluations (+1 for the first step).
 int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
-                           const float* q_noise /*tight [total, 80] or null*/, uint64_t seed, int interval, float* mel_tight) {
+                           const float* q_noise /*tight [total, 80] or null*/, int interval, float* mel_tight) {
   const Denoiser& d = m.melnet;
   SSB_CHECK(m.mel_decoder == SSB_MEL_DECODER_DIFFSINGER,
             "plms: the PLMS sampler needs a DiffSinger model (the ProDiff sampler predicts x0, not eps)");
@@ -872,7 +877,7 @@ int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float*
   WS_OK(c);
   RUN(prepare_cond(c, d, s, cond_g, b));
   auto acp = [&](int t) { return c.dry ? 0.5f : d.gtab_h[(size_t)t * 8 + 7]; };
-  RUN(mel_init(c, m, s, coarse_g, q_noise, seed, K, xm));
+  RUN(mel_init(c, m, s, coarse_g, q_noise, K, xm));
   int nh = 0;  // predictions in the history; hist[(head + k) % 3] is the k-th newest
   int head = 0;
   int t0 = 0;
@@ -916,8 +921,7 @@ int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float*
 // (stylesinger.py:223-225), so each phase of the table carries two entries (one per net, no barrier between them).
 static int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1,
                                             const float* lo, const float* hi, const float* const gnoise[2],
-                                            const float* const unoise[2], uint64_t seed, float* const z[2],
-                                            int32_t* const uv[2]) {
+                                            const float* const unoise[2], float* const z[2], int32_t* const uv[2]) {
   using P = PersistentNet;
   const int C = m.f0net[0].C, L = m.f0net[0].L, T = m.f0net[0].T;
   const int CS = 2;
@@ -933,7 +937,7 @@ static int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev
   const size_t per = (size_t)s.total;
   for (int n = 0; n < 2; ++n) {
     const Denoiser& d = m.f0net[n];
-    RUN(f0_init(c, s, z[n], uv[n], gnoise[n], seed, stream_f0_xt(n)));
+    RUN(f0_init(c, s, z[n], uv[n], gnoise[n], s.rng, stream_f0_xt(n)));
     RUN(ddiff_input(c, s, z[n], uv[n], d.in_w, d.in_b, d.uv_emb, d.dtab + (size_t)(T - 1) * L * C, net[n].x, nullptr, C,
                     net[n].pl[P::Y], net[n].pl[P::Y + 1]));
   }
@@ -951,7 +955,7 @@ static int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev
         q.tab = d.gtab + (size_t)t * 8; q.tab2 = d.mtab + (size_t)t * 8; q.tstep = t; q.log_eps = m.log_eps;
         q.noise = gnoise[n] ? gnoise[n] + per * (size_t)(T - t) : nullptr;
         q.noise2 = unoise[n] ? unoise[n] + per * 2 * (size_t)(T - 1 - t) : nullptr;
-        q.seed = seed; q.stream_id = stream_f0_gauss(n, t); q.stream2 = stream_f0_unif(n, t);
+        q.stream_id = stream_f0_gauss(n, t); q.stream2 = stream_f0_unif(n, t);
         q.has_next = t > 0; q.C = C; q.in_w = d.in_w; q.in_b = d.in_b; q.uv_emb = d.uv_emb; q.x_next = net[n].x;
         q.oh = net[n].pl[P::Y]; q.ol = net[n].pl[P::Y + 1]; q.ldh = C;
         q.vec2 = t > 0 ? d.dtab + (size_t)(t - 1) * L * C : nullptr;
@@ -976,7 +980,7 @@ static int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev
     }
     SSB_CUDA(cudaMemcpyAsync(maps_dev, maps.data(), sizeof(CUtensorMap) * nmaps, cudaMemcpyHostToDevice, c.stream));
     SSB_CUDA(cudaMemcpyAsync(ph_dev, ph.data(), sizeof(SPhase) * nph, cudaMemcpyHostToDevice, c.stream));
-    RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s.tiles, s.tile_tight, s.ntiles, 2 * (2 * C / 64), ctr, CS));
+    RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s, 2 * (2 * C / 64), ctr, CS));
   }
   c.release(mk);
   return 0;
@@ -992,7 +996,7 @@ static bool f0_pair_persistent_ok(const Model& m, const SeqDev& s) {
 
 // a13+a14: GaussianMultinomialDiffusion.sample (gaussian_multinomial_diffusion.py:921-942)
 int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const float* cond_g, const float* lo,
-                     const float* hi, const float* gnoise, const float* unoise, uint64_t seed, float* z, int32_t* uv) {
+                     const float* hi, const float* gnoise, const float* unoise, float* z, int32_t* uv) {
   const Denoiser& d = m.f0net[which];
   SSB_CHECK(d.T > 0, "f0 schedule not set: call ssb_model_set_schedule(which=1)");
   const size_t mk = c.mark();
@@ -1001,7 +1005,7 @@ int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const f
   RUN(prepare_cond(c, d, s, cond_g, b));
   const int T = d.T;
   const size_t per = (size_t)s.total;
-  RUN(f0_init(c, s, z, uv, gnoise, seed, stream_f0_xt(which)));
+  RUN(f0_init(c, s, z, uv, gnoise, s.rng, stream_f0_xt(which)));
   for (int t = T - 1; t >= 0; --t) {
     const float* dt = d.dtab + (size_t)t * d.L * d.C;
     RUN(ddiff_input(c, s, z, uv, d.in_w, d.in_b, d.uv_emb, dt, b.tc ? nullptr : b.x, b.y, d.C, b.yh, b.yl));
@@ -1011,7 +1015,7 @@ int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const f
     a.gnoise = gnoise ? gnoise + per * (size_t)(T - t) : nullptr;
     a.unoise = unoise ? unoise + per * 2 * (size_t)(T - 1 - t) : nullptr;
     a.gtab = d.gtab + (size_t)t * 8; a.mtab = d.mtab + (size_t)t * 8; a.t = t; a.log_eps = m.log_eps;
-    a.seed = seed; a.gauss_stream = stream_f0_gauss(which, t); a.unif_stream = stream_f0_unif(which, t);
+    a.rng = s.rng; a.gauss_stream = stream_f0_gauss(which, t); a.unif_stream = stream_f0_unif(which, t);
     RUN(f0_p_sample(c, s, a));
   }
   c.release(mk);
@@ -1019,9 +1023,9 @@ int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const f
 }
 
 int run_f0_samplers(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1, const float* lo,
-                    const float* hi, const float* const gnoise[2], const float* const unoise[2], uint64_t seed,
-                    float* const z[2], int32_t* const uv[2]) {
-  if (f0_pair_persistent_ok(m, s)) return run_f0_diffusion_pair_persistent(c, m, s, cond0, cond1, lo, hi, gnoise, unoise, seed, z, uv);
+                    const float* hi, const float* const gnoise[2], const float* const unoise[2], float* const z[2],
+                    int32_t* const uv[2]) {
+  if (f0_pair_persistent_ok(m, s)) return run_f0_diffusion_pair_persistent(c, m, s, cond0, cond1, lo, hi, gnoise, unoise, z, uv);
   // The two samplers are independent (stylesinger.py:223-225): run the second one on the model's auxiliary stream so
   // that their latency-bound dependent chains overlap.  Disjoint workspace regions.
   // Two streams only for small batches (latency-bound chains).  From ~8k frames on every GEMM fills the GPU on its
@@ -1033,12 +1037,12 @@ int run_f0_samplers(Ctx& c, const Model& m, const SeqDev& s, const float* cond0,
     SSB_CUDA(cudaStreamWaitEvent(m.aux_stream, m.ev_fork, 0));
   }
   const size_t off0 = c.off;
-  RUN(run_f0_diffusion(c, m, 0, s, cond0, lo, hi, gnoise[0], unoise[0], seed, z[0], uv[0]));
+  RUN(run_f0_diffusion(c, m, 0, s, cond0, lo, hi, gnoise[0], unoise[0], z[0], uv[0]));
   c.off = c.high;  // keep sampler 0's buffers alive: sampler 1 allocates above them
   {
     Ctx c2 = c;
     if (fork) c2.stream = m.aux_stream;
-    RUN(run_f0_diffusion(c2, m, 1, s, cond1, lo, hi, gnoise[1], unoise[1], seed, z[1], uv[1]));
+    RUN(run_f0_diffusion(c2, m, 1, s, cond1, lo, hi, gnoise[1], unoise[1], z[1], uv[1]));
     if (c2.high > c.high) c.high = c2.high;
     c.failed = c.failed || c2.failed;
   }
@@ -1057,7 +1061,7 @@ int run_f0_samplers(Ctx& c, const Model& m, const SeqDev& s, const float* cond0,
 // every conv), residuals / MRF accumulators stay fp32.  The narrow stage (C = 32) runs its ResBlocks through a
 // time-paired [rows/2, 64] view of the same memory with repacked weights (pack.cu, pack_conv_paired_tc).
 int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight, const float* f0_tight,
-                const float* rand_ini, const float* src_noise, uint64_t seed, float* wav_tight) {
+                const float* rand_ini, const float* src_noise, float* wav_tight) {
   const size_t mk0 = c.mark();
   int hop = 1;
   for (auto& st : v.stages) hop *= st.u;
@@ -1076,7 +1080,7 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
     const size_t mk = c.mark();
     double* scratch = c.alloc<double>(nsf_scratch_doubles(s256));
     WS_OK(c);
-    RUN(nsf_source(c, s1, s256, f0g, v.lin_w, v.lin_b, rand_ini, src_noise, har, scratch, seed, hop, (float)v.cfg.sample_rate));
+    RUN(nsf_source(c, s1, s256, f0g, v.lin_w, v.lin_b, rand_ini, src_noise, har, scratch, hop, (float)v.cfg.sample_rate));
     c.release(mk);
   }
   const bool tc = v.use_tc && tc_available();

@@ -57,19 +57,21 @@ int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, Denoiser
 int prepare_cond(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, DenoiserBufs& b);
 int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const float* x80, DenoiserBufs& b);
 int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBufs& b);
+// The samplers' Philox draws are keyed by the layout's table (SeqDev::rng, from Seq::seed / Seq::utt_seeds).
 // host_seq (optional): the host-side layout of `s`; needed for the utterance grouping of ssb_model_set_persistent_groups
 int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
-                      const float* noise, uint64_t seed, float* mel_tight, const Seq* host_seq = nullptr);
+                      const float* noise, float* mel_tight, const Seq* host_seq = nullptr);
 int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float* cond_g, const float* coarse_g,
-                           const float* q_noise, uint64_t seed, int interval, float* mel_tight);
+                           const float* q_noise, int interval, float* mel_tight);
 int run_f0_diffusion(Ctx& c, const Model& m, int which, const SeqDev& s, const float* cond_g, const float* lo,
-                     const float* hi, const float* gnoise, const float* unoise, uint64_t seed, float* z, int32_t* uv);
+                     const float* hi, const float* gnoise, const float* unoise, float* z, int32_t* uv);
 // both F0 samplers (agnostic: cond0, gnoise[0], ... ; specific: cond1, gnoise[1], ...)
 int run_f0_samplers(Ctx& c, const Model& m, const SeqDev& s, const float* cond0, const float* cond1, const float* lo,
-                    const float* hi, const float* const gnoise[2], const float* const unoise[2], uint64_t seed,
-                    float* const z[2], int32_t* const uv[2]);
+                    const float* hi, const float* const gnoise[2], const float* const unoise[2], float* const z[2],
+                    int32_t* const uv[2]);
+// seq.seed / seq.utt_seeds key the NSF source's draws
 int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight, const float* f0_tight,
-                const float* rand_ini, const float* src_noise, uint64_t seed, float* wav_tight);
+                const float* rand_ini, const float* src_noise, float* wav_tight);
 int denoiser_eval_api(Ctx& c, const Model& m, int which, const SeqDev& s, const float* x_tight, const int32_t* uv_tight,
                       int t, const float* cond_tight, float* out_tight);
 // ---- implicit-GEMM STFT pieces shared by the mel front-end and the vocoder output denoiser (frontend.cu) ----------------
@@ -89,7 +91,8 @@ std::vector<double> hann_window(int n_fft, int win);
 // 2 otherwise, i.e. irfft times the window of librosa.istft WITHOUT its 1/n_fft (the caller scales the GEMM's output).
 std::vector<float> dft_basis(int n_fft, int hop, int win, int nbp, bool inverse);
 
+// utt_seeds (host [B] or null): per-utterance Philox keys of the samplers; null keys them all by in.seed
 int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ssb_acoustic_outputs& out, bool durations_only,
-                 int32_t* dur_out, float* logdur_out);
+                 int32_t* dur_out, float* logdur_out, const uint64_t* utt_seeds = nullptr);
 
 }  // namespace ssb

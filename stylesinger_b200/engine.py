@@ -5,6 +5,7 @@ operation of the path runs in libstylesinger_b200.so (see include/stylesinger_b2
 """
 import ctypes as C
 import math
+import operator
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
 
@@ -33,6 +34,19 @@ def _ptr(t: Optional[torch.Tensor]):
     if not t.is_contiguous():
         raise ValueError("stylesinger_b200: tensors passed to the C ABI must be contiguous (call .contiguous())")
     return C.c_void_p(t.data_ptr())
+
+
+def utt_seeds(seeds, B) -> np.ndarray:
+    """One Philox seed per utterance -> host uint64 [B].  Each utterance then draws exactly the noise of a B = 1 call
+    with its seed, whatever batch it runs in (csrc/philox.cuh).  Raises ValueError for a length other than B or a seed
+    outside [0, 2**64), TypeError for a seed that is not an integer."""
+    s = [operator.index(v) for v in seeds]
+    if len(s) != B:
+        raise ValueError(f"seeds: expected one seed per utterance ({B}), got {len(s)}")
+    bad = [v for v in s if not 0 <= v < 2 ** 64]
+    if bad:
+        raise ValueError(f"seeds: every seed must be in [0, 2**64), got {bad[0]}")
+    return np.array(s, dtype=np.uint64)
 
 
 def _descs(named: Dict[str, torch.Tensor]):
@@ -281,10 +295,17 @@ class AcousticModel:
         return dur, logdur
 
     def forward(self, pb: PackedBatch, noise=None, seed=0, skip_mel_diffusion=False, dur=None,
-                want=("mel_out", "f0_denorm")):
+                want=("mel_out", "f0_denorm"), seeds=None):
         """StyleSinger.forward(infer=True). `pb` must carry frame_offsets (+ mel2ph, or pass `dur`).
-        Returns a dict of tight device tensors for the keys in `want`."""
+        Returns a dict of tight device tensors for the keys in `want`.
+        seeds: one seed per utterance (see utt_seeds) instead of `seed`: utterance b then gets the outputs of a B = 1
+        forward with seed=seeds[b].  Injected noise cannot be combined with it."""
         assert pb.frame_offsets is not None, "frame_offsets required (run predict_durations first)"
+        keys = None
+        if seeds is not None:
+            keys = utt_seeds(seeds, pb.B)
+            if noise and any(v is not None for v in noise.values()):
+                raise ValueError("seeds: per-utterance seeds key the in-kernel noise; injected noise must be None")
         a = self._inputs(pb, noise, seed, skip_mel_diffusion, dur)
         Fs, Ps, Rs = int(pb.frame_offsets[-1]), int(pb.ph_offsets[-1]), int(pb.ref_offsets[-1])
         shapes = {"mel_out": (Fs, 80), "f0_denorm": (Fs,), "encoder_out": (Ps, 256), "style": (Fs, 256),
@@ -306,8 +327,12 @@ class AcousticModel:
         if n == 0:
             check(-1, "ssb_acoustic_workspace_bytes")
         ws = self._ws.get(n)
-        check(lib.ssb_acoustic_forward(self._h, C.byref(a), C.byref(o), _ptr(ws), ws.numel(), self._stream()),
-              "ssb_acoustic_forward")
+        if keys is None:
+            check(lib.ssb_acoustic_forward(self._h, C.byref(a), C.byref(o), _ptr(ws), ws.numel(), self._stream()),
+                  "ssb_acoustic_forward")
+        else:
+            check(lib.ssb_acoustic_forward_keyed(self._h, C.byref(a), keys.ctypes.data, C.byref(o), _ptr(ws), ws.numel(),
+                                                 self._stream()), "ssb_acoustic_forward_keyed")
         return out
 
     def mel_diffusion(self, cond, coarse, frame_offsets, noise=None, seed=0):
@@ -493,14 +518,21 @@ class Vocoder:
 
     max_frames_per_call = 24000  # ~0.9 MB of stage buffers per frame: bounds the workspace to ~20 GB
 
-    def generate(self, mel, f0, frame_offsets, rand_ini=None, src_noise=None, seed=0, denoise_c=None):
+    def generate(self, mel, f0, frame_offsets, rand_ini=None, src_noise=None, seed=0, denoise_c=None, seeds=None):
         """mel [sumF,80], f0 [sumF] or None (device, tight) -> wav [sumF*hop] (device).
         Large batches are processed in groups of utterances (results are per-utterance, so grouping is exact).
         denoise_c: the denoiser strength for this call (None = the vocoder's own ``denoise_c``); > 0 denoises every group
-        in place right after it is generated."""
+        in place right after it is generated.
+        seeds: one seed per utterance (see utt_seeds) instead of `seed`: utterance b's wav is that of a B = 1 call with
+        seed=seeds[b], however the batch is grouped.  rand_ini / src_noise cannot be combined with it."""
         fo = np.ascontiguousarray(frame_offsets, np.int32)
         B = len(fo) - 1
         c = self.denoise_c if denoise_c is None else float(denoise_c)
+        keys = None
+        if seeds is not None:
+            keys = utt_seeds(seeds, B)
+            if rand_ini is not None or src_noise is not None:
+                raise ValueError("seeds: per-utterance seeds key the in-kernel noise; rand_ini / src_noise must be None")
         if B > 1 and int(fo[-1]) > self.max_frames_per_call:
             wav = torch.empty(int(fo[-1]) * self.hop, dtype=torch.float32, device=self.device)
             b0 = 0
@@ -512,7 +544,8 @@ class Vocoder:
                 a, e = int(fo[b0]), int(fo[b1])
                 w = self.generate(mel[a:e], None if f0 is None else f0[a:e], sub_fo,
                                   None if rand_ini is None else rand_ini[b0:b1].contiguous(),
-                                  None if src_noise is None else src_noise[a * self.hop:e * self.hop], seed + b0, c)
+                                  None if src_noise is None else src_noise[a * self.hop:e * self.hop], seed + b0, c,
+                                  None if keys is None else keys[b0:b1])
                 wav[a * self.hop:e * self.hop] = w
                 b0 = b1
             return wav
@@ -522,8 +555,13 @@ class Vocoder:
         ws = self._ws.get(n)
         wav = torch.empty(int(fo[-1]) * self.hop, dtype=torch.float32, device=self.device)
         stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-        check(lib.ssb_hifigan_generate(self._h, _ptr(mel), _ptr(f0), fo.ctypes.data, B, _ptr(rand_ini), _ptr(src_noise),
-                                       int(seed), _ptr(wav), _ptr(ws), ws.numel(), stream), "ssb_hifigan_generate")
+        if keys is None:
+            check(lib.ssb_hifigan_generate(self._h, _ptr(mel), _ptr(f0), fo.ctypes.data, B, _ptr(rand_ini),
+                                           _ptr(src_noise), int(seed), _ptr(wav), _ptr(ws), ws.numel(), stream),
+                  "ssb_hifigan_generate")
+        else:
+            check(lib.ssb_hifigan_generate_keyed(self._h, _ptr(mel), _ptr(f0), fo.ctypes.data, B, keys.ctypes.data,
+                                                 _ptr(wav), _ptr(ws), ws.numel(), stream), "ssb_hifigan_generate_keyed")
         if c > 0:  # hifigan_nsf.py:73-74: only a positive strength runs the denoiser
             if self._denoiser is None:
                 self._denoiser = WavDenoiser(self._denoise_hp if self._denoise_hp is not None else self.cfg, self.device)

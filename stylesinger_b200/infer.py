@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from ._lib import check, lib
-from .engine import AcousticModel, PackedBatch, Vocoder, pack_batch
+from .engine import AcousticModel, PackedBatch, Vocoder, pack_batch, utt_seeds
 from .formats import norm_interp_f0, pad_f0_to_mel
 from .hparams import resolve
 
@@ -145,12 +145,23 @@ class StyleSingerInfer:
         return (r[0][0], r[1][0]) if return_mel else r[0]
 
     # ---- batched path --------------------------------------------------------------------------------
-    def infer_batch(self, utts: List[dict], seed=0, use_mel2ph=True, return_mel=False):
-        return self.infer_packed(pack_batch(utts, use_mel2ph=use_mel2ph, pin=True), seed=seed, return_mel=return_mel)
+    def infer_batch(self, utts: List[dict], seed=0, use_mel2ph=True, return_mel=False, seeds=None):
+        """seeds: one seed per utterance instead of `seed`; utterance b then gets what forward_model(utts[b],
+        seed=seeds[b]) gives, whatever else the batch holds (see run_device)."""
+        if seeds is not None:  # validated before anything reaches the device
+            seeds = utt_seeds(seeds, len(utts))
+        return self.infer_packed(pack_batch(utts, use_mel2ph=use_mel2ph, pin=True), seed=seed, return_mel=return_mel,
+                                 seeds=seeds)
 
-    def run_device(self, pb_dev: PackedBatch, seed=0, noise=None, voc_noise=None):
+    def run_device(self, pb_dev: PackedBatch, seed=0, noise=None, voc_noise=None, seeds=None):
         """Device-resident ph -> mel -> wav: returns (mel [sumF,80] raw model output, f0 [sumF],
-        wav [sumF'*hop], frame_offsets of the wav) as device tensors."""
+        wav [sumF'*hop], frame_offsets of the wav) as device tensors.
+        seeds: one Philox seed per utterance (engine.utt_seeds) for the model and the vocoder alike, instead of the
+        call's `seed`; it cannot be combined with injected noise."""
+        if seeds is not None:
+            seeds = utt_seeds(seeds, pb_dev.B)
+            if noise or voc_noise:
+                raise ValueError("seeds: per-utterance seeds key the in-kernel noise; noise / voc_noise must be None")
         dur = None
         if pb_dev.frame_offsets is None:
             dur, _ = self.model.predict_durations(pb_dev)
@@ -158,7 +169,7 @@ class StyleSingerInfer:
             po = pb_dev.ph_offsets
             lens = [int(d[po[i]:po[i + 1]].sum()) for i in range(pb_dev.B)]
             pb_dev.frame_offsets = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
-        out = self.model.forward(pb_dev, noise=noise, seed=seed, dur=dur, want=("mel_out", "f0_denorm"))
+        out = self.model.forward(pb_dev, noise=noise, seed=seed, dur=dur, want=("mel_out", "f0_denorm"), seeds=seeds)
         mel, f0 = out["mel_out"], out["f0_denorm"]
         fo = pb_dev.frame_offsets
         n = int(fo[-1])
@@ -179,13 +190,15 @@ class StyleSingerInfer:
             melc, f0_v = melc[keep].contiguous(), f0[keep].contiguous()
         vn = voc_noise or {}
         wav = self.vocoder.generate(melc, f0_v if self.hparams.get("use_nsf") else None, fo_v,
-                                    rand_ini=vn.get("rand_ini"), src_noise=vn.get("src_noise"), seed=seed)
+                                    rand_ini=vn.get("rand_ini"), src_noise=vn.get("src_noise"), seed=seed, seeds=seeds)
         return mel, f0, wav, fo_v
 
-    def infer_packed(self, pb: PackedBatch, seed=0, return_mel=False, noise=None, voc_noise=None):
+    def infer_packed(self, pb: PackedBatch, seed=0, return_mel=False, noise=None, voc_noise=None, seeds=None):
         """Host buffers in, host buffers out (H2D of the inputs, D2H of the waveform)."""
+        if seeds is not None:  # validated before anything reaches the device
+            seeds = utt_seeds(seeds, pb.B)
         pb_dev = pb.to(self.device)
-        mel, f0, wav, fo_v = self.run_device(pb_dev, seed=seed, noise=noise, voc_noise=voc_noise)
+        mel, f0, wav, fo_v = self.run_device(pb_dev, seed=seed, noise=noise, voc_noise=voc_noise, seeds=seeds)
         wav_h = self._to_host(wav)
         hop = self.vocoder.hop
         wavs = [wav_h[fo_v[i] * hop:fo_v[i + 1] * hop] for i in range(pb_dev.B)]

@@ -17,7 +17,7 @@ from typing import Dict, List, Optional
 import numpy as np
 import torch
 
-from .engine import AcousticModel, PackedBatch, Vocoder, pack_batch
+from .engine import AcousticModel, PackedBatch, Vocoder, pack_batch, utt_seeds
 from .hparams import resolve
 
 
@@ -113,8 +113,14 @@ class StyleSinger:
 
     def forward(self, txt_tokens, mel2ph=None, spk_embed=None, emo_embed=None, ref_mels=None, ref_f0=None,
                 f0=None, uv=None, skip_decoder=False, global_steps=0, infer=False, note=None, note_dur=None,
-                note_type=None, seed=0, noise=None, **kwargs):
+                note_type=None, seed=0, noise=None, seeds=None, **kwargs):
+        """seeds: one seed per batch row instead of `seed` (AcousticModel.forward): row b then gets the outputs of the
+        B = 1 call with seed=seeds[b]."""
         hp = self.hparams
+        if seeds is not None:  # checked before anything reaches the device
+            seeds = utt_seeds(seeds, txt_tokens.shape[0])
+            if noise is not None:
+                raise ValueError("seeds: per-utterance seeds key the in-kernel noise; noise must be None")
         if not infer:
             raise NotImplementedError("stylesinger_b200 implements the inference path only (infer=True)")
         if f0 is not None or uv is not None:
@@ -144,7 +150,9 @@ class StyleSinger:
             want.append("mel_out" if run_diff else "coarse_mel")
         if callable(noise):  # parity hooks: the injected draws depend on the (possibly predicted) frame count
             noise = noise(pb.frame_offsets)
-        out = self.engine.forward(pb, noise=noise, seed=seed, skip_mel_diffusion=not run_diff, dur=dur, want=tuple(want))
+        keyed = {} if seeds is None else {"seeds": seeds}
+        out = self.engine.forward(pb, noise=noise, seed=seed, skip_mel_diffusion=not run_diff, dur=dur, want=tuple(want),
+                                  **keyed)
         fo = pb.frame_offsets
         m2p = packed_to_padded(out["mel2ph"].long(), fo)
         ret["mel2ph"] = m2p

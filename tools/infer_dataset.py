@@ -4,10 +4,15 @@ ragged batches and writes one wav per item.  Equivalent of `python tasks/run.py 
 (tasks/StyleSinger/stylesinger.py:168-275, which asserts B=1).
 
     python tools/infer_dataset.py --ckpt checkpoints/StyleSinger --vocoder checkpoints/hifigan --data data/binary/x/test \
-        --out infer_out [--batch 64] [--T 100] [--k-step 50] [--limit N] [--use-gt-dur] [--vocoder-denoise-c 0.1]
+        --out infer_out [--batch 64] [--T 100] [--k-step 50] [--limit N] [--use-gt-dur] [--vocoder-denoise-c 0.1] \
+        [--seed S] [--seed-per-item]
 
 Like the reference's test_step (tasks/StyleSinger/stylesinger.py:177-180 with `use_gt_dur: false` in egs/stylesinger.yaml) the
 durations come from the duration predictor unless --use-gt-dur is given (then the items' ground-truth mel2ph is fed).
+
+By default each batch draws its noise from one seed (--seed plus the batch's start), so an item's audio depends on
+--batch, --limit and the dataset's size.  --seed-per-item gives item i (its index in the dataset) the seed --seed + i:
+its wav is then that of StyleSingerInfer.forward_model(item, seed=--seed + i), whatever the batching.
 """
 import argparse
 import os
@@ -16,6 +21,11 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def item_seeds(seed, idx):
+    """--seed-per-item: the per-utterance seeds of the dataset items `idx`."""
+    return [seed + i for i in idx]
 
 
 def main():
@@ -30,6 +40,8 @@ def main():
                     help="reference hparam K_step (shallow diffusion): mel reverse steps from q_sample at K-1; default --T")
     ap.add_argument("--limit", type=int, default=0)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--seed-per-item", action="store_true",
+                    help="seed item i with --seed + i, so that its audio does not depend on the batching")
     ap.add_argument("--use-gt-dur", action="store_true", help="feed the items' ground-truth mel2ph (reference hparam use_gt_dur)")
     ap.add_argument("--vocoder-denoise-c", type=float, default=0.0,
                     help="reference hparam vocoder_denoise_c: > 0 denoises every waveform (hifigan_nsf.py:14-22,73-74)")
@@ -55,7 +67,10 @@ def main():
         for b0 in range(0, n, args.batch):
             idx = order[b0:b0 + args.batch]
             utts = [formats.item_to_utterance(ds[i], hp, with_mel2ph=args.use_gt_dur) for i in idx]
-            wavs = eng.infer_batch(utts, seed=args.seed + b0, use_mel2ph=args.use_gt_dur)
+            if args.seed_per_item:
+                wavs = eng.infer_batch(utts, seeds=item_seeds(args.seed, idx), use_mel2ph=args.use_gt_dur)
+            else:
+                wavs = eng.infer_batch(utts, seed=args.seed + b0, use_mel2ph=args.use_gt_dur)
             for i, u, w in zip(idx, utts, wavs):
                 name = str(u.get("item_name") or f"item{i}")
                 wavfile.write(os.path.join(args.out, name + ".wav"), sr, np.asarray(w, np.float32))

@@ -342,7 +342,8 @@ int ssb_melspec_create(ssb_melspec_t** out, int32_t sample_rate, int32_t fft_siz
                        int32_t n_mels, float fmin, float fmax, float eps);
 /* Same front-end with the defaults of librosa.feature.melspectrogram selectable, which is what the emotion encoder's features
  * are (data_gen/tts/emotion/audio.py:43-55: sr 16000, n_fft 400, hop 160, 40 mels, fmin 0, fmax sr / 2): pad_reflect != 0 =
- * np.pad "reflect" centring instead of zeros (needs more than n_fft / 2 samples per utterance, like numpy), power != 0 = |X|^2
+ * np.pad "reflect" centring instead of zeros (reflected as often as the pad needs, like numpy; an empty utterance is refused,
+ * as numpy refuses it), power != 0 = |X|^2
  * instead of |X|, take_log == 0 = no log10 / eps.  n_fft need not be a multiple of hop_size here (the frame is embedded in
  * the next multiple of 2 hop_size rows with zero weights).  ssb_melspec_create = (..., 0, 0, 1). */
 int ssb_melspec_create_ex(ssb_melspec_t** out, int32_t sample_rate, int32_t fft_size, int32_t hop_size, int32_t win_length,

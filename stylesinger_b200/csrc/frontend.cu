@@ -100,21 +100,30 @@ std::vector<float> dft_basis(int n_fft, int hop, int win, int nbp, bool inverse)
 
 namespace {
 
-// np.pad(y, n_fft / 2, mode="reflect") of librosa.stft's default centring: sample -i is y[i], sample n - 1 + i is y[n - 1 - i].
+// np.pad(y, n_fft / 2, mode="reflect") of librosa.stft's default centring.  numpy reflects as often as the pad needs, i.e.
+// sample p (p < 0 or p >= n) is the even periodic extension of y with period 2 (n - 1): sample -i is y[i], sample n - 1 + i
+// is y[n - 1 - i] while i < n, and a 1-sample clip pads with y[0].  (numpy refuses n == 0; so does run_melspec.)
+__device__ __forceinline__ int64_t reflect_src(int64_t p, int64_t n) {
+  if (n == 1) return 0;
+  const int64_t per = 2 * (n - 1);
+  int64_t q = p % per;
+  if (q < 0) q += per;
+  return q < n ? q : per - q;
+}
 // Written into the guard rows in front of the utterance and behind its last sample (pad <= 8 rows each side; the 16 guard
-// rows between neighbours keep the two utterances' pads apart).  Like numpy, needs n > pad.
+// rows between neighbours keep the two utterances' pads apart).
 __global__ void k_wav_reflect(const int4* utt, const int32_t* sample_offs, const float* wav, int hop, int pad, float* rows) {
   const int b = blockIdx.y;
   const int4 u = utt[b];
   const int64_t n = (int64_t)sample_offs[b + 1] - sample_offs[b];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;  // 0 .. 2 pad: [0, pad) = left pad, [pad, 2 pad) = right pad
-  if (i >= 2 * pad || n <= pad) return;
+  if (i >= 2 * pad || n == 0) return;
   const float* y = wav + sample_offs[b];
   if (i < pad) {
-    rows[(int64_t)u.x * hop - 1 - i] = y[1 + i];
+    rows[(int64_t)u.x * hop - 1 - i] = y[reflect_src(-1 - (int64_t)i, n)];
   } else {
     const int j = i - pad;
-    rows[(int64_t)u.x * hop + n + j] = y[n - 2 - j];
+    rows[(int64_t)u.x * hop + n + j] = y[reflect_src(n + j, n)];
   }
 }
 // |re + i im| for the [rows, 2 * nbp] (re | im) spectrum; columns >= nbins are padding (zero weights -> zero)
@@ -149,6 +158,9 @@ double mel_to_hz(double m) {
 }
 
 int run_melspec(Ctx& c, const ssb_melspec& m, const Seq& q, const float* wav, const int32_t* sample_offsets_host, int B, float* mel_out) {
+  if (m.reflect)  // before any copy or launch, and in the dry run that sizes the workspace
+    for (int b = 0; b < B; ++b)
+      SSB_CHECK(sample_offsets_host[b + 1] > sample_offsets_host[b], "reflect padding needs at least one sample per utterance (numpy refuses an empty array)");
   SeqDev s;
   RUN(upload_layout(c, q, 1, &s));
   int32_t* offs_dev = c.alloc<int32_t>((size_t)B + 1);
@@ -162,8 +174,6 @@ int run_melspec(Ctx& c, const ssb_melspec& m, const Seq& q, const float* wav, co
   RUN(wav_rows(c, s, offs_dev, wav, m.hop, rows));
   if (m.reflect) {
     const int pad = m.n_fft / 2;
-    for (int b = 0; b < B; ++b)
-      SSB_CHECK((int64_t)sample_offsets_host[b + 1] - sample_offsets_host[b] > pad, "reflect padding needs more than n_fft / 2 samples per utterance");
     k_wav_reflect<<<dim3((unsigned)((2 * pad + 255) / 256), (unsigned)B), 256, 0, c.stream>>>(s.utt, offs_dev, wav, m.hop, pad, rows);
     SSB_CUDA(cudaGetLastError());
     ++g_launches;
@@ -270,7 +280,10 @@ size_t ssb_melspec_workspace_bytes(const ssb_melspec_t* m, const int32_t* sample
 
 int ssb_melspec_forward(const ssb_melspec_t* m, const float* wav, const int32_t* sample_offsets, int32_t B, float* mel_out,
                         void* workspace, size_t workspace_bytes, void* stream) {
-  SSB_CHECK(m && wav && sample_offsets && mel_out && workspace && B >= 0, "bad argument");
+  SSB_CHECK(m && sample_offsets && workspace && B >= 0, "bad argument");
+  // an empty tensor may have no storage: no samples in the batch need no waveform pointer, no utterance no output
+  SSB_CHECK(wav || sample_offsets[B] == sample_offsets[0], "null waveform");
+  SSB_CHECK(mel_out || B == 0, "null output");
   Ctx c;
   c.base = (char*)workspace; c.cap = workspace_bytes; c.stream = (cudaStream_t)stream;
   Seq q;

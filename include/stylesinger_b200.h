@@ -83,6 +83,24 @@ typedef struct {
   int32_t sample_rate;
 } ssb_vocoder_config;
 
+/* ssb_vocoder_config plus the ResBlock type (config key 'resblock', modules/hifigan/hifigan_nsf.py:115):
+ *   1: ResBlock1 (:30-66), 3 dilations per block (res_dilations[j][0..2]), convs1.{m} / convs2.{m} per dilation;
+ *   2: ResBlock2 (:69-90), 2 dilations per block (res_dilations[j][0..1]; [j][2] is unread), convs.{m} per dilation.
+ * This covers the three published HiFi-GAN layouts: V1 (512 initial channels, ResBlock1), V2 (128, ResBlock1) and
+ * V3 (256, ResBlock2). */
+typedef struct {
+  int32_t n_up;
+  int32_t up_rates[8];
+  int32_t up_kernels[8];
+  int32_t initial_channel;
+  int32_t n_res;
+  int32_t res_kernels[4];
+  int32_t res_dilations[4][3];
+  int32_t use_pitch_embed;
+  int32_t sample_rate;
+  int32_t resblock; /* 1 or 2 */
+} ssb_vocoder_config_ex;
+
 int ssb_version(void);
 const char* ssb_last_error(void);
 
@@ -285,6 +303,17 @@ int ssb_rvq_lookup(const ssb_model_t* m, const float* x /*[sumR,256]*/, const in
 int ssb_vocoder_create(ssb_vocoder_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_vocoder_config* cfg);
 void ssb_vocoder_free(ssb_vocoder_t* v);
 
+/* HifiGanGenerator of any ResBlock type (HifiGanGenerator.__init__, modules/hifigan/hifigan_nsf.py:104-142, picks
+ * ResBlock1 or ResBlock2 at :115 from the checkpoint's config, tasks/tts/vocoder_infer/hifigan_nsf.py:24-60).
+ * ssb_vocoder_create(out, t, n, cfg) == ssb_vocoder_create_ex with the same fields and resblock = 1.
+ * ResBlock2 reads "resblocks.{i*n_res+j}.convs.{m}.{weight_g,weight_v,bias}", m = 0, 1 (:72-79), and runs
+ * x = convs[m](leaky_relu(x, 0.1)) + x (:82-87).  Stage i has initial_channel / 2^(i+1) channels: a multiple of 32, or
+ * 16 or 8 (HiFi-GAN V2's last two stages).  The ResBlock convs of a 16- or 8-channel stage run as 64-channel convs over
+ * groups of 64 / C consecutive samples, so the stage's cumulative upsampling rate prod(up_rates[0..i]) must be a multiple
+ * of 64 / C.  Fails, naming the cause and leaving *out NULL, before anything is allocated when resblock is not 1 or 2, a
+ * read dilation is below 1, or a stage's channel count or rate breaks the rules above. */
+int ssb_vocoder_create_ex(ssb_vocoder_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_vocoder_config_ex* cfg);
+
 /* HifiGAN.spec2wav / HifiGanGenerator.forward (tasks/tts/vocoder_infer/hifigan_nsf.py:62-75,
  * modules/hifigan/hifigan_nsf.py:144-169).  mel [sumF,80] (already masked/clipped as
  * inference/StyleSinger.py:56-58 does), f0 [sumF] Hz or NULL.  rand_ini [B,9] / src_noise [sumF*hop, 9]:
@@ -304,7 +333,8 @@ int ssb_hifigan_generate_keyed(const ssb_vocoder_t* v, const float* mel, const f
  * (3 MMAs per product, fp32 accumulate; default when available), 0 = fp32 FFMA.  Returns the mode in effect. */
 int ssb_model_set_tensor_cores(ssb_model_t* m, int32_t enable);
 
-/* Same switch for the vocoder's wide stages (C % 64 == 0). */
+/* Same switch for the vocoder's ResBlock convs (wide stages with C % 64 == 0, and the grouped 32-, 16- and 8-channel
+ * stages). */
 int ssb_vocoder_set_tensor_cores(ssb_vocoder_t* v, int32_t enable);
 
 /* 1 (default): small batches run the whole T-step mel sampler in ONE persistent cooperative kernel launch

@@ -32,6 +32,11 @@ class VocoderConfig(C.Structure):
                 ("res_dilations", (C.c_int32 * 3) * 4), ("use_pitch_embed", C.c_int32), ("sample_rate", C.c_int32)]
 
 
+class VocoderConfigEx(C.Structure):
+    """ssb_vocoder_config_ex: the VocoderConfig fields plus the ResBlock type (1 or 2)."""
+    _fields_ = VocoderConfig._fields_ + [("resblock", C.c_int32)]
+
+
 class AcousticInputs(C.Structure):
     _fields_ = [("B", C.c_int32),
                 ("ph_offsets", C.c_void_p), ("frame_offsets", C.c_void_p), ("ref_offsets", C.c_void_p),
@@ -69,6 +74,7 @@ EXPORTS = [
     "ssb_wav_denoise_set_tensor_cores",
     "ssb_model_set_mel_k_step",
     "ssb_acoustic_forward_keyed", "ssb_hifigan_generate_keyed",
+    "ssb_vocoder_create_ex",
 ]
 
 
@@ -105,6 +111,7 @@ def _load():
         "ssb_f0_diffusion_sample": (C.c_int, [vp, i32, vp, vp, vp, vp, i32, vp, vp, u64, vp, vp, vp, sz, vp]),
         "ssb_rvq_lookup": (C.c_int, [vp, vp, vp, i32, vp, vp, vp, sz, vp]),
         "ssb_vocoder_create": (C.c_int, [P(vp), P(TensorDesc), i32, P(VocoderConfig)]),
+        "ssb_vocoder_create_ex": (C.c_int, [P(vp), P(TensorDesc), i32, P(VocoderConfigEx)]),
         "ssb_vocoder_free": (None, [vp]),
         "ssb_vocoder_workspace_bytes": (sz, [vp, vp, i32]),
         "ssb_hifigan_generate": (C.c_int, [vp, vp, vp, vp, i32, vp, vp, u64, vp, vp, sz, vp]),

@@ -670,6 +670,56 @@ int ssb_rvq_lookup(const ssb_model_t* m, const float* x, const int32_t* ref_offs
 
 int ssb_vocoder_create(ssb_vocoder_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_vocoder_config* cfg) {
   SSB_CHECK(out && tensors && cfg, "ssb_vocoder_create: null argument");
+  ssb_vocoder_config_ex ex;
+  memset(&ex, 0, sizeof(ex));
+  ex.n_up = cfg->n_up;
+  memcpy(ex.up_rates, cfg->up_rates, sizeof(ex.up_rates));
+  memcpy(ex.up_kernels, cfg->up_kernels, sizeof(ex.up_kernels));
+  ex.initial_channel = cfg->initial_channel;
+  ex.n_res = cfg->n_res;
+  memcpy(ex.res_kernels, cfg->res_kernels, sizeof(ex.res_kernels));
+  memcpy(ex.res_dilations, cfg->res_dilations, sizeof(ex.res_dilations));
+  ex.use_pitch_embed = cfg->use_pitch_embed;
+  ex.sample_rate = cfg->sample_rate;
+  ex.resblock = 1;
+  return ssb_vocoder_create_ex(out, tensors, n, &ex);
+}
+
+// The layout rules of ssb_vocoder_create_ex, checked on the config alone (before any allocation)
+static int check_vocoder_config(const ssb_vocoder_config_ex& cfg) {
+  const std::string w = "ssb_vocoder_create: ";
+  SSB_CHECK(cfg.resblock == 1 || cfg.resblock == 2,
+            w + "resblock must be 1 (ResBlock1) or 2 (ResBlock2), got " + std::to_string(cfg.resblock));
+  SSB_CHECK(cfg.n_up >= 1 && cfg.n_up <= 8 && cfg.n_res >= 1 && cfg.n_res <= 4, w + "vocoder: unsupported config");
+  const int nd = cfg.resblock == 1 ? 3 : 2;  // ResBlock1 reads dilation[0..2], ResBlock2 dilation[0..1]
+  for (int j = 0; j < cfg.n_res; ++j)
+    for (int m = 0; m < nd; ++m)
+      SSB_CHECK(cfg.res_dilations[j][m] >= 1, w + "dilation " + std::to_string(cfg.res_dilations[j][m]) + " of resblock " +
+                                                  std::to_string(j) + " (entry " + std::to_string(m) + ") is below 1");
+  int rate = 1;
+  for (int i = 0; i < cfg.n_up; ++i) {
+    SSB_CHECK(cfg.up_rates[i] >= 1, w + "upsample rate " + std::to_string(i) + " is below 1");
+    rate *= cfg.up_rates[i];
+    const int div = 2 << i;
+    const int C = cfg.initial_channel / div;
+    SSB_CHECK(cfg.initial_channel > 0 && cfg.initial_channel % div == 0 && (C % 32 == 0 || C == 16 || C == 8),
+              w + "stage " + std::to_string(i) + " has initial_channel / 2^" + std::to_string(i + 1) + " = " +
+                  std::to_string(cfg.initial_channel) + " / " + std::to_string(div) +
+                  " channels: it must be a multiple of 32, or 16 or 8");
+    if (C < 32)
+      SSB_CHECK(rate % (64 / C) == 0, w + "stage " + std::to_string(i) + " has " + std::to_string(C) +
+                                          " channels and cumulative upsampling rate " + std::to_string(rate) +
+                                          ", which is not a multiple of 64 / " + std::to_string(C) +
+                                          " (its ResBlock convs run over groups of that many samples)");
+  }
+  return 0;
+}
+
+int ssb_vocoder_create_ex(ssb_vocoder_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_vocoder_config_ex* cfg) {
+  SSB_CHECK(out, "ssb_vocoder_create: null argument");
+  *out = nullptr;
+  SSB_CHECK(tensors && cfg, "ssb_vocoder_create: null argument");
+  if (check_vocoder_config(*cfg)) return -1;
   TensorMap tm;
   if (to_map(tensors, n, &tm)) return -1;
   ssb_vocoder* v = new ssb_vocoder();

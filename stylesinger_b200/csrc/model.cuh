@@ -165,16 +165,21 @@ struct VocStage {
   int u = 1, Cout = 0;
   float *nc_w = nullptr, *nc_b = nullptr; int nc_s = 1;  // noise conv
   float* nc_wt = nullptr;                                 // the same weights as [K, C] (tiled kernel)
-  struct RB { Dense c1[3], c2[3]; } rb[4];  // paired stage: the tensor-core halves hold the time-paired packing
-  bool res_tc = false;  // all ResBlock convs of this stage are tensor-core eligible (C % 64 == 0)
-  bool paired = false;  // C == 32: ResBlock convs packed as 64-channel convs over PAIRS of time steps (see pack.cu)
+  // ResBlock1: convs1.{m} / convs2.{m} in c1[m] / c2[m]; ResBlock2: convs.{m} in c1[m] (c2 unused).  A grouped stage
+  // (g > 1) holds the grouped packing in the tensor-core halves, and at C < 32 in the FFMA halves as well.
+  struct RB { Dense c1[3], c2[3]; } rb[4];
+  bool res_tc = false;  // all ResBlock convs of this stage have a tensor-core packing (C % 64 == 0, or grouped)
+  // time-group factor 64 / C (C = 32, 16, 8): the ResBlock convs are packed as 64-channel convs over groups of g
+  // consecutive time steps, i.e. over the [rows/g, 64] view of the [rows, C] buffers (see pack.cu); 1: not grouped
+  int g = 1;
 };
 struct Vocoder {
   DevicePool pool;
-  ssb_vocoder_config cfg;
+  ssb_vocoder_config_ex cfg;
   Conv pre, post;
   std::vector<VocStage> stages;
   int nk = 3;
+  int resblock = 1;  // 1: ResBlock1 (3 conv pairs per block), 2: ResBlock2 (2 single convs per block)
   float *lin_w = nullptr, *lin_b = nullptr;
   bool nsf = true;
   bool use_tc = true;
@@ -191,7 +196,7 @@ int pack_dense(DevicePool& pool, const HostTensor* w, const HostTensor* b, int d
 int pack_conv_transpose(DevicePool& pool, const HostTensor* v, const HostTensor* g, const HostTensor* b, int u, Conv* out);
 int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder = SSB_MEL_DECODER_DIFFSINGER,
                 int f0_gen = SSB_F0_GEN_GMDIFF);
-int build_vocoder(TensorMap& tm, const ssb_vocoder_config& cfg, Vocoder* v);
+int build_vocoder(TensorMap& tm, const ssb_vocoder_config_ex& cfg, Vocoder* v);
 int set_schedule(Model* m, int which, int T, const float* step_emb, const float* gtab, const float* mtab,
                  cudaStream_t stream);
 

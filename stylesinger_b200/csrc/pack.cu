@@ -75,9 +75,10 @@ static void fold_weight_norm(const HostTensor* v, const HostTensor* g, std::vect
   }
 }
 
+// cin16: the layer runs on conv_gemm, which takes Cin % 16 == 0 only (false: a layer only the vocoder's conv_post_tanh reads)
 static int pack_from_host(DevicePool& pool, const float* w, int N, int Cin, int k, const float* b, int dil, PackMode mode,
-                          Conv* out) {
-  SSB_CHECK(Cin % 16 == 0, "pack: Cin must be a multiple of 16");
+                          Conv* out, bool cin16 = true) {
+  SSB_CHECK(!cin16 || Cin % 16 == 0, "pack: Cin must be a multiple of 16");
   const int Npad = (N + 3) & ~3;
   std::vector<float> W((size_t)k * Cin * Npad, 0.f), B((size_t)Npad, 0.f);
   for (int n = 0; n < N; ++n) {
@@ -93,8 +94,8 @@ static int pack_from_host(DevicePool& pool, const float* w, int N, int Cin, int 
   return 0;
 }
 
-int pack_conv(DevicePool& pool, const HostTensor* w, const HostTensor* b, int dil, PackMode mode, Conv* out,
-              const HostTensor* g) {
+static int pack_conv_impl(DevicePool& pool, const HostTensor* w, const HostTensor* b, int dil, PackMode mode, Conv* out,
+                          const HostTensor* g, bool cin16) {
   if (!w) return -1;
   SSB_CHECK(w->shape.size() == 3 || w->shape.size() == 2, "pack_conv: weight must be [N,Cin,k] or [N,Cin]");
   const int N = (int)w->shape[0], Cin = (int)w->shape[1], k = w->shape.size() == 3 ? (int)w->shape[2] : 1;
@@ -104,7 +105,12 @@ int pack_conv(DevicePool& pool, const HostTensor* w, const HostTensor* b, int di
     fold_weight_norm(w, g, folded);
     src = folded.data();
   }
-  return pack_from_host(pool, src, N, Cin, k, b ? b->data : nullptr, dil, mode, out);
+  return pack_from_host(pool, src, N, Cin, k, b ? b->data : nullptr, dil, mode, out, cin16);
+}
+
+int pack_conv(DevicePool& pool, const HostTensor* w, const HostTensor* b, int dil, PackMode mode, Conv* out,
+              const HostTensor* g) {
+  return pack_conv_impl(pool, w, b, dil, mode, out, g, true);
 }
 
 // Tensor-core packing: W[tap][n'][c] as fp16 hi/lo planes (n' = permuted output column), + TMA maps.
@@ -155,39 +161,59 @@ int pack_dense(DevicePool& pool, const HostTensor* w, const HostTensor* b, int d
   t.shape = {nrows, Cin, k};
   return pack_conv_tc(pool, &t, dil, mode, out->f.bias, &out->t);
 }
-// Narrow convs (C = 32) on the 64-wide tensor-core K block: view [rows, 32] as [rows/2, 64] (two consecutive time
-// steps per "super row", super channel = phase*32 + c).  y[2q+phi, n] = sum_j sum_c W[n][c][j] x[2q + phi + s_j, c]
-// with s_j = (j - cen)*d becomes a conv over super rows with taps delta = floor((phi + s_j)/2) and input phase
-// (phi + s_j) mod 2:  W'[delta][phi'*32 + c][phi*32 + n] = W[n][c][j].  Half of each 64x64 block is zero, which the
-// tensor cores absorb easily (the fp32 FFMA kernel ran these convs at ~15 TFLOP/s).
-static int pack_conv_paired_tc(DevicePool& pool, const HostTensor* v, const HostTensor* g, int dil, const float* bias_host,
-                               ConvTC* out, float** bias_pair) {
+// Narrow convs (C = 64 / G channels, G = 2, 4, 8) on the 64-wide K block: view [rows, C] as [rows/G, 64] (G consecutive
+// time steps per "super row", super channel = phase*C + c).  y[Gq+phi, n] = sum_j sum_c W[n][c][j] x[Gq + phi + s_j, c]
+// with s_j = (j - cen)*d becomes a conv over super rows:
+//  * G does not divide d: taps delta = floor((phi + s_j)/G) with input phase (phi + s_j) mod G, the dense tap range
+//    [-ceil(cen*d/G), ceil(cen*d/G)] at dilation 1:  W'[delta][phi'*C + c][phi*C + n] = W[n][c][j];
+//  * G divides d: s_j moves every phase by the same (j - cen)*d/G super rows, so the conv keeps its k taps at dilation
+//    d/G and is block-diagonal over the phases:  W'[j][phi*C + c][phi*C + n] = W[n][c][j]  (7 taps instead of up to 37
+//    for HiFi-GAN V3's dilation 12 at C = 32).
+// Most of each 64x64 block is zero, which the tensor cores absorb easily (the fp32 FFMA kernel ran the C = 32 convs at
+// ~15 TFLOP/s ungrouped).  The tensor-core packing goes to out->t; with ffma also the FFMA one to out->f (C = 16, 8:
+// conv_gemm takes Cin % 16 == 0, and one grouped path serves both GEMMs).  At G = 2 a shape the packing does not take
+// (an even kernel) leaves out->t.ok false and the stage runs ungrouped on FFMA; at G > 2 it is an error.
+static int pack_conv_grouped(DevicePool& pool, const HostTensor* v, const HostTensor* g, int dil, int G, const float* bias_host,
+                             bool ffma, Dense* out) {
   if (!v || !g) return -1;
-  const int N = (int)v->shape[0], Cin = (int)v->shape[1], k = (int)v->shape[2];
-  if (N != 32 || Cin != 32 || k % 2 == 0) return 0;
+  const int C = 64 / G;
+  const int N = (int)v->shape[0], Cin = (int)v->shape[1], k = v->shape.size() == 3 ? (int)v->shape[2] : 0;
+  const bool ok = v->shape.size() == 3 && N == C && Cin == C && k % 2 == 1;
+  if (!ok && G == 2) return 0;
+  SSB_CHECK(ok, "ssb_vocoder_create: a ResBlock conv of a " + std::to_string(C) + "-channel stage must be [" +
+                    std::to_string(C) + ", " + std::to_string(C) + ", k] with k odd");
   std::vector<float> w;
   fold_weight_norm(v, g, w);
-  const int cen = (k - 1) / 2, reach = cen * dil;
-  auto fdiv2 = [](int a) { return a >= 0 ? a / 2 : -((-a + 1) / 2); };  // floor(a / 2)
-  const int dmin = fdiv2(-reach), dmax = fdiv2(1 + reach), taps = dmax - dmin + 1;
+  const int cen = (k - 1) / 2;
+  const bool dilated = dil % G == 0;
+  auto fdiv = [G](int a) { return a >= 0 ? a / G : -((-a + G - 1) / G); };  // floor(a / G)
+  const int dmin = dilated ? -cen : fdiv(-cen * dil), dmax = dilated ? cen : fdiv(G - 1 + cen * dil);
+  const int taps = dmax - dmin + 1;
   std::vector<float> t((size_t)64 * 64 * taps, 0.f);  // torch conv layout [N'=64][Cin'=64][taps]
-  for (int phi = 0; phi < 2; ++phi)
+  for (int phi = 0; phi < G; ++phi)
     for (int j = 0; j < k; ++j) {
       const int s = (j - cen) * dil;
-      const int delta = fdiv2(phi + s), ph_in = (phi + s) - 2 * delta;
-      for (int n = 0; n < 32; ++n)
-        for (int c = 0; c < 32; ++c)
-          t[((size_t)(phi * 32 + n) * 64 + (ph_in * 32 + c)) * taps + (delta - dmin)] = w[((size_t)n * 32 + c) * k + j];
+      const int delta = dilated ? j - cen : fdiv(phi + s), ph_in = dilated ? phi : (phi + s) - G * delta;
+      for (int n = 0; n < C; ++n)
+        for (int c = 0; c < C; ++c)
+          t[((size_t)(phi * C + n) * 64 + (ph_in * C + c)) * taps + (delta - dmin)] = w[((size_t)n * C + c) * k + j];
     }
+  const int dil_g = dilated ? dil / G : 1;
   std::vector<float> b2(64, 0.f);
   if (bias_host)
-    for (int i = 0; i < 64; ++i) b2[i] = bias_host[i % 32];
-  *bias_pair = pool.upload(b2);
+    for (int i = 0; i < 64; ++i) b2[i] = bias_host[i % C];
+  const float* bias_dev = nullptr;
+  if (ffma) {
+    if (pack_from_host(pool, t.data(), 64, 64, taps, b2.data(), dil_g, PACK_PLAIN, &out->f)) return -1;
+    bias_dev = out->f.bias;
+  } else {
+    bias_dev = pool.upload(b2);
+  }
   HostTensor ht;
   ht.data = t.data();
   ht.shape = {64, 64, taps};
-  if (pack_conv_tc(pool, &ht, 1, PACK_PLAIN, *bias_pair, out)) return -1;
-  if (out->ok && out->center != -dmin) return -1;  // symmetric by construction
+  if (pack_conv_tc(pool, &ht, dil_g, PACK_PLAIN, bias_dev, &out->t)) return -1;
+  if (out->t.ok && out->t.center != -dmin) return -1;  // symmetric by construction
   return 0;
 }
 
@@ -528,12 +554,14 @@ fail:
   return -1;
 }
 
-int build_vocoder(TensorMap& tm, const ssb_vocoder_config& cfg, Vocoder* v) {
+int build_vocoder(TensorMap& tm, const ssb_vocoder_config_ex& cfg, Vocoder* v) {
   DevicePool& pool = v->pool;
   v->cfg = cfg;
   v->nk = cfg.n_res;
+  v->resblock = cfg.resblock;
   v->nsf = cfg.use_pitch_embed != 0;
   SSB_CHECK(cfg.n_up >= 1 && cfg.n_up <= 8 && cfg.n_res >= 1 && cfg.n_res <= 4, "vocoder: unsupported config");
+  SSB_CHECK(cfg.resblock == 1 || cfg.resblock == 2, "vocoder: resblock must be 1 or 2");
   PK(pack_conv(pool, tm.get("conv_pre.weight_v"), tm.get("conv_pre.bias"), 1, PACK_PLAIN, &v->pre, tm.get("conv_pre.weight_g")));
   v->stages.resize(cfg.n_up);
   {
@@ -549,7 +577,6 @@ int build_vocoder(TensorMap& tm, const ssb_vocoder_config& cfg, Vocoder* v) {
       SSB_CHECK(cfg.up_kernels[i] == 2 * cfg.up_rates[i] || cfg.up_kernels[i] - cfg.up_rates[i] >= 0, "vocoder: bad upsample kernel");
       PK(pack_conv_transpose(pool, tm.get(u + "weight_v"), tm.get(u + "weight_g"), tm.get(u + "bias"), s.u, &s.up.f));
       PK(pack_conv_transpose_tc(pool, tm.get(u + "weight_v"), tm.get(u + "weight_g"), s.u, s.up.f.bias, &s.up.t));
-      s.res_tc = true;
       prod_after /= s.u;
       if (v->nsf) {
         const std::string n = "noise_convs." + std::to_string(i) + ".";
@@ -566,30 +593,48 @@ int build_vocoder(TensorMap& tm, const ssb_vocoder_config& cfg, Vocoder* v) {
           }
         }
       }
+      // C = 32, 16, 8: time-grouped packing (pack_conv_grouped).  At C = 32 the FFMA GEMM runs the convs as they are and
+      // only the tensor-core packing is grouped; at C = 16 and 8 both are (ssb_vocoder_create_ex checked the stage rate).
+      const int G = s.Cout < 64 && 64 % s.Cout == 0 ? 64 / s.Cout : 1;
+      s.g = G;
+      s.res_tc = true;
+      const int nconv = cfg.resblock == 1 ? 3 : 2;
       for (int j = 0; j < cfg.n_res; ++j) {
-        const int k = cfg.res_kernels[j];
-        (void)k;
-        for (int mI = 0; mI < 3; ++mI) {
+        for (int mI = 0; mI < nconv; ++mI) {
+          // ResBlock1 (hifigan_nsf.py:30-66): convs1.{m} at dilation d[m], then convs2.{m} at 1; ResBlock2 (:69-90): convs.{m}
           const std::string q = "resblocks." + std::to_string(i * cfg.n_res + j) + ".";
-          const std::string a = q + "convs1." + std::to_string(mI) + ".", b2 = q + "convs2." + std::to_string(mI) + ".";
-          PK(pack_dense(pool, tm.get(a + "weight_v"), tm.get(a + "bias"), cfg.res_dilations[j][mI], PACK_PLAIN, &s.rb[j].c1[mI], tm.get(a + "weight_g")));
-          PK(pack_dense(pool, tm.get(b2 + "weight_v"), tm.get(b2 + "bias"), 1, PACK_PLAIN, &s.rb[j].c2[mI], tm.get(b2 + "weight_g")));
-          if (!s.rb[j].c1[mI].t.ok || !s.rb[j].c2[mI].t.ok) s.res_tc = false;
-          if (s.Cout == 32) {  // narrow stage: time-paired packing instead
-            const HostTensor* b1 = tm.get(a + "bias");
-            const HostTensor* b3 = tm.get(b2 + "bias");
-            float* bp = nullptr;
-            PK(pack_conv_paired_tc(pool, tm.get(a + "weight_v"), tm.get(a + "weight_g"), cfg.res_dilations[j][mI], b1 ? b1->data : nullptr, &s.rb[j].c1[mI].t, &bp));
-            PK(pack_conv_paired_tc(pool, tm.get(b2 + "weight_v"), tm.get(b2 + "weight_g"), 1, b3 ? b3->data : nullptr, &s.rb[j].c2[mI].t, &bp));
-            if (mI == 0 && j == 0) s.paired = true;
-            if (!s.rb[j].c1[mI].t.ok || !s.rb[j].c2[mI].t.ok) s.paired = false;
+          struct { std::string p; int dil; Dense* d; } cv[2];
+          int ncv = 0;
+          if (cfg.resblock == 1) {
+            cv[ncv++] = {q + "convs1." + std::to_string(mI) + ".", cfg.res_dilations[j][mI], &s.rb[j].c1[mI]};
+            cv[ncv++] = {q + "convs2." + std::to_string(mI) + ".", 1, &s.rb[j].c2[mI]};
+          } else {
+            cv[ncv++] = {q + "convs." + std::to_string(mI) + ".", cfg.res_dilations[j][mI], &s.rb[j].c1[mI]};
+          }
+          if (G <= 2) {  // the ungrouped packing (C = 32: the FFMA path's)
+            for (int x = 0; x < ncv; ++x)
+              PK(pack_dense(pool, tm.get(cv[x].p + "weight_v"), tm.get(cv[x].p + "bias"), cv[x].dil, PACK_PLAIN, cv[x].d,
+                            tm.get(cv[x].p + "weight_g")));
+            if (G == 1)
+              for (int x = 0; x < ncv; ++x)
+                if (!cv[x].d->t.ok) s.res_tc = false;
+          }
+          if (G > 1) {
+            for (int x = 0; x < ncv; ++x) {
+              const HostTensor* b = tm.get(cv[x].p + "bias");
+              PK(pack_conv_grouped(pool, tm.get(cv[x].p + "weight_v"), tm.get(cv[x].p + "weight_g"), cv[x].dil, G,
+                                   b ? b->data : nullptr, G > 2, cv[x].d));
+              if (!cv[x].d->t.ok) s.res_tc = false;
+            }
           }
         }
       }
       c /= 2;
     }
   }
-  PK(pack_conv(pool, tm.get("conv_post.weight_v"), tm.get("conv_post.bias"), 1, PACK_PLAIN, &v->post, tm.get("conv_post.weight_g")));
+  // conv_post runs on conv_post_tanh (C % 4 == 0): no conv_gemm Cin % 16 rule, so V2's 8-channel last stage packs too
+  PK(pack_conv_impl(pool, tm.get("conv_post.weight_v"), tm.get("conv_post.bias"), 1, PACK_PLAIN, &v->post,
+                    tm.get("conv_post.weight_g"), false));
   if (v->nsf) {
     v->lin_w = upload_tensor(pool, tm.get("m_source.l_linear.weight", {1, 9}));
     v->lin_b = upload_tensor(pool, tm.get("m_source.l_linear.bias", {1}));

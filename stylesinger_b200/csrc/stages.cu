@@ -1058,8 +1058,10 @@ int run_f0_samplers(Ctx& c, const Model& m, const SeqDev& s, const float* cond0,
 // a20/a21: HifiGanGenerator.forward (hifigan_nsf.py:144-169)
 // Stages whose channel counts are multiples of 64 run on the tensor-core kernel: every conv input is carried as
 // fp16 hi/lo planes of leaky_relu(x) written by the producing epilogue (the reference applies leaky_relu before
-// every conv), residuals / MRF accumulators stay fp32.  The narrow stage (C = 32) runs its ResBlocks through a
-// time-paired [rows/2, 64] view of the same memory with repacked weights (pack.cu, pack_conv_paired_tc).
+// every conv), residuals / MRF accumulators stay fp32.  The narrow stages (C = 32, 16, 8) run their ResBlocks through a
+// time-grouped [rows/g, 64] view of the same memory with repacked weights, g = 64 / C (pack.cu, pack_conv_grouped).
+// ResBlock1 (hifigan_nsf.py:30-66): r = c2(lrelu(c1(lrelu(r)))) + r three times; ResBlock2 (:69-90): r = c(lrelu(r)) + r
+// twice.  The last conv of each block adds into the MRF accumulator (x 1/nk on the last block).
 int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight, const float* f0_tight,
                 const float* rand_ini, const float* src_noise, float* wav_tight) {
   const size_t mk0 = c.mark();
@@ -1109,14 +1111,17 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
     SeqDev so;
     RUN(upload_layout(c, seq, rate_out, &so));
     const bool up_tc = tc && st.up.t.ok && pin_h != nullptr;
-    const bool paired = tc && st.paired && (rate_out % 2 == 0);
-    const bool res_tc = tc && (st.res_tc || paired);
-    // paired stage: [rows, 32] is processed as [rows/2, 64] (same memory) with the time-paired weight packing
+    // grouped stage: [rows, C] is processed as [rows/g, 64] (same memory) with the time-grouped weight packing.  At C = 32
+    // only on tensor cores (the FFMA GEMM takes the 32-channel convs as they are); at C = 16 and 8 on both paths
+    // (ssb_vocoder_create_ex checked rate_out % g == 0 there).
+    const bool grouped = st.g > 1 && rate_out % st.g == 0 && (st.g > 2 || (tc && st.res_tc));
+    const int g = grouped ? st.g : 1;
+    const bool res_tc = tc && st.res_tc && (st.g == 1 || grouped);
     SeqDev sw = so;
-    const int Cw = paired ? 2 * Co : Co;
-    if (paired) {
-      RUN(upload_layout(c, seq, rate_out / 2, &sw));
-      sw.rows = so.rows / 2;  // exactly the memory of the [so.rows, Co] buffers (TMA zero-fills beyond)
+    const int Cw = g * Co;
+    if (grouped) {
+      RUN(upload_layout(c, seq, rate_out / g, &sw));
+      sw.rows = so.rows / g;  // exactly the memory of the [so.rows, Co] buffers (TMA zero-fills beyond)
     }
     const bool next_up_tc = tc && i + 1 < v.stages.size() && v.stages[i + 1].up.t.ok;
     float* xu = alloc_rows(c, so, Co);
@@ -1125,11 +1130,12 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
     float* xt = nullptr;
     __half *px_h = nullptr, *px_l = nullptr, *pt_h = nullptr, *pt_l = nullptr, *pr_h = nullptr, *pr_l = nullptr;
     __half *pa_h = nullptr, *pa_l = nullptr;
+    const bool rb2 = v.resblock == 2;  // ResBlock2 has no inner conv pair: no xt
     if (res_tc) {
       px_h = alloc_half_rows(c, so, Co); px_l = alloc_half_rows(c, so, Co);
-      pt_h = alloc_half_rows(c, so, Co); pt_l = alloc_half_rows(c, so, Co);
+      if (!rb2) { pt_h = alloc_half_rows(c, so, Co); pt_l = alloc_half_rows(c, so, Co); }
       pr_h = alloc_half_rows(c, so, Co); pr_l = alloc_half_rows(c, so, Co);
-    } else {
+    } else if (!rb2) {
       xt = alloc_rows(c, so, Co);
     }
     if (next_up_tc) { pa_h = alloc_half_rows(c, so, Co); pa_l = alloc_half_rows(c, so, Co); }
@@ -1145,19 +1151,20 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
       RUN(run_dense(c, st.up, up_tc, sin, {xin, C, pin_h, pin_l, ACT_LRELU, 0.1f}, e));
     }
     if (nsf) RUN(noise_conv_add(c, so, s256, xu, Co, Co, har, st.nc_w, st.nc_b, st.nc_s, res_tc ? px_h : nullptr, px_l, 0.1f, st.nc_wt));
+    const int nconv = rb2 ? 2 : 3;
     for (int j = 0; j < v.nk; ++j) {  // MRF: mean of the resblocks
       const float* rin = xu;
       const __half *rin_h = px_h, *rin_l = px_l;
-      for (int mI = 0; mI < 3; ++mI) {
-        const bool last = (mI == 2);
+      for (int mI = 0; mI < nconv; ++mI) {
+        const bool last = (mI == nconv - 1);
         const bool lastj = (j == v.nk - 1);
-        {  // xt = c1(leaky_relu(r)) ; on tensor cores only leaky_relu(xt) is ever consumed -> planes only
+        if (!rb2) {  // xt = c1(leaky_relu(r)) ; on tensor cores only leaky_relu(xt) is ever consumed -> planes only
           Epi e;
           if (res_tc) lrelu_planes(e, pt_h, pt_l, Cw);
           else { e.out = xt; e.ldo = Cw; }
           RUN(run_dense(c, st.rb[j].c1[mI], res_tc, sw, {rin, Cw, rin_h, rin_l, ACT_LRELU, 0.1f}, e));
         }
-        Epi e;  // r = c2(leaky_relu(xt)) + r
+        Epi e;  // ResBlock1: r = c2(leaky_relu(xt)) + r ; ResBlock2: r = c(leaky_relu(r)) + r
         e.res = rin; e.ld_res = Cw;
         if (!last) {
           e.out = r; e.ldo = Cw;
@@ -1166,7 +1173,8 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
           e.out = acc; e.ldo = Cw; e.accum = (j > 0); e.gamma = lastj ? 1.0f / (float)v.nk : 1.0f;
           if (lastj && next_up_tc) lrelu_planes(e, pa_h, pa_l, Cw);
         }
-        RUN(run_dense(c, st.rb[j].c2[mI], res_tc, sw, {xt, Cw, pt_h, pt_l, ACT_LRELU, 0.1f}, e));
+        if (rb2) RUN(run_dense(c, st.rb[j].c1[mI], res_tc, sw, {rin, Cw, rin_h, rin_l, ACT_LRELU, 0.1f}, e));
+        else RUN(run_dense(c, st.rb[j].c2[mI], res_tc, sw, {xt, Cw, pt_h, pt_l, ACT_LRELU, 0.1f}, e));
         rin = r; rin_h = pr_h; rin_l = pr_l;
       }
     }

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import AcousticInputs, AcousticOutputs, HParams, TensorDesc, VocoderConfig, check, lib
+from ._lib import AcousticInputs, AcousticOutputs, HParams, TensorDesc, VocoderConfigEx, check, lib
 from .hparams import DEFAULT_VOCODER_CONFIG, resolve
 from .schedules import multinomial_table, prodiff_table, sampler_table
 
@@ -470,6 +470,38 @@ class AcousticModel:
         return q, codes
 
 
+def vocoder_config_ex(h):
+    """The generator config keys HifiGanGenerator.__init__ reads (modules/hifigan/hifigan_nsf.py:104-142) -> the C struct.
+    ``resblock`` '1' builds ResBlock1 and '2' ResBlock2 (:115; an int is read as its string).  Like the reference's modules,
+    ResBlock1 reads the first 3 entries of each dilation list and ResBlock2 the first 2; a shorter list, which the
+    reference cannot build either, is refused."""
+    rb = str(h.get("resblock", "1"))
+    if rb not in ("1", "2"):
+        raise ValueError(f"resblock must be '1' (ResBlock1) or '2' (ResBlock2), got {h.get('resblock')!r}")
+    nd = 3 if rb == "1" else 2
+    ks, ds = h["resblock_kernel_sizes"], h["resblock_dilation_sizes"]
+    if len(ds) < len(ks):
+        raise ValueError(f"resblock_dilation_sizes has {len(ds)} lists for {len(ks)} resblock kernel sizes")
+    vc = VocoderConfigEx()
+    vc.n_up = len(h["upsample_rates"])
+    if not (1 <= vc.n_up <= 8 and 1 <= len(ks) <= 4):
+        raise ValueError("1-8 upsampling stages and 1-4 resblock kernel sizes are supported")
+    for i, (u, k) in enumerate(zip(h["upsample_rates"], h["upsample_kernel_sizes"])):
+        vc.up_rates[i], vc.up_kernels[i] = u, k
+    vc.initial_channel = h["upsample_initial_channel"]
+    vc.n_res = len(ks)
+    for j, (k, d) in enumerate(zip(ks, ds)):
+        if len(d) < nd:
+            raise ValueError(f"ResBlock{rb} reads {nd} dilations per block; resblock_dilation_sizes[{j}] = {list(d)}")
+        vc.res_kernels[j] = k
+        for m in range(nd):
+            vc.res_dilations[j][m] = d[m]
+    vc.use_pitch_embed = 1 if h.get("use_pitch_embed") else 0
+    vc.sample_rate = h.get("audio_sample_rate", 48000)
+    vc.resblock = int(rb)
+    return vc
+
+
 class Vocoder:
     """Packed HiFi-GAN(-NSF) generator on one GPU (ssb_vocoder_t).  ``denoise_c`` > 0 runs the reference's output denoiser
     (hparams['vocoder_denoise_c'], tasks/tts/vocoder_infer/hifigan_nsf.py:73-74) on every generated waveform, with the
@@ -485,25 +517,12 @@ class Vocoder:
         self.device = torch.device(device if device is not None else "cuda:0")
         torch.cuda.set_device(self.device)
         h = self.cfg
-        if str(h.get("resblock", "1")) != "1":
-            raise NotImplementedError("only ResBlock1 generators are supported")
-        vc = VocoderConfig()
-        vc.n_up = len(h["upsample_rates"])
-        for i, (u, k) in enumerate(zip(h["upsample_rates"], h["upsample_kernel_sizes"])):
-            vc.up_rates[i], vc.up_kernels[i] = u, k
-        vc.initial_channel = h["upsample_initial_channel"]
-        vc.n_res = len(h["resblock_kernel_sizes"])
-        for j, (k, d) in enumerate(zip(h["resblock_kernel_sizes"], h["resblock_dilation_sizes"])):
-            vc.res_kernels[j] = k
-            for m in range(3):
-                vc.res_dilations[j][m] = d[m]
-        vc.use_pitch_embed = 1 if h.get("use_pitch_embed") else 0
-        vc.sample_rate = h.get("audio_sample_rate", 48000)
+        vc = vocoder_config_ex(h)
         self.hop = int(np.prod(h["upsample_rates"]))
         sd = {k: v for k, v in state_dict.items() if isinstance(v, torch.Tensor)}
         arr, keep = _descs(sd)
         handle = C.c_void_p()
-        check(lib.ssb_vocoder_create(C.byref(handle), arr, len(sd), C.byref(vc)), "ssb_vocoder_create")
+        check(lib.ssb_vocoder_create_ex(C.byref(handle), arr, len(sd), C.byref(vc)), "ssb_vocoder_create_ex")
         self._h = handle
         self._ws = _Workspace(self.device)
 

@@ -65,7 +65,8 @@ def load_state_dict(ckpt_base: str, model_name: str = "model") -> Tuple[Dict[str
 def load_vocoder_checkpoint(base_dir: str) -> Tuple[Dict[str, torch.Tensor], dict, str]:
     """(generator state dict incl. weight_g / weight_v, config dict, path) as HifiGAN.__init__ + load_model find them
     (vocoder_infer/hifigan_nsf.py:24-60): ``config.yaml`` + newest ``model_ckpt_steps_*.ckpt`` ['state_dict']['model_gen'],
-    else ``config.json`` + ``generator_v1`` ['generator']."""
+    else ``config.json`` + ``generator_v1`` ['generator'] (without ``generator_v1``: the one ``generator_v2`` or
+    ``generator_v3`` present)."""
     ycfg, jcfg = os.path.join(base_dir, "config.yaml"), os.path.join(base_dir, "config.json")
     if os.path.exists(ycfg):
         import yaml
@@ -77,7 +78,17 @@ def load_vocoder_checkpoint(base_dir: str) -> Tuple[Dict[str, torch.Tensor], dic
         ck = torch.load(paths[0], map_location="cpu", weights_only=False)
         return dict(ck["state_dict"]["model_gen"]), cfg, paths[0]
     if os.path.exists(jcfg):
+        # the reference reads generator_v1 only; a directory of the official V2 or V3 release holds generator_v2 or
+        # generator_v3 instead, and its config.json describes that layout
         path = os.path.join(base_dir, "generator_v1")
+        if not os.path.exists(path):
+            found = [os.path.join(base_dir, n) for n in ("generator_v2", "generator_v3")
+                     if os.path.exists(os.path.join(base_dir, n))]
+            if len(found) > 1:
+                raise ValueError(f"{base_dir} holds both generator_v2 and generator_v3 and no generator_v1: "
+                                 "keep the one its config.json describes")
+            if found:
+                path = found[0]
         with open(jcfg) as f:
             cfg = json.load(f)
         ck = torch.load(path, map_location="cpu", weights_only=False)

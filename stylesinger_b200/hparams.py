@@ -6,7 +6,8 @@ loader utils/hparams.py:25-124).  The engine reads the same keys as the referenc
 reference ``hparams`` dict can be passed in unchanged; keys it does not contain fall back to
 these defaults.  HiFi-GAN architecture keys are NOT in the reference tree (they live in the
 downloaded ``checkpoints/hifigan/config.yaml``, reference tasks/tts/vocoder_infer/hifigan_nsf.py:48-60);
-``DEFAULT_VOCODER_CONFIG`` is the HiFi-GAN-V1 layout assumed by SURVEY.md §0.4.
+``DEFAULT_VOCODER_CONFIG`` is the HiFi-GAN-V1 layout assumed by SURVEY.md §0.4; ``HIFIGAN_V2`` / ``HIFIGAN_V3`` are the
+other two published layouts.
 """
 import copy
 
@@ -64,6 +65,14 @@ DEFAULT_VOCODER_CONFIG = {
     "audio_num_mel_bins": 80,
     "hop_size": 256,
 }
+
+# The two other published HiFi-GAN layouts (Kong et al. 2020, config_v2.json / config_v3.json), with the NSF source and
+# the rates that give StyleSinger's hop of 256.  V2: V1's layout at 128 initial channels (stages of 64, 32, 16 and 8
+# channels).  V3: ResBlock2 (two single convs per block, two dilations each) over three upsampling stages.
+HIFIGAN_V2 = dict(DEFAULT_VOCODER_CONFIG, upsample_initial_channel=128)
+HIFIGAN_V3 = dict(DEFAULT_VOCODER_CONFIG, upsample_rates=[8, 8, 4], upsample_kernel_sizes=[16, 16, 8],
+                  upsample_initial_channel=256, resblock="2", resblock_kernel_sizes=[3, 5, 7],
+                  resblock_dilation_sizes=[[1, 2], [2, 6], [3, 12]])
 
 # Mutable module-level dict with the same role as the reference's global `hparams`
 # (reference utils/hparams.py:8).

@@ -173,11 +173,13 @@ def vocoder_param_shapes(h):
         c = C0 // (2 ** (i + 1))
         out += [(f"ups.{i}.bias", (c,)), (f"ups.{i}.weight_g", (2 * c, 1, 1)), (f"ups.{i}.weight_v", (2 * c, c, k))]
     nk = len(h["resblock_kernel_sizes"])
+    # ResBlock1 (hifigan_nsf.py:30-66): convs1.{0,1,2} then convs2.{0,1,2}; ResBlock2 (:69-90, resblock != '1'): convs.{0,1}
+    groups = (("convs1", 3), ("convs2", 3)) if str(h.get("resblock", "1")) == "1" else (("convs", 2),)
     for i in range(len(h["upsample_rates"])):
         c = C0 // (2 ** (i + 1))
         for j, k in enumerate(h["resblock_kernel_sizes"]):
-            for grp in ("convs1", "convs2"):
-                for m in range(3):
+            for grp, n_conv in groups:
+                for m in range(n_conv):
                     q = f"resblocks.{i * nk + j}.{grp}.{m}."
                     out += [(q + "bias", (c,)), (q + "weight_g", (c, 1, 1)), (q + "weight_v", (c, c, k))]
     cl = C0 // (2 ** len(h["upsample_rates"]))

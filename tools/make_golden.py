@@ -252,6 +252,54 @@ def case_vocoder_edges(name, lengths=VOCODER_EDGE_LENGTHS, seed=37):
     print("wrote", name, {k: v.shape for k, v in d.items() if k != "meta"})
 
 
+VOCODER_LAYOUT_LENGTHS = (1, 2, 3, 5, 17, 24)
+
+
+def case_vocoder_layouts(name, lengths=VOCODER_LAYOUT_LENGTHS, seed=53):
+    """The reference HifiGanGenerator (B = 1) in HiFi-GAN's other two published layouts: V2 (ResBlock1, stages of 64,
+    32, 16 and 8 channels), V3 (ResBlock2 over stages of 128, 64 and 32 channels) and V3 without the NSF source (the
+    generator of a config with use_pitch_embed: False, run without f0).  Synthetic weights from synth.vocoder_state_dict,
+    loaded with strict=True, weight norm removed.  One mel / f0 pair per length (stored as mel_<L>, f0_<L>), shared by
+    the layouts; f0 has an unvoiced frame every third frame.  The noise of length L is NoiseSource(seed + L), as in
+    case_vocoder_edges.  The reference's state-dict keys (weight-norm form) are stored per layout in meta."""
+    import ref_import
+    ref_import.install(T=4)
+    from modules.hifigan.hifigan_nsf import HifiGanGenerator
+    from stylesinger_b200.hparams import HIFIGAN_V2, HIFIGAN_V3
+    layouts = {"v2": HIFIGAN_V2, "v3": HIFIGAN_V3, "v3_nonsf": dict(HIFIGAN_V3, use_pitch_embed=False)}
+    g = torch.Generator().manual_seed(seed)
+    d, keys = {}, {}
+    inputs = {}
+    for L in lengths:
+        mel = (-3.0 + 1.0 * torch.randn(L, 80, generator=g)).clamp(-6, 1.5)
+        f0 = 150 + 350 * torch.rand(L, generator=g)
+        f0[1::3] = 0
+        inputs[L] = (mel, f0)
+        d.update({f"mel_{L}": np32(mel), f"f0_{L}": np32(f0)})
+    for lname, h in layouts.items():
+        gen = HifiGanGenerator(h)
+        keys[lname] = list(gen.state_dict().keys())
+        gen.load_state_dict(synth.vocoder_state_dict(h, seed=0), strict=True)
+        gen.remove_weight_norm()
+        gen.eval()
+        for L in lengths:
+            mel, f0 = inputs[L]
+            c = mel.t()[None].contiguous()
+            if h["use_pitch_embed"]:
+                ns = NoiseSource(seed + L)
+                with torch.no_grad(), patched_rng(ns):
+                    y = gen(c, f0[None].clone()).view(-1)
+                d[f"wav_{lname}_{L}"] = np32(y)
+                print(f"{lname} L={L:2d} f0:    max |wav| {float(y.abs().max()):.3f} std {float(y.std()):.3f}")
+            with torch.no_grad():
+                y = gen(c).view(-1)
+            d[f"wav_nof0_{lname}_{L}"] = np32(y)
+            print(f"{lname} L={L:2d} no f0: max |wav| {float(y.abs().max()):.3f} std {float(y.std()):.3f}")
+    d["meta"] = json.dumps({"lengths": list(lengths), "seed": seed, "layouts": list(layouts), "keys": keys})
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, len(d) - 1, "arrays")
+
+
 def case_plms(name, T=100, interval=10, frames=48, seed=61):
     """f2: the reference's PLMS sampler (GaussianDiffusion.p_sample_plms, shallow_diffusion_tts.py:164-197) driven exactly
     as GaussianDiffusion.forward does under hparams['pndm_speedup'] (:254-260), on the StyleSinger mel denoiser (the
@@ -528,7 +576,7 @@ if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "convf0", "sched", "voc",
-                             "vocoder_edges", "emo", "registry", "kstep"]
+                             "vocoder_edges", "emo", "registry", "kstep", "vocoder_layouts"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
@@ -549,6 +597,8 @@ if __name__ == "__main__":
         case_vocoder("ref_vocoder_f24", frames=24, seed=31)
     if "vocoder_edges" in which:
         case_vocoder_edges("ref_vocoder_edges")
+    if "vocoder_layouts" in which:
+        case_vocoder_layouts("ref_vocoder_layouts")
     if "emo" in which:
         case_emotion_encoder("ref_emotion_encoder")
     if "registry" in which:

@@ -23,10 +23,12 @@ def _t64(t, B):
     return torch.full((B,), float(t), dtype=torch.float64)
 
 
-def diffnet64(spec, t, cond, hp):
-    """DiffNet.forward in float64. spec [B,1,80,F], t int, cond [B,256,F] -> eps [B,1,80,F]."""
+def diffnet64(spec, t, cond, hp, sd64=None, prefix="postdiff.denoise_fn."):
+    """DiffNet.forward in float64. spec [B,1,80,F], t int, cond [B,256,F] -> [B,1,80,F].  sd64 / prefix: a float64 state
+    dict and the net's key prefix (default: the DiffSinger mel denoiser of acoustic_sd64())."""
     with torch.no_grad():
-        return O.diffnet(spec.double(), _t64(t, spec.shape[0]), cond.double(), acoustic_sd64(), hp)
+        return O.diffnet(spec.double(), _t64(t, spec.shape[0]), cond.double(),
+                         acoustic_sd64() if sd64 is None else sd64, hp, p=prefix)
 
 
 def ddiffnet64(f0, uv, t, cond, hp, prefix):

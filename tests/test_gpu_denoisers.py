@@ -33,13 +33,14 @@ from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
 from tests import denoiser_oracle as DO
 from tests.common import acoustic_engine, hp_for
+from tests.gpu_checks import (Err, check_variants, cond_gemm, count, frame_offsets, launched, net_dims, ntiles,
+                              rel, split, step_gemms)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 T = 100
 STEPS = (0, 50, 99)
 F0_T = 4
-EDGE_ROWS = 8
 RF = 33  # rows one DDiffNet evaluation reaches on each side: the dilations 1, 2, 4, 8, 1, 2, 4, 8, 1, 2 summed
 MARGIN = 1e-4
 
@@ -65,115 +66,8 @@ RAGGED = [129, 1, 2, 3, 8, 9, 16, 17, 127, 128, 700]                            
 TILES48 = [EDGE[i % 9] for i in range(48)]                                       # 48 utterances, one row tile each
 
 
-def _offs(lens):
-    return np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
-
-
-def _ntiles(lens):
-    return sum((int(n) + 127) // 128 for n in lens)
-
-
-def _rel(a, b):
-    a = a.detach().cpu().double() if isinstance(a, torch.Tensor) else torch.as_tensor(np.asarray(a, np.float64))
-    b = b.detach().cpu().double() if isinstance(b, torch.Tensor) else torch.as_tensor(np.asarray(b, np.float64))
-    return ((a - b).abs() / b.abs().clamp(min=1.0)).reshape(a.shape[0], -1)
-
-
-def _split(x, offs):
-    x = x.detach().cpu()
-    return [x[int(offs[i]):int(offs[i + 1])] for i in range(len(offs) - 1)]
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# which tensor-core GEMM variants a call must launch: conv_gemm_tc's dispatch (CTA pairs, with the tap-reuse kernel for
-# 3-tap GATE / GENERIC convs, when ceil(ntiles / 2) * N / (2 hb) >= #SMs, hb = 64 if N % 128 == 0 else 32; else 64-wide
-# N tiles when N % 128 != 0 or ntiles * N / 128 < 2 #SMs; else 128-wide) over the denoiser's GEMMs
-def _variant(nt, N, mode, taps):
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    hb = 64 if N % 128 == 0 else 32
-    if ((nt + 1) // 2) * (N // (2 * hb)) >= sms:
-        return f"tc2{'r' if taps == 3 and mode != 'RES_SKIP' else ''}<{hb},{mode}>"
-    return f"tc<64,{mode}>" if N % 128 != 0 or nt * (N // 128) < 2 * sms else f"tc<128,{mode}>"
-
-
-def _count(gemms, nt):
-    out = {}
-    for N, mode, taps in gemms:
-        k = _variant(nt, N, mode, taps)
-        out[k] = out.get(k, 0) + 1
-    return out
-
-
-def _net(which):
-    hp = hp_for(T)
-    if which == 0:
-        return hp["residual_channels"], hp["residual_layers"], 256
-    return hp["f0_residual_channels"], hp["f0_residual_layers"], 128
-
-
-def cond_gemm(which):
-    """The hoisted conditioner projection of all layers, once per call."""
-    C, L, _ = _net(which)
-    return [(L * 2 * C, "GENERIC", 1)]
-
-
-def step_gemms(which):
-    """One evaluation after the conditioner: (mel) the input projection, L x (gate, residual + skip), skip_projection,
-    output_projection (N padded to 256 / 128)."""
-    C, L, n_out = _net(which)
-    g = [(C, "GENERIC", 1)] if which == 0 else []
-    return g + [(2 * C, "GATE", 3), (2 * C, "RES_SKIP", 1)] * L + [(256, "GENERIC", 1), (n_out, "GENERIC", 1)]
-
-
 def expected_eval(which, lens):
-    return _count(cond_gemm(which) + step_gemms(which), _ntiles(lens))
-
-
-def _launched(fn):
-    from stylesinger_b200._lib import lib, variant_launches
-    torch.cuda.synchronize()
-    before, l0 = variant_launches(), lib.ssb_launch_count()
-    r = fn()
-    torch.cuda.synchronize()
-    after, l1 = variant_launches(), lib.ssb_launch_count()
-    return r, {k: after[k] - before.get(k, 0) for k in after if after[k] > before.get(k, 0)}, l1 - l0
-
-
-def _check_variants(tag, got, want):
-    print(f"{tag}: tensor-core GEMM variants launched {got}")
-    assert got == want, (tag, got, want)
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# edge / interior errors
-class Err:
-    """Largest error on the interior rows and on the EDGE_ROWS rows at each utterance end, with where it is."""
-
-    def __init__(self):
-        self.v = {"interior": (0.0, None), "edge": (0.0, None)}
-
-    def add(self, i, a, b):
-        e = _rel(a, b)
-        n = e.shape[0]
-        edge = torch.zeros(n, dtype=torch.bool)
-        edge[:EDGE_ROWS] = True
-        edge[-EDGE_ROWS:] = True
-        for k, rows in (("edge", edge), ("interior", ~edge)):
-            if rows.any():
-                sub = torch.where(rows[:, None], e, torch.zeros_like(e))
-                j = int(sub.argmax())
-                v = float(sub.reshape(-1)[j])
-                if v > self.v[k][0]:
-                    self.v[k] = (v, (i, j // e.shape[1], j % e.shape[1]))
-
-    def max(self):
-        return max(self.v["interior"][0], self.v["edge"][0])
-
-    def report(self, tag, bar):
-        (vi, wi), (ve, we) = self.v["interior"], self.v["edge"]
-        print(f"{tag}: interior {vi:.3e} at (utterance, row, column) {wi}, edge {ve:.3e} at {we} (bar {bar:.1e})")
-        assert self.max() <= bar, (tag, self.v, bar)
-        assert ve <= 4 * vi, (tag, "edge rows err more than 4x the interior", self.v)
+    return count(cond_gemm(which) + step_gemms(which), ntiles(lens))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -204,10 +98,10 @@ def batch(name):
         out = m.forward(pb, seed=1, skip_mel_diffusion=True, want=("diff_cond", "coarse_mel"))
         lens = [len(u["mel2ph"]) for u in utts]
         midi = torch.cat([u["note"][u["mel2ph"] - 1] * (u["mel2ph"] > 0) for u in utts]).float()
-        _B[name] = dict(utts=utts, lens=lens, offs=_offs(lens), pb=pb, cond=out["diff_cond"].clone(),
+        _B[name] = dict(utts=utts, lens=lens, offs=frame_offsets(lens), pb=pb, cond=out["diff_cond"].clone(),
                         coarse=out["coarse_mel"].clone(), midi=midi)
         if name == "bench":
-            assert int(_B[name]["offs"][-1]) == 110119 and _ntiles(lens) == 890
+            assert int(_B[name]["offs"][-1]) == 110119 and ntiles(lens) == 890
     return _B[name]
 
 
@@ -260,22 +154,22 @@ def test_denoiser_eval_matches_float64(which, size):
     lens, offs = b["lens"], b["offs"]
     want = expected_eval(which, lens)
     if size == "mid":
-        assert want[f"tc{'2r<64' if which == 0 else '<64'},GATE>"] == _net(which)[1], want
+        assert want[f"tc{'2r<64' if which == 0 else '<64'},GATE>"] == net_dims(which)[1], want
     if size == "bench":
-        assert want["tc2r<64,GATE>"] == _net(which)[1] and want["tc2<64,RES_SKIP>"] == _net(which)[1], want
+        assert want["tc2r<64,GATE>"] == net_dims(which)[1] and want["tc2<64,RES_SKIP>"] == net_dims(which)[1], want
     t64 = 0.0
     try:
         for t in STEPS:
             x, uv = eval_inputs(which, t, b)
-            xs, uvs, cs = _split(x, offs), (_split(uv, offs) if uv is not None else None), _split(b["cond"], offs)
+            xs, uvs, cs = split(x, offs), (split(uv, offs) if uv is not None else None), split(b["cond"], offs)
             outs = {}
             for path in ("tc", "ffma"):
                 m.set_tensor_cores(path == "tc")
-                outs[path], got, _ = _launched(lambda: m.denoiser_eval(which, x, uv, t, b["cond"], offs).clone())
-                _check_variants(f"eval net {which} {size} t={t} {path}", got, want if path == "tc" else {})
+                outs[path], got, _ = launched(lambda: m.denoiser_eval(which, x, uv, t, b["cond"], offs).clone())
+                check_variants(f"eval net {which} {size} t={t} {path}", got, want if path == "tc" else {})
             for path in ("tc", "ffma"):
                 err, solo = Err(), 0.0
-                ys = _split(outs[path], offs)
+                ys = split(outs[path], offs)
                 t0 = time.time()
                 for i in _compared(size, which, t, lens):
                     err.add(i, ys[i], _f64_eval(which, t, size, i, xs[i], uvs[i] if uvs else None, cs[i]))
@@ -285,14 +179,14 @@ def test_denoiser_eval_matches_float64(which, size):
                     for i in range(len(lens)):
                         y1 = m.denoiser_eval(which, xs[i].to(DEV).contiguous(),
                                              uvs[i].to(DEV).contiguous() if uvs else None, t, cs[i].to(DEV).contiguous(),
-                                             _offs([lens[i]]))
-                        e = float(_rel(y1, ys[i]).max())
+                                             frame_offsets([lens[i]]))
+                        e = float(rel(y1, ys[i]).max())
                         solo = max(solo, e)
                         if path == "ffma":
                             assert torch.equal(y1.cpu(), ys[i]), (size, which, t, i, e)
                     print(f"eval net {which} {size} t={t} {path}: solo B=1 calls {solo:.3e} (bar {BARS['solo'][path]:.1e})")
                     assert solo <= BARS["solo"][path]
-                err.report(f"eval net {which} {size} t={t} {path} ({len(lens)} utterances, {_ntiles(lens)} row tiles)",
+                err.report(f"eval net {which} {size} t={t} {path} ({len(lens)} utterances, {ntiles(lens)} row tiles)",
                            BARS["eval"][path])
     finally:
         m.set_tensor_cores(True)
@@ -320,7 +214,7 @@ def _mel64(name, K, b, coarse, noise):
     key = ("mel", name, K)
     if key not in _CH:
         hp = dict(hp_for(T), K_step=K)
-        cs, co = _split(b["cond"], b["offs"]), _split(coarse, b["offs"])
+        cs, co = split(b["cond"], b["offs"]), split(coarse, b["offs"])
         a = b["offs"]
         _CH[key] = [DO.mel_chain64(cs[i], co[i], hp, K, noise[:, int(a[i]):int(a[i + 1])]) for i in range(len(cs))]
     return _CH[key]
@@ -334,7 +228,7 @@ def test_mel_sampler_chain_matches_float64(K):
         for name in ("one_tile", "ragged", "tiles48", "bench6"):
             b = batch(name) if name != "one_tile" else _one_tile()
             lens, offs = b["lens"], b["offs"]
-            nt = _ntiles(lens)
+            nt = ntiles(lens)
             noise = _mel_noise(K, int(offs[-1]), 50 + K)
             coarse = _chain_coarse(name, int(offs[-1]))
             t0 = time.time()
@@ -348,18 +242,18 @@ def test_mel_sampler_chain_matches_float64(K):
             for path in paths:
                 m.set_tensor_cores(path != "ffma")
                 m.set_persistent(path == "persistent")
-                mel, got, launches = _launched(lambda: m.mel_diffusion(b["cond"], coarse, offs, noise.to(DEV)).clone())
+                mel, got, launches = launched(lambda: m.mel_diffusion(b["cond"], coarse, offs, noise.to(DEV)).clone())
                 if path == "persistent":
                     print(f"mel chain {name} K={K} persistent: {launches} launches")
                     assert launches < 16
-                    want = _count(cond_gemm(0), nt)
+                    want = count(cond_gemm(0), nt)
                 elif path == "tc":
-                    want = _count(cond_gemm(0) + step_gemms(0) * K, nt)
+                    want = count(cond_gemm(0) + step_gemms(0) * K, nt)
                 else:
                     want = {}
-                _check_variants(f"mel chain {name} K={K} {path}", got, want)
+                check_variants(f"mel chain {name} K={K} {path}", got, want)
                 err = Err()
-                for i, y in enumerate(_split(mel, offs)):
+                for i, y in enumerate(split(mel, offs)):
                     err.add(i, y, ref[i]["mel"])
                 err.report(f"mel chain {name} K={K} {path} ({len(lens)} utterances, {nt} row tiles)",
                            BARS["mel_chain"][path])
@@ -374,7 +268,7 @@ def _one_tile():
         b = batch("small")
         i = b["lens"].index(127)
         a, e = int(b["offs"][i]), int(b["offs"][i + 1])
-        _B["one_tile"] = dict(lens=[127], offs=_offs([127]), cond=b["cond"][a:e].contiguous(),
+        _B["one_tile"] = dict(lens=[127], offs=frame_offsets([127]), cond=b["cond"][a:e].contiguous(),
                               coarse=b["coarse"][a:e].contiguous(), midi=b["midi"][a:e])
     return _B["one_tile"]
 
@@ -424,7 +318,7 @@ def test_f0_sampler_chain_matches_float64(which):
             gauss, unif = _f0_noise(n, 60 + which)
             t0 = time.time()
             chains, clip = [], []
-            for i, c in enumerate(_split(b["cond"], offs)):
+            for i, c in enumerate(split(b["cond"], offs)):
                 a, e = int(offs[i]), int(offs[i + 1])
                 r = DO.f0_chain64(c.t(), lo[a:e], hi[a:e], hp, DO.F0_PREFIX[which], gauss[:, a:e], unif[:, a:e])
                 chains.append((r["z"][-1], r["uv"][-1], torch.stack(r["margin"]).min(0).values))
@@ -435,12 +329,12 @@ def test_f0_sampler_chain_matches_float64(which):
             assert 0 < clip.mean() < 1
             for path in ("tc", "ffma"):
                 m.set_tensor_cores(path == "tc")
-                (z, uv), got, _ = _launched(lambda: m.f0_diffusion(which, b["cond"], lo.to(DEV).contiguous(),
+                (z, uv), got, _ = launched(lambda: m.f0_diffusion(which, b["cond"], lo.to(DEV).contiguous(),
                                                                    hi.to(DEV).contiguous(), offs, gauss.to(DEV),
                                                                    unif.to(DEV).contiguous()))
-                nt = _ntiles(lens)
-                _check_variants(f"f0 chain net {which} {name} {path}", got,
-                                _count(cond_gemm(1) + step_gemms(1) * F0_T, nt) if path == "tc" else {})
+                nt = ntiles(lens)
+                check_variants(f"f0 chain net {which} {name} {path}", got,
+                                count(cond_gemm(1) + step_gemms(1) * F0_T, nt) if path == "tc" else {})
                 _uv_z_check(f"f0 chain net {which} {name} {path} ({len(lens)} utterances, {nt} row tiles)", lens, offs,
                             uv.cpu().long(), z.cpu().double(), chains, BARS["f0_chain"][path])
     finally:
@@ -460,12 +354,12 @@ def test_f0_pair_persistent_through_forward_matches_float64():
     noise = {"f0_gauss": [g.to(DEV).contiguous() for g in gauss], "f0_unif": [u.to(DEV).contiguous() for u in unif]}
     m.set_persistent(True)
     m.set_tensor_cores(True)
-    out, got, _ = _launched(lambda: m.forward(pb, noise=noise, skip_mel_diffusion=True, want=(
+    out, got, _ = launched(lambda: m.forward(pb, noise=noise, skip_mel_diffusion=True, want=(
         "pitch_pred", "encoder_out", "spk_proj", "emo_proj", "style")))
     print(f"f0 pair persistent: tensor-core GEMM variants launched {got}")
     assert not any("GATE" in k or "RES_SKIP" in k for k in got), got  # the layer GEMMs ran inside the persistent kernel
-    enc = _split(out["encoder_out"], pb.ph_offsets)
-    sty = _split(out["style"], offs)
+    enc = split(out["encoder_out"], pb.ph_offsets)
+    sty = split(out["style"], offs)
     spk, emo = out["spk_proj"].cpu(), out["emo_proj"].cpu()
     lo, hi = (v.reshape(n) for v in O.midi_clip_band(b["midi"][None, None]))
     f0c, uvc, clip = [], [], []
@@ -486,5 +380,5 @@ def test_f0_pair_persistent_through_forward_matches_float64():
     print(f"f0 pair persistent: x0 clipped in {np.mean(clip):.3f} of the predictions")
     pp = out["pitch_pred"].cpu().double()
     # pitch_pred[:, 1] is the mean of the two UV decisions: compare their sum (0, 1, 2)
-    _uv_z_check(f"f0 pair persistent ({len(lens)} utterances, {_ntiles(lens)} row tiles)", lens, offs,
+    _uv_z_check(f"f0 pair persistent ({len(lens)} utterances, {ntiles(lens)} row tiles)", lens, offs,
                 (2 * pp[:, 1]).round().long(), pp[:, 0], f0c, BARS["f0_chain"]["persistent"])

@@ -350,7 +350,7 @@ int ssb_model_set_persistent_groups(ssb_model_t* m, int32_t enable);
  * new setting. */
 int ssb_model_set_fft_tensor_cores(ssb_model_t* m, int32_t enable);
 
-/* Unit-test granularity: ssb_op_conv1d through the tensor-core path (Cin % 64 == 0, N % 128 == 0, no activation). */
+/* Unit-test granularity: ssb_op_conv1d through the tensor-core path (Cin % 64 == 0, N % 64 == 0, no activation). */
 int ssb_op_conv1d_tc(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
                      const float* b_host, int32_t N, int32_t k, int32_t dilation, float* out, void* stream);
 
@@ -448,6 +448,63 @@ int32_t ssb_set_attention_tensor_cores(int32_t enable);
  * (packs on the fly with cudaMalloc; not for production use).  act: 0 none 1 relu 2 gelu 3 leaky(0.1) 4 tanh. */
 int ssb_op_conv1d(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
                   const float* b_host, int32_t N, int32_t k, int32_t dilation, int32_t act, float* out, void* stream);
+
+/* Unit-test granularity: exactly ONE dense GEMM - the fp32 FFMA kernel (path 0, csrc/conv_gemm.cu) or the tensor-core
+ * kernel (path 1, csrc/conv_gemm_tc.cu) - with any epilogue, over CALLER-OWNED device buffers in the guard-banded layout
+ * of frame_offsets: utterance b occupies rows [rs_b, rs_b + L_b), rs_0 = 16, rs_{b+1} = rs_b + L_b + 16, and `rows` must
+ * be rs_{B-1} + L_{B-1} + 16 + 256 (tail slack).  Nothing is copied in or out: buffers may alias (RES_SKIP rewriting its
+ * own residual planes, accumulation into `out`), and guard rows, tail slack, column-block-major `out` (out_nb) and the
+ * chunk-tiled skip accumulator (skip_tiled) are seen as stored.  Weights are HOST fp32 [N, Cin, k] + bias [N] (may be
+ * NULL) in torch layout, packed on the fly (gate != 0: the DiffNet gate interleave, column 2j = sigmoid half j, 2j+1 = tanh
+ * half j).  The A operand is fp32 rows [rows, lda] (path 0, with a_act / a_slope / a_scale applied on load) or fp16 hi/lo
+ * planes [rows, Cin] (path 1).  The epilogue fields are those of Epi (path 0) and EpiTC (path 1), passed through as they
+ * are; the kernels' own checks apply.  Refused before any launch: a conv reach (k - 1) / 2 * dilation beyond the 16 guard
+ * rows. */
+typedef struct ssb_op_gemm_args {
+  int32_t path;                 /* 0: fp32 FFMA, 1: tensor cores */
+  const int32_t* frame_offsets; /* host [B + 1] */
+  int32_t B;
+  int64_t rows;
+  int32_t Cin, N, k, dilation, gate;
+  const float* w_host;
+  const float* b_host;
+  const float* a;               /* path 0 */
+  int32_t lda, a_act;
+  float a_slope, a_scale;
+  const void* a_hi;             /* path 1: fp16 [rows, Cin] */
+  const void* a_lo;
+  int32_t mode;                 /* 0 GENERIC, 1 GATE, 2 RES_SKIP */
+  const float* add;
+  int32_t ld_add;
+  float alpha;
+  int32_t act;
+  float act_slope;
+  const float* res;
+  int32_t ld_res;
+  float beta;
+  const float* rowmask;
+  float* out;
+  int32_t ldo, accum;
+  float gamma;
+  float* out2;                  /* path 0 */
+  int32_t ldo2;
+  const float* vec1;            /* path 1, RES_SKIP with rh / rl */
+  const float* vec2;
+  void* oh;                     /* fp16 planes: out2_h / out2_l (path 0), oh / ol (path 1) */
+  void* ol;
+  int32_t ldh, plane_act;
+  float plane_slope;
+  float* skip;
+  int32_t ld_skip, C, skip_init;
+  const void* rh;               /* path 1 */
+  const void* rl;
+  int32_t ld_rh, skip_tiled, out_nb;
+  int64_t out_bs;
+  void* sh;
+  void* sl;
+  int32_t n_valid;
+} ssb_op_gemm_args;
+int ssb_op_gemm(const ssb_op_gemm_args* a, void* stream);
 /* Unit-test granularity: multi-head attention, 2 heads x 128; q [sumL,256], k/v [sumS,256]. */
 int ssb_op_attention(const float* q, const float* k, const float* v, const int32_t* q_offsets,
                      const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream);

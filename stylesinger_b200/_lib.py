@@ -53,6 +53,24 @@ class AcousticOutputs(C.Structure):
         "diff_cond", "mel2ph", "spk_proj", "emo_proj")]
 
 
+class OpGemmArgs(C.Structure):
+    """ssb_op_gemm_args: one conv_gemm (path 0) or conv_gemm_tc (path 1) call over caller-owned device buffers."""
+    _fields_ = [("path", C.c_int32), ("frame_offsets", C.c_void_p), ("B", C.c_int32), ("rows", C.c_int64),
+                ("Cin", C.c_int32), ("N", C.c_int32), ("k", C.c_int32), ("dilation", C.c_int32), ("gate", C.c_int32),
+                ("w_host", C.c_void_p), ("b_host", C.c_void_p),
+                ("a", C.c_void_p), ("lda", C.c_int32), ("a_act", C.c_int32), ("a_slope", C.c_float), ("a_scale", C.c_float),
+                ("a_hi", C.c_void_p), ("a_lo", C.c_void_p),
+                ("mode", C.c_int32), ("add", C.c_void_p), ("ld_add", C.c_int32), ("alpha", C.c_float), ("act", C.c_int32),
+                ("act_slope", C.c_float), ("res", C.c_void_p), ("ld_res", C.c_int32), ("beta", C.c_float),
+                ("rowmask", C.c_void_p), ("out", C.c_void_p), ("ldo", C.c_int32), ("accum", C.c_int32), ("gamma", C.c_float),
+                ("out2", C.c_void_p), ("ldo2", C.c_int32), ("vec1", C.c_void_p), ("vec2", C.c_void_p),
+                ("oh", C.c_void_p), ("ol", C.c_void_p), ("ldh", C.c_int32), ("plane_act", C.c_int32),
+                ("plane_slope", C.c_float), ("skip", C.c_void_p), ("ld_skip", C.c_int32), ("C", C.c_int32),
+                ("skip_init", C.c_int32), ("rh", C.c_void_p), ("rl", C.c_void_p), ("ld_rh", C.c_int32),
+                ("skip_tiled", C.c_int32), ("out_nb", C.c_int32), ("out_bs", C.c_int64), ("sh", C.c_void_p),
+                ("sl", C.c_void_p), ("n_valid", C.c_int32)]
+
+
 # every symbol declared in include/stylesinger_b200.h (tests/test_abi.py checks this list against the header)
 EXPORTS = [
     "ssb_version", "ssb_last_error", "ssb_model_create", "ssb_model_free", "ssb_model_set_schedule",
@@ -75,6 +93,7 @@ EXPORTS = [
     "ssb_model_set_mel_k_step",
     "ssb_acoustic_forward_keyed", "ssb_hifigan_generate_keyed",
     "ssb_vocoder_create_ex",
+    "ssb_op_gemm",
 ]
 
 
@@ -128,6 +147,7 @@ def _load():
         "ssb_model_set_fft_tensor_cores": (C.c_int, [vp, i32]),
         "ssb_vocoder_set_tensor_cores": (C.c_int, [vp, i32]),
         "ssb_op_conv1d_tc": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, vp]),
+        "ssb_op_gemm": (C.c_int, [P(OpGemmArgs), vp]),
         "ssb_fft_workspace_bytes": (sz, [vp, i32, vp, i32]),
         "ssb_fft_encoder": (C.c_int, [vp, vp, vp, i32, vp, vp, sz, vp]),
         "ssb_fft_decoder": (C.c_int, [vp, vp, vp, i32, vp, vp, sz, vp]),

@@ -316,6 +316,85 @@ static Ctx make_ctx(void* ws, size_t bytes, void* stream, bool dry = false) {
   return c;
 }
 
+// ---- one dense GEMM at unit-test granularity (ssb_op_gemm, ssb_op_conv1d, ssb_op_conv1d_tc) --------------------------
+struct OpWeights {  // the call's packed weights, freed with the pool when the call returns
+  DevicePool pool;
+  Conv cv;
+  ConvTC ct;
+};
+
+static ssb_op_gemm_args op_args(int path, const int32_t* offsets, int B, int Cin, const float* w_host, const float* b_host,
+                                int N, int k, int dilation) {
+  ssb_op_gemm_args a;
+  memset(&a, 0, sizeof(a));
+  a.path = path; a.frame_offsets = offsets; a.B = B;
+  a.Cin = Cin; a.N = N; a.k = k; a.dilation = dilation; a.w_host = w_host; a.b_host = b_host;
+  a.a_slope = a.act_slope = a.plane_slope = 0.1f;
+  a.a_scale = a.alpha = a.beta = a.gamma = 1.0f;
+  return a;
+}
+
+// Packs the host weights for the call's path.  A conv whose taps reach past the guard band would read the neighbouring
+// utterance (or, for the first one, whatever lies before the buffer), so it is refused here, before anything is launched.
+static int op_pack(const ssb_op_gemm_args& a, OpWeights* w) {
+  SSB_CHECK(a.path == 0 || a.path == 1, "op_gemm: path must be 0 (fp32 FFMA) or 1 (tensor cores)");
+  SSB_CHECK(a.w_host && a.Cin > 0 && a.N > 0 && a.k >= 1 && a.dilation >= 1, "op_gemm: bad weight shape");
+  SSB_CHECK(!a.gate || a.N % 2 == 0, "op_gemm: the gate packing needs an even N");
+  const int64_t reach = (int64_t)(a.k - 1) / 2 * a.dilation;
+  SSB_CHECK(reach <= GUARD, "op_gemm: conv reach (k - 1) / 2 * dilation = " + std::to_string(reach) + " exceeds the " +
+                                std::to_string(GUARD) + " guard rows between utterances");
+  HostTensor wt, bt;
+  wt.data = a.w_host; wt.shape = {a.N, a.Cin, a.k};
+  bt.data = a.b_host; bt.shape = {a.N};
+  const PackMode pm = a.gate ? PACK_GATE_SIG_TANH : PACK_PLAIN;
+  if (pack_conv(w->pool, &wt, a.b_host ? &bt : nullptr, a.dilation, pm, &w->cv)) return -1;
+  if (a.path == 1) {
+    SSB_CHECK(tc_available(), "tensor-core path unavailable (cuTensorMapEncodeTiled)");
+    if (pack_conv_tc(w->pool, &wt, a.dilation, pm, w->cv.bias, &w->ct)) return -1;
+    SSB_CHECK(w->ct.ok, "op_gemm: shape not eligible for the tensor-core path (Cin % 64, N % 64)");
+  }
+  return 0;
+}
+
+// One conv_gemm / conv_gemm_tc call over the layout s; every epilogue field of a goes to the kernel as it is.
+static int op_launch(Ctx& c, const SeqDev& s, const ssb_op_gemm_args& a, const OpWeights& w) {
+  if (a.path == 0) {
+    ConvGemm g = make_gemm(w.cv, s, a.a, a.lda);
+    g.a_act = a.a_act; g.a_slope = a.a_slope; g.a_scale = a.a_scale;
+    Epi& e = g.e;
+    e.mode = a.mode; e.add = a.add; e.ld_add = a.ld_add; e.alpha = a.alpha; e.act = a.act; e.act_slope = a.act_slope;
+    e.res = a.res; e.ld_res = a.ld_res; e.beta = a.beta; e.rowmask = a.rowmask;
+    e.out = a.out; e.ldo = a.ldo; e.accum = a.accum; e.gamma = a.gamma;
+    e.out2 = a.out2; e.ldo2 = a.ldo2; e.vec2 = a.vec2;
+    e.out2_h = (__half*)a.oh; e.out2_l = (__half*)a.ol; e.ldh = a.ldh; e.plane_act = a.plane_act; e.plane_slope = a.plane_slope;
+    e.skip = a.skip; e.ld_skip = a.ld_skip; e.C = a.C; e.skip_init = a.skip_init;
+    return conv_gemm(c, g);
+  }
+  GemmTC g = make_gemm_tc(w.ct, s, (const __half*)a.a_hi, (const __half*)a.a_lo);
+  EpiTC& e = g.e;
+  e.mode = a.mode; e.out = a.out; e.ldo = a.ldo;
+  e.oh = (__half*)a.oh; e.ol = (__half*)a.ol; e.ldh = a.ldh;
+  e.add = a.add; e.ld_add = a.ld_add; e.res = a.res; e.ld_res = a.ld_res;
+  e.rh = (const __half*)a.rh; e.rl = (const __half*)a.rl; e.ld_rh = a.ld_rh; e.vec1 = a.vec1; e.beta = a.beta;
+  e.vec2 = a.vec2; e.skip = a.skip; e.ld_skip = a.ld_skip; e.C = a.C; e.skip_init = a.skip_init;
+  e.act = a.act; e.act_slope = a.act_slope; e.accum = a.accum; e.gamma = a.gamma;
+  e.plane_act = a.plane_act; e.plane_slope = a.plane_slope; e.alpha = a.alpha; e.rowmask = a.rowmask;
+  e.n_valid = a.n_valid; e.skip_tiled = a.skip_tiled; e.out_nb = a.out_nb; e.out_bs = a.out_bs;
+  e.sh = (__half*)a.sh; e.sl = (__half*)a.sl;
+  return conv_gemm_tc(c, g);
+}
+
+// Waits for the call's work, frees its workspace and reports an asynchronous failure.
+static int op_finish(void* ws, void* stream, int rc, const char* what) {
+  const cudaError_t se = cudaStreamSynchronize((cudaStream_t)stream);
+  cudaFree(ws);
+  if (rc == 0 && se != cudaSuccess) {
+    ssb::set_error(std::string(what) + ": " + cudaGetErrorString(se));
+    rc = -2;
+  }
+  return rc;
+}
+
 extern "C" {
 
 int ssb_version(void) { return 101; }
@@ -791,19 +870,46 @@ int ssb_model_set_persistent_groups(ssb_model_t* m, int32_t enable) {
   return m->m.persistent_groups ? 1 : 0;
 }
 
+int ssb_mel_postprocess(float* mel, int64_t n_frames, float vmin, float vmax, int32_t* nonzero_frames, void* stream) {
+  SSB_CHECK(mel && nonzero_frames && n_frames >= 0, "bad argument");
+  return mel_postprocess_flat((cudaStream_t)stream, mel, n_frames, vmin, vmax, nonzero_frames);
+}
+int64_t ssb_launch_count(void) { return (int64_t)ssb::g_launches.load(); }
+int32_t ssb_set_attention_tensor_cores(int32_t enable) { return ssb::set_attention_tc_enabled(enable); }
+int64_t ssb_variant_launch_count(const char* variant) { return variant ? (int64_t)ssb::variant_launch_count(variant) : 0; }
+int32_t ssb_variant_names(char* buf, int32_t cap) { return buf && cap > 0 ? ssb::variant_names(buf, cap) : 0; }
+void ssb_tensor_map_cache_stats(int64_t* encodes, int64_t* hits) {
+  long long e = 0, h = 0;
+  ssb::tensor_map_cache_stats(&e, &h);
+  if (encodes) *encodes = e;
+  if (hits) *hits = h;
+}
+
+int ssb_op_gemm(const ssb_op_gemm_args* a, void* stream) {
+  SSB_CHECK(a && a->frame_offsets && a->B >= 1, "ssb_op_gemm: null argument");
+  OpWeights w;
+  if (op_pack(*a, &w)) return -1;
+  SSB_CHECK(a->path == 1 ? (a->a_hi && a->a_lo) : a->a != nullptr, "ssb_op_gemm: no A operand");
+  Seq q;
+  q.build(a->frame_offsets, a->B);
+  SSB_CHECK(a->rows == q.rows(), "ssb_op_gemm: rows is " + std::to_string(a->rows) + ", the layout has " +
+                                     std::to_string(q.rows()));
+  const size_t bytes = ((size_t)q.ntiles() + (size_t)a->B + 2) * 48 + 4096;  // the layout tables only
+  void* ws = nullptr;
+  SSB_CUDA(cudaMalloc(&ws, bytes));
+  Ctx c = make_ctx(ws, bytes, stream);
+  SeqDev s;
+  int rc = upload_layout(c, q, 1, &s);
+  if (rc == 0) rc = op_launch(c, s, *a, w);
+  return op_finish(ws, stream, rc, "ssb_op_gemm");
+}
+
 int ssb_op_conv1d_tc(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
                      const float* b_host, int32_t N, int32_t k, int32_t dilation, float* out, void* stream) {
   SSB_CHECK(x && offsets && w_host && out, "null argument");
-  SSB_CHECK(tc_available(), "tensor-core path unavailable (cuTensorMapEncodeTiled)");
-  DevicePool pool;
-  HostTensor w, b;
-  w.data = w_host; w.shape = {N, Cin, k};
-  b.data = b_host; b.shape = {N};
-  Conv cv;
-  ConvTC ct;
-  if (pack_conv(pool, &w, b_host ? &b : nullptr, dilation, PACK_PLAIN, &cv)) return -1;
-  if (pack_conv_tc(pool, &w, dilation, PACK_PLAIN, cv.bias, &ct)) return -1;
-  SSB_CHECK(ct.ok, "shape not eligible for the tensor-core path (Cin % 64, N % 128)");
+  ssb_op_gemm_args a = op_args(1, offsets, B, Cin, w_host, b_host, N, k, dilation);
+  OpWeights w;
+  if (op_pack(a, &w)) return -1;
   Seq q;
   q.build(offsets, B);
   const size_t bytes = ((size_t)q.rows() * (2 * Cin + N + 8) + 8 * (size_t)q.ntiles() + 1024) * sizeof(float) + (1 << 16);
@@ -820,66 +926,37 @@ int ssb_op_conv1d_tc(const float* x, const int32_t* offsets, int32_t B, int32_t 
   if (rc == 0) rc = pack_rows(c, s, x, Cin, xg, Cin, Cin);
   if (rc == 0) rc = split_planes(c, xg, Cin, s.rows, Cin, 1.0f, xh, xl);
   if (rc == 0) {
-    GemmTC g = make_gemm_tc(ct, s, xh, xl);
-    g.e.out = og; g.e.ldo = N;
-    rc = conv_gemm_tc(c, g);
+    a.a_hi = xh; a.a_lo = xl; a.out = og; a.ldo = N;
+    rc = op_launch(c, s, a, w);
   }
   if (rc == 0) rc = unpack_rows(c, s, og, N, out, N, N);
-  cudaError_t se = cudaStreamSynchronize((cudaStream_t)stream);
-  cudaFree(ws);
-  if (rc == 0 && se != cudaSuccess) {
-    ssb::set_error(std::string("ssb_op_conv1d_tc: ") + cudaGetErrorString(se));
-    rc = -2;
-  }
-  return rc;
-}
-
-int ssb_mel_postprocess(float* mel, int64_t n_frames, float vmin, float vmax, int32_t* nonzero_frames, void* stream) {
-  SSB_CHECK(mel && nonzero_frames && n_frames >= 0, "bad argument");
-  return mel_postprocess_flat((cudaStream_t)stream, mel, n_frames, vmin, vmax, nonzero_frames);
-}
-int64_t ssb_launch_count(void) { return (int64_t)ssb::g_launches.load(); }
-int32_t ssb_set_attention_tensor_cores(int32_t enable) { return ssb::set_attention_tc_enabled(enable); }
-int64_t ssb_variant_launch_count(const char* variant) { return variant ? (int64_t)ssb::variant_launch_count(variant) : 0; }
-int32_t ssb_variant_names(char* buf, int32_t cap) { return buf && cap > 0 ? ssb::variant_names(buf, cap) : 0; }
-void ssb_tensor_map_cache_stats(int64_t* encodes, int64_t* hits) {
-  long long e = 0, h = 0;
-  ssb::tensor_map_cache_stats(&e, &h);
-  if (encodes) *encodes = e;
-  if (hits) *hits = h;
+  return op_finish(ws, stream, rc, "ssb_op_conv1d_tc");
 }
 
 int ssb_op_conv1d(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
                   const float* b_host, int32_t N, int32_t k, int32_t dilation, int32_t act, float* out, void* stream) {
   SSB_CHECK(x && offsets && w_host && out, "null argument");
-  DevicePool pool;
-  HostTensor w, b;
-  w.data = w_host; w.shape = {N, Cin, k};
-  b.data = b_host; b.shape = {N};
-  Conv cv;
-  if (pack_conv(pool, &w, b_host ? &b : nullptr, dilation, PACK_PLAIN, &cv)) return -1;
+  ssb_op_gemm_args a = op_args(0, offsets, B, Cin, w_host, b_host, N, k, dilation);
+  OpWeights w;
+  if (op_pack(a, &w)) return -1;
   Seq q;
   q.build(offsets, B);
   const size_t bytes = ((size_t)q.rows() * (Cin + N + 8) + 8 * (size_t)q.ntiles() + 1024) * sizeof(float) + (1 << 16);
   void* ws = nullptr;
   SSB_CUDA(cudaMalloc(&ws, bytes));
   Ctx c = make_ctx(ws, bytes, stream);
-  int rc = 0;
   SeqDev s;
-  rc = upload_layout(c, q, 1, &s);
+  int rc = upload_layout(c, q, 1, &s);
   float* xg = alloc_rows(c, s, Cin);
   float* og = alloc_rows(c, s, N);
   if (rc == 0 && c.failed) rc = -1;
   if (rc == 0) rc = pack_rows(c, s, x, Cin, xg, Cin, Cin);
   if (rc == 0) {
-    ConvGemm g = make_gemm(cv, s, xg, Cin);
-    g.e.act = act; g.e.out = og; g.e.ldo = N;
-    rc = conv_gemm(c, g);
+    a.a = xg; a.lda = Cin; a.act = act; a.out = og; a.ldo = N;
+    rc = op_launch(c, s, a, w);
   }
   if (rc == 0) rc = unpack_rows(c, s, og, N, out, N, N);
-  cudaStreamSynchronize((cudaStream_t)stream);
-  cudaFree(ws);
-  return rc;
+  return op_finish(ws, stream, rc, "ssb_op_conv1d");
 }
 
 int ssb_op_attention(const float* q, const float* k, const float* v, const int32_t* q_offsets,

@@ -4,9 +4,9 @@
 //   warp 0 (1 lane)  TMA producer: per K block loads A_hi, A_lo [128x64] and W_hi, W_lo [BNx64] (128B swizzle)
 //   warps 4-11       two consumer warpgroups: each issues the 3-product wgmma chain (M64 N=BN K16, fp32 accumulators in
 //                    registers) for its 64 rows, then runs the fused epilogue through shared-memory transpose buffers
-// smem ring: BN=128: 3 stages x 64 KB, BN=64: 4 stages x 48 KB; mbarriers full/empty per stage.  BN=64 is picked for
-// small problems (more CTAs in flight).  The CTA-pair variant (cluster of 2) gives each CTA its own row tile and one half
-// of a shared weight tile, which TMA multicasts into both CTAs.
+// smem ring: BN=128: 3 stages x 64 KB, BN=64: 4 stages x 48 KB; mbarriers full/empty per stage.  The single-CTA kernel
+// (BN=64) serves problems too small to fill the GPU with pairs.  The CTA-pair variant (cluster of 2, BN = 2 hb = 64 or 128)
+// gives each CTA its own row tile and one half of a shared weight tile, which TMA multicasts into both CTAs.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -654,7 +654,7 @@ std::atomic<long long>* variant_counter(const char* name) {
 const char* mode_name(int mode) { return mode == EPI_GATE ? "GATE" : (mode == EPI_RES_SKIP ? "RES_SKIP" : "GENERIC"); }
 
 // index into ConvTC::tm_hi / tm_lo of the weight descriptor whose box has `rows` rows
-constexpr int map_index(int rows) { return rows == 128 ? 0 : (rows == 64 ? 1 : 2); }
+constexpr int map_index(int rows) { return rows == 64 ? 0 : 1; }
 // Cluster (CTA-pair) kernels from DIFFERENT streams are ordered against each other on the device: two such kernels in
 // flight from two streams hung an earlier build of this library, and the cause was never isolated.  Each pair launch on a
 // new stream first waits (cudaStreamWaitEvent) for the last pair launch of any other stream; same-stream launches are
@@ -772,14 +772,10 @@ void tensor_map_cache_stats(long long* encodes, long long* hits) {
 
 int make_weight_maps(ConvTC* w) {
   SSB_CHECK(w->Cin % BK == 0 && w->N % 64 == 0, "tensor-core path needs Cin % 64 == 0 and N % 64 == 0");
-  if (w->N % 128 == 0) {
-    if (make_map(&w->tm_hi[0], w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 128)) return -1;
-    if (make_map(&w->tm_lo[0], w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 128)) return -1;
-  }
-  if (make_map(&w->tm_hi[1], w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 64)) return -1;
-  if (make_map(&w->tm_lo[1], w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 64)) return -1;
-  if (make_map(&w->tm_hi[2], w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 32)) return -1;
-  if (make_map(&w->tm_lo[2], w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 32)) return -1;
+  if (make_map(&w->tm_hi[0], w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 64)) return -1;
+  if (make_map(&w->tm_lo[0], w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 64)) return -1;
+  if (make_map(&w->tm_hi[1], w->W_hi, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 32)) return -1;
+  if (make_map(&w->tm_lo[1], w->W_lo, (uint64_t)w->taps * w->N, (uint64_t)w->Cin, 32)) return -1;
   // CTA-pair kernel: each CTA of the pair loads hb weight rows of a 2*hb-wide N tile
   w->hb = w->N % 128 == 0 ? 64 : 32;
   w->ok = true;
@@ -809,10 +805,9 @@ int conv_gemm_tc(Ctx& ctx, const GemmTC& p) {
     }
     return w.hb == 64 ? launch<128, 2>(ctx, p, tp, num_sms) : launch<64, 2>(ctx, p, tp, num_sms);
   }
-  // small problems: 64-wide N tiles keep more SMs busy and shorten each tile's dependent chain
-  const bool small = (w.N % 128 != 0) || (int64_t)p.ntiles * (w.N / 128) < (int64_t)num_sms * 2;
-  if (small) return launch<64, 1>(ctx, p, tp, num_sms);
-  return launch<128, 1>(ctx, p, tp, num_sms);
+  // smaller problems: single CTAs on 64-wide N tiles.  (A 128-wide single-CTA tile would need ntiles * N / 128 >= 2 #SMs,
+  // which already meets the pair condition above when N % 128 == 0: it is never reached, so it is not built.)
+  return launch<64, 1>(ctx, p, tp, num_sms);
 }
 
 int split_planes(Ctx& ctx, const float* x, int ld, int64_t rows, int C, float scale, __half* hi, __half* lo) {

@@ -7,10 +7,11 @@
 //
 // Layout: A = activation planes [rows, C] fp16 row-major (guard-banded rows, see common.cuh), loaded by
 // TMA as [128 rows x 64 ch] boxes with 128B swizzle at row offset (tap - center) * dilation;
-// B = weights [taps*N, Cin] fp16 (K-major), boxes [BN n x 64 ch] (single-CTA kernel) or [hb x 64] (CTA-pair kernel:
-// each CTA of a 2-CTA cluster loads its own 128 rows of A and half of a 2*hb-wide weight tile, multicast to both CTAs).
-// CTAs are persistent over the tiles.  The pair kernel is used when there are >= num_SMs pair tiles, the 64-wide
-// single-CTA kernel for small problems, the 128-wide one otherwise (conv_gemm_tc()).
+// B = weights [taps*N, Cin] fp16 (K-major), boxes [64 n x 64 ch] (single-CTA kernel) or [hb x 64] (CTA-pair kernel:
+// each CTA of a 2-CTA cluster loads its own 128 rows of A and half of a 2*hb-wide weight tile, multicast to both CTAs;
+// hb = 64 when N % 128 == 0, else 32).  CTAs are persistent over the tiles.  The pair kernel is used when there are
+// >= num_SMs pair tiles (ceil(ntiles / 2) * N / (2 hb)), the single-CTA kernel with 64-wide N tiles otherwise
+// (conv_gemm_tc()).
 // 3-tap convs at pair sizes take the tap-reuse variant: one halo-extended activation tile per K block serves all three taps.
 // Pair launches from different streams are ordered against each other on the device (conv_gemm_tc.cu).
 #pragma once
@@ -24,7 +25,7 @@ namespace ssb {
 struct ConvTC {            // packed weights for the tensor-core path
   __half* W_hi = nullptr;  // [taps][N][Cin]
   __half* W_lo = nullptr;
-  CUtensorMap tm_hi[3], tm_lo[3];  // weight boxes of [0]: 128 rows, [1]: 64 rows, [2]: 32 rows
+  CUtensorMap tm_hi[2], tm_lo[2];  // weight boxes of [0]: 64 rows, [1]: 32 rows
   int hb = 0;                       // CTA-pair kernel: weight rows each CTA of a pair loads (half of a 2*hb-wide N tile)
   int taps = 1, Cin = 0, N = 0, dil = 1, center = 0;
   const float* bias = nullptr;  // [N] (packed column order)

@@ -693,7 +693,7 @@ static int persistent_net_maps(const PersistentNet& p, const SeqDev& s, int cs, 
   const Denoiser& d = *p.d;
   for (int i = 0; i < PersistentNet::NPL; ++i)
     if (make_act_map(&maps[p.mb + i], p.pl[i], s.rows, d.C, 128 / cs)) return -1;
-  auto put = [&](int idx, const ConvTC& w) { maps[idx] = w.tm_hi[1]; maps[idx + 1] = w.tm_lo[1]; };
+  auto put = [&](int idx, const ConvTC& w) { maps[idx] = w.tm_hi[0]; maps[idx + 1] = w.tm_lo[0]; };
   for (int l = 0; l < d.L; ++l) {
     put(p.w_layer(l), d.layers[l].dil.t);
     put(p.w_layer(l) + 2, d.layers[l].outp.t);
@@ -765,7 +765,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
     if (persistent_net_maps(net, s, CS, maps.data())) return -1;
     if (make_act_map(&maps[M_X80], x80h, s.rows, 128, 128 / CS)) return -1;
     if (make_act_map(&maps[M_X80 + 1], x80l, s.rows, 128, 128 / CS)) return -1;
-    maps[W_IN] = d.in_tc.tm_hi[1]; maps[W_IN + 1] = d.in_tc.tm_lo[1];
+    maps[W_IN] = d.in_tc.tm_hi[0]; maps[W_IN + 1] = d.in_tc.tm_lo[0];
     std::vector<SPhase> ph;
     ph.reserve((size_t)nph);
     for (int t = K - 1; t >= 0; --t) {

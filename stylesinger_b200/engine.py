@@ -786,6 +786,36 @@ def op_conv1d_tc(x, offsets, w, b, dilation=1):
     return out
 
 
+_OP_GEMM_BUFFERS = ("a", "a_hi", "a_lo", "add", "res", "rowmask", "out", "out2", "vec1", "vec2", "oh", "ol", "skip", "rh", "rl",
+                    "sh", "sl")
+
+
+def op_gemm(path, offsets, rows, w, b=None, dilation=1, gate=False, **epi):
+    """Exactly one conv_gemm (path 0, fp32 FFMA) or conv_gemm_tc (path 1, tensor cores) call (ssb_op_gemm) over
+    caller-owned device tensors in the guard-banded layout of `offsets` with `rows` rows (utterance b at rows
+    [rs_b, rs_b + L_b), rs_0 = 16, rs_{b+1} = rs_b + L_b + 16, plus 256 rows of tail slack).  w [N, Cin, k] / b [N]
+    are torch-layout weights (gate=True: the DiffNet gate interleave).  epi: the A operand (a / lda / a_act / a_slope /
+    a_scale on path 0, a_hi / a_lo on path 1) and the fields of ssb_op_gemm_args' epilogue; tensors are passed by
+    pointer, nothing is copied.  Returns nothing: the kernel writes into the given buffers."""
+    _require_cuda()
+    off = np.ascontiguousarray(offsets, np.int32)
+    N, Cin, k = w.shape
+    wc = w.detach().cpu().float().contiguous()
+    bc = None if b is None else b.detach().cpu().float().contiguous()
+    a = _lib.OpGemmArgs(path=path, frame_offsets=off.ctypes.data, B=len(off) - 1, rows=rows, Cin=Cin, N=N, k=k,
+                        dilation=dilation, gate=int(gate), w_host=wc.data_ptr(), b_host=None if bc is None else bc.data_ptr(),
+                        a_slope=0.1, a_scale=1.0, alpha=1.0, act_slope=0.1, beta=1.0, gamma=1.0, plane_slope=0.1)
+    dev = None
+    for name, v in epi.items():
+        if name in _OP_GEMM_BUFFERS:
+            if v is not None:
+                dev = v.device
+                v = _ptr(v).value
+        setattr(a, name, v)
+    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    check(lib.ssb_op_gemm(C.byref(a), stream), "ssb_op_gemm")
+
+
 def op_attention(q, k, v, q_offsets, k_offsets, scale, tc=False, keymask=None):
     """tc=True: the wgmma / TMA kernel (ssb_op_attention_tc) instead of the fp32 one.  keymask: optional [sumS] tensor on
     q's device, 0 = masked key (ssb_op_attention_masked); an utterance whose keys are all masked gets NaN rows."""

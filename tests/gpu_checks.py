@@ -29,15 +29,15 @@ def split(x, offs):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# which tensor-core GEMM variants a call must launch: conv_gemm_tc's dispatch (CTA pairs, with the tap-reuse kernel for
-# 3-tap GATE / GENERIC convs, when ceil(ntiles / 2) * N / (2 hb) >= #SMs, hb = 64 if N % 128 == 0 else 32; else 64-wide
-# N tiles when N % 128 != 0 or ntiles * N / 128 < 2 #SMs; else 128-wide) over the denoiser's GEMMs
-def variant(nt, N, mode, taps):
+# which tensor-core GEMM variants a call must launch: conv_gemm_tc's dispatch.  CTA pairs when ceil(ntiles / 2) * N / (2 hb)
+# >= #SMs, hb = 64 if N % 128 == 0 else 32, on the tap-reuse kernel for 3-tap GATE / GENERIC convs of dilation <= 8;
+# else single CTAs with 64-wide N tiles
+def variant(nt, N, mode, taps, dil=1):
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     hb = 64 if N % 128 == 0 else 32
     if ((nt + 1) // 2) * (N // (2 * hb)) >= sms:
-        return f"tc2{'r' if taps == 3 and mode != 'RES_SKIP' else ''}<{hb},{mode}>"
-    return f"tc<64,{mode}>" if N % 128 != 0 or nt * (N // 128) < 2 * sms else f"tc<128,{mode}>"
+        return f"tc2{'r' if taps == 3 and dil <= 8 and mode != 'RES_SKIP' else ''}<{hb},{mode}>"
+    return f"tc<64,{mode}>"
 
 
 def count(gemms, nt):

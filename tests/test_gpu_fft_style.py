@@ -22,6 +22,7 @@ import torch
 from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
 from tests.common import acoustic_engine, acoustic_sd, acoustic_sd64, golden, hp_for, registry_inputs
+from tests.gpu_checks import variant
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -88,19 +89,12 @@ def _report(name, errs, bars):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# which tensor-core GEMM variants a call must launch (conv_gemm_tc's dispatch: CTA pairs when ceil(ntiles / 2) * N / 128
-# >= #SMs, else 64-wide N tiles when ntiles * N / 128 < 2 * #SMs); the FFMA path (< 8 row tiles) launches none
-def _variant(nt, N):
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    if ((nt + 1) // 2) * (N // 128) >= sms:
-        return "tc2<64,GENERIC>"
-    return "tc<64,GENERIC>" if nt * (N // 128) < 2 * sms else "tc<128,GENERIC>"
-
-
+# which tensor-core GEMM variants a call must launch (conv_gemm_tc's dispatch, tests/gpu_checks.py; none of these GEMMs is a
+# 3-tap conv, so none takes the tap-reuse kernel); the FFMA path (< 8 row tiles) launches none
 def _expect(gemms):
     out = {}
     for nt, N in gemms:
-        k = _variant(nt, N)
+        k = variant(nt, N, "GENERIC", 1)
         out[k] = out.get(k, 0) + 1
     return out
 

@@ -7,7 +7,6 @@ Tolerances: mel L-inf < 1e-3 (north_star); waveform from the ORACLE's mel < 1e-3
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import stylesinger_oracle as O
 from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG
@@ -195,34 +194,6 @@ def test_f0_sampler_T100_pair_kernels_vs_oracle_two_utterances_of_the_batch():
         total += Fr
     print(f"f0 sampler T=100 inside a {n}-frame batch (pair kernels {ran}) vs oracle: {agree}/{total} frames agree")
     assert agree >= 0.99 * total
-
-
-# ---------------------------------------------------------------------------------------------------
-# (c) every kernel variant by name: CTA pairs (hb = 64 / 32 by N; tap reuse for 3-tap convs) and the single-CTA 64-wide tiles
-@pytest.mark.parametrize("cin,n_out,k,dil,reps,variant", [(256, 512, 3, 4, 1, "tc2r<64,GENERIC>"), (256, 384, 3, 2, 1, "tc2r<64,GENERIC>"),
-                                                         (256, 512, 3, 8, 1, "tc2r<64,GENERIC>"), (256, 512, 3, 1, 1, "tc2r<64,GENERIC>"),
-                                                         (256, 512, 1, 1, 1, "tc2<64,GENERIC>"), (192, 384, 5, 1, 1, "tc2<64,GENERIC>"),
-                                                         (128, 128, 7, 1, 2, "tc2<64,GENERIC>"), (64, 64, 11, 1, 2, "tc2<32,GENERIC>"),
-                                                         (128, 128, 3, 1, 1, "tc<64,GENERIC>")])
-def test_conv1d_tc_variant_by_name(cin, n_out, k, dil, reps, variant):
-    from stylesinger_b200.engine import op_conv1d_tc
-    g = torch.Generator().manual_seed(5 + n_out + k)
-    lens = [2800, 1500, 2999, 700, 2100, 1900, 2500, 3000, 1234, 2222] * reps + [77]
-    offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
-    x = torch.randn(int(offs[-1]), cin, generator=g)
-    w = torch.randn(n_out, cin, k, generator=g) / (cin * k) ** 0.5
-    b = torch.randn(n_out, generator=g)
-    before = _variants()
-    y = op_conv1d_tc(x.to(DEV), offs, w, b, dilation=dil).cpu()
-    ran = _delta(before, _variants())
-    assert ran == {variant: 1}, ran
-    worst = 0.0
-    for i in (0, 3, len(lens) // 2, len(lens) - 1):
-        xi = x[offs[i]:offs[i + 1]].t()[None]
-        ref = F.conv1d(xi, w, b, padding=dil * (k - 1) // 2, dilation=dil)[0].t()
-        worst = max(worst, _maxabs(y[offs[i]:offs[i + 1]], ref))
-    print(f"{variant}: {cin}->{n_out} k{k} on {int(offs[-1])} rows, max err {worst:.3e}")
-    assert worst < 1e-4
 
 
 # ---------------------------------------------------------------------------------------------------

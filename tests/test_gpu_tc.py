@@ -3,7 +3,6 @@ and against the reference-generated goldens; and SIMT-vs-tensor-core agreement o
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import stylesinger_oracle as O
 from tests.common import acoustic_engine, acoustic_sd, golden, hp_for
@@ -16,49 +15,6 @@ def _maxabs(a, b):
     a = a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
     b = b.detach().cpu().numpy() if isinstance(b, torch.Tensor) else np.asarray(b)
     return float(np.abs(a.astype(np.float64) - b.astype(np.float64)).max())
-
-
-@pytest.mark.parametrize("cin,n,k,dil", [(64, 128, 1, 1), (256, 512, 1, 1), (256, 512, 3, 8), (192, 384, 3, 2),
-                                         (192, 384, 1, 1), (256, 256, 3, 1)])
-def test_conv1d_tc_matches_torch(cin, n, k, dil):
-    from stylesinger_b200.engine import op_conv1d_tc
-    g = torch.Generator().manual_seed(cin + n + k)
-    lens = [5, 131, 64, 300, 128]
-    offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
-    x = torch.randn(int(offs[-1]), cin, generator=g) * 2.0
-    w = torch.randn(n, cin, k, generator=g) / (cin * k) ** 0.5
-    b = torch.randn(n, generator=g)
-    y = op_conv1d_tc(x.to(DEV), offs, w, b, dilation=dil).cpu()
-    worst = 0.0
-    for i in range(len(lens)):
-        xi = x[offs[i]:offs[i + 1]].t()[None].double()
-        ref = F.conv1d(xi, w.double(), b.double(), padding=dil * (k - 1) // 2, dilation=dil)[0].t()
-        worst = max(worst, _maxabs(y[offs[i]:offs[i + 1]], ref))
-    print(f"tc conv {cin}->{n} k{k} d{dil}: max err {worst:.3e}")
-    assert worst < 1e-4  # tensor-core fp32 accumulation truncates: ~1e-5 relative after 144 chained MMAs
-
-
-@pytest.mark.parametrize("cin,n_out,k,dil,reps,extra", [(256, 512, 3, 4, 1, 0), (256, 384, 3, 4, 1, 0), (256, 512, 3, 2, 1, 100),
-                                                       (192, 384, 1, 1, 1, 77), (128, 128, 7, 1, 1, 0), (64, 64, 11, 1, 2, 5),
-                                                       (64, 2048, 3, 1, 1, 0)])
-def test_conv1d_tc_large_problem_uses_cta_pairs(cin, n_out, k, dil, reps, extra):
-    """Enough row tiles for the CTA-pair kernel (2-CTA clusters, two row tiles x one 2*hb-wide N tile, the weight tile
-    multicast to both; hb = 64 / 32 by N): persistent tile loop, odd tile counts (the peer CTA of the last pair idles)."""
-    from stylesinger_b200.engine import op_conv1d_tc
-    g = torch.Generator().manual_seed(11 + n_out + k)
-    lens = [2800, 1500, 2999, 700, 2100, 1900, 2500, 3000, 1234, 2222] * reps + ([extra] if extra else [])
-    offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
-    x = torch.randn(int(offs[-1]), cin, generator=g)
-    w = torch.randn(n_out, cin, k, generator=g) / (cin * k) ** 0.5
-    b = torch.randn(n_out, generator=g)
-    y = op_conv1d_tc(x.to(DEV), offs, w, b, dilation=dil).cpu()
-    worst = 0.0
-    for i in (0, 3, 9, len(lens) - 1):
-        xi = x[offs[i]:offs[i + 1]].t()[None]
-        ref = F.conv1d(xi, w, b, padding=dil * (k - 1) // 2, dilation=dil)[0].t()
-        worst = max(worst, _maxabs(y[offs[i]:offs[i + 1]], ref))
-    print(f"tc conv large {cin}->{n_out} k{k}: max err {worst:.3e}")
-    assert worst < 1e-4
 
 
 def test_denoiser_large_batch_pair_kernel_matches_simt():

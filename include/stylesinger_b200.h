@@ -443,6 +443,9 @@ void ssb_tensor_map_cache_stats(int64_t* encodes, int64_t* hits);
  * (common_layers.py:277-286) and of the style aligner's cross-attention (lse.py:41); short batches always use the fp32
  * kernel.  Returns the new state. */
 int32_t ssb_set_attention_tensor_cores(int32_t enable);
+/* Launches so far of the fp32 attention kernel (tc = 0, csrc/attention.cu) or of the wgmma attention kernel (tc = 1,
+ * csrc/attention_tc.cu); any other tc returns 0.  Kept apart from ssb_variant_names, which lists GEMM variants only. */
+int64_t ssb_attention_launch_count(int32_t tc);
 
 /* Unit-test granularity: one Conv1d over ragged rows with torch-layout HOST weights [N,Cin,k]
  * (packs on the fly with cudaMalloc; not for production use).  act: 0 none 1 relu 2 gelu 3 leaky(0.1) 4 tanh. */
@@ -520,6 +523,48 @@ int ssb_op_attention_tc(const float* q, const float* k, const float* v, const in
 int ssb_op_attention_masked(const float* q, const float* k, const float* v, const int32_t* q_offsets,
                             const int32_t* k_offsets, int32_t B, float scale, const float* keymask, int32_t tc, float* out,
                             void* stream);
+/* Unit-test granularity: exactly ONE attention call - the fp32 kernel (path 0, csrc/attention.cu) or the wgmma kernel
+ * (path 1, csrc/attention_tc.cu) - over CALLER-OWNED device buffers in the guard-banded layouts of q_offsets (queries,
+ * rows_q rows) and k_offsets (keys and values, rows_k rows): utterance b at rows [rs_b, rs_b + L_b), rs_0 = 16,
+ * rs_{b+1} = rs_b + L_b + 16, and rows_* must be rs_{B-1} + L_{B-1} + 16 + 256 (tail slack).  Query utterance b attends to
+ * key utterance b; head h (of `heads`, 128 columns each) reads columns 128 h of each operand's window.  Nothing is copied
+ * in or out; rows outside the utterances are never written.
+ *   path 0: q / k / v fp32 [rows, ld*] (column windows by pointer offset, as the FFT blocks pass qkv + 256); output fp32
+ *           out [rows_q, ldo] only; qcol0 / kcol0 / vcol0 must be 0.
+ *   path 1: q_hi / q_lo, k_hi / k_lo, v_hi / v_lo fp16 planes [rows, ld*] with the window at column *col0; V's planes are
+ *           transposed into the call's own V^T scratch (ldvt = (rows_k + 7) & ~7) first, as the stage drivers do (one
+ *           transpose_planes launch).  Output fp32 out [rows_q, ldo], fp16 planes oh / ol [rows_q, ldh], or both.
+ * keymask: optional guarded device [rows_k], 0 = masked key.  An utterance with no valid key gets NaN rows.
+ * Refused before any launch: a path other than 0 / 1; no output, or a plane output on path 0; fp32 lds not multiples of 4
+ * or fp32 pointers not 16-byte aligned; path 1 lds or column offsets not multiples of 8, or planes not 16-byte aligned; a
+ * column window past its ld; heads outside {1, 2}; rows_q / rows_k that do not match their layout; B > 65535.  The stage
+ * drivers' attention calls make the same checks. */
+typedef struct ssb_op_attention_args {
+  int32_t path;                 /* 0: fp32 kernel, 1: wgmma kernel */
+  const int32_t* q_offsets;     /* host [B + 1] */
+  const int32_t* k_offsets;     /* host [B + 1] */
+  int32_t B;
+  int64_t rows_q, rows_k;
+  int32_t heads;
+  float scale;                  /* applied to q */
+  const float* keymask;
+  const float* q;               /* path 0 */
+  const float* k;
+  const float* v;
+  const void* q_hi;             /* path 1 */
+  const void* q_lo;
+  const void* k_hi;
+  const void* k_lo;
+  const void* v_hi;
+  const void* v_lo;
+  int32_t ldq, qcol0, ldk, kcol0, ldv, vcol0;
+  float* out;
+  int32_t ldo;
+  void* oh;                     /* path 1 */
+  void* ol;
+  int32_t ldh;
+} ssb_op_attention_args;
+int ssb_op_attention_ex(const ssb_op_attention_args* a, void* stream);
 
 #ifdef __cplusplus
 }

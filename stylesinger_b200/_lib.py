@@ -71,6 +71,19 @@ class OpGemmArgs(C.Structure):
                 ("sl", C.c_void_p), ("n_valid", C.c_int32)]
 
 
+class OpAttentionArgs(C.Structure):
+    """ssb_op_attention_args: one attention_kernel (path 0) or attention_tc_kernel (path 1) call over caller-owned
+    device buffers."""
+    _fields_ = [("path", C.c_int32), ("q_offsets", C.c_void_p), ("k_offsets", C.c_void_p), ("B", C.c_int32),
+                ("rows_q", C.c_int64), ("rows_k", C.c_int64), ("heads", C.c_int32), ("scale", C.c_float),
+                ("keymask", C.c_void_p), ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p),
+                ("q_hi", C.c_void_p), ("q_lo", C.c_void_p), ("k_hi", C.c_void_p), ("k_lo", C.c_void_p),
+                ("v_hi", C.c_void_p), ("v_lo", C.c_void_p),
+                ("ldq", C.c_int32), ("qcol0", C.c_int32), ("ldk", C.c_int32), ("kcol0", C.c_int32), ("ldv", C.c_int32),
+                ("vcol0", C.c_int32), ("out", C.c_void_p), ("ldo", C.c_int32), ("oh", C.c_void_p), ("ol", C.c_void_p),
+                ("ldh", C.c_int32)]
+
+
 # every symbol declared in include/stylesinger_b200.h (tests/test_abi.py checks this list against the header)
 EXPORTS = [
     "ssb_version", "ssb_last_error", "ssb_model_create", "ssb_model_free", "ssb_model_set_schedule",
@@ -94,6 +107,7 @@ EXPORTS = [
     "ssb_acoustic_forward_keyed", "ssb_hifigan_generate_keyed",
     "ssb_vocoder_create_ex",
     "ssb_op_gemm",
+    "ssb_op_attention_ex", "ssb_attention_launch_count",
 ]
 
 
@@ -148,6 +162,8 @@ def _load():
         "ssb_vocoder_set_tensor_cores": (C.c_int, [vp, i32]),
         "ssb_op_conv1d_tc": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, vp]),
         "ssb_op_gemm": (C.c_int, [P(OpGemmArgs), vp]),
+        "ssb_op_attention_ex": (C.c_int, [P(OpAttentionArgs), vp]),
+        "ssb_attention_launch_count": (C.c_int64, [i32]),
         "ssb_fft_workspace_bytes": (sz, [vp, i32, vp, i32]),
         "ssb_fft_encoder": (C.c_int, [vp, vp, vp, i32, vp, vp, sz, vp]),
         "ssb_fft_decoder": (C.c_int, [vp, vp, vp, i32, vp, vp, sz, vp]),

@@ -395,6 +395,36 @@ static int op_finish(void* ws, void* stream, int rc, const char* what) {
   return rc;
 }
 
+// ---- one attention call at unit-test granularity (ssb_op_attention_ex and the tight-row ssb_op_attention*) -----------
+// Path 1 first transposes V's planes into V^T scratch taken from c, as the stage drivers do.  Every check of the call
+// runs before that transpose, so a refused call launches nothing.
+static int op_attn_launch(Ctx& c, const SeqDev& dq, const SeqDev& dk, const ssb_op_attention_args& a) {
+  if (a.path == 0) {
+    AttnArgs t;
+    t.utt_q = dq.utt; t.utt_k = dk.utt; t.B = a.B; t.max_q = dq.maxlen; t.heads = a.heads;
+    t.Q = a.q; t.ldq = a.ldq; t.K = a.k; t.ldk = a.ldk; t.V = a.v; t.ldv = a.ldv;
+    t.keymask = a.keymask; t.scale = a.scale; t.out = a.out; t.ldo = a.ldo;
+    return attention(c, t);
+  }
+  AttnTCArgs t;
+  t.utt_q = dq.utt; t.utt_k = dk.utt; t.B = a.B; t.max_q = dq.maxlen; t.heads = a.heads;
+  t.Qh = (const __half*)a.q_hi; t.Ql = (const __half*)a.q_lo; t.rows_q = dq.rows; t.ldq = a.ldq; t.qcol0 = a.qcol0;
+  t.Kh = (const __half*)a.k_hi; t.Kl = (const __half*)a.k_lo; t.rows_k = dk.rows; t.ldk = a.ldk; t.kcol0 = a.kcol0;
+  t.ldvt = (dk.rows + 7) & ~int64_t(7);
+  t.keymask = a.keymask; t.scale = a.scale;
+  t.out = a.out; t.ldo = a.ldo; t.oh = (__half*)a.oh; t.ol = (__half*)a.ol; t.ldh = a.ldh;
+  if (attention_tc_check(t)) return -1;  // before the V^T scratch exists; it comes from c, 256-byte aligned
+  const int w = a.heads * 128;
+  SSB_CHECK(a.ldv % 8 == 0 && a.vcol0 >= 0 && a.vcol0 % 8 == 0 && a.vcol0 + w <= a.ldv,
+            "op_attention: V's ldv and vcol0 must be multiples of 8 and vcol0 + heads x 128 must not exceed ldv");
+  __half* vth = c.alloc<__half>((size_t)t.ldvt * w);
+  __half* vtl = c.alloc<__half>((size_t)t.ldvt * w);
+  SSB_CHECK(!c.failed, "op_attention: workspace too small");
+  t.Vth = vth; t.Vtl = vtl;
+  if (transpose_planes(c, (const __half*)a.v_hi, (const __half*)a.v_lo, a.ldv, a.vcol0, dk.rows, w, vth, vtl, t.ldvt)) return -1;
+  return attention_tc(c, t);
+}
+
 extern "C" {
 
 int ssb_version(void) { return 101; }
@@ -876,6 +906,7 @@ int ssb_mel_postprocess(float* mel, int64_t n_frames, float vmin, float vmax, in
 }
 int64_t ssb_launch_count(void) { return (int64_t)ssb::g_launches.load(); }
 int32_t ssb_set_attention_tensor_cores(int32_t enable) { return ssb::set_attention_tc_enabled(enable); }
+int64_t ssb_attention_launch_count(int32_t tc) { return tc == 0 || tc == 1 ? (int64_t)ssb::g_attn_launches[tc].load() : 0; }
 int64_t ssb_variant_launch_count(const char* variant) { return variant ? (int64_t)ssb::variant_launch_count(variant) : 0; }
 int32_t ssb_variant_names(char* buf, int32_t cap) { return buf && cap > 0 ? ssb::variant_names(buf, cap) : 0; }
 void ssb_tensor_map_cache_stats(int64_t* encodes, int64_t* hits) {
@@ -998,37 +1029,65 @@ int ssb_op_attention_masked(const float* q, const float* k, const float* v, cons
   if (rc == 0) rc = pack_rows(c, dk, k, 256, kg, 256, 256);
   if (rc == 0) rc = pack_rows(c, dk, v, 256, vg, 256, 256);
   if (rc == 0 && mg) rc = pack_rows(c, dk, keymask, 1, mg, 1, 1);
+  ssb_op_attention_args a;
+  memset(&a, 0, sizeof(a));
+  a.path = tc ? 1 : 0; a.B = B; a.heads = 2; a.scale = scale; a.keymask = mg;
+  a.ldq = a.ldk = a.ldv = 256; a.out = og; a.ldo = 256;
   if (rc == 0 && !tc) {
-    AttnArgs a;
-    a.utt_q = dq.utt; a.utt_k = dk.utt; a.B = B; a.max_q = dq.maxlen; a.heads = 2;
-    a.Q = qg; a.ldq = 256; a.K = kg; a.ldk = 256; a.V = vg; a.ldv = 256; a.keymask = mg; a.scale = scale;
-    a.out = og; a.ldo = 256;
-    rc = attention(c, a);
+    a.q = qg; a.k = kg; a.v = vg;
+    rc = op_attn_launch(c, dq, dk, a);
   }
   if (rc == 0 && tc) {
     __half* pl[6];  // q, k, v planes (hi, lo)
     for (int i = 0; i < 6; ++i) pl[i] = c.alloc<__half>((size_t)(i < 2 ? dq.rows : dk.rows) * 256);
-    __half* vth = c.alloc<__half>((size_t)ldvt * 256);
-    __half* vtl = c.alloc<__half>((size_t)ldvt * 256);
     if (c.failed) rc = -1;
     if (rc == 0) rc = split_planes(c, qg, 256, dq.rows, 256, 1.0f, pl[0], pl[1]);
     if (rc == 0) rc = split_planes(c, kg, 256, dk.rows, 256, 1.0f, pl[2], pl[3]);
     if (rc == 0) rc = split_planes(c, vg, 256, dk.rows, 256, 1.0f, pl[4], pl[5]);
-    if (rc == 0) rc = transpose_planes(c, pl[4], pl[5], 256, 0, dk.rows, 256, vth, vtl, ldvt);
     if (rc == 0) {
-      AttnTCArgs a;
-      a.utt_q = dq.utt; a.utt_k = dk.utt; a.B = B; a.max_q = dq.maxlen; a.heads = 2;
-      a.Qh = pl[0]; a.Ql = pl[1]; a.rows_q = dq.rows; a.ldq = 256;
-      a.Kh = pl[2]; a.Kl = pl[3]; a.rows_k = dk.rows; a.ldk = 256;
-      a.Vth = vth; a.Vtl = vtl; a.ldvt = ldvt;
-      a.keymask = mg; a.scale = scale; a.out = og; a.ldo = 256;
-      rc = attention_tc(c, a);
+      a.q_hi = pl[0]; a.q_lo = pl[1]; a.k_hi = pl[2]; a.k_lo = pl[3]; a.v_hi = pl[4]; a.v_lo = pl[5];
+      rc = op_attn_launch(c, dq, dk, a);
     }
   }
   if (rc == 0) rc = unpack_rows(c, dq, og, 256, out, 256, 256);
   cudaStreamSynchronize((cudaStream_t)stream);
   cudaFree(ws);
   return rc;
+}
+
+int ssb_op_attention_ex(const ssb_op_attention_args* a, void* stream) {
+  SSB_CHECK(a && a->q_offsets && a->k_offsets && a->B >= 1, "ssb_op_attention_ex: null argument");
+  SSB_CHECK(a->path == 0 || a->path == 1, "ssb_op_attention_ex: path must be 0 (fp32 kernel) or 1 (wgmma kernel)");
+  SSB_CHECK(a->B <= 65535, "ssb_op_attention_ex: B = " + std::to_string(a->B) + " exceeds gridDim.z (65535)");
+  if (a->path == 0) {
+    SSB_CHECK(a->q && a->k && a->v, "ssb_op_attention_ex: path 0 needs fp32 q, k and v");
+    SSB_CHECK(a->out && !a->oh && !a->ol, "ssb_op_attention_ex: path 0 writes fp32 out only (no planes)");
+    SSB_CHECK(a->qcol0 == 0 && a->kcol0 == 0 && a->vcol0 == 0,
+              "ssb_op_attention_ex: path 0 takes column windows as pointer offsets (qcol0 / kcol0 / vcol0 must be 0)");
+  } else {
+    SSB_CHECK(tc_available(), "tensor-core path unavailable (cuTensorMapEncodeTiled)");
+    SSB_CHECK(a->q_hi && a->q_lo && a->k_hi && a->k_lo && a->v_hi && a->v_lo, "ssb_op_attention_ex: path 1 needs q, k and v planes");
+    SSB_CHECK(a->out || (a->oh && a->ol), "ssb_op_attention_ex: no output");
+  }
+  Seq sq, sk;
+  sq.build(a->q_offsets, a->B);
+  sk.build(a->k_offsets, a->B);
+  SSB_CHECK(a->rows_q == sq.rows(), "ssb_op_attention_ex: rows_q is " + std::to_string(a->rows_q) + ", the query layout has " +
+                                        std::to_string(sq.rows()));
+  SSB_CHECK(a->rows_k == sk.rows(), "ssb_op_attention_ex: rows_k is " + std::to_string(a->rows_k) + ", the key layout has " +
+                                        std::to_string(sk.rows()));
+  const int64_t ldvt = (sk.rows() + 7) & ~int64_t(7);
+  // the layout tables, and on path 1 the V^T scratch (2 planes of at most 256 x ldvt halves)
+  const size_t bytes = ((size_t)sq.ntiles() + (size_t)sk.ntiles() + 2 * (size_t)a->B + 4) * 48 + 4096 +
+                       (a->path == 1 ? (size_t)ldvt * 256 * 2 * sizeof(__half) + 512 : 0);
+  void* ws = nullptr;
+  SSB_CUDA(cudaMalloc(&ws, bytes));
+  Ctx c = make_ctx(ws, bytes, stream);
+  SeqDev dq, dk;
+  int rc = upload_layout(c, sq, 1, &dq);
+  if (rc == 0) rc = upload_layout(c, sk, 1, &dk);
+  if (rc == 0) rc = op_attn_launch(c, dq, dk, *a);
+  return op_finish(ws, stream, rc, "ssb_op_attention_ex");
 }
 
 }  // extern "C"

@@ -156,7 +156,24 @@ __global__ void __launch_bounds__(256, 1) attention_kernel(AttnArgs a) {
 
 }  // namespace
 
+std::atomic<long long> g_attn_launches[2];
+
+int attention_check(const AttnArgs& a) {
+  SSB_CHECK(a.heads == 1 || a.heads == 2, "attention: heads must be 1 or 2, got " + std::to_string(a.heads));
+  SSB_CHECK(a.B >= 0 && a.B <= 65535, "attention: B = " + std::to_string(a.B) + " exceeds gridDim.z (65535)");
+  SSB_CHECK(a.out != nullptr, "attention: no output");
+  SSB_CHECK(a.ldq % 4 == 0 && a.ldk % 4 == 0 && a.ldv % 4 == 0 && a.ldo % 4 == 0,
+            "attention: ldq / ldk / ldv / ldo must be multiples of 4 (float4 loads and stores)");
+  SSB_CHECK(((uintptr_t)a.Q | (uintptr_t)a.K | (uintptr_t)a.V | (uintptr_t)a.out) % 16 == 0,
+            "attention: Q, K, V and out must be 16-byte aligned (float4 loads and stores)");
+  const int w = a.heads * HD;
+  SSB_CHECK(a.ldq >= w && a.ldk >= w && a.ldv >= w && a.ldo >= w,
+            "attention: an ld is narrower than heads x 128 = " + std::to_string(w) + " columns");
+  return 0;
+}
+
 int attention(Ctx& ctx, const AttnArgs& a) {
+  if (attention_check(a)) return -1;
   if (ctx.dry || a.B == 0 || a.max_q == 0) return 0;
   {  // the attribute is per device (one process may drive several GPUs)
     static std::atomic<bool> configured[64];
@@ -172,6 +189,7 @@ int attention(Ctx& ctx, const AttnArgs& a) {
   attention_kernel<<<grid, 256, sizeof(AttnSmem), ctx.stream>>>(a);
   SSB_CUDA(cudaGetLastError());
   ++g_launches;
+  ++g_attn_launches[0];
   return 0;
 }
 

@@ -17,6 +17,10 @@ struct AttnArgs {
   float* out = nullptr; int ldo = 0;
 };
 
+// attention() refuses (before any launch) heads outside {1, 2}, B > 65535 (gridDim.z), no output, an ld that is not a
+// multiple of 4 or a pointer that is not 16-byte aligned (the float4 loads and stores), and an ld narrower than heads x 128
+// columns.  attention_check() is that check alone, for callers that must refuse before launching anything else.
+int attention_check(const AttnArgs& a);
 int attention(Ctx& ctx, const AttnArgs& a);
 
 // wgmma / TMA attention for long batches (attention_tc.cu).  Operands are fp16 hi/lo planes:
@@ -35,10 +39,18 @@ struct AttnTCArgs {
   float* out = nullptr; int ldo = 0;
   __half* oh = nullptr; __half* ol = nullptr; int ldh = 0;
 };
+// attention_tc() refuses (before any launch) heads outside {1, 2}, B > 65535, no output (out, or both planes), an ld or
+// column offset that is not a multiple of 8 (TMA strides and inner coordinates are 16-byte multiples), a pointer that is
+// not 16-byte aligned, a column window past its ld (qcol0 + heads x 128 > ldq, kcol0 + heads x 128 > ldk: TMA would
+// read zero fill), an output narrower than heads x 128 columns, and V^T narrower than the key rows (ldvt < rows_k).
+int attention_tc_check(const AttnTCArgs& a);
 int attention_tc(Ctx& ctx, const AttnTCArgs& a);
-bool attention_tc_enabled();           // process-wide switch for the long-batch paths (ssb_set_attention_tensor_cores; default on)
+// launches so far of attention_kernel [0] and attention_tc_kernel [1] (ssb_attention_launch_count)
+extern std::atomic<long long> g_attn_launches[2];
+bool attention_tc_enabled();          // process-wide switch for the long-batch paths (ssb_set_attention_tensor_cores; default on)
 int set_attention_tc_enabled(int on);
-// planes [rows, ld] (columns col0 .. col0 + C) -> transposed planes [C, ldt]; columns rows .. ldt are zero-filled
+// planes [rows, ld] (columns col0 .. col0 + C) -> transposed planes [C, ldt]; columns rows .. ldt are zero-filled.
+// Refuses C not a multiple of 32, ldt < rows and a column window col0 + C past ld.
 int transpose_planes(Ctx& ctx, const __half* xh, const __half* xl, int ld, int col0, int64_t rows, int C, __half* th, __half* tl,
                      int64_t ldt);
 

@@ -304,8 +304,8 @@ int set_attention_tc_enabled(int on) {
 
 int transpose_planes(Ctx& ctx, const __half* xh, const __half* xl, int ld, int col0, int64_t rows, int C, __half* th, __half* tl,
                      int64_t ldt) {
+  SSB_CHECK(C % 32 == 0 && ldt >= rows && col0 >= 0 && col0 + C <= ld, "transpose_planes: bad shape");
   if (ctx.dry || rows == 0) return 0;
-  SSB_CHECK(C % 32 == 0 && ldt >= rows, "transpose_planes: bad shape");
   dim3 grid((unsigned)((ldt + 31) / 32), (unsigned)(C / 32));
   k_transpose_planes<<<grid, 256, 0, ctx.stream>>>(xh, xl, ld, col0, rows, th, tl, ldt);
   SSB_CUDA(cudaGetLastError());
@@ -313,10 +313,30 @@ int transpose_planes(Ctx& ctx, const __half* xh, const __half* xl, int ld, int c
   return 0;
 }
 
-int attention_tc(Ctx& ctx, const AttnTCArgs& a) {
-  if (ctx.dry || a.B == 0 || a.max_q == 0) return 0;
-  SSB_CHECK(a.heads * HD <= 256 && a.ldvt % 8 == 0 && a.ldq % 8 == 0 && a.ldk % 8 == 0, "attention_tc: bad layout");
+int attention_tc_check(const AttnTCArgs& a) {
+  SSB_CHECK(a.heads == 1 || a.heads == 2, "attention_tc: heads must be 1 or 2, got " + std::to_string(a.heads));
+  SSB_CHECK(a.B >= 0 && a.B <= 65535, "attention_tc: B = " + std::to_string(a.B) + " exceeds gridDim.z (65535)");
   SSB_CHECK(a.out || (a.oh && a.ol), "attention_tc: no output");
+  SSB_CHECK(a.ldq % 8 == 0 && a.ldk % 8 == 0 && a.ldvt % 8 == 0 && a.ldo % 8 == 0 && a.ldh % 8 == 0,
+            "attention_tc: ldq / ldk / ldvt / ldo / ldh must be multiples of 8");
+  SSB_CHECK(a.qcol0 >= 0 && a.kcol0 >= 0 && a.qcol0 % 8 == 0 && a.kcol0 % 8 == 0,
+            "attention_tc: qcol0 / kcol0 must be non-negative multiples of 8 (TMA inner coordinates)");
+  SSB_CHECK(((uintptr_t)a.Qh | (uintptr_t)a.Ql | (uintptr_t)a.Kh | (uintptr_t)a.Kl | (uintptr_t)a.Vth | (uintptr_t)a.Vtl |
+             (uintptr_t)a.out | (uintptr_t)a.oh | (uintptr_t)a.ol) % 16 == 0,
+            "attention_tc: every operand and output must be 16-byte aligned");
+  const int w = a.heads * HD;
+  SSB_CHECK(a.qcol0 + w <= a.ldq, "attention_tc: Q columns qcol0 + heads x 128 = " + std::to_string(a.qcol0 + w) +
+                                      " exceed ldq = " + std::to_string(a.ldq));
+  SSB_CHECK(a.kcol0 + w <= a.ldk, "attention_tc: K columns kcol0 + heads x 128 = " + std::to_string(a.kcol0 + w) +
+                                      " exceed ldk = " + std::to_string(a.ldk));
+  SSB_CHECK((!a.out || a.ldo >= w) && (!a.oh || a.ldh >= w), "attention_tc: an output ld is narrower than heads x 128");
+  SSB_CHECK(a.ldvt >= a.rows_k, "attention_tc: ldvt is smaller than the key rows");
+  return 0;
+}
+
+int attention_tc(Ctx& ctx, const AttnTCArgs& a) {
+  if (attention_tc_check(a)) return -1;
+  if (ctx.dry || a.B == 0 || a.max_q == 0) return 0;
   {
     static std::atomic<bool> configured[64];
     int dev = 0;
@@ -342,6 +362,7 @@ int attention_tc(Ctx& ctx, const AttnTCArgs& a) {
   attention_tc_kernel<<<grid, ATT_THREADS, ATT_SMEM, ctx.stream>>>(mq_h, mq_l, mk_h, mk_l, mv_h, mv_l, p);
   SSB_CUDA(cudaGetLastError());
   ++g_launches;
+  ++g_attn_launches[1];
   return 0;
 }
 

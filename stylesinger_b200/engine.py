@@ -816,6 +816,31 @@ def op_gemm(path, offsets, rows, w, b=None, dilation=1, gate=False, **epi):
     check(lib.ssb_op_gemm(C.byref(a), stream), "ssb_op_gemm")
 
 
+_OP_ATTN_BUFFERS = ("keymask", "q", "k", "v", "q_hi", "q_lo", "k_hi", "k_lo", "v_hi", "v_lo", "out", "oh", "ol")
+
+
+def op_attention_ex(path, q_offsets, k_offsets, rows_q, rows_k, scale, heads=2, **bufs):
+    """Exactly one attention_kernel (path 0, fp32) or attention_tc_kernel (path 1, wgmma) call (ssb_op_attention_ex) over
+    caller-owned device tensors in the guard-banded layouts of q_offsets (rows_q rows) and k_offsets (rows_k rows), the
+    layout of op_gemm.  bufs: the operands (q / k / v on path 0, q_hi ... v_lo on path 1), keymask, out / oh / ol, and the
+    ints ldq, qcol0, ldk, kcol0, ldv, vcol0, ldo, ldh; tensors are passed by pointer (a view's offset included), nothing
+    is copied.  Returns nothing: the kernel writes into the given buffers."""
+    _require_cuda()
+    qo = np.ascontiguousarray(q_offsets, np.int32)
+    ko = np.ascontiguousarray(k_offsets, np.int32)
+    a = _lib.OpAttentionArgs(path=path, q_offsets=qo.ctypes.data, k_offsets=ko.ctypes.data, B=len(qo) - 1, rows_q=rows_q,
+                             rows_k=rows_k, heads=heads, scale=float(scale))
+    dev = None
+    for name, v in bufs.items():
+        if name in _OP_ATTN_BUFFERS:
+            if v is not None:
+                dev = v.device
+                v = _ptr(v).value
+        setattr(a, name, v)
+    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    check(lib.ssb_op_attention_ex(C.byref(a), stream), "ssb_op_attention_ex")
+
+
 def op_attention(q, k, v, q_offsets, k_offsets, scale, tc=False, keymask=None):
     """tc=True: the wgmma / TMA kernel (ssb_op_attention_tc) instead of the fp32 one.  keymask: optional [sumS] tensor on
     q's device, 0 = masked key (ssb_op_attention_masked); an utterance whose keys are all masked gets NaN rows."""

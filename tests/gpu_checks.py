@@ -93,6 +93,7 @@ class Err:
 
     def __init__(self):
         self.v = {"interior": (0.0, None), "edge": (0.0, None)}
+        self.interior_rows = 0
 
     def add(self, i, a, b):
         e = rel(a, b)
@@ -100,6 +101,7 @@ class Err:
         edge = torch.zeros(n, dtype=torch.bool)
         edge[:EDGE_ROWS] = True
         edge[-EDGE_ROWS:] = True
+        self.interior_rows += int((~edge).sum())
         for k, rows in (("edge", edge), ("interior", ~edge)):
             if rows.any():
                 sub = torch.where(rows[:, None], e, torch.zeros_like(e))
@@ -115,4 +117,5 @@ class Err:
         (vi, wi), (ve, we) = self.v["interior"], self.v["edge"]
         print(f"{tag}: interior {vi:.3e} at (utterance, row, column) {wi}, edge {ve:.3e} at {we} (bar {bar:.1e})")
         assert self.max() <= bar, (tag, self.v, bar)
-        assert ve <= 4 * vi, (tag, "edge rows err more than 4x the interior", self.v)
+        if self.interior_rows:  # utterances of at most 2 x EDGE_ROWS rows have no interior to compare with
+            assert ve <= 4 * vi, (tag, "edge rows err more than 4x the interior", self.v)

@@ -21,24 +21,6 @@ def _maxabs(a, b):
     return float(np.abs(a.astype(np.float64) - b.astype(np.float64)).max())
 
 
-def test_attention_op_matches_torch():
-    from stylesinger_b200.engine import op_attention
-    g = torch.Generator().manual_seed(3)
-    ql, kl = [70, 1, 200], [33, 150, 64]
-    qo = np.concatenate([[0], np.cumsum(ql)]).astype(np.int32)
-    ko = np.concatenate([[0], np.cumsum(kl)]).astype(np.int32)
-    q = torch.randn(int(qo[-1]), 256, generator=g)
-    k = torch.randn(int(ko[-1]), 256, generator=g)
-    v = torch.randn(int(ko[-1]), 256, generator=g)
-    out = op_attention(q.to(DEV), k.to(DEV), v.to(DEV), qo, ko, 128 ** -0.5).cpu()
-    for i in range(3):
-        qi, ki, vi = q[qo[i]:qo[i + 1]], k[ko[i]:ko[i + 1]], v[ko[i]:ko[i + 1]]
-        for h in range(2):
-            s = (qi[:, h * 128:(h + 1) * 128] * 128 ** -0.5) @ ki[:, h * 128:(h + 1) * 128].t()
-            ref = torch.softmax(s, -1) @ vi[:, h * 128:(h + 1) * 128]
-            assert _maxabs(out[qo[i]:qo[i + 1], h * 128:(h + 1) * 128], ref) < 2e-5
-
-
 # ---------------------------------------------------------------------------------------------------
 def test_denoisers_match_reference_golden():
     g, meta = golden("ref_small_T4")

@@ -175,34 +175,6 @@ def test_decoder_fft_ffn_tensor_cores_match_ffma():
     assert err < 1e-4 * max(1.0, scale)
 
 
-# ---------------------------------------------------------------------------------------------------
-# wgmma / TMA attention kernel (csrc/attention_tc.cu) against torch fp32 (float64 accumulation as the arbiter)
-@pytest.mark.parametrize("ql,kl", [([70, 1, 200], [33, 150, 64]),            # ragged, single-tile keys, 1-row query
-                                   ([2812, 300, 129], [2812, 300, 129]),    # self-attention at the longest bench utterance
-                                   ([1500, 2200], [1125, 1125])])           # the style aligner's cross-attention shape
-def test_attention_tc_op_matches_torch(ql, kl):
-    from stylesinger_b200.engine import op_attention
-    g = torch.Generator().manual_seed(3 + len(ql) + ql[0])
-    qo = np.concatenate([[0], np.cumsum(ql)]).astype(np.int32)
-    ko = np.concatenate([[0], np.cumsum(kl)]).astype(np.int32)
-    q = torch.randn(int(qo[-1]), 256, generator=g) * 1.5
-    k = torch.randn(int(ko[-1]), 256, generator=g) * 1.5
-    v = torch.randn(int(ko[-1]), 256, generator=g)
-    out = op_attention(q.to(DEV), k.to(DEV), v.to(DEV), qo, ko, 128 ** -0.5, tc=True).cpu()
-    simt = op_attention(q.to(DEV), k.to(DEV), v.to(DEV), qo, ko, 128 ** -0.5).cpu()
-    worst = 0.0
-    for i in range(len(ql)):
-        qi, ki, vi = q[qo[i]:qo[i + 1]].double(), k[ko[i]:ko[i + 1]].double(), v[ko[i]:ko[i + 1]].double()
-        for h in range(2):
-            s = (qi[:, h * 128:(h + 1) * 128] * 128 ** -0.5) @ ki[:, h * 128:(h + 1) * 128].t()
-            ref = torch.softmax(s, -1) @ vi[:, h * 128:(h + 1) * 128]
-            worst = max(worst, float((out[qo[i]:qo[i + 1], h * 128:(h + 1) * 128].double() - ref).abs().max()))
-    print(f"attention_tc {ql} x {kl}: L-inf vs float64 {worst:.3e}; fp32 kernel vs tc {float((out - simt).abs().max()):.3e}")
-    # 3-pass fp16-split MMAs with the tensor core's fp32 accumulation over up to 44 key tiles: same error class as the other
-    # wgmma GEMMs (3e-5 at T=100); the fp32 kernel itself sits ~1e-5 from the float64 result at these lengths
-    assert torch.isfinite(out).all() and worst < 5e-5
-
-
 ATTN_TC_DEFAULT = 1  # library default of the switch (csrc/attention_tc.cu attention_tc_enabled)
 
 

@@ -350,10 +350,6 @@ int ssb_model_set_persistent_groups(ssb_model_t* m, int32_t enable);
  * new setting. */
 int ssb_model_set_fft_tensor_cores(ssb_model_t* m, int32_t enable);
 
-/* Unit-test granularity: ssb_op_conv1d through the tensor-core path (Cin % 64 == 0, N % 64 == 0, no activation). */
-int ssb_op_conv1d_tc(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
-                     const float* b_host, int32_t N, int32_t k, int32_t dilation, float* out, void* stream);
-
 /* StyleSingerInfer.forward_model glue between model and vocoder (inference/StyleSinger.py:56-58):
  * clips mel [n_frames,80] in place to [vmin, vmax] and counts the frames with sum|mel| > 0 into
  * *nonzero_frames (device int32; the reference drops all-zero frames, which only padding can produce). */
@@ -447,11 +443,6 @@ int32_t ssb_set_attention_tensor_cores(int32_t enable);
  * csrc/attention_tc.cu); any other tc returns 0.  Kept apart from ssb_variant_names, which lists GEMM variants only. */
 int64_t ssb_attention_launch_count(int32_t tc);
 
-/* Unit-test granularity: one Conv1d over ragged rows with torch-layout HOST weights [N,Cin,k]
- * (packs on the fly with cudaMalloc; not for production use).  act: 0 none 1 relu 2 gelu 3 leaky(0.1) 4 tanh. */
-int ssb_op_conv1d(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
-                  const float* b_host, int32_t N, int32_t k, int32_t dilation, int32_t act, float* out, void* stream);
-
 /* Unit-test granularity: exactly ONE dense GEMM - the fp32 FFMA kernel (path 0, csrc/conv_gemm.cu) or the tensor-core
  * kernel (path 1, csrc/conv_gemm_tc.cu) - with any epilogue, over CALLER-OWNED device buffers in the guard-banded layout
  * of frame_offsets: utterance b occupies rows [rs_b, rs_b + L_b), rs_0 = 16, rs_{b+1} = rs_b + L_b + 16, and `rows` must
@@ -508,21 +499,6 @@ typedef struct ssb_op_gemm_args {
   int32_t n_valid;
 } ssb_op_gemm_args;
 int ssb_op_gemm(const ssb_op_gemm_args* a, void* stream);
-/* Unit-test granularity: multi-head attention, 2 heads x 128; q [sumL,256], k/v [sumS,256]. */
-int ssb_op_attention(const float* q, const float* k, const float* v, const int32_t* q_offsets,
-                     const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream);
-/* Same contract on the wgmma / TMA attention kernel (csrc/attention_tc.cu; 3-pass fp16 hi/lo split MMAs for QK^T and PV,
- * TMA-staged K / V^T tiles), the path long batches take inside the FFT blocks (common_layers.py:277-286) and the style
- * aligner (lse.py:41). */
-int ssb_op_attention_tc(const float* q, const float* k, const float* v, const int32_t* q_offsets,
-                        const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream);
-/* Either kernel (tc = 0: fp32, tc = 1: wgmma) with a key-padding mask: keymask is a device array [sumS] in the tight
- * layout of k, 0 = masked (the -inf of key_padding_mask), anything else = attend.  Both kernels write NaN for every query
- * of an utterance whose keys are all masked (or that has no keys), as torch's softmax over all -inf does; the other
- * utterances of the batch are unaffected. */
-int ssb_op_attention_masked(const float* q, const float* k, const float* v, const int32_t* q_offsets,
-                            const int32_t* k_offsets, int32_t B, float scale, const float* keymask, int32_t tc, float* out,
-                            void* stream);
 /* Unit-test granularity: exactly ONE attention call - the fp32 kernel (path 0, csrc/attention.cu) or the wgmma kernel
  * (path 1, csrc/attention_tc.cu) - over CALLER-OWNED device buffers in the guard-banded layouts of q_offsets (queries,
  * rows_q rows) and k_offsets (keys and values, rows_k rows): utterance b at rows [rs_b, rs_b + L_b), rs_0 = 16,

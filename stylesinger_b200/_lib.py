@@ -90,16 +90,15 @@ EXPORTS = [
     "ssb_durations_workspace_bytes", "ssb_predict_durations", "ssb_acoustic_workspace_bytes", "ssb_acoustic_forward",
     "ssb_mel_diffusion_workspace_bytes", "ssb_mel_diffusion_sample", "ssb_denoiser_eval", "ssb_f0_diffusion_sample",
     "ssb_rvq_lookup", "ssb_vocoder_create", "ssb_vocoder_free", "ssb_vocoder_workspace_bytes", "ssb_hifigan_generate",
-    "ssb_op_conv1d", "ssb_op_attention", "ssb_mel_postprocess", "ssb_launch_count",
-    "ssb_model_set_tensor_cores", "ssb_op_conv1d_tc", "ssb_model_set_persistent", "ssb_model_set_fft_tensor_cores",
+    "ssb_mel_postprocess", "ssb_launch_count",
+    "ssb_model_set_tensor_cores", "ssb_model_set_persistent", "ssb_model_set_fft_tensor_cores",
     "ssb_vocoder_set_tensor_cores", "ssb_variant_launch_count", "ssb_variant_names", "ssb_tensor_map_cache_stats",
     "ssb_model_set_persistent_groups", "ssb_mel_diffusion_plms_workspace_bytes",
     "ssb_mel_diffusion_sample_plms", "ssb_fft_workspace_bytes", "ssb_fft_encoder", "ssb_fft_decoder",
-    "ssb_get_style_workspace_bytes", "ssb_get_style", "ssb_op_attention_tc", "ssb_set_attention_tensor_cores",
+    "ssb_get_style_workspace_bytes", "ssb_get_style", "ssb_set_attention_tensor_cores",
     "ssb_melspec_create", "ssb_melspec_free", "ssb_melspec_num_frames", "ssb_melspec_workspace_bytes", "ssb_melspec_forward",
     "ssb_melspec_create_ex", "ssb_lstm_encoder_create", "ssb_lstm_encoder_free", "ssb_lstm_encoder_workspace_bytes", "ssb_lstm_encoder_forward",
     "ssb_model_create_ex", "ssb_mel_prodiff_workspace_bytes", "ssb_mel_prodiff_sample",
-    "ssb_op_attention_masked",
     "ssb_model_create_ex2", "ssb_pitch_predictor_workspace_bytes", "ssb_pitch_predictor",
     "ssb_wav_denoise_create", "ssb_wav_denoise_free", "ssb_wav_denoise_workspace_bytes", "ssb_wav_denoise_forward",
     "ssb_wav_denoise_set_tensor_cores",
@@ -149,10 +148,6 @@ def _load():
         "ssb_vocoder_workspace_bytes": (sz, [vp, vp, i32]),
         "ssb_hifigan_generate": (C.c_int, [vp, vp, vp, vp, i32, vp, vp, u64, vp, vp, sz, vp]),
         "ssb_hifigan_generate_keyed": (C.c_int, [vp, vp, vp, vp, i32, vp, vp, vp, sz, vp]),
-        "ssb_op_conv1d": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, i32, i32, i32, vp, vp]),
-        "ssb_op_attention": (C.c_int, [vp, vp, vp, vp, vp, i32, C.c_float, vp, vp]),
-        "ssb_op_attention_tc": (C.c_int, [vp, vp, vp, vp, vp, i32, C.c_float, vp, vp]),
-        "ssb_op_attention_masked": (C.c_int, [vp, vp, vp, vp, vp, i32, C.c_float, vp, i32, vp, vp]),
         "ssb_mel_postprocess": (C.c_int, [vp, C.c_int64, C.c_float, C.c_float, vp, vp]),
         "ssb_launch_count": (C.c_int64, []),
         "ssb_model_set_tensor_cores": (C.c_int, [vp, i32]),
@@ -160,7 +155,6 @@ def _load():
         "ssb_model_set_persistent_groups": (C.c_int, [vp, i32]),
         "ssb_model_set_fft_tensor_cores": (C.c_int, [vp, i32]),
         "ssb_vocoder_set_tensor_cores": (C.c_int, [vp, i32]),
-        "ssb_op_conv1d_tc": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, vp]),
         "ssb_op_gemm": (C.c_int, [P(OpGemmArgs), vp]),
         "ssb_op_attention_ex": (C.c_int, [P(OpAttentionArgs), vp]),
         "ssb_attention_launch_count": (C.c_int64, [i32]),

@@ -316,23 +316,12 @@ static Ctx make_ctx(void* ws, size_t bytes, void* stream, bool dry = false) {
   return c;
 }
 
-// ---- one dense GEMM at unit-test granularity (ssb_op_gemm, ssb_op_conv1d, ssb_op_conv1d_tc) --------------------------
+// ---- one dense GEMM at unit-test granularity (ssb_op_gemm) ---------------------------------------------------------------
 struct OpWeights {  // the call's packed weights, freed with the pool when the call returns
   DevicePool pool;
   Conv cv;
   ConvTC ct;
 };
-
-static ssb_op_gemm_args op_args(int path, const int32_t* offsets, int B, int Cin, const float* w_host, const float* b_host,
-                                int N, int k, int dilation) {
-  ssb_op_gemm_args a;
-  memset(&a, 0, sizeof(a));
-  a.path = path; a.frame_offsets = offsets; a.B = B;
-  a.Cin = Cin; a.N = N; a.k = k; a.dilation = dilation; a.w_host = w_host; a.b_host = b_host;
-  a.a_slope = a.act_slope = a.plane_slope = 0.1f;
-  a.a_scale = a.alpha = a.beta = a.gamma = 1.0f;
-  return a;
-}
 
 // Packs the host weights for the call's path.  A conv whose taps reach past the guard band would read the neighbouring
 // utterance (or, for the first one, whatever lies before the buffer), so it is refused here, before anything is launched.
@@ -395,7 +384,7 @@ static int op_finish(void* ws, void* stream, int rc, const char* what) {
   return rc;
 }
 
-// ---- one attention call at unit-test granularity (ssb_op_attention_ex and the tight-row ssb_op_attention*) -----------
+// ---- one attention call at unit-test granularity (ssb_op_attention_ex) ---------------------------------------------------
 // Path 1 first transposes V's planes into V^T scratch taken from c, as the stage drivers do.  Every check of the call
 // runs before that transpose, so a refused call launches nothing.
 static int op_attn_launch(Ctx& c, const SeqDev& dq, const SeqDev& dk, const ssb_op_attention_args& a) {
@@ -427,7 +416,7 @@ static int op_attn_launch(Ctx& c, const SeqDev& dq, const SeqDev& dk, const ssb_
 
 extern "C" {
 
-int ssb_version(void) { return 101; }
+int ssb_version(void) { return 102; }
 const char* ssb_last_error(void) { return ssb::last_error(); }
 
 int ssb_model_create(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp) {
@@ -933,126 +922,6 @@ int ssb_op_gemm(const ssb_op_gemm_args* a, void* stream) {
   int rc = upload_layout(c, q, 1, &s);
   if (rc == 0) rc = op_launch(c, s, *a, w);
   return op_finish(ws, stream, rc, "ssb_op_gemm");
-}
-
-int ssb_op_conv1d_tc(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
-                     const float* b_host, int32_t N, int32_t k, int32_t dilation, float* out, void* stream) {
-  SSB_CHECK(x && offsets && w_host && out, "null argument");
-  ssb_op_gemm_args a = op_args(1, offsets, B, Cin, w_host, b_host, N, k, dilation);
-  OpWeights w;
-  if (op_pack(a, &w)) return -1;
-  Seq q;
-  q.build(offsets, B);
-  const size_t bytes = ((size_t)q.rows() * (2 * Cin + N + 8) + 8 * (size_t)q.ntiles() + 1024) * sizeof(float) + (1 << 16);
-  void* ws = nullptr;
-  SSB_CUDA(cudaMalloc(&ws, bytes));
-  Ctx c = make_ctx(ws, bytes, stream);
-  SeqDev s;
-  int rc = upload_layout(c, q, 1, &s);
-  float* xg = alloc_rows(c, s, Cin);
-  float* og = alloc_rows(c, s, N);
-  __half* xh = c.alloc<__half>((size_t)s.rows * Cin);
-  __half* xl = c.alloc<__half>((size_t)s.rows * Cin);
-  if (rc == 0 && c.failed) rc = -1;
-  if (rc == 0) rc = pack_rows(c, s, x, Cin, xg, Cin, Cin);
-  if (rc == 0) rc = split_planes(c, xg, Cin, s.rows, Cin, 1.0f, xh, xl);
-  if (rc == 0) {
-    a.a_hi = xh; a.a_lo = xl; a.out = og; a.ldo = N;
-    rc = op_launch(c, s, a, w);
-  }
-  if (rc == 0) rc = unpack_rows(c, s, og, N, out, N, N);
-  return op_finish(ws, stream, rc, "ssb_op_conv1d_tc");
-}
-
-int ssb_op_conv1d(const float* x, const int32_t* offsets, int32_t B, int32_t Cin, const float* w_host,
-                  const float* b_host, int32_t N, int32_t k, int32_t dilation, int32_t act, float* out, void* stream) {
-  SSB_CHECK(x && offsets && w_host && out, "null argument");
-  ssb_op_gemm_args a = op_args(0, offsets, B, Cin, w_host, b_host, N, k, dilation);
-  OpWeights w;
-  if (op_pack(a, &w)) return -1;
-  Seq q;
-  q.build(offsets, B);
-  const size_t bytes = ((size_t)q.rows() * (Cin + N + 8) + 8 * (size_t)q.ntiles() + 1024) * sizeof(float) + (1 << 16);
-  void* ws = nullptr;
-  SSB_CUDA(cudaMalloc(&ws, bytes));
-  Ctx c = make_ctx(ws, bytes, stream);
-  SeqDev s;
-  int rc = upload_layout(c, q, 1, &s);
-  float* xg = alloc_rows(c, s, Cin);
-  float* og = alloc_rows(c, s, N);
-  if (rc == 0 && c.failed) rc = -1;
-  if (rc == 0) rc = pack_rows(c, s, x, Cin, xg, Cin, Cin);
-  if (rc == 0) {
-    a.a = xg; a.lda = Cin; a.act = act; a.out = og; a.ldo = N;
-    rc = op_launch(c, s, a, w);
-  }
-  if (rc == 0) rc = unpack_rows(c, s, og, N, out, N, N);
-  return op_finish(ws, stream, rc, "ssb_op_conv1d");
-}
-
-int ssb_op_attention(const float* q, const float* k, const float* v, const int32_t* q_offsets,
-                     const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream) {
-  return ssb_op_attention_masked(q, k, v, q_offsets, k_offsets, B, scale, nullptr, 0, out, stream);
-}
-
-/* wgmma attention kernel at unit-test granularity: same contract as ssb_op_attention (fp32 in / out, tight rows) */
-int ssb_op_attention_tc(const float* q, const float* k, const float* v, const int32_t* q_offsets,
-                        const int32_t* k_offsets, int32_t B, float scale, float* out, void* stream) {
-  return ssb_op_attention_masked(q, k, v, q_offsets, k_offsets, B, scale, nullptr, 1, out, stream);
-}
-
-/* Either attention kernel with a key-padding mask (tight [sumS], 0 = masked), packed into the guarded layout the
- * FFT blocks and the style aligner hand the kernels. */
-int ssb_op_attention_masked(const float* q, const float* k, const float* v, const int32_t* q_offsets,
-                            const int32_t* k_offsets, int32_t B, float scale, const float* keymask, int32_t tc, float* out,
-                            void* stream) {
-  SSB_CHECK(q && k && v && q_offsets && k_offsets && out, "null argument");
-  SSB_CHECK(!tc || tc_available(), "tensor-core path unavailable (cuTensorMapEncodeTiled)");
-  Seq sq, sk;
-  sq.build(q_offsets, B);
-  sk.build(k_offsets, B);
-  const int64_t ldvt = (sk.rows() + 7) & ~int64_t(7);
-  const size_t bytes = ((size_t)sq.rows() * 768 + (size_t)sk.rows() * 1025 + (size_t)ldvt * 256 + 4096) * sizeof(float) + (1 << 16);
-  void* ws = nullptr;
-  SSB_CUDA(cudaMalloc(&ws, bytes));
-  Ctx c = make_ctx(ws, bytes, stream);
-  SeqDev dq, dk;
-  int rc = upload_layout(c, sq, 1, &dq);
-  if (rc == 0) rc = upload_layout(c, sk, 1, &dk);
-  float* qg = alloc_rows(c, dq, 256);
-  float* og = alloc_rows(c, dq, 256);
-  float* kg = alloc_rows(c, dk, 256);
-  float* vg = alloc_rows(c, dk, 256);
-  float* mg = keymask ? alloc_rows(c, dk, 1) : nullptr;
-  if (rc == 0 && c.failed) rc = -1;
-  if (rc == 0) rc = pack_rows(c, dq, q, 256, qg, 256, 256);
-  if (rc == 0) rc = pack_rows(c, dk, k, 256, kg, 256, 256);
-  if (rc == 0) rc = pack_rows(c, dk, v, 256, vg, 256, 256);
-  if (rc == 0 && mg) rc = pack_rows(c, dk, keymask, 1, mg, 1, 1);
-  ssb_op_attention_args a;
-  memset(&a, 0, sizeof(a));
-  a.path = tc ? 1 : 0; a.B = B; a.heads = 2; a.scale = scale; a.keymask = mg;
-  a.ldq = a.ldk = a.ldv = 256; a.out = og; a.ldo = 256;
-  if (rc == 0 && !tc) {
-    a.q = qg; a.k = kg; a.v = vg;
-    rc = op_attn_launch(c, dq, dk, a);
-  }
-  if (rc == 0 && tc) {
-    __half* pl[6];  // q, k, v planes (hi, lo)
-    for (int i = 0; i < 6; ++i) pl[i] = c.alloc<__half>((size_t)(i < 2 ? dq.rows : dk.rows) * 256);
-    if (c.failed) rc = -1;
-    if (rc == 0) rc = split_planes(c, qg, 256, dq.rows, 256, 1.0f, pl[0], pl[1]);
-    if (rc == 0) rc = split_planes(c, kg, 256, dk.rows, 256, 1.0f, pl[2], pl[3]);
-    if (rc == 0) rc = split_planes(c, vg, 256, dk.rows, 256, 1.0f, pl[4], pl[5]);
-    if (rc == 0) {
-      a.q_hi = pl[0]; a.q_lo = pl[1]; a.k_hi = pl[2]; a.k_lo = pl[3]; a.v_hi = pl[4]; a.v_lo = pl[5];
-      rc = op_attn_launch(c, dq, dk, a);
-    }
-  }
-  if (rc == 0) rc = unpack_rows(c, dq, og, 256, out, 256, 256);
-  cudaStreamSynchronize((cudaStream_t)stream);
-  cudaFree(ws);
-  return rc;
 }
 
 int ssb_op_attention_ex(const ssb_op_attention_args* a, void* stream) {

@@ -758,36 +758,61 @@ class LstmEncoder:
         return out
 
 
+def _guarded(offsets, device):
+    """Where the tight rows of the utterances at host offsets [B + 1] sit in the guard-banded layout of op_gemm and
+    op_attention_ex: (row of each tight row, on `device`; the layout's row count).  Utterance b starts at row
+    rs_b = 16 + off[b] + 16 b, and the layout has off[B] + 16 (B + 1) + 256 rows: 16 guard rows before and after every
+    utterance, then 256 rows of tail slack (Seq::build, GUARD and TAIL_SLACK in csrc/common.cuh)."""
+    off = np.ascontiguousarray(offsets, np.int64)
+    B = len(off) - 1
+    idx = np.arange(off[-1]) + 16 * np.repeat(np.arange(1, B + 1), np.diff(off))
+    return torch.from_numpy(idx).to(device), int(off[-1]) + 16 * (B + 1) + 256
+
+
+def _scatter(t, idx, rows):
+    """Tight rows t in a zeroed fp32 [rows, ...] buffer at the rows idx of _guarded."""
+    g = torch.zeros((rows,) + tuple(t.shape[1:]), dtype=torch.float32, device=idx.device)
+    g[idx] = t.to(g)
+    return g
+
+
+def _planes(x):
+    """fp16 hi / lo planes of fp32 x, bit for bit what k_split_planes writes: hi = fp16(x), lo = fp16(x - hi)."""
+    hi = x.half()
+    return hi, (x - hi.float()).half()
+
+
 def op_conv1d(x, offsets, w, b, dilation=1, act=0):
-    _require_cuda()
-    off = np.ascontiguousarray(offsets, np.int32)
-    N, Cin, k = w.shape
-    wc = w.detach().cpu().float().contiguous()
-    bc = None if b is None else b.detach().cpu().float().contiguous()
-    out = torch.empty((x.shape[0], N), dtype=torch.float32, device=x.device)
-    stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-    check(lib.ssb_op_conv1d(_ptr(x), off.ctypes.data, len(off) - 1, Cin, C.c_void_p(wc.data_ptr()),
-                            None if bc is None else C.c_void_p(bc.data_ptr()), N, k, dilation, act, _ptr(out), stream),
-          "ssb_op_conv1d")
-    return out
+    """One Conv1d on the fp32 FFMA GEMM (op_gemm path 0) over the tight rows x [sum L, Cin] of the utterances at host
+    offsets [B + 1], with torch-layout weights w [N, Cin, k] and bias b [N] (or None).  act: 0 none, 1 relu, 2 gelu,
+    3 leaky relu (slope 0.1), 4 tanh.  Returns the tight rows [sum L, N]."""
+    idx, rows = _guarded(offsets, x.device)
+    out = torch.empty(rows, w.shape[0], device=x.device)
+    op_gemm(0, offsets, rows, w, b, dilation=dilation, a=_scatter(x, idx, rows), lda=x.shape[1], act=act, out=out,
+            ldo=w.shape[0])
+    return out[idx]
 
 
 def op_conv1d_tc(x, offsets, w, b, dilation=1):
-    _require_cuda()
-    off = np.ascontiguousarray(offsets, np.int32)
-    N, Cin, k = w.shape
-    wc = w.detach().cpu().float().contiguous()
-    bc = None if b is None else b.detach().cpu().float().contiguous()
-    out = torch.empty((x.shape[0], N), dtype=torch.float32, device=x.device)
-    stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-    check(lib.ssb_op_conv1d_tc(_ptr(x), off.ctypes.data, len(off) - 1, Cin, C.c_void_p(wc.data_ptr()),
-                               None if bc is None else C.c_void_p(bc.data_ptr()), N, k, dilation, _ptr(out), stream),
-          "ssb_op_conv1d_tc")
-    return out
+    """op_conv1d (without activation) on the tensor-core GEMM (op_gemm path 1, Cin % 64 == 0, N % 64 == 0), x split
+    into fp16 hi / lo planes first."""
+    idx, rows = _guarded(offsets, x.device)
+    hi, lo = _planes(_scatter(x, idx, rows))
+    out = torch.empty(rows, w.shape[0], device=x.device)
+    op_gemm(1, offsets, rows, w, b, dilation=dilation, a_hi=hi, a_lo=lo, out=out, ldo=w.shape[0])
+    return out[idx]
 
 
-_OP_GEMM_BUFFERS = ("a", "a_hi", "a_lo", "add", "res", "rowmask", "out", "out2", "vec1", "vec2", "oh", "ol", "skip", "rh", "rl",
-                    "sh", "sl")
+def _op_call(args, fields, fn, what):
+    """Sets the keyword fields of a ctypes args struct (tensors by device pointer, a view's offset included; nothing is
+    copied) and calls fn on it on the current stream of the tensors' device."""
+    dev = None
+    for name, v in fields.items():
+        if isinstance(v, torch.Tensor):
+            dev = v.device
+            v = _ptr(v).value
+        setattr(args, name, v)
+    check(fn(C.byref(args), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), what)
 
 
 def op_gemm(path, offsets, rows, w, b=None, dilation=1, gate=False, **epi):
@@ -805,18 +830,7 @@ def op_gemm(path, offsets, rows, w, b=None, dilation=1, gate=False, **epi):
     a = _lib.OpGemmArgs(path=path, frame_offsets=off.ctypes.data, B=len(off) - 1, rows=rows, Cin=Cin, N=N, k=k,
                         dilation=dilation, gate=int(gate), w_host=wc.data_ptr(), b_host=None if bc is None else bc.data_ptr(),
                         a_slope=0.1, a_scale=1.0, alpha=1.0, act_slope=0.1, beta=1.0, gamma=1.0, plane_slope=0.1)
-    dev = None
-    for name, v in epi.items():
-        if name in _OP_GEMM_BUFFERS:
-            if v is not None:
-                dev = v.device
-                v = _ptr(v).value
-        setattr(a, name, v)
-    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    check(lib.ssb_op_gemm(C.byref(a), stream), "ssb_op_gemm")
-
-
-_OP_ATTN_BUFFERS = ("keymask", "q", "k", "v", "q_hi", "q_lo", "k_hi", "k_lo", "v_hi", "v_lo", "out", "oh", "ol")
+    _op_call(a, epi, lib.ssb_op_gemm, "ssb_op_gemm")
 
 
 def op_attention_ex(path, q_offsets, k_offsets, rows_q, rows_k, scale, heads=2, **bufs):
@@ -830,34 +844,28 @@ def op_attention_ex(path, q_offsets, k_offsets, rows_q, rows_k, scale, heads=2, 
     ko = np.ascontiguousarray(k_offsets, np.int32)
     a = _lib.OpAttentionArgs(path=path, q_offsets=qo.ctypes.data, k_offsets=ko.ctypes.data, B=len(qo) - 1, rows_q=rows_q,
                              rows_k=rows_k, heads=heads, scale=float(scale))
-    dev = None
-    for name, v in bufs.items():
-        if name in _OP_ATTN_BUFFERS:
-            if v is not None:
-                dev = v.device
-                v = _ptr(v).value
-        setattr(a, name, v)
-    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    check(lib.ssb_op_attention_ex(C.byref(a), stream), "ssb_op_attention_ex")
+    _op_call(a, bufs, lib.ssb_op_attention_ex, "ssb_op_attention_ex")
 
 
 def op_attention(q, k, v, q_offsets, k_offsets, scale, tc=False, keymask=None):
-    """tc=True: the wgmma / TMA kernel (ssb_op_attention_tc) instead of the fp32 one.  keymask: optional [sumS] tensor on
-    q's device, 0 = masked key (ssb_op_attention_masked); an utterance whose keys are all masked gets NaN rows."""
-    _require_cuda()
-    qo = np.ascontiguousarray(q_offsets, np.int32)
-    ko = np.ascontiguousarray(k_offsets, np.int32)
-    out = torch.empty_like(q)
-    stream = C.c_void_p(torch.cuda.current_stream(q.device).cuda_stream)
+    """Multi-head attention, 2 heads x 128, over tight rows: q [sum L, 256] of the query utterances at host q_offsets
+    [B + 1], k / v [sum S, 256] of the key utterances at k_offsets; query utterance b attends to key utterance b.  On the
+    fp32 kernel (op_attention_ex path 0), or with tc=True on the wgmma / TMA kernel (path 1, on fp16 hi / lo planes of q,
+    k and v).  keymask: optional [sum S] tensor, 0 = masked key; an utterance whose keys are all masked (or that has no
+    keys) gets NaN rows, as torch's softmax over all -inf does.  Returns the tight rows [sum L, 256]."""
+    iq, rows_q = _guarded(q_offsets, q.device)
+    ik, rows_k = _guarded(k_offsets, q.device)
+    bufs = {}
     if keymask is not None:
-        km = keymask.to(device=q.device, dtype=torch.float32).contiguous()
-        if km.shape != (k.shape[0],):
-            raise ValueError(f"keymask must have shape ({k.shape[0]},), got {tuple(km.shape)}")
-        check(lib.ssb_op_attention_masked(_ptr(q), _ptr(k), _ptr(v), qo.ctypes.data, ko.ctypes.data, len(qo) - 1,
-                                          float(scale), _ptr(km), 1 if tc else 0, _ptr(out), stream),
-              "ssb_op_attention_masked")
-        return out
-    fn = lib.ssb_op_attention_tc if tc else lib.ssb_op_attention
-    check(fn(_ptr(q), _ptr(k), _ptr(v), qo.ctypes.data, ko.ctypes.data, len(qo) - 1, float(scale),
-             _ptr(out), stream), "ssb_op_attention_tc" if tc else "ssb_op_attention")
-    return out
+        if keymask.shape != (k.shape[0],):
+            raise ValueError(f"keymask must have shape ({k.shape[0]},), got {tuple(keymask.shape)}")
+        bufs["keymask"] = _scatter(keymask, ik, rows_k)
+    for name, t, idx, rows in (("q", q, iq, rows_q), ("k", k, ik, rows_k), ("v", v, ik, rows_k)):
+        if tc:
+            bufs[name + "_hi"], bufs[name + "_lo"] = _planes(_scatter(t, idx, rows))
+        else:
+            bufs[name] = _scatter(t, idx, rows)
+    out = torch.empty(rows_q, 256, device=q.device)
+    op_attention_ex(int(tc), q_offsets, k_offsets, rows_q, rows_k, scale, ldq=256, ldk=256, ldv=256, out=out, ldo=256,
+                    **bufs)
+    return out[iq]

@@ -561,7 +561,7 @@ def test_refused_before_any_launch(case):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the tight-row entries (ssb_op_attention / _tc) at the shapes the op-level tests have always covered
+# the tight-row wrapper engine.op_attention (both kernels) at the shapes the op-level tests have always covered
 def wrapper_case(tc, ql, kl):
     from stylesinger_b200.engine import op_attention
     g = torch.Generator().manual_seed(3 + len(ql) + ql[0])
@@ -576,11 +576,11 @@ def wrapper_case(tc, ql, kl):
     err = Err()
     for i in range(len(ql)):
         err.add(i, out[qo[i]:qo[i + 1]], A.attention(q[qo[i]:qo[i + 1]], k[ko[i]:ko[i + 1]], v[ko[i]:ko[i + 1]], SCALE))
-    err.report(f"ssb_op_attention{'_tc' if tc else ''} {ql} x {kl}", BAR[(KERNEL[int(tc)], "typical")])
+    err.report(f"op_attention{' tc' if tc else ''} {ql} x {kl}", BAR[(KERNEL[int(tc)], "typical")])
 
 
 def test_op_attention_matches_float64():
-    """ssb_op_attention (the fp32 kernel) on ragged utterances with single-tile keys and a 1-row query."""
+    """op_attention (the fp32 kernel) on ragged utterances with single-tile keys and a 1-row query."""
     wrapper_case(False, [70, 1, 200], [33, 150, 64])
 
 

@@ -637,7 +637,7 @@ def test_refused_before_any_launch(case):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the tight-row op entries (ssb_op_conv1d / ssb_op_conv1d_tc) at the shapes the op-level tests have always covered
+# the tight-row wrappers engine.op_conv1d / op_conv1d_tc at the shapes the op-level tests have always covered
 def _tight_ref(x, offs, w, b, dil, act, idx):
     out = {}
     for i in idx:
@@ -663,7 +663,7 @@ def test_op_conv1d_shapes(cin, n, k, dil, act):
     err = Err()
     for i in ref:
         err.add(i, y[offs[i]:offs[i + 1]], ref[i])
-    err.report(f"ssb_op_conv1d {cin}->{n} k{k} d{dil} act {act}", BAR["op_conv1d"])
+    err.report(f"op_conv1d {cin}->{n} k{k} d{dil} act {act}", BAR["op_conv1d"])
 
 
 _TC_SHAPES = (  # (cin, n, k, dil, lens)
@@ -698,4 +698,4 @@ def test_op_conv1d_tc_shapes(cin, n, k, dil, lens_kind):
     err = Err()
     for i in idx:
         err.add(i, y[offs[i]:offs[i + 1]], ref[i])
-    err.report(f"ssb_op_conv1d_tc {cin}->{n} k{k} d{dil} on {int(offs[-1])} rows [{want}]", BAR["op_conv1d_tc"])
+    err.report(f"op_conv1d_tc {cin}->{n} k{k} d{dil} on {int(offs[-1])} rows [{want}]", BAR["op_conv1d_tc"])

@@ -28,7 +28,7 @@ def _rel(a, b):
 
 
 # ---------------------------------------------------------------------------------------------------
-# masked attention (ssb_op_attention_masked) against float64
+# masked attention (engine.op_attention with a keymask) against float64
 def _offsets(lens):
     return np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
 

@@ -136,6 +136,32 @@ int ssb_model_create_ex(ssb_model_t** out, const ssb_tensor_desc* tensors, int32
 int ssb_model_create_ex2(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
                          int32_t mel_decoder, int32_t f0_gen);
 
+/* The boolean model switches of egs/stylesinger.yaml's "choices of models" block and hparams['use_txt_cond'], each 0 or 1
+ * (modules/StyleSinger/stylesinger.py:53-64,92-110,119-187,313-331):
+ *   emo          emo_embed_proj (:53-54); emo is added to dur_inp (:136-137), pitch_inp_domain_specific (:159-160),
+ *                decoder_inp (:168-169) and concatenated into the ln_proj input (:321-323).
+ *   style        style_extractor / l1 / align (:61-64); get_style runs (:149-151) and style is added to
+ *                pitch_inp_domain_specific (:161-162), decoder_inp (:170-171) and concatenated into ln_proj's input (:324-326).
+ *   umln         norm (DistributionUncertainty, :57-58): the identity at inference (umln.py:49-50), so the switch only
+ *                decides whether "norm.affine_layer.*" belongs to the checkpoint.  It is never packed.
+ *   use_txt_cond decoder_inp concatenated into ln_proj's input (:94-95,317-318).
+ * ln_proj's input (DiffSinger models) is cat[coarse_mel, decoder_inp if use_txt_cond, spk, emo if emo, style if style],
+ * 80 + 256 (1 + use_txt_cond + emo + style) columns. */
+typedef struct {
+  int32_t emo, style, umln, use_txt_cond;
+} ssb_model_switches;
+
+/* ssb_model_create_ex2 with the model switches chosen: ssb_model_create_ex2(..., d, f) == ssb_model_create_ex3(..., d, f,
+ * {1, 1, 1, 1}).  Only the modules the switches build are read and packed; keys of switched-off modules are ignored, as
+ * the reference's load_ckpt(..., strict=False) ignores them (inference/StyleSinger.py:38).  On a model without emo,
+ * in->emo_embed may be NULL and is never read; without style, in->ref_offsets / ref_mels / ref_f0 may be NULL and are never
+ * read, no style adaptor, RVQ or aligner runs and its buffers are not taken from the workspace.  Asking such a model for
+ * out->emo_proj (no emo), out->style or out->rq_codes (no style) is an error, and so are ssb_get_style and ssb_rvq_lookup
+ * (no style).  Fails, naming the cause and leaving *out NULL, before anything is allocated when a switch is not 0 / 1, or
+ * (DiffSinger models) when "ln_proj.weight" is not [256, 80 + 256 (1 + use_txt_cond + emo + style)]. */
+int ssb_model_create_ex3(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
+                         int32_t mel_decoder, int32_t f0_gen, const ssb_model_switches* switches);
+
 /* Diffusion schedules (GaussianDiffusion.__init__ modules/diff/shallow_diffusion_tts.py:68-122;
  * GaussianMultinomialDiffusion.__init__ modules/diff/gaussian_multinomial_diffusion.py:208-284).
  * which: 0 = mel denoiser, 1 = both F0 denoisers.  Host arrays:
@@ -160,15 +186,15 @@ typedef struct {
   int32_t B;
   const int32_t* ph_offsets;    /* host [B+1] */
   const int32_t* frame_offsets; /* host [B+1]; required by ssb_acoustic_forward */
-  const int32_t* ref_offsets;   /* host [B+1] */
+  const int32_t* ref_offsets;   /* host [B+1]; NULL allowed on a model without style (ssb_model_create_ex3) */
   const int32_t* txt_tokens;    /* dev [sumP] */
   const int32_t* note;          /* dev [sumP] */
   const int32_t* note_type;     /* dev [sumP] */
   const float* note_dur;        /* dev [sumP] */
   const float* spk_embed;       /* dev [B,256] */
-  const float* emo_embed;       /* dev [B,256] */
-  const float* ref_mels;        /* dev [sumR,80] */
-  const float* ref_f0;          /* dev [sumR] */
+  const float* emo_embed;       /* dev [B,256]; NULL allowed on a model without emo */
+  const float* ref_mels;        /* dev [sumR,80]; NULL allowed on a model without style */
+  const float* ref_f0;          /* dev [sumR]; NULL allowed on a model without style */
   const int32_t* mel2ph;        /* dev [sumF] 1-based phone index per frame, or NULL -> use `dur` */
   const int32_t* dur;           /* dev [sumP] frames per phone (from ssb_predict_durations), or NULL */
   const float* f0;              /* dev [sumF] optional teacher-forced log2-Hz f0 (forward kwarg f0) */

@@ -26,6 +26,10 @@ class HParams(C.Structure):
         "f0_cycle", "mel_bins")]
 
 
+class ModelSwitches(C.Structure):  # ssb_model_switches: hparams emo / style / umln / use_txt_cond, each 0 or 1
+    _fields_ = [("emo", C.c_int32), ("style", C.c_int32), ("umln", C.c_int32), ("use_txt_cond", C.c_int32)]
+
+
 class VocoderConfig(C.Structure):
     _fields_ = [("n_up", C.c_int32), ("up_rates", C.c_int32 * 8), ("up_kernels", C.c_int32 * 8),
                 ("initial_channel", C.c_int32), ("n_res", C.c_int32), ("res_kernels", C.c_int32 * 4),
@@ -107,6 +111,7 @@ EXPORTS = [
     "ssb_vocoder_create_ex",
     "ssb_op_gemm",
     "ssb_op_attention_ex", "ssb_attention_launch_count",
+    "ssb_model_create_ex3",
 ]
 
 
@@ -123,6 +128,7 @@ def _load():
         "ssb_model_create": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams)]),
         "ssb_model_create_ex": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32]),
         "ssb_model_create_ex2": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32, i32]),
+        "ssb_model_create_ex3": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32, i32, P(ModelSwitches)]),
         "ssb_pitch_predictor_workspace_bytes": (sz, [vp, vp, i32]),
         "ssb_pitch_predictor": (C.c_int, [vp, i32, vp, vp, i32, vp, vp, sz, vp]),
         "ssb_model_free": (None, [vp]),

@@ -33,7 +33,12 @@ static int project_vec(Ctx& c, const Conv& w, const float* in_tight, int B, floa
 int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ssb_acoustic_outputs& out,
                  bool durations_only, int32_t* dur_out, float* logdur_out, const uint64_t* utt_seeds) {
   const int H = 256, B = in.B;
-  SSB_CHECK(B >= 1 && in.ph_offsets && in.ref_offsets, "acoustic: bad batch description");
+  const bool emo_on = m.sw.emo != 0, style_on = m.sw.style != 0;
+  SSB_CHECK(B >= 1 && in.ph_offsets && (in.ref_offsets || !style_on), "acoustic: bad batch description");
+  // switched-off modules (ssb_model_create_ex3): their outputs do not exist
+  SSB_CHECK(emo_on || !out.emo_proj, "acoustic: a model without emo (switch emo = 0) has no emo_proj");
+  SSB_CHECK(style_on || (!out.style && !out.rq_codes),
+            "acoustic: a model without style (switch style = 0) has no style / rq_codes");
   SSB_CHECK(durations_only || in.frame_offsets, "acoustic: frame_offsets required");
   SSB_CHECK(durations_only || in.mel2ph || in.dur, "acoustic: need mel2ph or dur");
   SSB_CHECK(m.mel_decoder != SSB_MEL_DECODER_PRODIFF || (!out.coarse_mel && !out.diff_cond),
@@ -43,11 +48,11 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
             "acoustic: a model with the conv F0 generator draws no F0 noise (f0_gauss_noise / f0_unif_noise must be NULL)");
   Seq qp, qr, qf;
   qp.build(in.ph_offsets, B);
-  qr.build(in.ref_offsets, B);
-  SSB_CHECK(qp.maxlen + 2 <= m.pos_rows && qr.maxlen + 2 <= m.pos_rows, "sequence longer than __pos_table");
+  if (style_on) qr.build(in.ref_offsets, B);
+  SSB_CHECK(qp.maxlen + 2 <= m.pos_rows && (!style_on || qr.maxlen + 2 <= m.pos_rows), "sequence longer than __pos_table");
   SeqDev sp, sr, sf;
   RUN(upload_layout(c, qp, 1, &sp));
-  RUN(upload_layout(c, qr, 1, &sr));
+  if (style_on) RUN(upload_layout(c, qr, 1, &sr));
   int32_t* tok = alloc_rows_i32(c, sp);
   int32_t* note = alloc_rows_i32(c, sp);
   int32_t* ntype = alloc_rows_i32(c, sp);
@@ -55,14 +60,14 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   float* srcmask = alloc_rows(c, sp, 1);
   float* enc = alloc_rows(c, sp, H);
   float* spk = c.alloc<float>((size_t)B * H);
-  float* emo = c.alloc<float>((size_t)B * H);
+  float* emo = emo_on ? c.alloc<float>((size_t)B * H) : nullptr;  // null: combine_rows / concat_cond skip it
   WS_OK(c);
   RUN(pack_rows_i32(c, sp, in.txt_tokens, tok));
   RUN(pack_rows_i32(c, sp, in.note, note));
   RUN(pack_rows_i32(c, sp, in.note_type, ntype));
   RUN(pack_rows(c, sp, in.note_dur, 1, ndur, 1, 1));
   RUN(project_vec(c, m.spk_proj, in.spk_embed, B, spk));
-  RUN(project_vec(c, m.emo_proj, in.emo_embed, B, emo));
+  if (emo_on) RUN(project_vec(c, m.emo_proj, in.emo_embed, B, emo));
   if (out.spk_proj && !c.dry) SSB_CUDA(cudaMemcpyAsync(out.spk_proj, spk, sizeof(float) * B * H, cudaMemcpyDeviceToDevice, c.stream));
   if (out.emo_proj && !c.dry) SSB_CUDA(cudaMemcpyAsync(out.emo_proj, emo, sizeof(float) * B * H, cudaMemcpyDeviceToDevice, c.stream));
   RUN(run_encoder(c, m, sp, tok, note, ntype, ndur, srcmask, enc));
@@ -73,7 +78,7 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
     float* logdur = alloc_rows(c, sp, 1);
     int32_t* dur = alloc_rows_i32(c, sp);
     WS_OK(c);
-    CombineArgs a;  // dur_inp = (encoder_out + spk + emo) * src_nonpadding (stylesinger.py:134-138)
+    CombineArgs a;  // dur_inp = (encoder_out + spk [+ emo]) * src_nonpadding (stylesinger.py:134-138)
     a.m[0] = enc; a.ldm[0] = H; a.v[0] = spk; a.v[1] = emo; a.rowmask = srcmask; a.out = dinp; a.ldo = H; a.C = H;
     RUN(combine_rows(c, sp, a));
     RUN(run_duration_predictor(c, m, sp, dinp, srcmask, logdur, dur));
@@ -91,10 +96,10 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   int32_t* midi = alloc_rows_i32(c, sf);
   float* tgt = alloc_rows(c, sf, 1);
   float* dec0 = alloc_rows(c, sf, H);
-  float* ref = alloc_rows(c, sr, 80);
-  float* reff0 = alloc_rows(c, sr, 1);
-  float* style = alloc_rows(c, sf, H);
-  int32_t* codes = alloc_rows_i32(c, sr, m.hp.rq_depth);
+  float* ref = style_on ? alloc_rows(c, sr, 80) : nullptr;
+  float* reff0 = style_on ? alloc_rows(c, sr, 1) : nullptr;
+  float* style = style_on ? alloc_rows(c, sf, H) : nullptr;  // null: combine_rows / concat_cond skip it
+  int32_t* codes = style_on ? alloc_rows_i32(c, sr, m.hp.rq_depth) : nullptr;
   WS_OK(c);
   if (in.mel2ph) {
     RUN(pack_rows_i32(c, sf, in.mel2ph, mel2ph));
@@ -106,13 +111,15 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   }
   if (out.mel2ph) RUN(unpack_rows_i32(c, sf, mel2ph, out.mel2ph));
   RUN(expand_states(c, sf, sp, mel2ph, enc, H, dec0, H, H, note, midi, tgt));
-  RUN(pack_rows(c, sr, in.ref_mels, 80, ref, 80, 80));
-  RUN(pack_rows(c, sr, in.ref_f0, 1, reff0, 1, 1));
-  RUN(run_style(c, m, sf, sr, dec0, ref, reff0, style, codes, nullptr));
-  if (out.style) RUN(unpack_rows(c, sf, style, H, out.style, H, H));
-  if (out.rq_codes) {
-    // codes are [rows, depth] int32: unpack column by column through the i32 row copier
-    for (int d = 0; d < m.hp.rq_depth; ++d) RUN(unpack_cols_i32(c, sr, codes, m.hp.rq_depth, d, out.rq_codes));
+  if (style_on) {  // get_style (stylesinger.py:149-151)
+    RUN(pack_rows(c, sr, in.ref_mels, 80, ref, 80, 80));
+    RUN(pack_rows(c, sr, in.ref_f0, 1, reff0, 1, 1));
+    RUN(run_style(c, m, sf, sr, dec0, ref, reff0, style, codes, nullptr));
+    if (out.style) RUN(unpack_rows(c, sf, style, H, out.style, H, H));
+    if (out.rq_codes) {
+      // codes are [rows, depth] int32: unpack column by column through the i32 row copier
+      for (int d = 0; d < m.hp.rq_depth; ++d) RUN(unpack_cols_i32(c, sr, codes, m.hp.rq_depth, d, out.rq_codes));
+    }
   }
 
   // ---- pitch (inpaint_pitch, stylesinger.py:216-247)
@@ -144,7 +151,7 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
       RUN(combine_rows(c, sf, a));
     }
     {
-      CombineArgs a;  // (decoder_inp + spk + emo + style) * tgt_nonpadding (:157-162)
+      CombineArgs a;  // (decoder_inp + spk [+ emo] [+ style]) * tgt_nonpadding (:157-163)
       a.m[0] = dec0; a.ldm[0] = H; a.m[1] = style; a.ldm[1] = H; a.v[0] = spk; a.v[1] = emo;
       a.rowmask = tgt; a.out = cond2; a.ldo = H; a.C = H;
       RUN(combine_rows(c, sf, a));
@@ -186,7 +193,7 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
         RUN(combine_rows(c, sf, a));
       }
       {
-        CombineArgs a;  // (decoder_inp + spk + emo + style) * tgt_nonpadding (:157-162)
+        CombineArgs a;  // (decoder_inp + spk [+ emo] [+ style]) * tgt_nonpadding (:157-163)
         a.m[0] = dec0; a.ldm[0] = H; a.m[1] = style; a.ldm[1] = H; a.v[0] = spk; a.v[1] = emo;
         a.rowmask = tgt; a.out = cond2; a.ldo = H; a.C = H;
         RUN(combine_rows(c, sf, a));
@@ -211,7 +218,7 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   WS_OK(c);
   RUN(embed_rows(c, sf, pitch, m.pitch_emb, 300, 1.0f, pemb, H, H, 0));
   {
-    CombineArgs a;
+    CombineArgs a;  // (decoder_inp + spk + pitch_embed [+ emo] [+ style]) * tgt_nonpadding (:167-172)
     a.m[0] = dec0; a.ldm[0] = H; a.m[1] = pemb; a.ldm[1] = H; a.m[2] = style; a.ldm[2] = H;
     a.v[0] = spk; a.v[1] = emo; a.rowmask = tgt; a.out = dec; a.ldo = H; a.C = H;
     RUN(combine_rows(c, sf, a));
@@ -244,12 +251,12 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
       g.e.rowmask = tgt; g.e.out = coarse; g.e.ldo = 80;
       RUN(conv_gemm(c, g));
     }
-    // run_diffsinger: g = ln_proj(cat[coarse, decoder_inp, spk, emo, style]) (stylesinger.py:313-327)
-    float* cat = alloc_rows(c, sf, 1104);
+    // run_diffsinger: g = ln_proj(cat[coarse, [decoder_inp], spk, [emo], [style]]) (stylesinger.py:313-327)
+    float* cat = alloc_rows(c, sf, m.cond_width);
     WS_OK(c);
-    RUN(concat_cond(c, sf, coarse, dec, spk, emo, style, cat));
+    RUN(concat_cond(c, sf, coarse, m.sw.use_txt_cond ? dec : nullptr, spk, emo, style, cat, m.cond_width));
     {
-      ConvGemm g = make_gemm(m.ln_proj, sf, cat, 1104);
+      ConvGemm g = make_gemm(m.ln_proj, sf, cat, m.cond_width);
       g.e.out = cond; g.e.ldo = H;
       RUN(conv_gemm(c, g));
     }
@@ -416,7 +423,7 @@ static int op_attn_launch(Ctx& c, const SeqDev& dq, const SeqDev& dk, const ssb_
 
 extern "C" {
 
-int ssb_version(void) { return 102; }
+int ssb_version(void) { return 103; }
 const char* ssb_last_error(void) { return ssb::last_error(); }
 
 int ssb_model_create(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp) {
@@ -428,17 +435,44 @@ int ssb_model_create_ex(ssb_model_t** out, const ssb_tensor_desc* tensors, int32
 }
 int ssb_model_create_ex2(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
                          int32_t mel_decoder, int32_t f0_gen) {
+  const ssb_model_switches all_on = {1, 1, 1, 1};
+  return ssb_model_create_ex3(out, tensors, n, hp, mel_decoder, f0_gen, &all_on);
+}
+int ssb_model_create_ex3(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
+                         int32_t mel_decoder, int32_t f0_gen, const ssb_model_switches* sw) {
+  if (out) *out = nullptr;
   SSB_CHECK(mel_decoder == SSB_MEL_DECODER_DIFFSINGER || mel_decoder == SSB_MEL_DECODER_PRODIFF,
             "ssb_model_create_ex: unknown mel_decoder " + std::to_string(mel_decoder) +
                 " (SSB_MEL_DECODER_DIFFSINGER = 0, SSB_MEL_DECODER_PRODIFF = 1)");
   SSB_CHECK(f0_gen == SSB_F0_GEN_GMDIFF || f0_gen == SSB_F0_GEN_CONV,
             "ssb_model_create_ex2: unknown f0_gen " + std::to_string(f0_gen) +
                 " (SSB_F0_GEN_GMDIFF = 0, SSB_F0_GEN_CONV = 1)");
+  SSB_CHECK(sw, "ssb_model_create_ex3: null switches");
+  {
+    const char* names[4] = {"emo", "style", "umln", "use_txt_cond"};
+    const int32_t vals[4] = {sw->emo, sw->style, sw->umln, sw->use_txt_cond};
+    for (int i = 0; i < 4; ++i)
+      SSB_CHECK(vals[i] == 0 || vals[i] == 1, std::string("ssb_model_create_ex3: switch ") + names[i] + " must be 0 or 1, got " +
+                                                  std::to_string(vals[i]));
+  }
   SSB_CHECK(out && tensors && hp, "ssb_model_create: null argument");
   TensorMap tm;
   if (to_map(tensors, n, &tm)) return -1;
+  if (mel_decoder == SSB_MEL_DECODER_DIFFSINGER) {  // ln_proj = Linear(cond_hs, H), cond_hs of stylesinger.py:92-100
+    const auto it = tm.t.find("ln_proj.weight");
+    if (it != tm.t.end()) {
+      const std::vector<int64_t>& sh = it->second.shape;
+      const int w = cond_width(*sw);
+      SSB_CHECK(sh.size() == 2 && sh[0] == hp->hidden_size && sh[1] == w,
+                "ssb_model_create_ex3: ln_proj.weight must be [" + std::to_string(hp->hidden_size) + ", " + std::to_string(w) +
+                    "] = 80 + 256 x (1 + use_txt_cond " + std::to_string(sw->use_txt_cond) + " + emo " +
+                    std::to_string(sw->emo) + " + style " + std::to_string(sw->style) + "), got [" +
+                    (sh.empty() ? std::string() : std::to_string(sh[0])) + (sh.size() > 1 ? ", " + std::to_string(sh[1]) : "") +
+                    (sh.size() > 2 ? ", ..." : "") + "]");
+    }
+  }
   ssb_model* m = new ssb_model();
-  if (build_model(tm, *hp, &m->m, mel_decoder, f0_gen) != 0) {
+  if (build_model(tm, *hp, &m->m, mel_decoder, f0_gen, *sw) != 0) {
     delete m;
     return -1;
   }
@@ -693,6 +727,7 @@ static int fft_decoder_impl(Ctx& c, const Model& m, const float* x, const int32_
 }
 static int get_style_impl(Ctx& c, const Model& m, const float* dec_inp, const int32_t* foffs, const float* ref_mels,
                           const float* ref_f0, const int32_t* roffs, int B, float* style_out, int32_t* codes_out) {
+  SSB_CHECK(m.sw.style, "ssb_get_style: a model without style (switch style = 0) has no style adaptor");
   Seq qf, qr;
   qf.build(foffs, B);
   qr.build(roffs, B);
@@ -749,6 +784,7 @@ int ssb_get_style(const ssb_model_t* m, const float* decoder_inp, const int32_t*
 int ssb_rvq_lookup(const ssb_model_t* m, const float* x, const int32_t* ref_offsets, int32_t B, float* quant_out,
                    int32_t* codes_out, void* workspace, size_t workspace_bytes, void* stream) {
   SSB_CHECK(m && x && ref_offsets && quant_out && codes_out && workspace, "null argument");
+  SSB_CHECK(m->m.sw.style, "ssb_rvq_lookup: a model without style (switch style = 0) has no RVQ codebooks");
   Ctx c = make_ctx(workspace, workspace_bytes, stream);
   Seq q;
   q.build(ref_offsets, B);

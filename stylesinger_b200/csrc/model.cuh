@@ -146,6 +146,10 @@ struct Model {
   // SSB_MEL_DECODER_DIFFSINGER: hparams['decoder'] == 'diffsinger' (FFT decoder + mel_out + ln_proj + DDPM over postdiff.*);
   // SSB_MEL_DECODER_PRODIFF: 'prodiff' (decoder_inp straight into the x0-predicting sampler over diff_decoder.*)
   int mel_decoder = SSB_MEL_DECODER_DIFFSINGER;
+  // model switches (ssb_model_create_ex3): emo_proj is packed only with emo; the style adaptor, codebooks, l1 and align only
+  // with style; umln builds nothing (identity at inference); use_txt_cond adds decoder_inp to ln_proj's input
+  ssb_model_switches sw = {1, 1, 1, 1};
+  int cond_width = 1104;  // ln_proj's input width: 80 + 256 (1 + use_txt_cond + emo + style)
   // hparams['K_step'] of the DiffSinger mel sampler (ssb_model_set_mel_k_step): q_sample at K-1, then K reverse steps on the
   // T-step schedule.  0 follows the schedule's T.
   int mel_k_step = 0;
@@ -194,8 +198,9 @@ int pack_linear(DevicePool& pool, const HostTensor* w, const HostTensor* b, Conv
 int pack_dense(DevicePool& pool, const HostTensor* w, const HostTensor* b, int dil, PackMode mode, Dense* out,
                const HostTensor* g = nullptr /* weight-norm g: w is v */, int row0 = 0, int nrows = -1);
 int pack_conv_transpose(DevicePool& pool, const HostTensor* v, const HostTensor* g, const HostTensor* b, int u, Conv* out);
-int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder = SSB_MEL_DECODER_DIFFSINGER,
-                int f0_gen = SSB_F0_GEN_GMDIFF);
+int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder, int f0_gen, const ssb_model_switches& sw);
+// ln_proj's input width under the switches sw (stylesinger.py:92-100)
+inline int cond_width(const ssb_model_switches& sw) { return 80 + 256 * (1 + sw.use_txt_cond + sw.emo + sw.style); }
 int build_vocoder(TensorMap& tm, const ssb_vocoder_config_ex& cfg, Vocoder* v);
 int set_schedule(Model* m, int which, int T, const float* step_emb, const float* gtab, const float* mtab,
                  cudaStream_t stream);

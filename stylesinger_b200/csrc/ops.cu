@@ -172,15 +172,17 @@ __global__ void k_concat2_pos(const int4* utt, const float* z, int C, const int3
   }
 }
 __global__ void k_concat_cond(const int4* utt, const float* coarse, const float* dec, const float* spk, const float* emo,
-                              const float* style, float* out) {
+                              const float* style, float* out, int ldo) {
   ROW_SETUP();
-  float* o = out + r * 1104;
+  float* o = out + r * ldo;
   for (int c = threadIdx.x; c < 80; c += 32) o[c] = coarse[r * 80 + c];
+  // the 256-column segments that are present, in the reference's order; dec / emo / style may be null
+  const int o_dec = 80, o_spk = o_dec + (dec ? 256 : 0), o_emo = o_spk + 256, o_sty = o_emo + (emo ? 256 : 0);
   for (int c = threadIdx.x; c < 256; c += 32) {
-    o[80 + c] = dec[r * 256 + c];
-    o[336 + c] = spk[(int64_t)b * 256 + c];
-    o[592 + c] = emo[(int64_t)b * 256 + c];
-    o[848 + c] = style[r * 256 + c];
+    if (dec) o[o_dec + c] = dec[r * 256 + c];
+    o[o_spk + c] = spk[(int64_t)b * 256 + c];
+    if (emo) o[o_emo + c] = emo[(int64_t)b * 256 + c];
+    if (style) o[o_sty + c] = style[r * 256 + c];
   }
 }
 __global__ void k_clip(const int4* utt, float* x, int ld, int C, float lo, float hi) {
@@ -806,8 +808,10 @@ int concat2_pos(Ctx& ctx, const SeqDev& s, const float* z, int C, const int32_t*
   return 0;
 }
 int concat_cond(Ctx& ctx, const SeqDev& s, const float* coarse, const float* dec, const float* spk, const float* emo,
-                const float* style, float* out) {
-  LAUNCH_ROWS(k_concat_cond, s, coarse, dec, spk, emo, style, out);
+                const float* style, float* out, int ldo) {
+  SSB_CHECK(ldo == 80 + 256 * (1 + (dec != nullptr) + (emo != nullptr) + (style != nullptr)),
+            "concat_cond: ldo does not match the segments present");
+  LAUNCH_ROWS(k_concat_cond, s, coarse, dec, spk, emo, style, out, ldo);
   return 0;
 }
 int clip_rows(Ctx& ctx, const SeqDev& s, float* x, int ld, int C, float lo, float hi) {

@@ -59,9 +59,10 @@ int scale_mask_add_rowscalar(Ctx&, const SeqDev&, const float* x, int ldx, int C
 // out[r, 0:C] = z[r, :], out[r, C:2C] = table[pos[r], :]   (cat[style, positions], stylesinger.py:199-200)
 int concat2_pos(Ctx&, const SeqDev&, const float* z, int C, const int32_t* pos, const float* table, int table_rows,
                 float* out, int ldo);
-// g[r, :] = cat[coarse(80) | dec(256) | spk[b](256) | emo[b](256) | style(256)]   (stylesinger.py:314-326)
+// g[r, :] = cat[coarse(80) | dec(256) | spk[b](256) | emo[b](256) | style(256)]   (stylesinger.py:314-326), leaving out
+// the segments whose pointer is null (dec, emo, style) and packing the rest in that order; ldo = the width that leaves
 int concat_cond(Ctx&, const SeqDev&, const float* coarse, const float* dec, const float* spk, const float* emo,
-                const float* style, float* out);
+                const float* style, float* out, int ldo);
 // x[r, c] = min(max(x, lo), hi) on valid rows
 int clip_rows(Ctx&, const SeqDev&, float* x, int ld, int C, float lo, float hi);
 

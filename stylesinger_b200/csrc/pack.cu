@@ -431,11 +431,13 @@ static int build_pitch_predictor(TensorMap& tm, DevicePool& pool, const std::str
   return 0;
 }
 
-int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder, int f0_gen) {
+int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder, int f0_gen, const ssb_model_switches& sw) {
   DevicePool& pool = m->pool;
   m->hp = hp;
   m->mel_decoder = mel_decoder;
   m->f0_gen = f0_gen;
+  m->sw = sw;
+  m->cond_width = cond_width(sw);
   const bool prodiff = mel_decoder == SSB_MEL_DECODER_PRODIFF;
   const int H = hp.hidden_size;
   SSB_CHECK(H == 256, "hidden_size must be 256");
@@ -462,7 +464,7 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder,
     m->spec_max = upload_tensor(pool, tm.get("postdiff.spec_max"));
   }
   PK(pack_linear(pool, tm.get("spk_embed_proj.weight"), tm.get("spk_embed_proj.bias"), &m->spk_proj));
-  PK(pack_linear(pool, tm.get("emo_embed_proj.weight"), tm.get("emo_embed_proj.bias"), &m->emo_proj));
+  if (sw.emo) PK(pack_linear(pool, tm.get("emo_embed_proj.weight"), tm.get("emo_embed_proj.bias"), &m->emo_proj));
   PK(build_fft(tm, pool, "encoder.", hp.enc_layers, hp.enc_ffn_kernel, false, &m->enc));
   PK(build_fft(tm, pool, "decoder.", hp.dec_layers, hp.dec_ffn_kernel, true, &m->dec));
   m->dp_layers = hp.dur_layers;
@@ -473,53 +475,55 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder,
     m->dp_ln_b[i] = upload_tensor(pool, tm.get(q + "3.bias"));
   }
   PK(pack_linear(pool, tm.get("dur_predictor.linear.weight"), tm.get("dur_predictor.linear.bias"), &m->dp_lin));
-  // style adaptor
-  for (int i = 0; i < 4; ++i) {
-    const std::string a = "style_extractor.wavenet.in_layers." + std::to_string(i) + ".";
-    const std::string r = "style_extractor.wavenet.res_skip_layers." + std::to_string(i) + ".";
-    PK(pack_conv(pool, tm.get(a + "weight_v"), tm.get(a + "bias"), 1, PACK_GATE_TANH_SIG, &m->wn_in[i], tm.get(a + "weight_g")));
-    PK(pack_conv(pool, tm.get(r + "weight_v"), tm.get(r + "bias"), 1, PACK_PLAIN, &m->wn_rs[i], tm.get(r + "weight_g")));
-  }
-  for (int i = 0; i < 5; ++i)
-    for (int j = 0; j < 2; ++j) {
-      const std::string q = "style_extractor.encoder.res_blocks." + std::to_string(i) + ".blocks." + std::to_string(j) + ".";
-      Model::CB& c = m->cb[i * 2 + j];
-      c.ln_g = upload_tensor(pool, tm.get(q + "0.weight"));
-      c.ln_b = upload_tensor(pool, tm.get(q + "0.bias"));
-      PK(pack_conv(pool, tm.get(q + "1.weight"), tm.get(q + "1.bias"), 1, PACK_PLAIN, &c.c1));
-      PK(pack_conv(pool, tm.get(q + "4.weight"), tm.get(q + "4.bias"), 1, PACK_PLAIN, &c.c2));
+  // style adaptor, RVQ, l1 and aligner (stylesinger.py:61-64): built only with style
+  if (sw.style) {
+    for (int i = 0; i < 4; ++i) {
+      const std::string a = "style_extractor.wavenet.in_layers." + std::to_string(i) + ".";
+      const std::string r = "style_extractor.wavenet.res_skip_layers." + std::to_string(i) + ".";
+      PK(pack_conv(pool, tm.get(a + "weight_v"), tm.get(a + "bias"), 1, PACK_GATE_TANH_SIG, &m->wn_in[i], tm.get(a + "weight_g")));
+      PK(pack_conv(pool, tm.get(r + "weight_v"), tm.get(r + "bias"), 1, PACK_PLAIN, &m->wn_rs[i], tm.get(r + "weight_g")));
     }
-  m->cb_last_g = upload_tensor(pool, tm.get("style_extractor.encoder.last_norm.weight"));
-  m->cb_last_b = upload_tensor(pool, tm.get("style_extractor.encoder.last_norm.bias"));
-  PK(pack_conv(pool, tm.get("style_extractor.encoder.post_net1.weight"), tm.get("style_extractor.encoder.post_net1.bias"), 1, PACK_PLAIN, &m->cb_post));
-  {
-    std::vector<float> cbs((size_t)hp.rq_depth * hp.n_rq * H);
-    for (int d = 0; d < hp.rq_depth; ++d) {
-      const HostTensor* c = tm.get("style_extractor.rqvae.codebooks." + std::to_string(d) + ".weight", {hp.n_rq + 1, H});
-      if (!c) goto fail;
-      memcpy(&cbs[(size_t)d * hp.n_rq * H], c->data, sizeof(float) * hp.n_rq * H);  // row n_rq = padding, unused (RQ.py:31)
+    for (int i = 0; i < 5; ++i)
+      for (int j = 0; j < 2; ++j) {
+        const std::string q = "style_extractor.encoder.res_blocks." + std::to_string(i) + ".blocks." + std::to_string(j) + ".";
+        Model::CB& c = m->cb[i * 2 + j];
+        c.ln_g = upload_tensor(pool, tm.get(q + "0.weight"));
+        c.ln_b = upload_tensor(pool, tm.get(q + "0.bias"));
+        PK(pack_conv(pool, tm.get(q + "1.weight"), tm.get(q + "1.bias"), 1, PACK_PLAIN, &c.c1));
+        PK(pack_conv(pool, tm.get(q + "4.weight"), tm.get(q + "4.bias"), 1, PACK_PLAIN, &c.c2));
+      }
+    m->cb_last_g = upload_tensor(pool, tm.get("style_extractor.encoder.last_norm.weight"));
+    m->cb_last_b = upload_tensor(pool, tm.get("style_extractor.encoder.last_norm.bias"));
+    PK(pack_conv(pool, tm.get("style_extractor.encoder.post_net1.weight"), tm.get("style_extractor.encoder.post_net1.bias"), 1, PACK_PLAIN, &m->cb_post));
+    {
+      std::vector<float> cbs((size_t)hp.rq_depth * hp.n_rq * H);
+      for (int d = 0; d < hp.rq_depth; ++d) {
+        const HostTensor* c = tm.get("style_extractor.rqvae.codebooks." + std::to_string(d) + ".weight", {hp.n_rq + 1, H});
+        if (!c) goto fail;
+        memcpy(&cbs[(size_t)d * hp.n_rq * H], c->data, sizeof(float) * hp.n_rq * H);  // row n_rq = padding, unused (RQ.py:31)
+      }
+      m->codebooks = pool.upload(cbs);
+      m->cb_norm2 = pool.alloc((size_t)hp.rq_depth * hp.n_rq);
+      Ctx c;
+      PK(codebook_norms(c, m->codebooks, hp.rq_depth * hp.n_rq, m->cb_norm2));
     }
-    m->codebooks = pool.upload(cbs);
-    m->cb_norm2 = pool.alloc((size_t)hp.rq_depth * hp.n_rq);
-    Ctx c;
-    PK(codebook_norms(c, m->codebooks, hp.rq_depth * hp.n_rq, m->cb_norm2));
-  }
-  PK(pack_linear(pool, tm.get("l1.weight"), tm.get("l1.bias"), &m->l1));
-  for (int i = 0; i < 2; ++i) {
-    const std::string q = "align.layers." + std::to_string(i) + ".";
-    AlignLayer& a = m->align[i];
-    const HostTensor* iw = tm.get(q + "multihead_attn.in_proj_weight", {3 * H, H});
-    const HostTensor* ib = tm.get(q + "multihead_attn.in_proj_bias", {3 * H});
-    PK(pack_dense(pool, iw, ib, 1, PACK_PLAIN, &a.q, nullptr, 0, H));
-    PK(pack_dense(pool, iw, ib, 1, PACK_PLAIN, &a.kv, nullptr, H, 2 * H));
-    PK(pack_dense(pool, tm.get(q + "multihead_attn.out_proj.weight"), tm.get(q + "multihead_attn.out_proj.bias"), 1, PACK_PLAIN, &a.out));
-    PK(pack_dense(pool, tm.get(q + "linear1.weight"), tm.get(q + "linear1.bias"), 1, PACK_PLAIN, &a.lin1));
-    PK(pack_dense(pool, tm.get(q + "linear2.weight"), tm.get(q + "linear2.bias"), 1, PACK_PLAIN, &a.lin2));
-    m->align_tc_ok = m->align_tc_ok && a.q.t.ok && a.kv.t.ok && a.out.t.ok && a.lin1.t.ok && a.lin2.t.ok;
-    a.n1_g = upload_tensor(pool, tm.get(q + "norm1.weight"));
-    a.n1_b = upload_tensor(pool, tm.get(q + "norm1.bias"));
-    a.n2_g = upload_tensor(pool, tm.get(q + "norm2.weight"));
-    a.n2_b = upload_tensor(pool, tm.get(q + "norm2.bias"));
+    PK(pack_linear(pool, tm.get("l1.weight"), tm.get("l1.bias"), &m->l1));
+    for (int i = 0; i < 2; ++i) {
+      const std::string q = "align.layers." + std::to_string(i) + ".";
+      AlignLayer& a = m->align[i];
+      const HostTensor* iw = tm.get(q + "multihead_attn.in_proj_weight", {3 * H, H});
+      const HostTensor* ib = tm.get(q + "multihead_attn.in_proj_bias", {3 * H});
+      PK(pack_dense(pool, iw, ib, 1, PACK_PLAIN, &a.q, nullptr, 0, H));
+      PK(pack_dense(pool, iw, ib, 1, PACK_PLAIN, &a.kv, nullptr, H, 2 * H));
+      PK(pack_dense(pool, tm.get(q + "multihead_attn.out_proj.weight"), tm.get(q + "multihead_attn.out_proj.bias"), 1, PACK_PLAIN, &a.out));
+      PK(pack_dense(pool, tm.get(q + "linear1.weight"), tm.get(q + "linear1.bias"), 1, PACK_PLAIN, &a.lin1));
+      PK(pack_dense(pool, tm.get(q + "linear2.weight"), tm.get(q + "linear2.bias"), 1, PACK_PLAIN, &a.lin2));
+      m->align_tc_ok = m->align_tc_ok && a.q.t.ok && a.kv.t.ok && a.out.t.ok && a.lin1.t.ok && a.lin2.t.ok;
+      a.n1_g = upload_tensor(pool, tm.get(q + "norm1.weight"));
+      a.n1_b = upload_tensor(pool, tm.get(q + "norm1.bias"));
+      a.n2_g = upload_tensor(pool, tm.get(q + "norm2.weight"));
+      a.n2_b = upload_tensor(pool, tm.get(q + "norm2.bias"));
+    }
   }
   if (f0_gen == SSB_F0_GEN_CONV) {
     // f0_gen 'conv' (stylesinger.py:73-82): FastSpeech2 built pitch_predictor (unused with gmdiff, not packed then) and
@@ -537,7 +541,7 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder,
   } else {
     PK(build_denoiser(tm, pool, "postdiff.denoise_fn.", hp.mel_channels, hp.mel_layers, hp.mel_cycle, hp.mel_bins, hp.mel_bins, false, &m->melnet));
     PK(pack_linear(pool, tm.get("mel_out.weight"), tm.get("mel_out.bias"), &m->mel_out));
-    PK(pack_linear(pool, tm.get("ln_proj.weight"), tm.get("ln_proj.bias"), &m->ln_proj));
+    PK(pack_linear(pool, tm.get("ln_proj.weight", {H, m->cond_width}), tm.get("ln_proj.bias"), &m->ln_proj));
   }
   m->log_eps = logf(1e-30f);
   if (cudaStreamCreateWithFlags(&m->aux_stream, cudaStreamNonBlocking) != cudaSuccess) m->aux_stream = nullptr;

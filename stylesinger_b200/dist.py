@@ -25,18 +25,21 @@ def _p2p_device(device):
 
 
 def scatter_utterances(utts: Optional[List[dict]], src: int = 0, device=None, pin: bool = False,
-                       keep_on_device: bool = False):
+                       keep_on_device: bool = False, emo: bool = True, style: bool = True):
     """Rank `src` owns `utts` (list of per-utterance CPU tensors, see synth.make_utterance); every rank returns
     (its PackedBatch, the global indices of its utterances).  Metadata goes through scatter_object_list, tensors
     through point-to-point send/recv (NCCL over NVLink when `device` is a CUDA device, gloo on CPU).
-    `keep_on_device`: with a CUDA `device` the received shard stays in HBM (no host bounce before the engine call)."""
+    `keep_on_device`: with a CUDA `device` the received shard stays in HBM (no host bounce before the engine call).
+    `emo` / `style`: the model switches of the receiving model (pack_batch): without them no emo_embed / reference mels
+    are packed or sent."""
     rank, world = dist.get_rank(), dist.get_world_size()
     dev = _p2p_device(device)
     if rank == src:
         lens = [int(u["mel2ph"].shape[0]) if "mel2ph" in u else int(len(u["txt_tokens"])) for u in utts]
         bins = lpt_assign(lens, world)
         # fewer utterances than ranks leaves some bins empty: those ranks get an empty batch (B = 0) and skip the compute
-        packed = [pack_batch([utts[i] for i in b], use_mel2ph=all("mel2ph" in utts[i] for i in b)) if b else empty_batch()
+        packed = [pack_batch([utts[i] for i in b], use_mel2ph=all("mel2ph" in utts[i] for i in b), emo=emo, style=style)
+                  if b else empty_batch()
                   for b in bins]
         meta = [{"B": p.B, "ph": p.ph_offsets, "ref": p.ref_offsets, "fr": p.frame_offsets, "idx": b, "pad": p.may_have_pad_frames,
                  "shapes": {k: (tuple(v.shape), str(v.dtype)) for k, v in p.t.items()}} for p, b in zip(packed, bins)]

@@ -13,8 +13,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import AcousticInputs, AcousticOutputs, HParams, TensorDesc, VocoderConfigEx, check, lib
-from .hparams import DEFAULT_VOCODER_CONFIG, resolve
+from ._lib import AcousticInputs, AcousticOutputs, HParams, ModelSwitches, TensorDesc, VocoderConfigEx, check, lib
+from .hparams import DEFAULT_VOCODER_CONFIG, resolve, switches
 from .schedules import multinomial_table, prodiff_table, sampler_table
 
 MEL_DECODERS = {"diffsinger": 0, "prodiff": 1}  # SSB_MEL_DECODER_* of include/stylesinger_b200.h
@@ -95,10 +95,10 @@ class PackedBatch:
     """A ragged batch in the library's tight layout. Offsets are host int32 arrays [B+1]."""
     B: int
     ph_offsets: np.ndarray
-    ref_offsets: np.ndarray
+    ref_offsets: Optional[np.ndarray]  # None for a model without style (no reference mels)
     frame_offsets: Optional[np.ndarray]
     t: Dict[str, torch.Tensor] = field(default_factory=dict)  # txt_tokens, note, note_type (int32), note_dur,
-    # spk_embed, emo_embed, ref_mels, ref_f0, [mel2ph int32], [f0], [uv]
+    # spk_embed, [emo_embed], [ref_mels, ref_f0], [mel2ph int32], [f0], [uv]
     may_have_pad_frames: bool = True  # False when the host knows every frame maps to a phone (mel2ph > 0 everywhere)
 
     def to(self, device, non_blocking=True):
@@ -114,21 +114,26 @@ class PackedBatch:
         return int(self.frame_offsets[-1]) if self.frame_offsets is not None else 0
 
 
-def pack_batch(utts: List[dict], use_mel2ph=True, pin=False) -> PackedBatch:
-    """Concatenate per-utterance CPU tensors (as produced by synth.make_utterance) into one PackedBatch."""
+def pack_batch(utts: List[dict], use_mel2ph=True, pin=False, emo=True, style=True) -> PackedBatch:
+    """Concatenate per-utterance CPU tensors (as produced by synth.make_utterance) into one PackedBatch.
+    emo / style: the model switches of the model the batch is for.  Without emo, no emo_embed is packed (utterances need
+    none); without style, no ref_mels / ref_f0 are packed and ref_offsets is None."""
     def offs(lens):
         return np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
 
     B = len(utts)
     po = offs([len(u["txt_tokens"]) for u in utts])
-    ro = offs([u["ref_mels"].shape[0] for u in utts])
+    ro = offs([u["ref_mels"].shape[0] for u in utts]) if style else None
     fo = offs([len(u["mel2ph"]) for u in utts]) if use_mel2ph else None
     cat = lambda k, dt: torch.cat([u[k].reshape(-1) if u[k].dim() == 1 else u[k] for u in utts]).to(dt).contiguous()
     t = {"txt_tokens": cat("txt_tokens", torch.int32), "note": cat("note", torch.int32),
          "note_type": cat("note_type", torch.int32), "note_dur": cat("note_dur", torch.float32),
-         "spk_embed": torch.stack([u["spk_embed"] for u in utts]).float().contiguous(),
-         "emo_embed": torch.stack([u["emo_embed"] for u in utts]).float().contiguous(),
-         "ref_mels": cat("ref_mels", torch.float32), "ref_f0": cat("ref_f0", torch.float32)}
+         "spk_embed": torch.stack([u["spk_embed"] for u in utts]).float().contiguous()}
+    if emo:
+        t["emo_embed"] = torch.stack([u["emo_embed"] for u in utts]).float().contiguous()
+    if style:
+        t["ref_mels"] = cat("ref_mels", torch.float32)
+        t["ref_f0"] = cat("ref_f0", torch.float32)
     pad = False  # predicted durations: the length regulator never emits a zero entry inside an utterance
     if use_mel2ph:
         t["mel2ph"] = cat("mel2ph", torch.int32)
@@ -154,7 +159,10 @@ class AcousticModel:
     """Packed StyleSinger acoustic model on one GPU (ssb_model_t).  hparams['decoder'] selects the mel decoder:
     'diffsinger' (FFT decoder + DDPM refinement, the default) or 'prodiff' (the ProDiff teacher, decoder_inp -> mel).
     hparams['f0_gen'] selects the F0 generator: 'gmdiff' (two F0 diffusion samplers, the default) or 'conv' (two
-    deterministic FastSpeech-2 PitchPredictors; no F0 schedule, no F0 noise)."""
+    deterministic FastSpeech-2 PitchPredictors; no F0 schedule, no F0 noise).  The model switches hparams['emo'],
+    ['style'], ['umln'] and ['use_txt_cond'] (all True by default) select the modules the checkpoint has
+    (ssb_model_create_ex3); batches for a model without emo / style need no emo_embed / reference mels
+    (pack_batch(..., emo=, style=), or ``self.pack_batch``)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], hparams=None, device=None, max_positions=4096):
         _require_cuda()
@@ -175,10 +183,12 @@ class AcousticModel:
                     hp["audio_num_mel_bins"])
         self.mel_decoder = hp["decoder"]
         self.f0_gen = hp["f0_gen"]
+        self.switches = switches(hp)
+        sw = ModelSwitches(**{k: int(v) for k, v in self.switches.items()})
         arr, keep = _descs(sd)
         handle = C.c_void_p()
-        check(lib.ssb_model_create_ex2(C.byref(handle), arr, len(sd), C.byref(h), MEL_DECODERS[self.mel_decoder],
-                                       F0_GENS[self.f0_gen]), "ssb_model_create_ex2")
+        check(lib.ssb_model_create_ex3(C.byref(handle), arr, len(sd), C.byref(h), MEL_DECODERS[self.mel_decoder],
+                                       F0_GENS[self.f0_gen], C.byref(sw)), "ssb_model_create_ex3")
         self._h = handle
         self._ws = _Workspace(self.device)
         self.T = self.f0_T = None
@@ -192,6 +202,10 @@ class AcousticModel:
         if h:
             lib.ssb_model_free(h)
             self._h = None
+
+    def pack_batch(self, utts: List[dict], use_mel2ph=True, pin=False) -> PackedBatch:
+        """pack_batch with the fields this model reads (no emo_embed without emo, no reference mels without style)."""
+        return pack_batch(utts, use_mel2ph, pin, emo=self.switches["emo"], style=self.switches["style"])
 
     def set_tensor_cores(self, enable=True):
         """wgmma (fp16 hi/lo split, 3 MMAs) vs fp32 FFMA for the denoiser layer GEMMs. Returns the mode in effect."""
@@ -245,15 +259,20 @@ class AcousticModel:
     def _inputs(self, pb: PackedBatch, noise=None, seed=0, skip_mel=False, dur=None, f0=None, uv=None):
         a = AcousticInputs()
         a.B = pb.B
-        self._keep = [np.ascontiguousarray(pb.ph_offsets, np.int32), np.ascontiguousarray(pb.ref_offsets, np.int32)]
+        self._keep = [np.ascontiguousarray(pb.ph_offsets, np.int32)]
         a.ph_offsets = self._keep[0].ctypes.data
-        a.ref_offsets = self._keep[1].ctypes.data
+        if self.switches["style"]:  # a model without style reads no reference offsets, mels or f0
+            self._keep.append(np.ascontiguousarray(pb.ref_offsets, np.int32))
+            a.ref_offsets = self._keep[-1].ctypes.data
         if pb.frame_offsets is not None:
             fo = np.ascontiguousarray(pb.frame_offsets, np.int32)
             self._keep.append(fo)
             a.frame_offsets = fo.ctypes.data
         t = pb.t
-        for k in ("txt_tokens", "note", "note_type", "note_dur", "spk_embed", "emo_embed", "ref_mels", "ref_f0"):
+        keys = ["txt_tokens", "note", "note_type", "note_dur", "spk_embed"]
+        keys += ["emo_embed"] if self.switches["emo"] else []  # forward_model passes none then (inference/StyleSinger.py:44-47)
+        keys += ["ref_mels", "ref_f0"] if self.switches["style"] else []
+        for k in keys:
             assert t[k].is_cuda and t[k].is_contiguous(), k
             setattr(a, k, t[k].data_ptr())
         if "mel2ph" in t and dur is None:
@@ -307,7 +326,8 @@ class AcousticModel:
             if noise and any(v is not None for v in noise.values()):
                 raise ValueError("seeds: per-utterance seeds key the in-kernel noise; injected noise must be None")
         a = self._inputs(pb, noise, seed, skip_mel_diffusion, dur)
-        Fs, Ps, Rs = int(pb.frame_offsets[-1]), int(pb.ph_offsets[-1]), int(pb.ref_offsets[-1])
+        Fs, Ps = int(pb.frame_offsets[-1]), int(pb.ph_offsets[-1])
+        Rs = int(pb.ref_offsets[-1]) if pb.ref_offsets is not None else 0
         shapes = {"mel_out": (Fs, 80), "f0_denorm": (Fs,), "encoder_out": (Ps, 256), "style": (Fs, 256),
                   "rq_codes": (Rs, self.hp["rq_depth"]), "pitch_pred": (Fs, 2), "decoder_inp": (Fs, 256),
                   "coarse_mel": (Fs, 80), "diff_cond": (Fs, 256), "mel2ph": (Fs,), "spk_proj": (pb.B, 256),
@@ -315,6 +335,11 @@ class AcousticModel:
         o = AcousticOutputs()
         out = {}
         want = set(want)
+        # outputs of switched-off modules do not exist (the library refuses them too; a style-off batch has no reference
+        # rows, so an empty rq_codes buffer would otherwise reach it as NULL)
+        for k, sw in (("emo_proj", "emo"), ("style", "style"), ("rq_codes", "style")):
+            if k in want and not self.switches[sw]:
+                raise _lib.SsbError(f"AcousticModel.forward: a model without {sw} (hparams {sw}=False) has no {k}")
         if skip_mel_diffusion:
             want.discard("mel_out")  # never written in that mode: do not hand back an uninitialised buffer
         else:

@@ -74,6 +74,16 @@ HIFIGAN_V3 = dict(DEFAULT_VOCODER_CONFIG, upsample_rates=[8, 8, 4], upsample_ker
                   upsample_initial_channel=256, resblock="2", resblock_kernel_sizes=[3, 5, 7],
                   resblock_dilation_sizes=[[1, 2], [2, 6], [3, 12]])
 
+# Boolean model switches (egs/stylesinger.yaml "choices of models", plus use_txt_cond, stylesinger.py:94,317): which
+# modules StyleSinger.__init__ builds and which terms its forward adds.  Order = the ssb_model_switches fields.
+SWITCHES = ("emo", "style", "umln", "use_txt_cond")
+
+
+def switches(hp):
+    """The model switches of a resolved hparams dict, as {name: bool}."""
+    return {k: bool(hp[k]) for k in SWITCHES}
+
+
 # Mutable module-level dict with the same role as the reference's global `hparams`
 # (reference utils/hparams.py:8).
 hparams = copy.deepcopy(DEFAULT_HPARAMS)
@@ -107,14 +117,18 @@ def _check_supported(hp):
            "dur_loss": "mse", "pitch_type": "frame", "f0_gen": "conv" if conv_f0 else "gmdiff",
            "decoder": "prodiff" if prodiff else "diffsinger",
            "diff_decoder_type": "wavenet", "schedule_type": "vpsde" if prodiff else "linear", "pitch_norm": "log",
-           "use_uv": True, "emo": True, "style": True, "umln": True, "use_spk_embed": True,
+           "use_uv": True, "use_spk_embed": True,
            "use_spk_id": False, "use_pitch_embed": True, "use_energy_embed": False,
-           "use_pos_embed": True, "use_txt_cond": True, "num_heads": 2, "hidden_size": 256}
+           "use_pos_embed": True, "num_heads": 2, "hidden_size": 256}
     for k, v in req.items():
         if hp.get(k) != v:
             raise NotImplementedError(
                 f"stylesinger_b200 implements the egs/stylesinger.yaml configuration only: "
                 f"hparams[{k!r}]={hp.get(k)!r}, required {v!r}")
+    # the model switches of egs/stylesinger.yaml's "choices of models" block (stylesinger.py:53-64,92-110,131-172,317-326)
+    for k in SWITCHES:
+        if not isinstance(hp.get(k), bool):
+            raise NotImplementedError(f"stylesinger_b200: hparams[{k!r}] must be True or False, got {hp.get(k)!r}")
     if hp.get("rel_pos"):
         raise NotImplementedError("rel_pos is not selected by egs/stylesinger.yaml")
     if prodiff:  # ProDiffusion.forward(infer=True) never reads K_step or pndm_speedup (prodiff.py:204-222)

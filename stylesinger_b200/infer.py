@@ -111,7 +111,7 @@ class StyleSingerInfer:
             raise ValueError("spk_embed_fn or inp['spk_embed'] required (resemblyzer VoiceEncoder is third-party)")
         if preprocess_wav_fn is not None:
             inp["emo_embed"] = self.emotion_embed(preprocess_wav_fn(ref_audio))
-        elif "emo_embed" not in inp:
+        elif "emo_embed" not in inp and self.hparams["emo"]:  # a model without emo reads none (StyleSinger.py:44-47)
             raise ValueError("preprocess_wav_fn or inp['emo_embed'] required")
         inp.update({"item_name": inp["name"], "ph_token": ph_token, "wav_fn": ref_audio})
         if pitch_fn is not None:
@@ -126,17 +126,23 @@ class StyleSingerInfer:
     def input_to_batch(self, item) -> PackedBatch:
         """reference inference/StyleSinger.py:139-170 (B=1 assembly).  ``item['f0']`` is the raw extractor output in Hz
         (0 = unvoiced), exactly what ``preprocess_input`` produces: like the reference (:152) it goes through
-        ``norm_interp_f0`` (log2 Hz, unvoiced frames interpolated) before it becomes the style extractor's ``ref_f0``."""
+        ``norm_interp_f0`` (log2 Hz, unvoiced frames interpolated) before it becomes the style extractor's ``ref_f0``.
+        A model without emo reads no ``emo_embed`` (forward_model passes None, :44-47), one without style no ``mel`` /
+        ``f0`` (get_style is skipped, stylesinger.py:149-151): the item may then leave them out."""
         hp = self.hparams
-        f0, _ = norm_interp_f0(np.asarray(item["f0"]), hp.get("pitch_norm", "log"), hp.get("use_uv", True),
-                               hp.get("f0_mean", 400.0), hp.get("f0_std", 100.0))
         u = {"txt_tokens": torch.as_tensor(item["ph_token"]).long(), "note": torch.as_tensor(item["note"]).long(),
              "note_dur": torch.as_tensor(item["note_dur"]).float(), "note_type": torch.as_tensor(item["note_type"]).long(),
-             "spk_embed": torch.as_tensor(item["spk_embed"]).float(), "emo_embed": torch.as_tensor(item["emo_embed"]).float(),
-             "ref_mels": torch.as_tensor(item["mel"]).float(), "ref_f0": torch.from_numpy(f0)}
+             "spk_embed": torch.as_tensor(item["spk_embed"]).float()}
+        if hp["emo"]:
+            u["emo_embed"] = torch.as_tensor(item["emo_embed"]).float()
+        if hp["style"]:
+            f0, _ = norm_interp_f0(np.asarray(item["f0"]), hp.get("pitch_norm", "log"), hp.get("use_uv", True),
+                                   hp.get("f0_mean", 400.0), hp.get("f0_std", 100.0))
+            u["ref_mels"] = torch.as_tensor(item["mel"]).float()
+            u["ref_f0"] = torch.from_numpy(f0)
         if item.get("mel2ph") is not None:
             u["mel2ph"] = torch.as_tensor(item["mel2ph"]).long()
-        return pack_batch([u], use_mel2ph="mel2ph" in u)
+        return pack_batch([u], use_mel2ph="mel2ph" in u, emo=hp["emo"], style=hp["style"])
 
     def forward_model(self, inp, seed=0, noise=None, voc_noise=None, return_mel=False):
         """reference inference/StyleSinger.py:41-64: returns the waveform (np.float32 [T*hop]).
@@ -150,7 +156,7 @@ class StyleSingerInfer:
         seed=seeds[b]) gives, whatever else the batch holds (see run_device)."""
         if seeds is not None:  # validated before anything reaches the device
             seeds = utt_seeds(seeds, len(utts))
-        return self.infer_packed(pack_batch(utts, use_mel2ph=use_mel2ph, pin=True), seed=seed, return_mel=return_mel,
+        return self.infer_packed(self.model.pack_batch(utts, use_mel2ph=use_mel2ph, pin=True), seed=seed, return_mel=return_mel,
                                  seeds=seeds)
 
     def run_device(self, pb_dev: PackedBatch, seed=0, noise=None, voc_noise=None, seeds=None):

@@ -28,29 +28,33 @@ def padded_to_utterances(txt_tokens, note, note_dur, note_type, spk_embed, emo_e
     Padding conventions of the reference collater (tasks/StyleSinger/dataset.py): token id 0 pads ``txt_tokens``
     (and the note tensors alongside), all-zero frames pad ``ref_mels`` (the reference derives its own mask from
     ``ref_mels[:, :, 0] != 0``, lse.py:104, and so does the kernel), 0 pads ``mel2ph``.
+    ``emo_embed`` None (a model without emo) or ``ref_mels`` None (without style) leaves those fields out.
     """
     txt_tokens = torch.as_tensor(txt_tokens).cpu()
     B = txt_tokens.shape[0]
-    ref_mels = torch.as_tensor(ref_mels).float().cpu()
-    ref_f0 = torch.as_tensor(ref_f0).float().cpu()
-    if ref_f0.dim() == 1:  # inference/StyleSinger.py passes [R] at B=1
-        ref_f0 = ref_f0[None]
+    if ref_mels is not None:
+        ref_mels = torch.as_tensor(ref_mels).float().cpu()
+        ref_f0 = torch.as_tensor(ref_f0).float().cpu()
+        if ref_f0.dim() == 1:  # inference/StyleSinger.py passes [R] at B=1
+            ref_f0 = ref_f0[None]
     utts = []
     for b in range(B):
         nz = (txt_tokens[b] != 0).nonzero()
         P = int(nz[-1]) + 1 if len(nz) else 0
         if P == 0:
             raise ValueError(f"utterance {b}: empty phone sequence")
-        rnz = (ref_mels[b].abs().sum(-1) > 0).nonzero()
-        R = int(rnz[-1]) + 1 if len(rnz) else 0
-        if R == 0:
-            raise ValueError(f"utterance {b}: empty reference mel")
         u = {"txt_tokens": txt_tokens[b, :P].long(), "note": torch.as_tensor(note)[b, :P].long().cpu(),
              "note_dur": torch.as_tensor(note_dur)[b, :P].float().cpu(),
              "note_type": torch.as_tensor(note_type)[b, :P].long().cpu(),
-             "spk_embed": torch.as_tensor(spk_embed)[b].float().reshape(-1).cpu(),
-             "emo_embed": torch.as_tensor(emo_embed)[b].float().reshape(-1).cpu(),
-             "ref_mels": ref_mels[b, :R], "ref_f0": ref_f0[b, :R]}
+             "spk_embed": torch.as_tensor(spk_embed)[b].float().reshape(-1).cpu()}
+        if emo_embed is not None:
+            u["emo_embed"] = torch.as_tensor(emo_embed)[b].float().reshape(-1).cpu()
+        if ref_mels is not None:
+            rnz = (ref_mels[b].abs().sum(-1) > 0).nonzero()
+            R = int(rnz[-1]) + 1 if len(rnz) else 0
+            if R == 0:
+                raise ValueError(f"utterance {b}: empty reference mel")
+            u["ref_mels"], u["ref_f0"] = ref_mels[b, :R], ref_f0[b, :R]
         if mel2ph is not None:
             m2p = torch.as_tensor(mel2ph)[b].long().cpu()
             fnz = (m2p != 0).nonzero()
@@ -128,10 +132,24 @@ class StyleSinger:
         if global_steps < hp.get("forcing", 0):
             raise NotImplementedError("global_steps < hparams['forcing'] selects the forced-alignment branch of "
                                       "ProsodyAligner (training warm-up); pass the checkpoint's step count")
-        if spk_embed is None or emo_embed is None or ref_mels is None or ref_f0 is None or note is None:
-            raise ValueError("spk_embed, emo_embed, ref_mels, ref_f0 and note/note_dur/note_type are required")
-        utts = padded_to_utterances(txt_tokens, note, note_dur, note_type, spk_embed, emo_embed, ref_mels, ref_f0, mel2ph)
-        pb: PackedBatch = pack_batch(utts, use_mel2ph=mel2ph is not None).to(self.engine.device)
+        if hp["emo"] and hp["style"]:
+            if spk_embed is None or emo_embed is None or ref_mels is None or ref_f0 is None or note is None:
+                raise ValueError("spk_embed, emo_embed, ref_mels, ref_f0 and note/note_dur/note_type are required")
+        else:  # the model switches decide what the model reads (stylesinger.py:131-137,149-151)
+            need = {"spk_embed": spk_embed, "note": note}
+            if hp["emo"]:
+                need["emo_embed"] = emo_embed
+            if hp["style"]:
+                need.update(ref_mels=ref_mels, ref_f0=ref_f0)
+            missing = [k for k, v in need.items() if v is None]
+            if missing:
+                raise ValueError(f"{', '.join(missing)} required by this model (hparams emo={hp['emo']}, "
+                                 f"style={hp['style']})")
+        # a switched-off module's input is not read, whatever the caller passes (the reference ignores it too)
+        utts = padded_to_utterances(txt_tokens, note, note_dur, note_type, spk_embed, emo_embed if hp["emo"] else None,
+                                    ref_mels if hp["style"] else None, ref_f0 if hp["style"] else None, mel2ph)
+        pb: PackedBatch = pack_batch(utts, use_mel2ph=mel2ph is not None, emo=hp["emo"],
+                                     style=hp["style"]).to(self.engine.device)
         ret = {}
         dur = None
         if pb.frame_offsets is None:  # FastSpeech2.add_dur at inference (fs2.py:151-174): predicted durations
@@ -145,7 +163,9 @@ class StyleSinger:
         # the ProDiff branch has no such gate and no coarse mel (:176-177)
         prodiff = hp["decoder"] == "prodiff"
         run_diff = (not skip_decoder) and (prodiff or global_steps > hp.get("diff_start", 0))
-        want = ["f0_denorm", "mel2ph", "decoder_inp", "style", "pitch_pred", "spk_proj", "emo_proj"]
+        want = ["f0_denorm", "mel2ph", "decoder_inp", "pitch_pred", "spk_proj"]
+        want += ["emo_proj"] if hp["emo"] else []
+        want += ["style"] if hp["style"] else []
         if not skip_decoder:
             want.append("mel_out" if run_diff else "coarse_mel")
         if callable(noise):  # parity hooks: the injected draws depend on the (possibly predicted) frame count
@@ -159,10 +179,12 @@ class StyleSinger:
         ret["x_mask"] = (m2p > 0).float()[:, :, None]
         ret["f0_denorm"] = packed_to_padded(out["f0_denorm"], fo)
         ret["decoder_inp"] = packed_to_padded(out["decoder_inp"], fo)
-        ret["style"] = packed_to_padded(out["style"], fo)
+        if hp["style"]:  # the reference sets ret['style'] only then (stylesinger.py:149-151)
+            ret["style"] = packed_to_padded(out["style"], fo)
         ret["pitch_pred"] = packed_to_padded(out["pitch_pred"], fo)
         ret["spk_embed"] = out["spk_proj"][:, None, :]
-        ret["emo_embed"] = out["emo_proj"][:, None, :]
+        if hp["emo"]:  # the reference sets ret['emo_embed'] only then (stylesinger.py:131-132)
+            ret["emo_embed"] = out["emo_proj"][:, None, :]
         if not skip_decoder:
             ret["mel_out"] = packed_to_padded(out["mel_out" if run_diff else "coarse_mel"], fo)
         # training-only entries the callers index unconditionally

@@ -92,9 +92,43 @@ def acoustic_param_shapes(hp):
     out += _predictor("pitch_predictor.", H, 5, hp["predictor_kernel"], 2)
     out += [("pitch_predictor.embed_positions._float_tensor", (1,)),
             ("note_encoder.emb.weight", (100, H)), ("note_encoder.type_emb.weight", (5, H)),
-            ("note_encoder.dur_ln.weight", (H, 1)), ("note_encoder.dur_ln.bias", (H,)),
-            ("emo_embed_proj.weight", (H, hp["emo_size"])), ("emo_embed_proj.bias", (H,)),
-            ("norm.affine_layer.linear_layer.weight", (2 * H, H)), ("norm.affine_layer.linear_layer.bias", (2 * H,))]
+            ("note_encoder.dur_ln.weight", (H, 1)), ("note_encoder.dur_ln.bias", (H,))]
+    if hp["emo"]:
+        out += [("emo_embed_proj.weight", (H, hp["emo_size"])), ("emo_embed_proj.bias", (H,))]
+    if hp["umln"]:
+        out += [("norm.affine_layer.linear_layer.weight", (2 * H, H)), ("norm.affine_layer.linear_layer.bias", (2 * H,))]
+    if hp["style"]:
+        out += _style_modules(hp, H)
+    Cf, Lf, Tf = hp["f0_residual_channels"], hp["f0_residual_layers"], hp["f0_timesteps"]
+    if hp["f0_gen"] == "conv":  # StyleSinger.__init__ (stylesinger.py:73-82): a second PitchPredictor, no F0 diffusion
+        out += [("pitch_inpainter_predictor.pos_embed_alpha", (1,))]
+        out += _predictor("pitch_inpainter_predictor.", H, 5, hp["predictor_kernel"], 2)
+        out += [("pitch_inpainter_predictor.embed_positions._float_tensor", (1,))]
+    f0_nets = () if hp["f0_gen"] == "conv" else (("gm_diffnet", "f0_gen"), ("gm_diffnet_inpainte", "f0_gen_inpainte"))
+    for net, gen in f0_nets:
+        out += _diffnet(net + ".", Cf, Lf, 1, 3, H, True)
+        out += [(f"{gen}.{b}", (Tf,)) for b in _MULTI_BUFS]
+        out += [(f"{gen}.Lt_history", (Tf,)), (f"{gen}.Lt_count", (Tf,))]
+        out += [(f"{gen}.{b}", (Tf,)) for b in _GAUSS_BUFS]
+        out += _diffnet(gen + "._denoise_fn.", Cf, Lf, 1, 3, H, True)
+    T = hp["timesteps"]
+    if hp["decoder"] == "prodiff":  # ProDiffusion (stylesinger.py:111-117, prodiff.py:59-117): buffers of length T+1
+        out += [("embed_positions._float_tensor", (1,)), ("diff_decoder.timesteps", ()), ("diff_decoder.timescale", ())]
+        out += [(f"diff_decoder.{b}", (T + 1,)) for b in _GAUSS_BUFS]
+        out += [("diff_decoder.spec_min", (1, 1, 80)), ("diff_decoder.spec_max", (1, 1, 80))]
+        out += _diffnet("diff_decoder.denoise_fn.", hp["residual_channels"], hp["residual_layers"], 80, 80, H, False)
+        return out
+    cond_hs = 80 + H * (1 + hp["use_txt_cond"] + hp["emo"] + hp["style"])  # stylesinger.py:92-100
+    out += [("embed_positions._float_tensor", (1,)), ("ln_proj.weight", (H, cond_hs)), ("ln_proj.bias", (H,))]
+    out += [(f"postdiff.{b}", (T,)) for b in _GAUSS_BUFS]
+    out += [("postdiff.spec_min", (1, 1, 80)), ("postdiff.spec_max", (1, 1, 80))]
+    out += _diffnet("postdiff.denoise_fn.", hp["residual_channels"], hp["residual_layers"], 80, 80, H, False)
+    return out
+
+
+def _style_modules(hp, H):
+    """LocalStyleAdaptor, l1 and ProsodyAligner (stylesinger.py:61-64): built only with hparams['style']."""
+    out = []
     for i in range(5):
         for j in range(2):
             q = f"style_extractor.encoder.res_blocks.{i}.blocks.{j}."
@@ -128,29 +162,6 @@ def acoustic_param_shapes(hp):
                 (q + "norm1.weight", (H,)), (q + "norm1.bias", (H,)),
                 (q + "linear2.weight", (H, 2048)), (q + "linear2.bias", (H,)),
                 (q + "norm2.weight", (H,)), (q + "norm2.bias", (H,))]
-    Cf, Lf, Tf = hp["f0_residual_channels"], hp["f0_residual_layers"], hp["f0_timesteps"]
-    if hp["f0_gen"] == "conv":  # StyleSinger.__init__ (stylesinger.py:73-82): a second PitchPredictor, no F0 diffusion
-        out += [("pitch_inpainter_predictor.pos_embed_alpha", (1,))]
-        out += _predictor("pitch_inpainter_predictor.", H, 5, hp["predictor_kernel"], 2)
-        out += [("pitch_inpainter_predictor.embed_positions._float_tensor", (1,))]
-    f0_nets = () if hp["f0_gen"] == "conv" else (("gm_diffnet", "f0_gen"), ("gm_diffnet_inpainte", "f0_gen_inpainte"))
-    for net, gen in f0_nets:
-        out += _diffnet(net + ".", Cf, Lf, 1, 3, H, True)
-        out += [(f"{gen}.{b}", (Tf,)) for b in _MULTI_BUFS]
-        out += [(f"{gen}.Lt_history", (Tf,)), (f"{gen}.Lt_count", (Tf,))]
-        out += [(f"{gen}.{b}", (Tf,)) for b in _GAUSS_BUFS]
-        out += _diffnet(gen + "._denoise_fn.", Cf, Lf, 1, 3, H, True)
-    T = hp["timesteps"]
-    if hp["decoder"] == "prodiff":  # ProDiffusion (stylesinger.py:111-117, prodiff.py:59-117): buffers of length T+1
-        out += [("embed_positions._float_tensor", (1,)), ("diff_decoder.timesteps", ()), ("diff_decoder.timescale", ())]
-        out += [(f"diff_decoder.{b}", (T + 1,)) for b in _GAUSS_BUFS]
-        out += [("diff_decoder.spec_min", (1, 1, 80)), ("diff_decoder.spec_max", (1, 1, 80))]
-        out += _diffnet("diff_decoder.denoise_fn.", hp["residual_channels"], hp["residual_layers"], 80, 80, H, False)
-        return out
-    out += [("embed_positions._float_tensor", (1,)), ("ln_proj.weight", (H, 80 + 4 * H)), ("ln_proj.bias", (H,))]
-    out += [(f"postdiff.{b}", (T,)) for b in _GAUSS_BUFS]
-    out += [("postdiff.spec_min", (1, 1, 80)), ("postdiff.spec_max", (1, 1, 80))]
-    out += _diffnet("postdiff.denoise_fn.", hp["residual_channels"], hp["residual_layers"], 80, 80, H, False)
     return out
 
 

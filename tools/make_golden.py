@@ -483,6 +483,82 @@ def case_convf0(name, T=4, frames=96, phones=12, ref_frames=64, seed=111, utt_id
     print("wrote", name, {k: (v.shape if hasattr(v, "shape") else "meta") for k, v in d.items()})
 
 
+# The model-switch configurations (egs/stylesinger.yaml "choices of models" + use_txt_cond): name -> hparams overrides
+_OFF4 = {"emo": False, "style": False, "umln": False, "use_txt_cond": False}
+SWITCH_CONFIGS = {
+    "no_emo": {"emo": False},
+    "no_style": {"style": False},
+    "no_umln": {"umln": False},
+    "no_txt_cond": {"use_txt_cond": False},
+    "all_off": _OFF4,
+    "prodiff_no_emo_style": dict(PRODIFF_OVERRIDES, emo=False, style=False),
+    "conv_no_style": dict(CONVF0_OVERRIDES, style=False),
+}
+SWITCH_DUR_CONFIG = "all_off"  # the configuration that also stores a forward with predicted durations
+
+
+def case_switches(name, T=4, frames=32, phones=4, ref_frames=32, seed=151, utt_idx=107):
+    """The reference's StyleSinger under each model-switch configuration (stylesinger.py:53-64,92-117,119-187,313-331):
+    per configuration the state dict's key list (the synthetic checkpoint loads with strict=True) and a B = 1 full forward
+    at T = f0_T = 4 with injected noise, mel2ph given.  emo_embed is passed as None without emo, as forward_model does
+    (inference/StyleSinger.py:44-47).  Stored per configuration c as c/<output>; c/coarse_mel (DiffSinger configurations)
+    comes from a second run below diff_start.  SWITCH_DUR_CONFIG also stores the forward with predicted durations
+    (c/dur_*)."""
+    import ref_import
+    u = synth.make_utterance(frames / 187.5, utt_idx=utt_idx, ref_frames=ref_frames, frames=frames, phones=phones)
+    d, cfg_meta = {}, {}
+    for c, ov in SWITCH_CONFIGS.items():
+        hp = ref_import.install(T=T, f0_T=T, overrides=ov)
+        import modules.diff.shallow_diffusion_tts as sdt
+        import modules.diff.gaussian_multinomial_diffusion as gmd
+        import modules.diff.prodiff as pdm
+        sdt.tqdm = gmd.tqdm = pdm.tqdm = lambda it, **k: it
+        from modules.StyleSinger.stylesinger import StyleSinger
+        model = StyleSinger(_Dict()).eval()
+        model.load_state_dict(synth.acoustic_state_dict(dict(hp), seed=0), strict=True)
+
+        def run(seed_, mel2ph=True, global_steps=320000):
+            ns = NoiseSource(seed_)
+            b = batchify(u)
+            cap, hooks = {}, []
+            if hp["style"]:
+                hooks.append(model.style_extractor.rqvae.register_forward_hook(
+                    lambda m, i, o: cap.__setitem__("rq_in", i[0].detach().clone())))
+            with torch.no_grad(), patched_rng(ns):
+                out = model(b["txt_tokens"], mel2ph=u["mel2ph"][None] if mel2ph else None, spk_embed=b["spk_embed"],
+                            emo_embed=b["emo_embed"] if hp["emo"] else None, ref_mels=b["ref_mels"].clone(),
+                            ref_f0=b["ref_f0"].clone(), global_steps=global_steps, infer=True, note=b["note"],
+                            note_dur=b["note_dur"], note_type=b["note_type"])
+                if hp["style"]:
+                    out["rq_codes"] = model.style_extractor.rqvae.quantize(cap["rq_in"])[1]
+            for h in hooks:
+                h.remove()
+            return out, ns.log
+
+        out, log = run(seed)
+        keys = ["mel_out", "f0_denorm", "pitch_pred", "decoder_inp", "spk_embed"]
+        keys += ["emo_embed"] if hp["emo"] else []
+        keys += ["style"] if hp["style"] else []
+        for k in keys:
+            d[f"{c}/{k}"] = np32(out[k][0])
+        if hp["style"]:
+            d[f"{c}/rq_codes"] = out["rq_codes"][0].numpy().astype(np.int64)
+        if hp["decoder"] == "diffsinger":
+            coarse, _ = run(seed, global_steps=50000)  # forcing < global_steps < diff_start: the coarse mel only
+            d[f"{c}/coarse_mel"] = np32(coarse["mel_out"][0])
+        cfg_meta[c] = {"overrides": ov, "noise_log": log,
+                       "state_dict": [[k, list(v.shape)] for k, v in model.state_dict().items()]}
+        if c == SWITCH_DUR_CONFIG:
+            o2, log2 = run(seed + 1, mel2ph=False)
+            d.update({f"{c}/dur_mel2ph": o2["mel2ph"][0].numpy().astype(np.int64), f"{c}/dur_logdur": np32(o2["dur"][0]),
+                      f"{c}/dur_mel_out": np32(o2["mel_out"][0]), f"{c}/dur_f0_denorm": np32(o2["f0_denorm"][0])})
+            cfg_meta[c]["dur_noise_log"] = log2
+    d["meta"] = json.dumps({"T": T, "frames": frames, "phones": phones, "ref_frames": ref_frames, "seed": seed,
+                            "utt_idx": utt_idx, "dur_config": SWITCH_DUR_CONFIG, "configs": cfg_meta})
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, len(d), "arrays")
+
+
 def case_registry(name, T=4, seed=131):
     """The reference's per-registry modules that the C ABI replaces one by one (FS_ENCODERS['fft'], FS_DECODERS['fft'],
     StyleSinger.get_style): FastspeechEncoder.forward and FastspeechDecoder.forward on padded B = 3 batches and on each
@@ -576,7 +652,7 @@ if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "convf0", "sched", "voc",
-                             "vocoder_edges", "emo", "registry", "kstep", "vocoder_layouts"]
+                             "vocoder_edges", "emo", "registry", "kstep", "vocoder_layouts", "switches"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
@@ -605,3 +681,5 @@ if __name__ == "__main__":
         case_registry("ref_registry")
     if "kstep" in which:
         case_kstep("ref_kstep")
+    if "switches" in which:
+        case_switches("ref_switches")

@@ -363,6 +363,23 @@ int ssb_model_set_tensor_cores(ssb_model_t* m, int32_t enable);
  * stages). */
 int ssb_vocoder_set_tensor_cores(ssb_vocoder_t* v, int32_t enable);
 
+/* Precision of the tensor-core GEMMs (ssb_model_set_mel_precision, ssb_vocoder_set_precision).  SSB_TC_SPLIT (the
+ * default): every fp32 operand is carried as fp16 hi/lo planes and each K step issues 3 MMAs (hi*hi + hi*lo + lo*hi, ~22
+ * mantissa bits).  SSB_TC_FP16: one MMA on the hi planes alone (operands rounded once to fp16, fp32 accumulation): a third
+ * of the MMAs and half the operand bytes, at a stated accuracy cost (README "Single-pass fp16 mode").  It is a choice of
+ * speed against accuracy, like K_step, not another path to the same result. */
+#define SSB_TC_SPLIT 0
+#define SSB_TC_FP16 1
+/* The mel DiffNet on every mel sampler that runs it on tensor cores: DDPM (persistent and per-launch, with the hoisted
+ * conditioner projection), K_step, PLMS, ProDiff, and ssb_denoiser_eval(which = 0).  Not the F0 samplers, attention, the
+ * FFT blocks, the style adaptor / RVQ, the pitch predictors, the front-end or the output denoiser; GEMMs that take the
+ * FFMA path (short batches, ssb_model_set_tensor_cores(0)) are unchanged.  An unknown mode fails and changes nothing.
+ * Returns 0 on success. */
+int ssb_model_set_mel_precision(ssb_model_t* m, int32_t mode);
+/* The vocoder's tensor-core GEMMs (every HiFi-GAN layout, with and without NSF): the ups convs and the ResBlock convs
+ * that run on tensor cores.  The FFMA convs (conv_pre, conv_post, narrow FFMA stages) are unchanged. */
+int ssb_vocoder_set_precision(ssb_vocoder_t* v, int32_t mode);
+
 /* 1 (default): small batches run the whole T-step mel sampler in ONE persistent cooperative kernel launch
  * (csrc/sampler_tc.cu); 0: one launch per GEMM (BASELINE.json configs[4] compares the two). */
 int ssb_model_set_persistent(ssb_model_t* m, int32_t enable);
@@ -523,6 +540,8 @@ typedef struct ssb_op_gemm_args {
   void* sh;
   void* sl;
   int32_t n_valid;
+  int32_t single_pass;          /* path 1 only: 0 = the 3-pass fp16 hi/lo split (a_lo read), 1 = one hi*hi pass (a_lo unread,
+                                   may be NULL) - the kernel of SSB_TC_FP16.  Anything else, or 1 on path 0, is refused. */
 } ssb_op_gemm_args;
 int ssb_op_gemm(const ssb_op_gemm_args* a, void* stream);
 /* Unit-test granularity: exactly ONE attention call - the fp32 kernel (path 0, csrc/attention.cu) or the wgmma kernel

@@ -72,7 +72,7 @@ class OpGemmArgs(C.Structure):
                 ("plane_slope", C.c_float), ("skip", C.c_void_p), ("ld_skip", C.c_int32), ("C", C.c_int32),
                 ("skip_init", C.c_int32), ("rh", C.c_void_p), ("rl", C.c_void_p), ("ld_rh", C.c_int32),
                 ("skip_tiled", C.c_int32), ("out_nb", C.c_int32), ("out_bs", C.c_int64), ("sh", C.c_void_p),
-                ("sl", C.c_void_p), ("n_valid", C.c_int32)]
+                ("sl", C.c_void_p), ("n_valid", C.c_int32), ("single_pass", C.c_int32)]
 
 
 class OpAttentionArgs(C.Structure):
@@ -112,6 +112,7 @@ EXPORTS = [
     "ssb_op_gemm",
     "ssb_op_attention_ex", "ssb_attention_launch_count",
     "ssb_model_create_ex3",
+    "ssb_model_set_mel_precision", "ssb_vocoder_set_precision",
 ]
 
 
@@ -161,6 +162,8 @@ def _load():
         "ssb_model_set_persistent_groups": (C.c_int, [vp, i32]),
         "ssb_model_set_fft_tensor_cores": (C.c_int, [vp, i32]),
         "ssb_vocoder_set_tensor_cores": (C.c_int, [vp, i32]),
+        "ssb_model_set_mel_precision": (C.c_int, [vp, i32]),
+        "ssb_vocoder_set_precision": (C.c_int, [vp, i32]),
         "ssb_op_gemm": (C.c_int, [P(OpGemmArgs), vp]),
         "ssb_op_attention_ex": (C.c_int, [P(OpAttentionArgs), vp]),
         "ssb_attention_launch_count": (C.c_int64, [i32]),

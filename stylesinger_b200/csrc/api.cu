@@ -281,6 +281,7 @@ int denoiser_eval_api(Ctx& c, const Model& m, int which, const SeqDev& s, const 
   float* cond = alloc_rows(c, s, 256);
   DenoiserBufs b;
   RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
+  b.single_pass = b.tc && which == 0 && m.mel_fp16;  // the mel net follows ssb_model_set_mel_precision, the F0 nets stay split
   RUN(pack_rows(c, s, cond_tight, 256, cond, 256, 256));
   RUN(prepare_cond(c, d, s, cond, b));
   if (which == 0) {
@@ -334,6 +335,8 @@ struct OpWeights {  // the call's packed weights, freed with the pool when the c
 // utterance (or, for the first one, whatever lies before the buffer), so it is refused here, before anything is launched.
 static int op_pack(const ssb_op_gemm_args& a, OpWeights* w) {
   SSB_CHECK(a.path == 0 || a.path == 1, "op_gemm: path must be 0 (fp32 FFMA) or 1 (tensor cores)");
+  SSB_CHECK(a.single_pass == 0 || (a.single_pass == 1 && a.path == 1),
+            "op_gemm: single_pass must be 0, or 1 on path 1 (the tensor-core kernel)");
   SSB_CHECK(a.w_host && a.Cin > 0 && a.N > 0 && a.k >= 1 && a.dilation >= 1, "op_gemm: bad weight shape");
   SSB_CHECK(!a.gate || a.N % 2 == 0, "op_gemm: the gate packing needs an even N");
   const int64_t reach = (int64_t)(a.k - 1) / 2 * a.dilation;
@@ -367,6 +370,7 @@ static int op_launch(Ctx& c, const SeqDev& s, const ssb_op_gemm_args& a, const O
     return conv_gemm(c, g);
   }
   GemmTC g = make_gemm_tc(w.ct, s, (const __half*)a.a_hi, (const __half*)a.a_lo);
+  g.single_pass = a.single_pass != 0;
   EpiTC& e = g.e;
   e.mode = a.mode; e.out = a.out; e.ldo = a.ldo;
   e.oh = (__half*)a.oh; e.ol = (__half*)a.ol; e.ldh = a.ldh;
@@ -907,6 +911,22 @@ int ssb_vocoder_set_tensor_cores(ssb_vocoder_t* v, int32_t enable) {
   return v->v.use_tc ? 1 : 0;
 }
 
+int ssb_model_set_mel_precision(ssb_model_t* m, int32_t mode) {
+  SSB_CHECK(m, "null model");
+  SSB_CHECK(mode == SSB_TC_SPLIT || mode == SSB_TC_FP16,
+            "ssb_model_set_mel_precision: mode must be SSB_TC_SPLIT (0) or SSB_TC_FP16 (1), got " + std::to_string(mode));
+  m->m.mel_fp16 = mode == SSB_TC_FP16;
+  return 0;
+}
+
+int ssb_vocoder_set_precision(ssb_vocoder_t* v, int32_t mode) {
+  SSB_CHECK(v, "null vocoder");
+  SSB_CHECK(mode == SSB_TC_SPLIT || mode == SSB_TC_FP16,
+            "ssb_vocoder_set_precision: mode must be SSB_TC_SPLIT (0) or SSB_TC_FP16 (1), got " + std::to_string(mode));
+  v->v.fp16 = mode == SSB_TC_FP16;
+  return 0;
+}
+
 int ssb_model_set_fft_tensor_cores(ssb_model_t* m, int32_t enable) {
   SSB_CHECK(m, "null model");
   m->m.fft_tc = enable != 0;
@@ -945,7 +965,7 @@ int ssb_op_gemm(const ssb_op_gemm_args* a, void* stream) {
   SSB_CHECK(a && a->frame_offsets && a->B >= 1, "ssb_op_gemm: null argument");
   OpWeights w;
   if (op_pack(*a, &w)) return -1;
-  SSB_CHECK(a->path == 1 ? (a->a_hi && a->a_lo) : a->a != nullptr, "ssb_op_gemm: no A operand");
+  SSB_CHECK(a->path == 1 ? (a->a_hi && (a->a_lo || a->single_pass)) : a->a != nullptr, "ssb_op_gemm: no A operand");
   Seq q;
   q.build(a->frame_offsets, a->B);
   SSB_CHECK(a->rows == q.rows(), "ssb_op_gemm: rows is " + std::to_string(a->rows) + ", the layout has " +

@@ -4,6 +4,8 @@
 //   warp 0 (1 lane)  TMA producer: per K block loads A_hi, A_lo [128x64] and W_hi, W_lo [BNx64] (128B swizzle)
 //   warps 4-11       two consumer warpgroups: each issues the 3-product wgmma chain (M64 N=BN K16, fp32 accumulators in
 //                    registers) for its 64 rows, then runs the fused epilogue through shared-memory transpose buffers
+// PASSES = 1 (single-pass fp16, GemmTC::single_pass): the producer loads only the A_hi / W_hi tiles and each K step issues
+// one wgmma (hi*hi); the stage layout and the epilogue are those of PASSES = 3, so the lo halves of each stage stay unused.
 // smem ring: BN=128: 3 stages x 64 KB, BN=64: 4 stages x 48 KB; mbarriers full/empty per stage.  The single-CTA kernel
 // (BN=64) serves problems too small to fill the GPU with pairs.  The CTA-pair variant (cluster of 2, BN = 2 hb = 64 or 128)
 // gives each CTA its own row tile and one half of a shared weight tile, which TMA multicasts into both CTAs.
@@ -312,11 +314,19 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb,
   }
 }
 
+// TMA loads of an operand's hi plane and, with NPL == 2, of its lo plane `stride` bytes further
+template <int NPL>
+__device__ __forceinline__ void tma_load_planes(uint32_t dst, uint32_t stride, const CUtensorMap* hi, const CUtensorMap* lo,
+                                                uint32_t bar, int c0, int c1) {
+  tma_load_2d(dst, hi, bar, c0, c1);
+  if constexpr (NPL == 2) tma_load_2d(dst + stride, lo, bar, c0, c1);
+}
+
 // REUSE (3-tap convs, centre tap 1, dilation <= HALO): per K block ONE halo-extended activation tile of
 // BM + 2 HALO rows is loaded into its own ring, and the three taps read it through wgmma descriptors whose start address
 // is moved by whole 128-byte rows (the 128B swizzle phase follows the shared-memory address, and the tile starts on a
 // 1024-byte boundary).  Per tap only the weight tile is loaded: a third of the activation bytes of the plain variant.
-template <int BN, int CL, int MODE, bool REUSE>
+template <int BN, int CL, int MODE, bool REUSE, int PASSES>
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
@@ -325,6 +335,8 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   constexpr int STAGES = K::STAGES;
   constexpr int HB = BN / CL;  // weight rows this CTA loads per K block (CL == 2: and multicasts to its peer)
   constexpr int NCH = BN / 32;
+  static_assert(PASSES == 3 || PASSES == 1, "3-pass hi/lo split or single-pass fp16");
+  constexpr int NPL = PASSES == 3 ? 2 : 1;  // fp16 planes loaded per operand
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // [activation ring (REUSE)][stage ring][transpose buffers][barriers]
@@ -362,15 +374,15 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       auto load_b = [&](const CUtensorMap* mb_h, const CUtensorMap* mb_l, int c0, int brow, uint32_t extra_bytes) {
         mbar_wait(empty0 + 8 * stage, phase ^ 1);
         const uint32_t fb = full0 + 8 * stage;
-        mbar_expect_tx(fb, 2 * K::B_TILE + extra_bytes);
+        mbar_expect_tx(fb, NPL * K::B_TILE + extra_bytes);
         const uint32_t sb = sbase + stage * K::STAGE + (REUSE ? 0u : (uint32_t)(2 * A_TILE));
         if (CL > 1) {
           const uint32_t boff = rank * (uint32_t)(HB * BK * 2);
           tma_load_2d_mc(sb + boff, mb_h, fb, c0, brow + (int)rank * HB, (uint16_t)3);
-          tma_load_2d_mc(sb + K::B_TILE + boff, mb_l, fb, c0, brow + (int)rank * HB, (uint16_t)3);
+          if constexpr (PASSES == 3) tma_load_2d_mc(sb + K::B_TILE + boff, mb_l, fb, c0, brow + (int)rank * HB, (uint16_t)3);
         } else {
           tma_load_2d(sb, mb_h, fb, c0, brow);
-          tma_load_2d(sb + K::B_TILE, mb_l, fb, c0, brow);
+          if constexpr (PASSES == 3) tma_load_2d(sb + K::B_TILE, mb_l, fb, c0, brow);
         }
         return fb;
       };
@@ -383,9 +395,8 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
           for (int kc = 0; kc < p.kchunks; ++kc) {
             mbar_wait(aempty0 + 8 * as, aph ^ 1);
             const uint32_t ab = afull0 + 8 * as, sa = abase + as * (2 * A3_TILE);
-            mbar_expect_tx(ab, 2 * A3_TILE);
-            tma_load_2d(sa, &tmA_hi, ab, kc * BK, row0 - HALO);
-            tma_load_2d(sa + A3_TILE, &tmA_lo, ab, kc * BK, row0 - HALO);
+            mbar_expect_tx(ab, NPL * A3_TILE);
+            tma_load_planes<NPL>(sa, A3_TILE, &tmA_hi, &tmA_lo, ab, kc * BK, row0 - HALO);
             if (++as == ASLOTS) { as = 0; aph ^= 1; }
             for (int tap = 0; tap < 3; ++tap) {
               load_b(&tmB_hi, &tmB_lo, kc * BK, tap * p.N + nt * BN, 0u);
@@ -397,11 +408,10 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
             const int tap = kb / p.kchunks;
             const int c0 = (kb - tap * p.kchunks) * BK;
             const int arow = row0 + (tap - p.center) * p.dil;
-            // the expect_tx of load_b also covers this CTA's two activation boxes of the same stage
-            const uint32_t fb = load_b(&tmB_hi, &tmB_lo, c0, tap * p.N + nt * BN, (uint32_t)(2 * A_TILE));
+            // the expect_tx of load_b also covers this CTA's activation boxes of the same stage
+            const uint32_t fb = load_b(&tmB_hi, &tmB_lo, c0, tap * p.N + nt * BN, (uint32_t)(NPL * A_TILE));
             const uint32_t sa = sbase + stage * K::STAGE;
-            tma_load_2d(sa, &tmA_hi, fb, c0, arow);
-            tma_load_2d(sa + A_TILE, &tmA_lo, fb, c0, arow);
+            tma_load_planes<NPL>(sa, A_TILE, &tmA_hi, &tmA_lo, fb, c0, arow);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
@@ -437,12 +447,16 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         const uint64_t off = (uint64_t)((ks * 32) >> 4);  // 16 fp16 = 32 bytes along K inside the swizzle atom
         if constexpr (BN == 128) {
           wgmma_n128(acc, dah + off, dbh + off, 1u);
-          wgmma_n128(acc, dah + off, dbl + off, 1u);
-          wgmma_n128(acc, dal + off, dbh + off, 1u);
+          if constexpr (PASSES == 3) {
+            wgmma_n128(acc, dah + off, dbl + off, 1u);
+            wgmma_n128(acc, dal + off, dbh + off, 1u);
+          }
         } else {
           wgmma_n64(acc, dah + off, dbh + off, 1u);
-          wgmma_n64(acc, dah + off, dbl + off, 1u);
-          wgmma_n64(acc, dal + off, dbh + off, 1u);
+          if constexpr (PASSES == 3) {
+            wgmma_n64(acc, dah + off, dbl + off, 1u);
+            wgmma_n64(acc, dal + off, dbh + off, 1u);
+          }
         }
       }
       wg_commit();
@@ -677,15 +691,16 @@ void pair_guard_end(int dev, cudaStream_t st) {  // g_pair_mu held
   g_pair_last_stream[dev] = st;
 }
 
-template <int BN, int CL, int MODE, bool REUSE>
+template <int BN, int CL, int MODE, bool REUSE, int PASSES>
 int launch_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
   using KCfg = Cfg<BN, REUSE>;
   static std::atomic<bool> configured[MAX_DEV];
-  if (configure_once(conv_gemm_wg_kernel<BN, CL, MODE, REUSE>, configured, KCfg::SMEM)) return -2;
+  if (configure_once(conv_gemm_wg_kernel<BN, CL, MODE, REUSE, PASSES>, configured, KCfg::SMEM)) return -2;
   static std::atomic<long long>* const counter = [] {
     static char name[48];
-    if (CL > 1) snprintf(name, sizeof(name), "tc2%s<%d,%s>", REUSE ? "r" : "", BN / 2, mode_name(MODE));
-    else snprintf(name, sizeof(name), "tc%s<%d,%s>", REUSE ? "r" : "", BN, mode_name(MODE));
+    const char* sp = PASSES == 1 ? ",fp16" : "";
+    if (CL > 1) snprintf(name, sizeof(name), "tc2%s<%d,%s%s>", REUSE ? "r" : "", BN / 2, mode_name(MODE), sp);
+    else snprintf(name, sizeof(name), "tc%s<%d,%s%s>", REUSE ? "r" : "", BN, mode_name(MODE), sp);
     return variant_counter(name);
   }();
   const ConvTC& w = *p.w;
@@ -693,7 +708,8 @@ int launch_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
   const uint32_t a_rows = REUSE ? A3_ROWS : BM;  // REUSE: halo-extended activation boxes
   CUtensorMap ta_hi, ta_lo;
   if (cached_act_map(&ta_hi, p.A_hi, (uint64_t)p.rows_total, (uint64_t)w.Cin, a_rows)) return -1;
-  if (cached_act_map(&ta_lo, p.A_lo, (uint64_t)p.rows_total, (uint64_t)w.Cin, a_rows)) return -1;
+  if (PASSES == 1) ta_lo = ta_hi;  // never loaded
+  else if (cached_act_map(&ta_lo, p.A_lo, (uint64_t)p.rows_total, (uint64_t)w.Cin, a_rows)) return -1;
   tp.NT = w.N / BN;
   const int total = (CL > 1 ? (tp.ntiles + 1) / 2 : tp.ntiles) * tp.NT;
   const int slots = num_sms / CL;
@@ -717,7 +733,7 @@ int launch_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
       pair_guard_begin(dev, ctx.stream);
     }
     const cudaError_t le =
-        cudaLaunchKernelEx(&cfg, conv_gemm_wg_kernel<BN, CL, MODE, REUSE>, ta_hi, ta_lo, w.tm_hi[bi], w.tm_lo[bi], tp);
+        cudaLaunchKernelEx(&cfg, conv_gemm_wg_kernel<BN, CL, MODE, REUSE, PASSES>, ta_hi, ta_lo, w.tm_hi[bi], w.tm_lo[bi], tp);
     if (guard) pair_guard_end(dev, ctx.stream);
     SSB_CUDA(le);
   }
@@ -725,18 +741,37 @@ int launch_m(Ctx& ctx, const GemmTC& p, TCParams tp, int num_sms) {
   counter->fetch_add(1, std::memory_order_relaxed);
   return 0;
 }
-template <int BN, int CL>
+template <int BN, int CL, int PASSES>
 int launch(Ctx& ctx, const GemmTC& p, const TCParams& tp, int num_sms) {
   switch (tp.e.mode) {
-    case EPI_GATE: return launch_m<BN, CL, EPI_GATE, false>(ctx, p, tp, num_sms);
-    case EPI_RES_SKIP: return launch_m<BN, CL, EPI_RES_SKIP, false>(ctx, p, tp, num_sms);
-    default: return launch_m<BN, CL, EPI_GENERIC, false>(ctx, p, tp, num_sms);
+    case EPI_GATE: return launch_m<BN, CL, EPI_GATE, false, PASSES>(ctx, p, tp, num_sms);
+    case EPI_RES_SKIP: return launch_m<BN, CL, EPI_RES_SKIP, false, PASSES>(ctx, p, tp, num_sms);
+    default: return launch_m<BN, CL, EPI_GENERIC, false, PASSES>(ctx, p, tp, num_sms);
   }
 }
 // the tap-reuse variant serves the CTA-pair sizes of 3-tap convs: the gate GEMMs of both denoisers, the vocoder's transposed
 // convs (3-tap, N = u * C) and its k = 3 ResBlock convs
 bool tap_reuse_eligible(const GemmTC& p, const ConvTC& w) {
   return w.taps == 3 && w.center == 1 && w.dil >= 1 && w.dil <= HALO && (p.e.mode == EPI_GATE || p.e.mode == EPI_GENERIC);
+}
+// large problems: CTA pairs (two row tiles x one 2*hb-wide N tile per cluster, the weight tile multicast to both) halve
+// the weight bytes each SM pulls through L2
+template <int PASSES>
+int dispatch(Ctx& ctx, const GemmTC& p, const TCParams& tp, int num_sms) {
+  const ConvTC& w = *p.w;
+  if ((int64_t)((p.ntiles + 1) / 2) * (w.N / (2 * w.hb)) >= (int64_t)num_sms) {
+    if (tap_reuse_eligible(p, w)) {
+      if (p.e.mode == EPI_GATE)
+        return w.hb == 64 ? launch_m<128, 2, EPI_GATE, true, PASSES>(ctx, p, tp, num_sms)
+                          : launch_m<64, 2, EPI_GATE, true, PASSES>(ctx, p, tp, num_sms);
+      return w.hb == 64 ? launch_m<128, 2, EPI_GENERIC, true, PASSES>(ctx, p, tp, num_sms)
+                        : launch_m<64, 2, EPI_GENERIC, true, PASSES>(ctx, p, tp, num_sms);
+    }
+    return w.hb == 64 ? launch<128, 2, PASSES>(ctx, p, tp, num_sms) : launch<64, 2, PASSES>(ctx, p, tp, num_sms);
+  }
+  // smaller problems: single CTAs on 64-wide N tiles.  (A 128-wide single-CTA tile would need ntiles * N / 128 >= 2 #SMs,
+  // which already meets the pair condition above when N % 128 == 0: it is never reached, so it is not built.)
+  return launch<64, 1, PASSES>(ctx, p, tp, num_sms);
 }
 
 }  // namespace
@@ -796,18 +831,7 @@ int conv_gemm_tc(Ctx& ctx, const GemmTC& p) {
   tp.tiles = p.tiles; tp.ntiles = p.ntiles; tp.taps = w.taps; tp.kchunks = w.Cin / BK;
   tp.dil = w.dil; tp.center = w.center; tp.N = w.N; tp.e = p.e;
   if (!tp.e.bias) tp.e.bias = w.bias;
-  // large problems: CTA pairs (two row tiles x one 2*hb-wide N tile per cluster, the weight tile multicast to both) halve
-  // the weight bytes each SM pulls through L2
-  if ((int64_t)((p.ntiles + 1) / 2) * (w.N / (2 * w.hb)) >= (int64_t)num_sms) {
-    if (tap_reuse_eligible(p, w)) {
-      if (p.e.mode == EPI_GATE) return w.hb == 64 ? launch_m<128, 2, EPI_GATE, true>(ctx, p, tp, num_sms) : launch_m<64, 2, EPI_GATE, true>(ctx, p, tp, num_sms);
-      return w.hb == 64 ? launch_m<128, 2, EPI_GENERIC, true>(ctx, p, tp, num_sms) : launch_m<64, 2, EPI_GENERIC, true>(ctx, p, tp, num_sms);
-    }
-    return w.hb == 64 ? launch<128, 2>(ctx, p, tp, num_sms) : launch<64, 2>(ctx, p, tp, num_sms);
-  }
-  // smaller problems: single CTAs on 64-wide N tiles.  (A 128-wide single-CTA tile would need ntiles * N / 128 >= 2 #SMs,
-  // which already meets the pair condition above when N % 128 == 0: it is never reached, so it is not built.)
-  return launch<64, 1>(ctx, p, tp, num_sms);
+  return p.single_pass ? dispatch<1>(ctx, p, tp, num_sms) : dispatch<3>(ctx, p, tp, num_sms);
 }
 
 int split_planes(Ctx& ctx, const float* x, int ld, int64_t rows, int C, float scale, __half* hi, __half* lo) {

@@ -12,6 +12,9 @@
 // hb = 64 when N % 128 == 0, else 32).  CTAs are persistent over the tiles.  The pair kernel is used when there are
 // >= num_SMs pair tiles (ceil(ntiles / 2) * N / (2 hb)), the single-CTA kernel with 64-wide N tiles otherwise
 // (conv_gemm_tc()).
+// single_pass (GemmTC): one wgmma per K step on the hi planes alone, i.e. the operands rounded once to fp16 (~11 mantissa
+// bits) with fp32 accumulation; the lo planes are not read.  A speed / accuracy choice of the mel denoiser and the vocoder
+// (ssb_model_set_mel_precision, ssb_vocoder_set_precision), not the default.
 // 3-tap convs at pair sizes take the tap-reuse variant: one halo-extended activation tile per K block serves all three taps.
 // Pair launches from different streams are ordered against each other on the device (conv_gemm_tc.cu).
 #pragma once
@@ -82,6 +85,7 @@ struct GemmTC {
   const int2* tiles = nullptr;
   int ntiles = 0;
   EpiTC e;
+  bool single_pass = false;  // true: hi*hi only (A_lo and W_lo unread); false: the 3-pass hi/lo split
 };
 
 bool tc_available();  // driver entry point for cuTensorMapEncodeTiled resolved

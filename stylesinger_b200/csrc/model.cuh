@@ -162,6 +162,8 @@ struct Model {
   bool persistent_groups = false;  // large batches: groups of <= 48 row tiles, one persistent launch each (mel sampler)
   bool use_tc = true;  // tensor-core path for the denoiser layer GEMMs (ssb_model_set_tensor_cores)
   bool fft_tc = true;  // tensor-core path for the decoder FFT blocks' FFN on long batches (ssb_model_set_fft_tensor_cores)
+  // SSB_TC_FP16 (ssb_model_set_mel_precision): the mel DiffNet's tensor-core GEMMs run single-pass fp16 (GemmTC::single_pass)
+  bool mel_fp16 = false;
 };
 
 struct VocStage {
@@ -187,6 +189,7 @@ struct Vocoder {
   float *lin_w = nullptr, *lin_b = nullptr;
   bool nsf = true;
   bool use_tc = true;
+  bool fp16 = false;  // SSB_TC_FP16 (ssb_vocoder_set_precision): tensor-core GEMMs single-pass fp16
 };
 
 // ---- packing helpers (pack.cu) -------------------------------------------------------------------

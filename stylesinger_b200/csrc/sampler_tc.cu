@@ -11,6 +11,8 @@
 // = 43 GEMM phases per step, separated by a grid-wide barrier (every phase reads what all CTAs wrote in
 // the previous one through +-dilation halos).  Tensor maps (activations + every layer's weights) live in a
 // device array; mbarrier phases and the smem ring persist across all 43*T phases.
+// PASSES = 1 (single-pass fp16, the mel sampler under ssb_model_set_mel_precision(SSB_TC_FP16)): only the hi planes of A and
+// W are loaded and each K step issues one wgmma per accumulator; the stage layout stays that of PASSES = 3.
 #include <cuda_fp16.h>
 #include <string.h>
 
@@ -250,6 +252,7 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
   }
 }
 
+template <int PASSES>
 __global__ void __launch_bounds__(256, 1)
 sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict__ phases, int nphases,
                   const int2* __restrict__ tiles, const int4* __restrict__ tile_pos, const UttRng* __restrict__ rng,
@@ -315,7 +318,7 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
           for (int kb = 0; kb < nk; ++kb) {
             mbar_wait(empty0 + 8 * stage, phase_bit ^ 1);
             const uint32_t fb = full0 + 8 * stage;
-            mbar_expect_tx(fb, STAGE);
+            mbar_expect_tx(fb, PASSES == 3 ? STAGE : A_TILE + B_TILE);
             const uint32_t sa = sbase + stage * STAGE;
             const int tap = kb / P.kchunks;
             const int c0 = (kb - tap * P.kchunks) * BK;
@@ -323,13 +326,13 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
             const int brow = tap * P.N + nt * BN;
             if (cs > 1) {
               tma_load_2d_mc(sa + cr * slice_bytes, mA, fb, c0, arow + cr * slice_rows, cmask);
-              tma_load_2d_mc(sa + A_TILE + cr * slice_bytes, mA + 1, fb, c0, arow + cr * slice_rows, cmask);
+              if constexpr (PASSES == 3) tma_load_2d_mc(sa + A_TILE + cr * slice_bytes, mA + 1, fb, c0, arow + cr * slice_rows, cmask);
             } else {
               tma_load_2d(sa, mA, fb, c0, arow);
-              tma_load_2d(sa + A_TILE, mA + 1, fb, c0, arow);
+              if constexpr (PASSES == 3) tma_load_2d(sa + A_TILE, mA + 1, fb, c0, arow);
             }
             tma_load_2d(sa + 2 * A_TILE, mW, fb, c0, brow);
-            tma_load_2d(sa + 2 * A_TILE + B_TILE, mW + 1, fb, c0, brow);
+            if constexpr (PASSES == 3) tma_load_2d(sa + 2 * A_TILE + B_TILE, mW + 1, fb, c0, brow);
             if (++stage == STAGES) { stage = 0; phase_bit ^= 1; }
           }
         }
@@ -375,12 +378,17 @@ sampler_tc_kernel(const CUtensorMap* __restrict__ maps, const SPhase* __restrict
 #pragma unroll
           for (int ks = 0; ks < BK / 16; ++ks) {
             const uint64_t off = (uint64_t)((ks * 32) >> 4);
-            wgmma_n64(acc0, dah + off, dbh + off, 1u);
-            wgmma_n64(acc0, dah + off, dbl + off, 1u);
-            wgmma_n64(acc0, dal + off, dbh + off, 1u);
-            wgmma_n64(acc1, dah + 512 + off, dbh + off, 1u);  // +8192 bytes: rows 64-127
-            wgmma_n64(acc1, dah + 512 + off, dbl + off, 1u);
-            wgmma_n64(acc1, dal + 512 + off, dbh + off, 1u);
+            if constexpr (PASSES == 3) {
+              wgmma_n64(acc0, dah + off, dbh + off, 1u);
+              wgmma_n64(acc0, dah + off, dbl + off, 1u);
+              wgmma_n64(acc0, dal + off, dbh + off, 1u);
+              wgmma_n64(acc1, dah + 512 + off, dbh + off, 1u);  // +8192 bytes: rows 64-127
+              wgmma_n64(acc1, dah + 512 + off, dbl + off, 1u);
+              wgmma_n64(acc1, dal + 512 + off, dbh + off, 1u);
+            } else {
+              wgmma_n64(acc0, dah + off, dbh + off, 1u);
+              wgmma_n64(acc1, dah + 512 + off, dbh + off, 1u);
+            }
           }
           wg_commit();
           fence_acc(acc0);
@@ -469,7 +477,9 @@ int sampler_tc_max_clusters(int cs) {
     init[dev] = true;
   }
   if (cache[cs] >= 0) return cache[cs];
-  cudaFuncSetAttribute(sampler_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+  // both pass counts have the same shared memory and launch bounds: one occupancy answer serves both
+  cudaFuncSetAttribute(sampler_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+  cudaFuncSetAttribute(sampler_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -481,7 +491,7 @@ int sampler_tc_max_clusters(int cs) {
   at[0].val.clusterDim.x = (unsigned)cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
   int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, sampler_tc_kernel, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+  if (cudaOccupancyMaxActiveClusters(&n, sampler_tc_kernel<3>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
   cache[cs] = n;
   return n;
 }
@@ -489,7 +499,7 @@ int sampler_tc_max_clusters(int cs) {
 int sampler_tc_max_ctas() { return sampler_tc_max_clusters(1); }
 
 int launch_sampler_tc(Ctx& ctx, const CUtensorMap* maps_dev, const SPhase* phases_dev, int nphases, const SeqDev& s,
-                      int max_nt, unsigned* barrier_ctr, int cs) {
+                      int max_nt, unsigned* barrier_ctr, int cs, bool single_pass) {
   const int ntiles = s.ntiles;
   if (ctx.dry) return 0;
   const int cap = sampler_tc_max_clusters(cs);
@@ -509,7 +519,7 @@ int launch_sampler_tc(Ctx& ctx, const CUtensorMap* maps_dev, const SPhase* phase
   at[1].id = cudaLaunchAttributeClusterDimension;
   at[1].val.clusterDim.x = (unsigned)cs; at[1].val.clusterDim.y = 1; at[1].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 2;
-  SSB_CUDA(cudaLaunchKernelEx(&cfg, sampler_tc_kernel, maps_dev, phases_dev, nphases, s.tiles, s.tile_pos, s.rng, ntiles,
+  SSB_CUDA(cudaLaunchKernelEx(&cfg, single_pass ? sampler_tc_kernel<1> : sampler_tc_kernel<3>, maps_dev, phases_dev, nphases, s.tiles, s.tile_pos, s.rng, ntiles,
                               barrier_ctr, cs));
   ++g_launches;
   return 0;

@@ -54,9 +54,10 @@ struct SPhase {
 
 int sampler_tc_max_ctas();
 int sampler_tc_max_clusters(int cs);  // co-resident clusters of size cs (cooperative launch limit)
-// runs the phases over the row tiles of `s`; the sampling phases draw with s.rng
+// runs the phases over the row tiles of `s`; the sampling phases draw with s.rng.  single_pass: one hi*hi wgmma per K step
+// (the lo planes are not read) instead of the 3-pass hi/lo split.
 int launch_sampler_tc(Ctx& ctx, const CUtensorMap* maps_dev, const SPhase* phases_dev, int nphases, const SeqDev& s,
-                      int max_nt, unsigned* barrier_ctr, int cs);
+                      int max_nt, unsigned* barrier_ctr, int cs, bool single_pass);
 int x80_planes(Ctx& ctx, const float* x, int64_t rows, __half* hi, __half* lo);
 
 }  // namespace ssb

@@ -21,7 +21,7 @@ GemmTC make_gemm_tc(const ConvTC& w, const SeqDev& s, const __half* A_hi, const 
   return g;
 }
 
-int run_dense(Ctx& c, const Dense& d, bool tc, const SeqDev& s, const DenseIn& in, const Epi& e) {
+int run_dense(Ctx& c, const Dense& d, bool tc, const SeqDev& s, const DenseIn& in, const Epi& e, bool single_pass) {
   SSB_CHECK(!e.bias, "run_dense: the bias is the layer's own");
   if (!tc) {
     SSB_CHECK(in.x != nullptr, "run_dense: the fp32 kernel needs the input as fp32 rows");
@@ -35,6 +35,7 @@ int run_dense(Ctx& c, const Dense& d, bool tc, const SeqDev& s, const DenseIn& i
   SSB_CHECK(e.mode == EPI_GENERIC && !e.add && e.beta == 1.0f && !e.out2,
             "run_dense: the tensor-core kernel's generic epilogue has no gate / skip mode, addend, beta or second fp32 output");
   GemmTC g = make_gemm_tc(d.t, s, in.hi, in.lo);
+  g.single_pass = single_pass;
   EpiTC& t = g.e;
   t.out = e.out; t.ldo = e.ldo;
   t.oh = e.out2_h; t.ol = e.out2_l; t.ldh = e.ldh; t.vec2 = e.vec2;
@@ -468,12 +469,14 @@ static int denoiser_heads(Ctx& c, const Denoiser& d, const SeqDev& s, DenoiserBu
   if (b.tc_heads) {
     {  // skip_projection (1/sqrt(L) folded into the packed weights) + ReLU -> planes
       GemmTC g = make_gemm_tc(d.skip_tc, s, b.skh, b.skl);
+      g.single_pass = b.single_pass;
       g.e.bias = d.skip_bias_pad; g.e.act = ACT_RELU; g.e.oh = b.sh; g.e.ol = b.sl; g.e.ldh = C;
       g.e.n_valid = C;
       RUN(conv_gemm_tc(c, g));
     }
     {  // output_projection (N padded to a tile multiple; only the first out_dims columns are meaningful)
       GemmTC g = make_gemm_tc(d.out_tc, s, b.sh, b.sl);
+      g.single_pass = b.single_pass;
       g.e.bias = d.out_bias_pad; g.e.out = b.head; g.e.ldo = b.ld_head;
       g.e.n_valid = (d.out_dims + 31) / 32 * 32;
       RUN(conv_gemm_tc(c, g));
@@ -502,6 +505,7 @@ int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBu
     if (b.tc) {
       {
         GemmTC g = make_gemm_tc(d.layers[l].dil.t, s, b.yh, b.yl);
+        g.single_pass = b.single_pass;
         // K = 3*C (taps of y); the hoisted conditioner projection arrives as an epilogue addend (one [rows, 2C] matrix per layer)
         g.e.add = b.condpre + (size_t)l * (size_t)s.rows * 2 * C; g.e.ld_add = 2 * C;
         g.e.mode = EPI_GATE; g.e.bias = d.layers[l].bias_gate_tc;
@@ -509,6 +513,7 @@ int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBu
         RUN(conv_gemm_tc(c, g));
       }
       GemmTC g = make_gemm_tc(d.layers[l].outp.t, s, b.zh, b.zl);
+      g.single_pass = b.single_pass;
       // residual stream carried ONLY as the fp16 hi/lo planes of y = x + step bias (in place: this epilogue reads
       // y_l[row] and writes y_{l+1}[row] for the same rows/columns): no fp32 x is read or written in the T x L loop
       g.e.mode = EPI_RES_SKIP; g.e.C = C; g.e.beta = 0.70710678118654752440f;
@@ -540,6 +545,7 @@ int denoiser_stack(Ctx& c, const Denoiser& d, const SeqDev& s, int t, DenoiserBu
 bool denoiser_tc_ok(const Model& m, const Denoiser& d) { return m.use_tc && d.tc_ok; }
 int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, DenoiserBufs* b) {
   b->tc = tc;
+  b->single_pass = false;
   b->condpre = nullptr;
   b->x = alloc_rows(c, s, d.C);
   b->y = b->zg = nullptr;
@@ -589,9 +595,10 @@ int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, Denoiser
 // once, [rows, 256] x [256, L*2C], once per sampler call.  condpre is layer-major (row pitch 2C floats instead of L * 2C):
 // matrix l is the GATE epilogue addend of layer l.
 static int hoist_cond_tc(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, __half* ch, __half* cl,
-                         float* condpre) {
+                         float* condpre, bool single_pass) {
   RUN(split_planes(c, cond_g, 256, s.rows, 256, 1.0f, ch, cl));
   GemmTC g = make_gemm_tc(d.cond_all_tc, s, ch, cl);
+  g.single_pass = single_pass;
   g.e.out = condpre; g.e.ldo = d.L * 2 * d.C;
   g.e.out_nb = 2 * d.C; g.e.out_bs = (int64_t)s.rows * 2 * d.C;
   return conv_gemm_tc(c, g);
@@ -599,7 +606,7 @@ static int hoist_cond_tc(Ctx& c, const Denoiser& d, const SeqDev& s, const float
 // Conditioner: the step-invariant projection of all L layers hoisted into one [rows, L*2C] buffer (tensor-core path:
 // hoist_cond_tc; SIMT path: row-major, the layers side by side).
 int prepare_cond(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, DenoiserBufs& b) {
-  if (b.tc) return hoist_cond_tc(c, d, s, cond_g, b.ch, b.cl, b.condpre);
+  if (b.tc) return hoist_cond_tc(c, d, s, cond_g, b.ch, b.cl, b.condpre, b.single_pass);
   ConvGemm g = make_gemm(d.cond_all, s, cond_g, 256);
   g.e.out = b.condall; g.e.ldo = d.L * 2 * d.C;
   return conv_gemm(c, g);
@@ -610,6 +617,7 @@ int mel_denoiser_eval(Ctx& c, const Denoiser& d, const SeqDev& s, int t, const f
   if (b.x80h) {  // tensor-core input projection: K padded 80 -> 128
     RUN(x80_planes(c, x80, s.rows, b.x80h, b.x80l));
     GemmTC g = make_gemm_tc(d.in_tc, s, b.x80h, b.x80l);
+    g.single_pass = b.single_pass;
     g.e.bias = d.in_proj.bias; g.e.act = ACT_RELU;  // planes of y = relu(in_proj) + step bias only
     g.e.oh = b.yh; g.e.ol = b.yl; g.e.ldh = d.C; g.e.vec2 = d.dtab + (size_t)t * d.L * d.C;
     RUN(conv_gemm_tc(c, g));
@@ -673,8 +681,9 @@ struct PersistentNet {
 };
 
 // Allocates the net's buffers and hoists its conditioner projection, so that its gate phases contract K = 3C and add
-// that projection in the epilogue.
-static int persistent_net_setup(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, int mb, PersistentNet* p) {
+// that projection in the epilogue.  single_pass: the hoisted projection's precision, that of the launch's GEMMs.
+static int persistent_net_setup(Ctx& c, const Denoiser& d, const SeqDev& s, const float* cond_g, int mb, bool single_pass,
+                                PersistentNet* p) {
   p->d = &d;
   p->mb = mb;
   p->x = alloc_rows(c, s, d.C);
@@ -684,7 +693,7 @@ static int persistent_net_setup(Ctx& c, const Denoiser& d, const SeqDev& s, cons
   __half* cl = alloc_half_rows(c, s, 256);
   p->condpre = alloc_rows(c, s, d.L * 2 * d.C, false);
   WS_OK(c);
-  return hoist_cond_tc(c, d, s, cond_g, ch, cl, p->condpre);
+  return hoist_cond_tc(c, d, s, cond_g, ch, cl, p->condpre, single_pass);
 }
 
 // Writes the net's tensor maps into maps[p.mb, p.mb + nmaps(L)); activation boxes of 128 / cs rows, one cs-th of an
@@ -748,7 +757,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
   const size_t mk = c.mark();
   float* xm = alloc_rows(c, s, 80);
   P net;
-  RUN(persistent_net_setup(c, d, s, cond_g, 0, &net));
+  RUN(persistent_net_setup(c, d, s, cond_g, 0, m.mel_fp16, &net));
   __half* x80h = alloc_half_rows(c, s, 128);  // planes of x_t, K padded 80 -> 128
   __half* x80l = alloc_half_rows(c, s, 128);
   const int M_X80 = P::nmaps(L), W_IN = M_X80 + 2, nmaps = W_IN + 2;
@@ -783,7 +792,7 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
     }
     SSB_CUDA(cudaMemcpyAsync(maps_dev, maps.data(), sizeof(CUtensorMap) * nmaps, cudaMemcpyHostToDevice, c.stream));
     SSB_CUDA(cudaMemcpyAsync(ph_dev, ph.data(), sizeof(SPhase) * nph, cudaMemcpyHostToDevice, c.stream));
-    RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s, 2 * C / 64, ctr, CS));
+    RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s, 2 * C / 64, ctr, CS, m.mel_fp16));
   }
   RUN(mel_finish(c, m, s, xm, mel_tight));
   c.release(mk);
@@ -841,6 +850,7 @@ int run_mel_diffusion(Ctx& c, const Model& m, const SeqDev& s, const float* cond
   const size_t mk = c.mark();
   DenoiserBufs b;
   RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
+  b.single_pass = b.tc && m.mel_fp16;
   float* xm = alloc_rows(c, s, 80);
   WS_OK(c);
   RUN(prepare_cond(c, d, s, cond_g, b));
@@ -871,6 +881,7 @@ int run_mel_diffusion_plms(Ctx& c, const Model& m, const SeqDev& s, const float*
   const size_t mk = c.mark();
   DenoiserBufs b;
   RUN(alloc_denoiser(c, d, s, denoiser_tc_ok(m, d), &b));
+  b.single_pass = b.tc && m.mel_fp16;
   float* xm = alloc_rows(c, s, 80);
   float* xp = alloc_rows(c, s, 80);
   float* hist[3] = {alloc_rows(c, s, 80), alloc_rows(c, s, 80), alloc_rows(c, s, 80)};
@@ -927,7 +938,8 @@ static int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev
   const int CS = 2;
   const size_t mk = c.mark();
   P net[2];
-  for (int n = 0; n < 2; ++n) RUN(persistent_net_setup(c, m.f0net[n], s, n == 0 ? cond0 : cond1, n * P::nmaps(L), &net[n]));
+  for (int n = 0; n < 2; ++n)
+    RUN(persistent_net_setup(c, m.f0net[n], s, n == 0 ? cond0 : cond1, n * P::nmaps(L), false, &net[n]));
   const int nmaps = 2 * P::nmaps(L);
   const int nph = 2 * T * (2 * L + 2);
   CUtensorMap* maps_dev = c.alloc<CUtensorMap>((size_t)nmaps);
@@ -980,7 +992,7 @@ static int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev
     }
     SSB_CUDA(cudaMemcpyAsync(maps_dev, maps.data(), sizeof(CUtensorMap) * nmaps, cudaMemcpyHostToDevice, c.stream));
     SSB_CUDA(cudaMemcpyAsync(ph_dev, ph.data(), sizeof(SPhase) * nph, cudaMemcpyHostToDevice, c.stream));
-    RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s, 2 * (2 * C / 64), ctr, CS));
+    RUN(launch_sampler_tc(c, maps_dev, ph_dev, nph, s, 2 * (2 * C / 64), ctr, CS, false));
   }
   c.release(mk);
   return 0;
@@ -1086,6 +1098,7 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
     c.release(mk);
   }
   const bool tc = v.use_tc && tc_available();
+  const bool sp = tc && v.fp16;  // single-pass fp16 tensor-core GEMMs (ssb_vocoder_set_precision)
   int C = v.cfg.initial_channel;
   float* x = alloc_rows(c, s1, C);
   __half *pin_h = nullptr, *pin_l = nullptr;  // planes of leaky_relu(stage input), when the next ups runs on tensor cores
@@ -1148,7 +1161,7 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
       Epi e;
       e.out = xu; e.ldo = st.u * Co;
       if (res_tc && !nsf) lrelu_planes(e, px_h, px_l, st.u * Co);
-      RUN(run_dense(c, st.up, up_tc, sin, {xin, C, pin_h, pin_l, ACT_LRELU, 0.1f}, e));
+      RUN(run_dense(c, st.up, up_tc, sin, {xin, C, pin_h, pin_l, ACT_LRELU, 0.1f}, e, sp));
     }
     if (nsf) RUN(noise_conv_add(c, so, s256, xu, Co, Co, har, st.nc_w, st.nc_b, st.nc_s, res_tc ? px_h : nullptr, px_l, 0.1f, st.nc_wt));
     const int nconv = rb2 ? 2 : 3;
@@ -1162,7 +1175,7 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
           Epi e;
           if (res_tc) lrelu_planes(e, pt_h, pt_l, Cw);
           else { e.out = xt; e.ldo = Cw; }
-          RUN(run_dense(c, st.rb[j].c1[mI], res_tc, sw, {rin, Cw, rin_h, rin_l, ACT_LRELU, 0.1f}, e));
+          RUN(run_dense(c, st.rb[j].c1[mI], res_tc, sw, {rin, Cw, rin_h, rin_l, ACT_LRELU, 0.1f}, e, sp));
         }
         Epi e;  // ResBlock1: r = c2(leaky_relu(xt)) + r ; ResBlock2: r = c(leaky_relu(r)) + r
         e.res = rin; e.ld_res = Cw;
@@ -1173,8 +1186,8 @@ int run_vocoder(Ctx& c, const Vocoder& v, const Seq& seq, const float* mel_tight
           e.out = acc; e.ldo = Cw; e.accum = (j > 0); e.gamma = lastj ? 1.0f / (float)v.nk : 1.0f;
           if (lastj && next_up_tc) lrelu_planes(e, pa_h, pa_l, Cw);
         }
-        if (rb2) RUN(run_dense(c, st.rb[j].c1[mI], res_tc, sw, {rin, Cw, rin_h, rin_l, ACT_LRELU, 0.1f}, e));
-        else RUN(run_dense(c, st.rb[j].c2[mI], res_tc, sw, {xt, Cw, pt_h, pt_l, ACT_LRELU, 0.1f}, e));
+        if (rb2) RUN(run_dense(c, st.rb[j].c1[mI], res_tc, sw, {rin, Cw, rin_h, rin_l, ACT_LRELU, 0.1f}, e, sp));
+        else RUN(run_dense(c, st.rb[j].c2[mI], res_tc, sw, {xt, Cw, pt_h, pt_l, ACT_LRELU, 0.1f}, e, sp));
         rin = r; rin_h = pr_h; rin_l = pr_l;
       }
     }

@@ -27,8 +27,9 @@ struct DenseIn {
   float slope = 0.1f;
 };
 // Enqueues the layer over the rows of `s` on the tensor-core (tc) or the fp32 FFMA kernel.  `e` describes the epilogue
-// for both (bias: the layer's own); a field the chosen kernel cannot honour is an error.
-int run_dense(Ctx& c, const Dense& d, bool tc, const SeqDev& s, const DenseIn& in, const Epi& e);
+// for both (bias: the layer's own); a field the chosen kernel cannot honour is an error.  single_pass: the tensor-core
+// kernel's single-pass fp16 mode (GemmTC::single_pass); the FFMA kernel ignores it.
+int run_dense(Ctx& c, const Dense& d, bool tc, const SeqDev& s, const DenseIn& in, const Epi& e, bool single_pass = false);
 
 int fft_blocks(Ctx& c, const FFT& f, const SeqDev& s, float* x, const float* keep, bool tc = false);
 int run_encoder(Ctx& c, const Model& m, const SeqDev& sp, const int32_t* tok_g, const int32_t* note_g,
@@ -51,6 +52,7 @@ struct DenoiserBufs {
   bool tc_heads;                // also: the skip accumulator is in the chunk-tiled layout (EpiTC::skip_tiled)
   int ld_head;
   bool tc;
+  bool single_pass;             // tensor-core path: single-pass fp16 GEMMs (the mel net under SSB_TC_FP16); false from alloc_denoiser
 };
 bool denoiser_tc_ok(const Model& m, const Denoiser& d);
 int alloc_denoiser(Ctx& c, const Denoiser& d, const SeqDev& s, bool tc, DenoiserBufs* b);

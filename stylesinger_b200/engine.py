@@ -14,7 +14,7 @@ import torch
 
 from . import _lib
 from ._lib import AcousticInputs, AcousticOutputs, HParams, ModelSwitches, TensorDesc, VocoderConfigEx, check, lib
-from .hparams import DEFAULT_VOCODER_CONFIG, resolve, switches
+from .hparams import DEFAULT_VOCODER_CONFIG, TC_PRECISIONS, resolve, switches
 from .schedules import multinomial_table, prodiff_table, sampler_table
 
 MEL_DECODERS = {"diffsinger": 0, "prodiff": 1}  # SSB_MEL_DECODER_* of include/stylesinger_b200.h
@@ -162,7 +162,8 @@ class AcousticModel:
     deterministic FastSpeech-2 PitchPredictors; no F0 schedule, no F0 noise).  The model switches hparams['emo'],
     ['style'], ['umln'] and ['use_txt_cond'] (all True by default) select the modules the checkpoint has
     (ssb_model_create_ex3); batches for a model without emo / style need no emo_embed / reference mels
-    (pack_batch(..., emo=, style=), or ``self.pack_batch``)."""
+    (pack_batch(..., emo=, style=), or ``self.pack_batch``).  hparams['tc_precision'] ('split' or 'fp16') sets the
+    precision of the mel DiffNet's tensor-core GEMMs (set_mel_precision)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], hparams=None, device=None, max_positions=4096):
         _require_cuda()
@@ -196,6 +197,7 @@ class AcousticModel:
         self.K = None  # K_step of the mel sampler; None follows T
         if self.mel_decoder == "diffsinger" and int(hp["K_step"]) != hp["timesteps"]:
             self.set_mel_k_step(int(hp["K_step"]))
+        self.set_mel_precision(hp["tc_precision"])
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -218,6 +220,16 @@ class AcousticModel:
     def set_persistent_groups(self, enable=True):
         """Large batches: run the mel sampler as one persistent launch per group of <= 48 row tiles (default off)."""
         return bool(lib.ssb_model_set_persistent_groups(self._h, 1 if enable else 0))
+
+    def set_mel_precision(self, mode: str):
+        """Precision of the mel DiffNet's tensor-core GEMMs on every mel sampler (DDPM, K_step, PLMS, ProDiff): 'split'
+        (fp16 hi/lo planes, 3 MMAs per K step; the default) or 'fp16' (one MMA on operands rounded once to fp16, faster, at
+        the accuracy cost stated in the README).  The F0 samplers and every other module stay split; GEMMs on the FFMA
+        path are unchanged.  An unknown mode raises ValueError and changes nothing."""
+        if mode not in TC_PRECISIONS:
+            raise ValueError(f"mel precision must be one of {sorted(TC_PRECISIONS)}, got {mode!r}")
+        check(lib.ssb_model_set_mel_precision(self._h, TC_PRECISIONS[mode]), "ssb_model_set_mel_precision")
+        self.mel_precision = mode
 
     def set_fft_tensor_cores(self, enable: bool) -> bool:
         """Decoder FFT-block FFN GEMMs on the tensor-core kernel for batches of >= 1024 frames (default on)."""
@@ -531,9 +543,10 @@ class Vocoder:
     """Packed HiFi-GAN(-NSF) generator on one GPU (ssb_vocoder_t).  ``denoise_c`` > 0 runs the reference's output denoiser
     (hparams['vocoder_denoise_c'], tasks/tts/vocoder_infer/hifigan_nsf.py:73-74) on every generated waveform, with the
     fft_size / hop_size / win_size of ``denoise_hp`` (the reference reads its global hparams; default: ``config``, then the
-    WavDenoiser defaults).  Nothing is created for the denoiser unless a call asks for it."""
+    WavDenoiser defaults).  Nothing is created for the denoiser unless a call asks for it.  ``tc_precision`` ('split' or
+    'fp16', hparams['tc_precision']) sets the precision of the tensor-core GEMMs (set_precision)."""
 
-    def __init__(self, state_dict, config=None, device=None, denoise_c=0.0, denoise_hp=None):
+    def __init__(self, state_dict, config=None, device=None, denoise_c=0.0, denoise_hp=None, tc_precision="split"):
         _require_cuda()
         self.denoise_c = float(denoise_c)
         self._denoise_hp = denoise_hp
@@ -550,6 +563,7 @@ class Vocoder:
         check(lib.ssb_vocoder_create_ex(C.byref(handle), arr, len(sd), C.byref(vc)), "ssb_vocoder_create_ex")
         self._h = handle
         self._ws = _Workspace(self.device)
+        self.set_precision(tc_precision)
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -559,6 +573,15 @@ class Vocoder:
 
     def set_tensor_cores(self, enable=True):
         return bool(lib.ssb_vocoder_set_tensor_cores(self._h, 1 if enable else 0))
+
+    def set_precision(self, mode: str):
+        """Precision of the generator's tensor-core GEMMs (the ups and ResBlock convs on tensor cores, every layout):
+        'split' (the default) or 'fp16' (single pass), as AcousticModel.set_mel_precision.  The output denoiser and the FFMA
+        convs are unchanged."""
+        if mode not in TC_PRECISIONS:
+            raise ValueError(f"vocoder precision must be one of {sorted(TC_PRECISIONS)}, got {mode!r}")
+        check(lib.ssb_vocoder_set_precision(self._h, TC_PRECISIONS[mode]), "ssb_vocoder_set_precision")
+        self.precision = mode
 
     max_frames_per_call = 24000  # ~0.9 MB of stage buffers per frame: bounds the workspace to ~20 GB
 
@@ -840,13 +863,14 @@ def _op_call(args, fields, fn, what):
     check(fn(C.byref(args), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), what)
 
 
-def op_gemm(path, offsets, rows, w, b=None, dilation=1, gate=False, **epi):
+def op_gemm(path, offsets, rows, w, b=None, dilation=1, gate=False, single_pass=False, **epi):
     """Exactly one conv_gemm (path 0, fp32 FFMA) or conv_gemm_tc (path 1, tensor cores) call (ssb_op_gemm) over
     caller-owned device tensors in the guard-banded layout of `offsets` with `rows` rows (utterance b at rows
     [rs_b, rs_b + L_b), rs_0 = 16, rs_{b+1} = rs_b + L_b + 16, plus 256 rows of tail slack).  w [N, Cin, k] / b [N]
     are torch-layout weights (gate=True: the DiffNet gate interleave).  epi: the A operand (a / lda / a_act / a_slope /
     a_scale on path 0, a_hi / a_lo on path 1) and the fields of ssb_op_gemm_args' epilogue; tensors are passed by
-    pointer, nothing is copied.  Returns nothing: the kernel writes into the given buffers."""
+    pointer, nothing is copied.  single_pass=True (path 1 only): one hi*hi MMA per K step, the kernel of the 'fp16'
+    tc_precision (a_lo is not read).  Returns nothing: the kernel writes into the given buffers."""
     _require_cuda()
     off = np.ascontiguousarray(offsets, np.int32)
     N, Cin, k = w.shape
@@ -854,7 +878,8 @@ def op_gemm(path, offsets, rows, w, b=None, dilation=1, gate=False, **epi):
     bc = None if b is None else b.detach().cpu().float().contiguous()
     a = _lib.OpGemmArgs(path=path, frame_offsets=off.ctypes.data, B=len(off) - 1, rows=rows, Cin=Cin, N=N, k=k,
                         dilation=dilation, gate=int(gate), w_host=wc.data_ptr(), b_host=None if bc is None else bc.data_ptr(),
-                        a_slope=0.1, a_scale=1.0, alpha=1.0, act_slope=0.1, beta=1.0, gamma=1.0, plane_slope=0.1)
+                        a_slope=0.1, a_scale=1.0, alpha=1.0, act_slope=0.1, beta=1.0, gamma=1.0, plane_slope=0.1,
+                        single_pass=int(bool(single_pass)))
     _op_call(a, epi, lib.ssb_op_gemm, "ssb_op_gemm")
 
 

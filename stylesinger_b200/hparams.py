@@ -50,7 +50,14 @@ DEFAULT_HPARAMS = {
     "predictor_grad": 1.0, "use_txt_cond": True, "vocoder_ckpt": "checkpoints/hifigan",
     "vocoder_denoise_c": 0.0, "spec_min": [-6.0] * 80, "spec_max": _SPEC_MAX,
     "processed_data_dir": "data/processed/style", "exp_name": "",
+    # not a reference key: precision of the tensor-core GEMMs of the mel DiffNet and the vocoder (TC_PRECISIONS)
+    "tc_precision": "split",
 }
+
+# hparams['tc_precision'] -> SSB_TC_SPLIT / SSB_TC_FP16.  'split' (the default): fp32 operands as fp16 hi/lo planes, 3 MMAs
+# per K step, mel within 1e-3 of the fp32 reference.  'fp16': one MMA on operands rounded once to fp16 - a third of the
+# MMAs, at the accuracy cost README "Single-pass fp16 mode" states.  Applies to the mel DiffNet and the vocoder only.
+TC_PRECISIONS = {"split": 0, "fp16": 1}
 
 # HiFi-GAN-V1 style generator; product(upsample_rates) must equal hop_size (256).
 DEFAULT_VOCODER_CONFIG = {
@@ -131,6 +138,8 @@ def _check_supported(hp):
             raise NotImplementedError(f"stylesinger_b200: hparams[{k!r}] must be True or False, got {hp.get(k)!r}")
     if hp.get("rel_pos"):
         raise NotImplementedError("rel_pos is not selected by egs/stylesinger.yaml")
+    if hp.get("tc_precision") not in TC_PRECISIONS:
+        raise ValueError(f"tc_precision must be one of {sorted(TC_PRECISIONS)}, got {hp.get('tc_precision')!r}")
     if prodiff:  # ProDiffusion.forward(infer=True) never reads K_step or pndm_speedup (prodiff.py:204-222)
         return
     # shallow diffusion (DiffusionDecoder.forward, shallow_diffusion_tts.py:297-304): q_sample at K_step - 1 of the

@@ -31,7 +31,8 @@ class StyleSingerInfer:
         self.model = AcousticModel(model_state_dict, self.hparams, self.device)
         # HifiGAN.spec2wav (tasks/tts/vocoder_infer/hifigan_nsf.py:73-74): denoise the waveform when vocoder_denoise_c > 0
         self.vocoder = Vocoder(vocoder_state_dict, vocoder_config, self.device,
-                               denoise_c=self.hparams.get("vocoder_denoise_c", 0.0), denoise_hp=self.hparams)
+                               denoise_c=self.hparams.get("vocoder_denoise_c", 0.0), denoise_hp=self.hparams,
+                               tc_precision=self.hparams["tc_precision"])
         self._cnt = torch.zeros(1, dtype=torch.int32, device=self.device)
         self._pinned = []  # [(pinned tensor, weakref to the numpy array handed out last)]: see _host_out
 

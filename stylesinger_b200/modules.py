@@ -303,11 +303,13 @@ class PitchPredictor(_Registered):
 
 class HifiGAN:
     """``spec2wav(mel, f0=...)`` with numpy in / numpy out (tasks/tts/vocoder_infer/hifigan_nsf.py:62-75).  ``denoise_c`` is
-    hparams['vocoder_denoise_c']: > 0 runs the reference's output denoiser (:14-22,73-74) on the waveform."""
+    hparams['vocoder_denoise_c']: > 0 runs the reference's output denoiser (:14-22,73-74) on the waveform.
+    ``tc_precision`` is hparams['tc_precision'] ('split' or 'fp16') of the vocoder this facade creates; a given ``engine``
+    keeps its own (Vocoder.set_precision)."""
 
     def __init__(self, state_dict=None, config=None, device=None, use_nsf=True, engine: Optional[Vocoder] = None,
-                 denoise_c=0.0):
-        self.v = engine if engine is not None else Vocoder(state_dict, config, device)
+                 denoise_c=0.0, tc_precision="split"):
+        self.v = engine if engine is not None else Vocoder(state_dict, config, device, tc_precision=tc_precision)
         self.use_nsf = use_nsf
         self.denoise_c = float(denoise_c)
 

@@ -45,6 +45,9 @@ def main():
     ap.add_argument("--use-gt-dur", action="store_true", help="feed the items' ground-truth mel2ph (reference hparam use_gt_dur)")
     ap.add_argument("--vocoder-denoise-c", type=float, default=0.0,
                     help="reference hparam vocoder_denoise_c: > 0 denoises every waveform (hifigan_nsf.py:14-22,73-74)")
+    ap.add_argument("--tc-precision", choices=("split", "fp16"), default="split",
+                    help="tensor-core GEMMs of the mel denoiser and the vocoder: 'split' (3 MMAs, the default) or 'fp16' "
+                         "(single pass: faster, less accurate; README 'Single-pass fp16 mode')")
     for sw in ("emo", "style", "umln", "use_txt_cond"):  # the checkpoint's model switches (egs/stylesinger.yaml)
         ap.add_argument(f"--{sw.replace('_', '-')}", type=int, choices=(0, 1), default=1,
                         help=f"reference hparam {sw} of the checkpoint (default 1)")
@@ -57,7 +60,7 @@ def main():
 
     hp = resolve(timesteps=args.T, K_step=args.T if args.k_step is None else args.k_step, f0_timesteps=args.T,
                  vocoder_denoise_c=args.vocoder_denoise_c, emo=bool(args.emo), style=bool(args.style),
-                 umln=bool(args.umln), use_txt_cond=bool(args.use_txt_cond))
+                 umln=bool(args.umln), use_txt_cond=bool(args.use_txt_cond), tc_precision=args.tc_precision)
     sd, path = formats.load_state_dict(args.ckpt, "model")
     vsd, vcfg, vpath = formats.load_vocoder_checkpoint(args.vocoder)
     print(f"| acoustic checkpoint {path} ({len(sd)} tensors); vocoder {vpath}")

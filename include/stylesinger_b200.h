@@ -115,6 +115,8 @@ void ssb_model_free(ssb_model_t* m);
 #define SSB_MEL_DECODER_DIFFSINGER 0 /* FFT decoder -> mel_out -> ln_proj -> DDPM over postdiff.denoise_fn (the default) */
 #define SSB_MEL_DECODER_PRODIFF 1    /* ProDiff teacher (modules/diff/prodiff.py:59-232): decoder_inp is the condition of an
                                       * x0-predicting sampler over diff_decoder.denoise_fn; no FFT decoder / mel_out / ln_proj */
+#define SSB_MEL_DECODER_FFT 2        /* FastSpeech 2 decoder alone (stylesinger.py:185-186, fs2.py:233-237): mel_out(decoder(
+                                      * decoder_inp)) * tgt_nonpadding is the mel; no ln_proj, no mel DiffNet, no diffusion */
 /* ssb_model_create with the mel decoder chosen: ssb_model_create(...) == ssb_model_create_ex(..., SSB_MEL_DECODER_DIFFSINGER).
  * PRODIFF loads the mel DiffNet from "diff_decoder.denoise_fn.*" and needs no "postdiff.*" / "ln_proj.*" ("decoder.*" is
  * still packed for ssb_fft_decoder; "mel_out.*" and the "diff_decoder.*" buffers are accepted and ignored).  The schedule
@@ -162,6 +164,26 @@ typedef struct {
 int ssb_model_create_ex3(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
                          int32_t mel_decoder, int32_t f0_gen, const ssb_model_switches* switches);
 
+/* ssb_model_create_ex3 with the speaker input chosen: ssb_model_create_ex3(..., d, f, sw) == ssb_model_create_ex4(..., d, f,
+ * sw, 0).  hparams['use_spk_id'] (modules/fastspeech/fs2.py:37-43): with use_spk_id = 1, "spk_embed_proj.weight" [rows, 256]
+ * (Embedding(num_spk + 1, 256), no bias) is packed as a lookup table, and every acoustic entry (ssb_acoustic_forward,
+ * ssb_acoustic_forward_keyed, ssb_predict_durations and their *_workspace_bytes) reads in->spk_ids instead of
+ * in->spk_embed: spk = table[spk_ids[b]] (stylesinger.py:130), out->spk_proj returns those rows.  The ids are checked on the
+ * host against [0, rows) before anything is launched; NULL spk_ids is an error.  Everything downstream of spk is unchanged.
+ * With use_spk_id = 0 "spk_embed_proj.weight" is the Linear(256, 256) over in->spk_embed (and .bias is required).
+ * "spk_embed_f0.*" / "spk_embed_dur.*" (use_split_spk_id) are never read.  use_spk_id combines with every mel decoder, F0
+ * generator and switch.
+ * SSB_MEL_DECODER_FFT models pack "decoder.*" and "mel_out.*"; "postdiff.*", "ln_proj.*" and "diff_decoder.*" are neither
+ * required nor read.  Their forward is the FFT decoder and mel_out with the tgt_nonpadding row mask into out->mel_out
+ * (out->coarse_mel, when asked for, holds the same values); skip_mel_diffusion has no effect, pndm_speedup is ignored as
+ * the reference ignores it.  On an FFT model these are errors, refused with a message before any launch: out->diff_cond,
+ * a non-NULL in->mel_noise, ssb_model_set_schedule(which = 0), ssb_model_set_mel_k_step (any K),
+ * ssb_mel_diffusion_sample[_plms], ssb_mel_prodiff_sample and ssb_denoiser_eval(which = 0).  ssb_model_set_mel_precision
+ * is accepted and changes nothing (there is no mel DiffNet).  Fails, naming the cause and leaving *out NULL, before anything
+ * is allocated when use_spk_id is not 0 / 1 or mel_decoder / f0_gen is unknown. */
+int ssb_model_create_ex4(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
+                         int32_t mel_decoder, int32_t f0_gen, const ssb_model_switches* switches, int32_t use_spk_id);
+
 /* Diffusion schedules (GaussianDiffusion.__init__ modules/diff/shallow_diffusion_tts.py:68-122;
  * GaussianMultinomialDiffusion.__init__ modules/diff/gaussian_multinomial_diffusion.py:208-284).
  * which: 0 = mel denoiser, 1 = both F0 denoisers.  Host arrays:
@@ -208,6 +230,8 @@ typedef struct {
   int32_t pndm_speedup;           /* 0: DDPM ancestral sampling, K steps (the StyleSinger default, DiffusionDecoder.forward);
                                    * k in [1, K): PLMS with iteration interval k (hparams['pndm_speedup'],
                                    * modules/diff/shallow_diffusion_tts.py:164-197,254-260): K / k (+1) denoiser evaluations */
+  const int32_t* spk_ids;         /* host [B]: speaker ids, read only on a model created with use_spk_id = 1
+                                   * (ssb_model_create_ex4), which then never reads spk_embed; other models never read it */
 } ssb_acoustic_inputs;
 
 /* Outputs (all optional except mel_out/f0_denorm when diffusion runs); device, tight packed. */

@@ -48,7 +48,8 @@ class AcousticInputs(C.Structure):
                 ("spk_embed", C.c_void_p), ("emo_embed", C.c_void_p), ("ref_mels", C.c_void_p), ("ref_f0", C.c_void_p),
                 ("mel2ph", C.c_void_p), ("dur", C.c_void_p), ("f0", C.c_void_p), ("uv", C.c_void_p),
                 ("f0_gauss_noise", C.c_void_p * 2), ("f0_unif_noise", C.c_void_p * 2), ("mel_noise", C.c_void_p),
-                ("seed", C.c_uint64), ("skip_mel_diffusion", C.c_int32), ("pndm_speedup", C.c_int32)]
+                ("seed", C.c_uint64), ("skip_mel_diffusion", C.c_int32), ("pndm_speedup", C.c_int32),
+                ("spk_ids", C.c_void_p)]
 
 
 class AcousticOutputs(C.Structure):
@@ -113,6 +114,7 @@ EXPORTS = [
     "ssb_op_attention_ex", "ssb_attention_launch_count",
     "ssb_model_create_ex3",
     "ssb_model_set_mel_precision", "ssb_vocoder_set_precision",
+    "ssb_model_create_ex4",
 ]
 
 
@@ -130,6 +132,7 @@ def _load():
         "ssb_model_create_ex": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32]),
         "ssb_model_create_ex2": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32, i32]),
         "ssb_model_create_ex3": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32, i32, P(ModelSwitches)]),
+        "ssb_model_create_ex4": (C.c_int, [P(vp), P(TensorDesc), i32, P(HParams), i32, i32, P(ModelSwitches), i32]),
         "ssb_pitch_predictor_workspace_bytes": (sz, [vp, vp, i32]),
         "ssb_pitch_predictor": (C.c_int, [vp, i32, vp, vp, i32, vp, vp, sz, vp]),
         "ssb_model_free": (None, [vp]),

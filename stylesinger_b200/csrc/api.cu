@@ -29,6 +29,25 @@ static int project_vec(Ctx& c, const Conv& w, const float* in_tight, int B, floa
   return 0;
 }
 
+// spk_embed_proj(spk_id) of a use_spk_id model (Embedding(num_spk + 1, 256), fs2.py:37-38): the ids (host, checked by the
+// caller) go into a one-sequence layout of B rows and pitch_embed's row gather reads the table rows
+static int gather_spk(Ctx& c, const Model& m, const int32_t* ids_host, int B, float* out_tight) {
+  Seq s1;
+  int32_t offs[2] = {0, B};
+  s1.build(offs, 1);
+  const size_t mk = c.mark();
+  SeqDev sd;
+  RUN(upload_layout(c, s1, 1, &sd));
+  int32_t* idx = alloc_rows_i32(c, sd);
+  float* o = alloc_rows(c, sd, 256);
+  WS_OK(c);
+  if (!c.dry) SSB_CUDA(cudaMemcpyAsync(idx + s1.rs[0], ids_host, sizeof(int32_t) * B, cudaMemcpyHostToDevice, c.stream));
+  RUN(embed_rows(c, sd, idx, m.spk_tab, m.spk_rows, 1.0f, o, 256, 256, 0));
+  RUN(unpack_rows(c, sd, o, 256, out_tight, 256, 256));
+  c.release(mk);
+  return 0;
+}
+
 // StyleSinger.forward(infer=True) (stylesinger.py:119-187); durations_only stops after add_dur.
 int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ssb_acoustic_outputs& out,
                  bool durations_only, int32_t* dur_out, float* logdur_out, const uint64_t* utt_seeds) {
@@ -46,6 +65,16 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   SSB_CHECK(m.f0_gen != SSB_F0_GEN_CONV || (!in.f0_gauss_noise[0] && !in.f0_gauss_noise[1] && !in.f0_unif_noise[0] &&
                                             !in.f0_unif_noise[1]),
             "acoustic: a model with the conv F0 generator draws no F0 noise (f0_gauss_noise / f0_unif_noise must be NULL)");
+  const bool fft = m.mel_decoder == SSB_MEL_DECODER_FFT;
+  SSB_CHECK(!fft || !out.diff_cond, "acoustic: a model with the FFT mel decoder has no diff_cond (there is no ln_proj)");
+  SSB_CHECK(!fft || !in.mel_noise, "acoustic: a model with the FFT mel decoder draws no mel noise (mel_noise must be NULL)");
+  if (m.spk_id) {  // use_spk_id: every id must index the table (checked here, before anything is launched)
+    SSB_CHECK(in.spk_ids, "acoustic: a model created with use_spk_id needs spk_ids (host [B] speaker ids)");
+    for (int b = 0; b < B; ++b)
+      SSB_CHECK(in.spk_ids[b] >= 0 && in.spk_ids[b] < m.spk_rows,
+                "acoustic: spk_ids[" + std::to_string(b) + "] = " + std::to_string(in.spk_ids[b]) + " is outside [0, " +
+                    std::to_string(m.spk_rows) + ") (the rows of spk_embed_proj.weight)");
+  }
   Seq qp, qr, qf;
   qp.build(in.ph_offsets, B);
   if (style_on) qr.build(in.ref_offsets, B);
@@ -66,7 +95,10 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
   RUN(pack_rows_i32(c, sp, in.note, note));
   RUN(pack_rows_i32(c, sp, in.note_type, ntype));
   RUN(pack_rows(c, sp, in.note_dur, 1, ndur, 1, 1));
-  RUN(project_vec(c, m.spk_proj, in.spk_embed, B, spk));
+  if (m.spk_id)
+    RUN(gather_spk(c, m, in.spk_ids, B, spk));
+  else
+    RUN(project_vec(c, m.spk_proj, in.spk_embed, B, spk));
   if (emo_on) RUN(project_vec(c, m.emo_proj, in.emo_embed, B, emo));
   if (out.spk_proj && !c.dry) SSB_CUDA(cudaMemcpyAsync(out.spk_proj, spk, sizeof(float) * B * H, cudaMemcpyDeviceToDevice, c.stream));
   if (out.emo_proj && !c.dry) SSB_CUDA(cudaMemcpyAsync(out.emo_proj, emo, sizeof(float) * B * H, cudaMemcpyDeviceToDevice, c.stream));
@@ -232,6 +264,21 @@ int run_acoustic(Ctx& c, const Model& m, const ssb_acoustic_inputs& in, const ss
       SSB_CHECK(out.mel_out != nullptr, "acoustic: mel_out required");
       RUN(run_mel_diffusion(c, m, sf, dec, nullptr, in.mel_noise, out.mel_out, &qf));
     }
+    return 0;
+  }
+
+  if (fft) {
+    // decoder 'fft' (stylesinger.py:185-186): ret['mel_out'] = run_decoder(decoder_inp) = mel_out(decoder(x)) *
+    // tgt_nonpadding (fs2.py:233-237) - the DiffSinger path's coarse mel, with no ln_proj and no diffusion after it
+    float* mel = alloc_rows(c, sf, 80);
+    float* xd = alloc_rows(c, sf, H);
+    WS_OK(c);
+    RUN(run_fft_decoder(c, m, sf, dec, xd, long_batch_tc(m, sf)));
+    ConvGemm g = make_gemm(m.mel_out, sf, xd, H);
+    g.e.rowmask = tgt; g.e.out = mel; g.e.ldo = 80;
+    RUN(conv_gemm(c, g));
+    if (out.mel_out) RUN(unpack_rows(c, sf, mel, 80, out.mel_out, 80, 80));
+    if (out.coarse_mel) RUN(unpack_rows(c, sf, mel, 80, out.coarse_mel, 80, 80));
     return 0;
   }
 
@@ -427,7 +474,7 @@ static int op_attn_launch(Ctx& c, const SeqDev& dq, const SeqDev& dk, const ssb_
 
 extern "C" {
 
-int ssb_version(void) { return 103; }
+int ssb_version(void) { return 104; }
 const char* ssb_last_error(void) { return ssb::last_error(); }
 
 int ssb_model_create(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp) {
@@ -444,14 +491,21 @@ int ssb_model_create_ex2(ssb_model_t** out, const ssb_tensor_desc* tensors, int3
 }
 int ssb_model_create_ex3(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
                          int32_t mel_decoder, int32_t f0_gen, const ssb_model_switches* sw) {
+  return ssb_model_create_ex4(out, tensors, n, hp, mel_decoder, f0_gen, sw, 0);
+}
+int ssb_model_create_ex4(ssb_model_t** out, const ssb_tensor_desc* tensors, int32_t n, const ssb_hparams* hp,
+                         int32_t mel_decoder, int32_t f0_gen, const ssb_model_switches* sw, int32_t use_spk_id) {
   if (out) *out = nullptr;
-  SSB_CHECK(mel_decoder == SSB_MEL_DECODER_DIFFSINGER || mel_decoder == SSB_MEL_DECODER_PRODIFF,
+  SSB_CHECK(mel_decoder == SSB_MEL_DECODER_DIFFSINGER || mel_decoder == SSB_MEL_DECODER_PRODIFF ||
+                mel_decoder == SSB_MEL_DECODER_FFT,
             "ssb_model_create_ex: unknown mel_decoder " + std::to_string(mel_decoder) +
-                " (SSB_MEL_DECODER_DIFFSINGER = 0, SSB_MEL_DECODER_PRODIFF = 1)");
+                " (SSB_MEL_DECODER_DIFFSINGER = 0, SSB_MEL_DECODER_PRODIFF = 1, SSB_MEL_DECODER_FFT = 2)");
   SSB_CHECK(f0_gen == SSB_F0_GEN_GMDIFF || f0_gen == SSB_F0_GEN_CONV,
             "ssb_model_create_ex2: unknown f0_gen " + std::to_string(f0_gen) +
                 " (SSB_F0_GEN_GMDIFF = 0, SSB_F0_GEN_CONV = 1)");
   SSB_CHECK(sw, "ssb_model_create_ex3: null switches");
+  SSB_CHECK(use_spk_id == 0 || use_spk_id == 1,
+            "ssb_model_create_ex4: use_spk_id must be 0 or 1, got " + std::to_string(use_spk_id));
   {
     const char* names[4] = {"emo", "style", "umln", "use_txt_cond"};
     const int32_t vals[4] = {sw->emo, sw->style, sw->umln, sw->use_txt_cond};
@@ -476,7 +530,7 @@ int ssb_model_create_ex3(ssb_model_t** out, const ssb_tensor_desc* tensors, int3
     }
   }
   ssb_model* m = new ssb_model();
-  if (build_model(tm, *hp, &m->m, mel_decoder, f0_gen, *sw) != 0) {
+  if (build_model(tm, *hp, &m->m, mel_decoder, f0_gen, *sw, use_spk_id != 0) != 0) {
     delete m;
     return -1;
   }
@@ -502,6 +556,8 @@ int ssb_model_set_schedule(ssb_model_t* m, int32_t which, int32_t T, const float
 
 int ssb_model_set_mel_k_step(ssb_model_t* m, int32_t K) {
   SSB_CHECK(m, "null model");
+  SSB_CHECK(m->m.mel_decoder != SSB_MEL_DECODER_FFT,
+            "ssb_model_set_mel_k_step: a model with the FFT mel decoder (SSB_MEL_DECODER_FFT) has no mel sampler and no K_step");
   SSB_CHECK(K >= 0, "ssb_model_set_mel_k_step: K must be >= 0 (0 follows the schedule's T), got " + std::to_string(K));
   SSB_CHECK(m->m.mel_decoder == SSB_MEL_DECODER_DIFFSINGER,
             "ssb_model_set_mel_k_step: a ProDiff model has no K_step (ProDiffusion.forward never reads it)");
@@ -549,8 +605,16 @@ int ssb_acoustic_forward_keyed(const ssb_model_t* m, const ssb_acoustic_inputs* 
   return run_acoustic(c, m->m, *in, *out, false, nullptr, nullptr, utt_seeds);
 }
 
+// The standalone mel-sampler entries need a mel DiffNet, which an FFT model does not have
+static int need_mel_diffnet(const Model& m, const char* what) {
+  SSB_CHECK(m.mel_decoder != SSB_MEL_DECODER_FFT,
+            std::string(what) + ": a model with the FFT mel decoder (SSB_MEL_DECODER_FFT) has no mel DiffNet");
+  return 0;
+}
+
 static int mel_diff_impl(Ctx& c, const Model& m, const float* cond, const float* coarse, const int32_t* offs, int B,
                          const float* noise, uint64_t seed, float* mel_out) {
+  RUN(need_mel_diffnet(m, "ssb_mel_diffusion_sample"));
   SSB_CHECK(m.mel_decoder == SSB_MEL_DECODER_DIFFSINGER,
             "ssb_mel_diffusion_sample: the DDPM sampler needs a DiffSinger model; use ssb_mel_prodiff_sample on a ProDiff model");
   Seq q;
@@ -567,6 +631,7 @@ static int mel_diff_impl(Ctx& c, const Model& m, const float* cond, const float*
 }
 static int mel_plms_impl(Ctx& c, const Model& m, const float* cond, const float* coarse, const int32_t* offs, int B,
                          const float* q_noise, uint64_t seed, int interval, float* mel_out) {
+  RUN(need_mel_diffnet(m, "ssb_mel_diffusion_sample_plms"));
   Seq q;
   q.build(offs, B);
   q.seed = seed;
@@ -581,6 +646,7 @@ static int mel_plms_impl(Ctx& c, const Model& m, const float* cond, const float*
 }
 static int mel_prodiff_impl(Ctx& c, const Model& m, const float* cond, const int32_t* offs, int B, const float* noise,
                             uint64_t seed, float* mel_out) {
+  RUN(need_mel_diffnet(m, "ssb_mel_prodiff_sample"));
   SSB_CHECK(m.mel_decoder == SSB_MEL_DECODER_PRODIFF,
             "ssb_mel_prodiff_sample: the ProDiff sampler needs a model created with SSB_MEL_DECODER_PRODIFF");
   Seq q;
@@ -636,6 +702,7 @@ int ssb_denoiser_eval(const ssb_model_t* m, int32_t which, const float* x, const
   SSB_CHECK(m && x && cond && frame_offsets && out && workspace && which >= 0 && which <= 2, "bad argument");
   SSB_CHECK(which == 0 || m->m.f0_gen == SSB_F0_GEN_GMDIFF,
             "ssb_denoiser_eval: a model with the conv F0 generator (SSB_F0_GEN_CONV) has no F0 denoisers (which = 1 / 2)");
+  if (which == 0) RUN(need_mel_diffnet(m->m, "ssb_denoiser_eval(which = 0)"));
   Ctx c = make_ctx(workspace, workspace_bytes, stream);
   Seq q;
   q.build(frame_offsets, B);

@@ -126,6 +126,11 @@ struct Model {
   float* pitch_emb = nullptr;
   float *spec_min = nullptr, *spec_max = nullptr;
   Conv spk_proj, emo_proj;
+  // hparams['use_spk_id'] (ssb_model_create_ex4): spk_embed_proj is an Embedding [spk_rows, 256] looked up by the host's
+  // speaker ids instead of the Linear spk_proj over a speaker vector
+  bool spk_id = false;
+  float* spk_tab = nullptr;
+  int spk_rows = 0;
   FFT enc, dec;
   Conv dp_conv[4]; float* dp_ln_g[4]; float* dp_ln_b[4]; Conv dp_lin; int dp_layers = 2;
   // style adaptor
@@ -142,9 +147,10 @@ struct Model {
   // SSB_F0_GEN_GMDIFF: hparams['f0_gen'] == 'gmdiff' (two F0 diffusion samplers); SSB_F0_GEN_CONV: 'conv' (pp above)
   int f0_gen = SSB_F0_GEN_GMDIFF;
   Denoiser melnet;
-  Conv mel_out, ln_proj;  // DiffSinger mode only
+  Conv mel_out, ln_proj;  // mel_out: DiffSinger and FFT modes; ln_proj: DiffSinger mode only
   // SSB_MEL_DECODER_DIFFSINGER: hparams['decoder'] == 'diffsinger' (FFT decoder + mel_out + ln_proj + DDPM over postdiff.*);
-  // SSB_MEL_DECODER_PRODIFF: 'prodiff' (decoder_inp straight into the x0-predicting sampler over diff_decoder.*)
+  // SSB_MEL_DECODER_PRODIFF: 'prodiff' (decoder_inp straight into the x0-predicting sampler over diff_decoder.*);
+  // SSB_MEL_DECODER_FFT: 'fft' (FFT decoder + mel_out is the mel; no melnet)
   int mel_decoder = SSB_MEL_DECODER_DIFFSINGER;
   // model switches (ssb_model_create_ex3): emo_proj is packed only with emo; the style adaptor, codebooks, l1 and align only
   // with style; umln builds nothing (identity at inference); use_txt_cond adds decoder_inp to ln_proj's input
@@ -201,7 +207,8 @@ int pack_linear(DevicePool& pool, const HostTensor* w, const HostTensor* b, Conv
 int pack_dense(DevicePool& pool, const HostTensor* w, const HostTensor* b, int dil, PackMode mode, Dense* out,
                const HostTensor* g = nullptr /* weight-norm g: w is v */, int row0 = 0, int nrows = -1);
 int pack_conv_transpose(DevicePool& pool, const HostTensor* v, const HostTensor* g, const HostTensor* b, int u, Conv* out);
-int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder, int f0_gen, const ssb_model_switches& sw);
+int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder, int f0_gen, const ssb_model_switches& sw,
+                bool use_spk_id);
 // ln_proj's input width under the switches sw (stylesinger.py:92-100)
 inline int cond_width(const ssb_model_switches& sw) { return 80 + 256 * (1 + sw.use_txt_cond + sw.emo + sw.style); }
 int build_vocoder(TensorMap& tm, const ssb_vocoder_config_ex& cfg, Vocoder* v);

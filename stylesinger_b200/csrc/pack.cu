@@ -431,14 +431,17 @@ static int build_pitch_predictor(TensorMap& tm, DevicePool& pool, const std::str
   return 0;
 }
 
-int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder, int f0_gen, const ssb_model_switches& sw) {
+int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder, int f0_gen, const ssb_model_switches& sw,
+                bool use_spk_id) {
   DevicePool& pool = m->pool;
   m->hp = hp;
   m->mel_decoder = mel_decoder;
   m->f0_gen = f0_gen;
   m->sw = sw;
   m->cond_width = cond_width(sw);
+  m->spk_id = use_spk_id;
   const bool prodiff = mel_decoder == SSB_MEL_DECODER_PRODIFF;
+  const bool fft = mel_decoder == SSB_MEL_DECODER_FFT;
   const int H = hp.hidden_size;
   SSB_CHECK(H == 256, "hidden_size must be 256");
   SSB_CHECK(hp.dur_layers <= 4 && hp.rq_depth <= 8, "unsupported dur_layers / rq_depth");
@@ -459,11 +462,23 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder,
   m->dur_w = upload_tensor(pool, tm.get("note_encoder.dur_ln.weight", {H, 1}));
   m->dur_b = upload_tensor(pool, tm.get("note_encoder.dur_ln.bias", {H}));
   m->pitch_emb = upload_tensor(pool, tm.get("pitch_embed.weight", {300, H}));
-  if (!prodiff) {  // ProDiffusion.norm_spec / denorm_spec are the identity (prodiff.py:225-229): its spec_min/max go unread
+  // ProDiffusion.norm_spec / denorm_spec are the identity (prodiff.py:225-229): its spec_min/max go unread; an FFT model
+  // has no diffusion at all
+  if (!prodiff && !fft) {
     m->spec_min = upload_tensor(pool, tm.get("postdiff.spec_min"));
     m->spec_max = upload_tensor(pool, tm.get("postdiff.spec_max"));
   }
-  PK(pack_linear(pool, tm.get("spk_embed_proj.weight"), tm.get("spk_embed_proj.bias"), &m->spk_proj));
+  if (use_spk_id) {
+    // Embedding(num_spk + 1, H) (fs2.py:37-38, common_layers.py:62-67): a lookup table, no bias
+    const HostTensor* t = tm.get("spk_embed_proj.weight");
+    if (!t) goto fail;
+    SSB_CHECK(t->shape.size() == 2 && t->shape[0] >= 1 && t->shape[1] == H,
+              "ssb_model_create_ex4: with use_spk_id, spk_embed_proj.weight must be [rows, " + std::to_string(H) + "]");
+    m->spk_tab = upload_tensor(pool, t);
+    m->spk_rows = (int)t->shape[0];
+  } else {
+    PK(pack_linear(pool, tm.get("spk_embed_proj.weight"), tm.get("spk_embed_proj.bias"), &m->spk_proj));
+  }
   if (sw.emo) PK(pack_linear(pool, tm.get("emo_embed_proj.weight"), tm.get("emo_embed_proj.bias"), &m->emo_proj));
   PK(build_fft(tm, pool, "encoder.", hp.enc_layers, hp.enc_ffn_kernel, false, &m->enc));
   PK(build_fft(tm, pool, "decoder.", hp.dec_layers, hp.dec_ffn_kernel, true, &m->dec));
@@ -538,6 +553,9 @@ int build_model(TensorMap& tm, const ssb_hparams& hp, Model* m, int mel_decoder,
     // StyleSinger.__init__ with decoder 'prodiff' (stylesinger.py:111-117): the mel DiffNet is diff_decoder.denoise_fn; there
     // is no postdiff / ln_proj, and mel_out (built by FastSpeech2.__init__) is not used at inference (:176-177)
     PK(build_denoiser(tm, pool, "diff_decoder.denoise_fn.", hp.mel_channels, hp.mel_layers, hp.mel_cycle, hp.mel_bins, hp.mel_bins, false, &m->melnet));
+  } else if (fft) {
+    // decoder 'fft' (stylesinger.py:185-186): run_decoder = mel_out(decoder(x)) * tgt_nonpadding; no ln_proj / postdiff
+    PK(pack_linear(pool, tm.get("mel_out.weight"), tm.get("mel_out.bias"), &m->mel_out));
   } else {
     PK(build_denoiser(tm, pool, "postdiff.denoise_fn.", hp.mel_channels, hp.mel_layers, hp.mel_cycle, hp.mel_bins, hp.mel_bins, false, &m->melnet));
     PK(pack_linear(pool, tm.get("mel_out.weight"), tm.get("mel_out.bias"), &m->mel_out));
@@ -725,6 +743,8 @@ static int build_dtab(Denoiser& d, DevicePool& pool, int T, const float* step_em
 
 int set_schedule(Model* m, int which, int T, const float* step_emb, const float* gtab, const float* mtab,
                  cudaStream_t stream) {
+  SSB_CHECK(which != 0 || m->mel_decoder != SSB_MEL_DECODER_FFT,
+            "set_schedule: a model with the FFT mel decoder (SSB_MEL_DECODER_FFT) has no mel diffusion schedule (which = 0)");
   SSB_CHECK(T >= 1 && T <= 4000, "set_schedule: bad T");
   SSB_CHECK(step_emb && gtab, "set_schedule: null tables");
   std::vector<float> g(gtab, gtab + (size_t)T * 8);

@@ -25,23 +25,25 @@ def _p2p_device(device):
 
 
 def scatter_utterances(utts: Optional[List[dict]], src: int = 0, device=None, pin: bool = False,
-                       keep_on_device: bool = False, emo: bool = True, style: bool = True):
+                       keep_on_device: bool = False, emo: bool = True, style: bool = True, spk_id: bool = False):
     """Rank `src` owns `utts` (list of per-utterance CPU tensors, see synth.make_utterance); every rank returns
     (its PackedBatch, the global indices of its utterances).  Metadata goes through scatter_object_list, tensors
     through point-to-point send/recv (NCCL over NVLink when `device` is a CUDA device, gloo on CPU).
     `keep_on_device`: with a CUDA `device` the received shard stays in HBM (no host bounce before the engine call).
     `emo` / `style`: the model switches of the receiving model (pack_batch): without them no emo_embed / reference mels
-    are packed or sent."""
+    are packed or sent.  `spk_id`: the receiving model uses speaker ids (use_spk_id): each shard carries its host ids
+    instead of spk_embed rows."""
     rank, world = dist.get_rank(), dist.get_world_size()
     dev = _p2p_device(device)
     if rank == src:
         lens = [int(u["mel2ph"].shape[0]) if "mel2ph" in u else int(len(u["txt_tokens"])) for u in utts]
         bins = lpt_assign(lens, world)
         # fewer utterances than ranks leaves some bins empty: those ranks get an empty batch (B = 0) and skip the compute
-        packed = [pack_batch([utts[i] for i in b], use_mel2ph=all("mel2ph" in utts[i] for i in b), emo=emo, style=style)
+        packed = [pack_batch([utts[i] for i in b], use_mel2ph=all("mel2ph" in utts[i] for i in b), emo=emo, style=style,
+                             spk_id=spk_id)
                   if b else empty_batch()
                   for b in bins]
-        meta = [{"B": p.B, "ph": p.ph_offsets, "ref": p.ref_offsets, "fr": p.frame_offsets, "idx": b, "pad": p.may_have_pad_frames,
+        meta = [{"B": p.B, "ph": p.ph_offsets, "ref": p.ref_offsets, "fr": p.frame_offsets, "idx": b, "pad": p.may_have_pad_frames, "spk": p.spk_ids,
                  "shapes": {k: (tuple(v.shape), str(v.dtype)) for k, v in p.t.items()}} for p, b in zip(packed, bins)]
     else:
         packed, meta = None, [None] * world
@@ -64,10 +66,10 @@ def scatter_utterances(utts: Optional[List[dict]], src: int = 0, device=None, pi
             buf = torch.empty(shape, dtype=getattr(torch, dt.replace("torch.", "")), device=dev)
             dist.recv(buf, src=src)
             t[k] = buf if (keep_on_device and dev.type == "cuda") else buf.cpu()
-        pb = PackedBatch(m["B"], m["ph"], m["ref"], m["fr"], t, m["pad"])
+        pb = PackedBatch(m["B"], m["ph"], m["ref"], m["fr"], t, m["pad"], m["spk"])
     if pin and torch.cuda.is_available() and not (keep_on_device and dev.type == "cuda"):
         pb = PackedBatch(pb.B, pb.ph_offsets, pb.ref_offsets, pb.frame_offsets, {k: v.pin_memory() for k, v in pb.t.items()},
-                         pb.may_have_pad_frames)
+                         pb.may_have_pad_frames, pb.spk_ids)
     return pb, m["idx"]
 
 

@@ -17,7 +17,7 @@ from ._lib import AcousticInputs, AcousticOutputs, HParams, ModelSwitches, Tenso
 from .hparams import DEFAULT_VOCODER_CONFIG, TC_PRECISIONS, resolve, switches
 from .schedules import multinomial_table, prodiff_table, sampler_table
 
-MEL_DECODERS = {"diffsinger": 0, "prodiff": 1}  # SSB_MEL_DECODER_* of include/stylesinger_b200.h
+MEL_DECODERS = {"diffsinger": 0, "prodiff": 1, "fft": 2}  # SSB_MEL_DECODER_* of include/stylesinger_b200.h
 F0_GENS = {"gmdiff": 0, "conv": 1}  # SSB_F0_GEN_*
 
 
@@ -98,13 +98,14 @@ class PackedBatch:
     ref_offsets: Optional[np.ndarray]  # None for a model without style (no reference mels)
     frame_offsets: Optional[np.ndarray]
     t: Dict[str, torch.Tensor] = field(default_factory=dict)  # txt_tokens, note, note_type (int32), note_dur,
-    # spk_embed, [emo_embed], [ref_mels, ref_f0], [mel2ph int32], [f0], [uv]
+    # [spk_embed], [emo_embed], [ref_mels, ref_f0], [mel2ph int32], [f0], [uv]
     may_have_pad_frames: bool = True  # False when the host knows every frame maps to a phone (mel2ph > 0 everywhere)
+    spk_ids: Optional[np.ndarray] = None  # host int32 [B] speaker ids, for a use_spk_id model (in place of t["spk_embed"])
 
     def to(self, device, non_blocking=True):
         return PackedBatch(self.B, self.ph_offsets, self.ref_offsets, self.frame_offsets,
                            {k: v.to(device, non_blocking=non_blocking) for k, v in self.t.items()},
-                           self.may_have_pad_frames)
+                           self.may_have_pad_frames, self.spk_ids)
 
     def h2d_bytes(self):
         return int(sum(v.numel() * v.element_size() for v in self.t.values()))
@@ -114,10 +115,11 @@ class PackedBatch:
         return int(self.frame_offsets[-1]) if self.frame_offsets is not None else 0
 
 
-def pack_batch(utts: List[dict], use_mel2ph=True, pin=False, emo=True, style=True) -> PackedBatch:
+def pack_batch(utts: List[dict], use_mel2ph=True, pin=False, emo=True, style=True, spk_id=False) -> PackedBatch:
     """Concatenate per-utterance CPU tensors (as produced by synth.make_utterance) into one PackedBatch.
     emo / style: the model switches of the model the batch is for.  Without emo, no emo_embed is packed (utterances need
-    none); without style, no ref_mels / ref_f0 are packed and ref_offsets is None."""
+    none); without style, no ref_mels / ref_f0 are packed and ref_offsets is None.  spk_id: the batch is for a use_spk_id
+    model: each utterance's integer u["spk_id"] goes to the host array spk_ids, and no spk_embed is packed."""
     def offs(lens):
         return np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
 
@@ -127,8 +129,12 @@ def pack_batch(utts: List[dict], use_mel2ph=True, pin=False, emo=True, style=Tru
     fo = offs([len(u["mel2ph"]) for u in utts]) if use_mel2ph else None
     cat = lambda k, dt: torch.cat([u[k].reshape(-1) if u[k].dim() == 1 else u[k] for u in utts]).to(dt).contiguous()
     t = {"txt_tokens": cat("txt_tokens", torch.int32), "note": cat("note", torch.int32),
-         "note_type": cat("note_type", torch.int32), "note_dur": cat("note_dur", torch.float32),
-         "spk_embed": torch.stack([u["spk_embed"] for u in utts]).float().contiguous()}
+         "note_type": cat("note_type", torch.int32), "note_dur": cat("note_dur", torch.float32)}
+    ids = None
+    if spk_id:
+        ids = np.array([operator.index(u["spk_id"]) for u in utts], dtype=np.int32)
+    else:
+        t["spk_embed"] = torch.stack([u["spk_embed"] for u in utts]).float().contiguous()
     if emo:
         t["emo_embed"] = torch.stack([u["emo_embed"] for u in utts]).float().contiguous()
     if style:
@@ -140,7 +146,7 @@ def pack_batch(utts: List[dict], use_mel2ph=True, pin=False, emo=True, style=Tru
         pad = bool((t["mel2ph"] <= 0).any())
     if pin and torch.cuda.is_available():
         t = {k: v.pin_memory() for k, v in t.items()}
-    return PackedBatch(B, po, ro, fo, t, pad)
+    return PackedBatch(B, po, ro, fo, t, pad, ids)
 
 
 class _Workspace:
@@ -162,7 +168,10 @@ class AcousticModel:
     deterministic FastSpeech-2 PitchPredictors; no F0 schedule, no F0 noise).  The model switches hparams['emo'],
     ['style'], ['umln'] and ['use_txt_cond'] (all True by default) select the modules the checkpoint has
     (ssb_model_create_ex3); batches for a model without emo / style need no emo_embed / reference mels
-    (pack_batch(..., emo=, style=), or ``self.pack_batch``).  hparams['tc_precision'] ('split' or 'fp16') sets the
+    (pack_batch(..., emo=, style=), or ``self.pack_batch``).  hparams['decoder'] 'fft' is the FastSpeech 2 decoder alone:
+    its mel is the output, with no diffusion.  hparams['use_spk_id'] makes spk_embed_proj a speaker table looked up by
+    integer ids (utterances carry ``spk_id`` instead of ``spk_embed``; ssb_model_create_ex4).  Both need
+    hparams['extended_models'] = True.  hparams['tc_precision'] ('split' or 'fp16') sets the
     precision of the mel DiffNet's tensor-core GEMMs (set_mel_precision)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], hparams=None, device=None, max_positions=4096):
@@ -185,15 +194,23 @@ class AcousticModel:
         self.mel_decoder = hp["decoder"]
         self.f0_gen = hp["f0_gen"]
         self.switches = switches(hp)
+        self.spk_id = bool(hp["use_spk_id"])
+        if self.spk_id and hp.get("num_spk") is not None:  # Embedding(num_spk + 1, H) (fs2.py:37-38)
+            rows = int(sd["spk_embed_proj.weight"].shape[0])
+            if rows != int(hp["num_spk"]) + 1:
+                raise ValueError(f"spk_embed_proj.weight has {rows} rows; hparams num_spk = {hp['num_spk']} needs "
+                                 f"num_spk + 1 = {int(hp['num_spk']) + 1}")
         sw = ModelSwitches(**{k: int(v) for k, v in self.switches.items()})
         arr, keep = _descs(sd)
         handle = C.c_void_p()
-        check(lib.ssb_model_create_ex3(C.byref(handle), arr, len(sd), C.byref(h), MEL_DECODERS[self.mel_decoder],
-                                       F0_GENS[self.f0_gen], C.byref(sw)), "ssb_model_create_ex3")
+        check(lib.ssb_model_create_ex4(C.byref(handle), arr, len(sd), C.byref(h), MEL_DECODERS[self.mel_decoder],
+                                       F0_GENS[self.f0_gen], C.byref(sw), int(self.spk_id)), "ssb_model_create_ex4")
         self._h = handle
         self._ws = _Workspace(self.device)
         self.T = self.f0_T = None
-        self.set_timesteps(hp["timesteps"], hp["f0_timesteps"] if self.f0_gen == "gmdiff" else None)
+        # an FFT model has no mel sampler, a conv-F0 model no F0 samplers: neither gets a schedule
+        self.set_timesteps(hp["timesteps"] if self.mel_decoder != "fft" else None,
+                           hp["f0_timesteps"] if self.f0_gen == "gmdiff" else None)
         self.K = None  # K_step of the mel sampler; None follows T
         if self.mel_decoder == "diffsinger" and int(hp["K_step"]) != hp["timesteps"]:
             self.set_mel_k_step(int(hp["K_step"]))
@@ -206,8 +223,9 @@ class AcousticModel:
             self._h = None
 
     def pack_batch(self, utts: List[dict], use_mel2ph=True, pin=False) -> PackedBatch:
-        """pack_batch with the fields this model reads (no emo_embed without emo, no reference mels without style)."""
-        return pack_batch(utts, use_mel2ph, pin, emo=self.switches["emo"], style=self.switches["style"])
+        """pack_batch with the fields this model reads (no emo_embed without emo, no reference mels without style, speaker
+        ids instead of spk_embed with use_spk_id)."""
+        return pack_batch(utts, use_mel2ph, pin, emo=self.switches["emo"], style=self.switches["style"], spk_id=self.spk_id)
 
     def set_tensor_cores(self, enable=True):
         """wgmma (fp16 hi/lo split, 3 MMAs) vs fp32 FFMA for the denoiser layer GEMMs. Returns the mode in effect."""
@@ -281,7 +299,13 @@ class AcousticModel:
             self._keep.append(fo)
             a.frame_offsets = fo.ctypes.data
         t = pb.t
-        keys = ["txt_tokens", "note", "note_type", "note_dur", "spk_embed"]
+        keys = ["txt_tokens", "note", "note_type", "note_dur"]
+        if self.spk_id:  # the library reads the host ids (a batch without them reaches it as NULL and is refused)
+            if pb.spk_ids is not None:
+                self._keep.append(np.ascontiguousarray(pb.spk_ids, np.int32))
+                a.spk_ids = self._keep[-1].ctypes.data
+        else:
+            keys.append("spk_embed")
         keys += ["emo_embed"] if self.switches["emo"] else []  # forward_model passes none then (inference/StyleSinger.py:44-47)
         keys += ["ref_mels", "ref_f0"] if self.switches["style"] else []
         for k in keys:
@@ -307,7 +331,8 @@ class AcousticModel:
         a.seed = int(seed)
         a.skip_mel_diffusion = 1 if skip_mel else 0
         # reference hparam: 0 / absent = DDPM (the StyleSinger default); the ProDiff sampler ignores it, as the reference does
-        a.pndm_speedup = 0 if self.mel_decoder == "prodiff" else int(self.hp.get("pndm_speedup") or 0)
+        # (an FFT model has no sampler at all)
+        a.pndm_speedup = 0 if self.mel_decoder != "diffsinger" else int(self.hp.get("pndm_speedup") or 0)
         return a
 
     # -- entry points ------------------------------------------------------------------------------
@@ -352,6 +377,8 @@ class AcousticModel:
         for k, sw in (("emo_proj", "emo"), ("style", "style"), ("rq_codes", "style")):
             if k in want and not self.switches[sw]:
                 raise _lib.SsbError(f"AcousticModel.forward: a model without {sw} (hparams {sw}=False) has no {k}")
+        if "diff_cond" in want and self.mel_decoder == "fft":
+            raise _lib.SsbError("AcousticModel.forward: a model with decoder 'fft' has no diff_cond (there is no ln_proj)")
         if skip_mel_diffusion:
             want.discard("mel_out")  # never written in that mode: do not hand back an uninitialised buffer
         else:

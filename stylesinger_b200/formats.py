@@ -187,8 +187,11 @@ def item_to_utterance(item: dict, hparams: dict, with_mel2ph: bool = True) -> Di
          "note": torch.as_tensor(np.asarray(item["ep_pitches"])[:mt]).long(),
          "note_dur": torch.as_tensor(np.asarray(item["ep_notedurs"], np.float32)[:mt]).float(),
          "note_type": torch.as_tensor(np.asarray(item["ep_types"])[:mt]).long(),
-         "spk_embed": torch.as_tensor(np.asarray(item["spk_embed"], np.float32)).float().reshape(-1),
          "ref_mels": torch.from_numpy(mel[:T].copy()), "ref_f0": torch.from_numpy(f0)}
+    if hparams.get("use_spk_id"):  # the dataset's speaker id (tasks/StyleSinger/dataset.py:63-64,93-95)
+        u["spk_id"] = int(item["spk_id"])
+    else:
+        u["spk_embed"] = torch.as_tensor(np.asarray(item["spk_embed"], np.float32)).float().reshape(-1)
     if hparams.get("emo", True):  # a model without emo reads no emotion embedding (the item may have none)
         u["emo_embed"] = torch.as_tensor(np.asarray(item["emo_embed"], np.float32)).float().reshape(-1)
     if with_mel2ph:

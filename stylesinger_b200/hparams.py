@@ -39,7 +39,7 @@ DEFAULT_HPARAMS = {
     "use_pos_embed": True, "encoder_type": "fft", "decoder_type": "fft", "dur_loss": "mse",
     "use_pitch_embed": True, "use_energy_embed": False, "pitch_type": "frame",
     "mel_vmin": -6, "mel_vmax": 1.5, "timesteps": 100, "K_step": 100, "f0_timesteps": 100,
-    "use_spk_id": False, "use_spk_embed": True, "emo": True, "emo_size": 256, "style": True,
+    "use_spk_id": False, "use_spk_embed": True, "num_spk": 150, "emo": True, "emo_size": 256, "style": True,
     "umln": True, "nRQ": 128, "rq_depth": 4, "f0_gen": "gmdiff", "f0_residual_layers": 10,
     "f0_residual_channels": 192, "f0_dilation_cycle_length": 4, "f0_max_beta": 0.06,
     "decoder": "diffsinger", "residual_layers": 20, "residual_channels": 256,
@@ -52,7 +52,15 @@ DEFAULT_HPARAMS = {
     "processed_data_dir": "data/processed/style", "exp_name": "",
     # not a reference key: precision of the tensor-core GEMMs of the mel DiffNet and the vocoder (TC_PRECISIONS)
     "tc_precision": "split",
+    # not a reference key: True admits the two model options of the reference's code that egs/stylesinger.yaml does not
+    # select, decoder 'fft' and use_spk_id (EXTENDED_MODELS).  Without it resolve keeps to the yaml's model family
+    "extended_models": False,
 }
+
+# The reference options that need hparams['extended_models'] = True: the FastSpeech 2 mel decoder alone (decoder 'fft',
+# stylesinger.py:185-186) and speaker ids (use_spk_id, fs2.py:37-43).  egs/stylesinger.yaml selects neither; a
+# checkpoint trained with one says so in its own hparams, and the caller states that it means to run such a model.
+EXTENDED_MODELS = ("decoder: fft", "use_spk_id: True")
 
 # hparams['tc_precision'] -> SSB_TC_SPLIT / SSB_TC_FP16.  'split' (the default): fp32 operands as fp16 hi/lo planes, 3 MMAs
 # per K step, mel within 1e-3 of the fp32 reference.  'fp16': one MMA on operands rounded once to fp16 - a third of the
@@ -117,16 +125,33 @@ def _check_supported(hp):
     """The CUDA path implements exactly the configuration egs/stylesinger.yaml selects.
     Anything else fails loudly instead of silently computing something different."""
     prodiff = hp.get("decoder") == "prodiff"  # the ProDiff teacher of the commented block egs/stylesinger.yaml:145-155
+    # decoder 'fft': the FastSpeech 2 decoder's mel is the output (stylesinger.py:185-186); no diffusion hparam is read
+    fft = hp.get("decoder") == "fft"
+    # use_spk_id: spk_embed_proj is an Embedding(num_spk + 1, 256) over speaker ids (fs2.py:37-43), whatever use_spk_embed
+    spk_id = hp.get("use_spk_id") is True
     # f0_gen 'conv': two FastSpeech-2 PitchPredictors instead of the two F0 diffusion samplers (stylesinger.py:66-82);
     # f0_timesteps / f0_max_beta are then unread
     conv_f0 = hp.get("f0_gen") == "conv"
     req = {"encoder_type": "fft", "decoder_type": "fft", "ffn_act": "gelu", "ffn_padding": "SAME",
            "dur_loss": "mse", "pitch_type": "frame", "f0_gen": "conv" if conv_f0 else "gmdiff",
-           "decoder": "prodiff" if prodiff else "diffsinger",
-           "diff_decoder_type": "wavenet", "schedule_type": "vpsde" if prodiff else "linear", "pitch_norm": "log",
-           "use_uv": True, "use_spk_embed": True,
-           "use_spk_id": False, "use_pitch_embed": True, "use_energy_embed": False,
+           "decoder": "prodiff" if prodiff else "fft" if fft else "diffsinger",
+           "diff_decoder_type": "wavenet", "pitch_norm": "log", "use_uv": True,
+           "use_spk_id": True if spk_id else False, "use_pitch_embed": True, "use_energy_embed": False,
            "use_pos_embed": True, "num_heads": 2, "hidden_size": 256}
+    if not fft:  # the schedule belongs to the mel sampler, which an FFT model does not have
+        req["schedule_type"] = "vpsde" if prodiff else "linear"
+    if not spk_id:  # with neither option the reference builds no spk_embed_proj, yet its forward calls it
+        req["use_spk_embed"] = True
+    if (fft or spk_id) and hp.get("extended_models") is not True:
+        raise NotImplementedError(
+            f"stylesinger_b200: {' and '.join(o for o, on in zip(EXTENDED_MODELS, (fft, spk_id)) if on)} is outside the "
+            f"egs/stylesinger.yaml model family; set hparams['extended_models'] = True to run such a checkpoint")
+    if not isinstance(hp.get("extended_models"), bool):
+        raise NotImplementedError(f"stylesinger_b200: hparams['extended_models'] must be True or False, got "
+                                  f"{hp.get('extended_models')!r}")
+    if not spk_id and hp.get("use_spk_embed") is False:
+        raise NotImplementedError("stylesinger_b200: use_spk_id and use_spk_embed are both False - the reference then builds "
+                                  "no spk_embed_proj (fs2.py:37-43), which StyleSinger.forward calls")
     for k, v in req.items():
         if hp.get(k) != v:
             raise NotImplementedError(
@@ -140,8 +165,8 @@ def _check_supported(hp):
         raise NotImplementedError("rel_pos is not selected by egs/stylesinger.yaml")
     if hp.get("tc_precision") not in TC_PRECISIONS:
         raise ValueError(f"tc_precision must be one of {sorted(TC_PRECISIONS)}, got {hp.get('tc_precision')!r}")
-    if prodiff:  # ProDiffusion.forward(infer=True) never reads K_step or pndm_speedup (prodiff.py:204-222)
-        return
+    if prodiff or fft:  # ProDiffusion.forward(infer=True) never reads K_step or pndm_speedup (prodiff.py:204-222), and an
+        return          # FFT model has no diffusion at all
     # shallow diffusion (DiffusionDecoder.forward, shallow_diffusion_tts.py:297-304): q_sample at K_step - 1 of the
     # timesteps-long schedule, then K_step reverse steps; beyond timesteps the reference indexes past its buffers
     K = int(hp["K_step"])

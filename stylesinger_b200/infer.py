@@ -106,7 +106,10 @@ class StyleSingerInfer:
         ref_audio = inp["ref_audio"]
         wav, mel = self.process_audio(ref_audio)
         inp["mel"] = mel
-        if spk_embed_fn is not None:
+        if hp.get("use_spk_id"):  # the speaker is an id of the training set, not an embedding of the reference audio
+            if "spk_id" not in inp:
+                raise ValueError("inp['spk_id'] required: the model was trained with use_spk_id")
+        elif spk_embed_fn is not None:
             inp["spk_embed"] = spk_embed_fn(wav)
         elif "spk_embed" not in inp:
             raise ValueError("spk_embed_fn or inp['spk_embed'] required (resemblyzer VoiceEncoder is third-party)")
@@ -129,11 +132,15 @@ class StyleSingerInfer:
         (0 = unvoiced), exactly what ``preprocess_input`` produces: like the reference (:152) it goes through
         ``norm_interp_f0`` (log2 Hz, unvoiced frames interpolated) before it becomes the style extractor's ``ref_f0``.
         A model without emo reads no ``emo_embed`` (forward_model passes None, :44-47), one without style no ``mel`` /
-        ``f0`` (get_style is skipped, stylesinger.py:149-151): the item may then leave them out."""
+        ``f0`` (get_style is skipped, stylesinger.py:149-151): the item may then leave them out.  A use_spk_id model reads
+        the integer ``item['spk_id']`` instead of ``spk_embed``."""
         hp = self.hparams
         u = {"txt_tokens": torch.as_tensor(item["ph_token"]).long(), "note": torch.as_tensor(item["note"]).long(),
-             "note_dur": torch.as_tensor(item["note_dur"]).float(), "note_type": torch.as_tensor(item["note_type"]).long(),
-             "spk_embed": torch.as_tensor(item["spk_embed"]).float()}
+             "note_dur": torch.as_tensor(item["note_dur"]).float(), "note_type": torch.as_tensor(item["note_type"]).long()}
+        if hp.get("use_spk_id"):  # the line the reference leaves commented out (inference/StyleSinger.py:146,159)
+            u["spk_id"] = int(item["spk_id"])
+        else:
+            u["spk_embed"] = torch.as_tensor(item["spk_embed"]).float()
         if hp["emo"]:
             u["emo_embed"] = torch.as_tensor(item["emo_embed"]).float()
         if hp["style"]:
@@ -143,7 +150,8 @@ class StyleSingerInfer:
             u["ref_f0"] = torch.from_numpy(f0)
         if item.get("mel2ph") is not None:
             u["mel2ph"] = torch.as_tensor(item["mel2ph"]).long()
-        return pack_batch([u], use_mel2ph="mel2ph" in u, emo=hp["emo"], style=hp["style"])
+        return pack_batch([u], use_mel2ph="mel2ph" in u, emo=hp["emo"], style=hp["style"],
+                          spk_id=bool(hp.get("use_spk_id")))
 
     def forward_model(self, inp, seed=0, noise=None, voc_noise=None, return_mel=False):
         """reference inference/StyleSinger.py:41-64: returns the waveform (np.float32 [T*hop]).

@@ -5,12 +5,14 @@
 tasks/StyleSinger/stylesinger.py:122-123,190-195).  ``HifiGAN`` mirrors the registered vocoder class
 (tasks/tts/vocoder_infer/hifigan_nsf.py:46-75: ``spec2wav(mel np[T,80], f0=np[T]) -> np[T*hop]``).
 
-Both mel decoders of ``hparams['decoder']`` are implemented: 'diffsinger' (the default) and 'prodiff', the ProDiff
-teacher (stylesinger.py:111-117,176-177), whose sampler always runs, whatever ``global_steps`` is.  Both F0 generators
-of ``hparams['f0_gen']`` are implemented: 'gmdiff' (the default) and 'conv' (stylesinger.py:73-82; ``PitchPredictor``).
-Only what the ph -> mel -> wav inference path uses is implemented; everything else raises instead of silently
-doing something different (training mode, teacher-forced f0/uv, the `forcing` aligner branch of early training
-steps, the fft decoder).
+The three mel decoders of ``hparams['decoder']`` are implemented: 'diffsinger' (the default), 'prodiff', the ProDiff
+teacher (stylesinger.py:111-117,176-177), whose sampler always runs, whatever ``global_steps`` is, and 'fft', the
+FastSpeech 2 decoder alone (:185-186), whose mel is the output at any ``global_steps``.  Both F0 generators of
+``hparams['f0_gen']`` are implemented: 'gmdiff' (the default) and 'conv' (stylesinger.py:73-82; ``PitchPredictor``).
+With ``hparams['use_spk_id']`` the ``spk_embed`` argument is a LongTensor [B] of speaker ids, as the reference's forward
+receives it (fs2.py:37-38).  'fft' and use_spk_id need ``hparams['extended_models'] = True``.  Only what the ph -> mel -> wav inference path uses is implemented; everything else raises
+instead of silently doing something different (training mode, teacher-forced f0/uv, the `forcing` aligner branch of
+early training steps).
 """
 from typing import Dict, List, Optional
 
@@ -22,13 +24,14 @@ from .hparams import resolve
 
 
 def padded_to_utterances(txt_tokens, note, note_dur, note_type, spk_embed, emo_embed, ref_mels, ref_f0,
-                         mel2ph=None) -> List[Dict[str, torch.Tensor]]:
+                         mel2ph=None, spk_id=False) -> List[Dict[str, torch.Tensor]]:
     """Split the reference's zero-padded batch tensors into per-utterance true-length CPU tensors.
 
     Padding conventions of the reference collater (tasks/StyleSinger/dataset.py): token id 0 pads ``txt_tokens``
     (and the note tensors alongside), all-zero frames pad ``ref_mels`` (the reference derives its own mask from
     ``ref_mels[:, :, 0] != 0``, lse.py:104, and so does the kernel), 0 pads ``mel2ph``.
     ``emo_embed`` None (a model without emo) or ``ref_mels`` None (without style) leaves those fields out.
+    ``spk_id``: ``spk_embed`` holds one integer speaker id per batch row (use_spk_id), stored as ``u["spk_id"]``.
     """
     txt_tokens = torch.as_tensor(txt_tokens).cpu()
     B = txt_tokens.shape[0]
@@ -45,8 +48,11 @@ def padded_to_utterances(txt_tokens, note, note_dur, note_type, spk_embed, emo_e
             raise ValueError(f"utterance {b}: empty phone sequence")
         u = {"txt_tokens": txt_tokens[b, :P].long(), "note": torch.as_tensor(note)[b, :P].long().cpu(),
              "note_dur": torch.as_tensor(note_dur)[b, :P].float().cpu(),
-             "note_type": torch.as_tensor(note_type)[b, :P].long().cpu(),
-             "spk_embed": torch.as_tensor(spk_embed)[b].float().reshape(-1).cpu()}
+             "note_type": torch.as_tensor(note_type)[b, :P].long().cpu()}
+        if spk_id:
+            u["spk_id"] = int(torch.as_tensor(spk_embed).reshape(B)[b])
+        else:
+            u["spk_embed"] = torch.as_tensor(spk_embed)[b].float().reshape(-1).cpu()
         if emo_embed is not None:
             u["emo_embed"] = torch.as_tensor(emo_embed)[b].float().reshape(-1).cpu()
         if ref_mels is not None:
@@ -147,9 +153,10 @@ class StyleSinger:
                                  f"style={hp['style']})")
         # a switched-off module's input is not read, whatever the caller passes (the reference ignores it too)
         utts = padded_to_utterances(txt_tokens, note, note_dur, note_type, spk_embed, emo_embed if hp["emo"] else None,
-                                    ref_mels if hp["style"] else None, ref_f0 if hp["style"] else None, mel2ph)
-        pb: PackedBatch = pack_batch(utts, use_mel2ph=mel2ph is not None, emo=hp["emo"],
-                                     style=hp["style"]).to(self.engine.device)
+                                    ref_mels if hp["style"] else None, ref_f0 if hp["style"] else None, mel2ph,
+                                    spk_id=hp["use_spk_id"])
+        pb: PackedBatch = pack_batch(utts, use_mel2ph=mel2ph is not None, emo=hp["emo"], style=hp["style"],
+                                     spk_id=hp["use_spk_id"]).to(self.engine.device)
         ret = {}
         dur = None
         if pb.frame_offsets is None:  # FastSpeech2.add_dur at inference (fs2.py:151-174): predicted durations
@@ -160,9 +167,10 @@ class StyleSinger:
             pb.frame_offsets = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
             ret["dur"] = packed_to_padded(dur, po)
         # the reference runs the shallow-diffusion refinement only once training passed diff_start (stylesinger.py:181);
-        # the ProDiff branch has no such gate and no coarse mel (:176-177)
-        prodiff = hp["decoder"] == "prodiff"
-        run_diff = (not skip_decoder) and (prodiff or global_steps > hp.get("diff_start", 0))
+        # the ProDiff branch has no such gate and no coarse mel (:176-177), and the FFT decoder's mel is always the output
+        # (:185-186)
+        ungated = hp["decoder"] in ("prodiff", "fft")
+        run_diff = (not skip_decoder) and (ungated or global_steps > hp.get("diff_start", 0))
         want = ["f0_denorm", "mel2ph", "decoder_inp", "pitch_pred", "spk_proj"]
         want += ["emo_proj"] if hp["emo"] else []
         want += ["style"] if hp["style"] else []

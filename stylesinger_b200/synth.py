@@ -84,8 +84,14 @@ def acoustic_param_shapes(hp):
     for i in range(hp["dec_layers"]):
         out += _enc_sa_layer(f"decoder.layers.{i}.op.", H, hp["dec_ffn_kernel_size"])
     out += [("decoder.layer_norm.weight", (H,)), ("decoder.layer_norm.bias", (H,)),
-            ("mel_out.weight", (80, H)), ("mel_out.bias", (80,)),
-            ("spk_embed_proj.weight", (H, 256)), ("spk_embed_proj.bias", (H,))]
+            ("mel_out.weight", (80, H)), ("mel_out.bias", (80,))]
+    if hp["use_spk_id"]:  # Embedding(num_spk + 1, H) tables, no bias (fs2.py:37-41)
+        rows = hp["num_spk"] + 1
+        out += [("spk_embed_proj.weight", (rows, H))]
+        if hp.get("use_split_spk_id"):
+            out += [("spk_embed_f0.weight", (rows, H)), ("spk_embed_dur.weight", (rows, H))]
+    else:
+        out += [("spk_embed_proj.weight", (H, 256)), ("spk_embed_proj.bias", (H,))]
     out += _predictor("dur_predictor.", H, hp["dur_predictor_layers"], hp["dur_predictor_kernel"], 1)
     out += [("pitch_embed.weight", (300, H)), ("pitch_predictor.pos_embed_alpha", (1,))]
     # constructed by FastSpeech2 (unused with gmdiff); f0_gen 'conv' rebuilds it in place with the same shapes
@@ -112,6 +118,8 @@ def acoustic_param_shapes(hp):
         out += [(f"{gen}.{b}", (Tf,)) for b in _GAUSS_BUFS]
         out += _diffnet(gen + "._denoise_fn.", Cf, Lf, 1, 3, H, True)
     T = hp["timesteps"]
+    if hp["decoder"] == "fft":  # stylesinger.py:92-117: neither ln_proj / postdiff nor diff_decoder
+        return out + [("embed_positions._float_tensor", (1,))]
     if hp["decoder"] == "prodiff":  # ProDiffusion (stylesinger.py:111-117, prodiff.py:59-117): buffers of length T+1
         out += [("embed_positions._float_tensor", (1,)), ("diff_decoder.timesteps", ()), ("diff_decoder.timescale", ())]
         out += [(f"diff_decoder.{b}", (T + 1,)) for b in _GAUSS_BUFS]

@@ -1,6 +1,6 @@
 """F0-generator timing: the two 100-step F0 diffusion samplers (f0_gen 'gmdiff') against the two PitchPredictors
-(f0_gen 'conv') on the same utterances, and the acoustic forward without the vocoder for {diffsinger, prodiff} x
-{gmdiff, conv}, all arms alternated in one process.
+(f0_gen 'conv') on the same utterances, the acoustic forward without the vocoder for {diffsinger, prodiff, fft} x
+{gmdiff, conv}, and the HiFi-GAN vocoder on the fft + conv model's mel, all arms alternated in one process.
 
     python tools/bench_f0gen.py [--workloads utt10s,batch64] [--reps 3] [--out FILE]
 
@@ -10,7 +10,10 @@ card's name, power limit and max SM clock.
   on the same two conditions (decoder_inp of the workload stands in for both; the timings depend on shapes only), the
   samplers with the widest clip band.  Inside the acoustic forward the two samplers overlap on two streams, so the
   forward's own F0 cost is somewhat lower than the pitch-stage number.
-- acoustic forward: ssb_acoustic_forward without the vocoder, Philox noise, DiffSinger T = 100 / ProDiff T = 8, F0 T = 100.
+- acoustic forward: ssb_acoustic_forward without the vocoder, Philox noise, DiffSinger T = 100 / ProDiff T = 8, F0 T = 100;
+  the FFT decoder (decoder 'fft') has no mel sampler.
+- vocoder: Vocoder.generate (HiFi-GAN V1 layout with NSF, Philox) on the mel and f0 of the fft + conv forward, so that
+  fft + conv's whole ph -> wav cost is the forward plus this arm.
 Synthetic weights (synth.py).  Writes nothing except --out.
 """
 import argparse
@@ -27,8 +30,8 @@ import torch  # noqa: E402
 
 from bench import make_workload  # noqa: E402
 from stylesinger_b200 import synth  # noqa: E402
-from stylesinger_b200.engine import AcousticModel, pack_batch  # noqa: E402
-from stylesinger_b200.hparams import resolve  # noqa: E402
+from stylesinger_b200.engine import AcousticModel, Vocoder, pack_batch  # noqa: E402
+from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG, resolve  # noqa: E402
 
 T_DS, T_PD, T_F0 = 100, 8, 100
 
@@ -57,6 +60,8 @@ def hparams(decoder, f0_gen):
     kw = dict(f0_timesteps=T_F0, f0_gen=f0_gen)
     if decoder == "prodiff":
         return resolve(timesteps=T_PD, decoder="prodiff", schedule_type="vpsde", timescale=1, **kw)
+    if decoder == "fft":
+        return resolve(decoder="fft", extended_models=True, **kw)
     return resolve(timesteps=T_DS, K_step=T_DS, **kw)
 
 
@@ -70,11 +75,13 @@ def main():
         raise SystemExit("bench_f0gen needs a CUDA device")
     dev = torch.device("cuda:0")
     models = {}
-    for dec in ("diffsinger", "prodiff"):
+    decoders = ("diffsinger", "prodiff", "fft")
+    for dec in decoders:
         for f0g in ("gmdiff", "conv"):
             hp = hparams(dec, f0g)
             models[f"{dec}+{f0g}"] = AcousticModel(synth.acoustic_state_dict(hp, seed=0), hp, dev)
     gm, cv = models["diffsinger+gmdiff"], models["diffsinger+conv"]
+    voc = Vocoder(synth.vocoder_state_dict(DEFAULT_VOCODER_CONFIG, seed=0), DEFAULT_VOCODER_CONFIG, dev)
     info = card()
     lines = []
     for wl in args.workloads.split(","):
@@ -87,7 +94,10 @@ def main():
         pitch = {"gmdiff_2x100_steps": lambda: [gm.f0_diffusion(w, cond, lo, hi, fo, seed=2) for w in (0, 1)],
                  "conv_2_predictors": lambda: [cv.pitch_predictor(w, cond, fo) for w in (0, 1)]}
         fwd = {k: (lambda m=m: m.forward(pb, seed=3)["mel_out"]) for k, m in models.items()}
-        arms = dict(pitch, **fwd)
+        o = models["fft+conv"].forward(pb, seed=3, want=("mel_out", "f0_denorm"))
+        mel, f0 = o["mel_out"], o["f0_denorm"]
+        vocoder = {"vocoder_on_fft+conv_mel": lambda: voc.generate(mel, f0, fo, seed=4)}
+        arms = dict(pitch, **fwd, **vocoder)
         ms = {k: [] for k in arms}
         for k in arms:  # warm-up of every shape
             arms[k]()
@@ -96,7 +106,7 @@ def main():
             for k in arms:  # alternated
                 t, r = timed(arms[k])
                 ms[k].append(t)
-                if k in fwd:
+                if k in fwd or k in vocoder:
                     finite[k] = bool(torch.isfinite(r).all())
         med = {k: float(np.median(v)) for k, v in ms.items()}
         res = {"workload": wl, "desc": desc, "frames": Fs, "card": info, "reps": args.reps,
@@ -104,7 +114,8 @@ def main():
                "pitch_stage_speedup": round(med["gmdiff_2x100_steps"] / med["conv_2_predictors"], 1),
                "acoustic_forward_ms": {k: round(med[k], 2) for k in fwd},
                "acoustic_forward_speedup_conv_vs_gmdiff": {
-                   d: round(med[f"{d}+gmdiff"] / med[f"{d}+conv"], 2) for d in ("diffsinger", "prodiff")},
+                   d: round(med[f"{d}+gmdiff"] / med[f"{d}+conv"], 2) for d in decoders},
+               "vocoder_ms": {k: round(med[k], 2) for k in vocoder},
                "ms_all": {k: [round(x, 3) for x in v] for k, v in ms.items()},
                "outputs_finite": finite}
         line = json.dumps(res)

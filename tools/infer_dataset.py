@@ -51,6 +51,11 @@ def main():
     for sw in ("emo", "style", "umln", "use_txt_cond"):  # the checkpoint's model switches (egs/stylesinger.yaml)
         ap.add_argument(f"--{sw.replace('_', '-')}", type=int, choices=(0, 1), default=1,
                         help=f"reference hparam {sw} of the checkpoint (default 1)")
+    ap.add_argument("--decoder", choices=("diffsinger", "fft"), default="diffsinger",
+                    help="reference hparam decoder of the checkpoint: 'fft' is the FastSpeech 2 decoder alone (no diffusion)")
+    ap.add_argument("--use-spk-id", type=int, choices=(0, 1), default=0,
+                    help="reference hparam use_spk_id: the checkpoint looks speakers up by the items' spk_id")
+    ap.add_argument("--num-spk", type=int, default=150, help="reference hparam num_spk (the speaker table has num_spk + 1 rows)")
     args = ap.parse_args()
 
     from scipy.io import wavfile
@@ -60,7 +65,9 @@ def main():
 
     hp = resolve(timesteps=args.T, K_step=args.T if args.k_step is None else args.k_step, f0_timesteps=args.T,
                  vocoder_denoise_c=args.vocoder_denoise_c, emo=bool(args.emo), style=bool(args.style),
-                 umln=bool(args.umln), use_txt_cond=bool(args.use_txt_cond), tc_precision=args.tc_precision)
+                 umln=bool(args.umln), use_txt_cond=bool(args.use_txt_cond), tc_precision=args.tc_precision,
+                 decoder=args.decoder, use_spk_id=bool(args.use_spk_id), num_spk=args.num_spk,
+                 extended_models=args.decoder == "fft" or bool(args.use_spk_id))
     sd, path = formats.load_state_dict(args.ckpt, "model")
     vsd, vcfg, vpath = formats.load_vocoder_checkpoint(args.vocoder)
     print(f"| acoustic checkpoint {path} ({len(sd)} tensors); vocoder {vpath}")

@@ -559,6 +559,81 @@ def case_switches(name, T=4, frames=32, phones=4, ref_frames=32, seed=151, utt_i
     print("wrote", name, len(d), "arrays")
 
 
+# decoder 'fft' and use_spk_id (stylesinger.py:185-186, fs2.py:37-43): name -> hparams overrides
+FFT_SPKID_CONFIGS = {
+    "fft_gmdiff": {"decoder": "fft"},
+    "fft_conv": dict(CONVF0_OVERRIDES, decoder="fft"),
+    "spkid_diffsinger": {"use_spk_id": True},
+    "spkid_fft": {"decoder": "fft", "use_spk_id": True},
+    "fft_no_emo_style": {"decoder": "fft", "emo": False, "style": False},
+}
+FFT_SPKID_DUR_CONFIG = "spkid_fft"  # the configuration that also stores a forward with predicted durations
+FFT_SPKID_SPEAKER = 37  # the speaker id the use_spk_id configurations look up (num_spk = 150: rows 0 .. 150)
+
+
+def case_fft_spkid(name, T=4, frames=32, phones=4, ref_frames=32, seed=161, utt_idx=108):
+    """The reference's StyleSinger with the FastSpeech 2 mel decoder (decoder 'fft') and with speaker ids (use_spk_id), in
+    the layout of ref_switches.npz: per configuration the state dict's key list (strict=True load) and a B = 1 full
+    forward at T = f0_T = 4 with injected noise, mel2ph given; c/coarse_mel for the DiffSinger configuration (a run below
+    diff_start).  A use_spk_id model gets spk_embed = LongTensor([FFT_SPKID_SPEAKER]), as the reference's forward receives
+    it; the others the utterance's speaker vector.  FFT_SPKID_DUR_CONFIG also stores the forward with predicted durations."""
+    import ref_import
+    u = synth.make_utterance(frames / 187.5, utt_idx=utt_idx, ref_frames=ref_frames, frames=frames, phones=phones)
+    d, cfg_meta = {}, {}
+    for c, ov in FFT_SPKID_CONFIGS.items():
+        hp = ref_import.install(T=T, f0_T=T, overrides=ov)
+        import modules.diff.shallow_diffusion_tts as sdt
+        import modules.diff.gaussian_multinomial_diffusion as gmd
+        sdt.tqdm = gmd.tqdm = lambda it, **k: it
+        from modules.StyleSinger.stylesinger import StyleSinger
+        model = StyleSinger(_Dict()).eval()
+        # (extended_models: the opt-in stylesinger_b200 needs for these options; the reference has no such key)
+        model.load_state_dict(synth.acoustic_state_dict(dict(hp, extended_models=True), seed=0), strict=True)
+        spk = torch.tensor([FFT_SPKID_SPEAKER]) if hp["use_spk_id"] else u["spk_embed"][None]
+
+        def run(seed_, mel2ph=True, global_steps=320000):
+            ns = NoiseSource(seed_)
+            b = batchify(u)
+            cap, hooks = {}, []
+            if hp["style"]:
+                hooks.append(model.style_extractor.rqvae.register_forward_hook(
+                    lambda m, i, o: cap.__setitem__("rq_in", i[0].detach().clone())))
+            with torch.no_grad(), patched_rng(ns):
+                out = model(b["txt_tokens"], mel2ph=u["mel2ph"][None] if mel2ph else None, spk_embed=spk,
+                            emo_embed=b["emo_embed"] if hp["emo"] else None, ref_mels=b["ref_mels"].clone(),
+                            ref_f0=b["ref_f0"].clone(), global_steps=global_steps, infer=True, note=b["note"],
+                            note_dur=b["note_dur"], note_type=b["note_type"])
+                if hp["style"]:
+                    out["rq_codes"] = model.style_extractor.rqvae.quantize(cap["rq_in"])[1]
+            for h in hooks:
+                h.remove()
+            return out, ns.log
+
+        out, log = run(seed)
+        keys = ["mel_out", "f0_denorm", "pitch_pred", "decoder_inp", "spk_embed"]
+        keys += ["emo_embed"] if hp["emo"] else []
+        keys += ["style"] if hp["style"] else []
+        for k in keys:
+            d[f"{c}/{k}"] = np32(out[k][0])
+        if hp["style"]:
+            d[f"{c}/rq_codes"] = out["rq_codes"][0].numpy().astype(np.int64)
+        if hp["decoder"] == "diffsinger":
+            coarse, _ = run(seed, global_steps=50000)  # forcing < global_steps < diff_start: the coarse mel only
+            d[f"{c}/coarse_mel"] = np32(coarse["mel_out"][0])
+        cfg_meta[c] = {"overrides": ov, "noise_log": log,
+                       "state_dict": [[k, list(v.shape)] for k, v in model.state_dict().items()]}
+        if c == FFT_SPKID_DUR_CONFIG:
+            o2, log2 = run(seed + 1, mel2ph=False)
+            d.update({f"{c}/dur_mel2ph": o2["mel2ph"][0].numpy().astype(np.int64), f"{c}/dur_logdur": np32(o2["dur"][0]),
+                      f"{c}/dur_mel_out": np32(o2["mel_out"][0]), f"{c}/dur_f0_denorm": np32(o2["f0_denorm"][0])})
+            cfg_meta[c]["dur_noise_log"] = log2
+    d["meta"] = json.dumps({"T": T, "frames": frames, "phones": phones, "ref_frames": ref_frames, "seed": seed,
+                            "utt_idx": utt_idx, "dur_config": FFT_SPKID_DUR_CONFIG, "spk_id": FFT_SPKID_SPEAKER,
+                            "configs": cfg_meta})
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print("wrote", name, len(d), "arrays")
+
+
 def case_registry(name, T=4, seed=131):
     """The reference's per-registry modules that the C ABI replaces one by one (FS_ENCODERS['fft'], FS_DECODERS['fft'],
     StyleSinger.get_style): FastspeechEncoder.forward and FastspeechDecoder.forward on padded B = 3 batches and on each
@@ -652,7 +727,7 @@ if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     which = sys.argv[1:] or ["small", "t25", "t100", "padded", "plms", "prodiff", "convf0", "sched", "voc",
-                             "vocoder_edges", "emo", "registry", "kstep", "vocoder_layouts", "switches"]
+                             "vocoder_edges", "emo", "registry", "kstep", "vocoder_layouts", "switches", "fft_spkid"]
     if "small" in which:
         case_model("ref_small_T4", T=4, frames=96, phones=12, ref_frames=64, seed=11, utt_idx=100)
     if "t25" in which:
@@ -683,3 +758,5 @@ if __name__ == "__main__":
         case_kstep("ref_kstep")
     if "switches" in which:
         case_switches("ref_switches")
+    if "fft_spkid" in which:
+        case_fft_spkid("ref_fft_spkid")

@@ -48,6 +48,7 @@ struct Cfg {
 struct TCParams {
   const int2* tiles;
   int ntiles, NT, taps, kchunks, dil, center, N;
+  float wscale;  // ConvTC::wscale: the accumulator holds the contraction with W * 2^s; the epilogue multiplies it by 2^-s
   EpiTC e;
 };
 
@@ -141,8 +142,8 @@ __device__ __forceinline__ float act_slope_of(int act, float slope) {  // act(v)
   return act == ACT_RELU ? 0.0f : (act == ACT_LRELU ? slope : 1.0f);
 }
 template <int MODE>
-__device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb, int64_t r0, int nrows, int n, int lane,
-                                               const Pre& pre, int tq) {
+__device__ __forceinline__ void epilogue_chunk(const EpiTC& e, float ws, const float4* xb, int64_t r0, int nrows, int n,
+                                               int lane, const Pre& pre, int tq) {
   if (e.n_valid > 0 && n >= e.n_valid) return;  // warp-uniform
   const int q = lane & 7, rq = lane >> 3;  // step i: row rq + 4i, columns n4 .. n4 + 3
   const int n4 = n + 4 * q;
@@ -154,6 +155,7 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb,
     const float4 bv = __ldg(reinterpret_cast<const float4*>(e.bias + n4));
     b0 = bv.x; b1 = bv.y; b2 = bv.z; b3 = bv.w;
   }
+  // acc * ws + bias is one fmaf: ws is a power of two, so it costs no instruction over acc + bias and rounds once.
   // Everything below is computed for all 8 steps; only the STORES are predicated on the row being valid (i < nsteps).
   const int nsteps = nrows > rq ? (nrows - rq + 3) >> 2 : 0;
   if constexpr (MODE == EPI_GATE) {
@@ -164,7 +166,7 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb,
 #pragma unroll
     for (int i = 0; i < 8; ++i, ph += st, pl += st) {
       const float4 acc = xr[i * 32 + (qx ^ (4 * (i & 1)))];
-      float g0 = acc.x + b0, f0 = acc.y + b1, g1 = acc.z + b2, f1 = acc.w + b3;
+      float g0 = fmaf(acc.x, ws, b0), f0 = fmaf(acc.y, ws, b1), g1 = fmaf(acc.z, ws, b2), f1 = fmaf(acc.w, ws, b3);
       if (has_add) {
         const float4 ad = pre.a[i];
         g0 += ad.x; f0 += ad.y; g1 += ad.z; f1 += ad.w;
@@ -205,8 +207,8 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb,
           const float2 l01 = __half22float2(*reinterpret_cast<const __half2*>(&u2)), l23 = __half22float2(*reinterpret_cast<const __half2*>(&u3));
           x0 = make_float4((h01.x + l01.x) - c0, (h01.y + l01.y) - c1, (h23.x + l23.x) - c2, (h23.y + l23.y) - c3);
         }
-        const float v0 = (acc.x + b0 + x0.x) * beta, v1 = (acc.y + b1 + x0.y) * beta;
-        const float v2 = (acc.z + b2 + x0.z) * beta, v3 = (acc.w + b3 + x0.w) * beta;
+        const float v0 = (fmaf(acc.x, ws, b0) + x0.x) * beta, v1 = (fmaf(acc.y, ws, b1) + x0.y) * beta;
+        const float v2 = (fmaf(acc.z, ws, b2) + x0.z) * beta, v3 = (fmaf(acc.w, ws, b3) + x0.w) * beta;
         uint2 yh, yl;
         split_pack4(v0 + s0, v1 + s1, v2 + s2, v3 + s3, yh, yl);
         const bool ok = i < nsteps;
@@ -229,7 +231,7 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb,
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const float4 acc = xr[i * 32 + (qx ^ (4 * (i & 1)))];
-        float v0 = acc.x + b0, v1 = acc.y + b1, v2 = acc.z + b2, v3 = acc.w + b3;
+        float v0 = fmaf(acc.x, ws, b0), v1 = fmaf(acc.y, ws, b1), v2 = fmaf(acc.z, ws, b2), v3 = fmaf(acc.w, ws, b3);
         if (!init) {
           const float4 o = pre.a[i];
           v0 += o.x; v1 += o.y; v2 += o.z; v3 += o.w;
@@ -280,7 +282,8 @@ __device__ __forceinline__ void epilogue_chunk(const EpiTC& e, const float4* xb,
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const float4 acc = xr[i * 32 + (qx ^ (4 * (i & 1)))];
-      float v0 = (acc.x + b0) * alpha, v1 = (acc.y + b1) * alpha, v2 = (acc.z + b2) * alpha, v3 = (acc.w + b3) * alpha;
+      float v0 = fmaf(acc.x, ws, b0) * alpha, v1 = fmaf(acc.y, ws, b1) * alpha, v2 = fmaf(acc.z, ws, b2) * alpha,
+            v3 = fmaf(acc.w, ws, b3) * alpha;
       if (gelu) {
         v0 = gelu_erf(v0); v1 = gelu_erf(v1); v2 = gelu_erf(v2); v3 = gelu_erf(v3);
       } else {
@@ -530,7 +533,8 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         const int ch = 2 * cp + eg;
         if (ch + 2 < NCH && nrows > 0) prefetch_chunk<MODE>(p.e, r0, nrows, n0 + (ch + 2) * 32, lane, nxt, tq);
         if (nrows > 0)
-          epilogue_chunk<MODE>(p.e, reinterpret_cast<float4*>(xb_pair + eg * 1024), r0, nrows, n0 + ch * 32, lane, cur, tq);
+          epilogue_chunk<MODE>(p.e, p.wscale, reinterpret_cast<float4*>(xb_pair + eg * 1024), r0, nrows, n0 + ch * 32, lane, cur,
+                              tq);
         cur = nxt;
         named_sync(pair_bar, 64);  // both chunks consumed before the buffers are refilled
       }
@@ -829,7 +833,7 @@ int conv_gemm_tc(Ctx& ctx, const GemmTC& p) {
   const int num_sms = device_sms();
   TCParams tp;
   tp.tiles = p.tiles; tp.ntiles = p.ntiles; tp.taps = w.taps; tp.kchunks = w.Cin / BK;
-  tp.dil = w.dil; tp.center = w.center; tp.N = w.N; tp.e = p.e;
+  tp.dil = w.dil; tp.center = w.center; tp.N = w.N; tp.wscale = w.wscale; tp.e = p.e;
   if (!tp.e.bias) tp.e.bias = w.bias;
   return p.single_pass ? dispatch<1>(ctx, p, tp, num_sms) : dispatch<3>(ctx, p, tp, num_sms);
 }

@@ -1,9 +1,16 @@
 // wgmma / TMA implicit-GEMM conv1d for the dense contractions of the denoisers (SURVEY.md §8 a13/a18).
 //
 // Precision: every fp32 operand is carried as TWO fp16 planes (hi = fp16(x), lo = fp16(x - hi));
-// each K step issues three wgmma (hi*hi + hi*lo + lo*hi) into one fp32 register accumulator, so the
-// contraction keeps ~22 mantissa bits (SURVEY.md §7: single-pass bf16/fp16/TF32 cannot meet the
-// mel L-inf < 1e-3 bar at T=100; a 3-pass split can).  Effective tensor peak = 1/3 of the fp16 peak.
+// each K step issues three wgmma (hi*hi + hi*lo + lo*hi) into one fp32 register accumulator (SURVEY.md §7: single-pass
+// bf16/fp16/TF32 cannot meet the mel L-inf < 1e-3 bar at T=100; a 3-pass split can).  Effective tensor peak = 1/3 of the
+// fp16 peak.  The split is exact to about 2^-22 of x only while lo is a normal fp16 number, |x| >= 2^-3, and exists only
+// for |x| < 65520 (hi = inf above).  So:
+//  * weights: the packer splits w * 2^s with one power of two per tensor, s = 14 - ceil(log2 max|w|) (ConvTC::wscale =
+//    2^-s, applied in the epilogue as fmaf(acc, wscale, bias)): about 22 bits at any weight magnitude, for every weight
+//    above max|w| * 2^-16;
+//  * activations: relative 2^-22 for |a| >= 2^-3, below that an absolute error floor of 2^-25 per element (lo is
+//    subnormal), and defined only for |a| < 65520;
+//  * single_pass: 2^-12 relative (one fp16 rounding) on the weights at any magnitude, the same activation range.
 //
 // Layout: A = activation planes [rows, C] fp16 row-major (guard-banded rows, see common.cuh), loaded by
 // TMA as [128 rows x 64 ch] boxes with 128B swizzle at row offset (tap - center) * dilation;
@@ -32,6 +39,7 @@ struct ConvTC {            // packed weights for the tensor-core path
   int hb = 0;                       // CTA-pair kernel: weight rows each CTA of a pair loads (half of a 2*hb-wide N tile)
   int taps = 1, Cin = 0, N = 0, dil = 1, center = 0;
   const float* bias = nullptr;  // [N] (packed column order)
+  float wscale = 1.0f;          // the planes hold W * 2^s; wscale = 2^-s multiplies the accumulator (pack_conv_tc)
   bool ok = false;
 };
 

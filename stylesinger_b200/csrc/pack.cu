@@ -113,17 +113,31 @@ int pack_conv(DevicePool& pool, const HostTensor* w, const HostTensor* b, int di
   return pack_conv_impl(pool, w, b, dil, mode, out, g, true);
 }
 
-// Tensor-core packing: W[tap][n'][c] as fp16 hi/lo planes (n' = permuted output column), + TMA maps.
+// Power-of-two exponent s for the planes of W * 2^s: s = 14 - ceil(log2 max|w|), so that max|W * 2^s| <= 2^14 and the lo
+// plane of every weight above max|w| * 2^-16 is a normal fp16 number (conv_gemm_tc.cuh, "Precision").  0 for an all-zero
+// (or non-finite) tensor; clamped so that 2^-s stays a normal fp32 number.
+static int plane_exponent(const float* w, size_t n) {
+  float mx = 0.f;
+  for (size_t i = 0; i < n; ++i) mx = fmaxf(mx, fabsf(w[i]));
+  if (!(mx > 0.f) || mx == HUGE_VALF) return 0;  // (fmaxf drops NaNs)
+  int e = 0;
+  const float m = frexpf(mx, &e);  // mx = m * 2^e, m in [0.5, 1): ceil(log2 mx) = e, or e - 1 when mx is a power of two
+  const int s = 14 - (m == 0.5f ? e - 1 : e);
+  return s < -126 ? -126 : (s > 126 ? 126 : s);
+}
+
+// Tensor-core packing: W[tap][n'][c] * 2^s as fp16 hi/lo planes (n' = permuted output column), wscale = 2^-s, + TMA maps.
 int pack_conv_tc(DevicePool& pool, const HostTensor* w, int dil, PackMode mode, const float* packed_bias, ConvTC* out) {
   if (!w) return -1;
   const int N = (int)w->shape[0], Cin = (int)w->shape[1], k = w->shape.size() == 3 ? (int)w->shape[2] : 1;
   if (Cin % 64 != 0 || N % 64 != 0 || !tc_available()) return 0;  // not eligible: out->ok stays false
+  const int s = plane_exponent(w->data, (size_t)k * N * Cin);
   std::vector<__half> hi((size_t)k * N * Cin), lo((size_t)k * N * Cin);
   for (int n = 0; n < N; ++n) {
     const int pn = perm_col(n, N, mode);
     for (int c = 0; c < Cin; ++c)
       for (int j = 0; j < k; ++j) {
-        const float v = w->data[((size_t)n * Cin + c) * k + j];
+        const float v = ldexpf(w->data[((size_t)n * Cin + c) * k + j], s);  // exact: a power-of-two scale
         const __half h = __float2half_rn(v);
         const size_t o = ((size_t)j * N + pn) * Cin + c;
         hi[o] = h;
@@ -139,6 +153,7 @@ int pack_conv_tc(DevicePool& pool, const HostTensor* w, int dil, PackMode mode, 
   SSB_CUDA(cudaMemcpy(dl, lo.data(), lo.size() * sizeof(__half), cudaMemcpyHostToDevice));
   out->W_hi = (__half*)dh; out->W_lo = (__half*)dl;
   out->taps = k; out->Cin = Cin; out->N = N; out->dil = dil; out->center = (k - 1) / 2; out->bias = packed_bias;
+  out->wscale = ldexpf(1.0f, -s);
   return make_weight_maps(out);
 }
 

@@ -98,7 +98,7 @@ __device__ __forceinline__ void epilogue32(const SPhase& e, int64_t r, int64_t t
                                            const uint32_t (&raw)[32], const Pre& pre) {
   float v[32];
 #pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]) + __ldg(e.bias + n + j);
+  for (int j = 0; j < 32; ++j) v[j] = fmaf(__uint_as_float(raw[j]), e.wscale, __ldg(e.bias + n + j));
   if (e.mode == SP_GATE) {
 #pragma unroll
     for (int q = 0; q < 8; ++q) {

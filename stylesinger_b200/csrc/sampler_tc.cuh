@@ -15,6 +15,7 @@ struct SPhase {
   int taps, kchunks, dil, center, N, NT;
   int mode;
   const float* bias;   // [N]
+  float wscale;        // ConvTC::wscale of the weights w1: the epilogue takes acc * wscale + bias
   float* out;          // fp32 output (x, or the sampler state x_t [rows,80])
   int ldo;
   __half* oh;          // fp16 hi/lo planes output

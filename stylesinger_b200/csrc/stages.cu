@@ -730,12 +730,12 @@ static void persistent_net_step(const PersistentNet& p, const SeqDev& s, int t, 
     SPhase a = sphase(sync_after);  // dilated conv (3 taps of y) + hoisted conditioner projection -> gate -> z planes
     a.a1 = p.mb + P::Y; a.w1 = p.w_layer(l); a.taps = 3; a.kchunks = C / 64;
     a.dil = d.layers[l].dil.t.dil; a.center = 1; a.N = 2 * C; a.NT = 2 * C / 64; a.mode = SP_GATE;
-    a.bias = d.layers[l].bias_gate_tc; a.oh = p.pl[P::Z]; a.ol = p.pl[P::Z + 1]; a.ldh = C;
+    a.bias = d.layers[l].bias_gate_tc; a.wscale = d.layers[l].dil.t.wscale; a.oh = p.pl[P::Z]; a.ol = p.pl[P::Z + 1]; a.ldh = C;
     a.add = p.condpre + (size_t)l * (size_t)s.rows * 2 * C; a.ld_add = 2 * C;
     ph.push_back(a);
     SPhase b = sphase(sync_after);  // 1x1 output projection -> residual stream, next layer's input planes, skip sum
     b.a1 = p.mb + P::Z; b.w1 = p.w_layer(l) + 2; b.kchunks = C / 64; b.N = 2 * C; b.NT = 2 * C / 64; b.mode = SP_RES_SKIP;
-    b.bias = d.layers[l].outp.f.bias; b.res = p.x; b.ld_res = C; b.out = p.x; b.ldo = C; b.beta = 0.70710678118654752440f;
+    b.bias = d.layers[l].outp.f.bias; b.wscale = d.layers[l].outp.t.wscale; b.res = p.x; b.ld_res = C; b.out = p.x; b.ldo = C; b.beta = 0.70710678118654752440f;
     if (l + 1 < L) { b.oh = p.pl[P::Y]; b.ol = p.pl[P::Y + 1]; b.ldh = C; b.vec2 = dt + (size_t)(l + 1) * C; }
     b.skip = p.skip; b.ld_skip = C; b.C = C; b.skip_init = (l == 0);
     if (l == L - 1) { b.sh = p.pl[P::SKIP]; b.sl = p.pl[P::SKIP + 1]; }
@@ -743,7 +743,7 @@ static void persistent_net_step(const PersistentNet& p, const SeqDev& s, int t, 
   }
   SPhase q = sphase(sync_after);  // skip_projection (1/sqrt(L) folded into the weights, N padded) + ReLU -> s planes
   q.a1 = p.mb + P::SKIP; q.w1 = p.w_skip(); q.kchunks = C / 64; q.N = d.skip_tc.N; q.NT = d.skip_tc.N / 64;
-  q.mode = SP_SKIPPROJ; q.bias = d.skip_bias_pad; q.oh = p.pl[P::S]; q.ol = p.pl[P::S + 1]; q.ldh = C; q.n_valid = C;
+  q.mode = SP_SKIPPROJ; q.bias = d.skip_bias_pad; q.wscale = d.skip_tc.wscale; q.oh = p.pl[P::S]; q.ol = p.pl[P::S + 1]; q.ldh = C; q.n_valid = C;
   ph.push_back(q);
 }
 
@@ -780,12 +780,13 @@ static int run_mel_diffusion_persistent(Ctx& c, const Model& m, const SeqDev& s,
     for (int t = K - 1; t >= 0; --t) {
       SPhase q = sphase(1);  // input_projection + ReLU ; y = x + step bias of layer 0
       q.a1 = M_X80; q.w1 = W_IN; q.kchunks = 2; q.N = C; q.NT = C / 64; q.mode = SP_INPROJ; q.bias = d.in_proj.bias;
+      q.wscale = d.in_tc.wscale;
       q.out = net.x; q.ldo = C; q.oh = net.pl[P::Y]; q.ol = net.pl[P::Y + 1]; q.ldh = C; q.vec2 = d.dtab + (size_t)t * L * C;
       ph.push_back(q);
       persistent_net_step(net, s, t, 1, ph);
       q = sphase(1);  // output_projection -> eps ; fused DDPM posterior step on x_t
       q.a1 = net.mb + P::S; q.w1 = net.w_out(); q.kchunks = C / 64; q.N = 256; q.NT = 4; q.mode = SP_MEL_SAMPLE;
-      q.bias = d.out_bias_pad; q.out = xm; q.ldo = 80; q.oh = x80h; q.ol = x80l; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
+      q.bias = d.out_bias_pad; q.wscale = d.out_tc.wscale; q.out = xm; q.ldo = 80; q.oh = x80h; q.ol = x80l; q.ldh = 128; q.tab = d.gtab + (size_t)t * 8;
       q.noise = noise ? noise + per * (size_t)(K - t) : nullptr; q.stream_id = stream_mel_step(t); q.n_valid = 80;
       q.no_clip = m.mel_decoder == SSB_MEL_DECODER_PRODIFF;
       ph.push_back(q);
@@ -963,7 +964,7 @@ static int run_f0_diffusion_pair_persistent(Ctx& c, const Model& m, const SeqDev
         persistent_net_step(net[n], s, t, n == 1, seq[n]);
         SPhase q = sphase(n == 1);  // output_projection -> (eps, logits) ; F0/UV step ; DDiffNet input of step t-1
         q.a1 = net[n].mb + P::S; q.w1 = net[n].w_out(); q.kchunks = C / 64; q.N = d.out_tc.N; q.NT = d.out_tc.N / 64;
-        q.mode = SP_F0_SAMPLE; q.bias = d.out_bias_pad; q.out = z[n]; q.uv = uv[n]; q.clip_lo = lo; q.clip_hi = hi;
+        q.mode = SP_F0_SAMPLE; q.bias = d.out_bias_pad; q.wscale = d.out_tc.wscale; q.out = z[n]; q.uv = uv[n]; q.clip_lo = lo; q.clip_hi = hi;
         q.tab = d.gtab + (size_t)t * 8; q.tab2 = d.mtab + (size_t)t * 8; q.tstep = t; q.log_eps = m.log_eps;
         q.noise = gnoise[n] ? gnoise[n] + per * (size_t)(T - t) : nullptr;
         q.noise2 = unoise[n] ? unoise[n] + per * 2 * (size_t)(T - 1 - t) : nullptr;

@@ -151,8 +151,9 @@ int run_denoise(Ctx& c, const ssb_wav_denoise& d, const Seq& q, const float* wav
     SSB_CUDA(cudaGetLastError());
     ++g_launches;
   }
-  // the synthesis weights are O(1) (their fp16 lo planes stay clear of the subnormal range); irfft's 1 / n_fft is the
-  // epilogue's alpha
+  // irfft's 1 / n_fft is the epilogue's alpha, not folded into the synthesis weights: n_fft need not be a power of two,
+  // and a rounded product in the weights would change the FFMA path's bits (the tensor-core packing scales its planes by
+  // a power of two of its own, so it would not need it)
   const float inv_n = 1.0f / (float)d.n_fft;
   if (tc) {
     GemmTC g = make_gemm_tc(d.inv_tc, s, sh, sl);

@@ -5,6 +5,8 @@ function of it, so one reference serves every option on that input.  Matrices he
 layout the kernels use (csrc/common.cuh): utterance b at rows [rs_b, rs_b + L_b), rs_0 = 16, rs_{b+1} = rs_b + L_b + 16, and
 256 rows of tail slack.  Column order is torch's unless a function says "packed": the gate GEMM's packed order interleaves
 the two halves (column 2j = sigmoid argument j, 2j + 1 = tanh argument j)."""
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -121,6 +123,31 @@ def split(x):
     x = x.float()
     hi = x.half()
     return hi, (x - hi.float()).half()
+
+
+def plane_exponent(w):
+    """The power of two pack_conv_tc (csrc/pack.cu) scales a weight tensor by before it splits it: s = 14 - ceil(log2
+    max|w|) over the fp32 tensor, so that max|w 2^s| <= 2^14; 0 for an all-zero or non-finite tensor; within [-126, 126]."""
+    mx = float(w.float().abs().max()) if w.numel() else 0.0
+    if not mx > 0.0 or mx == float("inf"):
+        return 0
+    m, e = math.frexp(mx)
+    return max(-126, min(126, 14 - (e - 1 if m == 0.5 else e)))
+
+
+def split_scaled(w):
+    """The packer's weight planes: (hi, lo, s) with hi / lo = split(w 2^s), s = plane_exponent(w).  The kernels multiply
+    the accumulator by 2^-s, so w is carried as (hi + lo) 2^-s."""
+    s = plane_exponent(w)
+    hi, lo = split(torch.ldexp(w.float(), torch.tensor(float(s))))
+    return hi, lo, s
+
+
+def weight_value(w, single_pass=False):
+    """The weight value the tensor-core GEMM multiplies, in float64: (hi + lo) 2^-s, or hi 2^-s in the single-pass form."""
+    hi, lo, s = split_scaled(w)
+    v = hi.double() if single_pass else hi.double() + lo.double()
+    return torch.ldexp(v, torch.tensor(float(-s), dtype=torch.float64))
 
 
 def skip_tiled_to_rows(buf, tl, C, rows):

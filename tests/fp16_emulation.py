@@ -5,16 +5,26 @@ emulation runs the existing float64 oracles (tests/denoiser_oracle.py, tests/sam
 tests/vocoder_layouts_ref.py, tests/conv_gemm_ref.py) with the activation and the weight of each such contraction
 rounded to fp16 and everything else, the sums included, in float64.  fp16_convs() patches torch.nn.functional's conv1d /
 conv_transpose1d for the duration of a block; `select(kind, x, w, stride)` says which calls are tensor-core GEMMs on the
-CUDA path.  Biases are not rounded: the kernels add them in fp32 in the epilogue."""
+CUDA path.  A weight is rounded as the tensor-core packer rounds it, fp16(w 2^s) 2^-s with one power of two s per tensor
+(tests/conv_gemm_ref.py plane_exponent): that is fp16(w) for every weight that is a normal fp16 number.  Biases are not
+rounded: the kernels add them in fp32 in the epilogue."""
 import contextlib
 
 import torch
 import torch.nn.functional as F
 
+from tests.conv_gemm_ref import plane_exponent
+
 
 def r16(t):
     """t rounded to fp16 (round to nearest even), returned in t's dtype."""
     return t.half().to(t.dtype)
+
+
+def r16w(w):
+    """A weight tensor rounded as the tensor-core packer rounds it: fp16(w 2^s) 2^-s, s = plane_exponent(w)."""
+    s = plane_exponent(w)
+    return torch.ldexp(torch.ldexp(w, torch.tensor(float(s))).half().to(w.dtype), torch.tensor(float(-s)))
 
 
 def every_conv(kind, x, w, stride):
@@ -42,14 +52,14 @@ def fp16_convs(select=every_conv):
     def c1(x, w, b=None, stride=1, *a, **k):
         if select("conv1d", x, w, stride):
             n["rounded"] += 1
-            return conv1d(r16(x), r16(w), b, stride, *a, **k)
+            return conv1d(r16(x), r16w(w), b, stride, *a, **k)
         n["kept"] += 1
         return conv1d(x, w, b, stride, *a, **k)
 
     def ct(x, w, b=None, stride=1, *a, **k):
         if select("conv_transpose1d", x, w, stride):
             n["rounded"] += 1
-            return convt(r16(x), r16(w), b, stride, *a, **k)
+            return convt(r16(x), r16w(w), b, stride, *a, **k)
         n["kept"] += 1
         return convt(x, w, b, stride, *a, **k)
 

@@ -59,7 +59,7 @@ def test_op_emulation_rounds_both_operands():
     x = torch.zeros(rows, 64, dtype=torch.float64)
     x[valid] = torch.randn(int(valid.sum()), 64, generator=g, dtype=torch.float64)
     w = torch.randn(128, 64, 3, generator=g, dtype=torch.float64) / 14
-    want = R.accumulator(E.r16(x), E.r16(w), 2, lens, rs)
+    want = R.accumulator(E.r16(x), E.r16w(w), 2, lens, rs)
     with E.fp16_convs() as n:
         got = torch.nn.functional.conv1d(x.t()[None], w, None, padding=2, dilation=2)[0].t()
     assert n["rounded"] == 1

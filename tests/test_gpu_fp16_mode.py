@@ -78,7 +78,7 @@ def test_op_gemm_single_pass_matches_fp16_emulation(case):
     w = torch.randn(N, Cin, k, generator=g) / (Cin * k) ** 0.5
     b = torch.randn(N, generator=g)
     hi, _ = R.split(x)
-    acc = R.accumulator(E.r16(x.double()), E.r16(w.double()), dil, lens, rs)
+    acc = R.accumulator(E.r16(x.double()), E.r16w(w.double()), dil, lens, rs)
     offs = frame_offsets(lens)
     args = dict(a_hi=hi.to(DEV))
     C = N // 2

@@ -2,13 +2,15 @@
 
 A CPU fp32 restatement (torch functional ops, one utterance at a time = the reference's B=1
 semantics) of every function on StyleSinger's ph -> mel -> wav inference path
-(SURVEY.md §8a rows a1-a22).  Each function cites the reference file:line it follows.
+(SURVEY.md §8a rows a1-a22), under every reference option the CUDA path runs (stylesinger_forward's hp keys,
+hifigan_generator's resblock).  Each function cites the reference file:line it follows.
 
 Pinning: the reference has NO tests / golden vectors for this path (SURVEY.md §4), so this oracle
 is pinned against outputs of the UNMODIFIED reference modules executed in the build container:
 tools/make_golden.py imports /root/reference, loads the synthetic checkpoints of
 stylesinger_b200/synth.py with strict=True, runs them with injected noise and writes
-tests/golden/*.npz; tests/test_oracle_golden.py checks this file against those fixtures.
+tests/golden/*.npz; tests/test_oracle_golden.py and the tests/test_*_cpu.py of each option check this file against
+those fixtures.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
 import this module (as the checker / the timed CPU baseline).  The product package
@@ -387,8 +389,22 @@ def _gauss_tables(T, max_beta):
     host, registered as fp32.  The oracle's OWN restatement (the product computes its tables in
     stylesinger_b200/schedules.py; tests/test_oracle_golden.py pins both against buffers dumped from the reference at
     T in {4, 25, 50, 100, 200, 500})."""
-    b = np.linspace(1e-4, max_beta, T)
+    return _schedule_buffers(np.linspace(1e-4, max_beta, T))
+
+
+def prodiff_tables(T):
+    """ProDiffusion.__init__ buffers for schedule_type 'vpsde' (prodiff.py:11-13 vpsde_beta_t, :28-49
+    get_noise_schedule_list(timesteps=T+1, min_beta=0.1, max_beta=40), :69-117): float64 on the host, registered as
+    fp32, length T+1 (the sampler reads rows 0..T-1)."""
+    n = T + 1
+    return _schedule_buffers(
+        np.array([1.0 - np.exp(-0.1 / n - 0.5 * (40.0 - 0.1) * (2 * t - 1) / (n * n)) for t in range(1, n + 1)]))
+
+
+def _schedule_buffers(b):
+    """The buffers both diffusion classes derive from their float64 betas b, registered as fp32."""
     a = 1.0 - b
+    T = len(b)
     ac = np.empty(T, np.float64)
     run = 1.0
     for i in range(T):  # np.cumprod
@@ -417,20 +433,28 @@ def _multi_tables(T, max_beta):
     return {k: torch.from_numpy(v.astype(np.float32)) for k, v in out.items()}
 
 
+def k_step(hp):
+    """hparams['K_step'] (the timesteps when absent): GaussianDiffusion.__init__ builds its buffers for the whole
+    `timesteps`-long schedule and stores K_step beside them (shallow_diffusion_tts.py:68-119); the samplers start from
+    t = K and read only the first K rows."""
+    return int(hp.get("K_step", hp["timesteps"]))
+
+
 def mel_diffusion_sample(cond, coarse_mel, sd, hp, noise, return_steps=False):
     """DiffusionDecoder.forward(infer=True) (shallow_diffusion_tts.py:284-307) with p_sample (:155-162),
-    p_mean_variance (:145-153), q_sample (:199-204), norm/denorm_spec (:271-275).
+    p_mean_variance (:145-153), q_sample (:199-204), norm/denorm_spec (:271-275): x_K = q_sample(norm_spec(coarse), K-1)
+    on the T-step schedule, then the K reverse steps t = K-1 .. 0 (:297-304), K = k_step(hp): K + 1 draws.
     cond [B,F,256], coarse_mel [B,F,80] -> mel [B,F,80]."""
-    T = hp["timesteps"]
-    s = _gauss_tables(T, hp["max_beta"])
+    K = k_step(hp)
+    s = _gauss_tables(hp["timesteps"], hp["max_beta"])
     smin = torch.tensor(hp["spec_min"], dtype=torch.float32)[None, None, :hp["keep_bins"]]
     smax = torch.tensor(hp["spec_max"], dtype=torch.float32)[None, None, :hp["keep_bins"]]
     c = cond.transpose(1, 2)
     x0 = ((coarse_mel - smin) / (smax - smin) * 2 - 1).transpose(1, 2)[:, None]
-    x = s["sqrt_alphas_cumprod"][T - 1] * x0 + s["sqrt_one_minus_alphas_cumprod"][T - 1] * noise.randn(x0.shape)
+    x = s["sqrt_alphas_cumprod"][K - 1] * x0 + s["sqrt_one_minus_alphas_cumprod"][K - 1] * noise.randn(x0.shape)
     steps = []
     B = x.shape[0]
-    for i in reversed(range(T)):
+    for i in reversed(range(K)):
         t = torch.full((B,), i, dtype=torch.long)
         eps = diffnet(x, t, c, sd, hp)
         x_recon = s["sqrt_recip_alphas_cumprod"][i] * x - s["sqrt_recipm1_alphas_cumprod"][i] * eps
@@ -447,16 +471,17 @@ def mel_diffusion_sample(cond, coarse_mel, sd, hp, noise, return_steps=False):
 def mel_diffusion_sample_plms(cond, coarse_mel, sd, hp, noise, interval):
     """PLMS / PNDM sampler over the same DiffNet (SURVEY.md section 8f, row f2): GaussianDiffusion.p_sample_plms
     (shallow_diffusion_tts.py:164-197) driven by the `pndm_speedup` loop of GaussianDiffusion.forward (:254-260):
-    T // interval denoiser evaluations (+1 for the first, second-order, step) instead of T; deterministic after q_sample.
+    K // interval denoiser evaluations (+1 for the first, second-order, step) instead of K, from the same t = K as the
+    DDPM sampler (K = k_step(hp): reversed(range(0, K, interval))); deterministic after q_sample at K-1.
     cond [B,F,256], coarse_mel [B,F,80] -> mel [B,F,80]."""
-    T = hp["timesteps"]
-    s = _gauss_tables(T, hp["max_beta"])
+    K = k_step(hp)
+    s = _gauss_tables(hp["timesteps"], hp["max_beta"])
     ac = s["alphas_cumprod"]
     smin = torch.tensor(hp["spec_min"], dtype=torch.float32)[None, None, :hp["keep_bins"]]
     smax = torch.tensor(hp["spec_max"], dtype=torch.float32)[None, None, :hp["keep_bins"]]
     c = cond.transpose(1, 2)
     x0 = ((coarse_mel - smin) / (smax - smin) * 2 - 1).transpose(1, 2)[:, None]
-    x = s["sqrt_alphas_cumprod"][T - 1] * x0 + s["sqrt_one_minus_alphas_cumprod"][T - 1] * noise.randn(x0.shape)
+    x = s["sqrt_alphas_cumprod"][K - 1] * x0 + s["sqrt_one_minus_alphas_cumprod"][K - 1] * noise.randn(x0.shape)
     B = x.shape[0]
 
     def x_pred(x, eps, i):  # get_x_pred (:170-178), fp32 like the reference's registered buffers
@@ -467,7 +492,7 @@ def mel_diffusion_sample_plms(cond, coarse_mel, sd, hp, noise, interval):
         return x + delta
 
     hist = []  # deque(maxlen=4) in the reference; only the last three entries are ever read
-    for i in reversed(range(0, T, interval)):
+    for i in reversed(range(0, K, interval)):
         t = torch.full((B,), i, dtype=torch.long)
         eps = diffnet(x, t, c, sd, hp)
         if len(hist) == 0:
@@ -484,6 +509,28 @@ def mel_diffusion_sample_plms(cond, coarse_mel, sd, hp, noise, interval):
         hist.append(eps)
         hist = hist[-4:]
     return (x[:, 0].transpose(1, 2) + 1) / 2 * (smax - smin) + smin
+
+
+PRODIFF_PREFIX = "diff_decoder.denoise_fn."  # the ProDiff teacher's DiffNet (stylesinger.py:111-117)
+
+
+def mel_prodiff_sample(cond, sd, hp, noise):
+    """ProDiffusion.forward(cond, infer=True) (prodiff.py:204-222), p_sample (:143-148), q_posterior_sample (:135-141):
+    x_T = randn [B,1,80,F]; per step x0 = denoise_fn(x_t, t, cond) (no eps conversion, no clip), then the posterior mean
+    plus nonzero_mask * exp(0.5 logvar) * randn (drawn at every step, t = 0 included); denorm_spec is the identity.
+    cond [B,F,256] (decoder_inp) -> mel [B,F,80]."""
+    T = hp["timesteps"]
+    s = prodiff_tables(T)
+    c = cond.transpose(1, 2)
+    B, Fr = cond.shape[0], cond.shape[1]
+    x = noise.randn((B, 1, hp["audio_num_mel_bins"], Fr))
+    for i in reversed(range(T)):
+        t = torch.full((B,), i, dtype=torch.long)
+        x0 = diffnet(x, t, c, sd, hp, p=PRODIFF_PREFIX)
+        mean = s["posterior_mean_coef1"][i] * x0 + s["posterior_mean_coef2"][i] * x
+        nz = noise.randn(x.shape)
+        x = mean + (0.0 if i == 0 else 1.0) * (0.5 * s["posterior_log_variance_clipped"][i]).exp() * nz
+    return x[:, 0].transpose(1, 2)
 
 
 def _log_add_exp(a, b):
@@ -577,18 +624,48 @@ def add_gmdiff_pitch(dec_inp, midi, sd, hp, which, noise):
     return torch.cat([f0[:, :, None], uv[:, :, None]], dim=2)
 
 
+PITCH_PREDICTORS = ("pitch_predictor.", "pitch_inpainter_predictor.")  # f0_gen 'conv': which = 0 agnostic, 1 specific
+
+
+def pitch_predictor(xs, sd, which, dtype=torch.float32):
+    """PitchPredictor.forward (tts_modules.py:221-234) in eval mode: xs [B,T,H] -> [B,T,2] in `dtype`.  positions come
+    from make_positions(xs[..., 0]) (padding_idx 0: a row whose channel 0 is exactly 0 gets the zero row and does not
+    count); then 5 x (zero SAME pad, Conv1d, ReLU, channel LayerNorm eps 1e-5); then Linear.  No mask anywhere."""
+    p = PITCH_PREDICTORS[which]
+    w = {k[len(p):]: v.to(dtype) for k, v in sd.items() if k.startswith(p)}
+    H = xs.shape[-1]
+    xs = xs.to(dtype)
+    pos = sinusoid_positions(xs[..., 0].cpu(), H).to(xs.device, dtype)
+    x = (xs + w["pos_embed_alpha"] * pos).transpose(1, -1)
+    i = 0
+    while f"conv.{i}.1.weight" in w:
+        k = w[f"conv.{i}.1.weight"].shape[-1]
+        x = F.pad(x, ((k - 1) // 2, (k - 1) // 2))
+        x = F.relu(F.conv1d(x, w[f"conv.{i}.1.weight"], w[f"conv.{i}.1.bias"]))
+        x = layer_norm_ch(x, w[f"conv.{i}.3.weight"], w[f"conv.{i}.3.bias"])
+        i += 1
+    return F.linear(x.transpose(1, -1), w["linear.weight"], w["linear.bias"])
+
+
 def inpaint_pitch(agn, spec, mel2ph, midi, sd, hp, noise, f0=None, uv=None):
-    """StyleSinger.inpaint_pitch (stylesinger.py:216-247). Returns dict."""
-    pad = mel2ph == 0
-    pa = add_gmdiff_pitch(agn, midi, sd, hp, 0, noise)
-    ps = add_gmdiff_pitch(spec, midi, sd, hp, 1, noise)
+    """StyleSinger.inpaint_pitch (stylesinger.py:216-247). Returns dict.  f0_gen 'gmdiff': the two F0 samplers, each
+    inside the MIDI band of midi [B,1,F], rests forced unvoiced.  f0_gen 'conv' (:73-82): the two pitch predictors,
+    which draw no noise and read no midi; f0 = pitch_pred[..., 0] is log2 Hz as is (the predictors run in fp32 whatever
+    the inputs' dtype).  f0 / uv: teacher forcing, else the averaged prediction's (uv = averaged logit > 0)."""
+    if hp.get("f0_gen", "gmdiff") == "conv":
+        pa = pitch_predictor(agn, sd, 0)
+        ps = pitch_predictor(spec, sd, 1)
+    else:
+        pa = add_gmdiff_pitch(agn, midi, sd, hp, 0, noise)
+        ps = add_gmdiff_pitch(spec, midi, sd, hp, 1, noise)
     pred = ps / 2 + pa / 2
     if f0 is None:
         f0 = pred[:, :, 0]
         uv = pred[:, :, 1] > 0
     f0_denorm = 2 ** f0
-    f0_denorm = torch.where(uv > 0, torch.zeros_like(f0_denorm), f0_denorm)
-    f0_denorm = torch.where(pad, torch.zeros_like(f0_denorm), f0_denorm)
+    if uv is not None:
+        f0_denorm = torch.where(uv > 0, torch.zeros_like(f0_denorm), f0_denorm)
+    f0_denorm = torch.where(mel2ph == 0, torch.zeros_like(f0_denorm), f0_denorm)
     pitch = f0_to_coarse(f0_denorm)
     emb = F.embedding(pitch, sd["pitch_embed.weight"], padding_idx=0)
     return {"pitch_pred": pred, "f0_denorm": f0_denorm, "pitch": pitch, "pitch_embed": emb,
@@ -598,39 +675,68 @@ def inpaint_pitch(agn, spec, mel2ph, midi, sd, hp, noise, f0=None, uv=None):
 # ----------------------------------------------------------------------------------------------
 # a17 + whole model
 # ----------------------------------------------------------------------------------------------
+def speaker(spk, sd, hp):
+    """ret['spk_embed'] [B,1,256] (stylesinger.py:130): with use_spk_id the rows of the Embedding(num_spk + 1, 256)
+    table at the ids spk (LongTensor [B], fs2.py:37-43), else the Linear over the speaker vectors spk [B,256]."""
+    if hp.get("use_spk_id", False):
+        return F.embedding(spk, sd["spk_embed_proj.weight"])[:, None, :]
+    return F.linear(spk, sd["spk_embed_proj.weight"], sd["spk_embed_proj.bias"])[:, None, :]
+
+
 def stylesinger_forward(sd, hp, txt_tokens, note, note_dur, note_type, spk_embed, emo_embed, ref_mels, ref_f0,
                         noise, mel2ph=None, f0=None, uv=None, skip_diffusion=False, codes=None):
-    """StyleSinger.forward(infer=True, global_steps > diff_start) (stylesinger.py:119-187) for B=1.
-    All tensors carry a leading batch dim of 1 (ref_f0 may be [R]); codes: see rq_quantize."""
+    """StyleSinger.forward(infer=True, global_steps > diff_start) (stylesinger.py:119-187) for B=1, under hp's model
+    options (each absent key reads as hparams.resolve's default): the mel decoder hp['decoder'] ('diffsinger',
+    'prodiff', 'fft'), the F0 generator hp['f0_gen'] ('gmdiff', 'conv'), the switches emo / style / use_txt_cond (umln
+    reads nothing: UMLN is the identity in eval), use_spk_id and K_step.
+    All tensors carry a leading batch dim of 1 (ref_f0 may be [R]).  spk_embed: the speaker ids [B] with use_spk_id,
+    else the speaker vectors [B,256]; emo_embed is unread without emo, ref_mels / ref_f0 without style; f0 / uv: see
+    inpaint_pitch; codes: see rq_quantize.  Draw order: the two F0 samplers (gmdiff), then the mel sampler (none with
+    decoder 'fft' or skip_diffusion)."""
+    emo_on, style_on = hp.get("emo", True), hp.get("style", True)
+    decoder = hp.get("decoder", "diffsinger")
     ret = {}
     enc = fastspeech_encoder(txt_tokens, sd, hp) + note_encoder(note, note_dur, note_type, sd, hp["hidden_size"])
     src_np = (txt_tokens > 0).float()[:, :, None]
-    spk = F.linear(spk_embed, sd["spk_embed_proj.weight"], sd["spk_embed_proj.bias"])[:, None, :]
-    emo = F.linear(emo_embed, sd["emo_embed_proj.weight"], sd["emo_embed_proj.bias"])[:, None, :]
-    ret["spk_embed"], ret["emo_embed"] = spk, emo
-    dur_inp = (enc + spk + emo) * src_np
-    if mel2ph is None:
-        dur, xs = duration_predictor(dur_inp, txt_tokens == 0, sd, hp)
+    spk = speaker(spk_embed, sd, hp)
+    ret["spk_embed"] = spk
+    emo = 0.0
+    if emo_on:  # :131-132
+        emo = F.linear(emo_embed, sd["emo_embed_proj.weight"], sd["emo_embed_proj.bias"])[:, None, :]
+        ret["emo_embed"] = emo
+    if mel2ph is None:  # dur_inp = (encoder_out + spk [+ emo]) * src_nonpadding (:134-139)
+        dur, xs = duration_predictor((enc + spk + emo) * src_np, txt_tokens == 0, sd, hp)
         ret["dur"], ret["dur_choice"] = xs, dur
         mel2ph = length_regulator(dur, txt_tokens == 0)
     ret["mel2ph"] = mel2ph
     tgt_np = (mel2ph > 0).float()[:, :, None]
-    dec = expand_states(enc, mel2ph)  # UMLN = identity in eval (umln.py:49-50)
+    dec = expand_states(enc, mel2ph)  # UMLN = identity in eval (umln.py:49-50), whatever hp['umln']
     ret["encoder_out"] = enc
-    style, codes = get_style(dec, ref_mels, ref_f0, sd, hp, codes)
-    ret["style"], ret["rq_codes"] = style, codes
+    style = 0.0
+    if style_on:  # :149-151
+        style, codes = get_style(dec, ref_mels, ref_f0, sd, hp, codes)
+        ret["style"], ret["rq_codes"] = style, codes
     midi = expand_states(note[:, :, None], mel2ph).transpose(-1, -2)
     agn = dec * tgt_np
-    spc = (dec + spk + emo + style) * tgt_np
+    spc = (dec + spk + emo + style) * tgt_np  # :157-163
     pit = inpaint_pitch(agn, spc, mel2ph, midi.float() if midi.dtype != torch.float32 else midi, sd, hp, noise, f0, uv)
-    ret.update({"pitch_pred": pit["pitch_pred"], "f0_denorm": pit["f0_denorm"], "pitch": pit["pitch"]})
-    dec = (dec + spk + pit["pitch_embed"] + emo + style) * tgt_np
+    ret.update({k: v for k, v in pit.items() if k != "pitch_embed"})
+    dec = (dec + spk + pit["pitch_embed"] + emo + style) * tgt_np  # :167-172
     ret["decoder_inp"] = dec
+    if decoder == "prodiff":  # :176-177
+        if not skip_diffusion:
+            ret["mel_out"] = mel_prodiff_sample(dec, sd, hp, noise)
+        return ret
     coarse = F.linear(fastspeech_decoder(dec, sd, hp), sd["mel_out.weight"], sd["mel_out.bias"]) * tgt_np
+    if decoder == "fft":  # :185-186: run_decoder's mel is the output
+        ret["mel_out"] = coarse
+        return ret
     ret["coarse_mel"] = coarse
     Fr = coarse.shape[1]
-    g = torch.cat([coarse, dec, spk.repeat(1, Fr, 1), emo.repeat(1, Fr, 1), style], dim=-1)
-    g = F.linear(g, sd["ln_proj.weight"], sd["ln_proj.bias"])
+    g = [coarse] + ([dec] if hp.get("use_txt_cond", True) else []) + [spk.repeat(1, Fr, 1)]  # run_diffsinger (:313-327)
+    g += [emo.repeat(1, Fr, 1)] if emo_on else []
+    g += [style] if style_on else []
+    g = F.linear(torch.cat(g, dim=-1), sd["ln_proj.weight"], sd["ln_proj.bias"])
     ret["diff_cond"] = g
     if not skip_diffusion:
         ret["mel_out"] = mel_diffusion_sample(g, coarse, sd, hp, noise)
@@ -668,13 +774,15 @@ def source_module(f0_up, sd, noise):
 
 
 def hifigan_generator(mel, f0, sd, h, noise, dtype=torch.float32):
-    """HifiGanGenerator.forward after remove_weight_norm (hifigan_nsf.py:144-178).
-    mel [B,80,F], f0 [B,F] or None -> wav [B,1,256F] in `dtype`.
+    """HifiGanGenerator.forward after remove_weight_norm (hifigan_nsf.py:144-178), h['resblock'] '1' (ResBlock1, :30-67)
+    or '2' (ResBlock2, :69-90: one conv per dilation, the first two of each list).
+    mel [B,80,F], f0 [B,F] or None -> wav [B,1,hop*F] in `dtype`.
     dtype=torch.float64 runs the conv stack, the leaky ReLUs and the tanh in double precision: an arbiter for the CUDA
     path.  The NSF source stays fp32 whatever `dtype` is: the reference accumulates the phase with an fp32 cumsum and the
     CUDA kernel reproduces that rounding; a float64 phase drifts from both by ~1e-2 over 10 s."""
     rates, ks = h["upsample_rates"], h["upsample_kernel_sizes"]
     nk = len(h["resblock_kernel_sizes"])
+    rb1 = str(h.get("resblock", "1")) == "1"
     W = lambda n: fold_weight_norm(sd[n + ".weight_g"], sd[n + ".weight_v"]).to(dtype)
     P = lambda n: sd[n].to(dtype)
     har = None
@@ -695,11 +803,13 @@ def hifigan_generator(mel, f0, sd, h, noise, dtype=torch.float32):
         for j, (rk, rd) in enumerate(zip(h["resblock_kernel_sizes"], h["resblock_dilation_sizes"])):
             r = x
             q = f"resblocks.{i * nk + j}."
-            for m_, d in enumerate(rd):
+            for m_, d in enumerate(rd if rb1 else rd[:2]):
+                c = f"{q}convs1.{m_}" if rb1 else f"{q}convs.{m_}"
                 xt = F.leaky_relu(r, 0.1)
-                xt = F.conv1d(xt, W(f"{q}convs1.{m_}"), P(f"{q}convs1.{m_}.bias"), padding=(rk * d - d) // 2, dilation=d)
-                xt = F.leaky_relu(xt, 0.1)
-                xt = F.conv1d(xt, W(f"{q}convs2.{m_}"), P(f"{q}convs2.{m_}.bias"), padding=(rk - 1) // 2)
+                xt = F.conv1d(xt, W(c), P(c + ".bias"), padding=(rk * d - d) // 2, dilation=d)
+                if rb1:
+                    xt = F.leaky_relu(xt, 0.1)
+                    xt = F.conv1d(xt, W(f"{q}convs2.{m_}"), P(f"{q}convs2.{m_}.bias"), padding=(rk - 1) // 2)
                 r = xt + r
             xs = r if xs is None else xs + r
         x = xs / nk
@@ -720,8 +830,8 @@ def postprocess_mel(mel_out, f0_denorm, hp):
 
 
 def spec2wav(mel, f0, vsd, h, noise, dtype=torch.float32):
-    """HifiGAN.spec2wav (tasks/tts/vocoder_infer/hifigan_nsf.py:62-75). mel np [F,80], f0 np [F] -> wav np in `dtype`
-    (see hifigan_generator)."""
+    """HifiGAN.spec2wav (tasks/tts/vocoder_infer/hifigan_nsf.py:62-75). mel np [F,80], f0 np [F] or None -> wav np in
+    `dtype` (see hifigan_generator)."""
     c = torch.from_numpy(np.ascontiguousarray(mel)).float().unsqueeze(0).transpose(2, 1)
     f = None if f0 is None else torch.from_numpy(np.ascontiguousarray(f0)).float()[None, :]
     return hifigan_generator(c, f, vsd, h, noise, dtype).view(-1).numpy()

@@ -7,7 +7,7 @@ import torch
 
 from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
-from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG, resolve
+from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG, HIFIGAN_V2, HIFIGAN_V3, resolve
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 _CACHE = {}
@@ -34,6 +34,69 @@ def acoustic_sd64():
     if "sd64" not in _CACHE:
         _CACHE["sd64"] = {k: (v.double() if v.is_floating_point() else v) for k, v in acoustic_sd().items()}
     return _CACHE["sd64"]
+
+
+# ---- the model options' fixtures: hparams and synthetic checkpoints (seed 0, cached) --------------------------------
+# Each keeps the resolve() arguments tools/make_golden.py generated its fixture with: the checkpoint draws follow them.
+def switch_hp(cfg):
+    """tests/golden/ref_switches.npz: cfg = {"T": ..., "overrides": {...}} (switches and decoder / f0_gen)."""
+    return resolve(timesteps=cfg["T"], K_step=cfg["T"], f0_timesteps=cfg["T"], **cfg["overrides"])
+
+
+def fft_spkid_hp(cfg):
+    """tests/golden/ref_fft_spkid.npz: switch_hp with the opt-in decoder 'fft' and use_spk_id need (extended_models)."""
+    return resolve(timesteps=cfg["T"], K_step=cfg["T"], f0_timesteps=cfg["T"], extended_models=True, **cfg["overrides"])
+
+
+def conv_hp(meta):
+    """tests/golden/ref_convf0.npz (meta, or meta['prodiff']): f0_gen 'conv' plus the fixture's overrides."""
+    return resolve(timesteps=meta["T"], K_step=meta["T"], **meta["overrides"])
+
+
+def prodiff_hp(T=None):
+    """tests/golden/ref_prodiff_T8.npz (decoder 'prodiff', schedule 'vpsde') at T steps (default the fixture's 8)."""
+    _, meta = golden("ref_prodiff_T8")
+    T = meta["T"] if T is None else T
+    return resolve(timesteps=T, K_step=T, f0_timesteps=meta["f0_T"], **meta["overrides"])
+
+
+def kstep_hp(T, K):
+    """tests/golden/ref_kstep.npz: the T-step schedule with K_step K (acoustic_sd() is its checkpoint)."""
+    return resolve(timesteps=T, K_step=K, f0_timesteps=T)
+
+
+def _synth_sd(hp_of, cfg):
+    key = (hp_of, cfg["T"], tuple(sorted(cfg["overrides"].items())))
+    if key not in _CACHE:
+        _CACHE[key] = synth.acoustic_state_dict(hp_of(cfg), seed=0)
+    return _CACHE[key]
+
+
+def switch_sd(cfg):
+    return _synth_sd(switch_hp, cfg)
+
+
+def fft_spkid_sd(cfg):
+    return _synth_sd(fft_spkid_hp, cfg)
+
+
+def conv_sd(meta):
+    return _synth_sd(conv_hp, meta)
+
+
+def prodiff_sd():
+    if "prodiff_sd" not in _CACHE:
+        _CACHE["prodiff_sd"] = synth.acoustic_state_dict(prodiff_hp(), seed=0)
+    return _CACHE["prodiff_sd"]
+
+
+def predictor_inputs(meta):
+    """The seeded inputs of ref_convf0's predictor-only case: [2, pred_frames, 256] (one per predictor), channel 0
+    exactly 0 in the rows meta['pred_zero_rows']."""
+    g = torch.Generator().manual_seed(meta["pred_seed"])
+    xs = torch.randn(2, 1, meta["pred_frames"], 256, generator=g)
+    xs[:, :, meta["pred_zero_rows"], 0] = 0
+    return xs[:, 0]
 
 
 def registry_inputs(seed=131):
@@ -71,10 +134,18 @@ def registry_inputs(seed=131):
     return d
 
 
-def vocoder_sd():
-    if "vsd" not in _CACHE:
-        _CACHE["vsd"] = synth.vocoder_state_dict(DEFAULT_VOCODER_CONFIG, seed=0)
-    return _CACHE["vsd"]
+# the layouts of tools/make_golden.py vocoder_layouts (tests/golden/ref_vocoder_layouts.npz): V3 without NSF is the
+# generator the `HifiGAN` registry class builds from a config without the harmonic source
+VOCODER_LAYOUTS = {"v2": HIFIGAN_V2, "v3": HIFIGAN_V3, "v3_nonsf": dict(HIFIGAN_V3, use_pitch_embed=False)}
+
+
+def vocoder_sd(layout=None):
+    """The synthetic checkpoint (seed 0, cached) of DEFAULT_VOCODER_CONFIG (V1), or of VOCODER_LAYOUTS[layout]."""
+    key = ("vsd", layout)
+    if key not in _CACHE:
+        _CACHE[key] = synth.vocoder_state_dict(DEFAULT_VOCODER_CONFIG if layout is None else VOCODER_LAYOUTS[layout],
+                                               seed=0)
+    return _CACHE[key]
 
 
 def utt_from_meta(meta):

@@ -3,7 +3,7 @@
 diffnet64 / ddiffnet64 run O.diffnet / O.ddiffnet on the state dict cast to float64 with the step t passed as a float64
 tensor (an integer t would make the step embedding fp32, and F.linear then meets float64 weights); the frequency table
 of the sinusoidal step embedding stays fp32, as the reference builds it.  mel_chain64 and f0_chain64 restate
-O.mel_diffusion_sample (through the K-step schedule slicing of tests/kstep_oracle.py) and O.f0_diffusion_sample step for
+O.mel_diffusion_sample (K_step steps on the T-step schedule) and O.f0_diffusion_sample step for
 step in float64 on the reference's fp32 schedule buffers, and return what a GPU comparison needs beyond the final
 sample: every x_t / z_t, the fraction of x0 predictions the clip changed, and the Gumbel margin of every UV decision.
 The noise comes in the C ABI's injected-noise layout (include/stylesinger_b200.h) for one utterance and is handed out
@@ -13,7 +13,6 @@ import torch
 import torch.nn.functional as F
 
 from oracle import stylesinger_oracle as O
-from tests import kstep_oracle as KO
 from tests.common import acoustic_sd64
 
 F0_PREFIX = ("gm_diffnet.", "gm_diffnet_inpainte.")  # which = 1 / 2 of ssb_denoiser_eval, 0 / 1 of the F0 sampler
@@ -37,9 +36,9 @@ def ddiffnet64(f0, uv, t, cond, hp, prefix):
         return O.ddiffnet(f0.double(), uv.long(), _t64(t, f0.shape[0]), cond.double(), acoustic_sd64(), hp, prefix)
 
 
-def _gauss64(hp, T, K, max_beta):
-    with KO._first_k_of_schedule(T, K):
-        return {k: v.double() for k, v in O._gauss_tables(K, max_beta).items()}
+def _gauss64(T, K, max_beta):
+    """The first K rows of the T-step schedule's fp32 buffers, as float64 (see O.k_step)."""
+    return {k: v[:K].double() for k, v in O._gauss_tables(T, max_beta).items()}
 
 
 def spec_bounds(hp):
@@ -53,8 +52,7 @@ def mel_chain64(cond, coarse, hp, K, noise):
     cond [F,256], coarse [F,80], noise [K+1, F, 80] (the q_sample draw, then one per step t = K-1 .. 0).
     Returns {"mel": [F,80], "x": [x_K, x_{K-1}, .., x_0] each [F,80] (normalised), "clip": per step t = K-1 .. 0 the
     fraction of x0 predictions with |x0| > 1}."""
-    T = hp["timesteps"]
-    s = _gauss64(hp, T, K, hp["max_beta"])
+    s = _gauss64(hp["timesteps"], K, hp["max_beta"])
     smin, smax = spec_bounds(hp)
     c = cond.double().t()[None]
     nz = noise.double()
@@ -80,7 +78,7 @@ def f0_chain64(cond, lo, hi, hp, prefix, gauss, unif):
     Returns {"z": [z_T, .., z_0], "uv": [uv_T, .., uv_0] (int64 [F]), "margin": per step t = T-1 .. 0 the float64
     |(g1 + logp1) - (g0 + logp0)| of every frame, "clip": per step the fraction of x0 predictions outside [lo, hi]}."""
     T = hp["f0_timesteps"]
-    s = _gauss64(hp, T, T, hp["f0_max_beta"])
+    s = _gauss64(T, T, hp["f0_max_beta"])
     m = {k: v.double() for k, v in O._multi_tables(T, hp["f0_max_beta"]).items()}
     c = cond.double()[None]
     lo, hi = lo.double(), hi.double()

@@ -1,13 +1,13 @@
 """Float64 emulation of the single-pass fp16 tensor-core mode (SSB_TC_FP16, hparams['tc_precision'] = 'fp16').
 
 In that mode every tensor-core contraction multiplies operands rounded once to fp16 and sums the products in fp32.  The
-emulation runs the existing float64 oracles (tests/denoiser_oracle.py, tests/sampler_oracle.py,
-tests/vocoder_layouts_ref.py, tests/conv_gemm_ref.py) with the activation and the weight of each such contraction
-rounded to fp16 and everything else, the sums included, in float64.  fp16_convs() patches torch.nn.functional's conv1d /
-conv_transpose1d for the duration of a block; `select(kind, x, w, stride)` says which calls are tensor-core GEMMs on the
-CUDA path.  A weight is rounded as the tensor-core packer rounds it, fp16(w 2^s) 2^-s with one power of two s per tensor
-(tests/conv_gemm_ref.py plane_exponent): that is fp16(w) for every weight that is a normal fp16 number.  Biases are not
-rounded: the kernels add them in fp32 in the epilogue."""
+emulation runs the existing float64 oracles (tests/denoiser_oracle.py, tests/sampler_oracle.py, the float64 mode of
+oracle/stylesinger_oracle.py's hifigan_generator, tests/conv_gemm_ref.py) with the activation and the weight of each
+such contraction rounded to fp16 and everything else, the sums included, in float64.  fp16_convs() patches
+torch.nn.functional's conv1d / conv_transpose1d for the duration of a block; `select(kind, x, w, stride)` says which
+calls are tensor-core GEMMs on the CUDA path.  A weight is rounded as the tensor-core packer rounds it, fp16(w 2^s) 2^-s
+with one power of two s per tensor (tests/conv_gemm_ref.py plane_exponent): that is fp16(w) for every weight that is a
+normal fp16 number.  Biases are not rounded: the kernels add them in fp32 in the epilogue."""
 import contextlib
 
 import torch

@@ -1,5 +1,4 @@
-"""The ProDiff and PLMS mel samplers in float64, over the test oracles (tests/prodiff_oracle.py,
-oracle/stylesinger_oracle.py through the K-step slicing of tests/kstep_oracle.py).
+"""The ProDiff and PLMS mel samplers in float64, over the test oracle (oracle/stylesinger_oracle.py).
 
 prodiff_chain64 restates ProDiffusion.forward(infer=True) (prodiff.py:204-222) and plms_chain64 the pndm_speedup loop of
 GaussianDiffusion.forward from t = K_step (shallow_diffusion_tts.py:164-197,244-260) step by step in float64, on the
@@ -10,26 +9,11 @@ output, and for PLMS the history order each step used.  Noise comes in the C ABI
 tests/test_sampler_f64_cpu.py pins both against the reference fixtures and the fp32 oracles."""
 import torch
 
-from stylesinger_b200 import synth
-from stylesinger_b200.hparams import resolve
+from oracle import stylesinger_oracle as O
 from tests import denoiser_oracle as DO
-from tests import prodiff_oracle as PO
-from tests.common import golden
+from tests.common import prodiff_sd
 
 _C = {}
-
-
-def prodiff_hp(T=None):
-    """The ProDiff model of tests/golden/ref_prodiff_T8.npz (decoder 'prodiff', schedule 'vpsde') at T steps (8)."""
-    _, meta = golden("ref_prodiff_T8")
-    T = meta["T"] if T is None else T
-    return resolve(timesteps=T, K_step=T, f0_timesteps=meta["f0_T"], **meta["overrides"])
-
-
-def prodiff_sd():
-    if "sd" not in _C:
-        _C["sd"] = synth.acoustic_state_dict(prodiff_hp(), seed=0)
-    return _C["sd"]
 
 
 def prodiff_sd64():
@@ -59,13 +43,13 @@ def _prodiff_chain64(cond, hp, noise):
     plus exp(0.5 logvar) noise; denorm_spec is the identity.
     Returns {"mel": [B,F,80], "x": [x_T, .., x_0], "x0": per step t = T-1 .. 0 the denoiser output}."""
     T = hp["timesteps"]
-    s = {k: v.double() for k, v in PO.prodiff_tables(T).items()}
+    s = {k: v.double() for k, v in O.prodiff_tables(T).items()}
     c = cond.double().transpose(1, 2)
     nz = noise.double()
     x = nz[0]
     xs, x0s = [x], []
     for k, i in enumerate(reversed(range(T))):
-        x0 = _eval(x, i, c, hp, prodiff_sd64(), PO.PREFIX)
+        x0 = _eval(x, i, c, hp, prodiff_sd64(), O.PRODIFF_PREFIX)
         x0s.append(x0)
         mean = s["posterior_mean_coef1"][i] * x0 + s["posterior_mean_coef2"][i] * x
         x = mean + (0.0 if i == 0 else 1.0) * (0.5 * s["posterior_log_variance_clipped"][i]).exp() * nz[k + 1]
@@ -98,7 +82,7 @@ def _plms_chain64(cond, coarse, hp, K, interval, q_noise):
     "calls": every denoiser evaluation as (t, input x), "order": per step the number of history entries used (0: the
     second-order start)}."""
     T = hp["timesteps"]
-    s = DO._gauss64(hp, T, K, hp["max_beta"])
+    s = DO._gauss64(T, K, hp["max_beta"])
     ac = s["alphas_cumprod"]
     smin, smax = DO.spec_bounds(hp)
     c = cond.double().transpose(1, 2)

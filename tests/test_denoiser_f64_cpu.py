@@ -6,7 +6,6 @@ import torch
 
 from oracle import stylesinger_oracle as O
 from tests import denoiser_oracle as DO
-from tests import kstep_oracle as KO
 from tests.common import acoustic_sd, golden, hp_for, utt_from_meta
 
 TOL = 2e-5  # the fp32 oracle's bar against the reference (tests/test_oracle_golden.py)
@@ -49,7 +48,7 @@ def test_mel_chain64_matches_fp32_oracle(T, K):
     ns = O.NoiseSource(7 + K)
     ns.record = []
     with torch.no_grad():
-        mel32, steps = KO.mel_diffusion_sample(cond[None], coarse[None], acoustic_sd(), hp, ns, return_steps=True)
+        mel32, steps = O.mel_diffusion_sample(cond[None], coarse[None], acoustic_sd(), hp, ns, return_steps=True)
     noise = torch.stack([n[0, 0].t() for n in ns.record])
     assert noise.shape == (K + 1, 70, 80)
     r = DO.mel_chain64(cond, coarse, hp, K, noise)

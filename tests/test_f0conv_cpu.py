@@ -1,4 +1,4 @@
-"""Convolutional F0 generator (hparams['f0_gen'] == 'conv'), CPU side: the test oracle's restatement and the synthetic
+"""Convolutional F0 generator (hparams['f0_gen'] == 'conv'), CPU side: the test oracle and the synthetic
 checkpoint against the unmodified reference (tests/golden/ref_convf0.npz), the hparams rules, and the C ABI's argument
 check (no GPU needed)."""
 import ctypes as C
@@ -10,8 +10,7 @@ import torch
 from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
 from stylesinger_b200.hparams import resolve
-from tests import f0conv_oracle as FO
-from tests.common import golden, hp_for, utt_from_meta
+from tests.common import conv_hp, conv_sd, golden, hp_for, predictor_inputs, utt_from_meta
 
 TOL = 2e-5  # fp32 CPU, same op order up to BLAS blocking (as tests/test_oracle_golden.py)
 
@@ -24,10 +23,10 @@ def _forward(meta, seed, use_mel2ph=True):
     u = utt_from_meta(meta)
     ns = O.NoiseSource(seed)
     with torch.no_grad():
-        r = FO.stylesinger_forward(FO.conv_sd(meta), FO.conv_hp(meta), u["txt_tokens"][None], u["note"][None],
-                                   u["note_dur"][None], u["note_type"][None], u["spk_embed"][None],
-                                   u["emo_embed"][None], u["ref_mels"][None], u["ref_f0"], ns,
-                                   mel2ph=u["mel2ph"][None] if use_mel2ph else None)
+        r = O.stylesinger_forward(conv_sd(meta), conv_hp(meta), u["txt_tokens"][None], u["note"][None],
+                                  u["note_dur"][None], u["note_type"][None], u["spk_embed"][None],
+                                  u["emo_embed"][None], u["ref_mels"][None], u["ref_f0"], ns,
+                                  mel2ph=u["mel2ph"][None] if use_mel2ph else None)
     return r, ns
 
 
@@ -56,13 +55,13 @@ def test_fixture_exercises_the_quantiser_and_both_uv_classes():
 
 def test_oracle_predictors_match_reference():
     g, meta = golden("ref_convf0")
-    xs = FO.predictor_inputs(meta)
+    xs = predictor_inputs(meta)
     assert np.array_equal(xs[:, :4].numpy(), g["pred_x_head"])  # the regenerated inputs are the reference's
     assert (xs[:, meta["pred_zero_rows"], 0] == 0).all()
-    sd = FO.conv_sd(meta)
+    sd = conv_sd(meta)
     with torch.no_grad():
         for which, key in ((0, "pred_out_agnostic"), (1, "pred_out_specific")):
-            out = FO.pitch_predictor(xs[which][None], sd, which)[0]
+            out = O.pitch_predictor(xs[which][None], sd, which)[0]
             err = _maxabs(out.numpy(), g[key])
             print(key, "L-inf", err)
             assert err < TOL, (key, err)
@@ -102,7 +101,7 @@ def test_oracle_prodiff_with_conv_f0_matches_reference():
 def test_synth_conv_state_dicts_have_the_reference_keys_and_shapes():
     g, meta = golden("ref_convf0")
     for m in (meta, meta["prodiff"]):
-        sd = FO.conv_sd(m)
+        sd = conv_sd(m)
         assert [[k, list(v.shape)] for k, v in sd.items()] == m["state_dict"]
         assert not any(k.startswith(("gm_diffnet", "f0_gen")) for k in sd)
         assert sum(k.startswith("pitch_inpainter_predictor.") for k in sd) == 24

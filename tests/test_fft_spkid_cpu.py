@@ -11,9 +11,7 @@ from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
 from stylesinger_b200.engine import pack_batch
 from stylesinger_b200.hparams import resolve
-from tests import fft_spkid_oracle as FO
-from tests import switches_oracle as SO
-from tests.common import golden, utt_from_meta
+from tests.common import fft_spkid_hp, fft_spkid_sd, golden, switch_sd, utt_from_meta
 
 TOL = 2e-5  # fp32 CPU, same op order up to BLAS blocking (as tests/test_switches_cpu.py)
 CONFIGS = ("fft_gmdiff", "fft_conv", "spkid_diffsinger", "spkid_fft", "fft_no_emo_style")
@@ -34,13 +32,13 @@ def _spk(meta, hp, u):
 
 def _forward(meta, c, seed, use_mel2ph=True):
     cfg = _cfg(meta, c)
-    hp = FO.switch_hp(cfg)
+    hp = fft_spkid_hp(cfg)
     u = utt_from_meta(meta)
     ns = O.NoiseSource(seed)
     with torch.no_grad():
-        r = FO.stylesinger_forward(FO.switch_sd(cfg), hp, u["txt_tokens"][None], u["note"][None], u["note_dur"][None],
-                                   u["note_type"][None], _spk(meta, hp, u), u["emo_embed"][None], u["ref_mels"][None],
-                                   u["ref_f0"], ns, mel2ph=u["mel2ph"][None] if use_mel2ph else None)
+        r = O.stylesinger_forward(fft_spkid_sd(cfg), hp, u["txt_tokens"][None], u["note"][None], u["note_dur"][None],
+                                  u["note_type"][None], _spk(meta, hp, u), u["emo_embed"][None], u["ref_mels"][None],
+                                  u["ref_f0"], ns, mel2ph=u["mel2ph"][None] if use_mel2ph else None)
     return r, ns
 
 
@@ -49,7 +47,7 @@ def test_fixture_covers_every_configuration():
     assert tuple(meta["configs"]) == CONFIGS
     seen = set()
     for c in CONFIGS:
-        hp = FO.switch_hp(_cfg(meta, c))
+        hp = fft_spkid_hp(_cfg(meta, c))
         seen.add((hp["decoder"], hp["f0_gen"], hp["use_spk_id"], hp["emo"] and hp["style"]))
         assert (f"{c}/style" in g.files) == hp["style"] and (f"{c}/emo_embed" in g.files) == hp["emo"]
         assert (f"{c}/coarse_mel" in g.files) == (hp["decoder"] == "diffsinger")
@@ -57,7 +55,7 @@ def test_fixture_covers_every_configuration():
     for want in (("fft", "gmdiff", False, True), ("fft", "conv", False, True), ("diffsinger", "gmdiff", True, True),
                  ("fft", "gmdiff", True, True), ("fft", "gmdiff", False, False)):
         assert want in seen, want
-    assert FO.switch_hp(_cfg(meta, meta["dur_config"]))["use_spk_id"]
+    assert fft_spkid_hp(_cfg(meta, meta["dur_config"]))["use_spk_id"]
 
 
 @pytest.mark.parametrize("c", CONFIGS)
@@ -75,7 +73,7 @@ def test_oracle_forward_matches_reference(c):
     assert errs["f0_denorm(Hz)"] < 1e-3
     if f"{c}/rq_codes" in g.files:
         assert np.array_equal(r["rq_codes"][0].numpy(), g[f"{c}/rq_codes"])  # RVQ indices: bit-exact
-    if FO.switch_hp(_cfg(meta, c))["decoder"] == "fft":
+    if fft_spkid_hp(_cfg(meta, c))["decoder"] == "fft":
         assert "coarse_mel" not in r and "diff_cond" not in r
 
 
@@ -92,29 +90,13 @@ def test_oracle_duration_path_matches_reference():
     assert _maxabs(r["f0_denorm"][0].numpy(), g[f"{c}/dur_f0_denorm"]) < 1e-3
 
 
-@pytest.mark.parametrize("ov", [{}, {"emo": False, "style": False}, {"f0_gen": "conv"}])
-def test_oracle_without_either_option_is_the_switches_oracle(ov):
-    """Neither option: the restatement is tests/switches_oracle.py's forward, bit for bit."""
-    cfg = {"T": 4, "overrides": ov}
-    hp, sd = SO.switch_hp(cfg), SO.switch_sd(cfg)
-    u = synth.make_utterance(0.2, utt_idx=3, ref_frames=24, frames=24, phones=4)
-    args = (u["txt_tokens"][None], u["note"][None], u["note_dur"][None], u["note_type"][None], u["spk_embed"][None],
-            u["emo_embed"][None], u["ref_mels"][None], u["ref_f0"])
-    with torch.no_grad():
-        a = SO.stylesinger_forward(sd, hp, *args, O.NoiseSource(9), mel2ph=u["mel2ph"][None])
-        b = FO.stylesinger_forward(sd, hp, *args, O.NoiseSource(9), mel2ph=u["mel2ph"][None])
-    assert set(a) == set(b)
-    for k in a:
-        assert torch.equal(a[k], b[k]), k
-
-
 @pytest.mark.parametrize("c", CONFIGS)
 def test_synth_keys_and_shapes_are_the_references(c):
     _, meta = golden("ref_fft_spkid")
-    hp = FO.switch_hp(_cfg(meta, c))
+    hp = fft_spkid_hp(_cfg(meta, c))
     ref = [[k, list(s)] for k, s in meta["configs"][c]["state_dict"]]
     assert [[k, list(s)] for k, s in synth.acoustic_param_shapes(hp)] == ref
-    sd = FO.switch_sd(_cfg(meta, c))
+    sd = fft_spkid_sd(_cfg(meta, c))
     assert [[k, list(v.shape)] for k, v in sd.items()] == ref
     keys = set(sd)
     if hp["decoder"] == "fft":
@@ -127,7 +109,7 @@ def test_default_synthetic_checkpoint_is_byte_identical_to_the_switch_configurat
     """The options off leave the synthetic checkpoints as they were: the default one and an emo-off one equal, tensor for
     tensor, those built with the options spelled out."""
     for ov in ({}, {"emo": False}):
-        a = SO.switch_sd({"T": 4, "overrides": ov})
+        a = switch_sd({"T": 4, "overrides": ov})
         b = synth.acoustic_state_dict(resolve(timesteps=4, K_step=4, f0_timesteps=4, decoder="diffsinger",
                                               use_spk_id=False, use_spk_embed=True, **ov), seed=0)
         assert list(a) == list(b) and all(torch.equal(a[k], b[k]) for k in a)

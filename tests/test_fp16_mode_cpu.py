@@ -115,15 +115,15 @@ def test_vocoder_emulation_is_near_the_fp32_generator():
     """HiFi-GAN V3 (the smallest layout) under the emulation: the ups and ResBlock convs rounded, conv_pre / conv_post /
     noise convs not; the waveform stays within the size of the fp16 rounding of the float64 generator's."""
     from oracle import stylesinger_oracle as O
-    from tests import vocoder_layouts_ref as VR
+    from tests.common import VOCODER_LAYOUTS, vocoder_sd
     g = torch.Generator().manual_seed(5)
     F_ = 12
     mel = (-3.0 + torch.randn(F_, 80, generator=g)).clamp(-6, 1.5).numpy()
     f0 = (150 + 350 * torch.rand(F_, generator=g)).numpy()
-    sd, h = VR.state_dict("v3"), VR.LAYOUTS["v3"]
-    ref = VR.spec2wav(mel, f0, sd, h, O.NoiseSource(3), torch.float64)
+    sd, h = vocoder_sd("v3"), VOCODER_LAYOUTS["v3"]
+    ref = O.spec2wav(mel, f0, sd, h, O.NoiseSource(3), torch.float64)
     with E.fp16_convs(E.vocoder_tc_conv) as n:
-        emu = VR.spec2wav(mel, f0, sd, h, O.NoiseSource(3), torch.float64)
+        emu = O.spec2wav(mel, f0, sd, h, O.NoiseSource(3), torch.float64)
     assert n["rounded"] == 3 + 3 * 3 * 2 and n["kept"] == 2 + 3  # ups + ResBlock2 convs; conv_pre, conv_post, noise convs
     d = float(np.abs(emu - ref).max())
     print(f"vocoder v3 emulation vs float64: L-inf {d:.2e}")

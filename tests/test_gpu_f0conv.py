@@ -1,6 +1,6 @@
 """Convolutional F0 generator (f0_gen 'conv') on the GPU, through the C ABI: ssb_model_create_ex2(..., SSB_F0_GEN_CONV),
 ssb_pitch_predictor and ssb_acoustic_forward on a conv model, against the unmodified reference's fixture
-(tests/golden/ref_convf0.npz) and a float64 restatement (tests/f0conv_oracle.py).  Bars, fixed before measuring and the
+(tests/golden/ref_convf0.npz) and the test oracle's pitch predictors in float64.  Bars, fixed before measuring and the
 same as the existing tests': pitch_pred / decoder_inp < 1e-4, f0_denorm < 5e-2 Hz, mel_out < 1e-3 (DiffSinger T=4, as
 tests/test_gpu_parity.py), ProDiff mel < 1e-4 max(1, |mel|) on fp32 and < 1e-3 max(1, |mel|) on tensor cores (as
 tests/test_gpu_prodiff.py), each predictor alone < 1e-4; coarse bins and uv exact against the fixture."""
@@ -11,8 +11,7 @@ import torch
 from oracle import stylesinger_oracle as O
 from stylesinger_b200 import _lib
 from stylesinger_b200._lib import SsbError
-from tests import f0conv_oracle as FO
-from tests.common import acoustic_engine, golden, utt_from_meta
+from tests.common import acoustic_engine, conv_hp, conv_sd, golden, predictor_inputs, utt_from_meta
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -40,7 +39,7 @@ def conv_engine(prodiff=False):
     m_meta = meta["prodiff"] if prodiff else meta
     key = "pd" if prodiff else "ds"
     if key not in _C:
-        _C[key] = AcousticModel(FO.conv_sd(m_meta), FO.conv_hp(m_meta))
+        _C[key] = AcousticModel(conv_sd(m_meta), conv_hp(m_meta))
     m = _C[key]
     m.set_tensor_cores(True)
     m.set_persistent(True)
@@ -119,7 +118,7 @@ def test_each_predictor_matches_reference_golden(tc):
     """B=1 at 300 frames takes the fp32 path whatever the switch says (3 row tiles < 8)."""
     g, meta = _fixture()
     m = conv_engine()
-    xs = FO.predictor_inputs(meta)
+    xs = predictor_inputs(meta)
     offs = np.array([0, xs.shape[1]], np.int32)
     try:
         m.set_tensor_cores(tc)
@@ -145,12 +144,12 @@ def _ragged_lengths(total=20000, seed=3):
 
 def _reference_f64(x, offs, sd, which):
     """float64 PitchPredictor per utterance (B=1 each), on the GPU for speed (test-side reference only)."""
-    sd64 = {k: v.to(DEV) for k, v in sd.items() if k.startswith(FO.PREFIXES[which])}
+    sd64 = {k: v.to(DEV) for k, v in sd.items() if k.startswith(O.PITCH_PREDICTORS[which])}
     out = []
     with torch.no_grad():
         for b in range(len(offs) - 1):
             a, e = int(offs[b]), int(offs[b + 1])
-            out.append(FO.pitch_predictor(x[None, a:e].to(DEV), sd64, which, dtype=torch.float64)[0])
+            out.append(O.pitch_predictor(x[None, a:e].to(DEV), sd64, which, dtype=torch.float64)[0])
     return torch.cat(out)
 
 
@@ -173,7 +172,7 @@ def _near_edge_flips(ref_pp, our_pp, bar):
 def test_ragged_batch_vs_float64_and_b1(tc):
     g, meta = _fixture()
     m = conv_engine()
-    sd = FO.conv_sd(meta)
+    sd = conv_sd(meta)
     lens = _ragged_lengths()
     offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
     tiles = sum((n + 127) // 128 for n in lens)

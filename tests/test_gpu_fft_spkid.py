@@ -11,8 +11,7 @@ import torch
 
 from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
-from tests import fft_spkid_oracle as FO
-from tests.common import engine_noise_from_stream, golden, utt_from_meta
+from tests.common import engine_noise_from_stream, fft_spkid_hp, fft_spkid_sd, golden, utt_from_meta
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -52,7 +51,7 @@ def _model(c, T=None):
     from stylesinger_b200.engine import AcousticModel
     key = (c, T)
     if key not in _C:
-        _C[key] = AcousticModel(FO.switch_sd(_cfg(c, T)), FO.switch_hp(_cfg(c, T)), DEV)
+        _C[key] = AcousticModel(fft_spkid_sd(_cfg(c, T)), fft_spkid_hp(_cfg(c, T)), DEV)
     m = _C[key]
     m.set_tensor_cores(True)
     m.set_persistent(True)
@@ -129,7 +128,7 @@ def test_forward_matches_reference_golden(c, tc):
 
 
 def m_table(c):
-    return FO.switch_sd(_cfg(c))["spk_embed_proj.weight"]
+    return fft_spkid_sd(_cfg(c))["spk_embed_proj.weight"]
 
 
 def test_duration_path_matches_reference_golden():
@@ -184,7 +183,7 @@ def test_ragged_batch_at_bench_lengths_matches_oracle(c):
     out = m.forward(pb, noise=noise, want=("mel_out", "decoder_inp", "pitch_pred", "f0_denorm"))
     torch.cuda.synchronize()
     fo = pb.frame_offsets
-    sd = FO.switch_sd(_cfg(c, T))
+    sd = fft_spkid_sd(_cfg(c, T))
     sd64 = {k: v.double() for k, v in sd.items()}
     worst = {"decoder_inp": 0.0, "pitch_pred": 0.0, "mel_out(own decoder_inp)": 0.0}
     f64 = hp["f0_gen"] == "conv"
@@ -193,10 +192,10 @@ def test_ragged_batch_at_bench_lengths_matches_oracle(c):
         u = utts[i]
         d = (lambda x: x.double()) if f64 else (lambda x: x)
         with torch.no_grad():
-            r = FO.stylesinger_forward(sd64 if f64 else sd, hp, u["txt_tokens"][None], u["note"][None],
-                                       d(u["note_dur"][None]), u["note_type"][None], d(u["spk_embed"][None]),
-                                       d(u["emo_embed"][None]), d(u["ref_mels"][None]), d(u["ref_f0"]),
-                                       _Noise64(300 + i) if f64 else O.NoiseSource(300 + i), mel2ph=u["mel2ph"][None])
+            r = O.stylesinger_forward(sd64 if f64 else sd, hp, u["txt_tokens"][None], u["note"][None],
+                                      d(u["note_dur"][None]), u["note_type"][None], d(u["spk_embed"][None]),
+                                      d(u["emo_embed"][None]), d(u["ref_mels"][None]), d(u["ref_f0"]),
+                                      _Noise64(300 + i) if f64 else O.NoiseSource(300 + i), mel2ph=u["mel2ph"][None])
         # a coarse pitch bin decided the other way (f0 within rounding of a bin edge) changes that frame's pitch_embed row:
         # decoder_inp is compared on the frames whose bins agree, and at most 2 may disagree
         bins = O.f0_to_coarse(out["f0_denorm"][fo[i]:fo[i + 1]].double().cpu()).reshape(-1)
@@ -227,9 +226,9 @@ def test_fft_model_is_the_diffsinger_models_coarse_mel(f0_gen):
     noise (short batches on FFMA, a long one on the tensor-core decoder path)."""
     from stylesinger_b200.engine import AcousticModel
     T = 4
-    hp_d = FO.switch_hp({"T": T, "overrides": {"f0_gen": f0_gen}})
-    hp_f = FO.switch_hp({"T": T, "overrides": {"f0_gen": f0_gen, "decoder": "fft"}})
-    sd_d = FO.switch_sd({"T": T, "overrides": {"f0_gen": f0_gen}})
+    hp_d = fft_spkid_hp({"T": T, "overrides": {"f0_gen": f0_gen}})
+    hp_f = fft_spkid_hp({"T": T, "overrides": {"f0_gen": f0_gen, "decoder": "fft"}})
+    sd_d = fft_spkid_sd({"T": T, "overrides": {"f0_gen": f0_gen}})
     a = AcousticModel(sd_d, hp_d, DEV)
     b = AcousticModel(_drop(sd_d, ("postdiff.", "ln_proj.")), hp_f, DEV)
     for utts in ([synth.make_utterance(0.3 + 0.2 * i, utt_idx=i, ref_frames=40 + 9 * i) for i in range(3)], _bench_utts(8)):
@@ -253,9 +252,9 @@ def test_speaker_table_equals_the_linear_projection(dec):
     from stylesinger_b200.engine import AcousticModel
     T = 4
     ov = {"decoder": dec, **({"schedule_type": "vpsde"} if dec == "prodiff" else {})}
-    hp = FO.switch_hp({"T": T, "overrides": ov})
-    hp_id = FO.switch_hp({"T": T, "overrides": dict(ov, use_spk_id=True)})
-    sd = FO.switch_sd({"T": T, "overrides": ov})
+    hp = fft_spkid_hp({"T": T, "overrides": ov})
+    hp_id = fft_spkid_hp({"T": T, "overrides": dict(ov, use_spk_id=True)})
+    sd = fft_spkid_sd({"T": T, "overrides": ov})
     lin = AcousticModel(sd, hp, DEV)
     utts = [synth.make_utterance(0.3 + 0.1 * i, utt_idx=20 + i, ref_frames=40) for i in range(4)]
     ids = [5, 150, 0, 77]
@@ -342,7 +341,7 @@ def test_documented_errors_launch_nothing():
     # a table whose rows do not match num_spk
     from stylesinger_b200.engine import AcousticModel
     with pytest.raises(ValueError, match="num_spk"):
-        AcousticModel(FO.switch_sd(_cfg("spkid_fft")), dict(FO.switch_hp(_cfg("spkid_fft")), num_spk=20), DEV)
+        AcousticModel(fft_spkid_sd(_cfg("spkid_fft")), dict(fft_spkid_hp(_cfg("spkid_fft")), num_spk=20), DEV)
 
 
 @pytest.mark.parametrize("c", ["fft_gmdiff", "spkid_diffsinger", "spkid_fft"])
@@ -392,8 +391,8 @@ def test_padding_frames_are_zero_and_dropped_before_the_vocoder():
     StyleSingerInfer drops them before the vocoder, as the reference drops all-zero frames (inference/StyleSinger.py:56-62)."""
     from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG
     from stylesinger_b200.infer import StyleSingerInfer
-    hp = FO.switch_hp({"T": 4, "overrides": {"decoder": "fft", "f0_gen": "conv"}})
-    inf = StyleSingerInfer(hp, DEV, FO.switch_sd({"T": 4, "overrides": {"decoder": "fft", "f0_gen": "conv"}}),
+    hp = fft_spkid_hp({"T": 4, "overrides": {"decoder": "fft", "f0_gen": "conv"}})
+    inf = StyleSingerInfer(hp, DEV, fft_spkid_sd({"T": 4, "overrides": {"decoder": "fft", "f0_gen": "conv"}}),
                            synth.vocoder_state_dict(DEFAULT_VOCODER_CONFIG, seed=0), DEFAULT_VOCODER_CONFIG)
     utts = [synth.make_utterance(0.5 + 0.2 * i, utt_idx=30 + i, ref_frames=48) for i in range(2)]
     for u in utts:

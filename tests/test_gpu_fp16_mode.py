@@ -183,6 +183,7 @@ def test_mel_sampler_fp16_matches_emulation(name, K, T):
 
 def test_plms_and_prodiff_fp16_match_emulation():
     from tests import sampler_oracle as SO
+    from tests.common import prodiff_hp, prodiff_sd
     from stylesinger_b200.engine import AcousticModel
     b = D.batch("ragged")
     offs = b["offs"]
@@ -209,8 +210,8 @@ def test_plms_and_prodiff_fp16_match_emulation():
         print(f"plms utt {i} fp16: L-inf vs emulation {e_emu:.2e}, vs float64 {e_gpu:.2e} (emulation {e_ref:.2e})")
         assert e_gpu <= 2 * e_ref and e_emu <= e_ref
     # ProDiff, T = 4, injected noise, persistent kernel
-    hpp = SO.prodiff_hp(4)
-    pm = AcousticModel(SO.prodiff_sd(), hpp)
+    hpp = prodiff_hp(4)
+    pm = AcousticModel(prodiff_sd(), hpp)
     pm.set_mel_precision("fp16")
     noise = D._mel_noise(4, int(offs[-1]), 93)
     mel = pm.mel_prodiff(b["cond"], offs, noise.to(DEV)).clone()
@@ -233,18 +234,17 @@ def test_vocoder_fp16_matches_emulation(name):
     from stylesinger_b200.engine import Vocoder
     from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG
     from tests import test_gpu_vocoder_layouts as VL
-    from tests import vocoder_layouts_ref as VR
-    from tests.common import vocoder_sd
-    h = DEFAULT_VOCODER_CONFIG if name == "v1" else VR.LAYOUTS[name]
-    sd = vocoder_sd() if name == "v1" else VR.state_dict(name)
+    from tests.common import VOCODER_LAYOUTS, vocoder_sd
+    h = DEFAULT_VOCODER_CONFIG if name == "v1" else VOCODER_LAYOUTS[name]
+    sd = vocoder_sd(None if name == "v1" else name)
     v = Vocoder(sd, h, tc_precision="fp16")
     utts = [VL.Utt(*VL._synth_utt(L, 40 + L), 40 + L) for L in (1, 37, 128, 400)]
     wav, variants, _ = launched(lambda: VL._generate(v, utts))
     assert variants and all(",fp16>" in k for k in variants), variants
     for u, w in zip(utts, VL._split(wav, utts)):
-        ref = VR.spec2wav(u.mel, u.f0, sd, h, O.NoiseSource(u.seed), torch.float64)
+        ref = O.spec2wav(u.mel, u.f0, sd, h, O.NoiseSource(u.seed), torch.float64)
         with E.fp16_convs(E.vocoder_tc_conv):
-            emu = VR.spec2wav(u.mel, u.f0, sd, h, O.NoiseSource(u.seed), torch.float64)
+            emu = O.spec2wav(u.mel, u.f0, sd, h, O.NoiseSource(u.seed), torch.float64)
         e_emu, e_gpu, e_ref = _linf(w, emu), _linf(w, ref), _linf(emu, ref)
         print(f"vocoder {name} L={u.L} fp16: wav L-inf vs emulation {e_emu:.2e}, vs float64 {e_gpu:.2e} "
               f"(emulation {e_ref:.2e})")

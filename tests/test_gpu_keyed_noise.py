@@ -16,9 +16,8 @@ import torch
 from stylesinger_b200 import synth
 from stylesinger_b200.engine import AcousticModel, Vocoder, pack_batch
 from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG, resolve
-from tests import f0conv_oracle as FO
 from tests import keyed_plan as K
-from tests.common import acoustic_sd, golden, hp_for, vocoder_sd
+from tests.common import acoustic_sd, conv_hp, conv_sd, golden, hp_for, vocoder_sd
 from tests.test_gpu_philox import TOL, _probe_schedule, _real_schedule
 
 pytestmark = pytest.mark.gpu
@@ -42,7 +41,7 @@ def _model(kind="diffsinger", T=8):
             _M[key] = AcousticModel(synth.acoustic_state_dict(hp, seed=0), hp)
         elif kind == "conv":
             _, meta = golden("ref_convf0")
-            _M[key] = AcousticModel(FO.conv_sd(meta), FO.conv_hp(meta))
+            _M[key] = AcousticModel(conv_sd(meta), conv_hp(meta))
         else:
             # positions for the 6300-frame utterance of test_keyed_draws_are_the_solo_draws_and_the_plan
             _M[key] = AcousticModel(acoustic_sd(), hp_for(T, T), max_positions=8192)

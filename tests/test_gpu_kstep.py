@@ -1,7 +1,7 @@
 """Shallow diffusion on the GPU: hparams['K_step'] < timesteps (ssb_model_set_mel_k_step) through ssb_acoustic_forward,
 ssb_mel_diffusion_sample (persistent single-launch, per-launch tensor-core and fp32 FFMA paths, persistent groups) and
-ssb_mel_diffusion_sample_plms, against the unmodified reference's fixture (tests/golden/ref_kstep.npz) and the K-step
-oracle (tests/kstep_oracle.py).  Bars, fixed before measuring: mel L-inf < 1e-3 for the DDPM sampler (the bar of the T=25
+ssb_mel_diffusion_sample_plms, against the unmodified reference's fixture (tests/golden/ref_kstep.npz) and the test
+oracle.  Bars, fixed before measuring: mel L-inf < 1e-3 for the DDPM sampler (the bar of the T=25
 forward test), 1e-4 max(1, |mel|) on FFMA and 1e-3 max(1, |mel|) on tensor cores for PLMS (as the PLMS / ProDiff tests);
 style, pitch and decoder_inp as tests/test_gpu_parity.py."""
 import ctypes as C
@@ -12,7 +12,6 @@ import torch
 
 from oracle import stylesinger_oracle as O
 from stylesinger_b200._lib import SsbError, lib
-from tests import kstep_oracle as KO
 from tests.common import acoustic_sd, engine_noise_from_stream, golden, hp_for, utt_from_meta
 
 pytestmark = pytest.mark.gpu
@@ -347,7 +346,7 @@ def test_k_step_errors():
 
 # ---------------------------------------------------------------------------------------------------
 def test_inference_driver_reads_k_step_from_hparams():
-    """StyleSingerInfer with hparams K_step 51 (timesteps 100) against the K-step oracle on the same injected draws."""
+    """StyleSingerInfer with hparams K_step 51 (timesteps 100) against the oracle on the same injected draws."""
     from stylesinger_b200 import synth
     from stylesinger_b200.engine import pack_batch
     from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG, resolve
@@ -359,9 +358,9 @@ def test_inference_driver_reads_k_step_from_hparams():
     Fr = u["mel2ph"].shape[0]
     ns = O.NoiseSource(seed)
     with torch.no_grad():
-        r = KO.stylesinger_forward(acoustic_sd(), hp, u["txt_tokens"][None], u["note"][None], u["note_dur"][None],
-                                   u["note_type"][None], u["spk_embed"][None], u["emo_embed"][None], u["ref_mels"][None],
-                                   u["ref_f0"], ns, mel2ph=u["mel2ph"][None])
+        r = O.stylesinger_forward(acoustic_sd(), hp, u["txt_tokens"][None], u["note"][None], u["note_dur"][None],
+                                  u["note_type"][None], u["spk_embed"][None], u["emo_embed"][None], u["ref_mels"][None],
+                                  u["ref_f0"], ns, mel2ph=u["mel2ph"][None])
     noise, ns2 = engine_noise_from_stream(seed, f0_T, K, Fr, DEV)
     assert ns2.log == ns.log  # the oracle consumed exactly the draws handed to the engine
     drv = StyleSingerInfer(hp, DEV, acoustic_sd(), vocoder_sd(), DEFAULT_VOCODER_CONFIG)
@@ -369,5 +368,5 @@ def test_inference_driver_reads_k_step_from_hparams():
     mel, _, wav, _ = drv.run_device(pack_batch([u]).to(DEV), seed=seed, noise=noise)
     torch.cuda.synchronize()
     err = _maxabs(mel, r["mel_out"][0])
-    print(f"StyleSingerInfer, timesteps {T}, K_step {K}: mel_out L-inf vs K-step oracle {err:.3e}; wav {tuple(wav.shape)}")
+    print(f"StyleSingerInfer, timesteps {T}, K_step {K}: mel_out L-inf vs oracle {err:.3e}; wav {tuple(wav.shape)}")
     assert err < 1e-3 and torch.isfinite(wav).all()

@@ -1,17 +1,14 @@
 """ProDiff teacher mel decoder on the GPU: the CUDA path (ssb_model_create_ex(..., SSB_MEL_DECODER_PRODIFF),
 ssb_mel_prodiff_sample, ssb_acoustic_forward on a ProDiff model) against the unmodified reference's fixture
-(tests/golden/ref_prodiff_T8.npz) and the test oracle (tests/prodiff_oracle.py).  Bars, fixed before measuring and the
+(tests/golden/ref_prodiff_T8.npz) and the test oracle.  Bars, fixed before measuring and the
 same as the PLMS sampler's: mel L-inf < 1e-4 max(1, |mel|) on the fp32 FFMA path, < 1e-3 max(1, |mel|) on tensor cores."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import stylesinger_oracle as O
-from stylesinger_b200 import synth
 from stylesinger_b200._lib import SsbError
-from stylesinger_b200.hparams import resolve
-from tests import prodiff_oracle as PO
-from tests.common import acoustic_engine, engine_noise_from_stream, golden, utt_from_meta
+from tests.common import acoustic_engine, engine_noise_from_stream, golden, prodiff_hp, prodiff_sd, utt_from_meta
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -31,17 +28,6 @@ def _meta():
     if "g" not in _C:
         _C["g"], _C["meta"] = golden("ref_prodiff_T8")
     return _C["g"], _C["meta"]
-
-
-def prodiff_hp():
-    _, meta = _meta()
-    return resolve(timesteps=meta["T"], K_step=meta["T"], f0_timesteps=meta["f0_T"], **meta["overrides"])
-
-
-def prodiff_sd():
-    if "sd" not in _C:
-        _C["sd"] = synth.acoustic_state_dict(prodiff_hp(), seed=0)
-    return _C["sd"]
 
 
 def prodiff_engine():
@@ -135,8 +121,8 @@ def test_prodiff_ragged_batch_vs_b1_oracle():
     for b in range(3):
         a, e = int(offs[b]), int(offs[b + 1])
         with torch.no_grad():
-            ref = PO.mel_prodiff_sample(cond[None, a:e], prodiff_sd(), hp,
-                                        ListNoise([noise[k, a:e].t().contiguous()[None, None] for k in range(T + 1)]))
+            ref = O.mel_prodiff_sample(cond[None, a:e], prodiff_sd(), hp,
+                                       ListNoise([noise[k, a:e].t().contiguous()[None, None] for k in range(T + 1)]))
         sc = max(1.0, float(ref.abs().max()))
         err = _maxabs(mel[a:e], ref[0])
         print(f"utterance {b} ({lens[b]} frames): L-inf vs B=1 oracle {err:.3e} (bar {1e-3 * sc:.1e})")

@@ -38,7 +38,7 @@ import torch
 from tests import philox_ref as P
 from tests import sampler_oracle as SO
 from tests import test_gpu_denoisers as D
-from tests.common import acoustic_engine, acoustic_sd, hp_for
+from tests.common import acoustic_engine, acoustic_sd, hp_for, prodiff_hp, prodiff_sd
 from tests.gpu_checks import (Err, check_variants, cond_gemm, count, frame_offsets, launched, net_dims, ntiles, rel,
                               split, step_gemms)
 
@@ -104,7 +104,7 @@ _E, _PB = {}, {}
 def prodiff_engine(T_=8):
     from stylesinger_b200.engine import AcousticModel
     if "m" not in _E:
-        _E["m"] = AcousticModel(SO.prodiff_sd(), SO.prodiff_hp())
+        _E["m"] = AcousticModel(prodiff_sd(), prodiff_hp())
     m = _E["m"]
     m.set_timesteps(T_)
     m.set_tensor_cores(True)
@@ -199,7 +199,7 @@ def _solo(tag, path, lens, offs, ys, run):
 def test_prodiff_sampler_matches_float64(T_, size):
     b = pd_batch(size)
     m = prodiff_engine(T_)
-    hp = SO.prodiff_hp(T_)
+    hp = prodiff_hp(T_)
     lens, offs = b["lens"], b["offs"]
     nt, n = ntiles(lens), int(offs[-1])
     noise = torch.randn(T_ + 1, n, 80, generator=torch.Generator().manual_seed(100 + T_))
@@ -237,7 +237,7 @@ def test_prodiff_philox_matches_float64(size):
     tiles, group g keyed seed + 0x9E3779B97F4A7C15 g with rows counted inside the group."""
     b = pd_batch(size)
     m = prodiff_engine()
-    hp = SO.prodiff_hp()
+    hp = prodiff_hp()
     lens, offs = b["lens"], b["offs"]
     grouped = size == "bench"
     groups = P.persistent_groups(lens) if grouped else [(0, len(lens))]
@@ -386,7 +386,7 @@ def test_forward_prodiff_matches_sampler_and_float64(size):
     """ProDiff forward with a seed and the persistent groups switched on (bench: 21 groups; ragged: one launch)."""
     b = pd_batch(size)
     m = prodiff_engine()
-    hp = SO.prodiff_hp()
+    hp = prodiff_hp()
     lens, offs = b["lens"], b["offs"]
     try:
         m.set_persistent_groups(True)

@@ -10,8 +10,7 @@ import torch
 
 from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
-from tests import switches_oracle as SO
-from tests.common import batch_noise, engine_noise_from_stream, golden, utt_from_meta
+from tests.common import batch_noise, engine_noise_from_stream, golden, switch_hp, switch_sd, utt_from_meta
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -55,7 +54,7 @@ def _model(c, T=None):
     from stylesinger_b200.engine import AcousticModel
     key = (c, T)
     if key not in _C:
-        _C[key] = AcousticModel(SO.switch_sd(_cfg(c, T)), SO.switch_hp(_cfg(c, T)), DEV)
+        _C[key] = AcousticModel(switch_sd(_cfg(c, T)), switch_hp(_cfg(c, T)), DEV)
     m = _C[key]
     m.set_tensor_cores(True)
     m.set_persistent(True)
@@ -152,9 +151,10 @@ def test_ragged_batch_at_bench_lengths_matches_oracle(c):
         u = utts[i]
         ns = O.NoiseSource(300 + i)
         with torch.no_grad():
-            r = SO.stylesinger_forward(SO.switch_sd(_cfg(c, T)), hp, u["txt_tokens"][None], u["note"][None],
-                                       u["note_dur"][None], u["note_type"][None], u["spk_embed"][None],
-                                       u["emo_embed"][None], u["ref_mels"][None], u["ref_f0"], ns, mel2ph=u["mel2ph"][None])
+            r = O.stylesinger_forward(switch_sd(_cfg(c, T)), hp, u["txt_tokens"][None], u["note"][None],
+                                      u["note_dur"][None], u["note_type"][None], u["spk_embed"][None],
+                                      u["emo_embed"][None], u["ref_mels"][None], u["ref_f0"], ns,
+                                      mel2ph=u["mel2ph"][None])
         for k in worst:
             worst[k] = max(worst[k], _maxabs(out[k][fo[i]:fo[i + 1]], r[k][0]))
     print(f"{c}: {len(utts)} utterances, {int(fo[-1])} frames; worst of 3 vs oracle: "
@@ -172,7 +172,7 @@ def test_ragged_batch_at_bench_lengths_matches_oracle(c):
 def test_ex3_with_every_switch_on_is_ex2_bitwise():
     from stylesinger_b200._lib import check, lib
     from stylesinger_b200.engine import AcousticModel
-    hp = SO.switch_hp({"T": 4, "overrides": {}})
+    hp = switch_hp({"T": 4, "overrides": {}})
     sd = synth.acoustic_state_dict(hp, seed=0)
     a = AcousticModel(sd, hp, DEV)  # ex3 (all on)
     b = AcousticModel(sd, hp, DEV)
@@ -241,7 +241,7 @@ def test_style_off_runs_no_aligner_and_no_rvq():
 
 def _model_default():
     from stylesinger_b200.engine import AcousticModel
-    hp = SO.switch_hp({"T": 4, "overrides": {}})
+    hp = switch_hp({"T": 4, "overrides": {}})
     _C["default"] = AcousticModel(synth.acoustic_state_dict(hp, seed=0), hp, DEV)
     return _C["default"]
 
@@ -304,9 +304,9 @@ def test_documented_errors():
         m.rvq(torch.zeros(20, 256, device=DEV), np.array([0, 20], np.int32))
     # a checkpoint whose ln_proj does not match the switches
     from stylesinger_b200.engine import AcousticModel
-    hp = SO.switch_hp(_cfg("no_emo"))
+    hp = switch_hp(_cfg("no_emo"))
     with pytest.raises(SsbError, match=r"ln_proj.weight must be \[256, 848\]"):
-        AcousticModel(synth.acoustic_state_dict(SO.switch_hp({"T": 4, "overrides": {}}), seed=0), hp, DEV)
+        AcousticModel(synth.acoustic_state_dict(switch_hp({"T": 4, "overrides": {}}), seed=0), hp, DEV)
     # the emo-off model works without emo_embed in the batch, the style-off one without reference mels
     out = m.forward(pb, seed=0, want=("mel_out",))
     assert torch.isfinite(out["mel_out"]).all()

@@ -4,7 +4,7 @@ ResBlock2.  Every check runs for V2, V3 and V3 without the NSF source:
 
   (a) against the reference's own generator (tests/golden/ref_vocoder_layouts.npz, noise injected as NoiseSource draws);
   (b) a ragged batch at the edge lengths of tests/test_gpu_vocoder.py and a bench-shaped batch against the float64
-      layout oracle (tests/vocoder_layouts_ref.py, pinned to the reference in tests/test_vocoder_layouts_cpu.py);
+      oracle (pinned to the reference in tests/test_vocoder_layouts_cpu.py);
   (c) every utterance of a batch against its solo call;
   (d) with per-utterance seeds, utterance b against the B = 1 call with seeds[b];
   (e) which kernels run: with tensor cores on, every ResBlock conv (the grouped narrow ones included) and every eligible
@@ -29,8 +29,7 @@ import torch
 from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
 from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG
-from tests import vocoder_layouts_ref as R
-from tests.common import golden, vocoder_sd
+from tests.common import VOCODER_LAYOUTS, golden, vocoder_sd
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -101,7 +100,7 @@ def _split(wav, utts):
 
 
 def _f0_modes(name):
-    return (True, False) if R.LAYOUTS[name]["use_pitch_embed"] else (False,)
+    return (True, False) if VOCODER_LAYOUTS[name]["use_pitch_embed"] else (False,)
 
 
 _V, _M = {}, {}
@@ -110,7 +109,7 @@ _V, _M = {}, {}
 def _voc(name, tc):
     from stylesinger_b200.engine import Vocoder
     if name not in _V:
-        _V[name] = Vocoder(R.state_dict(name), R.LAYOUTS[name])
+        _V[name] = Vocoder(vocoder_sd(name), VOCODER_LAYOUTS[name])
     v = _V[name]
     assert v.set_tensor_cores(tc) == tc
     return v
@@ -119,8 +118,8 @@ def _voc(name, tc):
 def _oracle(name, key, u, with_f0):
     k = (name, key, u.L, with_f0)
     if k not in _M:
-        _M[k] = R.spec2wav(u.mel, u.f0 if with_f0 else None, R.state_dict(name), R.LAYOUTS[name], O.NoiseSource(u.seed),
-                           torch.float64)
+        _M[k] = O.spec2wav(u.mel, u.f0 if with_f0 else None, vocoder_sd(name), VOCODER_LAYOUTS[name],
+                           O.NoiseSource(u.seed), torch.float64)
     return _M[k]
 
 
@@ -193,7 +192,7 @@ def test_bench_shaped_call(name):
     """(b, c) The call size Vocoder.generate hands the library in the batch64 workload, on both paths: the short
     utterances against the float64 oracle, every utterance tensor cores vs FFMA and against its solo call."""
     utts = bench_utts()
-    with_f0 = R.LAYOUTS[name]["use_pitch_embed"]
+    with_f0 = VOCODER_LAYOUTS[name]["use_pitch_embed"]
     w_tc = _split(_generate(_voc(name, True), utts, with_f0), utts)
     w_ffma = _split(_generate(_voc(name, False), utts, with_f0), utts)
     errs = {"oracle_tc": 0.0, "oracle_ffma": 0.0, "paths": 0.0, "solo_tc": 0.0, "solo_ffma": 0.0}
@@ -222,7 +221,7 @@ def test_keyed_seeds_match_solo_calls(name, tc):
     v = _voc(name, tc)
     utts = edge_utts()
     mel, f0, _, _, offs = _cat(utts)
-    f0 = f0 if R.LAYOUTS[name]["use_pitch_embed"] else None
+    f0 = f0 if VOCODER_LAYOUTS[name]["use_pitch_embed"] else None
     seeds = [1000003 * (b + 1) + 17 for b in range(len(utts))]
     wav = v.generate(mel, f0, offs, seeds=seeds).cpu().numpy()
     worst = 0.0
@@ -256,10 +255,10 @@ def test_variant_counts(name):
         v = _voc(name, tc)
         torch.cuda.synchronize()
         before = variant_launches()
-        _generate(v, utts, R.LAYOUTS[name]["use_pitch_embed"])
+        _generate(v, utts, VOCODER_LAYOUTS[name]["use_pitch_embed"])
         after = variant_launches()
         counts[tc] = sum(after[k] - before.get(k, 0) for k in after)
-    exp = _expected_tc_launches(R.LAYOUTS[name])
+    exp = _expected_tc_launches(VOCODER_LAYOUTS[name])
     print(f"{name}: tensor-core launches with tensor cores on {counts[True]} (expected {exp}), off {counts[False]}")
     _voc(name, True)
     assert counts[True] == exp and counts[False] == 0
@@ -297,7 +296,7 @@ def test_workspace_contract(name, tc):
     give the same bits), writes nothing past that size (a sentinel tail survives), and a workspace left over from a
     larger call of another shape changes nothing."""
     v = _voc(name, tc)
-    with_f0 = R.LAYOUTS[name]["use_pitch_embed"]
+    with_f0 = VOCODER_LAYOUTS[name]["use_pitch_embed"]
     big, small = bench_utts()[:6], edge_utts()
     nb, ns = _ws_bytes(v, big), _ws_bytes(v, small)
     print(f"{name} {_ids(tc)} workspace bytes: bench-shaped call {nb}, edge batch {ns}")
@@ -367,8 +366,8 @@ def test_checkpoint_directory_to_waveform(tmp_path, fname, name):
     import json
     from stylesinger_b200 import formats
     from stylesinger_b200.engine import Vocoder
-    h = DEFAULT_VOCODER_CONFIG if name is None else R.LAYOUTS[name]
-    sd = vocoder_sd() if name is None else R.state_dict(name)
+    h = DEFAULT_VOCODER_CONFIG if name is None else VOCODER_LAYOUTS[name]
+    sd = vocoder_sd(name)
     torch.save({"generator": sd}, str(tmp_path / fname))
     with open(tmp_path / "config.json", "w") as f:
         json.dump(h, f)

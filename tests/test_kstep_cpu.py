@@ -1,6 +1,6 @@
-"""Shallow diffusion (hparams['K_step'] < timesteps), CPU side: the K-step oracle (tests/kstep_oracle.py) against the
-unmodified reference's fixture (tests/golden/ref_kstep.npz, tools/make_golden.py kstep), its identity with the oracle
-at K_step == timesteps, and the hparams rules.  Bars: tests/test_oracle_golden.py's (TOL per operator, 5e-5 for the T=25
+"""Shallow diffusion (hparams['K_step'] < timesteps), CPU side: the oracle's K-step samplers against the
+unmodified reference's fixture (tests/golden/ref_kstep.npz, tools/make_golden.py kstep), K_step == timesteps as the
+full-schedule run, and the hparams rules.  Bars: tests/test_oracle_golden.py's (TOL per operator, 5e-5 for the T=25
 sampler, TOL * max(1, |mel|) for PLMS)."""
 import numpy as np
 import pytest
@@ -8,18 +8,13 @@ import torch
 
 from oracle import stylesinger_oracle as O
 from stylesinger_b200.hparams import resolve
-from tests import kstep_oracle as KO
-from tests.common import acoustic_sd, golden, utt_from_meta
+from tests.common import acoustic_sd, golden, kstep_hp, utt_from_meta
 
 TOL = 2e-5
 
 
 def _maxabs(a, b):
     return float(np.abs(np.asarray(a, np.float64) - np.asarray(b, np.float64)).max())
-
-
-def kstep_hp(T, K):
-    return resolve(timesteps=T, K_step=K, f0_timesteps=T)
 
 
 def _log(ns):
@@ -33,9 +28,9 @@ def test_full_forward_matches_reference():
     u = utt_from_meta(meta)
     ns = O.NoiseSource(meta["seed"])
     with torch.no_grad():
-        r = KO.stylesinger_forward(acoustic_sd(), hp, u["txt_tokens"][None], u["note"][None], u["note_dur"][None],
-                                   u["note_type"][None], u["spk_embed"][None], u["emo_embed"][None], u["ref_mels"][None],
-                                   u["ref_f0"], ns, mel2ph=u["mel2ph"][None])
+        r = O.stylesinger_forward(acoustic_sd(), hp, u["txt_tokens"][None], u["note"][None], u["note_dur"][None],
+                                  u["note_type"][None], u["spk_embed"][None], u["emo_embed"][None], u["ref_mels"][None],
+                                  u["ref_f0"], ns, mel2ph=u["mel2ph"][None])
     assert _log(ns) == meta["noise_log"]
     # the mel sampler's draws: q_sample + K_step steps
     assert sum(1 for k, sh in meta["noise_log"] if sh[-2:] == [80, meta["frames"]]) == meta["K_fwd"] + 1
@@ -54,8 +49,8 @@ def test_sampler_matches_reference(key, K):
     K = meta["K"] if K is None else K
     ns = O.NoiseSource(meta["seed"] + 2)
     with torch.no_grad():
-        mel = KO.mel_diffusion_sample(torch.from_numpy(g["smp_cond"])[None], torch.from_numpy(g["smp_coarse"])[None],
-                                      acoustic_sd(), kstep_hp(meta["T"], K), ns)
+        mel = O.mel_diffusion_sample(torch.from_numpy(g["smp_cond"])[None], torch.from_numpy(g["smp_coarse"])[None],
+                                     acoustic_sd(), kstep_hp(meta["T"], K), ns)
     assert _log(ns) == meta[key + "_noise_log"] and len(ns.log) == K + 1
     err = _maxabs(mel[0], g[key + "_mel"])
     print(f"timesteps {meta['T']}, K_step {K}: sampler L-inf vs reference {err:.3e}")
@@ -69,8 +64,8 @@ def test_plms_matches_reference(interval):
     assert meta[f"plms_i{interval}_t0"] == (meta["K"] - 1) // interval * interval
     ns = O.NoiseSource(meta["seed"] + 3)
     with torch.no_grad():
-        mel = KO.mel_diffusion_sample_plms(torch.from_numpy(g["smp_cond"])[None], torch.from_numpy(g["smp_coarse"])[None],
-                                           acoustic_sd(), kstep_hp(meta["T"], meta["K"]), ns, interval)
+        mel = O.mel_diffusion_sample_plms(torch.from_numpy(g["smp_cond"])[None], torch.from_numpy(g["smp_coarse"])[None],
+                                          acoustic_sd(), kstep_hp(meta["T"], meta["K"]), ns, interval)
     assert _log(ns) == meta[f"plms_i{interval}_noise_log"]
     ref = g[f"plms_i{interval}_mel"]
     err, scale = _maxabs(mel[0], ref), float(np.abs(ref).max())
@@ -79,6 +74,7 @@ def test_plms_matches_reference(interval):
 
 
 def test_k_step_equal_to_timesteps_is_the_oracle_bit_for_bit():
+    """K_step = timesteps and an hp without K_step run the same samplers, bit for bit; a smaller K_step does not."""
     T, Fr = 12, 20
     gen = torch.Generator().manual_seed(3)
     cond = torch.randn(1, Fr, 256, generator=gen)
@@ -86,14 +82,13 @@ def test_k_step_equal_to_timesteps_is_the_oracle_bit_for_bit():
     hp = kstep_hp(T, T)
     hp_nokey = {k: v for k, v in hp.items() if k != "K_step"}
     with torch.no_grad():
-        a = KO.mel_diffusion_sample(cond, coarse, acoustic_sd(), hp, O.NoiseSource(5))
+        a = O.mel_diffusion_sample(cond, coarse, acoustic_sd(), hp, O.NoiseSource(5))
         b = O.mel_diffusion_sample(cond, coarse, acoustic_sd(), hp_nokey, O.NoiseSource(5))
-        c = KO.mel_diffusion_sample(cond, coarse, acoustic_sd(), hp_nokey, O.NoiseSource(5))
-        p = KO.mel_diffusion_sample_plms(cond, coarse, acoustic_sd(), hp, O.NoiseSource(6), 5)
+        p = O.mel_diffusion_sample_plms(cond, coarse, acoustic_sd(), hp, O.NoiseSource(6), 5)
         q = O.mel_diffusion_sample_plms(cond, coarse, acoustic_sd(), hp_nokey, O.NoiseSource(6), 5)
-    assert torch.equal(a, b) and torch.equal(c, b) and torch.equal(p, q)
+    assert torch.equal(a, b) and torch.equal(p, q)
     with torch.no_grad():  # and a smaller K does change the result
-        d = KO.mel_diffusion_sample(cond, coarse, acoustic_sd(), kstep_hp(T, T - 3), O.NoiseSource(5))
+        d = O.mel_diffusion_sample(cond, coarse, acoustic_sd(), kstep_hp(T, T - 3), O.NoiseSource(5))
     assert not torch.equal(d, b)
 
 

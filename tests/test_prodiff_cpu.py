@@ -8,11 +8,9 @@ import pytest
 import torch
 
 from oracle import stylesinger_oracle as O
-from stylesinger_b200 import synth
 from stylesinger_b200.hparams import resolve
 from stylesinger_b200.schedules import prodiff_schedule, prodiff_table
-from tests import prodiff_oracle as PO
-from tests.common import golden, utt_from_meta
+from tests.common import golden, prodiff_hp, prodiff_sd, utt_from_meta
 
 TOL = 2e-5  # fp32 CPU, same op order up to BLAS blocking (as tests/test_oracle_golden.py)
 COMMENTED_CONFIG = {"timesteps": 8, "timescale": 1, "K_step": 1000, "schedule_type": "vpsde", "max_beta": 0.06,
@@ -23,23 +21,10 @@ def _maxabs(a, b):
     return float(np.abs(np.asarray(a, np.float64) - np.asarray(b, np.float64)).max())
 
 
-def prodiff_hp(meta):
-    return resolve(timesteps=meta["T"], K_step=meta["T"], f0_timesteps=meta["f0_T"], **meta["overrides"])
-
-
-_SD = {}
-
-
-def prodiff_sd(meta):
-    if "sd" not in _SD:
-        _SD["sd"] = synth.acoustic_state_dict(prodiff_hp(meta), seed=0)
-    return _SD["sd"]
-
-
 def test_prodiff_table_matches_reference_buffers():
     g, meta = golden("ref_prodiff_T8")
     T = meta["T"]
-    s, o = prodiff_schedule(T), PO.prodiff_tables(T)
+    s, o = prodiff_schedule(T), O.prodiff_tables(T)
     for k in s:
         ref = g["sched_" + k]
         assert ref.shape == (T + 1,)
@@ -58,10 +43,10 @@ def test_prodiff_table_matches_reference_buffers():
 
 def test_oracle_prodiff_sampler_matches_reference():
     g, meta = golden("ref_prodiff_T8")
-    hp = prodiff_hp(meta)
+    hp = prodiff_hp()
     ns = O.NoiseSource(meta["sampler_seed"])
     with torch.no_grad():
-        mel = PO.mel_prodiff_sample(torch.from_numpy(g["sampler_cond"])[None], prodiff_sd(meta), hp, ns)
+        mel = O.mel_prodiff_sample(torch.from_numpy(g["sampler_cond"])[None], prodiff_sd(), hp, ns)
     assert [[k, list(sh)] for k, sh in ns.log] == meta["sampler_noise_log"]
     err, scale = _maxabs(mel[0].numpy(), g["sampler_mel"]), float(np.abs(g["sampler_mel"]).max())
     print("oracle ProDiff sampler L-inf:", err, "|mel|max:", scale)
@@ -70,13 +55,13 @@ def test_oracle_prodiff_sampler_matches_reference():
 
 def test_oracle_prodiff_forward_matches_reference():
     g, meta = golden("ref_prodiff_T8")
-    hp = prodiff_hp(meta)
+    hp = prodiff_hp()
     u = utt_from_meta(meta)
     ns = O.NoiseSource(meta["seed"])
     with torch.no_grad():
-        r = PO.stylesinger_forward(prodiff_sd(meta), hp, u["txt_tokens"][None], u["note"][None], u["note_dur"][None],
-                                   u["note_type"][None], u["spk_embed"][None], u["emo_embed"][None], u["ref_mels"][None],
-                                   u["ref_f0"], ns, mel2ph=u["mel2ph"][None])
+        r = O.stylesinger_forward(prodiff_sd(), hp, u["txt_tokens"][None], u["note"][None], u["note_dur"][None],
+                                  u["note_type"][None], u["spk_embed"][None], u["emo_embed"][None], u["ref_mels"][None],
+                                  u["ref_f0"], ns, mel2ph=u["mel2ph"][None])
     assert [[k, list(sh)] for k, sh in ns.log] == meta["noise_log"]
     e_dec = _maxabs(r["decoder_inp"][0].numpy(), g["decoder_inp"])
     e_f0 = _maxabs(r["f0_denorm"][0].numpy(), g["f0_denorm"])
@@ -89,7 +74,7 @@ def test_oracle_prodiff_forward_matches_reference():
 
 def test_synth_prodiff_state_dict_has_the_reference_keys_and_shapes():
     g, meta = golden("ref_prodiff_T8")
-    sd = prodiff_sd(meta)
+    sd = prodiff_sd()
     ours = [[k, list(v.shape)] for k, v in sd.items()]
     assert ours == meta["state_dict"]
     assert not any(k.startswith(("postdiff.", "ln_proj.")) for k in sd)

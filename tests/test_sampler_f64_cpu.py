@@ -9,10 +9,8 @@ import pytest
 import torch
 
 from oracle import stylesinger_oracle as O
-from tests import kstep_oracle as KO
-from tests import prodiff_oracle as PO
 from tests import sampler_oracle as SO
-from tests.common import acoustic_sd, golden, hp_for
+from tests.common import acoustic_sd, golden, hp_for, prodiff_hp, prodiff_sd
 
 TOL = 2e-5  # the fp32 oracle's bar against the reference (tests/test_oracle_golden.py)
 PLMS_CONFIGS = [(100, 10), (100, 7), (37, 5), (6, 1), (4, 3), (2, 1)]  # (K_step, interval) on T = 100
@@ -71,13 +69,13 @@ def _fp32_calls_vs_f64(calls32, calls64):
 # ProDiff
 @pytest.mark.parametrize("T", [8, 4])
 def test_prodiff_chain64_matches_fp32_oracle(T):
-    hp = SO.prodiff_hp(T)
+    hp = prodiff_hp(T)
     Fr = 70
     cond, _ = _cond(Fr, 10 + T)
     noise = torch.randn(T + 1, Fr, 80, generator=torch.Generator().manual_seed(20 + T))
     with _recording_diffnet() as calls32, torch.no_grad():
-        mel32 = PO.mel_prodiff_sample(cond[None], SO.prodiff_sd(), hp,
-                                      ListNoise([noise[k].t().contiguous()[None, None] for k in range(T + 1)]))[0]
+        mel32 = O.mel_prodiff_sample(cond[None], prodiff_sd(), hp,
+                                     ListNoise([noise[k].t().contiguous()[None, None] for k in range(T + 1)]))[0]
     r = SO.prodiff_chain64(cond, hp, noise)
     # the k-th denoiser input is x_{T-k}
     e = _fp32_calls_vs_f64(calls32, [(T - 1 - k, x) for k, x in enumerate(r["x"][:T])])
@@ -92,7 +90,7 @@ def test_prodiff_chain64_matches_reference_fixture():
     whose mel sampler draws last: its decoder_inp and the last T + 1 draws of NoiseSource(seed)."""
     g, meta = golden("ref_prodiff_T8")
     T = meta["T"]
-    hp = SO.prodiff_hp()
+    hp = prodiff_hp()
     ns = O.NoiseSource(meta["sampler_seed"])
     Fr = g["sampler_cond"].shape[0]
     noise = torch.stack([ns.randn((1, 1, 80, Fr))[0, 0].t() for _ in range(T + 1)])
@@ -112,8 +110,8 @@ def test_prodiff_chain64_matches_reference_fixture():
 def _plms32(cond, coarse, K, interval, q):
     hp = dict(hp_for(100), K_step=K)
     with _recording_diffnet() as calls32, torch.no_grad():
-        mel32 = KO.mel_diffusion_sample_plms(cond[None], coarse[None], acoustic_sd(), hp,
-                                             ListNoise([q.t().contiguous()[None, None]]), interval)[0]
+        mel32 = O.mel_diffusion_sample_plms(cond[None], coarse[None], acoustic_sd(), hp,
+                                            ListNoise([q.t().contiguous()[None, None]]), interval)[0]
     return mel32, calls32
 
 

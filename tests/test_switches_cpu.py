@@ -11,8 +11,7 @@ from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
 from stylesinger_b200.engine import pack_batch
 from stylesinger_b200.hparams import SWITCHES, resolve
-from tests import switches_oracle as SO
-from tests.common import golden, utt_from_meta
+from tests.common import golden, switch_hp, switch_sd, utt_from_meta
 
 TOL = 2e-5  # fp32 CPU, same op order up to BLAS blocking (as tests/test_oracle_golden.py)
 CONFIGS = ("no_emo", "no_style", "no_umln", "no_txt_cond", "all_off", "prodiff_no_emo_style", "conv_no_style")
@@ -31,10 +30,10 @@ def _forward(meta, c, seed, use_mel2ph=True):
     u = utt_from_meta(meta)
     ns = O.NoiseSource(seed)
     with torch.no_grad():
-        r = SO.stylesinger_forward(SO.switch_sd(cfg), SO.switch_hp(cfg), u["txt_tokens"][None], u["note"][None],
-                                   u["note_dur"][None], u["note_type"][None], u["spk_embed"][None],
-                                   u["emo_embed"][None], u["ref_mels"][None], u["ref_f0"], ns,
-                                   mel2ph=u["mel2ph"][None] if use_mel2ph else None)
+        r = O.stylesinger_forward(switch_sd(cfg), switch_hp(cfg), u["txt_tokens"][None], u["note"][None],
+                                  u["note_dur"][None], u["note_type"][None], u["spk_embed"][None],
+                                  u["emo_embed"][None], u["ref_mels"][None], u["ref_f0"], ns,
+                                  mel2ph=u["mel2ph"][None] if use_mel2ph else None)
     return r, ns
 
 
@@ -42,7 +41,7 @@ def test_fixture_covers_every_configuration():
     g, meta = golden("ref_switches")
     assert tuple(meta["configs"]) == CONFIGS
     for c in CONFIGS:
-        hp = SO.switch_hp(_cfg(meta, c))
+        hp = switch_hp(_cfg(meta, c))
         assert (f"{c}/style" in g.files) == hp["style"] and (f"{c}/rq_codes" in g.files) == hp["style"]
         assert (f"{c}/emo_embed" in g.files) == hp["emo"]
         assert (f"{c}/coarse_mel" in g.files) == (hp["decoder"] == "diffsinger")
@@ -80,27 +79,13 @@ def test_oracle_duration_path_matches_reference():
     assert _maxabs(r["f0_denorm"][0].numpy(), g[f"{c}/dur_f0_denorm"]) < 1e-3
 
 
-def test_oracle_with_every_switch_on_is_the_shared_oracle():
-    """All four switches on: the restatement is the shared oracle's forward, bit for bit."""
-    hp = resolve(timesteps=4, K_step=4, f0_timesteps=4)
-    sd = synth.acoustic_state_dict(hp, seed=0)
-    u = synth.make_utterance(0.2, utt_idx=3, ref_frames=24, frames=24, phones=4)
-    args = (u["txt_tokens"][None], u["note"][None], u["note_dur"][None], u["note_type"][None], u["spk_embed"][None],
-            u["emo_embed"][None], u["ref_mels"][None], u["ref_f0"])
-    with torch.no_grad():
-        a = O.stylesinger_forward(sd, hp, *args, O.NoiseSource(9), mel2ph=u["mel2ph"][None])
-        b = SO.stylesinger_forward(sd, hp, *args, O.NoiseSource(9), mel2ph=u["mel2ph"][None])
-    for k in ("mel_out", "f0_denorm", "style", "rq_codes", "decoder_inp", "coarse_mel", "diff_cond"):
-        assert torch.equal(a[k], b[k]), k
-
-
 @pytest.mark.parametrize("c", CONFIGS)
 def test_synth_keys_and_shapes_are_the_references(c):
     _, meta = golden("ref_switches")
-    hp = SO.switch_hp(_cfg(meta, c))
+    hp = switch_hp(_cfg(meta, c))
     ref = [[k, list(s)] for k, s in meta["configs"][c]["state_dict"]]
     assert [[k, list(s)] for k, s in synth.acoustic_param_shapes(hp)] == ref
-    sd = SO.switch_sd(_cfg(meta, c))
+    sd = switch_sd(_cfg(meta, c))
     assert [[k, list(v.shape)] for k, v in sd.items()] == ref
 
 

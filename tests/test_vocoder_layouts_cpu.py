@@ -1,4 +1,4 @@
-"""HiFi-GAN V2 and V3 without a GPU: the layout oracle (tests/vocoder_layouts_ref.py) against the reference's own
+"""HiFi-GAN V2 and V3 without a GPU: the oracle's generator against the reference's own
 HifiGanGenerator (tools/make_golden.py vocoder_layouts: 1-24 frames, with and without f0), its float64 mode against its
 fp32 mode, synth's state-dict names against the reference's, and the config checks of ssb_vocoder_create_ex, which
 refuse a layout before anything is allocated."""
@@ -11,8 +11,7 @@ import torch
 from oracle import stylesinger_oracle as O
 from stylesinger_b200 import synth
 from stylesinger_b200.hparams import DEFAULT_VOCODER_CONFIG, HIFIGAN_V2, HIFIGAN_V3
-from tests import vocoder_layouts_ref as R
-from tests.common import golden
+from tests.common import VOCODER_LAYOUTS, golden, vocoder_sd
 
 TOL = 2e-6  # the reference bar of tests/test_vocoder_cpu.py
 F64_BAR = 1e-5  # fp32 vs float64 oracle, as in tests/test_vocoder_cpu.py
@@ -32,7 +31,7 @@ def _cases(g, meta):
     for name in meta["layouts"]:
         for L in meta["lengths"]:
             mel, f0 = g[f"mel_{L}"], g[f"f0_{L}"]
-            if R.LAYOUTS[name]["use_pitch_embed"]:
+            if VOCODER_LAYOUTS[name]["use_pitch_embed"]:
                 yield name, L, True, mel, f0, meta["seed"] + L, g[f"wav_{name}_{L}"]
             yield name, L, False, mel, None, meta["seed"] + L, g[f"wav_nof0_{name}_{L}"]
 
@@ -43,7 +42,7 @@ def test_fixture_covers_the_layouts(fx):
     assert "wav_v3_nonsf_24" not in g.files  # the generator without NSF has no f0 input
     for L in meta["lengths"]:
         assert g[f"mel_{L}"].shape == (L, 80) and g[f"f0_{L}"].shape == (L,)
-        for name, h in R.LAYOUTS.items():
+        for name, h in VOCODER_LAYOUTS.items():
             assert g[f"wav_nof0_{name}_{L}"].shape == (256 * L,)
 
 
@@ -54,7 +53,7 @@ def test_oracle_matches_reference(fx, name):
     for lname, L, with_f0, mel, f0, seed, ref in _cases(g, meta):
         if lname != name:
             continue
-        w = R.spec2wav(mel, f0, R.state_dict(name), R.LAYOUTS[name], O.NoiseSource(seed))
+        w = O.spec2wav(mel, f0, vocoder_sd(name), VOCODER_LAYOUTS[name], O.NoiseSource(seed))
         e = _maxabs(w, ref)
         print(f"{name} L={L:2d} f0={with_f0}: oracle vs reference max |d| {e:.2e} (bar {TOL:.0e})")
         assert w.shape == ref.shape
@@ -69,8 +68,8 @@ def test_float64_oracle_agrees_with_fp32_oracle(fx, name):
     for lname, L, with_f0, mel, f0, seed, _ in _cases(g, meta):
         if lname != name:
             continue
-        a = R.spec2wav(mel, f0, R.state_dict(name), R.LAYOUTS[name], O.NoiseSource(seed))
-        b = R.spec2wav(mel, f0, R.state_dict(name), R.LAYOUTS[name], O.NoiseSource(seed), torch.float64)
+        a = O.spec2wav(mel, f0, vocoder_sd(name), VOCODER_LAYOUTS[name], O.NoiseSource(seed))
+        b = O.spec2wav(mel, f0, vocoder_sd(name), VOCODER_LAYOUTS[name], O.NoiseSource(seed), torch.float64)
         assert b.dtype == np.float64
         worst = max(worst, _maxabs(a, b))
     print(f"{name}: fp32 vs float64 oracle max |d| {worst:.2e} (bar {F64_BAR:.0e})")
@@ -80,7 +79,7 @@ def test_float64_oracle_agrees_with_fp32_oracle(fx, name):
 def test_synth_names_are_the_reference_names(fx):
     g, meta = fx
     for name in meta["layouts"]:
-        assert [n for n, _ in synth.vocoder_param_shapes(R.LAYOUTS[name])] == meta["keys"][name], name
+        assert [n for n, _ in synth.vocoder_param_shapes(VOCODER_LAYOUTS[name])] == meta["keys"][name], name
     assert any(".convs.1." in k for k in meta["keys"]["v3"]) and not any("convs1" in k for k in meta["keys"]["v3"])
 
 

@@ -456,7 +456,7 @@ def case_convf0(name, T=4, frames=96, phones=12, ref_frames=64, seed=111, utt_id
          "dur_mel2ph": o2["mel2ph"][0].numpy().astype(np.int64), "dur_pitch_pred": np32(o2["pitch_pred"][0]),
          "dur_f0_denorm": np32(o2["f0_denorm"][0]), "dur_decoder_inp": np32(o2["decoder_inp"][0]),
          "dur_mel_out": np32(o2["mel_out"][0]),
-         # the predictor inputs are regenerated from pred_seed by the tests (tests/f0conv_oracle.predictor_inputs); their
+         # the predictor inputs are regenerated from pred_seed by the tests (tests/common.predictor_inputs); their
          # first rows are kept to check that
          "pred_x_head": np32(xs[:, 0, :4]), "pred_out_agnostic": np32(pa[0]), "pred_out_specific": np32(ps[0])}
     # (d) ProDiff decoder + conv F0 generator: the fast configuration
